@@ -1,9 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — DINOv3 SSL training step on B200: global-crops/sec, ViT-L/16, 224^2, 2 global + 8 local crops, bf16.
+"""bench.py — DINOv3 SSL training step on H100: global-crops/sec, ViT-L/16, 224^2, 2 global + 8 local crops, bf16.
 
 Contract (driver): `python bench.py --gpus N --steps K --warmup W` (torchrun launches N ranks for N > 1) prints ONE
 JSON line on rank 0.  `--impl reference` times the CPU restatement of the reference step (oracle/, "port") on the
 host cores instead (the reference's JAX stack is not installable here; see DESIGN.md).
+`--dump-outputs DIR` writes what the last timed step computed (loss terms, seeded samples of the updated parameters
+and of the gradients) as DIR/<name>.npy, so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -30,32 +32,34 @@ def f_img(D, L, Ng, Nl, n_local=8):
     return L * (2 * f_blk(Ng) + 3 * (2 * f_blk(Ng) + n_local * f_blk(Nl)))
 
 
-def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured"
-    return 1590.0, 1400.0, 6650.0, "fallback"
+# NVIDIA H100 SXM data sheet (700 W part): dense bf16 tensor-core rate.  An upper bound, not reached.
+H100_BF16_TFLOPS = 989.0
 
 
-def ncu_traffic():
-    """DRAM traffic of the roofline kernel from the committed `ncu --set full` capture of GEMM launches with KNOWN shapes
-    (profiles/r02_ncu_gemm_labeled.txt, tools/ncu_gemm_labeled.py): per labelled launch the measured dram read+write
-    bytes, the algorithmic bytes and their ratio; `traffic` in the JSON line is the first one (the qkv projection)."""
-    import re
-    p = os.path.join(ROOT, "profiles", "r02_ncu_gemm_labeled.txt")
-    if not os.path.exists(p):
-        return None
-    launches = []
-    for line in open(p):
-        m = re.match(r"\[(.*?)\] launch \d+: .*? = +([\d.]+) MB .*algorithmic ([\d.]+) MB -> traffic ratio ([\d.]+)", line)
-        if m:
-            launches.append({"launch": m.group(1), "dram_bytes": float(m.group(2)) * 1e6, "algorithmic_bytes": float(m.group(3)) * 1e6,
-                             "traffic_ratio": float(m.group(4))})
-    if not launches:
-        return None
-    return {"bytes_per_launch": launches[0]["dram_bytes"], "labelled_launches": launches,
-            "source": "profiles/r02_ncu_gemm_labeled.txt (ncu --set full --clock-control none, tools/ncu_gemm_labeled.py)"}
+def dump_outputs(eng, out_dir, write, per_tensor=4096):
+    """The last timed step's results as DIR/<name>.npy: every loss term / metric (float64), and for the student
+    parameters, the teacher parameters and the student gradients a fixed sample of `per_tensor` elements of every
+    tensor (float32, tensors in name order, indices drawn from a generator seeded by the tensor name).  Every rank
+    takes part (under FSDP the export gathers the shards); only the one with `write` set writes."""
+    import zlib
+
+    import numpy as np
+    metrics = eng.read_metrics()
+    trees = {"param": eng.params.export_reference_tree("param"), "grad": eng.params.export_reference_tree("grad")}
+    if not write:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in metrics.items():
+        np.save(os.path.join(out_dir, f"metric_{k}.npy"), np.array([v], dtype=np.float64))
+    for fname, what, prefix in (("student_params_sample", "param", "student_"), ("teacher_params_sample", "param", "teacher_"),
+                                ("student_grads_sample", "grad", "student_")):
+        parts = []
+        for name in sorted(k for k in trees[what] if k.startswith(prefix)):
+            flat = trees[what][name].reshape(-1)
+            g = torch.Generator().manual_seed(zlib.crc32(name.split("_", 1)[1].encode()))
+            idx = torch.randint(0, flat.numel(), (min(per_tensor, flat.numel()),), generator=g)
+            parts.append(flat[idx.to(flat.device)].float().cpu())
+        np.save(os.path.join(out_dir, f"{fname}.npy"), torch.cat(parts).numpy().astype(np.float32))
 
 
 class ClockSampler:
@@ -172,6 +176,8 @@ def main():
     ap.add_argument("--cpu-sample-batch", type=int, default=2, help="images per CPU-baseline step (bounded sample: ~15-25 s of CPU work)")
     ap.add_argument("--cpu-budget-s", type=float, default=150.0, help="wall-clock bound of the --impl reference arm")
     ap.add_argument("--no-checks", action="store_true", help="skip parity_check / fsdp_check")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss terms and seeded samples of parameters / gradients as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -185,7 +191,7 @@ def main():
     cfg_desc = {"workload": f"{args.arch}/{args.patch} student+teacher, 2x224^2 + 8x{args.local_size}^2 crops, {args.batch} img/GPU, "
                             f"K={args.prototypes} prototypes, DINO+iBOT+KoLeo, clip+AdamW+EMA (BASELINE configs[3] per-GPU shape)",
                 "global_batch": args.batch * world, "parallelism": f"fsdp{world}" if world > 1 else "single",
-                "l2": "inputs+activations per step >> 126 MB L2 (no flush needed)"}
+                "l2": "inputs+activations per step >> 50 MB L2 (no flush needed)"}
 
     if args.impl == "reference":
         if rank != 0:
@@ -217,7 +223,7 @@ def main():
         return
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the B200 engine has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device — the GPU engine has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local_rank)
     comm = None
     if world > 1:
@@ -283,6 +289,8 @@ def main():
     ms = e0.elapsed_time(e1) / args.steps
     log(f"timed region: {ms:.2f} ms/step")
     clocks = sampler.stop(t0, t1) if sampler else None
+    if args.dump_outputs:
+        dump_outputs(eng, args.dump_outputs, write=rank == 0)
     # ---- end-to-end: host buffers, H2D inside, loss read back every step
     for i in range(2):
         step_e2e(i)
@@ -313,9 +321,8 @@ def main():
     eng.fwd_overlap = fwd_overlap
     g_flops = sum(p[1] for p in prof)
     g_ms = sum(p[2].elapsed_time(p[3]) for p in prof)
-    burst, sustained, hbm, how = peaks()
+    peak = H100_BF16_TFLOPS
     gemm_tf = g_flops / (g_ms * 1e-3) / 1e12 if g_ms else 0.0
-    traffic = ncu_traffic()
     value = 2 * B * world / (ms * 1e-3)
     e2e_value = 2 * B * world / (ms_e2e * 1e-3)
     step_tf = value * flops_per_gcrop / world / 1e12
@@ -325,15 +332,12 @@ def main():
         "dtype": "bf16", "data": "synthetic", "config": cfg_desc, "clocks": clocks, "gpu_launches": int(launches),
         "e2e": {"value": e2e_value, "unit": "global-crops/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": 32,
                 "ms_per_step": ms_e2e, "loss": loss},
-        "roofline": {"bound": "tensor", "kernel": "gemm2sm_kernel + gemm1sm_kernel (every tcgen05 GEMM launch of one step)",
-                     "achieved": gemm_tf, "peak": sustained, "unit": "TFLOP/s", "frac": gemm_tf / sustained,
-                     "traffic": traffic["bytes_per_launch"] if traffic else None,
-                     "traffic_unit": "bytes of ONE labelled launch (dram__bytes_read.sum + dram__bytes_write.sum, ncu --set full): "
-                                     "labelled_launches[0], the qkv projection",
-                     "traffic_labelled_launches": traffic["labelled_launches"] if traffic else None,
-                     "traffic_source": traffic["source"] if traffic else None, "peak_source": f"bf16_tflops_sustained ({how})", "launches": len(prof),
+        "roofline": {"bound": "tensor", "kernel": "gemm_kernel (every wgmma GEMM launch of one step)",
+                     "achieved": gemm_tf, "peak": peak, "unit": "TFLOP/s", "frac": gemm_tf / peak,
+                     "traffic": None, "traffic_unit": "not measured",
+                     "peak_source": "H100 SXM data sheet, dense bf16 (not reached)", "launches": len(prof),
                      "share_of_step": g_ms / ms if ms else None},
-        "step_roofline": {"achieved": step_tf, "peak": sustained, "unit": "TFLOP/s", "frac": step_tf / sustained,
+        "step_roofline": {"achieved": step_tf, "peak": peak, "unit": "TFLOP/s", "frac": step_tf / peak,
                           "note": "attention+MLP algorithmic FLOPs (BASELINE.md §3) / step time / GPU"},
     }
     if world > 1 and not args.no_checks:

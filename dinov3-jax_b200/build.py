@@ -1,7 +1,8 @@
-"""Build libdinov3_b200.so in-tree with nvcc for sm_100a (no torch extension machinery: a plain C-ABI library)."""
+"""Build libdinov3_b200.so in-tree with nvcc for sm_90a (no torch extension machinery: a plain C-ABI library)."""
 from __future__ import annotations
 
 import os
+import shutil
 import subprocess
 import sys
 from concurrent.futures import ThreadPoolExecutor
@@ -10,8 +11,21 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent
 CSRC = ROOT / "csrc"
 OUT = ROOT / "libdinov3_b200.so"
-SOURCES = ["api.cu", "gemm_tc.cu", "attention.cu", "attention_ws.cu", "elementwise.cu", "losses.cu", "optim.cu", "augment.cu"]
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+SOURCES = ["api.cu", "gemm_tc.cu", "attention.cu", "elementwise.cu", "losses.cu", "optim.cu", "augment.cu"]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+
+
+def find_nvcc() -> str:
+    """$NVCC, then nvcc on PATH, then the toolkit under $CUDA_HOME (default /usr/local/cuda)."""
+    if os.environ.get("NVCC"):
+        return os.environ["NVCC"]
+    found = shutil.which("nvcc")
+    if found:
+        return found
+    cand = Path(os.environ.get("CUDA_HOME", "/usr/local/cuda")) / "bin" / "nvcc"
+    if cand.exists():
+        return str(cand)
+    raise RuntimeError("nvcc not found: set NVCC or CUDA_HOME, or put the CUDA toolkit's bin/ on PATH")
 
 
 def _stale(target: Path, deps) -> bool:
@@ -22,9 +36,13 @@ def _stale(target: Path, deps) -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    nvcc = os.environ.get("NVCC", "nvcc")
+    nvcc = find_nvcc()
     objdir = ROOT / "build"
     objdir.mkdir(exist_ok=True)
+    # objects built with other flags (another GPU architecture) are never reused
+    stamp = objdir / "flags.txt"
+    if not stamp.exists() or stamp.read_text() != " ".join(FLAGS):
+        force = True
     headers = list(CSRC.glob("*.h")) + list(CSRC.glob("*.cuh")) + [ROOT.parent / "include" / "dinov3_b200.h"]
     jobs = []
     for src in SOURCES:
@@ -50,6 +68,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         r = subprocess.run([nvcc, "-shared", "-o", str(OUT)] + objs + ["-lcudart"], capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
+    stamp.write_text(" ".join(FLAGS))
     return OUT
 
 

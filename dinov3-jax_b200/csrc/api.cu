@@ -1,4 +1,5 @@
 // C ABI glue: library state, error reporting, tensor-map encoding, extern "C" wrappers.
+#include <algorithm>
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
@@ -21,7 +22,7 @@ int set_error(int code, const char* msg) {
 }
 static int g_sm_limit = 0;
 int sm_count() {
-  const int n = g_sm_count > 0 ? g_sm_count : 148;
+  const int n = g_sm_count > 0 ? g_sm_count : 132;
   return (g_sm_limit > 0 && g_sm_limit < n) ? g_sm_limit : n;
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
@@ -62,6 +63,39 @@ int encode_tensor_map_2d(CUtensorMap* map, const void* ptr, int elt_bytes, cuuin
   return D3_OK;
 }
 
+float* slab_workspace(size_t floats, cudaStream_t st) {
+  void* p = nullptr;
+  cudaError_t e = cudaMallocAsync(&p, floats * sizeof(float), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, floats * sizeof(float), st);
+  if (e != cudaSuccess) { set_error(D3_ERR_CUDA, cudaGetErrorString(e)); return nullptr; }
+  return static_cast<float*>(p);
+}
+void slab_release(float* ws, cudaStream_t st) {
+  if (ws) cudaFreeAsync(ws, st);
+}
+
+__global__ void slab_combine_kernel(const float* __restrict__ ws, int slabs, long long stride, long long rows, int cols,
+                                    float* __restrict__ dst, long long ld) {
+  const long long n = rows * cols;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / cols, c = i - r * cols;
+    float tot = 0.f;
+    for (int k = 0; k < slabs; ++k) tot += ws[k * stride + i];
+    dst[r * ld + c] += tot;
+  }
+}
+int slab_combine(const float* ws, int slabs, long long stride, long long rows, int cols, float* dst, long long ld,
+                 cudaStream_t st) {
+  if (!dst || rows <= 0 || cols <= 0) return D3_OK;
+  const long long n = rows * cols;
+  const int blocks = (int)std::min<long long>((n + 255) / 256, (long long)sm_count() * 8);
+  slab_combine_kernel<<<blocks, 256, 0, st>>>(ws, slabs, stride, rows, cols, dst, ld);
+  cudaError_t e = cudaPeekAtLastError();
+  if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  count_launch();
+  return D3_OK;
+}
+
 }  // namespace d3
 
 static int g_scatter_mode = -1;
@@ -82,7 +116,7 @@ int d3_set_scatter_mode(int mode) { d3::set_scatter_mode(mode); return D3_OK; }
 int d3_abi_version(void) { return 3; }   // 2: d3_gemm_epilogue gained the sc_* scatter fields; 3: round-2 entry points (swiglu, ema, colmax, deterministic Sinkhorn sums, koleo rows, augmentation)
 int d3_set_sm_limit(int n) {
   if (n < 0) return set_error(D3_ERR_ARG, "d3_set_sm_limit: n < 0");
-  g_sm_limit = n & ~1;   // CTA pairs: keep it even
+  g_sm_limit = n;
   return D3_OK;
 }
 const char* d3_last_error(void) { return g_err; }
@@ -95,14 +129,21 @@ int d3_init(int device) {
   cudaDeviceProp prop;
   e = cudaGetDeviceProperties(&prop, device);
   if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     char buf[128];
-    snprintf(buf, sizeof(buf), "device %d is sm_%d%d; this library only has sm_100a code (no fallback)", device,
+    snprintf(buf, sizeof(buf), "device %d is sm_%d%d; this library only has sm_90a code (no fallback)", device,
              prop.major, prop.minor);
     return set_error(D3_ERR_DEVICE, buf);
   }
   g_sm_count = prop.multiProcessorCount;
-  if (const char* e = getenv("D3_GEMM_SMS")) g_sm_limit = atoi(e) & ~1;
+  {  // keep the stream-ordered workspaces of the deterministic reductions cached instead of returning them at every sync
+    cudaMemPool_t pool;
+    if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
+      uint64_t keep = UINT64_MAX;
+      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+    }
+  }
+  if (const char* e = getenv("D3_GEMM_SMS")) g_sm_limit = atoi(e);
   if (!g_encode) {
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult q;

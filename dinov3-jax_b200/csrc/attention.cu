@@ -1,12 +1,15 @@
-// Multi-head self-attention forward / backward on tcgen05 tensor cores for the short ViT sequences of the DINOv3
-// crops (N = 197 / 37 / 257 / 50 tokens, head_dim = 64): replaces flax `nn.dot_product_attention(q, k, v)` at
+// Multi-head self-attention forward / backward on the Hopper tensor cores (wgmma) for the short ViT sequences of the
+// DINOv3 crops (N = 197 / 37 / 257 / 50 tokens, head_dim = 64): replaces flax `nn.dot_product_attention(q, k, v)` at
 // dinov3_jax/layers/attention.py:116 (softmax((q / sqrt(64)) k^T) v, no mask, no dropout) and its jax.grad.
 //
-// Forward: one CTA per (q-tile of 128 rows, head, crop).  The whole key range of a crop fits one pass, so there is
-// no online softmax: S = Q K^T lands in tensor memory (<= 512 fp32 columns), each of the 128 threads owns one
-// query row (tcgen05.ld 32x32b), writes P = softmax(S) as a bf16 K-major SWIZZLE_128B tile into shared memory
-// (over the dead Q/K tiles), and a second UMMA computes O = P V with V consumed as an MN-major operand straight
-// from its TMA tile.  Operands come by TMA from the fused qkv buffer [T, 3D] (q | k | v thirds, heads contiguous).
+// Short crops (N <= 64) are packed G per 128-row tile with a block-diagonal mask, so one CTA covers a "crop group" of
+// span = G * N token rows.  Operands come by TMA (SWIZZLE_128B) from the fused qkv buffer [T, 3D] (q | k | v thirds,
+// heads contiguous); every product is a warpgroup MMA with fp32 accumulators in registers.
+//
+// Forward: one CTA per (q-tile of 128 rows, head, crop group), two warpgroups of 64 query rows each.  Q and the whole
+// key / value range of the group are staged once; each warpgroup walks the keys in blocks of 64: S = Q K^T (SS form),
+// online softmax on the accumulator fragment, then O += P V with P handed to the tensor core straight from registers
+// (RS form: the accumulator fragment of S is the A-operand fragment of the PV product).
 #include "ptx.cuh"
 #include <cstdlib>
 #include "d3_internal.h"
@@ -26,9 +29,7 @@ struct AttnShape {
   int span;      // G*N: token rows owned by one CTA (grid.z = ceil(n_crops / G))
   int n_crops;
   int N;         // tokens per crop
-  int Nkp;       // keys padded (multiple of 16 * nbox)
-  int nbox;      // TMA boxes per K / V tile
-  int box_rows;  // rows per box
+  int nkb;       // 64-key blocks covering the span
   int D;         // embed dim (row stride of o / do); qkv row stride = 3D
   int H;
   float scale;   // head_dim^-0.5
@@ -37,180 +38,145 @@ struct AttnShape {
   int prefix;          // tokens before the first patch token (cls + storage tokens)
 };
 
-// swizzled (SWIZZLE_128B, K-major) address of element (row, col) in a [128 x 64] bf16 chunk; col multiple of 8
+// swizzled (SWIZZLE_128B, K-major) byte offset of element (row, col) in a [rows x 64] bf16 chunk
 __device__ __forceinline__ uint32_t sw128_offset(int row, int col) {
-  return (uint32_t)(row * 128 + ((((col >> 3) ^ (row & 7)) & 7) << 4));
+  return (uint32_t)(row * 128 + ((((col >> 3) ^ (row & 7)) & 7) << 4) + (col & 7) * 2);
 }
 
-template <int TMEM_COLS>
+// the crop of a token row inside the group and its key range [klo, khi)
+struct RowInfo { int g, klo, khi; bool ok; };
+__device__ __forceinline__ RowInfo row_info(const AttnShape& sh, int c, int q) {
+  RowInfo ri;
+  ri.g = min(q / sh.N, sh.G - 1);
+  ri.klo = ri.g * sh.N;
+  ri.khi = ri.klo + sh.N;
+  ri.ok = (q < sh.span) && (c * sh.G + ri.g < sh.n_crops);
+  return ri;
+}
+
 __global__ void __launch_bounds__(256)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                 __nv_bfloat16* __restrict__ O, float* __restrict__ LSE, const AttnShape sh) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // layout: [ region A: Q (16 KB) | K (Nkp*128 B)  -- later overwritten by P (ceil(Nkp/64) * 16 KB) ] [ V (Nkp*128 B) ]
-  const int kv_bytes = sh.Nkp * 128;
-  const int p_chunks = (sh.Nkp + 63) / 64;
-  const int regA = max(16384 + kv_bytes, p_chunks * 16384);
+  // layout: [Q 128 x 128 B][K nkb x 8 KB][V nkb x 8 KB][barrier]
   uint8_t* sQ = smem;
   uint8_t* sK = smem + 16384;
-  uint8_t* sP = smem;
-  uint8_t* sV = smem + regA;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kv_bytes);
-  uint64_t* bar_load = bars;
-  uint64_t* bar_mma = bars + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
-  float* red = reinterpret_cast<float*>(bars + 4);   // [2][128] cross-warp row reductions
+  uint8_t* sV = sK + sh.nkb * 8192;
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sV + sh.nkb * 8192);
 
-  // 256 threads: two threads per query row (r = tid & 127), each owning one half of the key columns / output columns
-  const int warp = threadIdx.x >> 5;
-  const int r = threadIdx.x & 127;
-  const int ch = threadIdx.x >> 7;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int qt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
   const int q0 = qt * 128;
   const int row_base = c * sh.span;  // first token row of this CTA's crop group in [T, ...]
-  // this thread's query row, its crop inside the group and that crop's key range [klo, khi)
-  const int q_abs = q0 + r;
-  const int g = min(q_abs / sh.N, sh.G - 1);
-  const int klo = g * sh.N, khi = klo + sh.N;
-  const bool q_valid = (q_abs < sh.span) && (c * sh.G + g < sh.n_crops);
-
+  dbg_mark(0);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmKV);
-    mbar_init(bar_load, 1);
-    mbar_init(bar_mma, 1);
+    mbar_init(bar, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc<TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-
-  if (warp == 0 && elect_one()) {
-    mbar_expect_tx(bar_load, 16384 + 2 * kv_bytes);
-    tma_load_2d(&tmQ, bar_load, sQ, h * 64, row_base + q0);
-    for (int b = 0; b < sh.nbox; ++b) {
-      tma_load_2d(&tmKV, bar_load, sK + b * sh.box_rows * 128, sh.D + h * 64, row_base + b * sh.box_rows);
-      tma_load_2d(&tmKV, bar_load, sV + b * sh.box_rows * 128, 2 * sh.D + h * 64, row_base + b * sh.box_rows);
+  if (threadIdx.x < 32 && elect_one()) {
+    mbar_expect_tx(bar, 16384 + 2 * sh.nkb * 8192);
+    tma_load_2d(&tmQ, bar, sQ, h * 64, row_base + q0);
+    for (int b = 0; b < sh.nkb; ++b) {
+      tma_load_2d(&tmKV, bar, sK + b * 8192, sh.D + h * 64, row_base + b * 64);
+      tma_load_2d(&tmKV, bar, sV + b * 8192, 2 * sh.D + h * 64, row_base + b * 64);
     }
-    mbar_wait(bar_load, 0);
-    tc_fence_after();
-    // S[128, Nkp] = Q K^T   (A = Q K-major, B = K K-major; UMMA N <= 256 per instruction)
-    const uint32_t qa = smem_u32(sQ), ka = smem_u32(sK);
-    for (int n0 = 0; n0 < sh.Nkp; n0 += 256) {
-      const int nn = min(256, sh.Nkp - n0);
-      const uint32_t idesc = umma_idesc_bf16(128, nn, 0, 0);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const uint64_t ad = umma_desc_sw128(qa + k * 32, 16, 1024);
-        const uint64_t bd = umma_desc_sw128(ka + n0 * 128 + k * 32, 16, 1024);
-        umma_bf16(tmem + n0, ad, bd, idesc, k > 0);
-      }
-    }
-    umma_commit(bar_mma);
   }
-  __syncwarp();
-  mbar_wait(bar_mma, 0);
-  tc_fence_after();
+  // warpgroups whose 64 query rows all lie beyond the crop group (ragged last tile: 197 = 128 + 69) have nothing to do
+  const int wq0 = q0 + wg * 64;
+  if (wq0 >= sh.span) return;
+  mbar_wait(bar, 0);
 
-  // ---- softmax over this thread's half of the key columns
-  const uint32_t t_row = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-  const int csplit = ((sh.Nkp / 16 + 1) / 2) * 16;
-  const int cbeg = ch ? csplit : 0, cend = ch ? sh.Nkp : csplit;
+  const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
+  RowInfo ri[2];
+  ri[0] = row_info(sh, c, wq0 + r_in);
+  ri[1] = row_info(sh, c, wq0 + r_in + 8);
+  // key blocks any row of this warpgroup needs (packed short crops: only the blocks of its own crops)
+  const int b_lo = (min(wq0 / sh.N, sh.G - 1) * sh.N) >> 6;
+  const int b_hi = min(sh.nkb, ((min(min(wq0 + 63, sh.span - 1) / sh.N, sh.G - 1) + 1) * sh.N + 63) >> 6);
   const float cs = sh.scale * LOG2E;
-  float mx = -3.0e38f;
-  // warps whose 32 query rows all lie beyond the crop group (ragged last tile: 197 = 128 + 69) skip the row math; their
-  // P rows stay undefined, which only feeds output rows that are never stored
-  const bool warp_live = q0 + (warp & 3) * 32 < sh.span;
-  for (int c0 = cbeg; warp_live && c0 < cend; c0 += 16) {
-    uint32_t v[16];
-    tmem_ld16(t_row + c0, v);
-    tmem_ld_wait();
-    if (c0 >= klo && c0 + 16 <= khi) {
+  float m[2] = {-3.0e38f, -3.0e38f}, l[2] = {0.f, 0.f};
+  float o[32];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) mx = fmaxf(mx, __uint_as_float(v[j]));
-    } else {
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-        if (c0 + j >= klo && c0 + j < khi) mx = fmaxf(mx, __uint_as_float(v[j]));
-    }
-  }
-  red[ch * 128 + r] = mx;
-  __syncthreads();
-  mx = fmaxf(red[r], red[128 + r]);
-  __syncthreads();
-  const float mxs = mx * cs;
-  float sum = 0.f;
-  // the MMA that read sQ / sK has completed (bar_mma), so region A may now be overwritten with P
-  for (int c0 = cbeg; warp_live && c0 < cend; c0 += 16) {
-    uint32_t v[16];
-    tmem_ld16(t_row + c0, v);
-    tmem_ld_wait();
-    float p[16];
-    if (c0 >= klo && c0 + 16 <= khi) {          // whole chunk inside this row's crop
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        p[j] = ex2_approx(fmaf(__uint_as_float(v[j]), cs, -mxs));
-        sum += p[j];
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        p[j] = (c0 + j >= klo && c0 + j < khi) ? ex2_approx(fmaf(__uint_as_float(v[j]), cs, -mxs)) : 0.f;
-        sum += p[j];
-      }
-    }
-    uint8_t* chunk = sP + (c0 >> 6) * 16384;
-    const int cc = c0 & 63;
-    *reinterpret_cast<uint4*>(chunk + sw128_offset(r, cc)) =
-        make_uint4(pack_bf16(p[0], p[1]), pack_bf16(p[2], p[3]), pack_bf16(p[4], p[5]), pack_bf16(p[6], p[7]));
-    *reinterpret_cast<uint4*>(chunk + sw128_offset(r, cc + 8)) =
-        make_uint4(pack_bf16(p[8], p[9]), pack_bf16(p[10], p[11]), pack_bf16(p[12], p[13]), pack_bf16(p[14], p[15]));
-  }
-  red[ch * 128 + r] = sum;
-  fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-  tc_fence_before();
-  __syncthreads();
-  sum = red[r] + red[128 + r];
-  if (warp == 0 && elect_one()) {
-    tc_fence_after();
-    // O[128, 64] = P[128, Nkp] V[Nkp, 64]  (A = P K-major, B = V MN-major: 16 keys per UMMA_K = 2 x 1024 B)
-    const uint32_t pa = smem_u32(sP), va = smem_u32(sV);
-    const uint32_t idesc = umma_idesc_bf16(128, 64, 0, 1);
-    const int ksteps = sh.Nkp / 16;
-    for (int k = 0; k < ksteps; ++k) {
-      const uint64_t ad = umma_desc_sw128(pa + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024);
-      const uint64_t bd = umma_desc_sw128(va + k * 2048, 8192, 1024);
-      umma_bf16(tmem, ad, bd, idesc, k > 0);   // O aliases the (fully consumed) S columns [0, 64)
-    }
-    umma_commit(bar_mma);
-  }
-  __syncwarp();
-  mbar_wait(bar_mma, 1);
-  tc_fence_after();
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  const uint64_t qd = gmma_desc_sw128(smem_u32(sQ + wg * 8192), 16, 1024);
 
-  const float inv = 1.f / sum;
-  uint32_t o[32];
-  tmem_ld32(t_row + ch * 32, o);
-  tmem_ld_wait();
-  if (q_valid) {
-    __nv_bfloat16* dst = O + (size_t)(row_base + q_abs) * sh.D + h * 64 + ch * 32;
+#pragma unroll 1
+  for (int b = b_lo; b < b_hi; ++b) {
+    float s[32];
+    const uint64_t kd = gmma_desc_sw128(smem_u32(sK + b * 8192), 16, 1024);
+    fence_regs(o);
+    wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      reinterpret_cast<uint4*>(dst)[j] = make_uint4(
-          pack_bf16(__uint_as_float(o[8 * j]) * inv, __uint_as_float(o[8 * j + 1]) * inv),
-          pack_bf16(__uint_as_float(o[8 * j + 2]) * inv, __uint_as_float(o[8 * j + 3]) * inv),
-          pack_bf16(__uint_as_float(o[8 * j + 4]) * inv, __uint_as_float(o[8 * j + 5]) * inv),
-          pack_bf16(__uint_as_float(o[8 * j + 6]) * inv, __uint_as_float(o[8 * j + 7]) * inv));
+    for (int k = 0; k < 4; ++k) wgmma_m64n64k16_ss<0, 0>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    // ---- online softmax of the two rows this thread holds (columns 8i + c2 + {0,1})
+    const int kb0 = b * 64 + c2;
+    const bool full = kb0 - c2 >= max(ri[0].klo, ri[1].klo) && kb0 - c2 + 64 <= min(ri[0].khi, ri[1].khi);
+    float mx[2] = {-3.0e38f, -3.0e38f};
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int hh = j >> 1, kk = kb0 + 8 * i + (j & 1);
+        if (full || (kk >= ri[hh].klo && kk < ri[hh].khi)) mx[hh] = fmaxf(mx[hh], s[4 * i + j]);
+      }
+    float corr[2], ms[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+      const float mn = fmaxf(m[hh], mx[hh]);
+      corr[hh] = ex2_approx((m[hh] - mn) * cs);
+      m[hh] = mn;
+      ms[hh] = mn * cs;
+      l[hh] *= corr[hh];
     }
-    if (LSE && ch == 0)   // natural-log LSE of the scaled scores, indexed [crop, head, token]
-      LSE[((size_t)(c * sh.G + g) * sh.H + h) * sh.N + (q_abs - klo)] = mx * sh.scale + logf(sum);
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int hh = j >> 1, kk = kb0 + 8 * i + (j & 1);
+        const float p = (full || (kk >= ri[hh].klo && kk < ri[hh].khi)) ? ex2_approx(fmaf(s[4 * i + j], cs, -ms[hh])) : 0.f;
+        s[4 * i + j] = p;
+        l[hh] += p;
+        o[4 * i + j] *= corr[hh];
+      }
+    // ---- O += P V (A = P from registers, B = V block MN-major: 16 keys per k-step = 2048 B)
+    uint32_t a[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) a[kk][e] = pack_bf16(s[8 * kk + 2 * e], s[8 * kk + 2 * e + 1]);
+    const uint64_t vd = gmma_desc_sw128(smem_u32(sV + b * 8192), 8192, 1024);
+    fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs<1>(o, a[kk], vd + 128 * kk, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_free<TMEM_COLS>(tmem);
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+    const int q = wq0 + r_in + 8 * hh;
+    if (!ri[hh].ok) continue;
+    const float inv = 1.f / l[hh];
+    __nv_bfloat16* dst = O + (size_t)(row_base + q) * sh.D + h * 64 + c2;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
+    if (LSE && c2 == 0)   // natural-log LSE of the scaled scores, indexed [crop, head, token]
+      LSE[((size_t)(c * sh.G + ri[hh].g) * sh.H + h) * sh.N + (q - ri[hh].klo)] = m[hh] * sh.scale + logf(l[hh]);
+  }
+  dbg_mark(1);
 }
 
 // Delta[c,h,q] = sum_d dO[q, h, d] * O[q, h, d]    (backward softmax term)
@@ -239,591 +205,211 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ O, const __n
 }
 
 // ------------------------------------------------------------------------------------------------ backward
-// One CTA per (head, crop); N <= 256 (2 query tiles x 2 key tiles of 128).  For each key tile kt and query tile qt:
-//   S  = Q K^T, dP = dO V^T           (tensor memory, 128 + 128 columns)
-//   P  = exp(S*scale - lse), dS = P * (dP - Delta) * scale     -> bf16 tiles in shared memory
-//   dV[kt] += P^T dO,  dK[kt] += dS^T Q   (A = P / dS read MN-major, B = dO / Q read MN-major)
-//   dQ[qt] += dS K                        (A = dS K-major, B = K MN-major)
-// dQ accumulates in tensor memory across key tiles (2 x 64 columns), dK/dV across query tiles (64 + 64).
-// inverse RoPE on a gradient row held in registers (a[0..31] = first half, a[32..63] = second half of the head):
-// transpose of y = x*cos + rot_half(x)*sin  (dinov3_jax/layers/attention.py:14-20)
-__device__ __forceinline__ void rope_inverse_row(float (&a)[64], const float* __restrict__ sin_row,
-                                                 const float* __restrict__ cos_row) {
+// One CTA per (head, crop group); span <= 384 (up to 3 query tiles x 3 key tiles of 128), two warpgroups of 64 rows.
+// Q and dO tiles stay resident; K / V come one 128-key tile at a time.  For a tile pair (kt, qt):
+//   S  = Q K^T, dP = dO V^T                                    (registers)
+//   P  = exp(S*scale - lse), dS = P * (dP - Delta) * scale
+// Phase 1 (kt outer, qt inner): P and dS go to shared memory as bf16 SWIZZLE_128B tiles [128 q x 128 keys], then
+//   dV[kt] += P^T dO, dK[kt] += dS^T Q      (A = P / dS read MN-major: each warpgroup owns 64 keys)
+// Phase 2 (qt outer, kt inner): S and dP are recomputed and dQ[qt] += dS K with dS straight from registers (RS form).
+// The recomputation costs two small products per tile pair and keeps every accumulator in registers.
+// inverse RoPE on the gradient: transpose of y = x*cos + rot_half(x)*sin (dinov3_jax/layers/attention.py:14-20); this
+// thread holds columns d = 8i + c2 + {0,1} of a row, i.e. both partners (d, d + 32) of every rotation pair it touches.
+__device__ __forceinline__ void store_grad_rows(float (&a)[32], const AttnShape& sh, int c, int row_base, int tile_row0,
+                                                int r_in, int c2, int h, int third, bool rope, __nv_bfloat16* dQKV) {
 #pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const float4 s4 = *reinterpret_cast<const float4*>(sin_row + j);
-    const float4 c4 = *reinterpret_cast<const float4*>(cos_row + j);
-    const float sn[4] = {s4.x, s4.y, s4.z, s4.w}, cs[4] = {c4.x, c4.y, c4.z, c4.w};
+  for (int hh = 0; hh < 2; ++hh) {
+    const int row = tile_row0 + r_in + 8 * hh;
+    const RowInfo ri = row_info(sh, c, row);
+    if (!ri.ok) continue;
+    const int tok = row - ri.klo;
+    float v[16];
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float lo = a[j + e], hi = a[j + e + 32];
-      a[j + e] = lo * cs[e] + hi * sn[e];
-      a[j + e + 32] = hi * cs[e] - lo * sn[e];
+    for (int i = 0; i < 8; ++i) { v[2 * i] = a[4 * i + 2 * hh]; v[2 * i + 1] = a[4 * i + 2 * hh + 1]; }
+    if (rope && sh.sin_t && tok >= sh.prefix) {
+      const float* sn = sh.sin_t + (size_t)(tok - sh.prefix) * 64;
+      const float* cn = sh.cos_t + (size_t)(tok - sh.prefix) * 64;
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int d = 8 * i + c2 + j;
+          const float lo = v[2 * i + j], hi = v[2 * (i + 4) + j];
+          v[2 * i + j] = lo * cn[d] + hi * sn[d];
+          v[2 * (i + 4) + j] = hi * cn[d] - lo * sn[d];
+        }
     }
+    __nv_bfloat16* dst = dQKV + (size_t)(row_base + row) * (3 * sh.D) + third * sh.D + h * 64 + c2;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16(v[2 * i], v[2 * i + 1]);
   }
-}
-__device__ __forceinline__ void store_row64_bf16(__nv_bfloat16* dst, const float (&a)[64]) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j)
-    reinterpret_cast<uint4*>(dst)[j] = make_uint4(pack_bf16(a[8 * j], a[8 * j + 1]), pack_bf16(a[8 * j + 2], a[8 * j + 3]),
-                                                  pack_bf16(a[8 * j + 4], a[8 * j + 5]), pack_bf16(a[8 * j + 6], a[8 * j + 7]));
-}
-__device__ __forceinline__ void load_row64(uint32_t taddr, float (&a)[64]) {
-  uint32_t u[64];
-  tmem_ld32(taddr, u);
-  tmem_ld32(taddr + 32, u + 32);
-  tmem_ld_wait();
-#pragma unroll
-  for (int j = 0; j < 64; ++j) a[j] = __uint_as_float(u[j]);
 }
 
 __global__ void __launch_bounds__(256)
-attn_bwd_alias_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
+attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
                 const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
                 const AttnShape sh) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int nQ_ = (sh.span + 127) / 128;       // query tiles (all stay resident): 1..3
+  const int nQ = (sh.span + 127) / 128, nK = nQ;
   uint8_t* sQ = smem;                          // [nQ][128 x 64]
-  uint8_t* sDO = sQ + nQ_ * 16384;             // [nQ][128 x 64]
-  uint8_t* sK = sDO + nQ_ * 16384;             // 16 KB (current key tile)
+  uint8_t* sDO = sQ + nQ * 16384;              // [nQ][128 x 64]
+  uint8_t* sK = sDO + nQ * 16384;              // 16 KB (current key tile)
   uint8_t* sV = sK + 16384;                    // 16 KB
   uint8_t* sP = sV + 16384;                    // [2 chunks of 64 keys][128 q x 128 B] 32 KB
   uint8_t* sDS = sP + 32768;                   // 32 KB
   uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + 32768);
-  uint64_t* bar_q = bars;             // Q / dO tiles
+  uint64_t* bar_q = bars;
   uint64_t* bar_kv = bars + 1;
-  uint64_t* bar_mma = bars + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
 
-  // 256 threads: two per row (r = tid & 127); ch = tid >> 7 picks the key-column half in the elementwise phase,
-  // dK (ch 0) vs dV (ch 1) in the key-tile output phase, and the query tile in the dQ output phase
-  const int warp = threadIdx.x >> 5;
-  const int r = threadIdx.x & 127;
-  const int ch = threadIdx.x >> 7;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
   const int h = blockIdx.x, c = blockIdx.y;
   const int row_base = c * sh.span;
-  const int nQ = (sh.span + 127) / 128, nK = nQ;
-
+  const float cs = sh.scale * LOG2E;
+  dbg_mark(0);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmDO);
     mbar_init(bar_q, 1);
     mbar_init(bar_kv, 1);
-    mbar_init(bar_mma, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  // TMEM columns: S [0,128) | dP [128,256) | dK [256,320) | dV [320,384) | dQ[qt] [384 + 64 qt, ...)
-  // with three query tiles (256 < N <= 384) dP reuses the S columns (S is turned into P first) and everything moves down
-  const bool alias = nQ > 2;
-  const uint32_t tS = tmem, tDP = alias ? tmem : tmem + 128, tDK = tmem + (alias ? 128 : 256),
-                 tDV = tmem + (alias ? 192 : 320), tDQ = tmem + (alias ? 256 : 384);
-  const uint32_t t_lane = (uint32_t)((warp & 3) * 32) << 16;
-
-  if (threadIdx.x == 0) {
+  if (threadIdx.x < 32 && elect_one()) {
     mbar_expect_tx(bar_q, nQ * 2 * 16384);
     for (int qt = 0; qt < nQ; ++qt) {
       tma_load_2d(&tmQKV, bar_q, sQ + qt * 16384, h * 64, row_base + qt * 128);
       tma_load_2d(&tmDO, bar_q, sDO + qt * 16384, h * 64, row_base + qt * 128);
     }
   }
-  uint32_t mma_phase = 0, kv_phase = 0;
-  const float cs = sh.scale * LOG2E;
-
-  for (int kt = 0; kt < nK; ++kt) {
-    if (threadIdx.x == 0) {
+  uint32_t kv_phase = 0;
+  int kv_loaded = -1;
+  auto load_kv = [&](int kt) {       // every thread: K / V tile kt resident (the previous tile's readers are done)
+    if (kv_loaded == kt) return;
+    __syncthreads();
+    if (threadIdx.x < 32 && elect_one()) {
       mbar_expect_tx(bar_kv, 2 * 16384);
       tma_load_2d(&tmQKV, bar_kv, sK, sh.D + h * 64, row_base + kt * 128);
       tma_load_2d(&tmQKV, bar_kv, sV, 2 * sh.D + h * 64, row_base + kt * 128);
     }
-    for (int qt = 0; qt < nQ; ++qt) {
-      if (threadIdx.x == 0) {
-        if (kt == 0 && qt == 0) mbar_wait(bar_q, 0);
-        if (qt == 0) mbar_wait(bar_kv, kv_phase);
-        tc_fence_after();
-        const uint32_t qa = smem_u32(sQ + qt * 16384), doa = smem_u32(sDO + qt * 16384);
-        const uint32_t ka = smem_u32(sK), va = smem_u32(sV);
-        const uint32_t idesc = umma_idesc_bf16(128, 128, 0, 0);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(tS, umma_desc_sw128(qa + k * 32, 16, 1024), umma_desc_sw128(ka + k * 32, 16, 1024), idesc, k > 0);
-        if (!alias) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(tDP, umma_desc_sw128(doa + k * 32, 16, 1024), umma_desc_sw128(va + k * 32, 16, 1024), idesc, k > 0);
-        }
-        umma_commit(bar_mma);
-      }
-      __syncwarp();
-      mbar_wait(bar_mma, mma_phase);
-      mma_phase ^= 1;
-      tc_fence_after();
-
-      // ---- elementwise: this thread owns query row q = qt*128 + r and key columns [64 ch, 64 ch + 64)
-      const int q = qt * 128 + r;
-      const int g = min(q / sh.N, sh.G - 1);
-      const int klo = g * sh.N, khi = klo + sh.N;      // keys of the same crop (block-diagonal when crops are packed)
-      const bool q_ok = (q < sh.span) && (c * sh.G + g < sh.n_crops);
-      const size_t stat = ((size_t)(c * sh.G + g) * sh.H + h) * sh.N + (q_ok ? q - klo : 0);
-      const float lse2 = q_ok ? LSE[stat] * LOG2E : 0.f;
-      const float dl = q_ok ? Delta[stat] : 0.f;
-      uint8_t* pc = sP + ch * 16384;
-      uint8_t* dc = sDS + ch * 16384;
-      if (!alias) {
-#pragma unroll 1
-        for (int cc = 0; cc < 64; cc += 16) {
-          const int c0 = ch * 64 + cc;
-          uint32_t s[16], dp[16];
-          tmem_ld16(tS + t_lane + c0, s);
-          tmem_ld16(tDP + t_lane + c0, dp);
-          tmem_ld_wait();
-          float p[16], ds[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int kk = kt * 128 + c0 + j;
-            const bool ok = q_ok && kk >= klo && kk < khi;
-            p[j] = ok ? exp2f(__uint_as_float(s[j]) * cs - lse2) : 0.f;
-            ds[j] = ok ? p[j] * (__uint_as_float(dp[j]) - dl) * sh.scale : 0.f;
-          }
-          *reinterpret_cast<uint4*>(pc + sw128_offset(r, cc)) =
-              make_uint4(pack_bf16(p[0], p[1]), pack_bf16(p[2], p[3]), pack_bf16(p[4], p[5]), pack_bf16(p[6], p[7]));
-          *reinterpret_cast<uint4*>(pc + sw128_offset(r, cc + 8)) =
-              make_uint4(pack_bf16(p[8], p[9]), pack_bf16(p[10], p[11]), pack_bf16(p[12], p[13]), pack_bf16(p[14], p[15]));
-          *reinterpret_cast<uint4*>(dc + sw128_offset(r, cc)) =
-              make_uint4(pack_bf16(ds[0], ds[1]), pack_bf16(ds[2], ds[3]), pack_bf16(ds[4], ds[5]), pack_bf16(ds[6], ds[7]));
-          *reinterpret_cast<uint4*>(dc + sw128_offset(r, cc + 8)) = make_uint4(
-              pack_bf16(ds[8], ds[9]), pack_bf16(ds[10], ds[11]), pack_bf16(ds[12], ds[13]), pack_bf16(ds[14], ds[15]));
-        }
-      } else {
-        // pass 1: P from S (kept in registers as bf16 pairs, 64 columns -> 32 words), written to sP
-        uint32_t pk[32];
-#pragma unroll
-        for (int cc = 0; cc < 64; cc += 16) {
-          const int c0 = ch * 64 + cc;
-          uint32_t s[16];
-          tmem_ld16(tS + t_lane + c0, s);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            const int kk = kt * 128 + c0 + j;
-            const float p0 = (q_ok && kk >= klo && kk < khi) ? exp2f(__uint_as_float(s[j]) * cs - lse2) : 0.f;
-            const float p1 = (q_ok && kk + 1 >= klo && kk + 1 < khi) ? exp2f(__uint_as_float(s[j + 1]) * cs - lse2) : 0.f;
-            pk[(cc + j) >> 1] = pack_bf16(p0, p1);
-          }
-          *reinterpret_cast<uint4*>(pc + sw128_offset(r, cc)) = make_uint4(pk[cc / 2], pk[cc / 2 + 1], pk[cc / 2 + 2], pk[cc / 2 + 3]);
-          *reinterpret_cast<uint4*>(pc + sw128_offset(r, cc + 8)) = make_uint4(pk[cc / 2 + 4], pk[cc / 2 + 5], pk[cc / 2 + 6], pk[cc / 2 + 7]);
-        }
-        tc_fence_before();
-        __syncthreads();          // every thread has consumed S: the dP MMA may overwrite those columns
-        if (threadIdx.x == 0) {
-          tc_fence_after();
-          const uint32_t doa = smem_u32(sDO + qt * 16384), va = smem_u32(sV);
-          const uint32_t idesc = umma_idesc_bf16(128, 128, 0, 0);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(tDP, umma_desc_sw128(doa + k * 32, 16, 1024), umma_desc_sw128(va + k * 32, 16, 1024), idesc, k > 0);
-          umma_commit(bar_mma);
-        }
-        __syncwarp();
-        mbar_wait(bar_mma, mma_phase);
-        mma_phase ^= 1;
-        tc_fence_after();
-        // pass 2: dS = P * (dP - Delta) * scale
-#pragma unroll
-        for (int cc = 0; cc < 64; cc += 16) {
-          const int c0 = ch * 64 + cc;
-          uint32_t dp[16];
-          tmem_ld16(tDP + t_lane + c0, dp);
-          tmem_ld_wait();
-          uint32_t dsw[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            const float2 pp = unpack_bf16(pk[(cc + j) >> 1]);
-            dsw[j >> 1] = pack_bf16(pp.x * (__uint_as_float(dp[j]) - dl) * sh.scale, pp.y * (__uint_as_float(dp[j + 1]) - dl) * sh.scale);
-          }
-          *reinterpret_cast<uint4*>(dc + sw128_offset(r, cc)) = make_uint4(dsw[0], dsw[1], dsw[2], dsw[3]);
-          *reinterpret_cast<uint4*>(dc + sw128_offset(r, cc + 8)) = make_uint4(dsw[4], dsw[5], dsw[6], dsw[7]);
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        tc_fence_after();
-        const uint32_t pa = smem_u32(sP), dsa = smem_u32(sDS);
-        const uint32_t qa = smem_u32(sQ + qt * 16384), doa = smem_u32(sDO + qt * 16384), ka = smem_u32(sK);
-        // dV[128 keys, 64] += P^T dO : A = P as MN-major (M = keys: two 64-key groups 16 KB apart; K = 16 query rows
-        //                               = 2 x 1024 B), B = dO MN-major (N = d: one group)
-        const uint32_t id_tt = umma_idesc_bf16(128, 64, 1, 1);
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_bf16(tDV, umma_desc_sw128(pa + k * 2048, 16384, 1024), umma_desc_sw128(doa + k * 2048, 8192, 1024), id_tt,
-                    (qt > 0 || k > 0));
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_bf16(tDK, umma_desc_sw128(dsa + k * 2048, 16384, 1024), umma_desc_sw128(qa + k * 2048, 8192, 1024), id_tt,
-                    (qt > 0 || k > 0));
-        // dQ[128 q, 64] += dS K : A = dS K-major (64-key chunks 16 KB apart), B = K MN-major
-        const uint32_t id_nt = umma_idesc_bf16(128, 64, 0, 1);
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_bf16(tDQ + qt * 64, umma_desc_sw128(dsa + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
-                    umma_desc_sw128(ka + k * 2048, 8192, 1024), id_nt, (kt > 0 || k > 0));
-        umma_commit(bar_mma);
-      }
-      __syncwarp();
-      // the MMAs read sP / sDS / sK: wait before the next iteration overwrites them
-      mbar_wait(bar_mma, mma_phase);
-      mma_phase ^= 1;
-      tc_fence_after();
-    }
-    // ---- dK (ch 0) / dV (ch 1) of this key tile: thread owns key row kt*128 + r
-    {
-      const int key = kt * 128 + r;
-      const int kg = min(key / sh.N, sh.G - 1);
-      const int tok = key - kg * sh.N;                 // token index inside its crop
-      float a[64];
-      load_row64((ch ? tDV : tDK) + t_lane, a);
-      if (key < sh.span && c * sh.G + kg < sh.n_crops) {
-        if (!ch && sh.sin_t && tok >= sh.prefix)
-          rope_inverse_row(a, sh.sin_t + (size_t)(tok - sh.prefix) * 64, sh.cos_t + (size_t)(tok - sh.prefix) * 64);
-        store_row64_bf16(dQKV + (size_t)(row_base + key) * (3 * sh.D) + (ch ? 2 : 1) * sh.D + h * 64, a);
-      }
-    }
+    mbar_wait(bar_kv, kv_phase);
     kv_phase ^= 1;
-    tc_fence_before();
-    __syncthreads();   // all TMEM reads of dK/dV done before the next key tile's MMAs overwrite them
-    tc_fence_after();
-  }
-  // ---- dQ: query tile qt is written by the threads with ch == (qt & 1)
-  for (int qt = ch; qt < nQ; qt += 2) {
-    const int q = qt * 128 + r;
-    const int qg = min(q / sh.N, sh.G - 1);
-    const int tok = q - qg * sh.N;
-    float a[64];
-    load_row64(tDQ + qt * 64 + t_lane, a);
-    if (q < sh.span && c * sh.G + qg < sh.n_crops) {
-      if (sh.sin_t && tok >= sh.prefix)
-        rope_inverse_row(a, sh.sin_t + (size_t)(tok - sh.prefix) * 64, sh.cos_t + (size_t)(tok - sh.prefix) * 64);
-      store_row64_bf16(dQKV + (size_t)(row_base + q) * (3 * sh.D) + h * 64, a);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_free<512>(tmem);
-}
-
-__global__ void __launch_bounds__(256)
-attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
-                const __grid_constant__ CUtensorMap tmO, const float* __restrict__ LSE,
-                __nv_bfloat16* __restrict__ dQKV, const AttnShape sh, const int n_items) {
-  // Pipelined variant for up to two query / key tiles (span <= 256): one tensor-core commit per (kt, qt) iteration —
-  // the accumulate MMAs of iteration i and the S / dP MMAs of iteration i+1 are issued back to back, K / V tiles are
-  // double-buffered, and every MMA / column loop is trimmed to the valid extent of the (ragged) last tile.
-  // PERSISTENT over (crop group, head) items (item = blockIdx.x + k * gridDim.x, head fastest): tensor memory and the
-  // barriers are set up once per CTA, and the TMA loads of the NEXT item's Q / dO / O / K / V tiles are issued as soon as
-  // the last MMA of the current item has retired — they land while the dK / dV / dQ accumulators are read out, rotated
-  // back and stored (6 k of the 39 k cycles of an item were spent waiting for its tiles).
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int nQ = (sh.span + 127) / 128, nK = nQ;
-  uint8_t* sQ = smem;                          // [nQ][128 x 64]
-  uint8_t* sDO = sQ + nQ * 16384;              // [nQ][128 x 64]
-  uint8_t* sK = sDO + nQ * 16384;              // [2][128 x 64] double-buffered key tile
-  uint8_t* sV = sK + 32768;                    // [2][128 x 64]
-  uint8_t* sP = sV + 32768;                    // [2 chunks of 64 keys][128 q x 128 B] 32 KB
-  uint8_t* sDS = sP + 32768;                   // 32 KB
-  uint8_t* sO = sP;                            // [nQ][128 x 64] forward outputs: only live in the item's prologue (Delta)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + 32768);
-  uint64_t* bar_q = bars;
-  uint64_t* bar_kv = bars + 1;                 // [2]
-  uint64_t* bar_mma = bars + 3;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
-  float* red_delta = reinterpret_cast<float*>(bars + 8);     // [2 query tiles][2 column halves][128 rows]
-
-  const int warp = threadIdx.x >> 5;
-  const int r = threadIdx.x & 127;
-  const int ch = threadIdx.x >> 7;
-  int h = 0, c = 0, row_base = 0;              // the current item (lambdas below read them by reference)
-  const int n_it = nK * nQ;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmQKV);
-    tma_prefetch_desc(&tmDO);
-    tma_prefetch_desc(&tmO);
-    mbar_init(bar_q, 1);
-    mbar_init(&bar_kv[0], 1);
-    mbar_init(&bar_kv[1], 1);
-    mbar_init(bar_mma, 1);
-    fence_mbar_init();
-  }
-  dbg_mark(0);
-  if (warp == 0) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  dbg_mark(1);
-  const uint32_t tS = tmem, tDP = tmem + 128, tDK = tmem + 256, tDV = tmem + 320, tDQ = tmem + 384;
-  const uint32_t t_lane = (uint32_t)((warp & 3) * 32) << 16;
-  const float cs = sh.scale * LOG2E;
-
-  auto tile_extent = [&](int t) { return min(128, ((sh.span - t * 128) + 15) & ~15); };   // valid rows/cols, multiple of 16
-  auto load_item = [&](int item) {     // elected lane of warp 0: every tile of one (crop group, head) item
-    const int hh = item % sh.H, rb = (item / sh.H) * sh.span;
-    mbar_expect_tx(bar_q, nQ * 3 * 16384);
-    for (int qt = 0; qt < nQ; ++qt) {
-      tma_load_2d(&tmQKV, bar_q, sQ + qt * 16384, hh * 64, rb + qt * 128);
-      tma_load_2d(&tmDO, bar_q, sDO + qt * 16384, hh * 64, rb + qt * 128);
-      tma_load_2d(&tmO, bar_q, sO + qt * 16384, hh * 64, rb + qt * 128);
-    }
-    for (int kt = 0; kt < nK; ++kt) {
-      mbar_expect_tx(&bar_kv[kt], 2 * 16384);
-      tma_load_2d(&tmQKV, &bar_kv[kt], sK + kt * 16384, sh.D + hh * 64, rb + kt * 128);
-      tma_load_2d(&tmQKV, &bar_kv[kt], sV + kt * 16384, 2 * sh.D + hh * 64, rb + kt * 128);
-    }
+    kv_loaded = kt;
   };
-  auto issue_sdp = [&](int kt, int qt) {   // thread 0: S = Q K^T and dP = dO V^T for this tile pair, N trimmed
-    const uint64_t qd = umma_desc_sw128(smem_u32(sQ + qt * 16384), 16, 1024), dod = umma_desc_sw128(smem_u32(sDO + qt * 16384), 16, 1024);
-    const uint64_t kd = umma_desc_sw128(smem_u32(sK + (kt & 1) * 16384), 16, 1024), vd = umma_desc_sw128(smem_u32(sV + (kt & 1) * 16384), 16, 1024);
-    const uint32_t idesc = umma_idesc_bf16(128, tile_extent(kt), 0, 0);
+  // S and dP of this warpgroup's 64 query rows of tile qt against key tile kt, turned into P (in s) and dS (in dp)
+  auto p_ds = [&](int qt, int kt, float (&s)[64], float (&dp)[64]) {
+    const uint64_t qd = gmma_desc_sw128(smem_u32(sQ + qt * 16384 + wg * 8192), 16, 1024);
+    const uint64_t dod = gmma_desc_sw128(smem_u32(sDO + qt * 16384 + wg * 8192), 16, 1024);
+    const uint64_t kd = gmma_desc_sw128(smem_u32(sK), 16, 1024);
+    const uint64_t vd = gmma_desc_sw128(smem_u32(sV), 16, 1024);
+    wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k) {   // S and dP are independent accumulator chains: interleave them
-      umma_bf16(tS, qd + (uint64_t)(k * 2), kd + (uint64_t)(k * 2), idesc, k > 0 ? 1u : 0u);
-      umma_bf16(tDP, dod + (uint64_t)(k * 2), vd + (uint64_t)(k * 2), idesc, k > 0 ? 1u : 0u);
+      wgmma_m64n128k16_ss<0, 0>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
+      wgmma_m64n128k16_ss<0, 0>(dp, dod + 2 * k, vd + 2 * k, k > 0 ? 1u : 0u);
     }
-  };
-  auto store_dkdv = [&](int kt) {          // all threads: dK (ch 0) / dV (ch 1) rows of key tile kt
-    const int key = kt * 128 + r;
-    const int kg = min(key / sh.N, sh.G - 1);
-    const int tok = key - kg * sh.N;
-    float a[64];
-    load_row64((ch ? tDV : tDK) + t_lane, a);
-    if (key < sh.span && c * sh.G + kg < sh.n_crops) {
-      if (!ch && sh.sin_t && tok >= sh.prefix)
-        rope_inverse_row(a, sh.sin_t + (size_t)(tok - sh.prefix) * 64, sh.cos_t + (size_t)(tok - sh.prefix) * 64);
-      store_row64_bf16(dQKV + (size_t)(row_base + key) * (3 * sh.D) + (ch ? 2 : 1) * sh.D + h * 64, a);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    fence_regs(dp);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int q = qt * 128 + wg * 64 + r_in + 8 * hh;
+      const RowInfo ri = row_info(sh, c, q);
+      const size_t stat = ((size_t)(c * sh.G + ri.g) * sh.H + h) * sh.N + (ri.ok ? q - ri.klo : 0);
+      const float lse2 = ri.ok ? LSE[stat] * LOG2E : 0.f;
+      const float dl = ri.ok ? Delta[stat] : 0.f;
+      const int lo = ri.ok ? ri.klo - kt * 128 : 0, hi = ri.ok ? ri.khi - kt * 128 : 0;   // valid key columns
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int e = 4 * i + 2 * hh + j, col = 8 * i + c2 + j;
+          const bool ok = col >= lo && col < hi;
+          const float p = ok ? ex2_approx(fmaf(s[e], cs, -lse2)) : 0.f;
+          dp[e] = ok ? (p * sh.scale) * (dp[e] - dl) : 0.f;
+          s[e] = p;
+        }
     }
   };
 
-  // TMA / tcgen05 issue: one ELECTED lane of the converged warp 0 (under `threadIdx.x == 0` ptxas serialises every
-  // UTMALDG / UTCHMMA through an ELECT ... BRA.U.ANY loop, ~60-90 cycles per instruction: the accumulate MMAs of this
-  // kernel (N = 64: 32 tensor cycles each) were issue-bound)
-  if (warp == 0) {
-    if (elect_one() && (int)blockIdx.x < n_items) load_item(blockIdx.x);
-    __syncwarp();
-  }
-  uint32_t mma_phase = 0;
-  uint32_t par = 0;                            // parity of the per-item barriers (bar_q, bar_kv): one completion per item
+  mbar_wait(bar_q, 0);
+  // ---- phase 1: dK, dV of key tile kt (this warpgroup: keys kt*128 + wg*64 ..)
 #pragma unroll 1
-  for (int item = blockIdx.x; item < n_items; item += gridDim.x, par ^= 1) {
-  h = item % sh.H;
-  c = item / sh.H;
-  row_base = c * sh.span;
-  if (warp == 0) {
-    if (elect_one()) {
-      mbar_wait(bar_q, par);
-      mbar_wait(&bar_kv[0], par);
-      tc_fence_after();
-      issue_sdp(0, 0);
-      umma_commit(bar_mma);
-    }
-    __syncwarp();
-  }
-  dbg_mark(2);
-  // ---- Delta[q] = sum_d dO[q, d] * O[q, d] (softmax-backward row term) in the prologue, while the first S / dP products
-  // run: dO and O rows come from their TMA tiles in shared memory (SWIZZLE_128B; the O tile borrows the P staging area,
-  // which is first written after the barrier below); the two threads of a row each take 32 of the 64 head columns.
-  // (Replaces the separate attn_delta pass over O and dO.)
-  float dl_q0 = 0.f, dl_q1 = 0.f;
-  {
-    mbar_wait(bar_q, par);
+  for (int kt = 0; kt < nK; ++kt) {
+    load_kv(kt);
+    float dk[32], dv[32];
 #pragma unroll
-    for (int qt = 0; qt < 2; ++qt) {
-      float part = 0.f;
-      if (qt < nQ) {
-        const uint8_t* drow = sDO + qt * 16384;
-        const uint8_t* orow = sO + qt * 16384;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const uint4 a = *reinterpret_cast<const uint4*>(orow + sw128_offset(r, ch * 32 + i * 8));
-          const uint4 b = *reinterpret_cast<const uint4*>(drow + sw128_offset(r, ch * 32 + i * 8));
-          const float2 a0 = unpack_bf16(a.x), a1 = unpack_bf16(a.y), a2 = unpack_bf16(a.z), a3 = unpack_bf16(a.w);
-          const float2 b0 = unpack_bf16(b.x), b1 = unpack_bf16(b.y), b2 = unpack_bf16(b.z), b3 = unpack_bf16(b.w);
-          part += a0.x * b0.x + a0.y * b0.y + a1.x * b1.x + a1.y * b1.y + a2.x * b2.x + a2.y * b2.y + a3.x * b3.x + a3.y * b3.y;
-        }
-        red_delta[(qt * 2 + ch) * 128 + r] = part;
-      }
-    }
-  }
-  __syncthreads();
-  dl_q0 = red_delta[r] + red_delta[128 + r];
-  if (nQ > 1) dl_q1 = red_delta[256 + r] + red_delta[384 + r];
-
+    for (int i = 0; i < 32; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
 #pragma unroll 1
-  for (int it = 0; it < n_it; ++it) {
-    const int kt = it / nQ, qt = it - kt * nQ;
-    __syncwarp();
-    dbg_mark(3 + it * 4);
-    mbar_wait(bar_mma, mma_phase);     // S / dP of this iteration ready; accumulate MMAs of the previous one retired
-    mma_phase ^= 1;
-    tc_fence_after();
-    dbg_mark(4 + it * 4);
-    if (qt == 0 && kt > 0) {
-      store_dkdv(kt - 1);              // previous key tile complete (its K / V buffer is free again)
-      // (nK <= 2 here, so no further key tile needs that buffer)
-    }
-    // ---- elementwise: query row q = qt*128 + r, this thread's half of the valid key columns
-    const int kcols = tile_extent(kt);
-    const int csplit = ((kcols / 16 + 1) / 2) * 16;
-    const int cbeg = ch ? csplit : 0, cend = ch ? kcols : csplit;
-    const int q = qt * 128 + r;
-    const int g = min(q / sh.N, sh.G - 1);
-    const int klo = g * sh.N, khi = klo + sh.N;
-    const bool q_ok = (q < sh.span) && (c * sh.G + g < sh.n_crops);
-    const size_t stat = ((size_t)(c * sh.G + g) * sh.H + h) * sh.N + (q_ok ? q - klo : 0);
-    const float lse2 = q_ok ? LSE[stat] * LOG2E : 0.f;
-    const float dl = q_ok ? (qt ? dl_q1 : dl_q0) : 0.f;
-    {
-      // 16-column chunks, explicit register ping-pong: the TMEM loads of the next chunk are in flight while the current
-      // one is computed (tcgen05.wait::ld waits for every outstanding load of the thread)
-      auto compute = [&](const uint32_t (&sv)[16], const uint32_t (&dp)[16], int c0) {
-        uint32_t pw[8], dw[8];
-        const int kk0 = kt * 128 + c0;
-        if (q_ok && kk0 >= klo && kk0 + 16 <= khi) {
-          // all 16 keys belong to this row's crop: no per-element masking, SFU exponent
+    for (int qt = 0; qt < nQ; ++qt) {
+      float s[64], dp[64];
+      p_ds(qt, kt, s, dp);
 #pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            const float p0 = ex2_approx(fmaf(__uint_as_float(sv[j]), cs, -lse2));
-            const float p1 = ex2_approx(fmaf(__uint_as_float(sv[j + 1]), cs, -lse2));
-            pw[j >> 1] = pack_bf16(p0, p1);
-            dw[j >> 1] = pack_bf16((p0 * sh.scale) * (__uint_as_float(dp[j]) - dl), (p1 * sh.scale) * (__uint_as_float(dp[j + 1]) - dl));
-          }
-        } else {
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = wg * 64 + r_in + 8 * hh;
 #pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            const int kk = kk0 + j;
-            const bool ok0 = q_ok && kk >= klo && kk < khi, ok1 = q_ok && kk + 1 >= klo && kk + 1 < khi;
-            const float p0 = ok0 ? ex2_approx(fmaf(__uint_as_float(sv[j]), cs, -lse2)) : 0.f;
-            const float p1 = ok1 ? ex2_approx(fmaf(__uint_as_float(sv[j + 1]), cs, -lse2)) : 0.f;
-            pw[j >> 1] = pack_bf16(p0, p1);
-            dw[j >> 1] = pack_bf16((p0 * sh.scale) * (__uint_as_float(dp[j]) - dl), (p1 * sh.scale) * (__uint_as_float(dp[j + 1]) - dl));
-          }
-        }
-        uint8_t* pc = sP + (c0 >> 6) * 16384;
-        uint8_t* dc = sDS + (c0 >> 6) * 16384;
-        const int cc = c0 & 63;
-        *reinterpret_cast<uint4*>(pc + sw128_offset(r, cc)) = make_uint4(pw[0], pw[1], pw[2], pw[3]);
-        *reinterpret_cast<uint4*>(pc + sw128_offset(r, cc + 8)) = make_uint4(pw[4], pw[5], pw[6], pw[7]);
-        *reinterpret_cast<uint4*>(dc + sw128_offset(r, cc)) = make_uint4(dw[0], dw[1], dw[2], dw[3]);
-        *reinterpret_cast<uint4*>(dc + sw128_offset(r, cc + 8)) = make_uint4(dw[4], dw[5], dw[6], dw[7]);
-      };
-      uint32_t svA[16], dpA[16], svB[16], dpB[16];
-      if (cbeg < cend) {
-        tmem_ld16(tS + t_lane + cbeg, svA);
-        tmem_ld16(tDP + t_lane + cbeg, dpA);
-      }
-      tmem_ld_wait();
-#pragma unroll 1
-      for (int c0 = cbeg; c0 < cend; c0 += 32) {
-        const bool hasB = c0 + 16 < cend;
-        if (hasB) {
-          tmem_ld16(tS + t_lane + c0 + 16, svB);
-          tmem_ld16(tDP + t_lane + c0 + 16, dpB);
-        }
-        compute(svA, dpA, c0);
-        tmem_ld_wait();
-        if (hasB) {
-          if (c0 + 32 < cend) {
-            tmem_ld16(tS + t_lane + c0 + 32, svA);
-            tmem_ld16(tDP + t_lane + c0 + 32, dpA);
-          }
-          compute(svB, dpB, c0 + 16);
-          tmem_ld_wait();
+        for (int i = 0; i < 16; ++i) {
+          const uint32_t off = (i >> 3) * 16384 + sw128_offset(row, (8 * i + c2) & 63);
+          *reinterpret_cast<uint32_t*>(sP + off) = pack_bf16(s[4 * i + 2 * hh], s[4 * i + 2 * hh + 1]);
+          *reinterpret_cast<uint32_t*>(sDS + off) = pack_bf16(dp[4 * i + 2 * hh], dp[4 * i + 2 * hh + 1]);
         }
       }
-    }
-    dbg_mark(5 + it * 4);
-    fence_proxy_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    dbg_mark(6 + it * 4);
-    if (warp == 0 && elect_one()) {
-      tc_fence_after();
-      // descriptors are built once; each UMMA_K step only adds a constant to the 14-bit start-address field
-      const uint64_t dP_mn = umma_desc_sw128(smem_u32(sP), 16384, 1024);            // P  as MN-major A (keys x query rows)
-      const uint64_t dS_mn = umma_desc_sw128(smem_u32(sDS), 16384, 1024);           // dS as MN-major A
-      const uint64_t dS_k = umma_desc_sw128(smem_u32(sDS), 16, 1024);               // dS as K-major A (query rows x keys)
-      const uint64_t dO_mn = umma_desc_sw128(smem_u32(sDO + qt * 16384), 8192, 1024);
-      const uint64_t dQ_mn = umma_desc_sw128(smem_u32(sQ + qt * 16384), 8192, 1024);
-      const uint64_t dK_mn = umma_desc_sw128(smem_u32(sK + (kt & 1) * 16384), 8192, 1024);
-      const int qsteps = tile_extent(qt) / 16, ksteps = kcols / 16;
-      constexpr uint32_t id_tt = umma_idesc_bf16(128, 64, 1, 1);
-      constexpr uint32_t id_nt = umma_idesc_bf16(128, 64, 0, 1);
-      const uint32_t acc_kv = qt > 0 ? 1u : 0u, acc_q = kt > 0 ? 1u : 0u;
-      // dV[keys, 64] += P^T dO ; dK[keys, 64] += dS^T Q  (16 query rows per UMMA_K = 2048 B = 128 descriptor units)
-      // dQ[q, 64] += dS K  (A: 64-key chunks 16 KB apart, 32 B per UMMA_K inside a chunk; B: 2048 B per step).
-      // The three accumulators are independent dependency chains: their MMAs are interleaved so that back-to-back
-      // instructions never wait on each other's accumulate latency.
+      fence_proxy_async_smem();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
+      __syncthreads();
+      // dV[keys, 64] += P^T dO ; dK[keys, 64] += dS^T Q   (A MN-major: 16 query rows per k-step = 2048 B)
+      const uint64_t pd = gmma_desc_sw128(smem_u32(sP + wg * 16384), 16384, 1024);
+      const uint64_t sd = gmma_desc_sw128(smem_u32(sDS + wg * 16384), 16384, 1024);
+      const uint64_t dod = gmma_desc_sw128(smem_u32(sDO + qt * 16384), 8192, 1024);
+      const uint64_t qd = gmma_desc_sw128(smem_u32(sQ + qt * 16384), 8192, 1024);
+      fence_regs(dk);
+      fence_regs(dv);
+      wgmma_fence();
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
-        if (k < qsteps) {
-          umma_bf16(tDV, dP_mn + (uint64_t)(k * 128), dO_mn + (uint64_t)(k * 128), id_tt, k > 0 ? 1u : acc_kv);
-          umma_bf16(tDK, dS_mn + (uint64_t)(k * 128), dQ_mn + (uint64_t)(k * 128), id_tt, k > 0 ? 1u : acc_kv);
-        }
-        if (k < ksteps)
-          umma_bf16(tDQ + qt * 64, dS_k + (uint64_t)((k >> 2) * 1024 + (k & 3) * 2), dK_mn + (uint64_t)(k * 128), id_nt,
-                    k > 0 ? 1u : acc_q);
+        wgmma_m64n64k16_ss<1, 1>(dv, pd + 128 * k, dod + 128 * k, 1u);
+        wgmma_m64n64k16_ss<1, 1>(dk, sd + 128 * k, qd + 128 * k, 1u);
       }
-      if (it + 1 < n_it) {             // S / dP of the next iteration ride on the same commit
-        const int kt2 = (it + 1) / nQ, qt2 = (it + 1) - kt2 * nQ;
-        if (kt2 != kt) {
-          mbar_wait(&bar_kv[kt2 & 1], par);
-          tc_fence_after();
-        }
-        issue_sdp(kt2, qt2);
-      }
-      umma_commit(bar_mma);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(dk);
+      fence_regs(dv);
+      __syncthreads();            // both warpgroups are done reading sP / sDS before the next tile pair rewrites them
     }
+    store_grad_rows(dk, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 1, true, dQKV);
+    store_grad_rows(dv, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 2, false, dQKV);
   }
-  dbg_mark(20);
-  __syncwarp();
-  mbar_wait(bar_mma, mma_phase);
-  mma_phase ^= 1;
-  tc_fence_after();
-  dbg_mark(21);
-  // every MMA of this item has retired: its shared-memory tiles are dead -> start the next item's loads now, under the
-  // accumulator read-out below
-  if (warp == 0) {
-    if (elect_one() && item + (int)gridDim.x < n_items) load_item(item + gridDim.x);
-    __syncwarp();
-  }
-  store_dkdv(nK - 1);
-  dbg_mark(22);
-  // ---- dQ: query tile qt is written by the threads with ch == (qt & 1)
-  for (int qt = ch; qt < nQ; qt += 2) {
-    const int q = qt * 128 + r;
-    const int qg = min(q / sh.N, sh.G - 1);
-    const int tok = q - qg * sh.N;
-    float a[64];
-    load_row64(tDQ + qt * 64 + t_lane, a);
-    if (q < sh.span && c * sh.G + qg < sh.n_crops) {
-      if (sh.sin_t && tok >= sh.prefix)
-        rope_inverse_row(a, sh.sin_t + (size_t)(tok - sh.prefix) * 64, sh.cos_t + (size_t)(tok - sh.prefix) * 64);
-      store_row64_bf16(dQKV + (size_t)(row_base + q) * (3 * sh.D) + h * 64, a);
+  // ---- phase 2: dQ of query tile qt (this warpgroup: rows qt*128 + wg*64 ..); the key tiles are walked in alternating
+  // directions so that each walk starts with the tile that is still resident
+#pragma unroll 1
+  for (int qt = 0; qt < nQ; ++qt) {
+    float dq[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+#pragma unroll 1
+    for (int j = 0; j < nK; ++j) {
+      const int kt = (qt & 1) ? j : nK - 1 - j;
+      load_kv(kt);
+      float s[64], dp[64];
+      p_ds(qt, kt, s, dp);
+      uint32_t a[8][4];
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) a[kk][e] = pack_bf16(dp[8 * kk + 2 * e], dp[8 * kk + 2 * e + 1]);
+      const uint64_t kd = gmma_desc_sw128(smem_u32(sK), 8192, 1024);   // K as MN-major B (keys x d)
+      fence_regs(dq);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_rs<1>(dq, a[kk], kd + 128 * kk, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(dq);
     }
+    store_grad_rows(dq, sh, c, row_base, qt * 128 + wg * 64, r_in, c2, h, 0, true, dQKV);
   }
-  dbg_mark(23);
-  }   // items
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_free<512>(tmem);
-  dbg_mark(24);
+  dbg_mark(1);
 }
 
 static int make_map(CUtensorMap* map, const void* ptr, long rows, int cols, int ld, int box_rows) {
@@ -842,11 +428,8 @@ static int attn_shape(AttnShape* s, int n_crops, int N, int D, int H) {
   s->G = (N <= 64) ? (128 / N) : 1;                 // short crops: several per 128-row tile, block-diagonal mask
   if (s->G > n_crops) s->G = n_crops;
   s->span = s->G * N;
-  s->nbox = (s->span + 255) / 256;
-  const int q = 16 * s->nbox;
-  s->Nkp = (s->span + q - 1) / q * q;
-  s->box_rows = s->Nkp / s->nbox;
-  if (s->Nkp > 448) return set_error(D3_ERR_ARG, "attention: N > 448 tokens per crop not supported by the single-pass kernel");
+  s->nkb = (s->span + 63) / 64;
+  if (s->span > 448) return set_error(D3_ERR_ARG, "attention: N > 448 tokens per crop not supported by the single-pass kernel");
   return D3_OK;
 }
 
@@ -857,52 +440,23 @@ using namespace d3;
 extern "C" {
 
 int d3_debug_attn_trace(long long* buf /*device [64] or NULL*/) {
-  attn_ws_set_trace(buf ? buf + 64 : nullptr);      // warp-specialised kernels: [64, 64 + 320) of the same buffer
   cudaError_t e = cudaMemcpyToSymbol(g_attn_dbg, &buf, sizeof(buf));
   return e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
-}
-
-static int attn_ws_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("D3_ATTN_WS");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v;
 }
 
 int d3_attn_fwd(const void* qkv, void* o, float* lse, int n_crops, int N, int D, int H, void* stream) {
   AttnShape s;
   int rc = attn_shape(&s, n_crops, N, D, H);
   if (rc) return rc;
-  if (attn_ws_enabled()) {      // persistent warp-specialised kernel (N <= 256 tokens per crop)
-    int handled = 0;
-    if ((rc = attn_fwd_ws(qkv, o, lse, n_crops, N, D, H, reinterpret_cast<cudaStream_t>(stream), &handled))) return rc;
-    if (handled) return D3_OK;
-  }
   const long T = (long)n_crops * N;
   CUtensorMap tq, tkv;
   if ((rc = make_map(&tq, qkv, T, 3 * D, 3 * D, 128))) return rc;
-  if ((rc = make_map(&tkv, qkv, T, 3 * D, 3 * D, s.box_rows))) return rc;
-  const int kv_bytes = s.Nkp * 128;
-  const int p_chunks = (s.Nkp + 63) / 64;
-  const int regA = max(16384 + kv_bytes, p_chunks * 16384);
-  const int smem = regA + kv_bytes + 64 + 1024 + 1024;
+  if ((rc = make_map(&tkv, qkv, T, 3 * D, 3 * D, 64))) return rc;
+  const int smem = 16384 + 2 * s.nkb * 8192 + 64 + 1024;
+  static bool cfg = false;
+  if (!cfg) { cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); cfg = true; }
   dim3 grid((s.span + 127) / 128, H, (n_crops + s.G - 1) / s.G);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (s.Nkp <= 128) {        // short crops (local 96^2: three crops per tile): 128 TMEM columns -> four CTAs per SM
-    static bool cfg = false;
-    if (!cfg) { cudaFuncSetAttribute(attn_fwd_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); cfg = true; }
-    attn_fwd_kernel<128><<<grid, 256, smem, st>>>(tq, tkv, (__nv_bfloat16*)o, lse, s);
-  } else if (s.Nkp <= 256) {
-    static bool cfg = false;
-    if (!cfg) { cudaFuncSetAttribute(attn_fwd_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); cfg = true; }
-    attn_fwd_kernel<256><<<grid, 256, smem, st>>>(tq, tkv, (__nv_bfloat16*)o, lse, s);
-  } else {
-    static bool cfg = false;
-    if (!cfg) { cudaFuncSetAttribute(attn_fwd_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); cfg = true; }
-    attn_fwd_kernel<512><<<grid, 256, smem, st>>>(tq, tkv, (__nv_bfloat16*)o, lse, s);
-  }
+  attn_fwd_kernel<<<grid, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(tq, tkv, (__nv_bfloat16*)o, lse, s);
   D3_CHECK_LAUNCH();
   return D3_OK;
 }
@@ -915,40 +469,23 @@ int d3_attn_bwd(const void* qkv, const void* o, const void* d_o, const float* ls
   if (rc) return rc;
   if (N > 384) return set_error(D3_ERR_ARG, "d3_attn_bwd: N > 384 tokens per crop not supported (3 query tiles of 128)");
   if ((rope_sin == nullptr) != (rope_cos == nullptr)) return set_error(D3_ERR_ARG, "d3_attn_bwd: sin/cos tables");
+  if (!delta_scratch) return set_error(D3_ERR_ARG, "d3_attn_bwd: delta scratch buffer");
   s.sin_t = rope_sin; s.cos_t = rope_cos; s.prefix = rope_prefix;
   const long T = (long)n_crops * N;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int nq_ = (s.span + 127) / 128;
-  if (nq_ > 2) {       // three-tile (N > 256) kernel: Delta through the scratch buffer; the two-tile kernel computes it inline
-    const long threads = T * (D / 8);
-    attn_delta_kernel<<<(int)((threads + 255) / 256), 256, 0, st>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o,
-                                                                  delta_scratch, T, N, D, H);
-    D3_CHECK_LAUNCH();
-  }
-  CUtensorMap tqkv, tdo, to;
+  const long threads = T * (D / 8);
+  attn_delta_kernel<<<(int)((threads + 255) / 256), 256, 0, st>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o,
+                                                                delta_scratch, T, N, D, H);
+  D3_CHECK_LAUNCH();
+  CUtensorMap tqkv, tdo;
   if ((rc = make_map(&tqkv, qkv, T, 3 * D, 3 * D, 128))) return rc;
   if ((rc = make_map(&tdo, d_o, T, D, D, 128))) return rc;
-  if ((rc = make_map(&to, o, T, D, D, 128))) return rc;
   static bool cfg = false;
-  if (!cfg) {
-    cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-    cudaFuncSetAttribute(attn_bwd_alias_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-    cfg = true;
-  }
+  if (!cfg) { cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024); cfg = true; }
   const int nq = (s.span + 127) / 128;
+  const int smem = 2 * nq * 16384 + 32768 + 65536 + 64 + 1024;
   dim3 grid(H, (n_crops + s.G - 1) / s.G);
-  if (nq > 2) {
-    const int smem = 2 * nq * 16384 + 32768 + 65536 + 64 + 1024;
-    attn_bwd_alias_kernel<<<grid, 256, smem, st>>>(tqkv, tdo, lse, delta_scratch, (__nv_bfloat16*)dqkv, s);
-  } else {
-    const int smem = 2 * nq * 16384 + 65536 + 65536 + 64 + 2048 + 1024;
-    // persistent: one CTA per SM walks the (crop group, head) items; D3_ATTN_BWD_PERSIST=0 launches one CTA per item
-    static int persist = -1;
-    if (persist < 0) { const char* e = getenv("D3_ATTN_BWD_PERSIST"); persist = (e && e[0] == '0') ? 0 : 1; }
-    const int n_items = (int)grid.x * (int)grid.y;
-    const int ctas = persist ? min(n_items, sm_count()) : n_items;
-    attn_bwd_kernel<<<ctas, 256, smem, st>>>(tqkv, tdo, to, lse, (__nv_bfloat16*)dqkv, s, n_items);
-  }
+  attn_bwd_kernel<<<grid, 256, smem, st>>>(tqkv, tdo, lse, delta_scratch, (__nv_bfloat16*)dqkv, s);
   D3_CHECK_LAUNCH();
   return D3_OK;
 }

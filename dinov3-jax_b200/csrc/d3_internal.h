@@ -20,10 +20,8 @@ enum : int {
   EP_ACCUM = D3_EP_ACCUM,
   EP_SCATTER = D3_EP_SCATTER,
   EP_SLOW = 1 << 30,      // internal: force the bounds-checked scalar epilogue
-  EP_ATOMIC = 1 << 29,    // internal: split-K partial sums, fp32 atomic reduction into out
-  EP_DEBUG_NOSTORE = 1 << 27,  // internal (D3_GEMM_DEBUG=1): skip epilogue global traffic
-  EP_M_FASTEST = 1 << 26,      // internal (D3_GEMM_DEBUG=2): M-fastest tile order
-  EP_TMA_EPI = 1 << 25,        // internal: epilogue tiles move through swizzled smem staging + TMA store / load
+  EP_ATOMIC = 1 << 29,    // internal: EP_SCATTER contributions, fp32 atomic adds into the owners' shards
+  EP_SLABS = 1 << 27,     // internal: split-K slice s stores its partial tile at rows [s*M, s*M + M) of `out`
   EP_FAST_ACT = 1 << 28,  // internal: hardware tanh in GELU / GELU' (bf16-rounded outputs)
 };
 
@@ -57,13 +55,17 @@ int encode_tensor_map_2d_bf16(CUtensorMap* map, const void* ptr, const cuuint64_
 int encode_tensor_map_2d(CUtensorMap* map, const void* ptr, int elt_bytes, cuuint64_t cols, cuuint64_t rows,
                          cuuint64_t row_stride_bytes, cuuint32_t box_cols, cuuint32_t box_rows, int swizzle_bytes);
 
+// Deterministic reductions.  A kernel that would add one partial per (slab, element) into a destination with a float
+// atomic (whose order, and so whose rounding, changes from run to run) writes it into slab s of a zeroed, stream-ordered
+// workspace instead; slab_combine then adds the slabs to the destination in slab order, the same bits every run.
+float* slab_workspace(size_t floats, cudaStream_t st);          // nullptr (error set) on failure
+void slab_release(float* ws, cudaStream_t st);
+// dst[r * ld + c] += sum_s ws[s * stride + r * cols + c] for r < rows, c < cols (dst == nullptr: nothing)
+int slab_combine(const float* ws, int slabs, long long stride, long long rows, int cols, float* dst, long long ld,
+                 cudaStream_t st);
+
 int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K,
               GemmEpilogue ep, int tile_n, int split_k, cudaStream_t stream);
-
-// warp-specialised persistent attention (attention_ws.cu); *handled = 0 when the shape must take the single-pass kernels
-int attn_fwd_ws(const void* qkv, void* o, float* lse, int n_crops, int N, int D, int H, cudaStream_t st, int* handled);
-
-void attn_ws_set_trace(long long* buf);
 
 #define D3_CHECK_LAUNCH()                                               \
   do {                                                                  \

@@ -61,11 +61,10 @@ __global__ void assemble_tokens_kernel(const float* __restrict__ tok, const floa
     for (int e = threadIdx.x; e < D4; e += blockDim.x) dst[e] = src[e];
   }
 }
-// backward: dX fp32 [n,1+R+P,D] -> dTok bf16 [n*P, D] (0 where masked); dcls[D] += sum_c dX[c,0];
-// dstorage[R,D] += sum_c dX[c,1..R]; dmask[D] += masked rows
+// backward: dX fp32 [n,1+R+P,D] -> dTok bf16 [n*P, D] (0 where masked); the crop slab's sums of dX[c,0] (cls),
+// of the masked rows (mask token) and of dX[c,1..R] (storage tokens) go to its workspace slab [cls D | mask D | R*D]
 __global__ void assemble_tokens_bwd_kernel(const float* __restrict__ dX, const uint8_t* __restrict__ masks,
-                                           __nv_bfloat16* __restrict__ dTok, float* __restrict__ dcls,
-                                           float* __restrict__ dstorage, float* __restrict__ dmask, int n, int P, int R,
+                                           __nv_bfloat16* __restrict__ dTok, float* __restrict__ ws, int n, int P, int R,
                                            int D) {
   // grid.x = column chunks of 128 floats (threads 128: one column each), grid.y = slabs of whole crops
   const int col = blockIdx.x * blockDim.x + threadIdx.x;
@@ -74,10 +73,15 @@ __global__ void assemble_tokens_bwd_kernel(const float* __restrict__ dX, const u
   const long c0 = blockIdx.y * slab, c1 = min((long)n, c0 + slab);
   if (col >= D) return;
   float acc_cls = 0.f, acc_mask = 0.f;
+  float* slab_ws = ws + (long)blockIdx.y * (2 + R) * D;
+  for (int t = 1; t <= R; ++t) {
+    float acc = 0.f;
+    for (long c = c0; c < c1; ++c) acc += dX[c * N * (long)D + (long)t * D + col];
+    slab_ws[(long)(1 + t) * D + col] = acc;
+  }
   for (long c = c0; c < c1; ++c) {
     const float* row = dX + c * N * (long)D + col;
     acc_cls += row[0];
-    for (int t = 1; t <= R; ++t) atomicAdd(&dstorage[(long)(t - 1) * D + col], row[(long)t * D]);
     for (int t = 0; t < P; ++t) {
       const float g = row[(long)(1 + R + t) * D];
       const bool m = masks && masks[c * P + t];
@@ -85,8 +89,8 @@ __global__ void assemble_tokens_bwd_kernel(const float* __restrict__ dX, const u
       dTok[(c * P + t) * (long)D + col] = __float2bfloat16(m ? 0.f : g);
     }
   }
-  atomicAdd(&dcls[col], acc_cls);
-  if (masks) atomicAdd(&dmask[col], acc_mask);
+  slab_ws[col] = acc_cls;
+  slab_ws[D + col] = acc_mask;
 }
 
 // ------------------------------------------------------------------------------------------------ LayerNorm
@@ -320,7 +324,8 @@ ln_bwd_ls_kernel(const InT* __restrict__ dy, const float* __restrict__ x, const 
                  const float* __restrict__ rstd, const float* __restrict__ scale, const float* __restrict__ dx_add,
                  float* __restrict__ dx, float* __restrict__ dscale, float* __restrict__ dbias, int T, int D,
                  const float* __restrict__ ls_gamma, const __nv_bfloat16* __restrict__ ls_u, int ls_gelu,
-                 __nv_bfloat16* __restrict__ ls_du, float* __restrict__ ls_dgamma, float* __restrict__ ls_dbias) {
+                 __nv_bfloat16* __restrict__ ls_du, float* __restrict__ ls_dgamma, float* __restrict__ ls_dbias,
+                 float* __restrict__ ws) {
   extern __shared__ float part[];                 // [4][D] cross-group reduction of the column sums
   __shared__ float red[2][2][4][2];               // [group][parity][warp][a | b]
   const int grp = threadIdx.x >> 7, t = threadIdx.x & 127, wig = t >> 5, lane = threadIdx.x & 31;
@@ -417,7 +422,7 @@ ln_bwd_ls_kernel(const InT* __restrict__ dy, const float* __restrict__ x, const 
       }
     }
   }
-  // ---- column sums: group 1 -> shared, group 0 adds its own and issues one global atomic per column and quantity
+  // ---- column sums: group 1 -> shared, group 0 adds its own and stores the CTA's partial into its workspace slab
   const bool want_ln = dscale != nullptr;
   if (!want_ln && !tail) return;
   if (grp == 1) {
@@ -441,13 +446,14 @@ ln_bwd_ls_kernel(const InT* __restrict__ dy, const float* __restrict__ x, const 
       if (col < D) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
+          float* slab_ws = ws + (long)blockIdx.x * 4 * D + col + j;   // [dscale | dbias | ls_dgamma | ls_dbias]
           if (want_ln) {
-            atomicAdd(&dscale[col + j], ads[c][j] + part[col + j]);
-            atomicAdd(&dbias[col + j], adb[c][j] + part[D + col + j]);
+            slab_ws[0] = ads[c][j] + part[col + j];
+            slab_ws[D] = adb[c][j] + part[D + col + j];
           }
           if (tail) {
-            if (ls_dgamma && ls_u) atomicAdd(&ls_dgamma[col + j], tdg[c][j] + part[2 * D + col + j]);
-            if (ls_dbias) atomicAdd(&ls_dbias[col + j], tdb[c][j] + part[3 * D + col + j]);
+            if (ls_dgamma && ls_u) slab_ws[2 * D] = tdg[c][j] + part[2 * D + col + j];
+            if (ls_dbias) slab_ws[3 * D] = tdb[c][j] + part[3 * D + col + j];
           }
         }
       }
@@ -476,7 +482,8 @@ ln_bwd_ring_kernel(const InT* __restrict__ dy, const float* __restrict__ x, cons
                    const float* __restrict__ rstd, const float* __restrict__ scale, const float* __restrict__ dx_add,
                    float* __restrict__ dx, float* __restrict__ dscale, float* __restrict__ dbias, int T, int stages,
                    const float* __restrict__ ls_gamma, const __nv_bfloat16* __restrict__ ls_u, int ls_gelu,
-                   __nv_bfloat16* __restrict__ ls_du, float* __restrict__ ls_dgamma, float* __restrict__ ls_dbias) {
+                   __nv_bfloat16* __restrict__ ls_du, float* __restrict__ ls_dgamma, float* __restrict__ ls_dbias,
+                   float* __restrict__ ws) {
   constexpr int D = VPL * 128;
   extern __shared__ __align__(128) uint8_t lnr_smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(lnr_smem);
@@ -609,10 +616,11 @@ ln_bwd_ring_kernel(const InT* __restrict__ dy, const float* __restrict__ x, cons
     if (lane == 0) mbar_arrive(&empty[st]);
   }
 
-  // ---- column sums: every consumer warp has drained its rows; reuse the ring as [8 warps][D] slabs, one quantity at a time
+  // ---- column sums: every consumer warp has drained its rows; reuse the ring as [8 warps][D] slabs, one quantity at a
+  // time; the CTA's totals go to its workspace slab [dscale | dbias | ls_dgamma | ls_dbias]
   float* slab = reinterpret_cast<float*>(ring);
   const int ct = threadIdx.x;                 // consumer threads only
-#define LNR_REDUCE(ACC, DST)                                                                         \
+#define LNR_REDUCE(ACC, DST, Q)                                                                      \
   {                                                                                                  \
     float* dst__ = (DST);                                                                            \
     asm volatile("bar.sync 1, %0;" ::"n"(32 * LNR_CONSUMERS) : "memory");                           \
@@ -626,14 +634,14 @@ ln_bwd_ring_kernel(const InT* __restrict__ dy, const float* __restrict__ x, cons
       for (int e = ct; e < D; e += 32 * LNR_CONSUMERS) {                                             \
         float tot = 0.f;                                                                             \
         _Pragma("unroll") for (int w = 0; w < LNR_CONSUMERS; ++w) tot += slab[w * D + e];            \
-        atomicAdd(&dst__[e], tot);                                                                   \
+        ws[((long)blockIdx.x * 4 + (Q)) * D + e] = tot;                                              \
       }                                                                                              \
     }                                                                                                \
   }
-  LNR_REDUCE(ads, dscale)
-  LNR_REDUCE(adb, dscale ? dbias : nullptr)
-  LNR_REDUCE(tdg, (tail && uB) ? ls_dgamma : nullptr)
-  LNR_REDUCE(tdb, tail ? ls_dbias : nullptr)
+  LNR_REDUCE(ads, dscale, 0)
+  LNR_REDUCE(adb, dscale ? dbias : nullptr, 1)
+  LNR_REDUCE(tdg, (tail && uB) ? ls_dgamma : nullptr, 2)
+  LNR_REDUCE(tdb, tail ? ls_dbias : nullptr, 3)
 #undef LNR_REDUCE
 }
 
@@ -642,7 +650,7 @@ ln_bwd_ring_kernel(const InT* __restrict__ dy, const float* __restrict__ x, cons
 // W bf16 [K, N] (the compute copy the forward used), dW fp32 [K, N]; one CTA per 32 columns.
 __global__ void ls_gamma_from_wgrad_kernel(const __nv_bfloat16* __restrict__ W, const float* __restrict__ dW,
                                            const float* __restrict__ bias, const float* __restrict__ dbias,
-                                           const float* __restrict__ gamma, float* __restrict__ dgamma, int K, int N) {
+                                           const float* __restrict__ gamma, float* __restrict__ ws, int K, int N) {
   // grid (N / 64, K-slabs): a thread owns two adjacent columns of a slab of rows; the 8 warps of the CTA interleave rows
   __shared__ float acc[8][64];
   const int lane = threadIdx.x & 31, wy = threadIdx.x >> 5;
@@ -669,7 +677,7 @@ __global__ void ls_gamma_from_wgrad_kernel(const __nv_bfloat16* __restrict__ W, 
       for (int k = 0; k < 8; ++k) tot += acc[k][threadIdx.x];
       if (blockIdx.y == 0) tot += bias[c] * dbias[c];
       const float g = gamma[c];
-      if (g != 0.f) atomicAdd(&dgamma[c], tot / g);
+      if (g != 0.f) ws[(long)blockIdx.y * N + c] = tot / g;   // this K-slab's share of dgamma[c]
     }
   }
 }
@@ -804,7 +812,7 @@ __global__ void l2norm_bwd_kernel(const __nv_bfloat16* __restrict__ g, const flo
 // given dX fp32 [T,D] and the bf16 stash u: du bf16 = dX*gamma*act'(u); dgamma += colsum(dX*act(u)); dbias += colsum(du)
 __global__ void ls_act_bwd_kernel(const float* __restrict__ dX, const __nv_bfloat16* __restrict__ u,
                                   const float* __restrict__ gamma, __nv_bfloat16* __restrict__ du,
-                                  float* __restrict__ dgamma, float* __restrict__ dbias, int T, int D, int use_gelu) {
+                                  float* __restrict__ ws, int T, int D, int use_gelu) {
   const int col = blockIdx.x * blockDim.x + threadIdx.x;
   const long slab = ((long)T + gridDim.y - 1) / gridDim.y;
   const long r0 = blockIdx.y * slab, r1 = min((long)T, r0 + slab);
@@ -821,12 +829,12 @@ __global__ void ls_act_bwd_kernel(const float* __restrict__ dX, const __nv_bfloa
     ab += d;
     du[r * D + col] = __float2bfloat16(d);
   }
-  atomicAdd(&dgamma[col], ag);
-  atomicAdd(&dbias[col], ab);
+  ws[(long)blockIdx.y * 2 * D + col] = ag;        // row slab's share of [dgamma | dbias]
+  ws[(long)blockIdx.y * 2 * D + D + col] = ab;
 }
 
-// out[n] += sum_t x[t, n]   (bias gradients).  x bf16 [T, N]
-__global__ void colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out, long T, int N, int ld) {
+// ws[slab][n] = sum over the row slab of x[t, n]   (bias gradients; the slabs are added in order).  x bf16 [T, N]
+__global__ void colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ ws, long T, int N, int ld) {
   const int col = (blockIdx.x * blockDim.x + threadIdx.x) * 2;
   const long slab = (T + gridDim.y - 1) / gridDim.y;
   const long r0 = blockIdx.y * slab, r1 = min(T, r0 + slab);
@@ -837,18 +845,18 @@ __global__ void colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, float* _
       float2 v = unpack_bf16(*reinterpret_cast<const uint32_t*>(x + r * ld + col));
       a0 += v.x; a1 += v.y;
     }
-    atomicAdd(&out[col], a0);
-    atomicAdd(&out[col + 1], a1);
+    ws[(long)blockIdx.y * N + col] = a0;
+    ws[(long)blockIdx.y * N + col + 1] = a1;
   } else {
     for (long r = r0; r < r1; ++r) a0 += __bfloat162float(x[r * ld + col]);
-    atomicAdd(&out[col], a0);
+    ws[(long)blockIdx.y * N + col] = a0;
   }
 }
 
 
 // 128-bit version: a thread owns 8 adjacent columns; blockDim = (32, 8): 8 row phases per CTA, reduced in shared memory
 __global__ void __launch_bounds__(256)
-colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out, long T, int N, int ld) {
+colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ ws, long T, int N, int ld) {
   __shared__ float red[8][32][9];
   const int col = (blockIdx.x * 32 + threadIdx.x) * 8;
   const long slab = (T + gridDim.y - 1) / gridDim.y;
@@ -873,7 +881,7 @@ colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ 
     float tot = 0.f;
 #pragma unroll
     for (int y = 0; y < 8; ++y) tot += red[y][lc][j];
-    atomicAdd(&out[c], tot);
+    ws[(long)blockIdx.y * N + c] = tot;
   }
 }
 
@@ -1066,8 +1074,19 @@ static void launch_ln_bwd_fused(const void* dy, int dy_is_f32, const float* x, c
 }
 
 
+// adds the CTAs' [dscale | dbias | ls_dgamma | ls_dbias] slabs of the LayerNorm backward kernels to the destinations
+// (nullptr: skipped; a quantity a kernel did not compute adds zeros) and releases the workspace
+static int combine_ln_slabs(float* ws, int slabs, int D, float* dscale, float* dbias, float* ls_dgamma, float* ls_dbias,
+                            cudaStream_t st) {
+  float* dst[4] = {dscale, dbias, ls_dgamma, ls_dbias};
+  int rc = D3_OK;
+  for (int q = 0; q < 4 && !rc; ++q) rc = slab_combine(ws + (long)q * D, slabs, 4LL * D, 1, D, dst[q], D, st);
+  slab_release(ws, st);
+  return rc;
+}
+
 template <int NC>
-static void launch_ln_bwd_ls(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
+static int launch_ln_bwd_ls(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
                              const float* scale, const float* dx_add, float* dx, float* dscale, float* dbias, int T, int D,
                              const float* ls_gamma, const void* ls_u, int ls_gelu, void* ls_du, float* ls_dgamma,
                              float* ls_dbias, cudaStream_t st) {
@@ -1078,20 +1097,26 @@ static void launch_ln_bwd_ls(const void* dy, int dy_is_f32, const float* x, cons
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f32, ln_bwd_ls_kernel<NC, float>, 256, smem);
     occ_bf16 = max(occ_bf16, 1); occ_f32 = max(occ_f32, 1);
   }
+  const int blocks = min((T + 1) / 2, sm_count() * (dy_is_f32 ? occ_f32 : occ_bf16));
+  float* ws = slab_workspace((size_t)blocks * 4 * D, st);
+  if (!ws) return D3_ERR_CUDA;
   if (dy_is_f32) {
-    const int blocks = min((T + 1) / 2, sm_count() * occ_f32);
     ln_bwd_ls_kernel<NC, float><<<blocks, 256, smem, st>>>((const float*)dy, x, mean, rstd, scale, dx_add, dx, dscale, dbias,
-        T, D, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias);
+        T, D, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias, ws);
   } else {
-    const int blocks = min((T + 1) / 2, sm_count() * occ_bf16);
     ln_bwd_ls_kernel<NC, __nv_bfloat16><<<blocks, 256, smem, st>>>((const __nv_bfloat16*)dy, x, mean, rstd, scale, dx_add, dx,
-        dscale, dbias, T, D, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias);
+        dscale, dbias, T, D, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias, ws);
   }
+  cudaError_t e = cudaPeekAtLastError();
+  if (e != cudaSuccess) { slab_release(ws, st); return set_error(D3_ERR_CUDA, cudaGetErrorString(e)); }
+  count_launch();
+  return combine_ln_slabs(ws, blocks, D, dscale, dbias, ls_dgamma, ls_dbias, st);
 }
 
 
+// 1: shape not served by the ring kernel; otherwise D3_OK or an error
 template <int VPL>
-static bool launch_ln_bwd_ring(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
+static int launch_ln_bwd_ring(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
                                const float* scale, const float* dx_add, float* dx, float* dscale, float* dbias, int T,
                                const float* ls_gamma, const void* ls_u, int ls_gelu, void* ls_du, float* ls_dgamma,
                                float* ls_dbias, cudaStream_t st) {
@@ -1104,22 +1129,27 @@ static bool launch_ln_bwd_ring(const void* dy, int dy_is_f32, const float* x, co
   // a warp can never start waiting for use u of a stage before use u-1 has completed (an mbarrier parity wait that is
   // two phases ahead would return immediately).
   stages = stages / LNR_CONSUMERS * LNR_CONSUMERS;
-  if (stages < LNR_CONSUMERS) return false;
+  if (stages < LNR_CONSUMERS) return 1;
   const size_t need = max(stageB * stages, (size_t)LNR_CONSUMERS * D * sizeof(float));    // ring doubles as the reduction slabs
   const size_t smem = fixed + need;
   static bool cfg_b = false, cfg_f = false;
   const int grid = min(T, sm_count());
   const int threads = 32 * (LNR_CONSUMERS + 1);
+  float* ws = slab_workspace((size_t)grid * 4 * D, st);
+  if (!ws) return D3_ERR_CUDA;
   if (dy_is_f32) {
     if (!cfg_f) { cudaFuncSetAttribute(ln_bwd_ring_kernel<VPL, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024); cfg_f = true; }
     ln_bwd_ring_kernel<VPL, float><<<grid, threads, smem, st>>>((const float*)dy, x, mean, rstd, scale, dx_add, dx, dscale,
-        dbias, T, stages, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias);
+        dbias, T, stages, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias, ws);
   } else {
     if (!cfg_b) { cudaFuncSetAttribute(ln_bwd_ring_kernel<VPL, __nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024); cfg_b = true; }
     ln_bwd_ring_kernel<VPL, __nv_bfloat16><<<grid, threads, smem, st>>>((const __nv_bfloat16*)dy, x, mean, rstd, scale, dx_add,
-        dx, dscale, dbias, T, stages, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias);
+        dx, dscale, dbias, T, stages, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias, ws);
   }
-  return true;
+  cudaError_t e = cudaPeekAtLastError();
+  if (e != cudaSuccess) { slab_release(ws, st); return set_error(D3_ERR_CUDA, cudaGetErrorString(e)); }
+  count_launch();
+  return combine_ln_slabs(ws, grid, D, dscale, dbias, ls_dgamma, ls_dbias, st);
 }
 
 
@@ -1150,10 +1180,21 @@ int d3_assemble_tokens_bwd(const float* dX, const unsigned char* masks, void* dT
                            float* dmask, int n, int P, int R, int D, void* stream) {
   if (R < 0 || (R > 0 && !dstorage)) return set_error(D3_ERR_ARG, "d3_assemble_tokens_bwd: storage gradient pointer");
   dim3 grid((D + 127) / 128, max(1, min(n, 128)));
-  assemble_tokens_bwd_kernel<<<grid, 128, 0, STREAM(stream)>>>(dX, masks, (__nv_bfloat16*)dTok, dcls, dstorage, dmask, n, P,
-                                                              R, D);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  const long long stride = (long long)(2 + R) * D;        // per crop slab: [cls D | mask token D | storage R*D]
+  float* ws = slab_workspace((size_t)grid.y * stride, st);
+  if (!ws) return D3_ERR_CUDA;
+  assemble_tokens_bwd_kernel<<<grid, 128, 0, st>>>(dX, masks, (__nv_bfloat16*)dTok, ws, n, P, R, D);
+  cudaError_t e = cudaPeekAtLastError();
+  int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  if (!rc) {
+    count_launch();
+    rc = slab_combine(ws, grid.y, stride, 1, D, dcls, D, st);
+    if (!rc && masks) rc = slab_combine(ws + D, grid.y, stride, 1, D, dmask, D, st);
+    if (!rc && R > 0) rc = slab_combine(ws + 2 * D, grid.y, stride, 1, R * D, dstorage, R * D, st);
+  }
+  slab_release(ws, st);
+  return rc;
 }
 
 int d3_layernorm_fwd(const float* x, const float* scale, const float* bias, void* y, int y_is_f32, float* mean,
@@ -1229,27 +1270,27 @@ int d3_layernorm_bwd_ls(const void* dy, int dy_is_f32, const float* x, const flo
                        !getenv("D3_LN_NO_RING");
 #define LN_RING_ARGS dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, ls_gamma, ls_u, ls_gelu, ls_du, ls_dgamma, ls_dbias, st
   if (ring_ok && D % 128 == 0 && D / 128 <= 8) {
-    bool done = false;
+    int rc = 1;
     switch (D / 128) {
-      case 1: done = launch_ln_bwd_ring<1>(LN_RING_ARGS); break;
-      case 2: done = launch_ln_bwd_ring<2>(LN_RING_ARGS); break;
-      case 3: done = launch_ln_bwd_ring<3>(LN_RING_ARGS); break;
-      case 4: done = launch_ln_bwd_ring<4>(LN_RING_ARGS); break;
-      case 6: done = launch_ln_bwd_ring<6>(LN_RING_ARGS); break;
-      case 8: done = launch_ln_bwd_ring<8>(LN_RING_ARGS); break;
+      case 1: rc = launch_ln_bwd_ring<1>(LN_RING_ARGS); break;
+      case 2: rc = launch_ln_bwd_ring<2>(LN_RING_ARGS); break;
+      case 3: rc = launch_ln_bwd_ring<3>(LN_RING_ARGS); break;
+      case 4: rc = launch_ln_bwd_ring<4>(LN_RING_ARGS); break;
+      case 6: rc = launch_ln_bwd_ring<6>(LN_RING_ARGS); break;
+      case 8: rc = launch_ln_bwd_ring<8>(LN_RING_ARGS); break;
       default: break;
     }
-    if (done) { D3_CHECK_LAUNCH(); return D3_OK; }
+    if (rc != 1) return rc;
   }
 #undef LN_RING_ARGS
   const int nc = (D + 511) / 512;
 #define LN_LS_ARGS dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, D, ls_gamma, ls_u, ls_gelu, ls_du, ls_dgamma, ls_dbias, st
-  if (nc == 1) launch_ln_bwd_ls<1>(LN_LS_ARGS);
-  else if (nc == 2) launch_ln_bwd_ls<2>(LN_LS_ARGS);
-  else launch_ln_bwd_ls<3>(LN_LS_ARGS);
+  int rc;
+  if (nc == 1) rc = launch_ln_bwd_ls<1>(LN_LS_ARGS);
+  else if (nc == 2) rc = launch_ln_bwd_ls<2>(LN_LS_ARGS);
+  else rc = launch_ln_bwd_ls<3>(LN_LS_ARGS);
 #undef LN_LS_ARGS
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  return rc;
 }
 
 int d3_ls_gamma_from_wgrad(const void* W, const float* dW, const float* bias, const float* dbias, const float* gamma,
@@ -1257,9 +1298,15 @@ int d3_ls_gamma_from_wgrad(const void* W, const float* dW, const float* bias, co
   if (K <= 0 || N <= 0) return D3_OK;
   if (N % 2) return set_error(D3_ERR_ARG, "d3_ls_gamma_from_wgrad: N must be even");
   dim3 grid((N + 63) / 64, max(1, min(32, K / 32)));
-  ls_gamma_from_wgrad_kernel<<<grid, 256, 0, STREAM(stream)>>>((const __nv_bfloat16*)W, dW, bias, dbias, gamma, dgamma, K, N);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  float* ws = slab_workspace((size_t)grid.y * N, st);
+  if (!ws) return D3_ERR_CUDA;
+  ls_gamma_from_wgrad_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)W, dW, bias, dbias, gamma, ws, K, N);
+  cudaError_t e = cudaPeekAtLastError();
+  int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  if (!rc) { count_launch(); rc = slab_combine(ws, grid.y, N, 1, N, dgamma, N, st); }
+  slab_release(ws, st);
+  return rc;
 }
 
 int d3_scatter_add_peers(const float* src, long long n, float* const* peers /*host array [world]*/, int world,
@@ -1365,27 +1412,43 @@ int d3_l2norm_bwd(const void* g, const float* u, const float* nrm, void* du, int
 int d3_ls_act_bwd(const float* dX, const void* u, const float* gamma, void* du, float* dgamma, float* dbias, int T,
                   int D, int use_gelu, void* stream) {
   dim3 grid((D + 127) / 128, min(256, max(1, T / 64)));
-  ls_act_bwd_kernel<<<grid, 128, 0, STREAM(stream)>>>(dX, (const __nv_bfloat16*)u, gamma, (__nv_bfloat16*)du, dgamma,
-                                                     dbias, T, D, use_gelu);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  float* ws = slab_workspace((size_t)grid.y * 2 * D, st);
+  if (!ws) return D3_ERR_CUDA;
+  ls_act_bwd_kernel<<<grid, 128, 0, st>>>(dX, (const __nv_bfloat16*)u, gamma, (__nv_bfloat16*)du, ws, T, D, use_gelu);
+  cudaError_t e = cudaPeekAtLastError();
+  int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  if (!rc) {
+    count_launch();
+    rc = slab_combine(ws, grid.y, 2LL * D, 1, D, dgamma, D, st);
+    if (!rc) rc = slab_combine(ws + D, grid.y, 2LL * D, 1, D, dbias, D, st);
+  }
+  slab_release(ws, st);
+  return rc;
 }
 
 int d3_colsum_bf16(const void* x, float* out, long long T, int N, int ld, void* stream) {
   if (T <= 0) return D3_OK;
   if (ld % 2) return set_error(D3_ERR_ARG, "d3_colsum_bf16: ld % 2");
-  if (N % 8 == 0 && ld % 8 == 0 && (uintptr_t)x % 16 == 0 && T >= 64) {
-    const int gx = (N / 8 + 31) / 32;
-    const int gy = (int)max(1LL, min(T / 32, (long long)(sm_count() * 8 + gx - 1) / gx));
-    colsum_bf16_vec_kernel<<<dim3(gx, gy), dim3(32, 8), 0, STREAM(stream)>>>((const __nv_bfloat16*)x, out, T, N, ld);
-    D3_CHECK_LAUNCH();
-    return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  const bool vec = N % 8 == 0 && ld % 8 == 0 && (uintptr_t)x % 16 == 0 && T >= 64;
+  dim3 grid;
+  if (vec) {
+    grid.x = (N / 8 + 31) / 32;
+    grid.y = (int)max(1LL, min(T / 32, (long long)(sm_count() * 8 + grid.x - 1) / grid.x));
+  } else {
+    grid = dim3((N / 2 + 127) / 128 + ((N / 2) % 128 == 0 && N % 2 ? 1 : 0), (int)min(256LL, max(1LL, T / 64)));
+    if (((N + 1) / 2 + 127) / 128 > (int)grid.x) grid.x = ((N + 1) / 2 + 127) / 128;
   }
-  dim3 grid((N / 2 + 127) / 128 + ((N / 2) % 128 == 0 && N % 2 ? 1 : 0), (int)min(256LL, max(1LL, T / 64)));
-  if (((N + 1) / 2 + 127) / 128 > (int)grid.x) grid.x = ((N + 1) / 2 + 127) / 128;
-  colsum_bf16_kernel<<<grid, 128, 0, STREAM(stream)>>>((const __nv_bfloat16*)x, out, T, N, ld);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  float* ws = slab_workspace((size_t)grid.y * N, st);
+  if (!ws) return D3_ERR_CUDA;
+  if (vec) colsum_bf16_vec_kernel<<<grid, dim3(32, 8), 0, st>>>((const __nv_bfloat16*)x, ws, T, N, ld);
+  else colsum_bf16_kernel<<<grid, 128, 0, st>>>((const __nv_bfloat16*)x, ws, T, N, ld);
+  cudaError_t e = cudaPeekAtLastError();
+  int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  if (!rc) { count_launch(); rc = slab_combine(ws, grid.y, N, 1, N, out, N, st); }
+  slab_release(ws, st);
+  return rc;
 }
 
 int d3_cast_f32_bf16(const float* src, void* dst, long long n, void* stream) {

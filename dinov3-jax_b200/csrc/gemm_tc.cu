@@ -1,25 +1,23 @@
-// Persistent, warp-specialised bf16 GEMM on the 5th-gen tensor cores (tcgen05.mma, TMEM accumulators, TMA
-// operand staging).  One kernel family covers every dense contraction on the DINOv3 training path:
+// Persistent, warp-specialised bf16 GEMM on the Hopper tensor cores (wgmma, register accumulators, TMA operand
+// staging through an mbarrier ring).  One kernel family covers every dense contraction on the DINOv3 training path:
 //   forward  Y = X W        (A K-major, B MN-major: reference kernels are stored [in,out])
 //   dgrad    dX = dY W^T    (A K-major, B K-major)
-//   wgrad    dW = X^T dY    (A MN-major, B MN-major, fp32 output, split-K with fp32 reductions)
+//   wgrad    dW = X^T dY    (A MN-major, B MN-major, fp32 output, split-K reduced in a fixed order)
 // replacing nn.Dense / nn.Conv(stride=kernel) call sites of the reference:
 //   dinov3_jax/layers/attention.py:63-65,94,101   dinov3_jax/layers/ffn_layers.py:36-47
 //   dinov3_jax/layers/patch_embed.py:38-51        dinov3_jax/layers/dino_head.py:20-43,65-85
 // The epilogue fuses bias, tanh-GELU, GELU', LayerScale (gamma) and the residual add
 // (dinov3_jax/layers/block.py:198-199, dinov3_jax/layers/layer_scale.py:17-21).
 //
-// Two kernels:
-//   gemm2sm_kernel — CTA pairs (cluster 2x1, tcgen05 cta_group::2): a 256x256 output tile per pair, each CTA stages
-//                    its 128 A rows and half (128) of the B columns, halving L2->SM operand traffic per FLOP
-//                    (a 1-CTA 128x256 tile needs 96 B/clk/SM of operands: above what L2 can feed 148 SMs).
-//   gemm1sm_kernel — single-CTA 128 x {64,128,256} tiles for small / ragged problems.
-// Issue discipline: TMA and tcgen05 instructions are issued by the ELECTED lane (elect.sync) of a converged warp; under a
-// `lane == 0` branch ptxas wraps every UTMALDG / UTCHMMA / UTMASTG in an ELECT ... BRA.U.ANY loop (~60-90 cycles each),
-// which is more than the 64 tensor cycles of one 256x256x16 pair MMA (tools/microbench/mma_lat.cu).
-// Roles: warp0 = TMA producer, warp1 = MMA issuer (one elected lane), warp2 = TMEM allocator, warps4-11 = epilogue
-// (TMEM -> registers -> global; two warps per TMEM lane quarter, each taking half of the tile's columns).
-// Two accumulator stages in TMEM let the epilogue of tile i overlap the main loop of tile i+1.
+// One kernel, 128 x {64,128} output tiles, 384 threads:
+//   warpgroup 0      TMA producer (one elected thread): A and B k-blocks of 64, tile after tile of this CTA's work
+//                    list, into the shared-memory ring of the consumer that owns the tile;
+//   warpgroups 1, 2  consumers in ping-pong: the CTA's tiles alternate between them, so one warpgroup's epilogue
+//                    (straight from its accumulator registers) runs under the other's main loop.  A tile is two
+//                    m64nBNk16 wgmma chains (rows 0-63 / 64-127) over SWIZZLE_128B operands, K-major or MN-major through
+//                    the descriptor transpose bits.
+// Each consumer has its own ring (half of the stages) and waits on every fill of it in order: with one shared ring the
+// consumer of tile j+1 would wait on fills two barrier phases ahead, which the phase parity cannot tell apart.
 #include <cstdlib>
 #include <cstring>
 #include "ptx.cuh"
@@ -29,339 +27,101 @@ namespace d3 {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int EPI_WARPS = 8;
-constexpr int GEMM_THREADS = 128 + 32 * EPI_WARPS;
+constexpr int GEMM_THREADS = 384;
 
 // ---------------------------------------------------------------------------------------------------------------
-// epilogue for one row x 32 consecutive columns held in registers
-__device__ __forceinline__ void epilogue_chunk(const GemmEpilogue& ep, size_t ro, int nc, int N, float (&v)[32],
-                                               bool full) {
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] *= ep.alpha;
+// epilogue for two adjacent columns (n, n+1) of one row; `vec`: both columns in range and every operand 16-byte
+// aligned with even leading dimensions (vector loads / stores of pairs)
+__device__ __forceinline__ void epilogue_pair(const GemmEpilogue& ep, size_t row, int n, int N, float v0, float v1,
+                                              bool vec) {
+  v0 *= ep.alpha;
+  v1 *= ep.alpha;
   if (ep.flags & EP_SCATTER) {  // fused reduce-scatter: add into the owning rank's shard slice (NVLink peer mapping)
-    const unsigned long long g0 = (unsigned long long)ep.sc_off + ro * ep.ld_out + nc;
-    const unsigned shard = (unsigned)ep.sc_shard;
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      if (!full && nc + j + 3 >= N) {
-        for (int t = 0; t < 4; ++t)
-          if (nc + j + t < N) {
-            const unsigned long long g = g0 + j + t;
-            const unsigned r = (unsigned)(g / shard);
-            atomicAdd(ep.sc_peer[r] + (g - (unsigned long long)r * shard), v[j + t]);
-          }
-        continue;
-      }
-      const unsigned long long g = g0 + j;                      // a float4 never straddles two owners (shard % 4 == 0)
+    const unsigned long long g = (unsigned long long)ep.sc_off + row * ep.ld_out + n;
+    const unsigned long long shard = (unsigned long long)ep.sc_shard;
+    if (n + 1 < N) {                                         // a pair never straddles two owners (shard % 4 == 0)
       const unsigned r = (unsigned)(g / shard);
-      float* dst = ep.sc_peer[r] + (g - (unsigned long long)r * shard);
+      float* dst = ep.sc_peer[r] + (g - r * shard);
       if (ep.sc_sys) {
-        atomicAdd_system(dst, v[j]); atomicAdd_system(dst + 1, v[j + 1]);
-        atomicAdd_system(dst + 2, v[j + 2]); atomicAdd_system(dst + 3, v[j + 3]);
+        atomicAdd_system(dst, v0); atomicAdd_system(dst + 1, v1);
       } else {
-        atomicAdd(reinterpret_cast<float4*>(dst), make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]));
+        atomicAdd(reinterpret_cast<float2*>(dst), make_float2(v0, v1));
       }
-    }
-    return;
-  }
-  if (ep.flags & EP_ATOMIC) {   // split-K partial: fp32 reduction into a zero-initialised output
-    float* o = reinterpret_cast<float*>(ep.out) + ro * ep.ld_out + nc;
-    if (full) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) atomicAdd(reinterpret_cast<float4*>(o + j), make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]));
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (nc + j < N) atomicAdd(o + j, v[j]);
+    } else if (n < N) {
+      const unsigned r = (unsigned)(g / shard);
+      atomicAdd(ep.sc_peer[r] + (g - r * shard), v0);
     }
     return;
   }
   const bool fast_act = (ep.flags & EP_FAST_ACT) != 0;
-  if (ep.flags & EP_DEBUG_NOSTORE) {   // diagnostic: keep the math, drop the global traffic
-    float acc = 0.f;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) acc += (ep.flags & EP_GELU) ? gelu_tanh_fast(v[j]) : v[j];
-    if (acc == 1.2345e38f) reinterpret_cast<float*>(ep.out)[0] = acc;
-    return;
-  }
-  if (full) {
+  if (vec) {
     if (ep.flags & EP_BIAS) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        float4 b = *reinterpret_cast<const float4*>(ep.bias + nc + j);
-        v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
-      }
+      const float2 b = *reinterpret_cast<const float2*>(ep.bias + n);
+      v0 += b.x; v1 += b.y;
     }
-    if (ep.flags & EP_STORE_PRE) {
-      uint4* dst = reinterpret_cast<uint4*>(ep.aux_out + ro * ep.ld_aux + nc);
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        dst[j] = make_uint4(pack_bf16(v[8 * j], v[8 * j + 1]), pack_bf16(v[8 * j + 2], v[8 * j + 3]),
-                            pack_bf16(v[8 * j + 4], v[8 * j + 5]), pack_bf16(v[8 * j + 6], v[8 * j + 7]));
-    }
+    if (ep.flags & EP_STORE_PRE) *reinterpret_cast<uint32_t*>(ep.aux_out + row * ep.ld_aux + n) = pack_bf16(v0, v1);
     if (ep.flags & EP_GELU) {
-      if (fast_act) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = gelu_tanh_fast(v[j]);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = gelu_tanh(v[j]);
-      }
+      v0 = fast_act ? gelu_tanh_fast(v0) : gelu_tanh(v0);
+      v1 = fast_act ? gelu_tanh_fast(v1) : gelu_tanh(v1);
     }
     if (ep.flags & EP_MUL_DGELU) {
-      const uint4* src = reinterpret_cast<const uint4*>(ep.aux_in + ro * ep.ld_aux + nc);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        uint4 u = src[j];
-        float2 a = unpack_bf16(u.x), b = unpack_bf16(u.y), cc = unpack_bf16(u.z), d = unpack_bf16(u.w);
-        if (fast_act) {
-          v[8 * j] *= gelu_tanh_grad_fast(a.x); v[8 * j + 1] *= gelu_tanh_grad_fast(a.y);
-          v[8 * j + 2] *= gelu_tanh_grad_fast(b.x); v[8 * j + 3] *= gelu_tanh_grad_fast(b.y);
-          v[8 * j + 4] *= gelu_tanh_grad_fast(cc.x); v[8 * j + 5] *= gelu_tanh_grad_fast(cc.y);
-          v[8 * j + 6] *= gelu_tanh_grad_fast(d.x); v[8 * j + 7] *= gelu_tanh_grad_fast(d.y);
-        } else {
-          v[8 * j] *= gelu_tanh_grad(a.x); v[8 * j + 1] *= gelu_tanh_grad(a.y);
-          v[8 * j + 2] *= gelu_tanh_grad(b.x); v[8 * j + 3] *= gelu_tanh_grad(b.y);
-          v[8 * j + 4] *= gelu_tanh_grad(cc.x); v[8 * j + 5] *= gelu_tanh_grad(cc.y);
-          v[8 * j + 6] *= gelu_tanh_grad(d.x); v[8 * j + 7] *= gelu_tanh_grad(d.y);
-        }
-      }
+      const float2 u = unpack_bf16(*reinterpret_cast<const uint32_t*>(ep.aux_in + row * ep.ld_aux + n));
+      v0 *= fast_act ? gelu_tanh_grad_fast(u.x) : gelu_tanh_grad(u.x);
+      v1 *= fast_act ? gelu_tanh_grad_fast(u.y) : gelu_tanh_grad(u.y);
     }
     if (ep.flags & EP_GAMMA) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        float4 g = *reinterpret_cast<const float4*>(ep.gamma + nc + j);
-        v[j] *= g.x; v[j + 1] *= g.y; v[j + 2] *= g.z; v[j + 3] *= g.w;
-      }
+      const float2 g = *reinterpret_cast<const float2*>(ep.gamma + n);
+      v0 *= g.x; v1 *= g.y;
     }
     if (ep.flags & EP_RESID) {
-      const float4* rs = reinterpret_cast<const float4*>(ep.resid + ro * ep.ld_resid + nc);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4 x = rs[j];
-        v[4 * j] += x.x; v[4 * j + 1] += x.y; v[4 * j + 2] += x.z; v[4 * j + 3] += x.w;
-      }
+      const float2 x = *reinterpret_cast<const float2*>(ep.resid + row * ep.ld_resid + n);
+      v0 += x.x; v1 += x.y;
     }
     if (ep.flags & EP_OUT_F32) {
-      float4* dst = reinterpret_cast<float4*>(reinterpret_cast<float*>(ep.out) + ro * ep.ld_out + nc);
+      float2* dst = reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.out) + row * ep.ld_out + n);
       if (ep.flags & EP_ACCUM) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float4 x = dst[j];
-          v[4 * j] += x.x; v[4 * j + 1] += x.y; v[4 * j + 2] += x.z; v[4 * j + 3] += x.w;
-        }
+        const float2 x = *dst;
+        v0 += x.x; v1 += x.y;
       }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+      *dst = make_float2(v0, v1);
     } else {
-      uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + ro * ep.ld_out + nc);
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        dst[j] = make_uint4(pack_bf16(v[8 * j], v[8 * j + 1]), pack_bf16(v[8 * j + 2], v[8 * j + 3]),
-                            pack_bf16(v[8 * j + 4], v[8 * j + 5]), pack_bf16(v[8 * j + 6], v[8 * j + 7]));
+      *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + row * ep.ld_out + n) = pack_bf16(v0, v1);
     }
-  } else {
-    // ragged / unaligned edge: scalar path with bounds checks
-#pragma unroll 1
-    for (int j = 0; j < 32; ++j) {
-      const int n = nc + j;
-      if (n >= N) break;
-      float x = v[j];
-      if (ep.flags & EP_BIAS) x += ep.bias[n];
-      if (ep.flags & EP_STORE_PRE) ep.aux_out[ro * ep.ld_aux + n] = __float2bfloat16(x);
-      if (ep.flags & EP_GELU) x = fast_act ? gelu_tanh_fast(x) : gelu_tanh(x);
-      if (ep.flags & EP_MUL_DGELU) {
-        const float u = __bfloat162float(ep.aux_in[ro * ep.ld_aux + n]);
-        x *= fast_act ? gelu_tanh_grad_fast(u) : gelu_tanh_grad(u);
-      }
-      if (ep.flags & EP_GAMMA) x *= ep.gamma[n];
-      if (ep.flags & EP_RESID) x += ep.resid[ro * ep.ld_resid + n];
-      if (ep.flags & EP_OUT_F32) {
-        float* o = reinterpret_cast<float*>(ep.out) + ro * ep.ld_out + n;
-        if (ep.flags & EP_ACCUM) x += *o;
-        *o = x;
-      } else {
-        reinterpret_cast<__nv_bfloat16*>(ep.out)[ro * ep.ld_out + n] = __float2bfloat16(x);
-      }
-    }
+    return;
   }
-}
-
-// drain one accumulator stage: this warp owns TMEM lanes [32q, 32q+32) and the column half `half` of the tile
-template <int BN>
-__device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, uint32_t t_addr, int row, int n0, int M, int N,
-                                              int half) {
-  const bool row_ok = row < M;
-  const bool fast = (ep.flags & EP_SLOW) == 0;
-  constexpr int CHUNKS = BN / 32 / 2 > 0 ? BN / 32 / 2 : 1;
-  const int c_begin = (BN >= 64) ? half * CHUNKS : 0;
-  if (BN < 64 && half == 1) return;
+  // ragged / unaligned edge: scalar path with bounds checks
 #pragma unroll 1
-  for (int c = c_begin; c < c_begin + CHUNKS; ++c) {
-    const int nc = n0 + c * 32;
-    if (nc >= N) break;  // warp-uniform
-    uint32_t r[32];
-    tmem_ld32(t_addr + c * 32, r);
-    tmem_ld_wait();
-    if (!row_ok) continue;
-    float v[32];
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-    epilogue_chunk(ep, (size_t)row, nc, N, v, fast && (nc + 32 <= N));
-  }
-}
-
-
-// ---------------------------------------------------------------------------------------------------------------
-// TMA epilogue (CTA-pair kernel): every [32 rows x 32 cols] unit of a warp moves through swizzled shared-memory
-// staging: residual / GELU' operands arrive by TMA load, results leave by TMA store, so global traffic is in full
-// 128-byte lines regardless of the row-per-thread TMEM layout.  sOut: 4 KB (fp32: 128-B rows, SWIZZLE_128B; bf16:
-// 64-B rows, SWIZZLE_64B), sAux: 2 KB bf16 (SWIZZLE_64B).
-__device__ __forceinline__ uint32_t stg128(int row, int chunk) { return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4)); }
-__device__ __forceinline__ uint32_t stg64(int row, int chunk) { return (uint32_t)(row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4)); }
-
-// Per-warp epilogue pipeline state: two staging buffers (out 4 KB + aux 2 KB each); unit u uses buffer u & 1, the
-// residual / GELU' tiles of unit u+1 are prefetched by TMA while unit u is processed, and a buffer is rewritten only
-// after the bulk-store group that read it has drained (cp.async.bulk.wait_group.read 1).
-struct EpiPipe {
-  uint8_t* buf;          // 2 x (4096 + 2048) bytes, 1024-aligned
-  uint64_t* ld_bar;      // [2] one per buffer
-  uint32_t phase[2];
-  uint32_t unit;         // running unit counter of this warp
-};
-
-template <int BN>
-__device__ __forceinline__ void epilogue_tile_tma(const GemmEpilogue& ep, const CUtensorMap* tmOut,
-                                                  const CUtensorMap* tmAux, const CUtensorMap* tmRes, uint32_t t_addr,
-                                                  int row0, int n0, int M, int N, int half, EpiPipe& pp) {
-  const int lane = threadIdx.x & 31;
-  const bool out_f32 = (ep.flags & EP_OUT_F32) != 0;
-  const bool has_res = (ep.flags & EP_RESID) != 0;
-  const bool has_auxin = (ep.flags & EP_MUL_DGELU) != 0;
-  const bool store_pre = (ep.flags & EP_STORE_PRE) != 0;
-  const bool fast_act = (ep.flags & EP_FAST_ACT) != 0;
-  const bool has_loads = has_res || has_auxin;
-  const uint32_t ld_bytes = (has_res ? 4096u : 0u) + (has_auxin ? 2048u : 0u);
-  constexpr int CHUNKS = BN / 64;
-  if (row0 >= M) return;   // warp-uniform: this warp's 32 rows are all padding
-  const int c_beg = half * CHUNKS;
-  int c_end = (half + 1) * CHUNKS;
-  while (c_end > c_beg && n0 + (c_end - 1) * 32 >= N) --c_end;   // warp-uniform clipping at the N edge
-  if (c_end <= c_beg) return;
-
-  auto issue_loads = [&](int c, uint32_t u) {   // lane 0 only
-    const uint32_t b = u & 1;
-    uint8_t* sOut = pp.buf + b * 6144;
-    mbar_expect_tx(&pp.ld_bar[b], ld_bytes);
-    if (has_res) tma_load_2d_cta(tmRes, &pp.ld_bar[b], sOut, n0 + c * 32, row0);
-    if (has_auxin) tma_load_2d_cta(tmAux, &pp.ld_bar[b], sOut + 4096, n0 + c * 32, row0);
-  };
-  // prologue: the first unit's buffer was last used two units ago -> its store group has drained after wait<1>
-  if (elect_one()) {
-    tma_store_wait_read1();
-    if (has_loads) issue_loads(c_beg, pp.unit);
-  }
-#pragma unroll 1
-  for (int c = c_beg; c < c_end; ++c) {
-    const uint32_t u = pp.unit;
-    const uint32_t b = u & 1;
-    uint8_t* sOut = pp.buf + b * 6144;
-    uint8_t* sAux = sOut + 4096;
-    const int nc = n0 + c * 32;
-    if (c + 1 < c_end && elect_one()) {
-      // buffer (u+1)&1 was used by unit u-1: allow only the most recent store group (none issued since) to be pending
-      tma_store_wait_read0();
-      if (has_loads) issue_loads(c + 1, u + 1);
+  for (int j = 0; j < 2; ++j) {
+    const int c = n + j;
+    if (c >= N) break;
+    float x = j ? v1 : v0;
+    if (ep.flags & EP_BIAS) x += ep.bias[c];
+    if (ep.flags & EP_STORE_PRE) ep.aux_out[row * ep.ld_aux + c] = __float2bfloat16(x);
+    if (ep.flags & EP_GELU) x = fast_act ? gelu_tanh_fast(x) : gelu_tanh(x);
+    if (ep.flags & EP_MUL_DGELU) {
+      const float u = __bfloat162float(ep.aux_in[row * ep.ld_aux + c]);
+      x *= fast_act ? gelu_tanh_grad_fast(u) : gelu_tanh_grad(u);
     }
-    __syncwarp();
-    uint32_t r[32];
-    tmem_ld32(t_addr + c * 32, r);
-    tmem_ld_wait();
-    float v[32];
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * ep.alpha;
-    if (ep.flags & EP_BIAS) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        float4 bb = *reinterpret_cast<const float4*>(ep.bias + nc + j);
-        v[j] += bb.x; v[j + 1] += bb.y; v[j + 2] += bb.z; v[j + 3] += bb.w;
-      }
-    }
-    if (store_pre) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        *reinterpret_cast<uint4*>(sAux + stg64(lane, j)) =
-            make_uint4(pack_bf16(v[8 * j], v[8 * j + 1]), pack_bf16(v[8 * j + 2], v[8 * j + 3]),
-                       pack_bf16(v[8 * j + 4], v[8 * j + 5]), pack_bf16(v[8 * j + 6], v[8 * j + 7]));
-    }
-    if (ep.flags & EP_GELU) {
-      if (fast_act) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = gelu_tanh_fast(v[j]);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = gelu_tanh(v[j]);
-      }
-    }
-    if (has_loads) {
-      mbar_wait(&pp.ld_bar[b], pp.phase[b]);
-      pp.phase[b] ^= 1;
-    }
-    if (has_auxin) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint4 uu = *reinterpret_cast<const uint4*>(sAux + stg64(lane, j));
-        const float2 a = unpack_bf16(uu.x), bq = unpack_bf16(uu.y), cc = unpack_bf16(uu.z), d = unpack_bf16(uu.w);
-        v[8 * j] *= gelu_tanh_grad_fast(a.x); v[8 * j + 1] *= gelu_tanh_grad_fast(a.y);
-        v[8 * j + 2] *= gelu_tanh_grad_fast(bq.x); v[8 * j + 3] *= gelu_tanh_grad_fast(bq.y);
-        v[8 * j + 4] *= gelu_tanh_grad_fast(cc.x); v[8 * j + 5] *= gelu_tanh_grad_fast(cc.y);
-        v[8 * j + 6] *= gelu_tanh_grad_fast(d.x); v[8 * j + 7] *= gelu_tanh_grad_fast(d.y);
-      }
-    }
-    if (ep.flags & EP_GAMMA) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        float4 g = *reinterpret_cast<const float4*>(ep.gamma + nc + j);
-        v[j] *= g.x; v[j + 1] *= g.y; v[j + 2] *= g.z; v[j + 3] *= g.w;
-      }
-    }
-    if (has_res) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 x = *reinterpret_cast<const float4*>(sOut + stg128(lane, j));
-        v[4 * j] += x.x; v[4 * j + 1] += x.y; v[4 * j + 2] += x.z; v[4 * j + 3] += x.w;
-      }
-    }
-    if (out_f32) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<float4*>(sOut + stg128(lane, j)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+    if (ep.flags & EP_GAMMA) x *= ep.gamma[c];
+    if (ep.flags & EP_RESID) x += ep.resid[row * ep.ld_resid + c];
+    if (ep.flags & EP_OUT_F32) {
+      float* o = reinterpret_cast<float*>(ep.out) + row * ep.ld_out + c;
+      if (ep.flags & EP_ACCUM) x += *o;
+      *o = x;
     } else {
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        *reinterpret_cast<uint4*>(sOut + stg64(lane, j)) =
-            make_uint4(pack_bf16(v[8 * j], v[8 * j + 1]), pack_bf16(v[8 * j + 2], v[8 * j + 3]),
-                       pack_bf16(v[8 * j + 4], v[8 * j + 5]), pack_bf16(v[8 * j + 6], v[8 * j + 7]));
+      reinterpret_cast<__nv_bfloat16*>(ep.out)[row * ep.ld_out + c] = __float2bfloat16(x);
     }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (elect_one()) {
-      tma_store_2d(tmOut, sOut, nc, row0);
-      if (store_pre) tma_store_2d(tmAux, sAux, nc, row0);
-      tma_store_commit();
-    }
-    pp.unit = u + 1;
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 template <int BN>
-struct Cfg1 {
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
+struct Cfg {
+  static constexpr int STAGES = BN == 128 ? 6 : 8;   // two rings of STAGES / 2
+  static constexpr int RS = STAGES / 2;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int TMEM_COLS = 2 * BN;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
@@ -369,350 +129,147 @@ struct Cfg1 {
 struct WorkRange { int m0, n0, kb0, kb1; };
 // Tiles are rasterised N-fastest: the CTAs resident at any moment cover a few M row-panels times all N tiles, so the
 // large activation operand streams from HBM once while the (small) weight operand stays L2-resident.
-__device__ __forceinline__ WorkRange work_item(int w, int num_m, int num_n, int num_k, int splits, int tile_m,
-                                               int tile_n, int m_fastest) {
+__device__ __forceinline__ WorkRange work_item(int w, int num_n, int num_k, int splits, int tile_n) {
   const int tile = w / splits, sp = w % splits;
   const int per = (num_k + splits - 1) / splits;
   WorkRange r;
-  if (m_fastest) {
-    r.m0 = (tile % num_m) * tile_m;
-    r.n0 = (tile / num_m) * tile_n;
-  } else {
-    r.n0 = (tile % num_n) * tile_n;
-    r.m0 = (tile / num_n) * tile_m;
-  }
+  r.n0 = (tile % num_n) * tile_n;
+  r.m0 = (tile / num_n) * BM;
   r.kb0 = sp * per;
   r.kb1 = min(num_k, r.kb0 + per);
   return r;
 }
 
 template <int BN, int A_MN, int B_MN>
+__device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint32_t sa, uint32_t sb, bool first) {
+  // A rows 64-127 start 8 KB into the stage in both layouts (64 rows x 128 B, or the second 64-row box)
+  const uint64_t bd = B_MN ? gmma_desc_sw128(sb, 8192, 1024) : gmma_desc_sw128(sb, 16, 1024);
+  constexpr uint64_t a_adv = A_MN ? (2048 >> 4) : (32 >> 4);
+  constexpr uint64_t b_adv = B_MN ? (2048 >> 4) : (32 >> 4);
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k) {
+    const uint32_t sc = (first && k == 0) ? 0u : 1u;
+#pragma unroll
+    for (int mh = 0; mh < 2; ++mh) {
+      const uint64_t ad = A_MN ? gmma_desc_sw128(sa + mh * 8192, 8192, 1024) : gmma_desc_sw128(sa + mh * 8192, 16, 1024);
+      if constexpr (BN == 128) wgmma_m64n128k16_ss<A_MN, B_MN>(acc[mh], ad + k * a_adv, bd + k * b_adv, sc);
+      else wgmma_m64n64k16_ss<A_MN, B_MN>(acc[mh], ad + k * a_adv, bd + k * b_adv, sc);
+    }
+  }
+}
+
+template <int BN, int A_MN, int B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm1sm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const GemmEpilogue ep, int M, int N, int K, int splits) {
-  using Cfg = Cfg1<BN>;
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmEpilogue ep,
+            int M, int N, int K, int splits) {
+  using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + Cfg::STAGES;
-  uint64_t* tfull_bar = bars + 2 * Cfg::STAGES;
-  uint64_t* tempty_bar = bars + 2 * Cfg::STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);   // [ring * RS + stage]
+  uint64_t* empty_bar = full_bar + C::STAGES;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  const int wg = threadIdx.x >> 7;
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], EPI_WARPS); }
+    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_m = (M + BM - 1) / BM;
   const int num_n = (N + BN - 1) / BN;
   const int num_k = (K + BK - 1) / BK;
   const int num_work = num_m * num_n * splits;
 
-  if (warp == 0) {
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-        const WorkRange wr = work_item(w, num_m, num_n, num_k, splits, BM, BN, ep.flags & EP_M_FASTEST);
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 32 && elect_one()) {
+      int stage[2] = {0, 0};
+      uint32_t phase[2] = {0, 0};
+      int j = 0;
+      for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++j) {
+        const WorkRange wr = work_item(w, num_n, num_k, splits, BN);
+        const int r = j & 1;                   // the ring of the consumer that owns tile j
         for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + Cfg::A_BYTES;
-          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+          const int slot = r * C::RS + stage[r];
+          mbar_wait(&empty_bar[slot], phase[r] ^ 1);
+          uint8_t* sa = smem + slot * C::STAGE_BYTES;
+          uint8_t* sb = sa + C::A_BYTES;
+          mbar_expect_tx(&full_bar[slot], C::STAGE_BYTES);
           if (A_MN) {
 #pragma unroll
-            for (int j = 0; j < BM / 64; ++j) tma_load_2d(&tmA, &full_bar[stage], sa + j * 8192, wr.m0 + j * 64, kb * BK);
+            for (int i = 0; i < BM / 64; ++i) tma_load_2d(&tmA, &full_bar[slot], sa + i * 8192, wr.m0 + i * 64, kb * BK);
           } else {
-            tma_load_2d(&tmA, &full_bar[stage], sa, kb * BK, wr.m0);
+            tma_load_2d(&tmA, &full_bar[slot], sa, kb * BK, wr.m0);
           }
           if (B_MN) {
 #pragma unroll
-            for (int j = 0; j < BN / 64; ++j) tma_load_2d(&tmB, &full_bar[stage], sb + j * 8192, wr.n0 + j * 64, kb * BK);
+            for (int i = 0; i < BN / 64; ++i) tma_load_2d(&tmB, &full_bar[slot], sb + i * 8192, wr.n0 + i * 64, kb * BK);
           } else {
-            tma_load_2d(&tmB, &full_bar[stage], sb, kb * BK, wr.n0);
+            tma_load_2d(&tmB, &full_bar[slot], sb, kb * BK, wr.n0);
           }
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+          if (++stage[r] == C::RS) { stage[r] = 0; phase[r] ^= 1; }
         }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN, A_MN, B_MN);
-      constexpr uint32_t a_adv = A_MN ? (2 * 1024 >> 4) : (32 >> 4);
-      constexpr uint32_t b_adv = B_MN ? (2 * 1024 >> 4) : (32 >> 4);
-      int stage = 0;
-      uint32_t phase = 0;
-      int local = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++local) {
-        const WorkRange wr = work_item(w, num_m, num_n, num_k, splits, BM, BN, ep.flags & EP_M_FASTEST);
-        const int acc = local & 1;
-        const uint32_t acc_phase = (local >> 1) & 1;
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sb = sa + Cfg::A_BYTES;
-          const uint64_t adesc = A_MN ? umma_desc_sw128(sa, 8192, 1024) : umma_desc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = B_MN ? umma_desc_sw128(sb, 8192, 1024) : umma_desc_sw128(sb, 16, 1024);
+  } else {
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;                     // consumer warpgroup: tiles j of this CTA with j % 2 == cw
+    const int t = threadIdx.x & 127;
+    const int r_in = 16 * (t >> 5) + ((t & 31) >> 2);
+    const int c_in = 2 * (t & 3);
+    const bool fast = (ep.flags & EP_SLOW) == 0;
+    int stage = 0;                             // position in this consumer's ring
+    uint32_t phase = 0;
+    for (int w = blockIdx.x + cw * gridDim.x; w < num_work; w += 2 * gridDim.x) {
+      const WorkRange wr = work_item(w, num_n, num_k, splits, BN);
+      const int nkb = wr.kb1 - wr.kb0;
+      float acc[2][BN / 2];
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_bf16(d_tmem, adesc + (uint64_t)(k * a_adv), bdesc + (uint64_t)(k * b_adv), idesc,
-                      (kb > wr.kb0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull_bar[acc]);
-      }
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int q = warp & 3;            // TMEM lane quarter == warp % 4
-    const int half = (warp - 4) >> 2;  // column half of the tile
-    int local = 0;
-    for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++local) {
-      const WorkRange wr = work_item(w, num_m, num_n, num_k, splits, BM, BN, ep.flags & EP_M_FASTEST);
-      const int acc = local & 1;
-      const uint32_t acc_phase = (local >> 1) & 1;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      if (wr.kb1 > wr.kb0)
-        epilogue_tile<BN>(ep, tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN, wr.m0 + q * 32 + lane, wr.n0, M, N, half);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_free<Cfg::TMEM_COLS>(tmem_base);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// CTA-pair kernel: 256 x 256 tile per cluster; per CTA and stage: A 128x64 (16 KB) + B 128x64 (16 KB)
-// TMA_EPI: TMA-store epilogue (4 operand stages + 96 KB of double-buffered staging); otherwise direct / atomic
-// epilogue (weight gradients) with 6 operand stages.
-template <int TMA_EPI>
-struct Cfg2 {
-  static constexpr int BN = 256;
-  static constexpr int STAGES = TMA_EPI ? 4 : 6;
-  static constexpr int A_BYTES = 128 * BK * 2;
-  static constexpr int B_BYTES = 128 * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int TMEM_COLS = 512;
-  static constexpr int STG_WARP = 2 * (4096 + 2048);           // per epilogue warp: two (out tile + aux tile) buffers
-  static constexpr int STG_BYTES = TMA_EPI ? EPI_WARPS * STG_WARP : 0;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + 1024 + 256 + 256;   // + CLC ring
-};
-
-// Dynamic tile scheduling (SCHED = 1): the grid has one cluster per work item; a resident cluster finishes its own item
-// and then takes over not-yet-launched clusters with clusterlaunchcontrol.try_cancel, so work follows whichever SMs are
-// actually free (NCCL or the other stream's kernels may hold some) instead of a static stride that leaves a late
-// cluster with a full share.  One scheduler warp in the leader CTA issues the queries; the 16-byte responses are
-// multicast into a small ring in both CTAs and consumed by every role (TMA producers, MMA issuer, epilogue warps).
-__device__ int g_gemm_stagger_ns = 0;   // optional de-phasing of the clusters' tile loops (D3_GEMM_STAGGER_NS)
-constexpr int CLC_STAGES = 4;
-struct ClcRing {
-  uint8_t* resp;      // [CLC_STAGES][16]
-  uint64_t* full;     // [CLC_STAGES] local: 1 arrival (expect_tx) + 16 transaction bytes
-  uint64_t* empty;    // [CLC_STAGES] in the leader CTA: one arrival per consumer role of both CTAs
-  uint32_t it;
-};
-constexpr int CLC_CONSUMERS = 2 /*TMA producers*/ + 1 /*MMA issuer*/ + 2 * EPI_WARPS;
-// next work index for a consumer role.  WARP = true: called by all 32 lanes of a warp (lane 0 releases the slot after
-// every lane has read it); WARP = false: called by a single elected thread.
-template <bool WARP>
-__device__ __forceinline__ int clc_next(ClcRing& r, bool arrive) {
-  const uint32_t slot = r.it % CLC_STAGES, ph = (r.it / CLC_STAGES) & 1;
-  mbar_wait(&r.full[slot], ph);
-  uint32_t x;
-  const bool valid = clc_query(r.resp + slot * 16, x);
-  fence_proxy_async_smem();
-  if (WARP) __syncwarp();
-  if (arrive) mbar_arrive_cluster(&r.empty[slot], 0);
-  ++r.it;
-  return valid ? (int)(x >> 1) : -1;
-}
-
-template <int A_MN, int B_MN, int TMA_EPI, int SCHED>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm2sm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmAux,
-               const __grid_constant__ CUtensorMap tmRes, const GemmEpilogue ep, int M, int N, int K, int splits) {
-  using Cfg = Cfg2<TMA_EPI>;
-  static_assert(2 * Cfg::STAGES + 4 + 2 * EPI_WARPS + 1 <= 40, "barrier block");
-  constexpr int BN = Cfg::BN;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STG_BYTES);
-  uint64_t* full_bar = bars;                          // used in the leader CTA: 2 producer arrivals + 4 TMA transactions
-  uint64_t* empty_bar = bars + Cfg::STAGES;           // per CTA, signalled by the leader's multicast commit
-  uint64_t* tfull_bar = bars + 2 * Cfg::STAGES;       // per CTA, multicast commit
-  uint64_t* tempty_bar = bars + 2 * Cfg::STAGES + 2;  // leader: 2 x EPI_WARPS arrivals
-  uint64_t* ld_bar = bars + 2 * Cfg::STAGES + 4;      // [2 * EPI_WARPS] epilogue TMA loads (residual / GELU' operand)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4 + 2 * EPI_WARPS);
-  uint64_t* clc_full = bars + 40;
-  uint64_t* clc_empty = clc_full + CLC_STAGES;
-  uint8_t* clc_resp = reinterpret_cast<uint8_t*>(clc_empty + CLC_STAGES);      // 16-byte aligned (bars is 1024-aligned)
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 2); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], 2 * EPI_WARPS); }
-    for (int s = 0; s < 2 * EPI_WARPS; ++s) mbar_init(&ld_bar[s], 1);
-    if (SCHED) for (int s = 0; s < CLC_STAGES; ++s) { mbar_init(&clc_full[s], 1); mbar_init(&clc_empty[s], CLC_CONSUMERS); }
-    if (TMA_EPI) { tma_prefetch_desc(&tmOut); tma_prefetch_desc(&tmAux); tma_prefetch_desc(&tmRes); }
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc_2sm<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int num_m = (M + 255) / 256;
-  const int num_n = (N + BN - 1) / BN;
-  const int num_k = (K + BK - 1) / BK;
-  const int num_work = num_m * num_n * splits;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      ClcRing ring{clc_resp, clc_full, clc_empty, 0};
-      if (g_gemm_stagger_ns > 0 && num_work > num_clusters) __nanosleep((unsigned)(cluster_id * g_gemm_stagger_ns));
-      for (int w = cluster_id; w >= 0 && w < num_work; w = SCHED ? clc_next<false>(ring, true) : w + num_clusters) {
-        const WorkRange wr = work_item(w, num_m, num_n, num_k, splits, 256, BN, ep.flags & EP_M_FASTEST);
-        const int m0 = wr.m0 + rank * 128;     // this CTA's 128 A rows
-        const int n0 = wr.n0 + rank * 128;     // this CTA's half of the B tile
-        for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + Cfg::A_BYTES;
-          if (leader) mbar_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-          else mbar_arrive_cluster(&full_bar[stage], 0);
-          if (A_MN) {
-            tma_load_2d_2sm(&tmA, &full_bar[stage], sa, m0, kb * BK);
-            tma_load_2d_2sm(&tmA, &full_bar[stage], sa + 8192, m0 + 64, kb * BK);
-          } else {
-            tma_load_2d_2sm(&tmA, &full_bar[stage], sa, kb * BK, m0);
-          }
-          if (B_MN) {
-            tma_load_2d_2sm(&tmB, &full_bar[stage], sb, n0, kb * BK);
-            tma_load_2d_2sm(&tmB, &full_bar[stage], sb + 8192, n0 + 64, kb * BK);
-          } else {
-            tma_load_2d_2sm(&tmB, &full_bar[stage], sb, kb * BK, n0);
-          }
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (leader && elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(256, BN, A_MN, B_MN);
-      constexpr uint32_t a_adv = A_MN ? (2 * 1024 >> 4) : (32 >> 4);
-      constexpr uint32_t b_adv = B_MN ? (2 * 1024 >> 4) : (32 >> 4);
-      int stage = 0;
-      uint32_t phase = 0;
-      int local = 0;
-      ClcRing ring{clc_resp, clc_full, clc_empty, 0};
-      for (int w = cluster_id; w >= 0 && w < num_work; w = SCHED ? clc_next<false>(ring, true) : w + num_clusters, ++local) {
-        const WorkRange wr = work_item(w, num_m, num_n, num_k, splits, 256, BN, ep.flags & EP_M_FASTEST);
-        const int acc = local & 1;
-        const uint32_t acc_phase = (local >> 1) & 1;
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sb = sa + Cfg::A_BYTES;
-          const uint64_t adesc = A_MN ? umma_desc_sw128(sa, 8192, 1024) : umma_desc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = B_MN ? umma_desc_sw128(sb, 8192, 1024) : umma_desc_sw128(sb, 16, 1024);
+      for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_bf16_2sm(d_tmem, adesc + (uint64_t)(k * a_adv), bdesc + (uint64_t)(k * b_adv), idesc,
-                          (kb > wr.kb0 || k > 0) ? 1u : 0u);
-          umma_commit_2sm(&empty_bar[stage]);   // frees the slot in both CTAs
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+        for (int i = 0; i < BN / 2; ++i) acc[mh][i] = 0.f;
+      int prev = -1;
+      for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
+        const int slot = cw * C::RS + stage;
+        mbar_wait(&full_bar[slot], phase);
+        const uint32_t sa = smem_u32(smem + slot * C::STAGE_BYTES);
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        wgmma_fence();
+        mma_kblock<BN, A_MN, B_MN>(acc, sa, sa + C::A_BYTES, kb == wr.kb0);
+        wgmma_commit();
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        if (prev >= 0) {                       // the k-block before this one has been consumed: release its stage
+          wgmma_wait<1>();
+          if (t == 0) mbar_arrive(&empty_bar[prev]);
         }
-        umma_commit_2sm(&tfull_bar[acc]);       // accumulator complete in both CTAs
+        prev = slot;
+        if (++stage == C::RS) { stage = 0; phase ^= 1; }
       }
+      wgmma_wait<0>();
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+      if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
+      if (nkb <= 0) continue;                  // empty split-K slice: nothing to add
+#pragma unroll
+      for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = wr.m0 + mh * 64 + r_in + 8 * h;
+          if (row >= M) continue;
+          const size_t orow = (ep.flags & EP_SLABS) ? (size_t)(w % splits) * M + row : (size_t)row;
+#pragma unroll
+          for (int i = 0; i < BN / 8; ++i) {
+            const int n = wr.n0 + 8 * i + c_in;
+            if (n >= N) break;
+            epilogue_pair(ep, orow, n, N, acc[mh][4 * i + 2 * h], acc[mh][4 * i + 2 * h + 1], fast && n + 1 < N);
+          }
+        }
     }
-    __syncwarp();
-  } else if (SCHED && warp == 3) {
-    if (leader) {
-      for (uint32_t it = 0;; ++it) {
-        const uint32_t slot = it % CLC_STAGES, ph = (it / CLC_STAGES) & 1;
-        if (it >= CLC_STAGES) mbar_wait(&clc_empty[slot], ph ^ 1);          // every consumer has read the old response
-        if (lane < 2) mbar_arrive_expect_tx_cluster(&clc_full[slot], lane, 16);
-        __syncwarp();
-        if (lane == 0) clc_try_cancel_multicast(clc_resp + slot * 16, &clc_full[slot]);
-        mbar_wait(&clc_full[slot], ph);
-        uint32_t x;
-        if (!clc_query(clc_resp + slot * 16, x)) break;                     // nothing left: no further queries allowed
-      }
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    const int half = (warp - 4) >> 2;
-    EpiPipe pp;
-    pp.buf = staging + (warp - 4) * Cfg::STG_WARP;
-    pp.ld_bar = &ld_bar[2 * (warp - 4)];
-    pp.phase[0] = pp.phase[1] = 0;
-    pp.unit = 0;
-    constexpr bool tma_epi = TMA_EPI != 0;
-    int local = 0;
-    ClcRing ring{clc_resp, clc_full, clc_empty, 0};
-    for (int w = cluster_id; w >= 0 && w < num_work; w = SCHED ? clc_next<true>(ring, lane == 0) : w + num_clusters, ++local) {
-      const WorkRange wr = work_item(w, num_m, num_n, num_k, splits, 256, BN, ep.flags & EP_M_FASTEST);
-      const int acc = local & 1;
-      const uint32_t acc_phase = (local >> 1) & 1;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      if (wr.kb1 > wr.kb0) {
-        const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN;
-        if (tma_epi)
-          epilogue_tile_tma<BN>(ep, &tmOut, &tmAux, &tmRes, t_addr, wr.m0 + rank * 128 + q * 32, wr.n0, M, N, half, pp);
-        else
-          epilogue_tile<BN>(ep, t_addr, wr.m0 + rank * 128 + q * 32 + lane, wr.n0, M, N, half);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tempty_bar[acc], 0);   // the leader's MMA thread waits for both CTAs
-    }
-    if (tma_epi && lane == 0) tma_store_wait_all();
   }
-  tc_fence_before();
-  cluster_sync_all();   // peer smem / barriers stay valid until both CTAs are done
-  if (warp == 2) tmem_free_2sm<Cfg::TMEM_COLS>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -730,47 +287,20 @@ static int make_operand_map(CUtensorMap* map, const void* ptr, int mn, int k, in
   return encode_tensor_map_2d_bf16(map, ptr, dims, strides, box, estr);
 }
 
-template <typename KernT>
-static int configure_once(KernT kern, int smem, bool* done) {
-  if (!*done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
-    *done = true;
-  }
-  return D3_OK;
-}
-
 template <int BN, int A_MN, int B_MN>
-static int launch1(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M, int N, int K,
-                   int splits, cudaStream_t stream) {
-  using Cfg = Cfg1<BN>;
-  auto kern = gemm1sm_kernel<BN, A_MN, B_MN>;
+static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M, int N, int K,
+                  int splits, cudaStream_t stream) {
+  using C = Cfg<BN>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN>;
   static bool configured = false;
-  int rc = configure_once(kern, Cfg::SMEM_BYTES, &configured);
-  if (rc) return rc;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+    configured = true;
+  }
   const int work = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * splits;
   const int grid = work < sm_count() ? work : sm_count();
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, ep, M, N, K, splits);
-  cudaError_t e = cudaPeekAtLastError();
-  if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
-  count_launch();
-  return D3_OK;
-}
-
-struct EpiMaps { CUtensorMap out, aux, res; };
-
-template <int A_MN, int B_MN, int TMA_EPI, int SCHED>
-static int launch2(const CUtensorMap& ta, const CUtensorMap& tb, const EpiMaps& em, const GemmEpilogue& ep, int M, int N,
-                   int K, int splits, cudaStream_t stream) {
-  using Cfg2 = Cfg2<TMA_EPI>;
-  auto kern = gemm2sm_kernel<A_MN, B_MN, TMA_EPI, SCHED>;
-  static bool configured = false;
-  int rc = configure_once(kern, Cfg2::SMEM_BYTES, &configured);
-  if (rc) return rc;
-  const int work = ((M + 255) / 256) * ((N + 255) / 256) * splits;
-  const int max_clusters = sm_count() / 2;
-  const int clusters = SCHED ? work : (work < max_clusters ? work : max_clusters);
-  kern<<<2 * clusters, GEMM_THREADS, Cfg2::SMEM_BYTES, stream>>>(ta, tb, em.out, em.aux, em.res, ep, M, N, K, splits);
+  kern<<<grid, GEMM_THREADS, C::SMEM_BYTES, stream>>>(ta, tb, ep, M, N, K, splits);
   cudaError_t e = cudaPeekAtLastError();
   if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
   count_launch();
@@ -778,48 +308,15 @@ static int launch2(const CUtensorMap& ta, const CUtensorMap& tb, const EpiMaps& 
 }
 
 template <int BN>
-static int dispatch1(int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M,
-                     int N, int K, int splits, cudaStream_t s) {
-  if (!a_mn && !b_mn) return launch1<BN, 0, 0>(ta, tb, ep, M, N, K, splits, s);
-  if (!a_mn && b_mn) return launch1<BN, 0, 1>(ta, tb, ep, M, N, K, splits, s);
-  if (a_mn && !b_mn) return launch1<BN, 1, 0>(ta, tb, ep, M, N, K, splits, s);
-  return launch1<BN, 1, 1>(ta, tb, ep, M, N, K, splits, s);
-}
-static void apply_stagger_env() {
-  static bool done = false;
-  if (done) return;
-  done = true;
-  const char* e = getenv("D3_GEMM_STAGGER_NS");
-  const int ns = e ? atoi(e) : 0;
-  if (ns > 0) cudaMemcpyToSymbol(g_gemm_stagger_ns, &ns, sizeof(ns));
-}
-static bool clc_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("D3_GEMM_CLC"); v = (e && e[0] == '1') ? 1 : 0; }   // measured slower in-step: opt-in
-  return v == 1;
-}
-template <int SCHED>
-static int dispatch2s(int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const EpiMaps& em,
-                      const GemmEpilogue& ep, int M, int N, int K, int splits, cudaStream_t s) {
-  if (ep.flags & EP_TMA_EPI) {
-    if (!a_mn && !b_mn) return launch2<0, 0, 1, SCHED>(ta, tb, em, ep, M, N, K, splits, s);
-    if (!a_mn && b_mn) return launch2<0, 1, 1, SCHED>(ta, tb, em, ep, M, N, K, splits, s);
-    if (a_mn && !b_mn) return launch2<1, 0, 1, SCHED>(ta, tb, em, ep, M, N, K, splits, s);
-    return launch2<1, 1, 1, SCHED>(ta, tb, em, ep, M, N, K, splits, s);
-  }
-  if (!a_mn && !b_mn) return launch2<0, 0, 0, SCHED>(ta, tb, em, ep, M, N, K, splits, s);
-  if (!a_mn && b_mn) return launch2<0, 1, 0, SCHED>(ta, tb, em, ep, M, N, K, splits, s);
-  if (a_mn && !b_mn) return launch2<1, 0, 0, SCHED>(ta, tb, em, ep, M, N, K, splits, s);
-  return launch2<1, 1, 0, SCHED>(ta, tb, em, ep, M, N, K, splits, s);
-}
-static int dispatch2(int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const EpiMaps& em,
-                     const GemmEpilogue& ep, int M, int N, int K, int splits, cudaStream_t s) {
-  apply_stagger_env();
-  return clc_enabled() ? dispatch2s<1>(a_mn, b_mn, ta, tb, em, ep, M, N, K, splits, s)
-                       : dispatch2s<0>(a_mn, b_mn, ta, tb, em, ep, M, N, K, splits, s);
+static int dispatch(int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M,
+                    int N, int K, int splits, cudaStream_t s) {
+  if (!a_mn && !b_mn) return launch<BN, 0, 0>(ta, tb, ep, M, N, K, splits, s);
+  if (!a_mn && b_mn) return launch<BN, 0, 1>(ta, tb, ep, M, N, K, splits, s);
+  if (a_mn && !b_mn) return launch<BN, 1, 0>(ta, tb, ep, M, N, K, splits, s);
+  return launch<BN, 1, 1>(ta, tb, ep, M, N, K, splits, s);
 }
 
-// tile_n: 0 = auto; 64/128/256 force the single-CTA kernel with that tile; 512 forces the CTA-pair kernel.
+// tile_n: 0 = auto; 64/128 force that tile width; 256 and 512 (wider tiles) are taken as 128.
 // split_k: 0 = auto (only when the epilogue is a plain fp32 accumulate-able output), >= 1 forced.
 int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K,
               GemmEpilogue ep, int tile_n, int split_k, cudaStream_t stream) {
@@ -828,39 +325,32 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
     return set_error(D3_ERR_ARG, "gemm: operands must be 16-byte aligned with ld % 8 == 0");
   const int sms = sm_count();
   const int num_k = (K + BK - 1) / BK;
-  // ---- kernel / tile choice
-  bool use2 = false;
-  int bn = tile_n;
-  if (tile_n == 512) {
-    use2 = true;
-  } else if (tile_n == 0) {
-    const long tiles2 = (long)((M + 255) / 256) * ((N + 255) / 256);
-    const double eff2 = (double)M * N / ((double)tiles2 * 256 * 256);        // padding efficiency of 256x256 tiles
-    if (tiles2 >= 8 && eff2 >= 0.70) {
-      use2 = true;
-    } else {
-      const int cand[3] = {256, 128, 64};
-      long best = -1;
-      for (int i = 0; i < 3; ++i) {
-        long tiles = (long)((M + BM - 1) / BM) * ((N + cand[i] - 1) / cand[i]);
-        long waves = (tiles + sms - 1) / sms;
-        long cost = waves * (cand[i] + 24);
-        if (best < 0 || cost < best) { best = cost; bn = cand[i]; }
-      }
+  // ---- tile choice: fewest waves of (tile width + fixed per-tile cost) over the SMs
+  int bn = tile_n >= 256 ? 128 : tile_n;
+  if (tile_n == 0) {
+    const int cand[2] = {128, 64};
+    long best = -1;
+    for (int i = 0; i < 2; ++i) {
+      const long tiles = (long)((M + BM - 1) / BM) * ((N + cand[i] - 1) / cand[i]);
+      const long waves = (tiles + sms - 1) / sms;
+      const long cost = waves * (cand[i] + 24);
+      if (best < 0 || cost < best) { best = cost; bn = cand[i]; }
     }
   }
-  // ---- split-K: only for plain fp32 outputs (weight gradients); partial sums are reduced with fp32 atomics into
-  //      an output the caller has zeroed (or wants accumulated into: EP_ACCUM semantics)
+  // ---- split-K: only for plain fp32 outputs (weight gradients) accumulated into (EP_ACCUM); every slice stores its
+  //      partial tile into a workspace and the slices are added to out in slice order (reproducible bit for bit)
   const bool plain_f32 = (ep.flags & EP_OUT_F32) && !(ep.flags & (EP_BIAS | EP_GELU | EP_STORE_PRE | EP_MUL_DGELU |
                                                                   EP_GAMMA | EP_RESID));
   int splits = 1;
   if (split_k >= 1) {
     splits = split_k;
   } else if (plain_f32 && (ep.flags & EP_ACCUM)) {
-    const long units = use2 ? (long)((M + 255) / 256) * ((N + 255) / 256) : (long)((M + BM - 1) / BM) * ((N + bn - 1) / bn);
-    const long slots = use2 ? sms / 2 : sms;
-    if (units * 2 <= slots && num_k >= 16) {
-      splits = (int)(slots / units);
+    const long units = (long)((M + BM - 1) / BM) * ((N + bn - 1) / bn);
+    if (units <= sms && num_k >= 16) {
+      // fill the SMs; and keep every accumulation chain within 64 k-blocks: the tensor core's fp32 accumulation drifts
+      // measurably (> 1e-5 relative) over longer chains, the fp32 reduction of the slices does not
+      splits = units * 2 <= sms ? (int)(sms / units) : 1;
+      if (splits < (num_k + 63) / 64) splits = (num_k + 63) / 64;
       if (splits > num_k / 4) splits = num_k / 4;
       if (splits < 1) splits = 1;
     }
@@ -877,7 +367,6 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
     if (!plain_f32) return set_error(D3_ERR_ARG, "gemm: split-K needs a plain fp32 output");
     if (!(ep.flags & EP_ACCUM)) return set_error(D3_ERR_ARG, "gemm: split-K accumulates into out (set ACCUM, zero it first)");
     if (splits > num_k) splits = num_k;
-    ep.flags |= EP_ATOMIC;
   }
   // ---- epilogue fast-path eligibility
   const int out_elt = (ep.flags & EP_OUT_F32) ? 4 : 2;
@@ -889,53 +378,31 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
   if (ep.flags & EP_MUL_DGELU) aligned = aligned && ((uintptr_t)ep.aux_in % 16 == 0) && (ep.ld_aux % 8 == 0);
   if (!aligned) ep.flags |= EP_SLOW;
   ep.flags |= EP_FAST_ACT;   // hardware tanh (rel. error 2^-11, below the bf16 rounding of the GEMM operands feeding it)
-  {
-    static int dbg = -1;
-    if (dbg < 0) { const char* e = getenv("D3_GEMM_DEBUG"); dbg = e ? atoi(e) : 0; }
-    if (dbg & 1) ep.flags |= EP_DEBUG_NOSTORE;
-    if (dbg & 2) ep.flags |= EP_M_FASTEST;
-  }
 
   CUtensorMap ta, tb;
-  int rc = make_operand_map(&ta, A, M, K, lda, a_mn, 128);
+  int rc = make_operand_map(&ta, A, M, K, lda, a_mn, BM);
   if (rc) return rc;
-  rc = make_operand_map(&tb, B, N, K, ldb, b_mn, use2 ? 128 : bn);
+  rc = make_operand_map(&tb, B, N, K, ldb, b_mn, bn);
   if (rc) return rc;
-  if (use2) {
-    EpiMaps em;
-    memset(&em, 0, sizeof(em));
-    static int no_tma = -1;
-    if (no_tma < 0) { const char* e = getenv("D3_GEMM_NO_TMA_EPI"); no_tma = e ? atoi(e) : 0; }
-    const bool tma_ok = aligned && !no_tma && (N % 32 == 0) && !(ep.flags & (EP_ATOMIC | EP_ACCUM | EP_DEBUG_NOSTORE));
-    if (tma_ok) {
-      const int oe = (ep.flags & EP_OUT_F32) ? 4 : 2;
-      rc = encode_tensor_map_2d(&em.out, ep.out, oe, N, M, (cuuint64_t)ep.ld_out * oe, 32, 32, oe == 4 ? 128 : 64);
-      if (rc) return rc;
-      if (ep.flags & (EP_STORE_PRE | EP_MUL_DGELU)) {
-        const void* ap = (ep.flags & EP_STORE_PRE) ? (const void*)ep.aux_out : (const void*)ep.aux_in;
-        rc = encode_tensor_map_2d(&em.aux, ap, 2, N, M, (cuuint64_t)ep.ld_aux * 2, 32, 32, 64);
-        if (rc) return rc;
-      } else {
-        em.aux = em.out;
-      }
-      if (ep.flags & EP_RESID) {
-        rc = encode_tensor_map_2d(&em.res, ep.resid, 4, N, M, (cuuint64_t)ep.ld_resid * 4, 32, 32, 128);
-        if (rc) return rc;
-      } else {
-        em.res = em.out;
-      }
-      ep.flags |= EP_TMA_EPI;
-    } else {
-      em.out = ta; em.aux = ta; em.res = ta;   // valid descriptors, never dereferenced
-    }
-    return dispatch2(a_mn, b_mn, ta, tb, em, ep, M, N, K, splits, stream);
+  float* ws = nullptr;
+  GemmEpilogue out_ep = ep;
+  if (splits > 1 && !(ep.flags & EP_SCATTER)) {   // slices -> [splits * M, N] workspace, then the ordered reduction
+    ws = slab_workspace((size_t)splits * M * N, stream);
+    if (!ws) return D3_ERR_CUDA;
+    ep.out = ws;
+    ep.ld_out = N;
+    ep.flags = (ep.flags & ~(EP_ACCUM | EP_SLOW)) | EP_SLABS | (N % 4 ? EP_SLOW : 0);
   }
   switch (bn) {
-    case 256: return dispatch1<256>(a_mn, b_mn, ta, tb, ep, M, N, K, splits, stream);
-    case 128: return dispatch1<128>(a_mn, b_mn, ta, tb, ep, M, N, K, splits, stream);
-    case 64: return dispatch1<64>(a_mn, b_mn, ta, tb, ep, M, N, K, splits, stream);
+    case 128: rc = dispatch<128>(a_mn, b_mn, ta, tb, ep, M, N, K, splits, stream); break;
+    case 64: rc = dispatch<64>(a_mn, b_mn, ta, tb, ep, M, N, K, splits, stream); break;
+    default: rc = set_error(D3_ERR_ARG, "gemm: bad tile N");
   }
-  return set_error(D3_ERR_ARG, "gemm: bad tile N");
+  if (ws) {
+    if (!rc) rc = slab_combine(ws, splits, (long long)M * N, M, N, reinterpret_cast<float*>(out_ep.out), out_ep.ld_out, stream);
+    slab_release(ws, stream);
+  }
+  return rc;
 }
 
 }  // namespace d3

@@ -161,14 +161,14 @@ __global__ void center_update_kernel(float* __restrict__ center, const float* __
 // ------------------------------------------------------------------------------------------------ cross-entropy
 // per student row i (logits S[i,:]):  loss_i = - sum_p sum_k Q_p[k] * log_softmax(S[i,:]/ts)[k]   over its teacher
 // rows p in {t0[i], t1[i]} (-1 = none), Q_p from the Sinkhorn scalings above.
-// metric[slot[i]] += wm[i] * loss_i ;  dS[i,k] = wg[i]/ts * (npairs * softmax[k] - sum_p Q_p[k])   (bf16)
+// row_loss[i] = wm[i] * loss_i (added to metric[slot[i]] by metric_rows_kernel) ;  dS[i,k] = wg[i]/ts * (npairs * softmax[k] - sum_p Q_p[k])   (bf16)
 // (dino_clstoken_loss.py:66-89; ibot_patch_loss.py:13-14,55-67; weights per train/ssl_meta_arch.py:480-525)
 __global__ void __launch_bounds__(256)
 ce_fwd_bwd_kernel(const float* __restrict__ S, float inv_ts, const float* __restrict__ Lt,
                   const float* __restrict__ mx, float inv_tt, const float* __restrict__ s_t,
                   const float* __restrict__ a_t, const float* __restrict__ btot, const int* __restrict__ t0,
                   const int* __restrict__ t1, const float* __restrict__ wm, const float* __restrict__ wg,
-                  const int* __restrict__ slot, float* __restrict__ metric, __nv_bfloat16* __restrict__ dS, int K) {
+                  const int* __restrict__ slot, float* __restrict__ row_loss, __nv_bfloat16* __restrict__ dS, int K) {
   __shared__ float sh[32];
   const int i = blockIdx.x;
   const float* Si = S + (long)i * K;
@@ -206,7 +206,7 @@ ce_fwd_bwd_kernel(const float* __restrict__ S, float inv_ts, const float* __rest
     if (dS) dS[(long)i * K + k] = __float2bfloat16(g * (np * __expf(lsm) - q));
   }
   loss = block_sum(loss, sh);
-  if (threadIdx.x == 0) atomicAdd(&metric[slot[i]], wm[i] * loss);
+  if (threadIdx.x == 0) row_loss[i] = wm[i] * loss;
 }
 
 
@@ -299,7 +299,7 @@ ce_fwd_bwd_vec_kernel(const float* __restrict__ S, float inv_ts, const float* __
                       const float* __restrict__ mx, float inv_tt, const float* __restrict__ s_t,
                       const float* __restrict__ a_t, const float* __restrict__ btot, const int* __restrict__ t0,
                       const int* __restrict__ t1, const float* __restrict__ wm, const float* __restrict__ wg,
-                      const int* __restrict__ slot, float* __restrict__ metric, __nv_bfloat16* __restrict__ dS, int K) {
+                      const int* __restrict__ slot, float* __restrict__ row_loss, __nv_bfloat16* __restrict__ dS, int K) {
   __shared__ float sh[32];
   const int i = blockIdx.x;
   const int K4 = K >> 2;
@@ -361,7 +361,7 @@ ce_fwd_bwd_vec_kernel(const float* __restrict__ S, float inv_ts, const float* __
                           pack2(g * (np * exp2f(l2[2]) - q[2]), g * (np * exp2f(l2[3]) - q[3])));
   }
   loss = block_sum(loss, sh);
-  if (threadIdx.x == 0) atomicAdd(&metric[slot[i]], wm[i] * loss);
+  if (threadIdx.x == 0) row_loss[i] = wm[i] * loss;
 }
 
 // ------------------------------------------------------------------------------------------------ KoLeo
@@ -382,7 +382,7 @@ __global__ void koleo_norm_kernel(const float* __restrict__ x, float* __restrict
 // over all B rows.  row0 = 0, nrows = B is the plain KoLeo; a sub-range is KoLeoLossDistributed (loss/koleo_loss.py:39-70:
 // local rows against the all-gathered rows of every rank).
 __global__ void koleo_nn_kernel(const float* __restrict__ xn, int* __restrict__ nn, float* __restrict__ coef,
-                                float* __restrict__ metric, int B, int D, float eps, float w_metric, float w_grad,
+                                float* __restrict__ row_loss, int B, int D, float eps, float w_metric, float w_grad,
                                 int row0, int nrows) {
   __shared__ float sh[32];
   __shared__ float best_v;
@@ -415,7 +415,7 @@ __global__ void koleo_nn_kernel(const float* __restrict__ xn, int* __restrict__ 
     const float dn = sqrtf(dd);
     const float dist = dn + eps;                  // pairwise_distance(...) + eps
     nn[i] = j;
-    atomicAdd(metric, -w_metric * logf(dist + eps) / nrows);
+    row_loss[i] = -w_metric * logf(dist + eps) / nrows;
     // d(-w/nrows * log(dist+eps))/d(delta) = -w/nrows / (dist+eps) * delta/||delta||
     coef[i] = dn > 0.f ? -w_grad / nrows / (dist + eps) / dn : 0.f;
   }
@@ -447,7 +447,7 @@ __global__ void koleo_bwd_kernel(const float* __restrict__ x, const float* __res
 }
 
 // ---- Gram-anchoring loss (loss/gram_loss.py:13-50): elementwise stage between the similarity GEMMs and the backward
-// GEMM.  Ss = Xs Xs^T and St = Xt Xt^T are fp32 [n, n] (tcgen05 GEMMs); per element
+// GEMM.  Ss = Xs Xs^T and St = Xt Xt^T are fp32 [n, n] (wgmma GEMMs); per element
 //   mode 1 (remove_neg):              s' = max(s, 0), t' = max(t, 0),            ds'/ds = [s > 0]
 //   mode 2 (remove_only_teacher_neg): s' = (s < 0 && t < 0) ? 0 : s, t' = max(t, 0), ds'/ds = !(s < 0 && t < 0)
 //   mode 0:                           s' = s, t' = t
@@ -583,32 +583,81 @@ int d3_center_update(float* center, const float* colsum, const float* total_rows
   D3_CHECK_LAUNCH();
   return D3_OK;
 }
+}  // extern "C"
+
+namespace d3 {
+// metric[slot[i]] += row_loss[i] (slot == nullptr: every row to metric[0]; slots 0..7), rows added in a fixed order
+__global__ void __launch_bounds__(256) metric_rows_kernel(const float* __restrict__ row_loss, const int* __restrict__ slot,
+                                                          int n, float* __restrict__ metric) {
+  __shared__ float sh[8][256];
+  __shared__ int used;
+  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  int seen = 0;
+  if (threadIdx.x == 0) used = 0;
+  for (int i = threadIdx.x; i < n; i += 256) {
+    const int sl = slot ? slot[i] : 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      if (sl == k) { acc[k] += row_loss[i]; seen |= 1 << k; }
+  }
+  __syncthreads();
+  if (seen) atomicOr(&used, seen);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) sh[k][threadIdx.x] = acc[k];
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w)
+#pragma unroll
+      for (int k = 0; k < 8; ++k) sh[k][threadIdx.x] += sh[k][threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x < 8 && (used >> threadIdx.x & 1)) metric[threadIdx.x] += sh[threadIdx.x][0];
+}
+static int add_row_losses(float* row_loss, const int* slot, int n, float* metric, cudaStream_t st) {
+  metric_rows_kernel<<<1, 256, 0, st>>>(row_loss, slot, n, metric);
+  cudaError_t e = cudaPeekAtLastError();
+  slab_release(row_loss, st);
+  if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  count_launch();
+  return D3_OK;
+}
+}  // namespace d3
+
+extern "C" {
+
 int d3_ce_fwd_bwd(const float* S, float student_temp, const float* Lt, const float* mx, float teacher_temp,
                   const float* s_t, const float* a_t, const float* btot, const int* t0, const int* t1, const float* wm,
                   const float* wg, const int* slot, float* metric, void* dS, int Rs, int K, void* stream) {
   if (Rs <= 0) return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  float* rows = slab_workspace(Rs, st);
+  if (!rows) return D3_ERR_CUDA;
   if (K % 4 == 0 && ((uintptr_t)S | (uintptr_t)Lt | (uintptr_t)s_t | (uintptr_t)dS | (uintptr_t)mx) % 16 == 0)
-    ce_fwd_bwd_vec_kernel<<<Rs, 512, 0, STREAM(stream)>>>(S, 1.f / student_temp, Lt, mx, 1.f / teacher_temp, s_t, a_t, btot,
-                                                         t0, t1, wm, wg, slot, metric, (__nv_bfloat16*)dS, K);
+    ce_fwd_bwd_vec_kernel<<<Rs, 512, 0, st>>>(S, 1.f / student_temp, Lt, mx, 1.f / teacher_temp, s_t, a_t, btot,
+                                             t0, t1, wm, wg, slot, rows, (__nv_bfloat16*)dS, K);
   else
-    ce_fwd_bwd_kernel<<<Rs, 256, 0, STREAM(stream)>>>(S, 1.f / student_temp, Lt, mx, 1.f / teacher_temp, s_t, a_t, btot, t0,
-                                                     t1, wm, wg, slot, metric, (__nv_bfloat16*)dS, K);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+    ce_fwd_bwd_kernel<<<Rs, 256, 0, st>>>(S, 1.f / student_temp, Lt, mx, 1.f / teacher_temp, s_t, a_t, btot, t0,
+                                         t1, wm, wg, slot, rows, (__nv_bfloat16*)dS, K);
+  cudaError_t e = cudaPeekAtLastError();
+  if (e != cudaSuccess) { slab_release(rows, st); return set_error(D3_ERR_CUDA, cudaGetErrorString(e)); }
+  count_launch();
+  return add_row_losses(rows, slot, Rs, metric, st);
 }
 int d3_koleo_fwd_bwd_rows(const float* x, float* xn_scratch, float* nrm_scratch, int* nn_scratch, float* coef_scratch,
                           float* metric, float* dx, int B, int D, int row0, int nrows, float eps, float w_metric,
                           float w_grad, void* stream) {
   if (B <= 1 || nrows <= 0) return D3_OK;
   if (row0 < 0 || row0 + nrows > B) return set_error(D3_ERR_ARG, "d3_koleo_fwd_bwd_rows: local row range outside [0, B)");
-  koleo_norm_kernel<<<B, 256, 0, STREAM(stream)>>>(x, xn_scratch, nrm_scratch, D, eps);
-  koleo_nn_kernel<<<B, 256, 0, STREAM(stream)>>>(xn_scratch, nn_scratch, coef_scratch, metric, B, D, eps, w_metric,
-                                                w_grad, row0, nrows);
-  koleo_bwd_kernel<<<B, 256, D * sizeof(float), STREAM(stream)>>>(x, xn_scratch, nrm_scratch, nn_scratch, coef_scratch,
-                                                                dx, B, D, eps);
-  D3_CHECK_LAUNCH();
-  count_launch(2);
-  return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  float* rows = slab_workspace(B, st);
+  if (!rows) return D3_ERR_CUDA;
+  koleo_norm_kernel<<<B, 256, 0, st>>>(x, xn_scratch, nrm_scratch, D, eps);
+  koleo_nn_kernel<<<B, 256, 0, st>>>(xn_scratch, nn_scratch, coef_scratch, rows, B, D, eps, w_metric, w_grad, row0, nrows);
+  koleo_bwd_kernel<<<B, 256, D * sizeof(float), st>>>(x, xn_scratch, nrm_scratch, nn_scratch, coef_scratch, dx, B, D, eps);
+  cudaError_t e = cudaPeekAtLastError();
+  if (e != cudaSuccess) { slab_release(rows, st); return set_error(D3_ERR_CUDA, cudaGetErrorString(e)); }
+  count_launch(3);
+  return add_row_losses(rows, nullptr, B, metric, st);
 }
 int d3_gram_diff(const float* Ss, const float* St, void* G_bf16, long long n_elems, int mode, float inv_count, float* loss,
                  int n, int block, void* stream) {
@@ -628,14 +677,16 @@ int d3_gram_diff(const float* Ss, const float* St, void* G_bf16, long long n_ele
 int d3_koleo_fwd_bwd(const float* x, float* xn_scratch, float* nrm_scratch, int* nn_scratch, float* coef_scratch,
                      float* metric, float* dx, int B, int D, float eps, float w_metric, float w_grad, void* stream) {
   if (B <= 1) return D3_OK;
-  koleo_norm_kernel<<<B, 256, 0, STREAM(stream)>>>(x, xn_scratch, nrm_scratch, D, eps);
-  koleo_nn_kernel<<<B, 256, 0, STREAM(stream)>>>(xn_scratch, nn_scratch, coef_scratch, metric, B, D, eps, w_metric,
-                                                w_grad, 0, B);
-  koleo_bwd_kernel<<<B, 256, D * sizeof(float), STREAM(stream)>>>(x, xn_scratch, nrm_scratch, nn_scratch, coef_scratch,
-                                                                dx, B, D, eps);
-  D3_CHECK_LAUNCH();
-  count_launch(2);
-  return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  float* rows = slab_workspace(B, st);
+  if (!rows) return D3_ERR_CUDA;
+  koleo_norm_kernel<<<B, 256, 0, st>>>(x, xn_scratch, nrm_scratch, D, eps);
+  koleo_nn_kernel<<<B, 256, 0, st>>>(xn_scratch, nn_scratch, coef_scratch, rows, B, D, eps, w_metric, w_grad, 0, B);
+  koleo_bwd_kernel<<<B, 256, D * sizeof(float), st>>>(x, xn_scratch, nrm_scratch, nn_scratch, coef_scratch, dx, B, D, eps);
+  cudaError_t e = cudaPeekAtLastError();
+  if (e != cudaSuccess) { slab_release(rows, st); return set_error(D3_ERR_CUDA, cudaGetErrorString(e)); }
+  count_launch(3);
+  return add_row_losses(rows, nullptr, B, metric, st);
 }
 
 }  // extern "C"

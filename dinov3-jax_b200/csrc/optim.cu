@@ -7,7 +7,8 @@
 
 namespace d3 {
 
-__global__ void sumsq_kernel(const float* __restrict__ g, long n, float* __restrict__ out) {
+// each CTA's share of sum(g^2) goes to ws[blockIdx.x]; the shares are added in CTA order (reproducible clip factor)
+__global__ void sumsq_kernel(const float* __restrict__ g, long n, float* __restrict__ ws) {
   __shared__ float sh[32];
   float acc = 0.f;
   const long n4 = n / 4;
@@ -25,7 +26,7 @@ __global__ void sumsq_kernel(const float* __restrict__ g, long n, float* __restr
     float t = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.f;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if (threadIdx.x == 0) atomicAdd(out, t);
+    if (threadIdx.x == 0) ws[blockIdx.x] = t;
   }
 }
 
@@ -109,9 +110,16 @@ extern "C" {
 int d3_sumsq(const float* g, long long n, float* out, void* stream) {
   if (n <= 0) return D3_OK;
   if ((uintptr_t)g & 15) return set_error(D3_ERR_ARG, "d3_sumsq: alignment");
-  sumsq_kernel<<<(int)min((n / 4 + 255) / 256 + 1, (long long)sm_count() * 8), 256, 0, STREAM(stream)>>>(g, n, out);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  const int blocks = (int)min((n / 4 + 255) / 256 + 1, (long long)sm_count() * 8);
+  float* ws = slab_workspace(blocks, st);
+  if (!ws) return D3_ERR_CUDA;
+  sumsq_kernel<<<blocks, 256, 0, st>>>(g, n, ws);
+  cudaError_t e = cudaPeekAtLastError();
+  int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  if (!rc) { count_launch(); rc = slab_combine(ws, blocks, 1, 1, 1, out, 1, st); }
+  slab_release(ws, st);
+  return rc;
 }
 
 int d3_adamw_ema(float* p, const float* g, float* m, float* v, float* teacher, void* p_bf16, void* t_bf16,

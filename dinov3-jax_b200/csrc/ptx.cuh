@@ -1,7 +1,6 @@
-// sm_100a PTX wrappers used by every tensor-core kernel in this library:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), proxy fences.
-// Hand-written; encodings follow the PTX ISA 8.7 tcgen05 chapter (descriptor bit layouts are
-// documented next to each builder).
+// sm_90a PTX wrappers used by every tensor-core kernel in this library:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (descriptors / fence / commit / wait, SS and RS forms), proxy fences.
+// Hand-written; encodings follow the PTX ISA wgmma chapter (descriptor bit layout documented next to the builder).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -14,9 +13,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
-// One lane of a CONVERGED warp.  tcgen05.mma / commit / TMA are warp-uniform instructions: issued under this predicate
-// from warp-uniform control flow they compile to a single UTCHMMA / UTMALDG; issued under `lane == 0` (divergent code)
-// ptxas wraps every one of them in an ELECT ... BRA.U.ANY serialisation loop (~60-90 cycles per instruction).
+// One lane of a CONVERGED warp: TMA and bulk copies issued under this predicate from warp-uniform control flow compile
+// to a single instruction instead of a per-lane serialisation loop.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -57,12 +55,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
 
 // ------------------------------------------------------------------ TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -96,165 +88,67 @@ __device__ __forceinline__ void tma_load_2d_cta(const CUtensorMap* m, uint64_t* 
       : "memory");
 }
 
-// ------------------------------------------------------------------ TMEM
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-  static_assert(COLS == 32 || COLS == 64 || COLS == 128 || COLS == 256 || COLS == 512, "tmem cols");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_free(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(COLS) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread t <-> lane base+t).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM: thread t writes lane base+t, 8 / 16 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------ UMMA descriptors
+// ------------------------------------------------------------------ wgmma
 // Shared-memory matrix descriptor (64 bit):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4   [46,48) version = 1 (Blackwell)
-//   [49,52) base offset (0: tiles are 1024 B aligned)   [61,64) layout: 2 = SWIZZLE_128B
+//   [32,46) stride-dim byte offset >> 4   [49,52) base offset (0: tiles are 1024 B aligned)   [62,64) 1 = SWIZZLE_128B
 // K-major SW128 tile  : rows of 128 B (64 bf16 along K); 8-row groups SBO = 1024 B apart; LBO unused (1).
+//                       One k16 step advances the start address by 32 B.
 // MN-major SW128 tile : rows of 128 B (64 bf16 along M/N) indexed by k; 8-k groups SBO = 1024 B apart;
-//                       64-element M/N groups LBO bytes apart.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+//                       64-element M/N groups LBO bytes apart.  One k16 step advances the start address by 2048 B.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32:
-//   [4,6) c_format=1 (F32)  [7,10) a_format=1 (BF16)  [10,13) b_format=1 (BF16)
-//   [15] a_major (0=K,1=MN) [16] b_major  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// register budget of a warp-specialised role (whole warpgroup executes it)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// D (+)= A * B for one warpgroup, A and B from shared memory (SS) or A from registers (RS).  TA / TB: 0 = K-major,
+// 1 = MN-major operand.  Accumulator fragment of m64nN: thread t of the warpgroup holds rows 16 (t/32) + (t%32)/4 and
+// that + 8; register 4i + {0,1} are columns 8i + 2 (t%4) + {0,1} of the first row, 4i + {2,3} of the second.
+// The RS A fragment (m64k16) has the same layout for columns 0..15, packed two bf16 per register.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M = 128 rows in lanes, K-major) is read from tensor memory —
-// 16-bit elements packed two per 32-bit column (element 2j in bits [0,16) of column j), 8 columns per UMMA_K = 16.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB));
 }
 
-
-// ------------------------------------------------------------------ clusters / 2-CTA (cta_group::2) variants
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // clears the CTA-rank bit of a shared::cluster address -> CTA 0 of the pair
-// arrive (count 1) on the mbarrier at the same offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
-}
-// TMA load into this CTA's smem, completing transaction bytes on the LEADER CTA's mbarrier (same offset)
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_free_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(COLS) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem of both CTAs: 128 rows each] * B[smem of both CTAs: N/2 columns each]
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit: arrive on the mbarrier at this offset in both CTAs of the pair when the issued MMAs retire
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
-}
 // 2^x on the SFU (ex2.approx, rel. error 2^-22; -inf -> 0)
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -279,40 +173,6 @@ __device__ __forceinline__ float gelu_tanh_grad_fast(float u) {
   return 0.5f * (1.0f + t) + 0.5f * u * (1.0f - t * t) * dz;
 }
 
-
-// ------------------------------------------------------------------ cluster launch control (dynamic tile scheduling)
-// arrive + expect_tx on the mbarrier at the same offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_expect_tx_cluster(uint64_t* bar, uint32_t cta, uint32_t bytes) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.expect_tx.shared::cluster.b64 _, [ra], %2;\n\t}"
-      ::"r"(smem_u32(bar)), "r"(cta), "r"(bytes)
-      : "memory");
-}
-// Try to cancel the launch of a not-yet-started cluster of this grid; the 16-byte response is written to `resp` and
-// 16 transaction bytes are completed on `bar`, at the same shared-memory offsets in EVERY CTA of the cluster.
-__device__ __forceinline__ void clc_try_cancel_multicast(void* resp, uint64_t* bar) {
-  asm volatile(
-      "clusterlaunchcontrol.try_cancel.async.shared::cta.mbarrier::complete_tx::bytes.multicast::cluster::all.b128 [%0], [%1];"
-      ::"r"(smem_u32(resp)), "r"(smem_u32(bar))
-      : "memory");
-}
-// Decode a response: true + ctaid.x of the first CTA of the cancelled cluster, or false when nothing was left to cancel.
-__device__ __forceinline__ bool clc_query(const void* resp, uint32_t& ctaid_x) {
-  uint32_t valid = 0, x = 0;
-  asm volatile(
-      "{\n\t.reg .pred p1;\n\t.reg .b128 r;\n\t"
-      "ld.shared.b128 r, [%2];\n\t"
-      "clusterlaunchcontrol.query_cancel.is_canceled.pred.b128 p1, r;\n\t"
-      "selp.u32 %1, 1, 0, p1;\n\t"
-      "@p1 clusterlaunchcontrol.query_cancel.get_first_ctaid.v4.b32.b128 {%0, _, _, _}, r;\n\t}"
-      : "+r"(x), "=r"(valid)
-      : "r"(smem_u32(resp))
-      : "memory");
-  ctaid_x = x;
-  return valid != 0;
-}
 
 // ------------------------------------------------------------------ math helpers
 __device__ __forceinline__ float gelu_tanh(float u) {

@@ -1,4 +1,4 @@
-"""B200-native DINOv3 SSL training hot path behind the reference's module names (Dhia-naouali/dinov3-jax).
+"""CUDA-native DINOv3 SSL training hot path behind the reference's module names (Dhia-naouali/dinov3-jax).
 
 This package provides `dinov3_jax.{train, fsdp, layers, loss, models, checkpointer, configs, distributed}` and the
 jax-free pieces of `dinov3_jax.data` (collate, masking).  It is an OVERLAY: put it first on PYTHONPATH and, if the

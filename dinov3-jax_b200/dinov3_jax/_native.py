@@ -1,6 +1,6 @@
 """ctypes binding of libdinov3_b200.so (the C ABI declared in include/dinov3_b200.h).
 
-There is deliberately no fallback: if the shared library is missing, or the process has no sm_100 GPU, every
+There is deliberately no fallback: if the shared library is missing, or the process has no sm_90 GPU, every
 entry point raises.  PyTorch tensors are only containers for device memory here (``tensor.data_ptr()``).
 """
 from __future__ import annotations
@@ -96,7 +96,7 @@ def lib() -> C.CDLL:
         path = os.environ.get("DINOV3_B200_LIB", str(LIB_PATH))
         if not os.path.exists(path):
             raise NativeError(
-                f"{path} not found: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+                f"{path} not found: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
                 "There is no CPU / PyTorch fallback for the training hot path.")
         _LIB = C.CDLL(path)
         _LIB.d3_last_error.restype = C.c_char_p
@@ -114,11 +114,11 @@ def check(rc: int, what: str = "") -> None:
 
 
 def init(device: int | None = None) -> C.CDLL:
-    """Bind the library to a CUDA device; raises if it is not a Blackwell (sm_100) part."""
+    """Bind the library to a CUDA device; raises if it is not a Hopper (sm_90) part."""
     global _INIT_DEVICE
     l = lib()
     if not torch.cuda.is_available():
-        raise NativeError("no CUDA device: the dinov3 B200 engine has no CPU fallback")
+        raise NativeError("no CUDA device: the dinov3 GPU engine has no CPU fallback")
     if device is None:
         device = torch.cuda.current_device()
     if _INIT_DEVICE != device:

@@ -2,7 +2,7 @@
 `key=value` overrides, dotted attribute access, and the learning-rate scaling rules (:43-56).
 
 The reference's own `ssl_default_config.yaml` / `configs/train/*.yaml` load unchanged (pass them as `config_file`);
-`DEFAULTS` below only carries the keys the B200 engine honours, with the reference's default values
+`DEFAULTS` below only carries the keys the GPU engine honours, with the reference's default values
 (ssl_default_config.yaml line numbers in SURVEY.md §5), so the package also runs without the reference checkout.
 """
 from __future__ import annotations

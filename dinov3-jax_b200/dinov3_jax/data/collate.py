@@ -1,6 +1,6 @@
 """Batch collation with the reference's dict contract (dinov3_jax/data/collate.py:16-93), torch tensors out.
 
-The reference converts to jax arrays through dlpack (:85-91); the B200 engine consumes the torch tensors directly
+The reference converts to jax arrays through dlpack (:85-91); the GPU engine consumes the torch tensors directly
 (NHWC, `compute_precision.param_dtype`), so that conversion is dropped — everything else keeps its key and meaning.
 """
 from __future__ import annotations

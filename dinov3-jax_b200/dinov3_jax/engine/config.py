@@ -1,4 +1,4 @@
-"""Static description of one training configuration for the B200 engine (derived from the reference's YAML keys).
+"""Static description of one training configuration for the GPU engine (derived from the reference's YAML keys).
 
 Field names follow dinov3_jax/configs/ssl_default_config.yaml; arch table follows
 dinov3_jax/models/vision_transformer.py:325-408.
@@ -122,9 +122,9 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
                  "swiglu128": ("swiglu", 128)}                      # models/vision_transformer.py:30-36
     if cfg.student.ffn_layer not in ffn_table or cfg.student.norm_layer not in ("layernorm", "layernormbf16"):
         raise NotImplementedError("ffn_layer must be mlp | swiglu[32|64|128] and norm_layer layernorm | layernormbf16 "
-                                  "(RMSNorm is not on the B200 path, SURVEY 8f)")
+                                  "(RMSNorm is not on the GPU path, SURVEY 8f)")
     if cfg.dino.koleo_loss_distributed or cfg.dino.reweight_dino_local_loss:
-        raise NotImplementedError("distributed KoLeo inside the step / local-loss reweighting are not on the B200 path yet")
+        raise NotImplementedError("distributed KoLeo inside the step / local-loss reweighting are not on the GPU path yet")
     gram_kw = {}
     if cfg.gram.use_loss:
         gg = cfg.gram
@@ -134,7 +134,7 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
             raise ValueError("gram.tokens_used masked | unmasked needs gram.img_level: false (ssl_meta_arch.py:222-223)")
         if gg.get("compute_stats", False):
             import warnings
-            warnings.warn("gram.compute_stats: the stats_only/* metrics are not produced by the B200 engine", stacklevel=2)
+            warnings.warn("gram.compute_stats: the stats_only/* metrics are not produced by the GPU engine", stacklevel=2)
         if gg.get("ckpt", None) is not None:
             raise NotImplementedError("gram.ckpt: load the gram teacher with dinov3_jax.checkpointer and Engine.gram_teacher_load "
                                       "instead of a path in the config")
@@ -171,7 +171,7 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
     if not g(cfg.dino, "global_ignore_diagonal", True):
         raise NotImplementedError("dino.global_ignore_diagonal=false: the pair tables implement the default (true)")
     if int(g(cfg.dino, "head_nlayers", 3)) != 3 or int(g(cfg.ibot, "head_nlayers", 3)) != 3:
-        raise NotImplementedError("head_nlayers != 3 (layers/dino_head.py default) is not on the B200 path")
+        raise NotImplementedError("head_nlayers != 3 (layers/dino_head.py default) is not on the GPU path")
     if "multidistillation" in cfg and g(cfg["multidistillation"], "enabled", False):
         raise NotImplementedError("multidistillation is outside the training hot path (SURVEY §2 out of scope)")
     if float(g(cfg.student, "drop_path_rate", 0.0) or 0.0) > 0.0:

@@ -1,4 +1,4 @@
-"""B200 step executor for the DINOv3 SSL hot path (replaces the jitted `train_step` of the reference,
+"""GPU step executor for the DINOv3 SSL hot path (replaces the jitted `train_step` of the reference,
 dinov3_jax/train/train.py:491-565, and `SSLMetaArch.__call__`, train/ssl_meta_arch.py:289-363).
 
 There is no autograd and no PyTorch math here: the forward and the hand-derived backward are explicit sequences of
@@ -222,7 +222,7 @@ class Engine:
             self.dH = e(T, Hd)
             self.dZ32 = e(T, D, dt=f32)
         self.dQKV = [e(T, 3 * D) for _ in range(nbuf)]
-        self.fwd_overlap = os.environ.get("D3_FWD_STREAMS", "0") == "1"   # measured: no gain (step is power-capped), off by default
+        self.fwd_overlap = os.environ.get("D3_FWD_STREAMS", "0") == "1"   # off by default
         if self.fwd_overlap:
             self.tstream = torch.cuda.Stream(device=self.device)
             self._ev_fwd = [torch.cuda.Event(), torch.cuda.Event()]

@@ -1,4 +1,4 @@
-"""Flat parameter / gradient / optimiser-state storage for the B200 engine.
+"""Flat parameter / gradient / optimiser-state storage for the GPU engine.
 
 One `ModuleStore` per top-level module of the reference's parameter tree (`backbone`, `dino_head`, `ibot_head`;
 train/ssl_meta_arch.py:62-64,86-87,130-131), holding the student (fp32 master, bf16 compute copy, fp32 gradient, Adam

@@ -87,11 +87,8 @@ class FsdpRuntime:
         self._push_side = os.environ.get("D3_FSDP_PUSH_SIDE", "1") != "0"          # 0: stand-alone pushes on the compute stream
         self._vec_perm = {}
         self._vec_tmp = {}
-        # Default: on at every world size.  Round 1 saw an asynchronous launch failure with the GEMM-epilogue scatter at 8
-        # ranks on ViT-L; in round 2 it no longer occurs (tools/check_fsdp_push.py: pushed shards == NCCL reduce-scatter
-        # to 8e-8 at 8 ranks with ViT-L block shapes; bench.py --gpus 8 with the push path: profiles/r02_*8gpu*), after the
-        # issue path of every TMA / tcgen05 / bulk-copy instruction moved to elect.sync.  D3_FSDP_PUSH=0 selects the
-        # NCCL reduce-scatter.
+        # Default: on at every world size (tools/check_fsdp_push.py compares the pushed shards with the NCCL
+        # reduce-scatter).  D3_FSDP_PUSH=0 selects the NCCL reduce-scatter.
         want = os.environ.get("D3_FSDP_PUSH", "auto")
         if self.cuda and self.world > 1 and comm.backend == "nccl" and want in ("1", "auto"):
             self._setup_push()

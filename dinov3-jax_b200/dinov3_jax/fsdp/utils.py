@@ -84,6 +84,6 @@ def sync_grads(grads, axis_name="dp"):
 
 
 def fsdp_wrapper(target, axis_name="dp", min_param_size=2 ** 4):
-    """The reference returns nn.map_variables(target, gather on read, shard on write) (:87-94).  The B200 engine shards
+    """The reference returns nn.map_variables(target, gather on read, shard on write) (:87-94).  The GPU engine shards
     by FSDP unit inside Engine(comm=...); wrapping a module class is therefore the identity, kept for API compatibility."""
     return target

@@ -1,5 +1,5 @@
 """Layer objects with the reference's names and constructor fields (dinov3_jax/layers/*.py), forward pass on CUDA
-tensors through the B200 kernels.  Parameters are passed as a dict with the reference's leaf names and layouts
+tensors through the CUDA kernels.  Parameters are passed as a dict with the reference's leaf names and layouts
 (Dense `kernel` [in, out], `bias`; LayerNorm `scale`, `bias`; LayerScale `gamma`).  These are inference-style
 wrappers for unit-level use and tests; the training engine fuses the same kernels block-wise (engine/core.py).
 """
@@ -28,7 +28,7 @@ class RopePositionEmbedding:
                  normalize_coords: str = "separate", shift_coords=None, jitter_coords=None, rescale_coords=None, dtype=None):
         assert embed_dim % (4 * num_heads) == 0
         if base is None or min_period is not None or max_period is not None:
-            raise NotImplementedError("only the `base` parametrisation is on the B200 path")
+            raise NotImplementedError("only the `base` parametrisation is on the GPU path")
         if normalize_coords != "separate":
             raise NotImplementedError("normalize_coords must be 'separate' (default)")
         self.head_dim, self.base = embed_dim // num_heads, base
@@ -155,7 +155,7 @@ class DINOHead:
     def __init__(self, params: dict, in_dim: int, out_dim: int, use_bn: bool = False, nlayers: int = 3,
                  hidden_dim: int = 2048, bottleneck_dim: int = 256, mlp_bias: bool = True):
         if use_bn or nlayers != 3:
-            raise NotImplementedError("DINOHead on the B200 path: nlayers=3, no batch norm (reference defaults)")
+            raise NotImplementedError("DINOHead on the GPU path: nlayers=3, no batch norm (reference defaults)")
         m = params["mlp"]
         self.w = [_w(m[f"layers_{i}"]["kernel"]) for i in (0, 2, 4)]
         self.b = [_v(m[f"layers_{i}"]["bias"]) for i in (0, 2, 4)]

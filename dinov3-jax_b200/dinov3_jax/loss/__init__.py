@@ -1,4 +1,4 @@
-"""Loss objects with the reference's class / method names (dinov3_jax/loss/*.py), forward values computed by the B200
+"""Loss objects with the reference's class / method names (dinov3_jax/loss/*.py), forward values computed by the CUDA
 kernels on CUDA tensors.  (The training engine uses the same kernels in their fused forward+backward form.)"""
 from __future__ import annotations
 
@@ -155,7 +155,7 @@ class KoLeoLossDistributed:
 
     def __init__(self, topk: int = 1, loss_group_size=None, comm=None):
         if topk != 1:
-            raise NotImplementedError("KoLeoLossDistributed: topk > 1 is not on the B200 path")
+            raise NotImplementedError("KoLeoLossDistributed: topk > 1 is not on the GPU path")
         self.comm, self.loss_group_size = comm, loss_group_size
 
     def __call__(self, student_output, eps=1e-8):

@@ -1,5 +1,5 @@
 """Model factories with the reference's names (dinov3_jax/models/__init__.py:17-72, vision_transformer.py:325-408).
-On the B200 path a "model" is its static description (EngineConfig); parameters live in the engine's flat buffers."""
+On the GPU path a "model" is its static description (EngineConfig); parameters live in the engine's flat buffers."""
 from __future__ import annotations
 
 from dataclasses import replace
@@ -22,7 +22,7 @@ vit_so400m, vit_huge2, vit_giant2 = _factory("vit_so400m"), _factory("vit_huge2"
 def build_model(args, only_teacher: bool = False, img_size: int = 224):
     """models/__init__.py:17-55: returns (student, teacher, embed_dim) — here two (equal) static descriptions."""
     if args.arch not in ARCHS:
-        raise ValueError(f"unknown arch {args.arch!r} (ConvNeXt and vit_7b are not on the B200 path)")
+        raise ValueError(f"unknown arch {args.arch!r} (ConvNeXt and vit_7b are not on the GPU path)")
     cfg = config_for(args.arch, patch=args.patch_size)
     if only_teacher:
         return cfg, cfg.embed_dim

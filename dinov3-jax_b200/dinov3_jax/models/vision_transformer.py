@@ -1,5 +1,5 @@
 """`DinoVisionTransformer` with the reference's constructor fields and call signature
-(dinov3_jax/models/vision_transformer.py:55-321), forward pass through the B200 kernels.
+(dinov3_jax/models/vision_transformer.py:55-321), forward pass through the CUDA kernels.
 
 This is the feature-extraction entry point (`model(x)` / `model([global, local], masks=[m, None], is_training=True)`);
 training goes through engine/core.py, which runs the same kernels on packed multi-crop streams with the stash the
@@ -28,11 +28,11 @@ class DinoVisionTransformer:
                  untie_global_and_local_cls_norm: bool = False, device="cuda"):
         if norm_layer not in ("layernorm", "layernormbf16") or ffn_layer != "mlp" or mask_k_bias \
                 or untie_cls_and_patch_norms or untie_global_and_local_cls_norm:
-            raise NotImplementedError("B200 path: layernorm(bf16) + mlp blocks, tied norms, no mask_k_bias (SURVEY §8f.1)")
+            raise NotImplementedError("GPU path: layernorm(bf16) + mlp blocks, tied norms, no mask_k_bias (SURVEY §8f.1)")
         self.eps = 1e-5 if norm_layer == "layernormbf16" else 1e-6        # models/vision_transformer.py:38-42
         self.n_storage_tokens = n_storage_tokens
         if drop_path_rate:
-            raise NotImplementedError("stochastic depth is not on the B200 path (reference default 0 is asserted upstream)")
+            raise NotImplementedError("stochastic depth is not on the GPU path (reference default 0 is asserted upstream)")
         dev = torch.device(device)
         to = lambda t: torch.as_tensor(t).to(dev)
         mv = lambda tree: {k: (mv(v) if isinstance(v, dict) else to(v)) for k, v in tree.items()}

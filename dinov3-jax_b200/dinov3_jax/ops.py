@@ -28,7 +28,7 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, a_mn: bool = Fa
          dgelu_of: torch.Tensor | None = None, gamma: torch.Tensor | None = None,
          resid: torch.Tensor | None = None, accum: bool = False, alpha: float = 1.0, tile_n: int = 0,
          split_k: int = 0, scatter=None) -> torch.Tensor:
-    """out[M,N] = epilogue(alpha * A.B) on the tcgen05 tensor cores (d3_gemm_bf16).
+    """out[M,N] = epilogue(alpha * A.B) on the wgmma tensor cores (d3_gemm_bf16).
 
     A is [M,K] (a_mn=False) or stored transposed [K,M] (a_mn=True); B is [N,K] (b_mn=False) or [K,N] (b_mn=True).
     """

@@ -1,7 +1,7 @@
 """`SSLMetaArch` with the reference's constructor and helper names (dinov3_jax/train/ssl_meta_arch.py:32-660).
 
 The reference class is a Flax module whose `__call__` is traced by jax.jit; here it is a plain object that owns the
-configuration and builds the B200 step executor.  The top-level parameter keys (`student_backbone`, `student_dino_head`,
+configuration and builds the GPU step executor.  The top-level parameter keys (`student_backbone`, `student_dino_head`,
 `student_ibot_head`, `teacher_*`; :62-64,86-87,130-131) and the batch-dict contract are unchanged.
 """
 from __future__ import annotations
@@ -42,7 +42,7 @@ class SSLMetaArch:
     def gram_teacher_initialized(self) -> bool:
         return bool(self.engine is not None and self.engine.gram_active and self.has_gram_teacher)
 
-    # -- B200 engine -------------------------------------------------------------------------------------------------
+    # -- GPU engine -------------------------------------------------------------------------------------------------
     def build_engine(self, device="cuda", comm=None, max_masked=None) -> Engine:
         # train.checkpointing (ssl_default_config.yaml:88-89): activation rematerialisation of the student blocks
         remat = bool(self.config.train.get("checkpointing", False) or self.config.train.get("checkpointing_full", False))

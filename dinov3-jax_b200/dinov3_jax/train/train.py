@@ -30,7 +30,7 @@ from .ssl_meta_arch import SSLMetaArch
 
 def get_args_parser(add_help: bool = True):
     """Flags of the reference parser (train/train.py:51-72): same names, positional `seed` (optional here, default 12)."""
-    p = argparse.ArgumentParser("DINOv3 training (B200 engine)", add_help=add_help)
+    p = argparse.ArgumentParser("DINOv3 training (GPU engine)", add_help=add_help)
     p.add_argument("--config-file", default="", metavar="FILE")
     p.add_argument("--no-resume", action="store_true")
     p.add_argument("--eval-only", action="store_true", help="eval only")
@@ -47,7 +47,7 @@ def get_args_parser(add_help: bool = True):
     p.add_argument("--record-ref-losses", action="store_true")
     p.add_argument("--ref-losses-path", default="", type=str)
     p.add_argument("--multi-distillation", action="store_true")
-    # B200-engine extras
+    # GPU-engine extras
     p.add_argument("--max-iters", default=0, type=int, help="stop after this many iterations (0 = full schedule)")
     p.add_argument("--print-freq", default=10, type=int)
     return p
@@ -75,7 +75,7 @@ def build_schedulers(config):
 
 def build_optimizer(config, param_groups, lr_schedule=None, wd_schedule=None, last_layer_lr_schedule=None):
     """train/train.py:75-122 builds optax.multi_transform(adamw per group) with the schedules injected as functions of
-    the step count.  The B200 optimizer is the fused clip+AdamW(+EMA) kernel inside the engine; this returns the
+    the step count.  The GPU optimizer is the fused clip+AdamW(+EMA) kernel inside the engine; this returns the
     description it is driven by (the per-tensor multipliers come from `SSLMetaArch.get_params_groups`)."""
     return {"groups": param_groups, "lr": lr_schedule, "wd": wd_schedule, "last_layer_lr": last_layer_lr_schedule,
             "b1": config.optim.adamw_beta1, "b2": config.optim.adamw_beta2, "clip_grad": config.optim.clip_grad}
@@ -154,7 +154,7 @@ def build_multi_resolution_data_loader_from_cfg(config, model, start_iter: int =
     ratios = as_list(config.crops.get("global_local_crop_pairs_ratios", 1.0))
     assert len(gs) == len(ls) == len(gram) == len(ratios)
     if len(gs) != 1:
-        raise NotImplementedError("multi-resolution crop lists: the B200 engine is built for one (global, local, gram) size "
+        raise NotImplementedError("multi-resolution crop lists: the GPU engine is built for one (global, local, gram) size "
                                   "triple; run one engine per resolution stage")
     config_i = copy.deepcopy(config)
     config_i.crops.global_crops_size, config_i.crops.local_crops_size = gs[0], ls[0]

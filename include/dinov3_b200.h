@@ -1,4 +1,4 @@
-/* dinov3_b200.h — C ABI of libdinov3_b200.so: the B200 (sm_100a) kernels behind the DINOv3 SSL training hot path.
+/* dinov3_b200.h — C ABI of libdinov3_b200.so: the H100 (sm_90a) kernels behind the DINOv3 SSL training hot path.
  *
  * The reference (Dhia-naouali/dinov3-jax) has no FFI: its hot path is Flax modules traced by jax.jit.  Each entry
  * point below therefore cites the reference *module call site* (path:line under dinov3_jax/) whose arithmetic it
@@ -10,7 +10,7 @@
  *   - return value: D3_OK (0) or a negative d3_status; d3_last_error() gives the message for the calling thread.
  *     Launch-configuration errors are reported synchronously, asynchronous faults surface at the next sync.
  *   - one process per GPU, calls come from that process' single training thread.
- *   - there is NO CPU fallback: without a Blackwell GPU d3_init() fails.
+ *   - there is NO CPU fallback: without an sm_90 (Hopper) GPU d3_init() fails.
  */
 #ifndef DINOV3_B200_H
 #define DINOV3_B200_H
@@ -22,7 +22,7 @@ typedef enum {
   D3_OK = 0,
   D3_ERR_ARG = -1,     /* bad shape / alignment / null pointer */
   D3_ERR_CUDA = -2,    /* CUDA runtime or driver error (message has the CUDA string) */
-  D3_ERR_DEVICE = -3,  /* not an sm_100 device */
+  D3_ERR_DEVICE = -3,  /* not an sm_90 device */
 } d3_status;
 
 /* ---- library ------------------------------------------------------------------------------------------------ */
@@ -35,8 +35,8 @@ int d3_set_sm_limit(int n);
 long long d3_launch_count(void);        /* kernels launched by this library since the last reset (bench: gpu_launches) */
 void d3_reset_launch_count(void);
 
-/* ---- dense contraction (tcgen05 / TMEM / TMA) ------------------------------------------------------------------
- * D[M,N] = epilogue( alpha * A[M,K] . B[K,N] ), bf16 operands, fp32 accumulation in tensor memory.
+/* ---- dense contraction (wgmma / TMA) -----------------------------------------------------------------------------
+ * D[M,N] = epilogue( alpha * A[M,K] . B[K,N] ), bf16 operands, fp32 accumulation in registers.
  *   a_major = 0: A stored [M][K] (row stride lda)      a_major = 1: A stored [K][M]
  *   b_major = 0: B stored [N][K] (row stride ldb)      b_major = 1: B stored [K][N]   (reference kernel layout [in,out])
  * Replaces nn.Dense / nn.Conv(stride=kernel) at layers/attention.py:63-65,94,101, layers/ffn_layers.py:36-47,
@@ -73,9 +73,9 @@ typedef struct {
   long long sc_off;
   int sc_shard, sc_world;
 } d3_gemm_epilogue;
-/* tile_n : 0 = auto; 64 / 128 / 256 = single-CTA kernel with that tile width; 512 = CTA-pair (cta_group::2) 256x256 kernel.
- * split_k: 0 = auto (used only for plain fp32 outputs with D3_EP_ACCUM, i.e. weight gradients: partial sums are reduced
- *          with fp32 atomics into `out`, which the caller zeroes or wants accumulated into); >= 1 = forced.            */
+/* tile_n : 0 = auto; 64 / 128 = 128-row tiles of that width; 256 and 512 (wider tiles) are taken as 128.
+ * split_k: 0 = auto (used only for plain fp32 outputs with D3_EP_ACCUM, i.e. weight gradients: the slices' partial sums
+ *          are added to `out`, which the caller zeroes or wants accumulated into, in slice order); >= 1 = forced.  */
 int d3_gemm_bf16(const void* A, int lda, int a_major, const void* B, int ldb, int b_major, int M, int N, int K,
                  const d3_gemm_epilogue* ep, int tile_n, int split_k, void* stream);
 

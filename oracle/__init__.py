@@ -13,7 +13,7 @@ PARITY STATUS: the reference ships no golden vectors, known-answer tests or nume
 its third-party stack (jax 0.7.1 / flax 0.11.2 / optax 0.2.5) is not installable in the build container, so the
 reference cannot be executed end to end here.  The oracle is pinned as far as that allows:
   * `data/masking.py`, `data/collate.py` (mask part), `train/cosine_lr_scheduler.py` are pure numpy/torch and ARE
-    imported from /root/reference by `tests/golden/make_golden.py`; the oracle's restatement is bit-exact against them;
+    imported from a reference checkout by `tests/golden/make_golden.py`; the oracle's restatement is bit-exact against them;
   * the loss / RoPE / param-group files and the whole model side — `models/vision_transformer.py`
     (DinoVisionTransformer on multi-crop input with iBOT masks) with every layer under it (patch_embed, block,
     attention, ffn_layers, layer_scale, rope) and `layers/dino_head.py` — are executed *unmodified* under a small

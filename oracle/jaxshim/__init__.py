@@ -1,6 +1,6 @@
 """A minimal numpy-backed stand-in for the parts of jax / flax.linen that the reference's *loss, RoPE,
 param-group, layer, ViT, DINOHead and SSLMetaArch* modules touch — TEST INFRASTRUCTURE, used only by tests/golden/make_golden.py in the build container
-(where /root/reference exists and the real jax/flax cannot be installed) to execute those reference files UNMODIFIED
+(where a reference checkout exists and the real jax/flax cannot be installed) to execute those reference files UNMODIFIED
 and record golden vectors.  It is not a JAX implementation: only single-device, eager, float64 numpy semantics.
 Third-party semantics restated here (SURVEY.md Appendix F): nn.softmax / nn.log_softmax are the max-subtracted
 forms; jax.lax.psum / pmean over one device are the identity; jax.lax.cond picks a branch eagerly.

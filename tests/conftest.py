@@ -10,7 +10,7 @@ for p in (os.path.join(ROOT, "dinov3-jax_b200"), ROOT):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100) GPU; run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90) GPU; run with -m gpu on a GPU machine")
 
 
 @pytest.fixture(scope="session")
@@ -24,3 +24,15 @@ def native():
 
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
+
+
+def reference_vectors():
+    """The golden vectors of tests/golden/make_golden.py as one dict (stored in parts of under 1 MB each)."""
+    import glob
+
+    import numpy as np
+    out = {}
+    for p in sorted(glob.glob(os.path.join(GOLDEN, "reference_vectors_*.npz"))):
+        with np.load(p) as z:
+            out.update({k: z[k] for k in z.files})
+    return out

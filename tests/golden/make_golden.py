@@ -1,4 +1,5 @@
-"""Regenerate tests/golden/*.npz by EXECUTING reference files from /root/reference (build container only).
+"""Regenerate tests/golden/reference_vectors_*.npz by EXECUTING reference files from a checkout of the reference
+(Dhia-naouali/dinov3-jax) named by $DINOV3_JAX_REFERENCE.
 
   * data/masking.py, train/cosine_lr_scheduler.py      — imported as they are (pure numpy / random)
   * data/collate.py mask section                       — re-executed with the reference MaskingGenerator
@@ -32,7 +33,8 @@
     indices, weights, dlpack hand-over through the shim).
   * fsdp/utils.py: `shard_params` (:19-53) called for every rank of a 2- and 3-device axis (axis_index / psum patched).
   * fsdp/ac_compile_parallelize.py: called with recording stand-ins for NamedSharding / PartitionSpec / device_put.
-Usage:  python tests/golden/make_golden.py      (writes next to this file; the .npz files are committed)
+Usage:  DINOV3_JAX_REFERENCE=<checkout> python tests/golden/make_golden.py
+        (writes next to this file, in parts of under 1 MB; the .npz files are committed)
 """
 from __future__ import annotations
 
@@ -45,7 +47,8 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = "/root/reference/dinov3_jax"
+REF_ROOT = os.path.abspath(os.environ.get("DINOV3_JAX_REFERENCE", "dinov3-jax-reference"))
+REF = os.path.join(REF_ROOT, "dinov3_jax")
 sys.path.insert(0, ROOT)
 
 
@@ -57,7 +60,7 @@ def load(name, rel):
 
 
 def main():
-    assert os.path.isdir(REF), "reference checkout not present: golden vectors can only be regenerated in the build container"
+    assert os.path.isdir(REF), "reference checkout not found: set DINOV3_JAX_REFERENCE"
     import torch
     from oracle.jaxshim import install, Arr
     install()
@@ -168,10 +171,10 @@ def main():
     from oracle.model import init_params, sub
     for k in [k for k in sys.modules if k == "dinov3_jax" or k.startswith("dinov3_jax.")]:
         del sys.modules[k]
-    sys.path.insert(0, "/root/reference")
+    sys.path.insert(0, REF_ROOT)
     vt = importlib.import_module("dinov3_jax.models.vision_transformer")
     dh = importlib.import_module("dinov3_jax.layers.dino_head")
-    assert vt.__file__.startswith("/root/reference/") and dh.__file__.startswith("/root/reference/")
+    assert vt.__file__.startswith(REF_ROOT + os.sep) and dh.__file__.startswith(REF_ROOT + os.sep)
     cfg = ModelCfg(embed_dim=128, depth=2, heads=2, global_size=64, local_size=32, n_prototypes=48, head_hidden=64,
                    head_bottleneck=32, layerscale=0.5)
     P = {k: v.double() for k, v in init_params(cfg, 3, perturb=0.05, dtype=torch.float32).items()}   # f32-representable
@@ -240,7 +243,7 @@ def main():
     trainpkg = types.ModuleType("dinov3_jax.train"); trainpkg.__path__ = [REF + "/train"]
     sys.modules["dinov3_jax.train"] = trainpkg
     arch_mod = importlib.import_module("dinov3_jax.train.ssl_meta_arch")
-    assert arch_mod.__file__.startswith("/root/reference/")
+    assert arch_mod.__file__.startswith(REF_ROOT + os.sep)
     vt.vit_test = lambda patch_size=16, **kw: vt.DinoVisionTransformer(patch_size=patch_size, embed_dim=128, n_blocks=2,
                                                                        num_heads=2, ffn_ratio=4, **kw)
 
@@ -279,7 +282,7 @@ def main():
 
     # ---- torch-hub key mapping (hubconf.py:40-70)
     import re as _re
-    src = open("/root/reference/hubconf.py").read()
+    src = open(os.path.join(REF_ROOT, "hubconf.py")).read()
     fn_src = src[src.index("def setup_checkpoint("): src.index("checkpoint = setup_checkpoint(")]
     ns = {"re": _re, "t2j": lambda x: x.detach().cpu().numpy()}
     exec(fn_src, ns)
@@ -307,7 +310,7 @@ def main():
     # ---- fsdp/utils.py shard_params (:19-53) for every rank of a 2- and a 3-device "dp" axis
     import jax as _jx
     futils = importlib.import_module("dinov3_jax.fsdp.utils")
-    assert futils.__file__.startswith("/root/reference/")
+    assert futils.__file__.startswith(REF_ROOT + os.sep)
     srng = np.random.default_rng(3)
     ptree = {"w": J(srng.standard_normal((6, 8))), "odd": J(srng.standard_normal((3, 5))), "tiny": J(srng.standard_normal(4)),
              "cube": {"k": J(srng.standard_normal((9, 6, 4))), "sq": J(srng.standard_normal((6, 6)))}}
@@ -326,7 +329,7 @@ def main():
 
     # ---- fsdp/ac_compile_parallelize.py (:20-44): which axis every leaf is placed on, for 2 and 3 devices
     acp = importlib.import_module("dinov3_jax.fsdp.ac_compile_parallelize")
-    assert acp.__file__.startswith("/root/reference/")
+    assert acp.__file__.startswith(REF_ROOT + os.sep)
 
     class _Spec:
         def __init__(self, *axes): self.axes = axes
@@ -395,8 +398,15 @@ def main():
         out[f"clip_in/{m_}"] = clip_inputs[m_]
         out[f"clip_out/{m_}"] = flat3(ns3["grads"][m_])
         out[f"clip_norm/{m_}"] = np.asarray(ns3["metrics_dict"][f"{m_}_grad_norm"], dtype=np.float64)
-    np.savez_compressed(os.path.join(HERE, "reference_vectors.npz"), **out)
-    print("wrote", os.path.join(HERE, "reference_vectors.npz"), len(out), "arrays")
+    parts, cur, size = [], {}, 0
+    for k, v in out.items():                 # parts of under 1 MB (tests/conftest.py: reference_vectors)
+        if cur and size + np.asarray(v).nbytes > 800_000:
+            parts.append(cur); cur, size = {}, 0
+        cur[k] = v; size += np.asarray(v).nbytes
+    parts.append(cur)
+    for i, p in enumerate(parts):
+        np.savez_compressed(os.path.join(HERE, f"reference_vectors_{i}.npz"), **p)
+    print("wrote", len(parts), "parts,", len(out), "arrays")
 
 
 if __name__ == "__main__":

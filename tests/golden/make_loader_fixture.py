@@ -1,8 +1,8 @@
 """Generates tests/golden/loader_batch.npz: ONE batch produced by the reference's own host data path
-(`dinov3_jax/data/augmentations.py::DataAugmentationDINO` executed from /root/reference through the package overlay,
+(`dinov3_jax/data/augmentations.py::DataAugmentationDINO` executed from a reference checkout through the package overlay,
 on the noise images of the reference's decoder, data/datasets/decoders.py:31-34) and collated by this repo's
 `collate_data_and_cast` (pinned bit-exactly against the reference function in test_golden_reference.py).
-Run here (the GPU box has no reference checkout):  python tests/golden/make_loader_fixture.py
+Usage:  DINOV3_JAX_REFERENCE=<checkout of Dhia-naouali/dinov3-jax> python tests/golden/make_loader_fixture.py
 """
 import os
 import random
@@ -13,7 +13,8 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200"))
-sys.path.append("/root/reference")          # AFTER the package: only what the overlay does not define resolves there
+REF_ROOT = os.path.abspath(os.environ.get("DINOV3_JAX_REFERENCE", "dinov3-jax-reference"))
+sys.path.append(REF_ROOT)          # AFTER the package: only what the overlay does not define resolves there
 
 from dinov3_jax.configs import DinoV3SetupArgs, setup_config  # noqa: E402
 from dinov3_jax.train.ssl_meta_arch import SSLMetaArch  # noqa: E402
@@ -30,7 +31,7 @@ def make():
     config = setup_config(DinoV3SetupArgs(opts=OPTS))
     model = SSLMetaArch(config)
     import dinov3_jax.data.augmentations as aug
-    assert aug.__file__.startswith("/root/reference/"), aug.__file__
+    assert aug.__file__.startswith(REF_ROOT + os.sep), aug.__file__
     loader = build_data_loader_from_cfg(config, model, start_iter=0)
     return next(iter(loader))
 

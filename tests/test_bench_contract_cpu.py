@@ -1,5 +1,5 @@
 """CPU: the reference arm of bench.py (`--impl reference`: the oracle port timed on host cores) prints one JSON line with
-the keys the driver reads.  (The B200 arm needs a GPU and is exercised by the driver.)"""
+the keys its consumers read.  (The GPU arm needs a GPU.)"""
 import json
 import os
 import subprocess

@@ -6,9 +6,9 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN
+from conftest import reference_vectors
 
-G = np.load(os.path.join(GOLDEN, "reference_vectors.npz"))
+G = reference_vectors()
 
 
 def _hub_state_dict(D=8, p=2):

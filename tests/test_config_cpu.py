@@ -40,7 +40,7 @@ def test_cli_surface():
 
 
 def test_storage_tokens_and_norm_layer_map_onto_the_engine_config():
-    """student.n_storage_tokens / student.norm_layer (models/vision_transformer.py:38-42,106-111) are on the B200 path;
+    """student.n_storage_tokens / student.norm_layer (models/vision_transformer.py:38-42,106-111) are on the GPU path;
     so are SwiGLU (all four alignments) and mask_k_bias (SURVEY §8f.1); RMSNorm is not and is rejected loudly."""
     cfg = setup_config(DinoV3SetupArgs(opts=["student.n_storage_tokens=4", "student.norm_layer=layernormbf16"]))
     e = config_from_reference_cfg(cfg)
@@ -69,7 +69,7 @@ def test_parameter_spec_contains_storage_tokens_with_the_reference_multipliers()
 
 def test_gram_keys_map_onto_the_engine_config():
     """gram.* (configs/ssl_default_config.yaml:55-73; train/ssl_meta_arch.py:165-254): the batch-level Gram term with the
-    EMA teacher or a frozen snapshot is on the B200 path (SURVEY 8f.2); the variants that are not raise."""
+    EMA teacher or a frozen snapshot is on the GPU path (SURVEY 8f.2); the variants that are not raise."""
     e = config_from_reference_cfg(setup_config(DinoV3SetupArgs(opts=["gram.use_loss=true", "gram.ema_teacher=true",
                                                                       "gram.loss_weight=2.0", "gram.remove_only_teacher_neg=true"])))
     assert e.gram_use_loss and e.gram_ema_teacher and e.gram_loss_weight == 2.0 and e.gram_remove_only_teacher_neg

@@ -11,46 +11,38 @@ import torch
 
 from conftest import GOLDEN, ROOT
 
-REF = "/root/reference"
-needs_ref = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "dinov3_jax")), reason="reference checkout not present")
+
+def _stub_reference(root):
+    """A stand-in reference checkout: the two data modules the overlay leaves to the reference (augmentations,
+    transforms), each recording where it was imported from."""
+    data = root / "dinov3_jax" / "data"
+    data.mkdir(parents=True)
+    for name in ("augmentations", "transforms"):
+        (data / f"{name}.py").write_text("ORIGIN = 'reference'\n")
+    return str(root)
 
 
-@needs_ref
-def test_overlay_resolves_reference_data_modules_but_hot_path_stays_here():
+def test_overlay_resolves_reference_data_modules_but_hot_path_stays_here(tmp_path):
+    ref = _stub_reference(tmp_path / "reference")
     code = ("import sys; sys.path.insert(0, %r); sys.path.append(%r)\n"
             "import dinov3_jax.data.augmentations as a, dinov3_jax.data.transforms as t\n"
             "import dinov3_jax.data.masking as m, dinov3_jax.data.collate as c, dinov3_jax.train.train as tr, dinov3_jax.loss as l\n"
             "print(a.__file__); print(t.__file__); print(m.__file__); print(c.__file__); print(tr.__file__); print(l.__file__)\n"
-            % (os.path.join(ROOT, "dinov3-jax_b200"), REF))
+            % (os.path.join(ROOT, "dinov3-jax_b200"), ref))
     out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0, out.stderr[-2000:]
     files = out.stdout.strip().splitlines()
-    assert files[0].startswith(REF) and files[1].startswith(REF)                    # stay in the reference
+    assert files[0].startswith(ref) and files[1].startswith(ref)                    # stay in the reference
     assert all(f.startswith(ROOT) for f in files[2:]), files                        # hot path + jax-free data pieces
 
 
 def test_missing_reference_loader_raises_a_helpful_import_error():
+    import importlib.util
     import dinov3_jax.data as d
-    if os.path.isdir(REF) and REF in sys.path:
-        pytest.skip("reference on sys.path")
+    if importlib.util.find_spec("dinov3_jax.data.loaders") is not None:
+        pytest.skip("a reference checkout is on sys.path")
     with pytest.raises(ImportError, match="reference"):
         d.make_data_loader  # noqa: B018
-
-
-@needs_ref
-def test_fixture_is_what_the_reference_augmentation_produces_today():
-    """Regenerates the loader batch (same seeds) in a subprocess with the reference on the path and compares it with
-    the committed fixture bit for bit."""
-    code = ("import sys, numpy as np, torch; sys.path.insert(0, %r)\n"
-            "import make_loader_fixture as f\n"
-            "b = f.make()\n"
-            "np.savez('/tmp/_loader_batch_check.npz', **{k: (v.view(torch.int16).numpy() if v.dtype == torch.bfloat16 else v.numpy()) "
-            "for k, v in b.items() if torch.is_tensor(v)})\n" % GOLDEN)
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    got, want = np.load("/tmp/_loader_batch_check.npz"), np.load(os.path.join(GOLDEN, "loader_batch.npz"))
-    for k in got.files:
-        assert np.array_equal(got[k], want[k]), k
 
 
 def test_fixture_has_the_collate_contract():

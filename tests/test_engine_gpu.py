@@ -167,12 +167,10 @@ def test_engine_loss_against_reference_meta_arch_golden(case):
     """Engine forward vs numbers produced by the reference's own SSLMetaArch.__call__ (tests/golden/make_golden.py);
     the oracle is not involved.  Loss terms 1e-3 rel would be the fp32 bar; these fixtures use large-amplitude head
     weights (peaky softmax), so the bf16-operand tolerance 5e-3 is stated here."""
-    import os
-    import numpy as np
-    from conftest import GOLDEN
+    from conftest import reference_vectors
     from dinov3_jax.engine import Engine, from_oracle_cfg
     from test_golden_reference import ssl_case
-    G = np.load(os.path.join(GOLDEN, "reference_vectors.npz"))
+    G = reference_vectors()
     cfg, P, batch, temp = ssl_case(case, dtype=torch.float32)
     B = batch["global_batch_size"]
     batch["collated_global_crops"] = batch["collated_global_crops"].to(torch.bfloat16)
@@ -525,3 +523,28 @@ def test_gram_term_gradient_alone():
     for k, g in grads.items():
         if not k.startswith("student_backbone/"):
             assert float(grads_e[k].abs().max()) == 0.0, k        # no gradient reaches the heads
+
+
+def test_training_steps_are_bit_reproducible():
+    """Two engines with the same parameters and batch run three training steps each: every gradient, parameter and
+    metric is the same bit for bit (the step's reductions add their partial sums in a fixed order)."""
+    from dinov3_jax.engine import Engine, config_for
+    from dinov3_jax.engine.synth import reference_like_params, synthetic_batch
+    cfg = dataclasses.replace(config_for("vit_small", n_prototypes=4096), depth=2)
+    params = reference_like_params(cfg, 0)
+    B = 4
+    batch = synthetic_batch(cfg, B, seed=3)
+    runs = []
+    for _ in range(2):
+        eng = Engine(cfg, B, max_masked=int(batch["mask_indices_list"].shape[0]))
+        eng.params.load_reference_tree(params)
+        for _ in range(3):
+            eng.train_step(batch, **HYPER)
+        torch.cuda.synchronize()
+        runs.append((eng.read_metrics(), {k: v.cpu() for k, v in eng.params.export_reference_tree("grad").items()},
+                     {k: v.cpu() for k, v in eng.params.export_reference_tree("param").items()}))
+        del eng
+    (m0, g0, p0), (m1, g1, p1) = runs
+    assert m0 == m1
+    assert all(torch.equal(g0[k], g1[k]) for k in g0), [k for k in g0 if not torch.equal(g0[k], g1[k])][:5]
+    assert all(torch.equal(p0[k], p1[k]) for k in p0), [k for k in p0 if not torch.equal(p0[k], p1[k])][:5]

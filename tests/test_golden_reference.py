@@ -1,7 +1,7 @@
 """Pins the oracle (and the product's host-side mirrors) against golden vectors produced by EXECUTING reference files
 (tests/golden/make_golden.py): masks / collate / schedules directly, losses / RoPE / param groups under the numpy
 stand-in for jax+flax; DinoVisionTransformer (+ every layer under it) and DINOHead under the shim's mini flax.linen.
-Nothing here reads /root/reference."""
+Nothing here reads the reference checkout."""
 import os
 import random
 
@@ -9,9 +9,9 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN
+from conftest import reference_vectors
 
-G = np.load(os.path.join(GOLDEN, "reference_vectors.npz"))
+G = reference_vectors()
 T = lambda a: torch.from_numpy(np.asarray(a))
 
 
@@ -105,7 +105,7 @@ def test_param_group_multipliers_match_reference_code(impl):
 
 
 def _golden_tree(prefix):
-    return {k[len(prefix):]: T(G[k]).double() for k in G.files if k.startswith(prefix)}
+    return {k[len(prefix):]: T(G[k]).double() for k in G if k.startswith(prefix)}
 
 
 def test_backbone_matches_reference_module_code():
@@ -175,7 +175,7 @@ def test_ssl_forward_matches_reference_meta_arch(case):
     cfg, P, batch, temp = ssl_case(case)
     loss, metrics = ssl_forward(P, batch, temp, cfg, dtype=torch.float64)
     assert abs(float(loss) - float(G[f"ssl_{case}_loss"])) < 1e-9 * abs(float(G[f"ssl_{case}_loss"]))
-    keys = [k.split("/", 1)[1] for k in G.files if k.startswith(f"ssl_{case}_metric/")]
+    keys = [k.split("/", 1)[1] for k in G if k.startswith(f"ssl_{case}_metric/")]
     assert set(keys) == {"local_batch_size", "dino_local_crops_loss", "dino_local_loss_weight", "dino_global_crops_loss",
                          "koleo_loss", "ibot_loss"}
     for k in keys:
@@ -226,7 +226,7 @@ def test_collate_data_and_cast_matches_reference_function():
     random.seed(13); np.random.seed(13)
     mg = MaskingGenerator(input_size=(4, 4), max_num_patches=0.5 * 16)
     d = collate_data_and_cast(samples, (0.1, 0.5), 0.5, torch.bfloat16, n_tokens=16, mask_generator=mg)
-    keys = {k.split("/", 1)[1] for k in G.files if k.startswith("collate/")}
+    keys = {k.split("/", 1)[1] for k in G if k.startswith("collate/")}
     assert keys == set(d.keys())
     for k in keys:
         want = G[f"collate/{k}"]
@@ -308,7 +308,7 @@ def test_swiglu_ffn_matches_reference_class():
     executed from the reference source vs the oracle's SwiGLU branch — groundwork for SURVEY §8f.1."""
     import torch.nn.functional as F
     x = T(G["swiglu_x"])
-    w = {k.split("/", 1)[1]: T(G[k]) for k in G.files if k.startswith("swiglu_param/")}
+    w = {k.split("/", 1)[1]: T(G[k]) for k in G if k.startswith("swiglu_param/")}
     assert w["w1/kernel"].shape == (32, 64)
     y = (F.silu(x @ w["w1/kernel"] + w["w1/bias"]) * (x @ w["w2/kernel"] + w["w2/bias"])) @ w["w3/kernel"] + w["w3/bias"]
     assert np.abs(y.numpy() - G["swiglu_y"]).max() < 1e-13

@@ -61,7 +61,7 @@ def test_gemm_epilogues():
 @pytest.mark.parametrize("a_mn,b_mn", [(0, 0), (0, 1), (1, 1)])
 @pytest.mark.parametrize("shape", [(1000, 512, 256), (776, 1024, 320)])
 def test_gemm_pair_kernel_tma_epilogue(a_mn, b_mn, shape):
-    """CTA-pair (cta_group::2) kernel with the TMA-store epilogue: every epilogue combination the engine uses, ragged M."""
+    """Widest-tile kernel (tile_n=512): every epilogue combination the engine uses, ragged M."""
     from dinov3_jax import ops
     M, N, K = shape
     A = torch.randn(M, K, device="cuda").to(torch.bfloat16); B = (torch.randn(K, N, device="cuda") * 0.1).to(torch.bfloat16)
@@ -93,6 +93,9 @@ def test_gemm_split_k_accumulates(M, N, K, bn, sk):
     out = torch.ones(M, N, device="cuda")
     ops.gemm(A, B, out, a_mn=True, b_mn=True, accum=True, tile_n=bn, split_k=sk)
     assert rel(out, 1 + A.float().t() @ B.float()) < 1e-5
+    again = torch.ones(M, N, device="cuda")
+    ops.gemm(A, B, again, a_mn=True, b_mn=True, accum=True, tile_n=bn, split_k=sk)
+    assert torch.equal(out, again)                   # the slices are reduced in a fixed order
 
 
 def test_gemm_rejects_bad_arguments():
@@ -545,7 +548,8 @@ def test_gram_loss_reference_golden_value():
     27 tokens x 16 channels, zero-padded here to the kernels' 8-element granularity; zero rows add nothing to the sum)."""
     import numpy as np
     import os
-    G = np.load(os.path.join(os.path.dirname(__file__), "golden", "reference_vectors.npz"))
+    from conftest import reference_vectors
+    G = reference_vectors()
     s, t = torch.from_numpy(G["gram_s"]).float().reshape(-1, 16), torch.from_numpy(G["gram_t"]).float().reshape(-1, 16)
     n = s.shape[0]
     pad = lambda x: torch.nn.functional.pad(x, (0, 64 - 16, 0, 32 - n)).contiguous().cuda()
@@ -576,7 +580,8 @@ def test_gram_loss_class_against_the_reference_fixture():
     import os
     from dinov3_jax.loss import GramLoss
     from oracle.losses import gram_loss
-    G = np.load(os.path.join(os.path.dirname(__file__), "golden", "reference_vectors.npz"))
+    from conftest import reference_vectors
+    G = reference_vectors()
     s, t = torch.from_numpy(G["gram_s"]).float().cuda(), torch.from_numpy(G["gram_t"]).float().cuda()
     gl = GramLoss()
     assert abs(float(gl(s, t, img_level=True)) - float(G["gram_img"])) < 2e-2 * float(G["gram_img"])

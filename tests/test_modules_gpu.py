@@ -138,13 +138,11 @@ def test_vit_and_head_against_reference_golden(native):
     """CUDA forward (dinov3_jax.models.DinoVisionTransformer, dinov3_jax.layers.DINOHead) against vectors produced by
     executing the reference's own module code (tests/golden/make_golden.py) — no oracle in between.  bf16-operand /
     fp32-accumulate tolerance, norm-wise."""
-    import os
-    import numpy as np
-    from conftest import GOLDEN
+    from conftest import reference_vectors
     from dinov3_jax.layers import DINOHead
     from dinov3_jax.models import DinoVisionTransformer
-    G = np.load(os.path.join(GOLDEN, "reference_vectors.npz"))
-    tree = lambda prefix: nest({k[len(prefix):]: torch.from_numpy(G[k]) for k in G.files if k.startswith(prefix)})
+    G = reference_vectors()
+    tree = lambda prefix: nest({k[len(prefix):]: torch.from_numpy(G[k]) for k in G if k.startswith(prefix)})
     model = DinoVisionTransformer(tree("vit_param/"), img_size=64, patch_size=16, embed_dim=128, n_blocks=2, num_heads=2,
                                   layerscale_init=0.5)
     og, ol = model([torch.from_numpy(G["vit_global"]), torch.from_numpy(G["vit_local"])],

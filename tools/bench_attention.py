@@ -1,6 +1,5 @@
 """Isolated timing of the attention kernels at the ViT-L/16 B=64 shapes of the headline step (CUDA events, 20 launches
-after 3 warm-ups, inputs larger than L2): python tools/bench_attention.py [fwd|bwd|all].
-D3_ATTN_WS=0 selects the round-1 single-pass kernels for an A/B comparison (separate process: the switch is read once)."""
+after 3 warm-ups, inputs larger than L2): python tools/bench_attention.py [fwd|bwd|all]."""
 import os
 import sys
 
@@ -28,7 +27,6 @@ def timeit(fn, n=20, warm=3):
     return e0.elapsed_time(e1) / n * 1e3     # us
 
 
-print(f"D3_ATTN_WS={os.environ.get('D3_ATTN_WS', '1')}")
 for name, n, N in (("global 128 crops x 197", 128, 197), ("local 512 crops x 37", 512, 37)):
     T = n * N
     qkv = torch.randn(T, 3 * D, device="cuda").to(bf)

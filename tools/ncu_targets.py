@@ -1,5 +1,5 @@
 """One launch of each HBM-bound / attention kernel at the ViT-L student-stream shape, for
-`ncu --set full --clock-control none -k regex:d3 -o gpurun_out/r01_ncu_hbm python tools/ncu_targets.py`."""
+`ncu --set full --clock-control none -k regex:d3 -o profile_out/r01_ncu_hbm python tools/ncu_targets.py`."""
 import os, sys
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "dinov3-jax_b200"))
 import torch

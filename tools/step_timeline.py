@@ -3,7 +3,7 @@
   python tools/step_timeline.py [arch] [B]                       (1 GPU)
   torchrun --nproc-per-node N tools/step_timeline.py [arch] [B]  (N ranks; rank 0 writes)
 
-Writes gpurun_out/timeline_w<world>.json: every GPU activity (kernels, memcpys, memsets) of 2 steps with stream, start,
+Writes profile_out/timeline_w<world>.json: every GPU activity (kernels, memcpys, memsets) of 2 steps with stream, start,
 duration; and prints a summary: busy time per stream, idle gaps on the compute stream, time per kernel name.
 `tools/timeline_diff.py a.json b.json` compares two of them (1 GPU vs N GPUs: where the extra milliseconds go).
 """
@@ -54,8 +54,8 @@ if rank == 0:
             for e in acts]
     # steps are delimited by the AdamW kernels of the backbone (the largest adamw launch ends a step)
     ends = [i for i, r in enumerate(rows) if "adamw_ema" in r["name"]]
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    out = os.path.join(ROOT, "gpurun_out", f"timeline_w{world}.json")
+    os.makedirs(os.path.join(ROOT, "profile_out"), exist_ok=True)
+    out = os.path.join(ROOT, "profile_out", f"timeline_w{world}.json")
     json.dump({"world": world, "arch": arch, "B": B, "nstep": NSTEP, "rows": rows}, open(out, "w"))
     t0, t1 = rows[0]["ts"], max(r["ts"] + r["dur"] for r in rows)
     print(f"== {arch} B={B} world={world}: {len(rows)} GPU activities over {(t1 - t0) / 1e3:.2f} ms = {(t1 - t0) / 1e3 / NSTEP:.2f} ms/step (under CUPTI)")
