@@ -11,13 +11,20 @@
 //
 // One kernel, 128 x {64,128} output tiles, 384 threads:
 //   warpgroup 0      TMA producer (one elected thread): A and B k-blocks of 64, tile after tile of this CTA's work
-//                    list, into the shared-memory ring of the consumer that owns the tile;
+//                    list, into one shared-memory ring;
 //   warpgroups 1, 2  consumers in ping-pong: the CTA's tiles alternate between them, so one warpgroup's epilogue
 //                    (straight from its accumulator registers) runs under the other's main loop.  A tile is two
 //                    m64nBNk16 wgmma chains (rows 0-63 / 64-127) over SWIZZLE_128B operands, K-major or MN-major through
 //                    the descriptor transpose bits.
-// Each consumer has its own ring (half of the stages) and waits on every fill of it in order: with one shared ring the
-// consumer of tile j+1 would wait on fills two barrier phases ahead, which the phase parity cannot tell apart.
+// Both consumers walk the whole ring in fill order, stepping over the other's k-blocks.  The main loops take turns: a
+// consumer starts its main loop only after the other has passed its last full-barrier wait (named barriers 1 / 2), so
+// every fill of a stage is waited on by exactly one consumer, in order, and no wait can be two phases ahead (which the
+// phase parity could not tell apart).  The main loop of one tile so has the whole ring in flight.
+//
+// The epilogue flags are a template parameter.  The flag sets one training step issues are compiled with their flags
+// fixed (dispatch() lists them): bias and gamma are staged in shared memory by cp.async during the main loop, and each
+// thread issues all loads of a row before the row's first store.  Every other call (fused reduce-scatter, misaligned
+// operands, odd N, other flag sets) runs the same kernel with the flags read at run time (EPI_RUNTIME).
 #include <cstdlib>
 #include <cstring>
 #include "ptx.cuh"
@@ -30,6 +37,16 @@ constexpr int BK = 64;
 constexpr int GEMM_THREADS = 384;
 
 // ---------------------------------------------------------------------------------------------------------------
+// gelu_tanh_grad_fast with every rounding step written out.  Its last add has a product on both sides, and which one
+// the compiler contracts into an FMA depends on the surrounding code; fixing it to fma(0.5u (1 - t^2), dz, 0.5 (1 + t))
+// makes every epilogue variant give the same bits.
+__device__ __forceinline__ float gelu_grad_epi(float u) {
+  const float u2 = __fmul_rn(u, u);
+  const float t = tanh_approx(__fmul_rn(u, fmaf(0.0356774081363001f, u2, 0.7978845608028654f)));
+  const float dz = fmaf(0.1070322244089003f, u2, 0.7978845608028654f);
+  return fmaf(__fmul_rn(__fmul_rn(0.5f, u), fmaf(-t, t, 1.0f)), dz, __fmul_rn(0.5f, __fadd_rn(1.0f, t)));
+}
+
 // epilogue for two adjacent columns (n, n+1) of one row; `vec`: both columns in range and every operand 16-byte
 // aligned with even leading dimensions (vector loads / stores of pairs)
 __device__ __forceinline__ void epilogue_pair(const GemmEpilogue& ep, size_t row, int n, int N, float v0, float v1,
@@ -66,8 +83,8 @@ __device__ __forceinline__ void epilogue_pair(const GemmEpilogue& ep, size_t row
     }
     if (ep.flags & EP_MUL_DGELU) {
       const float2 u = unpack_bf16(*reinterpret_cast<const uint32_t*>(ep.aux_in + row * ep.ld_aux + n));
-      v0 *= fast_act ? gelu_tanh_grad_fast(u.x) : gelu_tanh_grad(u.x);
-      v1 *= fast_act ? gelu_tanh_grad_fast(u.y) : gelu_tanh_grad(u.y);
+      v0 *= fast_act ? gelu_grad_epi(u.x) : gelu_tanh_grad(u.x);
+      v1 *= fast_act ? gelu_grad_epi(u.y) : gelu_tanh_grad(u.y);
     }
     if (ep.flags & EP_GAMMA) {
       const float2 g = *reinterpret_cast<const float2*>(ep.gamma + n);
@@ -100,7 +117,7 @@ __device__ __forceinline__ void epilogue_pair(const GemmEpilogue& ep, size_t row
     if (ep.flags & EP_GELU) x = fast_act ? gelu_tanh_fast(x) : gelu_tanh(x);
     if (ep.flags & EP_MUL_DGELU) {
       const float u = __bfloat162float(ep.aux_in[row * ep.ld_aux + c]);
-      x *= fast_act ? gelu_tanh_grad_fast(u) : gelu_tanh_grad(u);
+      x *= fast_act ? gelu_grad_epi(u) : gelu_tanh_grad(u);
     }
     if (ep.flags & EP_GAMMA) x *= ep.gamma[c];
     if (ep.flags & EP_RESID) x += ep.resid[row * ep.ld_resid + c];
@@ -115,14 +132,91 @@ __device__ __forceinline__ void epilogue_pair(const GemmEpilogue& ep, size_t row
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Epilogue with the flags EF fixed at compile time, for a call that passed gemm_bf16's alignment checks and has an even
+// N (a column pair is in range as a whole, and every access is a vector one).  The fp32 operations are those of
+// epilogue_pair in the same order, none contracted into an FMA, so both paths give the same bits.  A thread issues
+// every load of one row before the row's first store: it waits on memory once per row, not once per column pair.
+// `resid` may alias `out`: each element is read before it is written, by the same thread.
+constexpr int EPI_RUNTIME = -1;
+constexpr int EPI_FLAGS = EP_BIAS | EP_GELU | EP_STORE_PRE | EP_MUL_DGELU | EP_GAMMA | EP_RESID | EP_OUT_F32 | EP_ACCUM |
+                          EP_SLABS;
+
+template <int BN, int EF>
+__device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, float (&acc)[2][BN / 2], const float* s_bias,
+                                              const float* s_gamma, int m0, int n0, int M, int N, size_t slab_row0,
+                                              int r_in, int c_in) {
+  constexpr int NP = BN / 8;      // column pairs of one row held by a thread
+  float* const out_f = reinterpret_cast<float*>(ep.out);
+  __nv_bfloat16* const out_h = reinterpret_cast<__nv_bfloat16*>(ep.out);
+#pragma unroll
+  for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = m0 + mh * 64 + r_in + 8 * h;
+      if (row >= M) continue;
+      const size_t orow = slab_row0 + row;
+      float2 xr[NP], xo[NP];
+      uint32_t xu[NP];
+#pragma unroll
+      for (int i = 0; i < NP; ++i) {
+        const int n = n0 + 8 * i + c_in;
+        if (n < N) {
+          if constexpr ((EF & EP_RESID) != 0)
+            xr[i] = *reinterpret_cast<const float2*>(ep.resid + (size_t)row * ep.ld_resid + n);
+          if constexpr ((EF & EP_MUL_DGELU) != 0)
+            xu[i] = *reinterpret_cast<const uint32_t*>(ep.aux_in + (size_t)row * ep.ld_aux + n);
+          if constexpr ((EF & EP_ACCUM) != 0) xo[i] = *reinterpret_cast<const float2*>(out_f + orow * ep.ld_out + n);
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < NP; ++i) {
+        const int cl = 8 * i + c_in;          // column within the tile
+        const int n = n0 + cl;
+        if (n >= N) continue;
+        float v0 = __fmul_rn(acc[mh][4 * i + 2 * h], ep.alpha);
+        float v1 = __fmul_rn(acc[mh][4 * i + 2 * h + 1], ep.alpha);
+        if constexpr ((EF & EP_BIAS) != 0) {
+          const float2 b = *reinterpret_cast<const float2*>(s_bias + cl);
+          v0 = __fadd_rn(v0, b.x); v1 = __fadd_rn(v1, b.y);
+        }
+        if constexpr ((EF & EP_STORE_PRE) != 0)
+          *reinterpret_cast<uint32_t*>(ep.aux_out + (size_t)row * ep.ld_aux + n) = pack_bf16(v0, v1);
+        if constexpr ((EF & EP_GELU) != 0) {
+          v0 = gelu_tanh_fast(v0); v1 = gelu_tanh_fast(v1);
+        }
+        if constexpr ((EF & EP_MUL_DGELU) != 0) {
+          const float2 u = unpack_bf16(xu[i]);
+          v0 = __fmul_rn(v0, gelu_grad_epi(u.x)); v1 = __fmul_rn(v1, gelu_grad_epi(u.y));
+        }
+        if constexpr ((EF & EP_GAMMA) != 0) {
+          const float2 g = *reinterpret_cast<const float2*>(s_gamma + cl);
+          v0 = __fmul_rn(v0, g.x); v1 = __fmul_rn(v1, g.y);
+        }
+        if constexpr ((EF & EP_RESID) != 0) {
+          v0 = __fadd_rn(v0, xr[i].x); v1 = __fadd_rn(v1, xr[i].y);
+        }
+        if constexpr ((EF & EP_OUT_F32) != 0) {
+          if constexpr ((EF & EP_ACCUM) != 0) {
+            v0 = __fadd_rn(v0, xo[i].x); v1 = __fadd_rn(v1, xo[i].y);
+          }
+          *reinterpret_cast<float2*>(out_f + orow * ep.ld_out + n) = make_float2(v0, v1);
+        } else {
+          *reinterpret_cast<uint32_t*>(out_h + orow * ep.ld_out + n) = pack_bf16(v0, v1);
+        }
+      }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 template <int BN>
 struct Cfg {
-  static constexpr int STAGES = BN == 128 ? 6 : 8;   // two rings of STAGES / 2
-  static constexpr int RS = STAGES / 2;
+  static constexpr int STAGES = BN == 128 ? 6 : 8;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
+  static constexpr int BAR_BYTES = 256;                       // full and empty mbarriers
+  static constexpr int VEC_BYTES = 2 * 2 * BN * 4;            // per consumer: bias and gamma of its tile (fp32)
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + VEC_BYTES + 1024;
 };
 
 // work item = (tile, split): k-blocks [kb0, kb1)
@@ -158,15 +252,17 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint32_t sa,
   }
 }
 
-template <int BN, int A_MN, int B_MN>
+template <int BN, int A_MN, int B_MN, int EF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmEpilogue ep,
             int M, int N, int K, int splits) {
   using C = Cfg<BN>;
+  static_assert(2 * C::STAGES * 8 <= C::BAR_BYTES, "mbarriers overflow their slot");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);   // [ring * RS + stage]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + C::STAGES;
+  float* vecs = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + C::BAR_BYTES);
 
   const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
@@ -185,31 +281,28 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (wg == 0) {
     setmaxnreg_dec<40>();
     if (threadIdx.x < 32 && elect_one()) {
-      int stage[2] = {0, 0};
-      uint32_t phase[2] = {0, 0};
-      int j = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++j) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
         const WorkRange wr = work_item(w, num_n, num_k, splits, BN);
-        const int r = j & 1;                   // the ring of the consumer that owns tile j
         for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
-          const int slot = r * C::RS + stage[r];
-          mbar_wait(&empty_bar[slot], phase[r] ^ 1);
-          uint8_t* sa = smem + slot * C::STAGE_BYTES;
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * C::STAGE_BYTES;
           uint8_t* sb = sa + C::A_BYTES;
-          mbar_expect_tx(&full_bar[slot], C::STAGE_BYTES);
+          mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
           if (A_MN) {
 #pragma unroll
-            for (int i = 0; i < BM / 64; ++i) tma_load_2d(&tmA, &full_bar[slot], sa + i * 8192, wr.m0 + i * 64, kb * BK);
+            for (int i = 0; i < BM / 64; ++i) tma_load_2d(&tmA, &full_bar[stage], sa + i * 8192, wr.m0 + i * 64, kb * BK);
           } else {
-            tma_load_2d(&tmA, &full_bar[slot], sa, kb * BK, wr.m0);
+            tma_load_2d(&tmA, &full_bar[stage], sa, kb * BK, wr.m0);
           }
           if (B_MN) {
 #pragma unroll
-            for (int i = 0; i < BN / 64; ++i) tma_load_2d(&tmB, &full_bar[slot], sb + i * 8192, wr.n0 + i * 64, kb * BK);
+            for (int i = 0; i < BN / 64; ++i) tma_load_2d(&tmB, &full_bar[stage], sb + i * 8192, wr.n0 + i * 64, kb * BK);
           } else {
-            tma_load_2d(&tmB, &full_bar[slot], sb, kb * BK, wr.n0);
+            tma_load_2d(&tmB, &full_bar[stage], sb, kb * BK, wr.n0);
           }
-          if (++stage[r] == C::RS) { stage[r] = 0; phase[r] ^= 1; }
+          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
@@ -219,12 +312,29 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     const int t = threadIdx.x & 127;
     const int r_in = 16 * (t >> 5) + ((t & 31) >> 2);
     const int c_in = 2 * (t & 3);
-    const bool fast = (ep.flags & EP_SLOW) == 0;
-    int stage = 0;                             // position in this consumer's ring
+    float* const s_bias = vecs + cw * 2 * BN;
+    float* const s_gamma = s_bias + BN;
+    constexpr bool stage_vecs = EF != EPI_RUNTIME && (EF & (EP_BIAS | EP_GAMMA)) != 0;
+    int stage = 0;                             // position in the ring, counting the other consumer's k-blocks too
     uint32_t phase = 0;
-    for (int w = blockIdx.x + cw * gridDim.x; w < num_work; w += 2 * gridDim.x) {
+    int j = 0;
+    for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++j) {
       const WorkRange wr = work_item(w, num_n, num_k, splits, BN);
-      const int nkb = wr.kb1 - wr.kb0;
+      const int nkb = wr.kb1 > wr.kb0 ? wr.kb1 - wr.kb0 : 0;
+      if ((j & 1) != cw) {                     // the other consumer's tile: step over its fills
+        stage += nkb;
+        phase ^= (stage / C::STAGES) & 1;
+        stage %= C::STAGES;
+        continue;
+      }
+      if constexpr (stage_vecs) {
+        named_bar_sync(3 + cw, 128);           // this consumer's previous epilogue has read its bias / gamma
+        if (t < BN && wr.n0 + t < N) {
+          if constexpr ((EF & EP_BIAS) != 0) cp_async_4(s_bias + t, ep.bias + wr.n0 + t);
+          if constexpr ((EF & EP_GAMMA) != 0) cp_async_4(s_gamma + t, ep.gamma + wr.n0 + t);
+        }
+      }
+      if (j > 0) named_bar_sync(1 + cw, 256);  // tile j-1's main loop has passed its last full-barrier wait
       float acc[2][BN / 2];
 #pragma unroll
       for (int mh = 0; mh < 2; ++mh)
@@ -232,9 +342,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         for (int i = 0; i < BN / 2; ++i) acc[mh][i] = 0.f;
       int prev = -1;
       for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
-        const int slot = cw * C::RS + stage;
-        mbar_wait(&full_bar[slot], phase);
-        const uint32_t sa = smem_u32(smem + slot * C::STAGE_BYTES);
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
         fence_regs(acc[0]);
         fence_regs(acc[1]);
         wgmma_fence();
@@ -246,28 +355,39 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           wgmma_wait<1>();
           if (t == 0) mbar_arrive(&empty_bar[prev]);
         }
-        prev = slot;
-        if (++stage == C::RS) { stage = 0; phase ^= 1; }
+        prev = stage;
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
+      if (w + (int)gridDim.x < num_work) named_bar_arrive(1 + (cw ^ 1), 256);   // tile j+1 may start its main loop
       wgmma_wait<0>();
       fence_regs(acc[0]);
       fence_regs(acc[1]);
       if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
+      if constexpr (stage_vecs) {
+        cp_async_wait_all();
+        named_bar_sync(3 + cw, 128);           // bias / gamma of this tile are in shared memory
+      }
       if (nkb <= 0) continue;                  // empty split-K slice: nothing to add
+      const size_t slab_row0 = (EF == EPI_RUNTIME ? (ep.flags & EP_SLABS) : (EF & EP_SLABS)) ? (size_t)(w % splits) * M : 0;
+      if constexpr (EF != EPI_RUNTIME) {
+        epilogue_tile<BN, EF>(ep, acc, s_bias, s_gamma, wr.m0, wr.n0, M, N, slab_row0, r_in, c_in);
+      } else {
+        const bool fast = (ep.flags & EP_SLOW) == 0;
 #pragma unroll
-      for (int mh = 0; mh < 2; ++mh)
+        for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = wr.m0 + mh * 64 + r_in + 8 * h;
-          if (row >= M) continue;
-          const size_t orow = (ep.flags & EP_SLABS) ? (size_t)(w % splits) * M + row : (size_t)row;
+          for (int h = 0; h < 2; ++h) {
+            const int row = wr.m0 + mh * 64 + r_in + 8 * h;
+            if (row >= M) continue;
+            const size_t orow = slab_row0 + row;
 #pragma unroll
-          for (int i = 0; i < BN / 8; ++i) {
-            const int n = wr.n0 + 8 * i + c_in;
-            if (n >= N) break;
-            epilogue_pair(ep, orow, n, N, acc[mh][4 * i + 2 * h], acc[mh][4 * i + 2 * h + 1], fast && n + 1 < N);
+            for (int i = 0; i < BN / 8; ++i) {
+              const int n = wr.n0 + 8 * i + c_in;
+              if (n >= N) break;
+              epilogue_pair(ep, orow, n, N, acc[mh][4 * i + 2 * h], acc[mh][4 * i + 2 * h + 1], fast && n + 1 < N);
+            }
           }
-        }
+      }
     }
   }
 }
@@ -287,11 +407,11 @@ static int make_operand_map(CUtensorMap* map, const void* ptr, int mn, int k, in
   return encode_tensor_map_2d_bf16(map, ptr, dims, strides, box, estr);
 }
 
-template <int BN, int A_MN, int B_MN>
+template <int BN, int A_MN, int B_MN, int EF>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M, int N, int K,
                   int splits, cudaStream_t stream) {
   using C = Cfg<BN>;
-  auto kern = gemm_kernel<BN, A_MN, B_MN>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EF>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
@@ -310,10 +430,34 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilog
 template <int BN>
 static int dispatch(int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M,
                     int N, int K, int splits, cudaStream_t s) {
-  if (!a_mn && !b_mn) return launch<BN, 0, 0>(ta, tb, ep, M, N, K, splits, s);
-  if (!a_mn && b_mn) return launch<BN, 0, 1>(ta, tb, ep, M, N, K, splits, s);
-  if (a_mn && !b_mn) return launch<BN, 1, 0>(ta, tb, ep, M, N, K, splits, s);
-  return launch<BN, 1, 1>(ta, tb, ep, M, N, K, splits, s);
+  // (A layout, B layout, flags) of the calls in one training step, compiled with their epilogue fixed
+  if (!(ep.flags & (EP_SLOW | EP_SCATTER)) && N % 2 == 0) {
+    const int f = ep.flags & EPI_FLAGS;
+#define D3_EPI(A, B, F) \
+    if (a_mn == A && b_mn == B && f == (F)) return launch<BN, A, B, (F)>(ta, tb, ep, M, N, K, splits, s);
+    // forward: qkv, patch embedding and head layers, fc1, proj, fc2, prototype logits
+    D3_EPI(0, 1, EP_BIAS)
+    D3_EPI(0, 1, EP_BIAS | EP_OUT_F32)
+    D3_EPI(0, 1, EP_BIAS | EP_GELU)
+    D3_EPI(0, 1, EP_BIAS | EP_GELU | EP_STORE_PRE)
+    D3_EPI(0, 1, EP_BIAS | EP_GAMMA | EP_RESID | EP_OUT_F32)
+    D3_EPI(0, 1, EP_BIAS | EP_STORE_PRE | EP_GAMMA | EP_RESID | EP_OUT_F32)
+    D3_EPI(0, 1, EP_BIAS | EP_GELU | EP_GAMMA | EP_RESID | EP_OUT_F32)
+    D3_EPI(0, 1, EP_BIAS | EP_GELU | EP_STORE_PRE | EP_GAMMA | EP_RESID | EP_OUT_F32)
+    D3_EPI(0, 1, EP_OUT_F32)
+    // input gradients
+    D3_EPI(0, 0, 0)
+    D3_EPI(0, 0, EP_MUL_DGELU)
+    D3_EPI(0, 0, EP_OUT_F32)
+    // weight gradients: split-K slabs, or accumulated in place
+    D3_EPI(1, 1, EP_OUT_F32 | EP_SLABS)
+    D3_EPI(1, 1, EP_OUT_F32 | EP_ACCUM)
+#undef D3_EPI
+  }
+  if (!a_mn && !b_mn) return launch<BN, 0, 0, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
+  if (!a_mn && b_mn) return launch<BN, 0, 1, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
+  if (a_mn && !b_mn) return launch<BN, 1, 0, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
+  return launch<BN, 1, 1, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
 }
 
 // tile_n: 0 = auto; 64/128 force that tile width; 256 and 512 (wider tiles) are taken as 128.
