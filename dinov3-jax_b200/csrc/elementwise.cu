@@ -174,141 +174,6 @@ layernorm_fwd_reg_kernel(const float* __restrict__ x, const float* __restrict__ 
   }
 }
 
-// backward: dx = rstd * (g*scale - mean_D(g*scale) - xhat * mean_D(g*scale*xhat));   dx_out = dx (+ dx_add)
-// One warp per row (row pass); parameter gradients come from a second, column-major pass (coalesced, no atomics in
-// the inner loop): dscale[D] += sum_rows g*xhat ; dbias[D] += sum_rows g.
-template <typename InT>
-__global__ void layernorm_bwd_kernel(const InT* __restrict__ dy, const float* __restrict__ x,
-                                     const float* __restrict__ mean, const float* __restrict__ rstd,
-                                     const float* __restrict__ scale, const float* __restrict__ dx_add,
-                                     float* __restrict__ dx, int T, int D) {
-  const int warps = blockDim.x >> 5;
-  const int lane = threadIdx.x & 31;
-  for (long row = (long)blockIdx.x * warps + (threadIdx.x >> 5); row < T; row += (long)gridDim.x * warps) {
-    const float mu = mean[row], rs = rstd[row];
-    const float* xr = x + row * (long)D;
-    const InT* gr = dy + row * (long)D;
-    float a = 0.f, b = 0.f;
-    for (int e = lane; e < D; e += 32) {
-      float g;
-      if constexpr (sizeof(InT) == 2) g = __bfloat162float(gr[e]); else g = gr[e];
-      const float xh = (xr[e] - mu) * rs;
-      const float gs = g * scale[e];
-      a += gs;
-      b += gs * xh;
-    }
-    a = warp_sum(a) / D;
-    b = warp_sum(b) / D;
-    for (int e = lane; e < D; e += 32) {
-      float g;
-      if constexpr (sizeof(InT) == 2) g = __bfloat162float(gr[e]); else g = gr[e];
-      const float xh = (xr[e] - mu) * rs;
-      float v = rs * (g * scale[e] - a - xh * b);
-      if (dx_add) v += dx_add[row * (long)D + e];
-      dx[row * (long)D + e] = v;
-    }
-  }
-}
-template <typename InT>
-__global__ void layernorm_param_grad_kernel(const InT* __restrict__ dy, const float* __restrict__ x,
-                                            const float* __restrict__ mean, const float* __restrict__ rstd,
-                                            float* __restrict__ dscale, float* __restrict__ dbias, int T, int D) {
-  const int col = blockIdx.x * blockDim.x + threadIdx.x;
-  const long slab = ((long)T + gridDim.y - 1) / gridDim.y;
-  const long r0 = blockIdx.y * slab, r1 = min((long)T, r0 + slab);
-  if (col >= D) return;
-  float as = 0.f, ab = 0.f;
-  for (long r = r0; r < r1; ++r) {
-    float g;
-    if constexpr (sizeof(InT) == 2) g = __bfloat162float(dy[r * D + col]); else g = dy[r * D + col];
-    as += g * (x[r * D + col] - mean[r]) * rstd[r];
-    ab += g;
-  }
-  atomicAdd(&dscale[col], as);
-  atomicAdd(&dbias[col], ab);
-}
-
-// Fused row + parameter-gradient backward for D = 128 * VPL: each lane keeps its 4*VPL columns of x / dy in registers
-// between the two row passes (one HBM read each), accumulates dscale / dbias partials in registers over all rows of
-// the warp, reduces them across the CTA's warps in shared memory and issues one global atomic per column per CTA.
-template <int VPL, typename InT>
-__global__ void __launch_bounds__(256)
-layernorm_bwd_fused_kernel(const InT* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ mean,
-                           const float* __restrict__ rstd, const float* __restrict__ scale,
-                           const float* __restrict__ dx_add, float* __restrict__ dx, float* __restrict__ dscale,
-                           float* __restrict__ dbias, int T) {
-  constexpr int D = VPL * 128;
-  __shared__ float part[2 * D];
-  for (int e = threadIdx.x; e < 2 * D; e += blockDim.x) part[e] = 0.f;
-  __syncthreads();
-  const int warps = blockDim.x >> 5, lane = threadIdx.x & 31;
-  float ads[VPL][4], adb[VPL][4];
-#pragma unroll
-  for (int k = 0; k < VPL; ++k)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) { ads[k][j] = 0.f; adb[k][j] = 0.f; }
-  for (long row = (long)blockIdx.x * warps + (threadIdx.x >> 5); row < T; row += (long)gridDim.x * warps) {
-    const float mu = mean[row], rs = rstd[row];
-    float xh[VPL][4], gs[VPL][4];
-    float a = 0.f, b = 0.f;
-#pragma unroll
-    for (int k = 0; k < VPL; ++k) {
-      const int e = (k * 32 + lane) * 4;
-      const float4 xv = *reinterpret_cast<const float4*>(x + row * (long)D + e);
-      float g[4];
-      if constexpr (sizeof(InT) == 2) {
-        const uint2 u = *reinterpret_cast<const uint2*>(dy + row * (long)D + e);
-        const float2 g0 = unpack_bf16(u.x), g1 = unpack_bf16(u.y);
-        g[0] = g0.x; g[1] = g0.y; g[2] = g1.x; g[3] = g1.y;
-      } else {
-        const float4 gv = *reinterpret_cast<const float4*>(dy + row * (long)D + e);
-        g[0] = gv.x; g[1] = gv.y; g[2] = gv.z; g[3] = gv.w;
-      }
-      const float4 sc = *reinterpret_cast<const float4*>(scale + e);
-      const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, scs[4] = {sc.x, sc.y, sc.z, sc.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        xh[k][j] = (xs[j] - mu) * rs;
-        gs[k][j] = g[j] * scs[j];
-        a += gs[k][j];
-        b += gs[k][j] * xh[k][j];
-        ads[k][j] += g[j] * xh[k][j];
-        adb[k][j] += g[j];
-      }
-    }
-    a = warp_sum(a) * (1.f / D);
-    b = warp_sum(b) * (1.f / D);
-#pragma unroll
-    for (int k = 0; k < VPL; ++k) {
-      const int e = (k * 32 + lane) * 4;
-      float o[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) o[j] = rs * (gs[k][j] - a - xh[k][j] * b);
-      if (dx_add) {
-        const float4 r4 = *reinterpret_cast<const float4*>(dx_add + row * (long)D + e);
-        o[0] += r4.x; o[1] += r4.y; o[2] += r4.z; o[3] += r4.w;
-      }
-      *reinterpret_cast<float4*>(dx + row * (long)D + e) = make_float4(o[0], o[1], o[2], o[3]);
-    }
-  }
-  if (dscale) {
-#pragma unroll
-    for (int k = 0; k < VPL; ++k)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int e = (k * 32 + lane) * 4 + j;
-        atomicAdd(&part[e], ads[k][j]);
-        atomicAdd(&part[D + e], adb[k][j]);
-      }
-    __syncthreads();
-    for (int e = threadIdx.x; e < D; e += blockDim.x) {
-      atomicAdd(&dscale[e], part[e]);
-      atomicAdd(&dbias[e], part[D + e]);
-    }
-  }
-}
-
-
 // LayerNorm backward fused with the LayerScale/GELU backward of the branch that *feeds on* its result.
 // The row gradient dx (fp32 residual-stream gradient) produced here is exactly the dX the next branch upstream
 // needs (block.py:198-199: x_out = x_in + gamma * act(u)), so the same pass also writes
@@ -1060,20 +925,6 @@ __global__ void allreduce_peers_kernel(PeerCPtrs peers, int world, float* __rest
 using namespace d3;
 #define STREAM(s) reinterpret_cast<cudaStream_t>(s)
 
-template <int VPL>
-static void launch_ln_bwd_fused(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
-                                const float* scale, const float* dx_add, float* dx, float* dscale, float* dbias, int T,
-                                cudaStream_t st) {
-  const int blocks = min((T + 7) / 8, sm_count() * 2);
-  if (dy_is_f32)
-    layernorm_bwd_fused_kernel<VPL, float><<<blocks, 256, 0, st>>>((const float*)dy, x, mean, rstd, scale, dx_add, dx,
-                                                                  dscale, dbias, T);
-  else
-    layernorm_bwd_fused_kernel<VPL, __nv_bfloat16><<<blocks, 256, 0, st>>>((const __nv_bfloat16*)dy, x, mean, rstd, scale,
-                                                                          dx_add, dx, dscale, dbias, T);
-}
-
-
 // adds the CTAs' [dscale | dbias | ls_dgamma | ls_dbias] slabs of the LayerNorm backward kernels to the destinations
 // (nullptr: skipped; a quantity a kernel did not compute adds zeros) and releases the workspace
 static int combine_ln_slabs(float* ws, int slabs, int D, float* dscale, float* dbias, float* ls_dgamma, float* ls_dbias,
@@ -1224,37 +1075,6 @@ int d3_layernorm_fwd(const float* x, const float* scale, const float* bias, void
   return D3_OK;
 }
 
-int d3_layernorm_bwd(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
-                     const float* scale, const float* dx_add, float* dx, float* dscale, float* dbias, int T, int D,
-                     void* stream) {
-  if (T <= 0) return D3_OK;
-  cudaStream_t st = STREAM(stream);
-  const bool vec_ok = (D % 128 == 0) && (((uintptr_t)dy | (uintptr_t)x | (uintptr_t)dx | (uintptr_t)scale | (uintptr_t)dx_add) % 16 == 0);
-  if (vec_ok && (D == 128 || D == 256 || D == 384 || D == 768 || D == 1024)) {
-    switch (D / 128) {
-      case 1: launch_ln_bwd_fused<1>(dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, st); break;
-      case 2: launch_ln_bwd_fused<2>(dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, st); break;
-      case 3: launch_ln_bwd_fused<3>(dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, st); break;
-      case 6: launch_ln_bwd_fused<6>(dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, st); break;
-      default: launch_ln_bwd_fused<8>(dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, st); break;
-    }
-    D3_CHECK_LAUNCH();
-    return D3_OK;
-  }
-  int blocks = min((T + 7) / 8, sm_count() * 8);
-  dim3 pgrid((D + 127) / 128, min(128, max(1, T / 64)));
-  if (dy_is_f32) {
-    layernorm_bwd_kernel<float><<<blocks, 256, 0, st>>>((const float*)dy, x, mean, rstd, scale, dx_add, dx, T, D);
-    if (dscale) layernorm_param_grad_kernel<float><<<pgrid, 128, 0, st>>>((const float*)dy, x, mean, rstd, dscale, dbias, T, D);
-  } else {
-    layernorm_bwd_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>((const __nv_bfloat16*)dy, x, mean, rstd, scale, dx_add, dx, T, D);
-    if (dscale) layernorm_param_grad_kernel<__nv_bfloat16><<<pgrid, 128, 0, st>>>((const __nv_bfloat16*)dy, x, mean, rstd, dscale, dbias, T, D);
-  }
-  D3_CHECK_LAUNCH();
-  if (dscale) count_launch();
-  return D3_OK;
-}
-
 int d3_layernorm_bwd_ls(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
                         const float* scale, const float* dx_add, float* dx, float* dscale, float* dbias, int T, int D,
                         const float* ls_gamma, const void* ls_u, int ls_gelu, void* ls_du, float* ls_dgamma,
@@ -1266,8 +1086,7 @@ int d3_layernorm_bwd_ls(const void* dy, int dy_is_f32, const float* x, const flo
        (uintptr_t)ls_u | (uintptr_t)ls_du) % 8 != 0 || ((uintptr_t)x | (uintptr_t)dx | (uintptr_t)dx_add) % 16 != 0)
     return set_error(D3_ERR_ARG, "d3_layernorm_bwd_ls: misaligned buffer");
   cudaStream_t st = STREAM(stream);
-  const bool ring_ok = (((uintptr_t)dy | (uintptr_t)x | (uintptr_t)dx | (uintptr_t)dx_add | (uintptr_t)ls_u | (uintptr_t)ls_du) % 16 == 0) &&
-                       !getenv("D3_LN_NO_RING");
+  const bool ring_ok = ((uintptr_t)dy | (uintptr_t)x | (uintptr_t)dx | (uintptr_t)dx_add | (uintptr_t)ls_u | (uintptr_t)ls_du) % 16 == 0;
 #define LN_RING_ARGS dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, ls_gamma, ls_u, ls_gelu, ls_du, ls_dgamma, ls_dbias, st
   if (ring_ok && D % 128 == 0 && D / 128 <= 8) {
     int rc = 1;

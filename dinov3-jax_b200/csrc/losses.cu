@@ -92,18 +92,6 @@ __global__ void colmax_vec_kernel(const float* __restrict__ L, float* __restrict
   atomic_max_float(&cm[k], m.x); atomic_max_float(&cm[k + 1], m.y);
   atomic_max_float(&cm[k + 2], m.z); atomic_max_float(&cm[k + 3], m.w);
 }
-// s[k] += sum_b E[b,k] * a[b]      (a == nullptr -> a = 1)
-__global__ void sk_colsum_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
-                                 const float* __restrict__ a, float* __restrict__ s, int R, int K) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  const int slab = (R + gridDim.y - 1) / gridDim.y;
-  const int r0 = blockIdx.y * slab, r1 = min(R, r0 + slab);
-  if (k >= K) return;
-  const float m = mx[k];
-  float acc = 0.f;
-  for (int b = r0; b < r1; ++b) acc += __expf((L[(long)b * K + k] - m) * inv_temp) * (a ? a[b] : 1.f);
-  atomicAdd(&s[k], acc);
-}
 // a[b] = 1 / (Btot * sum_k E[b,k] * r[k]),  r[k] = 1/(K*s[k])
 __global__ void sk_rowsum_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
                                  const float* __restrict__ s, const float* __restrict__ btot, float* __restrict__ a,
@@ -134,14 +122,15 @@ __global__ void sk_probs_kernel(const float* __restrict__ L, const float* __rest
 //   center <- m*center + (1-m)*mean_rows(L)  (mean all-reduced over ranks), probs = softmax((L - center)/temp).
 // With s[k] = exp((center[k]-cmax)/temp)/K the existing row-sum kernel yields a[b] such that
 // Btot*E*a[b]/(K*s[k]) = softmax((L-center)/temp): the cross-entropy kernel is shared with the Sinkhorn path.
-__global__ void colsum_f32_kernel(const float* __restrict__ L, float* __restrict__ out, int R, int K) {
+// ws[slab][k] = sum over the row slab of L[b, k]   (the slabs are added in order by slab_combine)
+__global__ void colsum_f32_kernel(const float* __restrict__ L, float* __restrict__ ws, int R, int K) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   const int slab = (R + gridDim.y - 1) / gridDim.y;
   const int r0 = blockIdx.y * slab, r1 = min(R, r0 + slab);
   if (k >= K) return;
   float acc = 0.f;
   for (int b = r0; b < r1; ++b) acc += L[(long)b * K + k];
-  atomicAdd(&out[k], acc);
+  ws[(long)blockIdx.y * K + k] = acc;
 }
 __global__ void center_update_kernel(float* __restrict__ center, const float* __restrict__ colsum,
                                      const float* __restrict__ total_rows, float momentum, float inv_temp,
@@ -221,57 +210,38 @@ __global__ void absmax_vec_kernel(const float4* __restrict__ L, long n4, float* 
   m = block_max(m, sh);
   if (threadIdx.x == 0) atomic_max_float(out, m);
 }
-__global__ void sk_colsum_vec_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
-                                     const float* __restrict__ a, float* __restrict__ s, int R, int K) {
-  const int k = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-  const int slab = (R + gridDim.y - 1) / gridDim.y;
-  const int r0 = blockIdx.y * slab, r1 = min(R, r0 + slab);
-  if (k >= K) return;
-  const float c = inv_temp * 1.4426950408889634f;
-  const float4 m4 = *reinterpret_cast<const float4*>(mx + k);
-  const float4 mc = make_float4(m4.x * c, m4.y * c, m4.z * c, m4.w * c);
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 4
-  for (int b = r0; b < r1; ++b) {
-    const float4 v = *reinterpret_cast<const float4*>(L + (long)b * K + k);
-    const float w = a ? a[b] : 1.f;
-    acc.x += exp2f(v.x * c - mc.x) * w; acc.y += exp2f(v.y * c - mc.y) * w;
-    acc.z += exp2f(v.z * c - mc.z) * w; acc.w += exp2f(v.w * c - mc.w) * w;
-  }
-  atomicAdd(&s[k], acc.x); atomicAdd(&s[k + 1], acc.y); atomicAdd(&s[k + 2], acc.z); atomicAdd(&s[k + 3], acc.w);
-}
-// Deterministic column sums: every row slab writes its partial sums to part[slab][K] (no atomics), a second kernel adds
-// the slabs in a fixed order.  The atomic version perturbs s[k] in the last bit from run to run, which flips a few bf16
-// roundings of the iBOT d(logits) and grows to ~3e-3 in the embedding gradients through the bf16 backward chain
-// (tools/check_determinism.py); with this the whole dX chain of a step is bit-reproducible.
+// Sinkhorn column sums, part[slab][k] = sum over the row slab of E[b,k] * a[b]  (a == nullptr -> a = 1); slab_combine
+// then adds the slabs in a fixed order.  Float atomics here would perturb s[k] in the last bit from run to run, which
+// flips a few bf16 roundings of the iBOT d(logits) and grows to ~3e-3 in the embedding gradients through the bf16
+// backward chain (tools/check_determinism.py); with the slabs the whole dX chain of a step is bit-reproducible.
+// VEC: four columns per thread with 128-bit loads (K % 4 == 0, 16-byte aligned L and mx); otherwise one column.
+template <bool VEC>
 __global__ void sk_colsum_part_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
                                       const float* __restrict__ a, float* __restrict__ part, int R, int K) {
-  const int k = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  const int k = (blockIdx.x * blockDim.x + threadIdx.x) * (VEC ? 4 : 1);
   const int slab = (R + gridDim.y - 1) / gridDim.y;
   const int r0 = blockIdx.y * slab, r1 = min(R, r0 + slab);
   if (k >= K) return;
   const float c = inv_temp * 1.4426950408889634f;
-  const float4 m4 = *reinterpret_cast<const float4*>(mx + k);
-  const float4 mc = make_float4(m4.x * c, m4.y * c, m4.z * c, m4.w * c);
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  if constexpr (VEC) {
+    const float4 m4 = *reinterpret_cast<const float4*>(mx + k);
+    const float4 mc = make_float4(m4.x * c, m4.y * c, m4.z * c, m4.w * c);
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 4
-  for (int b = r0; b < r1; ++b) {
-    const float4 v = *reinterpret_cast<const float4*>(L + (long)b * K + k);
-    const float w = a ? a[b] : 1.f;
-    acc.x += exp2f(v.x * c - mc.x) * w; acc.y += exp2f(v.y * c - mc.y) * w;
-    acc.z += exp2f(v.z * c - mc.z) * w; acc.w += exp2f(v.w * c - mc.w) * w;
+    for (int b = r0; b < r1; ++b) {
+      const float4 v = *reinterpret_cast<const float4*>(L + (long)b * K + k);
+      const float w = a ? a[b] : 1.f;
+      acc.x += exp2f(v.x * c - mc.x) * w; acc.y += exp2f(v.y * c - mc.y) * w;
+      acc.z += exp2f(v.z * c - mc.z) * w; acc.w += exp2f(v.w * c - mc.w) * w;
+    }
+    *reinterpret_cast<float4*>(part + (long)blockIdx.y * K + k) = acc;
+  } else {
+    const float mc = mx[k] * c;
+    float acc = 0.f;
+#pragma unroll 4
+    for (int b = r0; b < r1; ++b) acc += exp2f(L[(long)b * K + k] * c - mc) * (a ? a[b] : 1.f);
+    part[(long)blockIdx.y * K + k] = acc;
   }
-  *reinterpret_cast<float4*>(part + (long)blockIdx.y * K + k) = acc;
-}
-__global__ void sk_colsum_combine_kernel(const float* __restrict__ part, float* __restrict__ s, int slabs, int K) {
-  const int k = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-  if (k >= K) return;
-  float4 acc = *reinterpret_cast<const float4*>(s + k);
-  for (int i = 0; i < slabs; ++i) {
-    const float4 v = *reinterpret_cast<const float4*>(part + (long)i * K + k);
-    acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-  }
-  *reinterpret_cast<float4*>(s + k) = acc;
 }
 __global__ void sk_rowsum_vec_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
                                      const float* __restrict__ s, const float* __restrict__ btot, float* __restrict__ a,
@@ -451,12 +421,13 @@ __global__ void koleo_bwd_kernel(const float* __restrict__ x, const float* __res
 //   mode 1 (remove_neg):              s' = max(s, 0), t' = max(t, 0),            ds'/ds = [s > 0]
 //   mode 2 (remove_only_teacher_neg): s' = (s < 0 && t < 0) ? 0 : s, t' = max(t, 0), ds'/ds = !(s < 0 && t < 0)
 //   mode 0:                           s' = s, t' = t
-// loss += inv_count * sum (s' - t')^2 ;  G = (s' - t') * ds'/ds  (bf16: the A operand of dX = (4 w / n^2) G Xs).
+// ws[CTA] = inv_count * sum over the CTA's elements of (s' - t')^2 (added to loss in CTA order by slab_combine);
+// G = (s' - t') * ds'/ds  (bf16: the A operand of dX = (4 w / n^2) G Xs).
 // block > 0 (gram.img_level: true, gram_loss.py:24-26): only the diagonal blocks of `block` x `block` tokens (one image each)
 // count; everything else contributes nothing and gets G = 0 (the full similarity GEMM is kept: one launch, 128x the
 // needed FLOPs at 196 tokens per image, still ~1 ms on the tensor cores).
 __global__ void gram_diff_kernel(const float* __restrict__ Ss, const float* __restrict__ St, __nv_bfloat16* __restrict__ G,
-                                 long n4, int mode, float inv_count, float* __restrict__ loss, int n, int block) {
+                                 long n4, int mode, float inv_count, float* __restrict__ ws, int n, int block) {
   __shared__ float sh[32];
   float acc = 0.f;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
@@ -487,7 +458,7 @@ __global__ void gram_diff_kernel(const float* __restrict__ Ss, const float* __re
     float t = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.f;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if (threadIdx.x == 0 && loss) atomicAdd(loss, t * inv_count);
+    if (threadIdx.x == 0 && ws) ws[blockIdx.x] = t * inv_count;
   }
 }
 
@@ -521,35 +492,23 @@ int d3_colmax(const float* L, float* cm /* [K] pre-set to -inf */, int R, int K,
   D3_CHECK_LAUNCH();
   return D3_OK;
 }
-int d3_sinkhorn_colsum(const float* L, const float* mx, float temp, const float* a, float* s /* zeroed */, int R, int K,
-                       void* stream) {
+int d3_sinkhorn_colsum(const float* L, const float* mx, float temp, const float* a, float* s /* zeroed, += */, int R,
+                       int K, void* stream) {
   if (R <= 0) return D3_OK;
-  if (K % 4 == 0 && ((uintptr_t)L | (uintptr_t)mx) % 16 == 0) {
-    // (K/4)/128 column CTAs x row slabs: aim at ~8 CTAs per SM
-    const int cx = (K / 4 + 127) / 128;
-    dim3 grid(cx, max(1, min(R / 8, max(1, sm_count() * 8 / cx))));
-    sk_colsum_vec_kernel<<<grid, 128, 0, STREAM(stream)>>>(L, mx, 1.f / temp, a, s, R, K);
-  } else {
-    dim3 grid((K + 255) / 256, max(1, min(R / 8, 64)));
-    sk_colsum_kernel<<<grid, 256, 0, STREAM(stream)>>>(L, mx, 1.f / temp, a, s, R, K);
-  }
-  D3_CHECK_LAUNCH();
-  return D3_OK;
-}
-int d3_sinkhorn_colsum_det(const float* L, const float* mx, float temp, const float* a, float* s /* zeroed, += */,
-                           float* scratch /* [D3_SK_SLABS, K] */, int R, int K, void* stream) {
-  if (R <= 0) return D3_OK;
-  if (K % 4 || (((uintptr_t)L | (uintptr_t)mx | (uintptr_t)s | (uintptr_t)scratch) % 16))
-    return set_error(D3_ERR_ARG, "d3_sinkhorn_colsum_det: K % 4 == 0 and 16-byte aligned buffers");
-  const int cx = (K / 4 + 127) / 128;
-  int slabs = max(1, min(R / 8, max(1, sm_count() * 8 / cx)));
-  if (slabs > D3_SK_SLABS) slabs = D3_SK_SLABS;
-  dim3 grid(cx, slabs);
-  sk_colsum_part_kernel<<<grid, 128, 0, STREAM(stream)>>>(L, mx, 1.f / temp, a, scratch, R, K);
-  sk_colsum_combine_kernel<<<cx, 128, 0, STREAM(stream)>>>(scratch, s, slabs, K);
-  D3_CHECK_LAUNCH();
-  count_launch(1);
-  return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  const bool vec = K % 4 == 0 && ((uintptr_t)L | (uintptr_t)mx) % 16 == 0;
+  // column CTAs of 128 threads x row slabs: aim at ~8 CTAs per SM, at most 16 slabs
+  const int cx = ((vec ? K / 4 : K) + 127) / 128;
+  const dim3 grid(cx, min(16, max(1, min(R / 8, max(1, sm_count() * 8 / cx)))));
+  float* ws = slab_workspace((size_t)grid.y * K, st);
+  if (!ws) return D3_ERR_CUDA;
+  if (vec) sk_colsum_part_kernel<true><<<grid, 128, 0, st>>>(L, mx, 1.f / temp, a, ws, R, K);
+  else sk_colsum_part_kernel<false><<<grid, 128, 0, st>>>(L, mx, 1.f / temp, a, ws, R, K);
+  cudaError_t e = cudaPeekAtLastError();
+  int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  if (!rc) { count_launch(); rc = slab_combine(ws, grid.y, K, 1, K, s, K, st); }
+  slab_release(ws, st);
+  return rc;
 }
 int d3_sinkhorn_rowsum(const float* L, const float* mx, float temp, const float* s, const float* btot, float* a, int R,
                        int K, void* stream) {
@@ -572,10 +531,16 @@ int d3_sinkhorn_probs(const float* L, const float* mx, float temp, const float* 
 }
 int d3_colsum_f32(const float* L, float* out /*[K] zeroed, +=*/, int R, int K, void* stream) {
   if (R <= 0) return D3_OK;
-  dim3 grid((K + 255) / 256, max(1, min(R / 8, 64)));
-  colsum_f32_kernel<<<grid, 256, 0, STREAM(stream)>>>(L, out, R, K);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  const dim3 grid((K + 255) / 256, max(1, min(R / 8, 64)));
+  float* ws = slab_workspace((size_t)grid.y * K, st);
+  if (!ws) return D3_ERR_CUDA;
+  colsum_f32_kernel<<<grid, 256, 0, st>>>(L, ws, R, K);
+  cudaError_t e = cudaPeekAtLastError();
+  int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  if (!rc) { count_launch(); rc = slab_combine(ws, grid.y, K, 1, K, out, K, st); }
+  slab_release(ws, st);
+  return rc;
 }
 int d3_center_update(float* center, const float* colsum, const float* total_rows, float momentum, float temp,
                      float* s_out, int K, void* stream) {
@@ -669,9 +634,15 @@ int d3_gram_diff(const float* Ss, const float* St, void* G_bf16, long long n_ele
   const int blocks = (int)std::min<long>((n4 + 255) / 256, (long)sm_count() * 8);
   if (block > 0 && (n <= 0 || (n % 4) || (long long)n * n != n_elems || (n % block)))
     return set_error(D3_ERR_ARG, "d3_gram_diff: block-diagonal form needs n % 4 == 0, n % block == 0 and n_elems == n * n");
-  gram_diff_kernel<<<blocks, 256, 0, STREAM(stream)>>>(Ss, St, (__nv_bfloat16*)G_bf16, n4, mode, inv_count, loss, n, block);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  cudaStream_t st = STREAM(stream);
+  float* ws = nullptr;
+  if (loss && !(ws = slab_workspace(blocks, st))) return D3_ERR_CUDA;
+  gram_diff_kernel<<<blocks, 256, 0, st>>>(Ss, St, (__nv_bfloat16*)G_bf16, n4, mode, inv_count, ws, n, block);
+  cudaError_t e = cudaPeekAtLastError();
+  int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  if (!rc) { count_launch(); rc = slab_combine(ws, blocks, 1, 1, 1, loss, 1, st); }
+  slab_release(ws, st);
+  return rc;
 }
 
 int d3_koleo_fwd_bwd(const float* x, float* xn_scratch, float* nrm_scratch, int* nn_scratch, float* coef_scratch,

@@ -48,7 +48,6 @@ SIGNATURES = {
     "d3_assemble_tokens": [P, P, P, P, P, P, I, I, I, I, P],
     "d3_assemble_tokens_bwd": [P, P, P, P, P, P, I, I, I, I, P],
     "d3_layernorm_fwd": [P, P, P, P, I, P, P, I, I, F, P],
-    "d3_layernorm_bwd": [P, I, P, P, P, P, P, P, P, P, I, I, P],
     "d3_layernorm_bwd_ls": [P, I, P, P, P, P, P, P, P, P, I, I, P, P, I, P, P, P, P],
     "d3_ls_gamma_from_wgrad": [P, P, P, P, P, P, I, I, P],
     "d3_rope": [P, P, P, LL, I, I, I, I, I, P],
@@ -68,7 +67,6 @@ SIGNATURES = {
     "d3_absmax": [P, LL, P, P],
     "d3_colmax": [P, P, I, I, P],
     "d3_sinkhorn_colsum": [P, P, F, P, P, I, I, P],
-    "d3_sinkhorn_colsum_det": [P, P, F, P, P, P, I, I, P],
     "d3_sinkhorn_rowsum": [P, P, F, P, P, P, I, I, P],
     "d3_sinkhorn_probs": [P, P, F, P, P, P, P, I, I, P],
     "d3_colsum_f32": [P, P, I, I, P],

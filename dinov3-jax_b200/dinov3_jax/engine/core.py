@@ -186,7 +186,6 @@ class Engine:
         self._ar_stage = self.fsdp.setup_small_allreduce(2 * K + 2 * (2 * K + 4) + 4) if comm is not None else None
         self.sk_dino = SinkhornBufs(ng, K, dev, joint=(self.sk_mx2, self.sk_s2), slot=0)
         self.sk_ibot = SinkhornBufs(self.max_masked, K, dev, joint=(self.sk_mx2, self.sk_s2), slot=1)
-        self.sk_scratch = torch.empty(ops.SK_SLABS * K, dtype=f32, device=dev) if K % 4 == 0 else None
         # centers of the optional softmax-centering path ("state" collection of the reference: dino_clstoken_loss.py:19-22)
         self.center_dino = torch.zeros(K, dtype=f32, device=dev)
         self.center_ibot = torch.zeros(K, dtype=f32, device=dev)
@@ -561,11 +560,7 @@ class Engine:
             s_in.zero_()
             s_in[2 * K:].copy_(self.sk_btot_local)
             for slot, sk, L, R in heads:
-                tgt = s_in[slot * K:(slot + 1) * K]
-                if self.sk_scratch is not None:  # atomics-free column sums: the step's dX chain is bit-reproducible
-                    ops.sinkhorn_colsum_det(L, sk.mx, temp, a[slot], tgt, self.sk_scratch)
-                else:
-                    ops.sinkhorn_colsum(L, sk.mx, temp, a[slot], tgt)
+                ops.sinkhorn_colsum(L, sk.mx, temp, a[slot], s_in[slot * K:(slot + 1) * K])
             if stage is not None:
                 self.fsdp.small_allreduce(off, 2 * K + 4, self.sk_s2, "sum")   # psum of the row sums (:53 / ibot :99), of B
             elif self.comm is not None:

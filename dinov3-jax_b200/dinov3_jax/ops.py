@@ -124,14 +124,6 @@ def layernorm_fwd(x, scale, bias, y, mean=None, rstd=None, eps=1e-6):
     return y
 
 
-def layernorm_bwd(dy, x, mean, rstd, scale, dx, dx_add=None, dscale=None, dbias=None):
-    T, D = x.shape
-    assert dy.shape == x.shape and dx.dtype == f32 and dy.is_contiguous()
-    N.check(N.init().d3_layernorm_bwd(_p(dy), int(dy.dtype == f32), _p(x), _p(mean), _p(rstd), _p(scale), _p(dx_add),
-                                      _p(dx), _p(dscale), _p(dbias), T, D, _s()), "d3_layernorm_bwd")
-    return dx
-
-
 def layernorm_bwd_ls(dy, x, mean, rstd, scale, dx, dx_add=None, dscale=None, dbias=None, *, ls_gamma=None, ls_u=None,
                      ls_gelu=False, ls_du=None, ls_dgamma=None, ls_dbias=None):
     """LayerNorm backward + the LayerScale/activation backward of the branch upstream (d3_layernorm_bwd_ls)."""
@@ -267,16 +259,6 @@ def colmax(L, cm):
 def sinkhorn_colsum(L, mx, temp, a, s):
     R, K = L.shape
     N.check(N.init().d3_sinkhorn_colsum(_p(L), _p(mx), temp, _p(a), _p(s), R, K, _s()), "d3_sinkhorn_colsum")
-
-
-SK_SLABS = 16     # D3_SK_SLABS (include/dinov3_b200.h)
-
-
-def sinkhorn_colsum_det(L, mx, temp, a, s, scratch):
-    """sinkhorn_colsum without atomics (bit-reproducible); scratch: fp32 [SK_SLABS, K]."""
-    R, K = L.shape
-    assert scratch.dtype == f32 and scratch.numel() >= SK_SLABS * K
-    N.check(N.init().d3_sinkhorn_colsum_det(_p(L), _p(mx), temp, _p(a), _p(s), _p(scratch), R, K, _s()), "d3_sinkhorn_colsum_det")
 
 
 def sinkhorn_rowsum(L, mx, temp, s, btot, a):

@@ -94,16 +94,15 @@ int d3_assemble_tokens_bwd(const float* dX, const unsigned char* masks, void* dT
 /* ---- LayerNorm (models/vision_transformer.py:40: eps 1e-6, biased variance E[x^2]-E[x]^2, fp32 statistics) ------- */
 int d3_layernorm_fwd(const float* x /*[T,D]*/, const float* scale, const float* bias, void* y, int y_is_f32,
                      float* mean /*[T] or NULL*/, float* rstd, int T, int D, float eps, void* stream);
-int d3_layernorm_bwd(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
-                     const float* scale, const float* dx_add /*residual-stream gradient or NULL*/, float* dx,
-                     float* dscale /*[D] += or NULL*/, float* dbias /*[D] +=*/, int T, int D, void* stream);
-/* LayerNorm backward fused with the LayerScale (+GELU) backward of the branch upstream of it
- * (layers/block.py:198-199 x_out = x_in + gamma * act(u); layers/layer_scale.py:17-21): with dx the row gradient it
- * has just produced it also writes du = bf16(dx * gamma * act'(u)), ls_dbias += colsum(du) and, when the stash `ls_u`
- * is given, ls_dgamma += colsum(dx * act(u)) (act = tanh-GELU if ls_gelu else identity).  ls_u == NULL: act =
- * identity, dgamma comes from d3_ls_gamma_from_wgrad.  ls_gamma == NULL: plain LayerNorm backward.                   */
+/* LayerNorm backward: dx = LN'(dy) (+ dx_add), dscale += colsum(dy * xhat), dbias += colsum(dy); with ls_gamma == NULL
+ * that is all it does (the plain LayerNorm backward).  With ls_gamma it is fused with the LayerScale (+GELU) backward
+ * of the branch upstream of it (layers/block.py:198-199 x_out = x_in + gamma * act(u); layers/layer_scale.py:17-21):
+ * with dx the row gradient it has just produced it also writes du = bf16(dx * gamma * act'(u)), ls_dbias += colsum(du)
+ * and, when the stash `ls_u` is given, ls_dgamma += colsum(dx * act(u)) (act = tanh-GELU if ls_gelu else identity).
+ * ls_u == NULL: act = identity, dgamma comes from d3_ls_gamma_from_wgrad.                                           */
 int d3_layernorm_bwd_ls(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
-                        const float* scale, const float* dx_add, float* dx, float* dscale, float* dbias, int T, int D,
+                        const float* scale, const float* dx_add /*residual-stream gradient or NULL*/, float* dx,
+                        float* dscale /*[D] += or NULL*/, float* dbias /*[D] +=*/, int T, int D,
                         const float* ls_gamma /*[D] or NULL*/, const void* ls_u_bf16 /*[T,D] or NULL*/, int ls_gelu,
                         void* ls_du_bf16 /*[T,D]*/, float* ls_dgamma /*[D] += or NULL*/, float* ls_dbias /*[D] +=*/,
                         void* stream);
@@ -186,11 +185,6 @@ int d3_absmax(const float* L, long long n, float* out /*pre-set to -inf*/, void*
 int d3_colmax(const float* L /*[R,K]*/, float* cm /*[K] pre-set to -inf*/, int R, int K, void* stream);
 int d3_sinkhorn_colsum(const float* L /*[R,K]*/, const float* mx, float temp, const float* a /*[R] or NULL (=1)*/,
                        float* s /*[K] zeroed, +=*/, int R, int K, void* stream);
-/* Same sums without atomics (bit-reproducible): row slabs write partial sums to scratch[D3_SK_SLABS][K], which a second
- * launch adds to s in a fixed order.                                                                                */
-#define D3_SK_SLABS 16
-int d3_sinkhorn_colsum_det(const float* L, const float* mx, float temp, const float* a, float* s /*[K] zeroed, +=*/,
-                           float* scratch /*[D3_SK_SLABS, K]*/, int R, int K, void* stream);
 int d3_sinkhorn_rowsum(const float* L, const float* mx, float temp, const float* s, const float* btot /*device*/,
                        float* a /*[R]*/, int R, int K, void* stream);
 int d3_sinkhorn_probs(const float* L, const float* mx, float temp, const float* s, const float* a, const float* btot,

@@ -28,10 +28,11 @@ def test_python_signature_table_matches_header():
     assert declared == bound, (declared - bound, bound - declared)
 
 
-def test_abi_version_and_error_string():
+def test_abi_version_4_and_error_string():
+    """Version 4: the plain LayerNorm backward and the atomic-free Sinkhorn sums have no entry points of their own."""
     from dinov3_jax import _native
     lib = _native.lib()
-    assert lib.d3_abi_version() == 3
+    assert lib.d3_abi_version() == 4
     assert isinstance(lib.d3_last_error(), bytes)
 
 

@@ -528,6 +528,15 @@ def test_gram_term_gradient_alone():
 def test_training_steps_are_bit_reproducible():
     """Two engines with the same parameters and batch run three training steps each: every gradient, parameter and
     metric is the same bit for bit (the step's reductions add their partial sums in a fixed order)."""
+    _assert_steps_bit_reproducible("sinkhorn_knopp")
+
+
+def test_training_steps_with_softmax_centering_are_bit_reproducible():
+    """The same with the optional softmax centering, whose column sums are slab reductions too."""
+    _assert_steps_bit_reproducible("softmax")
+
+
+def _assert_steps_bit_reproducible(centering):
     from dinov3_jax.engine import Engine, config_for
     from dinov3_jax.engine.synth import reference_like_params, synthetic_batch
     cfg = dataclasses.replace(config_for("vit_small", n_prototypes=4096), depth=2)
@@ -536,7 +545,7 @@ def test_training_steps_are_bit_reproducible():
     batch = synthetic_batch(cfg, B, seed=3)
     runs = []
     for _ in range(2):
-        eng = Engine(cfg, B, max_masked=int(batch["mask_indices_list"].shape[0]))
+        eng = Engine(cfg, B, max_masked=int(batch["mask_indices_list"].shape[0]), centering=centering)
         eng.params.load_reference_tree(params)
         for _ in range(3):
             eng.train_step(batch, **HYPER)

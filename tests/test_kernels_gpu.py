@@ -213,7 +213,8 @@ def test_token_rows_gather_scatter_bit_exact():
 
 # --------------------------------------------------------------------------------------------------- normalisation / rope
 @pytest.mark.parametrize("T,D", [(1000, 384), (333, 1024), (7, 128), (2051, 768), (100, 256), (300, 1536), (64, 192)])
-def test_layernorm_forward_backward(T, D):
+def test_layernorm_forward_and_plain_backward(T, D):
+    """d3_layernorm_fwd and d3_layernorm_bwd_ls without a LayerScale tail (the plain LayerNorm backward), fp32 dy."""
     from dinov3_jax import ops
     from oracle.model import layer_norm
     x = torch.randn(T, D, device="cuda") * 2 + 0.5
@@ -227,7 +228,7 @@ def test_layernorm_forward_backward(T, D):
     dy, add = torch.randn(T, D, device="cuda"), torch.randn(T, D, device="cuda")
     ref.backward(dy)
     dx, ds, db = torch.empty(T, D, device="cuda"), torch.zeros(D, device="cuda"), torch.zeros(D, device="cuda")
-    ops.layernorm_bwd(dy, x, mean, rstd, sc, dx, dx_add=add, dscale=ds, dbias=db)
+    ops.layernorm_bwd_ls(dy, x, mean, rstd, sc, dx, dx_add=add, dscale=ds, dbias=db)
     assert rel(dx, xr.grad + add) < 1e-4 and rel(ds, scr.grad) < 1e-4 and rel(db, bir.grad) < 1e-4
 
 
@@ -342,9 +343,18 @@ def test_l2norm_and_layerscale_backward():
 
 # --------------------------------------------------------------------------------------------------- losses
 def test_sinkhorn_ce_koleo_match_oracle():
+    _sinkhorn_ce_koleo_vs_oracle(4096)
+
+
+def test_sinkhorn_ce_koleo_match_oracle_with_k_not_a_multiple_of_4():
+    """K % 4 != 0: the scalar Sinkhorn column-sum, row-sum, colmax and cross-entropy paths."""
+    _sinkhorn_ce_koleo_vs_oracle(1001)
+
+
+def _sinkhorn_ce_koleo_vs_oracle(K):
     from dinov3_jax import ops
     from oracle.losses import dino_loss, ibot_loss_masked, koleo_loss, sinkhorn_knopp
-    R, K, temp = 24, 4096, 0.05
+    R, temp = 24, 0.05
     L = torch.randn(R, K, device="cuda") * 0.3
     gmx = torch.full((1,), float("-inf"), device="cuda"); ops.absmax(L, gmx)
     assert gmx.item() == L.max().item()
@@ -409,6 +419,61 @@ def test_adamw_ema_clip_matches_optax_formula():
     ops.adamw_ema(p, g, m, v, t, pb, tb, 8192, segs, 3, ss, maxn, lr, llr, wd, step, mom)
     assert rel(p, P1) < 1e-6 and rel(m, M1) < 1e-6 and rel(v, V1) < 1e-6 and rel(t, T1) < 1e-6
     assert torch.equal(pb, p[:8192].to(torch.bfloat16)) and torch.equal(tb, t[:8192].to(torch.bfloat16))
+
+
+def _gram_ref(Ss, St, mode, block):
+    """float64 sum of (s' - t')^2 over the counted elements (d3_gram_diff's modes and block-diagonal form)."""
+    s, t = Ss.double(), St.double()
+    if mode == 1:
+        s = s.clamp(min=0)
+    elif mode == 2:
+        s = torch.where((s < 0) & (t < 0), torch.zeros_like(s), s)
+    if mode:
+        t = t.clamp(min=0)
+    d2 = (s - t) ** 2
+    if block:
+        i = torch.arange(s.shape[0], device=s.device) // block
+        d2 = d2 * (i[:, None] == i[None, :])
+    return d2.sum()
+
+
+@pytest.mark.parametrize("case", ["sinkhorn_colsum", "sinkhorn_colsum_k1001", "colsum_f32", "gram_diff", "gram_diff_blocks"])
+def test_sums_are_bit_reproducible(case):
+    """Column sums and the Gram loss add their slab partials in a fixed order: two calls on the same input give the same
+    bits; the result matches a float64 sum."""
+    from dinov3_jax import ops
+    if case.startswith("sinkhorn"):
+        R, K, temp = 3771, (65536 if case == "sinkhorn_colsum" else 1001), 0.05
+        L = torch.randn(R, K, device="cuda") * 0.3
+        mx = L.max(0).values
+        a = torch.rand(R, device="cuda") + 0.5
+
+        def run():
+            s = torch.zeros(K, device="cuda")
+            ops.sinkhorn_colsum(L, mx, temp, a, s)
+            return s
+        ref = (torch.exp((L.double() - mx.double()) / temp) * a.double()[:, None]).sum(0)
+    elif case == "colsum_f32":
+        L = torch.randn(3771, 65536, device="cuda")
+
+        def run():
+            out = torch.zeros(L.shape[1], device="cuda")
+            ops.colsum_f32(L, out)
+            return out
+        ref = L.double().sum(0)
+    else:
+        n, block, mode = (1024, 0, 1) if case == "gram_diff" else (980, 196, 2)
+        Ss, St = torch.rand(n, n, device="cuda") * 2 - 1, torch.rand(n, n, device="cuda") * 2 - 1
+        inv = 1.0 / (n * n)
+
+        def run():
+            loss = torch.full((1,), 0.5, device="cuda")          # the loss is accumulated into
+            ops.gram_diff(Ss, St, None, mode, inv, loss, block=block)
+            return loss
+        ref = (0.5 + inv * _gram_ref(Ss, St, mode, block)).reshape(1)
+    first, second = run(), run()
+    assert torch.equal(first, second)
+    assert rel(first, ref) < 1e-5
 
 
 # --------------------------------------------------------------------------------------------------- fused reduce-scatter

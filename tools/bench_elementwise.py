@@ -34,7 +34,6 @@ def timeit(name, fn, nbytes, it=20):
 
 TD = T * D
 print(f"T={T} D={D}")
-timeit("layernorm_bwd (old fused) bf16 dy + dx_add", lambda: ops.layernorm_bwd(dyb, x, mean, rstd, sc, dx, dx_add=add, dscale=ds, dbias=db), TD * (2 + 4 + 4 + 4))
 timeit("layernorm_bwd_ls plain", lambda: ops.layernorm_bwd_ls(dyb, x, mean, rstd, sc, dx, dx_add=add, dscale=ds, dbias=db), TD * (2 + 4 + 4 + 4))
 timeit("layernorm_bwd_ls linear tail", lambda: ops.layernorm_bwd_ls(dyb, x, mean, rstd, sc, dx, dx_add=add, dscale=ds, dbias=db, ls_gamma=gam, ls_du=du, ls_dbias=dbl), TD * (2 + 4 + 4 + 4 + 2))
 timeit("layernorm_bwd_ls gelu tail", lambda: ops.layernorm_bwd_ls(dyb, x, mean, rstd, sc, dx, dx_add=add, dscale=ds, dbias=db, ls_gamma=gam, ls_u=u, ls_gelu=True, ls_du=du, ls_dgamma=dg, ls_dbias=dbl), TD * (2 + 4 + 4 + 4 + 2 + 2))

@@ -110,10 +110,10 @@ def g_elementwise():
         dy = torch.randn(T, D, device=dev); ref.backward(dy)
         add = torch.randn(T, D, device=dev)
         dx = torch.empty(T, D, device=dev); ds = torch.zeros(D, device=dev); db = torch.zeros(D, device=dev)
-        ops.layernorm_bwd(dy, x, mean, rstd, sc, dx, dx_add=add, dscale=ds, dbias=db)
+        ops.layernorm_bwd_ls(dy, x, mean, rstd, sc, dx, dx_add=add, dscale=ds, dbias=db)
         report("ln_bwd dx(f32 dy)", dx, xr.grad + add, 1e-4); report("ln_bwd dscale", ds, scr.grad, 1e-4); report("ln_bwd dbias", db, bir.grad, 1e-4)
         dyb = dy.to(torch.bfloat16); dx2 = torch.empty(T, D, device=dev)
-        ops.layernorm_bwd(dyb, x, mean, rstd, sc, dx2)
+        ops.layernorm_bwd_ls(dyb, x, mean, rstd, sc, dx2)
         xr.grad = None; layer_norm(xr, sc, bi, 1e-6).backward(dyb.float())
         report("ln_bwd dx(bf16 dy)", dx2, xr.grad, 1e-4)
     # rope
