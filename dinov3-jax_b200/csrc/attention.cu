@@ -10,7 +10,12 @@
 // key / value range of the group are staged once; each warpgroup walks the keys in blocks of 64: S = Q K^T (SS form),
 // online softmax on the accumulator fragment, then O += P V with P handed to the tensor core straight from registers
 // (RS form: the accumulator fragment of S is the A-operand fragment of the PV product).
+//
+// Crops longer than the resident kernels hold (span > 448 forward, N > 384 backward; G = 1 there) take streamed kernels
+// with the same per-tile arithmetic: a producer warpgroup fills an mbarrier ring of 128-row K / V (or Q / dO) tiles that both
+// consumer warpgroups read, so shared memory no longer grows with N.  Any N up to ATTN_MAX_TOKENS.
 #include "ptx.cuh"
+#include <climits>
 #include <cstdlib>
 #include "d3_internal.h"
 
@@ -52,6 +57,65 @@ __device__ __forceinline__ RowInfo row_info(const AttnShape& sh, int c, int q) {
   ri.khi = ri.klo + sh.N;
   ri.ok = (q < sh.span) && (c * sh.G + ri.g < sh.n_crops);
   return ri;
+}
+
+// Online softmax of one block of 8*NI keys starting at key k0, on the S accumulator fragment (this thread: rows ri[0],
+// ri[1], columns k0 + 8i + c2 + {0,1}).  S becomes P; the running max m, sum l and the output accumulator o are rescaled.
+// Keys outside a row's [klo, khi) give exactly 0.
+template <int NI>
+__device__ __forceinline__ void online_softmax(float (&s)[4 * NI], float (&o)[32], float (&m)[2], float (&l)[2],
+                                               const RowInfo (&ri)[2], int k0, int c2, float cs) {
+  const int kb0 = k0 + c2;
+  const bool full = k0 >= max(ri[0].klo, ri[1].klo) && k0 + 8 * NI <= min(ri[0].khi, ri[1].khi);
+  float mx[2] = {-3.0e38f, -3.0e38f};
+#pragma unroll
+  for (int i = 0; i < NI; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int hh = j >> 1, kk = kb0 + 8 * i + (j & 1);
+      if (full || (kk >= ri[hh].klo && kk < ri[hh].khi)) mx[hh] = fmaxf(mx[hh], s[4 * i + j]);
+    }
+  float corr[2], ms[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+    const float mn = fmaxf(m[hh], mx[hh]);
+    corr[hh] = ex2_approx((m[hh] - mn) * cs);
+    m[hh] = mn;
+    ms[hh] = mn * cs;
+    l[hh] *= corr[hh];
+  }
+#pragma unroll
+  for (int i = 0; i < NI; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int hh = j >> 1, kk = kb0 + 8 * i + (j & 1);
+      const float p = (full || (kk >= ri[hh].klo && kk < ri[hh].khi)) ? ex2_approx(fmaf(s[4 * i + j], cs, -ms[hh])) : 0.f;
+      s[4 * i + j] = p;
+      l[hh] += p;
+      if (i < 8) o[4 * i + j] *= corr[hh];
+    }
+}
+
+// O = o / l as bf16 and the natural-log LSE of the scaled scores ([crop, head, token]) for this thread's two rows
+__device__ __forceinline__ void store_o_lse(const float (&o)[32], float (&l)[2], const float (&m)[2], const RowInfo (&ri)[2],
+                                            const AttnShape& sh, int c, int h, int row_base, int wq0, int r_in, int c2,
+                                            __nv_bfloat16* O, float* LSE) {
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+    const int q = wq0 + r_in + 8 * hh;
+    if (!ri[hh].ok) continue;
+    const float inv = 1.f / l[hh];
+    __nv_bfloat16* dst = O + (size_t)(row_base + q) * sh.D + h * 64 + c2;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
+    if (LSE && c2 == 0)
+      LSE[((size_t)(c * sh.G + ri[hh].g) * sh.H + h) * sh.N + (q - ri[hh].klo)] = m[hh] * sh.scale + logf(l[hh]);
+  }
 }
 
 __global__ void __launch_bounds__(256)
@@ -115,38 +179,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(s);
-    // ---- online softmax of the two rows this thread holds (columns 8i + c2 + {0,1})
-    const int kb0 = b * 64 + c2;
-    const bool full = kb0 - c2 >= max(ri[0].klo, ri[1].klo) && kb0 - c2 + 64 <= min(ri[0].khi, ri[1].khi);
-    float mx[2] = {-3.0e38f, -3.0e38f};
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int hh = j >> 1, kk = kb0 + 8 * i + (j & 1);
-        if (full || (kk >= ri[hh].klo && kk < ri[hh].khi)) mx[hh] = fmaxf(mx[hh], s[4 * i + j]);
-      }
-    float corr[2], ms[2];
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
-      const float mn = fmaxf(m[hh], mx[hh]);
-      corr[hh] = ex2_approx((m[hh] - mn) * cs);
-      m[hh] = mn;
-      ms[hh] = mn * cs;
-      l[hh] *= corr[hh];
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int hh = j >> 1, kk = kb0 + 8 * i + (j & 1);
-        const float p = (full || (kk >= ri[hh].klo && kk < ri[hh].khi)) ? ex2_approx(fmaf(s[4 * i + j], cs, -ms[hh])) : 0.f;
-        s[4 * i + j] = p;
-        l[hh] += p;
-        o[4 * i + j] *= corr[hh];
-      }
+    online_softmax<8>(s, o, m, l, ri, b * 64, c2, cs);
     // ---- O += P V (A = P from registers, B = V block MN-major: 16 keys per k-step = 2048 B)
     uint32_t a[4][4];
 #pragma unroll
@@ -162,21 +195,108 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wgmma_wait<0>();
     fence_regs(o);
   }
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
-    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
-    const int q = wq0 + r_in + 8 * hh;
-    if (!ri[hh].ok) continue;
-    const float inv = 1.f / l[hh];
-    __nv_bfloat16* dst = O + (size_t)(row_base + q) * sh.D + h * 64 + c2;
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-      *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
-    if (LSE && c2 == 0)   // natural-log LSE of the scaled scores, indexed [crop, head, token]
-      LSE[((size_t)(c * sh.G + ri[hh].g) * sh.H + h) * sh.N + (q - ri[hh].klo)] = m[hh] * sh.scale + logf(l[hh]);
-  }
+  store_o_lse(o, l, m, ri, sh, c, h, row_base, wq0, r_in, c2, O, LSE);
   dbg_mark(1);
+}
+
+// ------------------------------------------------------------------------------------------------ streamed forward
+// One CTA per (128-row query tile, head, crop), G = 1, any N.  Warpgroup 2 is the producer (one warp issues the fills):
+// Q once, then every 128-key K / V
+// block through a ring of FWD_STAGES 32 KB stages (full barrier: TMA bytes; empty barrier: one arrive per consumer warp
+// that has rows in this crop).  Per block each consumer warpgroup runs S = Q K^T (m64n128), the resident kernel's online
+// softmax, and O += P V as 8 RS k-steps.  Block b sits in stage b % STAGES; its fill is use u = b / STAGES of the stage,
+// so consumers wait on full parity u & 1, and the producer waits on empty parity (u - 1) & 1 before fill u >= 1.
+constexpr int FWD_STAGES = 4, DKDV_STAGES = 3, DQ_STAGES = 4;
+constexpr int RING_THREADS = 384;            // two consumer warpgroups + a producer warpgroup (registers: 232 / 40)
+
+__global__ void __launch_bounds__(RING_THREADS, 1)
+attn_fwd_stream_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ O, float* __restrict__ LSE,
+                       const AttnShape sh) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // layout: [Q 128 x 128 B][STAGES x (K 16 KB, V 16 KB)][full][empty][q barrier]
+  uint8_t* sQ = smem;
+  uint8_t* ring = smem + 16384;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + FWD_STAGES * 32768);
+  uint64_t* empty = full + FWD_STAGES;
+  uint64_t* bar_q = empty + FWD_STAGES;
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int qt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
+  const int q0 = qt * 128, row_base = c * sh.N, nkb = (sh.N + 127) >> 7;
+  const int n_wg = (q0 + 64 < sh.N) ? 2 : 1;   // consumer warpgroups with at least one query row of the crop
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    for (int st = 0; st < FWD_STAGES; ++st) {
+      mbar_init(full + st, 1);
+      mbar_init(empty + st, 4 * n_wg);
+    }
+    mbar_init(bar_q, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 288 && elect_one()) {
+      mbar_expect_tx(bar_q, 16384);
+      tma_load_2d(&tmQKV, bar_q, sQ, h * 64, row_base + q0);
+      for (int b = 0; b < nkb; ++b) {
+        const int st = b % FWD_STAGES, u = b / FWD_STAGES;
+        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
+        mbar_expect_tx(full + st, 32768);
+        tma_load_2d(&tmQKV, full + st, ring + st * 32768, sh.D + h * 64, row_base + b * 128);
+        tma_load_2d(&tmQKV, full + st, ring + st * 32768 + 16384, 2 * sh.D + h * 64, row_base + b * 128);
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int wq0 = q0 + wg * 64;
+  if (wq0 >= sh.N) return;                     // not counted by the empty barriers (n_wg)
+  mbar_wait(bar_q, 0);
+
+  const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
+  RowInfo ri[2];
+  ri[0] = row_info(sh, c, wq0 + r_in);
+  ri[1] = row_info(sh, c, wq0 + r_in + 8);
+  const float cs = sh.scale * LOG2E;
+  float m[2] = {-3.0e38f, -3.0e38f}, l[2] = {0.f, 0.f};
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  const uint64_t qd = gmma_desc_sw128(smem_u32(sQ + wg * 8192), 16, 1024);
+
+#pragma unroll 1
+  for (int b = 0; b < nkb; ++b) {
+    const int st = b % FWD_STAGES;
+    uint8_t* sK = ring + st * 32768;
+    mbar_wait(full + st, (b / FWD_STAGES) & 1);
+    float s[64];
+    const uint64_t kd = gmma_desc_sw128(smem_u32(sK), 16, 1024);
+    fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_m64n128k16_ss<0, 0>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    online_softmax<16>(s, o, m, l, ri, b * 128, c2, cs);
+    uint32_t a[8][4];
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) a[kk][e] = pack_bf16(s[8 * kk + 2 * e], s[8 * kk + 2 * e + 1]);
+    const uint64_t vd = gmma_desc_sw128(smem_u32(sK + 16384), 8192, 1024);   // V MN-major: 16 keys per k-step
+    fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_rs<1>(o, a[kk], vd + 128 * kk, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
+    if (lane_id() == 0) mbar_arrive(empty + st);   // this warp no longer reads the stage
+  }
+  store_o_lse(o, l, m, ri, sh, c, h, row_base, wq0, r_in, c2, O, LSE);
 }
 
 // Delta[c,h,q] = sum_d dO[q, h, d] * O[q, h, d]    (backward softmax term)
@@ -245,6 +365,103 @@ __device__ __forceinline__ void store_grad_rows(float (&a)[32], const AttnShape&
   }
 }
 
+// S and dP of one warpgroup's 64 query rows (first row q0 of the crop group, tiles sQw / sDOw: 64 rows x 128 B) against
+// the 128-key tile kt (sK, sV), turned into P (in s) and dS (in dp).  Keys outside a row's crop and rows outside the group
+// give exactly 0.
+__device__ __forceinline__ void p_ds_tile(const AttnShape& sh, const float* __restrict__ LSE, const float* __restrict__ Delta,
+                                          int c, int h, int q0, int kt, const uint8_t* sQw, const uint8_t* sDOw,
+                                          const uint8_t* sK, const uint8_t* sV, int r_in, int c2, float (&s)[64],
+                                          float (&dp)[64]) {
+  const float cs = sh.scale * LOG2E;
+  const uint64_t qd = gmma_desc_sw128(smem_u32(sQw), 16, 1024);
+  const uint64_t dod = gmma_desc_sw128(smem_u32(sDOw), 16, 1024);
+  const uint64_t kd = gmma_desc_sw128(smem_u32(sK), 16, 1024);
+  const uint64_t vd = gmma_desc_sw128(smem_u32(sV), 16, 1024);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {   // S and dP are independent accumulator chains: interleave them
+    wgmma_m64n128k16_ss<0, 0>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
+    wgmma_m64n128k16_ss<0, 0>(dp, dod + 2 * k, vd + 2 * k, k > 0 ? 1u : 0u);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_regs(s);
+  fence_regs(dp);
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int q = q0 + r_in + 8 * hh;
+    const RowInfo ri = row_info(sh, c, q);
+    const size_t stat = ((size_t)(c * sh.G + ri.g) * sh.H + h) * sh.N + (ri.ok ? q - ri.klo : 0);
+    const float lse2 = ri.ok ? LSE[stat] * LOG2E : 0.f;
+    const float dl = ri.ok ? Delta[stat] : 0.f;
+    const int lo = ri.ok ? ri.klo - kt * 128 : 0, hi = ri.ok ? ri.khi - kt * 128 : 0;   // valid key columns
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int e = 4 * i + 2 * hh + j, col = 8 * i + c2 + j;
+        const bool ok = col >= lo && col < hi;
+        const float p = ok ? ex2_approx(fmaf(s[e], cs, -lse2)) : 0.f;
+        dp[e] = ok ? (p * sh.scale) * (dp[e] - dl) : 0.f;
+        s[e] = p;
+      }
+  }
+}
+
+// P and dS of this thread's rows `row`, `row + 8` of the 128-row query tile into bf16 SWIZZLE_128B tiles
+// [2 chunks of 64 keys][128 q x 128 B] (sP, sDS), read back MN-major by dkdv_mma
+__device__ __forceinline__ void stash_p_ds(const float (&s)[64], const float (&dp)[64], uint8_t* sP, uint8_t* sDS, int row,
+                                           int c2) {
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const uint32_t off = (i >> 3) * 16384 + sw128_offset(row + 8 * hh, (8 * i + c2) & 63);
+      *reinterpret_cast<uint32_t*>(sP + off) = pack_bf16(s[4 * i + 2 * hh], s[4 * i + 2 * hh + 1]);
+      *reinterpret_cast<uint32_t*>(sDS + off) = pack_bf16(dp[4 * i + 2 * hh], dp[4 * i + 2 * hh + 1]);
+    }
+  }
+}
+
+// dV[keys, 64] += P^T dO ; dK[keys, 64] += dS^T Q over the 128 query rows of one tile (sDOt, sQt), for this warpgroup's
+// 64 keys (A MN-major: 16 query rows per k-step = 2048 B)
+__device__ __forceinline__ void dkdv_mma(float (&dk)[32], float (&dv)[32], const uint8_t* sP, const uint8_t* sDS,
+                                         const uint8_t* sDOt, const uint8_t* sQt, int wg) {
+  const uint64_t pd = gmma_desc_sw128(smem_u32(sP + wg * 16384), 16384, 1024);
+  const uint64_t sd = gmma_desc_sw128(smem_u32(sDS + wg * 16384), 16384, 1024);
+  const uint64_t dod = gmma_desc_sw128(smem_u32(sDOt), 8192, 1024);
+  const uint64_t qd = gmma_desc_sw128(smem_u32(sQt), 8192, 1024);
+  fence_regs(dk);
+  fence_regs(dv);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    wgmma_m64n64k16_ss<1, 1>(dv, pd + 128 * k, dod + 128 * k, 1u);
+    wgmma_m64n64k16_ss<1, 1>(dk, sd + 128 * k, qd + 128 * k, 1u);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_regs(dk);
+  fence_regs(dv);
+}
+
+// dQ += dS K over one 128-key tile, dS straight from registers (RS form), K as MN-major B (keys x d)
+__device__ __forceinline__ void dq_mma(float (&dq)[32], const float (&dp)[64], const uint8_t* sK) {
+  uint32_t a[8][4];
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) a[kk][e] = pack_bf16(dp[8 * kk + 2 * e], dp[8 * kk + 2 * e + 1]);
+  const uint64_t kd = gmma_desc_sw128(smem_u32(sK), 8192, 1024);
+  fence_regs(dq);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_rs<1>(dq, a[kk], kd + 128 * kk, 1u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_regs(dq);
+}
+
 __global__ void __launch_bounds__(256)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
                 const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
@@ -266,7 +483,6 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
   const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
   const int h = blockIdx.x, c = blockIdx.y;
   const int row_base = c * sh.span;
-  const float cs = sh.scale * LOG2E;
   dbg_mark(0);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
@@ -297,41 +513,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
     kv_phase ^= 1;
     kv_loaded = kt;
   };
-  // S and dP of this warpgroup's 64 query rows of tile qt against key tile kt, turned into P (in s) and dS (in dp)
   auto p_ds = [&](int qt, int kt, float (&s)[64], float (&dp)[64]) {
-    const uint64_t qd = gmma_desc_sw128(smem_u32(sQ + qt * 16384 + wg * 8192), 16, 1024);
-    const uint64_t dod = gmma_desc_sw128(smem_u32(sDO + qt * 16384 + wg * 8192), 16, 1024);
-    const uint64_t kd = gmma_desc_sw128(smem_u32(sK), 16, 1024);
-    const uint64_t vd = gmma_desc_sw128(smem_u32(sV), 16, 1024);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {   // S and dP are independent accumulator chains: interleave them
-      wgmma_m64n128k16_ss<0, 0>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
-      wgmma_m64n128k16_ss<0, 0>(dp, dod + 2 * k, vd + 2 * k, k > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(s);
-    fence_regs(dp);
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      const int q = qt * 128 + wg * 64 + r_in + 8 * hh;
-      const RowInfo ri = row_info(sh, c, q);
-      const size_t stat = ((size_t)(c * sh.G + ri.g) * sh.H + h) * sh.N + (ri.ok ? q - ri.klo : 0);
-      const float lse2 = ri.ok ? LSE[stat] * LOG2E : 0.f;
-      const float dl = ri.ok ? Delta[stat] : 0.f;
-      const int lo = ri.ok ? ri.klo - kt * 128 : 0, hi = ri.ok ? ri.khi - kt * 128 : 0;   // valid key columns
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const int e = 4 * i + 2 * hh + j, col = 8 * i + c2 + j;
-          const bool ok = col >= lo && col < hi;
-          const float p = ok ? ex2_approx(fmaf(s[e], cs, -lse2)) : 0.f;
-          dp[e] = ok ? (p * sh.scale) * (dp[e] - dl) : 0.f;
-          s[e] = p;
-        }
-    }
+    p_ds_tile(sh, LSE, Delta, c, h, qt * 128 + wg * 64, kt, sQ + qt * 16384 + wg * 8192, sDO + qt * 16384 + wg * 8192,
+              sK, sV, r_in, c2, s, dp);
   };
 
   mbar_wait(bar_q, 0);
@@ -346,35 +530,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
     for (int qt = 0; qt < nQ; ++qt) {
       float s[64], dp[64];
       p_ds(qt, kt, s, dp);
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int row = wg * 64 + r_in + 8 * hh;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const uint32_t off = (i >> 3) * 16384 + sw128_offset(row, (8 * i + c2) & 63);
-          *reinterpret_cast<uint32_t*>(sP + off) = pack_bf16(s[4 * i + 2 * hh], s[4 * i + 2 * hh + 1]);
-          *reinterpret_cast<uint32_t*>(sDS + off) = pack_bf16(dp[4 * i + 2 * hh], dp[4 * i + 2 * hh + 1]);
-        }
-      }
+      stash_p_ds(s, dp, sP, sDS, wg * 64 + r_in, c2);
       fence_proxy_async_smem();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
       __syncthreads();
-      // dV[keys, 64] += P^T dO ; dK[keys, 64] += dS^T Q   (A MN-major: 16 query rows per k-step = 2048 B)
-      const uint64_t pd = gmma_desc_sw128(smem_u32(sP + wg * 16384), 16384, 1024);
-      const uint64_t sd = gmma_desc_sw128(smem_u32(sDS + wg * 16384), 16384, 1024);
-      const uint64_t dod = gmma_desc_sw128(smem_u32(sDO + qt * 16384), 8192, 1024);
-      const uint64_t qd = gmma_desc_sw128(smem_u32(sQ + qt * 16384), 8192, 1024);
-      fence_regs(dk);
-      fence_regs(dv);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        wgmma_m64n64k16_ss<1, 1>(dv, pd + 128 * k, dod + 128 * k, 1u);
-        wgmma_m64n64k16_ss<1, 1>(dk, sd + 128 * k, qd + 128 * k, 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(dk);
-      fence_regs(dv);
+      dkdv_mma(dk, dv, sP, sDS, sDO + qt * 16384, sQ + qt * 16384, wg);
       __syncthreads();            // both warpgroups are done reading sP / sDS before the next tile pair rewrites them
     }
     store_grad_rows(dk, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 1, true, dQKV);
@@ -393,23 +552,155 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
       load_kv(kt);
       float s[64], dp[64];
       p_ds(qt, kt, s, dp);
-      uint32_t a[8][4];
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) a[kk][e] = pack_bf16(dp[8 * kk + 2 * e], dp[8 * kk + 2 * e + 1]);
-      const uint64_t kd = gmma_desc_sw128(smem_u32(sK), 8192, 1024);   // K as MN-major B (keys x d)
-      fence_regs(dq);
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_rs<1>(dq, a[kk], kd + 128 * kk, 1u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(dq);
+      dq_mma(dq, dp, sK);
     }
     store_grad_rows(dq, sh, c, row_base, qt * 128 + wg * 64, r_in, c2, h, 0, true, dQKV);
   }
   dbg_mark(1);
+}
+
+// ------------------------------------------------------------------------------------------------ streamed backward
+// Any N, G = 1, as two grids that each write their outputs once, with every sum in ascending tile order (no atomics):
+//   dK / dV: one CTA per (128-key tile, head, crop).  K / V stay resident; the query tiles' Q / dO stream through a ring
+//            of DKDV_STAGES stages.  Per query tile: p_ds_tile, P and dS staged in shared memory, dkdv_mma (the resident
+//            kernel's phase 1).
+//   dQ:      one CTA per (128-row query tile, head, crop).  Q / dO stay resident; K / V stream through a ring of DQ_STAGES
+//            stages.  Per key tile: p_ds_tile, dq_mma (the resident kernel's phase 2).
+// Warpgroup 2 is the producer; the ring protocol is the streamed forward's (tile j in stage j % STAGES, use u = j / STAGES:
+// consumers wait on full parity u & 1, the producer waits on empty parity (u - 1) & 1 before fill u >= 1).
+__global__ void __launch_bounds__(RING_THREADS, 1)
+attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
+                     const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
+                     const AttnShape sh) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sK = smem;                          // 16 KB
+  uint8_t* sV = sK + 16384;                    // 16 KB
+  uint8_t* sP = sV + 16384;                    // 32 KB
+  uint8_t* sDS = sP + 32768;                   // 32 KB
+  uint8_t* ring = sDS + 32768;                 // STAGES x (Q 16 KB, dO 16 KB)
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + DKDV_STAGES * 32768);
+  uint64_t* empty = full + DKDV_STAGES;
+  uint64_t* bar_kv = empty + DKDV_STAGES;
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
+  const int kt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
+  const int row_base = c * sh.N, nq = (sh.N + 127) >> 7;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    tma_prefetch_desc(&tmDO);
+    for (int st = 0; st < DKDV_STAGES; ++st) {
+      mbar_init(full + st, 1);
+      mbar_init(empty + st, 8);                // both consumer warpgroups read every query tile
+    }
+    mbar_init(bar_kv, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 288 && elect_one()) {
+      mbar_expect_tx(bar_kv, 32768);
+      tma_load_2d(&tmQKV, bar_kv, sK, sh.D + h * 64, row_base + kt * 128);
+      tma_load_2d(&tmQKV, bar_kv, sV, 2 * sh.D + h * 64, row_base + kt * 128);
+      for (int qt = 0; qt < nq; ++qt) {
+        const int st = qt % DKDV_STAGES, u = qt / DKDV_STAGES;
+        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
+        mbar_expect_tx(full + st, 32768);
+        tma_load_2d(&tmQKV, full + st, ring + st * 32768, h * 64, row_base + qt * 128);
+        tma_load_2d(&tmDO, full + st, ring + st * 32768 + 16384, h * 64, row_base + qt * 128);
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<232>();
+  mbar_wait(bar_kv, 0);
+  float dk[32], dv[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
+#pragma unroll 1
+  for (int qt = 0; qt < nq; ++qt) {
+    const int st = qt % DKDV_STAGES;
+    const uint8_t* sQt = ring + st * 32768;
+    const uint8_t* sDOt = sQt + 16384;
+    mbar_wait(full + st, (qt / DKDV_STAGES) & 1);
+    float s[64], dp[64];
+    p_ds_tile(sh, LSE, Delta, c, h, qt * 128 + wg * 64, kt, sQt + wg * 8192, sDOt + wg * 8192, sK, sV, r_in, c2, s, dp);
+    stash_p_ds(s, dp, sP, sDS, wg * 64 + r_in, c2);
+    fence_proxy_async_smem();
+    named_bar_sync(1, 256);                    // the consumer warpgroups only: P / dS of all 128 query rows are staged
+    dkdv_mma(dk, dv, sP, sDS, sDOt, sQt, wg);
+    if (lane_id() == 0) mbar_arrive(empty + st);
+    named_bar_sync(1, 256);                    // both are done reading sP / sDS before the next tile rewrites them
+  }
+  store_grad_rows(dk, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 1, true, dQKV);
+  store_grad_rows(dv, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 2, false, dQKV);
+}
+
+__global__ void __launch_bounds__(RING_THREADS, 1)
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
+                   const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
+                   const AttnShape sh) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;                          // 16 KB
+  uint8_t* sDO = sQ + 16384;                   // 16 KB
+  uint8_t* ring = sDO + 16384;                 // STAGES x (K 16 KB, V 16 KB)
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + DQ_STAGES * 32768);
+  uint64_t* empty = full + DQ_STAGES;
+  uint64_t* bar_q = empty + DQ_STAGES;
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
+  const int qt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
+  const int q0 = qt * 128, row_base = c * sh.N, nk = (sh.N + 127) >> 7;
+  const int n_wg = (q0 + 64 < sh.N) ? 2 : 1;   // consumer warpgroups with at least one query row of the crop
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    tma_prefetch_desc(&tmDO);
+    for (int st = 0; st < DQ_STAGES; ++st) {
+      mbar_init(full + st, 1);
+      mbar_init(empty + st, 4 * n_wg);
+    }
+    mbar_init(bar_q, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 288 && elect_one()) {
+      mbar_expect_tx(bar_q, 32768);
+      tma_load_2d(&tmQKV, bar_q, sQ, h * 64, row_base + q0);
+      tma_load_2d(&tmDO, bar_q, sDO, h * 64, row_base + q0);
+      for (int kt = 0; kt < nk; ++kt) {
+        const int st = kt % DQ_STAGES, u = kt / DQ_STAGES;
+        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
+        mbar_expect_tx(full + st, 32768);
+        tma_load_2d(&tmQKV, full + st, ring + st * 32768, sh.D + h * 64, row_base + kt * 128);
+        tma_load_2d(&tmQKV, full + st, ring + st * 32768 + 16384, 2 * sh.D + h * 64, row_base + kt * 128);
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int wq0 = q0 + wg * 64;
+  if (wq0 >= sh.N) return;                     // not counted by the empty barriers (n_wg)
+  mbar_wait(bar_q, 0);
+  float dq[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+#pragma unroll 1
+  for (int kt = 0; kt < nk; ++kt) {
+    const int st = kt % DQ_STAGES;
+    const uint8_t* sK = ring + st * 32768;
+    mbar_wait(full + st, (kt / DQ_STAGES) & 1);
+    float s[64], dp[64];
+    p_ds_tile(sh, LSE, Delta, c, h, wq0, kt, sQ + wg * 8192, sDO + wg * 8192, sK, sK + 16384, r_in, c2, s, dp);
+    dq_mma(dq, dp, sK);
+    if (lane_id() == 0) mbar_arrive(empty + st);
+  }
+  store_grad_rows(dq, sh, c, row_base, wq0, r_in, c2, h, 0, true, dQKV);
 }
 
 static int make_map(CUtensorMap* map, const void* ptr, long rows, int cols, int ld, int box_rows) {
@@ -420,16 +711,31 @@ static int make_map(CUtensorMap* map, const void* ptr, long rows, int cols, int 
   return encode_tensor_map_2d_bf16(map, ptr, dims, strides, box, estr);
 }
 
+// Largest crop the attention entry points take.  The streamed kernels need no resource that grows with N; the bound keeps
+// every token coordinate (crop * N + token, TMA row coordinates and kernel offsets are 32-bit) and the grid inside what
+// is checked below.  It covers a 2 880^2 crop at patch 16 with 5 prefix tokens (32 405 tokens).
+constexpr int ATTN_MAX_TOKENS = 32768;
+constexpr int ATTN_FWD_RESIDENT_SPAN = 448;   // attn_fwd_kernel: Q and all of K / V of a crop group in shared memory
+constexpr int ATTN_BWD_RESIDENT_N = 384;      // attn_bwd_kernel: every Q / dO tile of a crop in shared memory
+
 static int attn_shape(AttnShape* s, int n_crops, int N, int D, int H) {
   if (D != H * 64) return set_error(D3_ERR_ARG, "attention: head_dim must be 64");
   if (N <= 0 || n_crops <= 0) return set_error(D3_ERR_ARG, "attention: empty problem");
+  if (N > ATTN_MAX_TOKENS) return set_error(D3_ERR_ARG, "attention: N > 32768 tokens per crop");
+  if ((long)n_crops * N > INT_MAX) return set_error(D3_ERR_ARG, "attention: n_crops * N must be below 2^31 token rows");
   s->N = N; s->D = D; s->H = H; s->scale = 0.125f; s->n_crops = n_crops;
   s->sin_t = nullptr; s->cos_t = nullptr; s->prefix = 0;
   s->G = (N <= 64) ? (128 / N) : 1;                 // short crops: several per 128-row tile, block-diagonal mask
   if (s->G > n_crops) s->G = n_crops;
   s->span = s->G * N;
   s->nkb = (s->span + 63) / 64;
-  if (s->span > 448) return set_error(D3_ERR_ARG, "attention: N > 448 tokens per crop not supported by the single-pass kernel");
+  return D3_OK;
+}
+
+// grid of the streamed kernels: (128-row tiles, head, crop); G = 1 there
+static int stream_grid(const AttnShape& s, dim3* grid) {
+  if (s.H > 65535 || s.n_crops > 65535) return set_error(D3_ERR_ARG, "attention: H and n_crops must be <= 65535 for long crops");
+  *grid = dim3((s.N + 127) / 128, s.H, s.n_crops);
   return D3_OK;
 }
 
@@ -449,6 +755,22 @@ int d3_attn_fwd(const void* qkv, void* o, float* lse, int n_crops, int N, int D,
   int rc = attn_shape(&s, n_crops, N, D, H);
   if (rc) return rc;
   const long T = (long)n_crops * N;
+  if (s.span > ATTN_FWD_RESIDENT_SPAN) {
+    dim3 grid;
+    if ((rc = stream_grid(s, &grid))) return rc;
+    CUtensorMap tqkv;
+    if ((rc = make_map(&tqkv, qkv, T, 3 * D, 3 * D, 128))) return rc;
+    const int smem = 16384 + FWD_STAGES * 32768 + (2 * FWD_STAGES + 1) * 8 + 1024;
+    static bool cfg_stream = false;
+    if (!cfg_stream) {
+      cudaFuncSetAttribute(attn_fwd_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      cfg_stream = true;
+    }
+    attn_fwd_stream_kernel<<<grid, RING_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(tqkv, (__nv_bfloat16*)o,
+                                                                                                 lse, s);
+    D3_CHECK_LAUNCH();
+    return D3_OK;
+  }
   CUtensorMap tq, tkv;
   if ((rc = make_map(&tq, qkv, T, 3 * D, 3 * D, 128))) return rc;
   if ((rc = make_map(&tkv, qkv, T, 3 * D, 3 * D, 64))) return rc;
@@ -467,9 +789,11 @@ int d3_attn_bwd(const void* qkv, const void* o, const void* d_o, const float* ls
   AttnShape s;
   int rc = attn_shape(&s, n_crops, N, D, H);
   if (rc) return rc;
-  if (N > 384) return set_error(D3_ERR_ARG, "d3_attn_bwd: N > 384 tokens per crop not supported (3 query tiles of 128)");
   if ((rope_sin == nullptr) != (rope_cos == nullptr)) return set_error(D3_ERR_ARG, "d3_attn_bwd: sin/cos tables");
   if (!delta_scratch) return set_error(D3_ERR_ARG, "d3_attn_bwd: delta scratch buffer");
+  const bool streamed = N > ATTN_BWD_RESIDENT_N;
+  dim3 sgrid;
+  if (streamed && (rc = stream_grid(s, &sgrid))) return rc;
   s.sin_t = rope_sin; s.cos_t = rope_cos; s.prefix = rope_prefix;
   const long T = (long)n_crops * N;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -480,6 +804,22 @@ int d3_attn_bwd(const void* qkv, const void* o, const void* d_o, const float* ls
   CUtensorMap tqkv, tdo;
   if ((rc = make_map(&tqkv, qkv, T, 3 * D, 3 * D, 128))) return rc;
   if ((rc = make_map(&tdo, d_o, T, D, D, 128))) return rc;
+  if (streamed) {
+    const int smem_kv = 16384 * 2 + 32768 * 2 + DKDV_STAGES * 32768 + (2 * DKDV_STAGES + 1) * 8 + 1024;
+    const int smem_q = 16384 * 2 + DQ_STAGES * 32768 + (2 * DQ_STAGES + 1) * 8 + 1024;
+    static bool cfg_stream = false;
+    if (!cfg_stream) {
+      cudaFuncSetAttribute(attn_bwd_dkdv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_kv);
+      cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_q);
+      cfg_stream = true;
+    }
+    // key tiles and query tiles are both (N + 127) / 128: the same grid shape for the two kernels
+    attn_bwd_dkdv_kernel<<<sgrid, RING_THREADS, smem_kv, st>>>(tqkv, tdo, lse, delta_scratch, (__nv_bfloat16*)dqkv, s);
+    D3_CHECK_LAUNCH();
+    attn_bwd_dq_kernel<<<sgrid, RING_THREADS, smem_q, st>>>(tqkv, tdo, lse, delta_scratch, (__nv_bfloat16*)dqkv, s);
+    D3_CHECK_LAUNCH();
+    return D3_OK;
+  }
   static bool cfg = false;
   if (!cfg) { cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024); cfg = true; }
   const int nq = (s.span + 127) / 128;

@@ -1,6 +1,8 @@
-"""Isolated timing of the attention kernels at the ViT-L/16 B=64 shapes of the headline step (CUDA events, 20 launches
-after 3 warm-ups, inputs larger than L2): python tools/bench_attention.py [fwd|bwd|all]."""
+"""Isolated timing of the attention kernels at the ViT-L/16 B=64 shapes of the headline step, then at the long crops
+of the high-resolution recipes (streamed kernels), all at ViT-L heads (CUDA events, 20 launches after 3 warm-ups, inputs
+larger than L2): python tools/bench_attention.py [fwd|bwd|all]."""
 import os
+import subprocess
 import sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -27,7 +29,21 @@ def timeit(fn, n=20, warm=3):
     return e0.elapsed_time(e1) / n * 1e3     # us
 
 
-for name, n, N in (("global 128 crops x 197", 128, 197), ("local 512 crops x 37", 512, 37)):
+def card():
+    """Card name and power limit, read in the same run as the numbers they belong to."""
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        q = ""
+    return q or f"{torch.cuda.get_device_name(0)}, power limit not read"
+
+
+print(card())
+SHORT = (("global 128 crops x 197", 128, 197, True), ("local 512 crops x 37", 512, 37, True))
+LONG = (("512^2 16 crops x 1029", 16, 1029, True), ("768^2 16 crops x 2309", 16, 2309, True),
+        ("gram 1152^2 8 crops x 5189", 8, 5189, False))        # B = 8 global crops, 4 storage tokens
+for name, n, N, with_bwd in SHORT + LONG:
     T = n * N
     qkv = torch.randn(T, 3 * D, device="cuda").to(bf)
     o = torch.empty(T, D, device="cuda", dtype=bf)
@@ -37,7 +53,7 @@ for name, n, N in (("global 128 crops x 197", 128, 197), ("local 512 crops x 37"
         us = timeit(lambda: ops.attn_fwd(qkv, o, lse, n, N, D, H))
         byt = T * 3 * D * 2 + T * D * 2
         print(f"fwd {name}: {us:8.1f} us  {flops / us / 1e6:7.1f} TFLOP/s  {byt / us / 1e3:7.1f} GB/s (algorithmic qkv in + o out)")
-    if what in ("bwd", "all"):
+    if what in ("bwd", "all") and with_bwd:
         ops.attn_fwd(qkv, o, lse, n, N, D, H)
         do = torch.randn(T, D, device="cuda").to(bf)
         dqkv = torch.empty(T, 3 * D, device="cuda", dtype=bf)
