@@ -22,9 +22,10 @@
 // phase parity could not tell apart).  The main loop of one tile so has the whole ring in flight.
 //
 // The epilogue flags are a template parameter.  The flag sets one training step issues are compiled with their flags
-// fixed (dispatch() lists them): bias and gamma are staged in shared memory by cp.async during the main loop, and each
-// thread issues all loads of a row before the row's first store.  Every other call (fused reduce-scatter, misaligned
-// operands, odd N, other flag sets) runs the same kernel with the flags read at run time (EPI_RUNTIME).
+// fixed (dispatch() lists them): bias and gamma are staged in shared memory by cp.async during the main loop, each
+// thread issues all loads of a chunk before its first store, and the results go through a shared-memory staging area
+// to TMA stores (all but the weight gradients', which store from registers).  Every other call (fused reduce-scatter,
+// misaligned operands, odd N, other flag sets) runs the same kernel with the flags read at run time (EPI_RUNTIME).
 #include <cstdlib>
 #include <cstring>
 #include "ptx.cuh"
@@ -208,16 +209,125 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, float (&ac
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-template <int BN>
+// The same epilogue, stored through shared memory with TMA (the flag sets of kStaged below).  Storing from the
+// accumulator fragment, a warp's store covers 8 rows x 16 B (bf16); through TMA the tile leaves in whole lines.  The
+// tile is cut into 64 x 64 chunks (a 64-row half by 64 columns); a chunk's outputs are 64-row boxes of 128 B rows
+// (64 bf16 or 32 fp32 columns) in SWIZZLE_128B layout, so the fragment's st.shared of 8 consecutive rows hit 8
+// different 16-byte bank groups.  The consumer's staging area holds NBUF chunks in a ring; thread 0 of the consumer
+// commits one bulk group per chunk and, before a chunk is written, waits until the group that last read its buffer is
+// done.  The chunk's loads are issued before that wait, so a `resid` that aliases `out` is read before it is stored.
+// TMA clips rows >= M and columns >= N.
+constexpr int STG_BOX = 64 * 128;
+constexpr int STG_BYTES = 3 * STG_BOX;    // per consumer
+__device__ __forceinline__ uint32_t sw128(int r, int byte) {
+  return r * 128 + ((((byte >> 4) ^ r) & 7) << 4) + (byte & 15);
+}
+
+template <int BN, int EF>
+__device__ __forceinline__ void epilogue_tile_staged(const GemmEpilogue& ep, const CUtensorMap* tm_out,
+                                                     const CUtensorMap* tm_pre, float (&acc)[2][BN / 2],
+                                                     const float* s_bias, const float* s_gamma, uint8_t* stg,
+                                                     int& seq, int bar, int t, int m0, int n0, int M, int N, int r_in,
+                                                     int c_in) {
+  constexpr bool F32 = (EF & EP_OUT_F32) != 0;
+  constexpr int OUT_BOXES = F32 ? 2 : 1;
+  constexpr int CHUNK = (OUT_BOXES + ((EF & EP_STORE_PRE) ? 1 : 0)) * STG_BOX;
+  constexpr int NBUF = STG_BYTES / CHUNK;
+  static_assert(NBUF >= 1, "a chunk must fit the staging area");
+  static_assert((EF & (EP_ACCUM | EP_SLABS)) == 0, "ACCUM and split-K slabs store from registers");
+#pragma unroll
+  for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+    for (int cb = 0; cb < BN / 64; ++cb) {
+      const int row0 = m0 + mh * 64, col0 = n0 + cb * 64;
+      if (row0 >= M || col0 >= N) continue;   // uniform over the warpgroup
+      float2 xr[2][8];
+      uint32_t xu[2][8];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const size_t row = (size_t)row0 + r_in + 8 * h;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int n = col0 + 8 * i + c_in;
+          if (row < (size_t)M && n < N) {
+            if constexpr ((EF & EP_RESID) != 0)
+              xr[h][i] = *reinterpret_cast<const float2*>(ep.resid + row * ep.ld_resid + n);
+            if constexpr ((EF & EP_MUL_DGELU) != 0)
+              xu[h][i] = *reinterpret_cast<const uint32_t*>(ep.aux_in + row * ep.ld_aux + n);
+          }
+        }
+      }
+      uint8_t* const buf = stg + (seq % NBUF) * CHUNK;
+      if (t == 0) tma_store_wait_read<NBUF - 1>();   // the group that last read `buf` is done
+      named_bar_sync(bar, 128);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r_in + 8 * h;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int cl = cb * 64 + 8 * i + c_in;   // column within the tile
+          float v0 = __fmul_rn(acc[mh][4 * (cl >> 3) + 2 * h], ep.alpha);
+          float v1 = __fmul_rn(acc[mh][4 * (cl >> 3) + 2 * h + 1], ep.alpha);
+          if constexpr ((EF & EP_BIAS) != 0) {
+            const float2 b = *reinterpret_cast<const float2*>(s_bias + cl);
+            v0 = __fadd_rn(v0, b.x); v1 = __fadd_rn(v1, b.y);
+          }
+          if constexpr ((EF & EP_STORE_PRE) != 0)
+            *reinterpret_cast<uint32_t*>(buf + OUT_BOXES * STG_BOX + sw128(r, 16 * i + 2 * c_in)) = pack_bf16(v0, v1);
+          if constexpr ((EF & EP_GELU) != 0) {
+            v0 = gelu_tanh_fast(v0); v1 = gelu_tanh_fast(v1);
+          }
+          if constexpr ((EF & EP_MUL_DGELU) != 0) {
+            const float2 u = unpack_bf16(xu[h][i]);
+            v0 = __fmul_rn(v0, gelu_grad_epi(u.x)); v1 = __fmul_rn(v1, gelu_grad_epi(u.y));
+          }
+          if constexpr ((EF & EP_GAMMA) != 0) {
+            const float2 g = *reinterpret_cast<const float2*>(s_gamma + cl);
+            v0 = __fmul_rn(v0, g.x); v1 = __fmul_rn(v1, g.y);
+          }
+          if constexpr ((EF & EP_RESID) != 0) {
+            v0 = __fadd_rn(v0, xr[h][i].x); v1 = __fadd_rn(v1, xr[h][i].y);
+          }
+          if constexpr (F32) {
+            *reinterpret_cast<float2*>(buf + (i >> 2) * STG_BOX + sw128(r, 32 * (i & 3) + 4 * c_in)) =
+                make_float2(v0, v1);
+          } else {
+            *reinterpret_cast<uint32_t*>(buf + sw128(r, 16 * i + 2 * c_in)) = pack_bf16(v0, v1);
+          }
+        }
+      }
+      fence_proxy_async_smem();                // the writes above are visible to the TMA (async proxy)
+      named_bar_sync(bar, 128);
+      if (t == 0) {
+        tma_store_2d(tm_out, buf, col0, row0);
+        if (F32 && col0 + 32 < N) tma_store_2d(tm_out, buf + STG_BOX, col0 + 32, row0);
+        if constexpr ((EF & EP_STORE_PRE) != 0) tma_store_2d(tm_pre, buf + OUT_BOXES * STG_BOX, col0, row0);
+        tma_store_commit();
+      }
+      ++seq;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// STAGED: the epilogue stores through shared memory, which takes one ring stage's worth of space (227 KB in all)
+template <int BN, bool STAGED>
 struct Cfg {
-  static constexpr int STAGES = BN == 128 ? 6 : 8;
+  static constexpr int STAGES = (BN == 128 ? 6 : 8) - (STAGED ? 1 : 0);
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int BAR_BYTES = 256;                       // full and empty mbarriers
   static constexpr int VEC_BYTES = 2 * 2 * BN * 4;            // per consumer: bias and gamma of its tile (fp32)
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + VEC_BYTES + 1024;
+  static constexpr int VEC_END = STAGES * STAGE_BYTES + BAR_BYTES + VEC_BYTES;
+  static constexpr int STG_OFF = (VEC_END + 1023) / 1024 * 1024;   // SWIZZLE_128B staging: 1024-byte aligned
+  static constexpr int SMEM_BYTES = (STAGED ? STG_OFF + 2 * STG_BYTES : VEC_END) + 1024;
+  static_assert(SMEM_BYTES <= 227 * 1024, "over the opt-in shared-memory limit");
 };
+
+// The epilogue stores through shared memory: every fixed flag set but the weight gradients' (split-K slabs, ACCUM),
+// whose main loop runs over all tokens and so hides a register-store epilogue, and which keep the deeper ring.
+template <int EF>
+constexpr bool kStaged = EF != EPI_RUNTIME && (EF & (EP_SLABS | EP_ACCUM)) == 0;
 
 // work item = (tile, split): k-blocks [kb0, kb1)
 struct WorkRange { int m0, n0, kb0, kb1; };
@@ -254,9 +364,11 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint32_t sa,
 
 template <int BN, int A_MN, int B_MN, int EF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmEpilogue ep,
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmP, const GemmEpilogue ep,
             int M, int N, int K, int splits) {
-  using C = Cfg<BN>;
+  constexpr bool staged = kStaged<EF>;   // tmO / tmP (out, pre-activation stash) are used only then
+  using C = Cfg<BN, staged>;
   static_assert(2 * C::STAGES * 8 <= C::BAR_BYTES, "mbarriers overflow their slot");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -268,6 +380,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if constexpr (staged) {
+      tma_prefetch_desc(&tmO);
+      if constexpr ((EF & EP_STORE_PRE) != 0) tma_prefetch_desc(&tmP);
+    }
     for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
     fence_mbar_init();
   }
@@ -315,6 +431,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     float* const s_bias = vecs + cw * 2 * BN;
     float* const s_gamma = s_bias + BN;
     constexpr bool stage_vecs = EF != EPI_RUNTIME && (EF & (EP_BIAS | EP_GAMMA)) != 0;
+    uint8_t* const stg = smem + C::STG_OFF + cw * STG_BYTES;   // output staging (staged epilogues only)
+    int stg_seq = 0;                           // chunks this consumer has staged
     int stage = 0;                             // position in the ring, counting the other consumer's k-blocks too
     uint32_t phase = 0;
     int j = 0;
@@ -369,7 +487,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       }
       if (nkb <= 0) continue;                  // empty split-K slice: nothing to add
       const size_t slab_row0 = (EF == EPI_RUNTIME ? (ep.flags & EP_SLABS) : (EF & EP_SLABS)) ? (size_t)(w % splits) * M : 0;
-      if constexpr (EF != EPI_RUNTIME) {
+      if constexpr (staged) {
+        epilogue_tile_staged<BN, EF>(ep, &tmO, &tmP, acc, s_bias, s_gamma, stg, stg_seq, 5 + cw, t, wr.m0, wr.n0, M, N,
+                                     r_in, c_in);
+      } else if constexpr (EF != EPI_RUNTIME) {
         epilogue_tile<BN, EF>(ep, acc, s_bias, s_gamma, wr.m0, wr.n0, M, N, slab_row0, r_in, c_in);
       } else {
         const bool fast = (ep.flags & EP_SLOW) == 0;
@@ -389,6 +510,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           }
       }
     }
+    if (staged && t == 0) tma_store_wait_all();   // shared memory stays valid until the last store has read it
   }
 }
 
@@ -410,7 +532,7 @@ static int make_operand_map(CUtensorMap* map, const void* ptr, int mn, int k, in
 template <int BN, int A_MN, int B_MN, int EF>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M, int N, int K,
                   int splits, cudaStream_t stream) {
-  using C = Cfg<BN>;
+  using C = Cfg<BN, kStaged<EF>>;
   auto kern = gemm_kernel<BN, A_MN, B_MN, EF>;
   static bool configured = false;
   if (!configured) {
@@ -418,9 +540,21 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilog
     if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
     configured = true;
   }
+  // output maps of the staged epilogue: the logical [M, N] with the real leading dimension, so TMA clips ragged rows
+  // and columns (gemm_bf16's alignment checks already meet TMA's 16-byte address and stride rules)
+  CUtensorMap to{}, tp{};
+  if constexpr (kStaged<EF>) {
+    const int elt = (EF & EP_OUT_F32) ? 4 : 2;
+    int rc = encode_tensor_map_2d(&to, ep.out, elt, N, M, (cuuint64_t)ep.ld_out * elt, 128 / elt, 64, 128);
+    if (rc) return rc;
+    if constexpr ((EF & EP_STORE_PRE) != 0) {
+      rc = encode_tensor_map_2d(&tp, ep.aux_out, 2, N, M, (cuuint64_t)ep.ld_aux * 2, 64, 64, 128);
+      if (rc) return rc;
+    }
+  }
   const int work = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * splits;
   const int grid = work < sm_count() ? work : sm_count();
-  kern<<<grid, GEMM_THREADS, C::SMEM_BYTES, stream>>>(ta, tb, ep, M, N, K, splits);
+  kern<<<grid, GEMM_THREADS, C::SMEM_BYTES, stream>>>(ta, tb, to, tp, ep, M, N, K, splits);
   cudaError_t e = cudaPeekAtLastError();
   if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
   count_launch();

@@ -91,9 +91,9 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
                : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
+// the committing thread's bulk groups: at most N still reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // plain (this-CTA) tiled load, usable inside a cluster launch as well
 __device__ __forceinline__ void tma_load_2d_cta(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {

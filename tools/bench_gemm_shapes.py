@@ -1,5 +1,5 @@
 """GPU microbench: every GEMM call shape of one ViT-L/16 B=64 training step, with its real epilogue, timed in isolation."""
-import os, sys
+import os, subprocess, sys
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200"))
 import torch
@@ -9,6 +9,16 @@ dev = "cuda"
 bf, f32 = torch.bfloat16, torch.float32
 D, Hd = 1024, 4096
 Tt, Ts = 25216, 44160
+
+
+def card():
+    """Card name and power limit, read in the same run as the numbers they belong to."""
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        q = ""
+    return q or f"{torch.cuda.get_device_name(0)}, power limit not read"
 
 
 def timeit(fn, iters=8):
@@ -57,6 +67,7 @@ def run(tile_n=0, only=None):
 
 
 if __name__ == "__main__":
+    print(card())
     print(f"== student stream T={Ts}, tile_n auto"); run(0)
     if len(sys.argv) > 1:
         for bn in (128, 256):
