@@ -20,9 +20,7 @@ enum : int {
   EP_ACCUM = D3_EP_ACCUM,
   EP_SCATTER = D3_EP_SCATTER,
   EP_SLOW = 1 << 30,      // internal: force the bounds-checked scalar epilogue
-  EP_ATOMIC = 1 << 29,    // internal: EP_SCATTER contributions, fp32 atomic adds into the owners' shards
   EP_SLABS = 1 << 27,     // internal: split-K slice s stores its partial tile at rows [s*M, s*M + M) of `out`
-  EP_FAST_ACT = 1 << 28,  // internal: hardware tanh in GELU / GELU' (bf16-rounded outputs)
 };
 
 struct GemmEpilogue {

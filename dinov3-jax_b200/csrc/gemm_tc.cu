@@ -13,19 +13,20 @@
 //   warpgroup 0      TMA producer (one elected thread): A and B k-blocks of 64, tile after tile of this CTA's work
 //                    list, into one shared-memory ring;
 //   warpgroups 1, 2  consumers in ping-pong: the CTA's tiles alternate between them, so one warpgroup's epilogue
-//                    (straight from its accumulator registers) runs under the other's main loop.  A tile is two
-//                    m64nBNk16 wgmma chains (rows 0-63 / 64-127) over SWIZZLE_128B operands, K-major or MN-major through
-//                    the descriptor transpose bits.
+//                    runs under the other's main loop.  A tile is two m64nBNk16 wgmma chains (rows 0-63 / 64-127)
+//                    over SWIZZLE_128B operands, K-major or MN-major through the descriptor transpose bits.
 // Both consumers walk the whole ring in fill order, stepping over the other's k-blocks.  The main loops take turns: a
 // consumer starts its main loop only after the other has passed its last full-barrier wait (named barriers 1 / 2), so
 // every fill of a stage is waited on by exactly one consumer, in order, and no wait can be two phases ahead (which the
 // phase parity could not tell apart).  The main loop of one tile so has the whole ring in flight.
 //
-// The epilogue flags are a template parameter.  The flag sets one training step issues are compiled with their flags
-// fixed (dispatch() lists them): bias and gamma are staged in shared memory by cp.async during the main loop, each
-// thread issues all loads of a chunk before its first store, and the results go through a shared-memory staging area
-// to TMA stores (all but the weight gradients', which store from registers).  Every other call (fused reduce-scatter,
-// misaligned operands, odd N, other flag sets) runs the same kernel with the flags read at run time (EPI_RUNTIME).
+// The epilogue's arithmetic is one function, epi_value (one element, accumulator to stored value), under two tile
+// walkers.  The epilogue flags are a template parameter.  The flag sets one training step issues are compiled with
+// their flags fixed (dispatch() lists them) and run epilogue_tile: bias and gamma are staged in shared memory by
+// cp.async during the main loop, each thread issues all loads of a 64 x 64 chunk before its first store, and the
+// results go through a shared-memory staging area to TMA stores (all but the weight gradients', which store from
+// registers).  Every other call (fused reduce-scatter, misaligned operands, odd N, other flag sets) runs the same
+// kernel with the flags read at run time (EPI_RUNTIME) and epilogue_tile_runtime, which loads per column pair.
 #include <cstdlib>
 #include <cstring>
 #include "ptx.cuh"
@@ -38,9 +39,28 @@ constexpr int BK = 64;
 constexpr int GEMM_THREADS = 384;
 
 // ---------------------------------------------------------------------------------------------------------------
+// Epilogue.  epi_value takes one element from the fp32 accumulator to the value stored; the two tile walkers below
+// load its operands and store its results, and repeat none of its steps.  Every step is rounded on its own
+// (__fmul_rn / __fadd_rn, GELU' spelled out in gelu_grad_epi), so no FMA contraction depends on the code around it and
+// a fixed flag set gives the bits of the run-time flags.
+constexpr int EPI_RUNTIME = -1;
+constexpr int EPI_FLAGS = EP_BIAS | EP_GELU | EP_STORE_PRE | EP_MUL_DGELU | EP_GAMMA | EP_RESID | EP_OUT_F32 | EP_ACCUM |
+                          EP_SLABS;
+
+// The epilogue stores through shared memory: every fixed flag set but the weight gradients' (split-K slabs, ACCUM),
+// whose main loop runs over all tokens and so hides a register-store epilogue, and which keep the deeper ring.
+template <int EF>
+constexpr bool kStaged = EF != EPI_RUNTIME && (EF & (EP_SLABS | EP_ACCUM)) == 0;
+
+// flag f: a compile-time constant for a fixed flag set EF, read from ep.flags for EPI_RUNTIME
+template <int EF>
+__device__ __forceinline__ bool epi_has(const GemmEpilogue& ep, int f) {
+  return EF == EPI_RUNTIME ? (ep.flags & f) != 0 : (EF & f) != 0;
+}
+
 // gelu_tanh_grad_fast with every rounding step written out.  Its last add has a product on both sides, and which one
 // the compiler contracts into an FMA depends on the surrounding code; fixing it to fma(0.5u (1 - t^2), dz, 0.5 (1 + t))
-// makes every epilogue variant give the same bits.
+// makes the result independent of the code it is inlined into.
 __device__ __forceinline__ float gelu_grad_epi(float u) {
   const float u2 = __fmul_rn(u, u);
   const float t = tanh_approx(__fmul_rn(u, fmaf(0.0356774081363001f, u2, 0.7978845608028654f)));
@@ -48,175 +68,114 @@ __device__ __forceinline__ float gelu_grad_epi(float u) {
   return fmaf(__fmul_rn(__fmul_rn(0.5f, u), fmaf(-t, t, 1.0f)), dz, __fmul_rn(0.5f, __fadd_rn(1.0f, t)));
 }
 
-// epilogue for two adjacent columns (n, n+1) of one row; `vec`: both columns in range and every operand 16-byte
-// aligned with even leading dimensions (vector loads / stores of pairs)
-__device__ __forceinline__ void epilogue_pair(const GemmEpilogue& ep, size_t row, int n, int N, float v0, float v1,
-                                              bool vec) {
-  v0 *= ep.alpha;
-  v1 *= ep.alpha;
-  if (ep.flags & EP_SCATTER) {  // fused reduce-scatter: add into the owning rank's shard slice (NVLink peer mapping)
-    const unsigned long long g = (unsigned long long)ep.sc_off + row * ep.ld_out + n;
-    const unsigned long long shard = (unsigned long long)ep.sc_shard;
-    if (n + 1 < N) {                                         // a pair never straddles two owners (shard % 4 == 0)
-      const unsigned r = (unsigned)(g / shard);
-      float* dst = ep.sc_peer[r] + (g - r * shard);
-      if (ep.sc_sys) {
-        atomicAdd_system(dst, v0); atomicAdd_system(dst + 1, v1);
-      } else {
-        atomicAdd(reinterpret_cast<float2*>(dst), make_float2(v0, v1));
-      }
-    } else if (n < N) {
-      const unsigned r = (unsigned)(g / shard);
-      atomicAdd(ep.sc_peer[r] + (g - r * shard), v0);
-    }
-    return;
-  }
-  const bool fast_act = (ep.flags & EP_FAST_ACT) != 0;
+// alpha, bias, GELU, GELU' (of the bf16 pre-activation u), gamma, residual, accumulate (old: the fp32 `out`), in this
+// order; the operands of flags that are not set are ignored.  `pre` receives the value before the activation
+// (EP_STORE_PRE).  GELU and GELU' use the hardware tanh (rel. error 2^-11, below the bf16 rounding of the GEMM operands).
+template <int EF>
+__device__ __forceinline__ float epi_value(const GemmEpilogue& ep, float acc, float bias, float u, float gamma,
+                                           float resid, float old, float& pre) {
+  float v = __fmul_rn(acc, ep.alpha);
+  if (epi_has<EF>(ep, EP_BIAS)) v = __fadd_rn(v, bias);
+  pre = v;
+  if (epi_has<EF>(ep, EP_GELU)) v = gelu_tanh_fast(v);
+  if (epi_has<EF>(ep, EP_MUL_DGELU)) v = __fmul_rn(v, gelu_grad_epi(u));
+  if (epi_has<EF>(ep, EP_GAMMA)) v = __fmul_rn(v, gamma);
+  if (epi_has<EF>(ep, EP_RESID)) v = __fadd_rn(v, resid);
+  if (epi_has<EF>(ep, EP_ACCUM)) v = __fadd_rn(v, old);
+  return v;
+}
+
+// Columns (n, n + 1) of one row: one access of the pair when `vec`, else scalar accesses of the columns in range
+// (`two`: n + 1 < N).
+__device__ __forceinline__ float2 ld_pair(const float* p, bool vec, bool two) {
+  if (vec) return *reinterpret_cast<const float2*>(p);
+  return make_float2(p[0], two ? p[1] : 0.f);
+}
+__device__ __forceinline__ float2 ld_pair(const __nv_bfloat16* p, bool vec, bool two) {
+  if (vec) return unpack_bf16(*reinterpret_cast<const uint32_t*>(p));
+  return make_float2(__bfloat162float(p[0]), two ? __bfloat162float(p[1]) : 0.f);
+}
+__device__ __forceinline__ void st_pair(float* p, float a, float b, bool vec, bool two) {
   if (vec) {
-    if (ep.flags & EP_BIAS) {
-      const float2 b = *reinterpret_cast<const float2*>(ep.bias + n);
-      v0 += b.x; v1 += b.y;
-    }
-    if (ep.flags & EP_STORE_PRE) *reinterpret_cast<uint32_t*>(ep.aux_out + row * ep.ld_aux + n) = pack_bf16(v0, v1);
-    if (ep.flags & EP_GELU) {
-      v0 = fast_act ? gelu_tanh_fast(v0) : gelu_tanh(v0);
-      v1 = fast_act ? gelu_tanh_fast(v1) : gelu_tanh(v1);
-    }
-    if (ep.flags & EP_MUL_DGELU) {
-      const float2 u = unpack_bf16(*reinterpret_cast<const uint32_t*>(ep.aux_in + row * ep.ld_aux + n));
-      v0 *= fast_act ? gelu_grad_epi(u.x) : gelu_tanh_grad(u.x);
-      v1 *= fast_act ? gelu_grad_epi(u.y) : gelu_tanh_grad(u.y);
-    }
-    if (ep.flags & EP_GAMMA) {
-      const float2 g = *reinterpret_cast<const float2*>(ep.gamma + n);
-      v0 *= g.x; v1 *= g.y;
-    }
-    if (ep.flags & EP_RESID) {
-      const float2 x = *reinterpret_cast<const float2*>(ep.resid + row * ep.ld_resid + n);
-      v0 += x.x; v1 += x.y;
-    }
-    if (ep.flags & EP_OUT_F32) {
-      float2* dst = reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.out) + row * ep.ld_out + n);
-      if (ep.flags & EP_ACCUM) {
-        const float2 x = *dst;
-        v0 += x.x; v1 += x.y;
-      }
-      *dst = make_float2(v0, v1);
-    } else {
-      *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + row * ep.ld_out + n) = pack_bf16(v0, v1);
-    }
-    return;
+    *reinterpret_cast<float2*>(p) = make_float2(a, b);
+  } else {
+    p[0] = a;
+    if (two) p[1] = b;
   }
-  // ragged / unaligned edge: scalar path with bounds checks
-#pragma unroll 1
-  for (int j = 0; j < 2; ++j) {
-    const int c = n + j;
-    if (c >= N) break;
-    float x = j ? v1 : v0;
-    if (ep.flags & EP_BIAS) x += ep.bias[c];
-    if (ep.flags & EP_STORE_PRE) ep.aux_out[row * ep.ld_aux + c] = __float2bfloat16(x);
-    if (ep.flags & EP_GELU) x = fast_act ? gelu_tanh_fast(x) : gelu_tanh(x);
-    if (ep.flags & EP_MUL_DGELU) {
-      const float u = __bfloat162float(ep.aux_in[row * ep.ld_aux + c]);
-      x *= fast_act ? gelu_grad_epi(u) : gelu_tanh_grad(u);
-    }
-    if (ep.flags & EP_GAMMA) x *= ep.gamma[c];
-    if (ep.flags & EP_RESID) x += ep.resid[row * ep.ld_resid + c];
-    if (ep.flags & EP_OUT_F32) {
-      float* o = reinterpret_cast<float*>(ep.out) + row * ep.ld_out + c;
-      if (ep.flags & EP_ACCUM) x += *o;
-      *o = x;
-    } else {
-      reinterpret_cast<__nv_bfloat16*>(ep.out)[row * ep.ld_out + c] = __float2bfloat16(x);
-    }
+}
+__device__ __forceinline__ void st_pair(__nv_bfloat16* p, float a, float b, bool vec, bool two) {
+  if (vec) {
+    *reinterpret_cast<uint32_t*>(p) = pack_bf16(a, b);
+  } else {
+    p[0] = __float2bfloat16(a);
+    if (two) p[1] = __float2bfloat16(b);
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Epilogue with the flags EF fixed at compile time, for a call that passed gemm_bf16's alignment checks and has an even
-// N (a column pair is in range as a whole, and every access is a vector one).  The fp32 operations are those of
-// epilogue_pair in the same order, none contracted into an FMA, so both paths give the same bits.  A thread issues
-// every load of one row before the row's first store: it waits on memory once per row, not once per column pair.
-// `resid` may alias `out`: each element is read before it is written, by the same thread.
-constexpr int EPI_RUNTIME = -1;
-constexpr int EPI_FLAGS = EP_BIAS | EP_GELU | EP_STORE_PRE | EP_MUL_DGELU | EP_GAMMA | EP_RESID | EP_OUT_F32 | EP_ACCUM |
-                          EP_SLABS;
-
-template <int BN, int EF>
-__device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, float (&acc)[2][BN / 2], const float* s_bias,
-                                              const float* s_gamma, int m0, int n0, int M, int N, size_t slab_row0,
-                                              int r_in, int c_in) {
-  constexpr int NP = BN / 8;      // column pairs of one row held by a thread
+// Run-time flags (EPI_RUNTIME): the fused reduce-scatter, operands that fail gemm_bf16's alignment checks, odd N and
+// flag sets not compiled fixed.  Each column pair loads its own operands (prefetching a row's under run-time flags
+// would cost registers), with vector accesses unless EP_SLOW is set or N cuts the pair.
+template <int BN>
+__device__ __forceinline__ void epilogue_tile_runtime(const GemmEpilogue& ep, float (&acc)[2][BN / 2], int m0, int n0,
+                                                      int M, int N, size_t slab_row0, int r_in, int c_in) {
   float* const out_f = reinterpret_cast<float*>(ep.out);
   __nv_bfloat16* const out_h = reinterpret_cast<__nv_bfloat16*>(ep.out);
+  const bool aligned = (ep.flags & EP_SLOW) == 0;
 #pragma unroll
   for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int row = m0 + mh * 64 + r_in + 8 * h;
-      if (row >= M) continue;
+      const size_t row = (size_t)(m0 + mh * 64 + r_in + 8 * h);
+      if (row >= (size_t)M) continue;
       const size_t orow = slab_row0 + row;
-      float2 xr[NP], xo[NP];
-      uint32_t xu[NP];
 #pragma unroll
-      for (int i = 0; i < NP; ++i) {
+      for (int i = 0; i < BN / 8; ++i) {
         const int n = n0 + 8 * i + c_in;
-        if (n < N) {
-          if constexpr ((EF & EP_RESID) != 0)
-            xr[i] = *reinterpret_cast<const float2*>(ep.resid + (size_t)row * ep.ld_resid + n);
-          if constexpr ((EF & EP_MUL_DGELU) != 0)
-            xu[i] = *reinterpret_cast<const uint32_t*>(ep.aux_in + (size_t)row * ep.ld_aux + n);
-          if constexpr ((EF & EP_ACCUM) != 0) xo[i] = *reinterpret_cast<const float2*>(out_f + orow * ep.ld_out + n);
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < NP; ++i) {
-        const int cl = 8 * i + c_in;          // column within the tile
-        const int n = n0 + cl;
-        if (n >= N) continue;
-        float v0 = __fmul_rn(acc[mh][4 * i + 2 * h], ep.alpha);
-        float v1 = __fmul_rn(acc[mh][4 * i + 2 * h + 1], ep.alpha);
-        if constexpr ((EF & EP_BIAS) != 0) {
-          const float2 b = *reinterpret_cast<const float2*>(s_bias + cl);
-          v0 = __fadd_rn(v0, b.x); v1 = __fadd_rn(v1, b.y);
-        }
-        if constexpr ((EF & EP_STORE_PRE) != 0)
-          *reinterpret_cast<uint32_t*>(ep.aux_out + (size_t)row * ep.ld_aux + n) = pack_bf16(v0, v1);
-        if constexpr ((EF & EP_GELU) != 0) {
-          v0 = gelu_tanh_fast(v0); v1 = gelu_tanh_fast(v1);
-        }
-        if constexpr ((EF & EP_MUL_DGELU) != 0) {
-          const float2 u = unpack_bf16(xu[i]);
-          v0 = __fmul_rn(v0, gelu_grad_epi(u.x)); v1 = __fmul_rn(v1, gelu_grad_epi(u.y));
-        }
-        if constexpr ((EF & EP_GAMMA) != 0) {
-          const float2 g = *reinterpret_cast<const float2*>(s_gamma + cl);
-          v0 = __fmul_rn(v0, g.x); v1 = __fmul_rn(v1, g.y);
-        }
-        if constexpr ((EF & EP_RESID) != 0) {
-          v0 = __fadd_rn(v0, xr[i].x); v1 = __fadd_rn(v1, xr[i].y);
-        }
-        if constexpr ((EF & EP_OUT_F32) != 0) {
-          if constexpr ((EF & EP_ACCUM) != 0) {
-            v0 = __fadd_rn(v0, xo[i].x); v1 = __fadd_rn(v1, xo[i].y);
+        if (n >= N) break;
+        const bool two = n + 1 < N, vec = aligned && two;
+        float2 b{}, u{}, g{}, x{}, o{};
+        if (epi_has<EPI_RUNTIME>(ep, EP_BIAS)) b = ld_pair(ep.bias + n, vec, two);
+        if (epi_has<EPI_RUNTIME>(ep, EP_MUL_DGELU)) u = ld_pair(ep.aux_in + row * ep.ld_aux + n, vec, two);
+        if (epi_has<EPI_RUNTIME>(ep, EP_GAMMA)) g = ld_pair(ep.gamma + n, vec, two);
+        if (epi_has<EPI_RUNTIME>(ep, EP_RESID)) x = ld_pair(ep.resid + row * ep.ld_resid + n, vec, two);
+        if (epi_has<EPI_RUNTIME>(ep, EP_ACCUM)) o = ld_pair(out_f + orow * ep.ld_out + n, vec, two);
+        float p0, p1;
+        const float v0 = epi_value<EPI_RUNTIME>(ep, acc[mh][4 * i + 2 * h], b.x, u.x, g.x, x.x, o.x, p0);
+        const float v1 = epi_value<EPI_RUNTIME>(ep, acc[mh][4 * i + 2 * h + 1], b.y, u.y, g.y, x.y, o.y, p1);
+        if (epi_has<EPI_RUNTIME>(ep, EP_SCATTER)) {   // add into the owning rank's shard slice (NVLink peer mapping)
+          const unsigned long long g_idx = (unsigned long long)ep.sc_off + orow * ep.ld_out + n;
+          const unsigned long long shard = (unsigned long long)ep.sc_shard;
+          const unsigned r = (unsigned)(g_idx / shard);   // a pair never straddles two owners (shard % 4 == 0)
+          float* const dst = ep.sc_peer[r] + (g_idx - r * shard);
+          if (!two) {
+            atomicAdd(dst, v0);
+          } else if (ep.sc_sys) {
+            atomicAdd_system(dst, v0); atomicAdd_system(dst + 1, v1);
+          } else {
+            atomicAdd(reinterpret_cast<float2*>(dst), make_float2(v0, v1));
           }
-          *reinterpret_cast<float2*>(out_f + orow * ep.ld_out + n) = make_float2(v0, v1);
-        } else {
-          *reinterpret_cast<uint32_t*>(out_h + orow * ep.ld_out + n) = pack_bf16(v0, v1);
+          continue;
         }
+        if (epi_has<EPI_RUNTIME>(ep, EP_STORE_PRE)) st_pair(ep.aux_out + row * ep.ld_aux + n, p0, p1, vec, two);
+        if (epi_has<EPI_RUNTIME>(ep, EP_OUT_F32)) st_pair(out_f + orow * ep.ld_out + n, v0, v1, vec, two);
+        else st_pair(out_h + orow * ep.ld_out + n, v0, v1, vec, two);
       }
     }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// The same epilogue, stored through shared memory with TMA (the flag sets of kStaged below).  Storing from the
-// accumulator fragment, a warp's store covers 8 rows x 16 B (bf16); through TMA the tile leaves in whole lines.  The
-// tile is cut into 64 x 64 chunks (a 64-row half by 64 columns); a chunk's outputs are 64-row boxes of 128 B rows
-// (64 bf16 or 32 fp32 columns) in SWIZZLE_128B layout, so the fragment's st.shared of 8 consecutive rows hit 8
-// different 16-byte bank groups.  The consumer's staging area holds NBUF chunks in a ring; thread 0 of the consumer
-// commits one bulk group per chunk and, before a chunk is written, waits until the group that last read its buffer is
-// done.  The chunk's loads are issued before that wait, so a `resid` that aliases `out` is read before it is stored.
-// TMA clips rows >= M and columns >= N.
+// Fixed flag sets EF, for a call that passed gemm_bf16's alignment checks and has an even N (a column pair is in range
+// as a whole, and every access is a vector one).  The tile is walked in 64 x 64 chunks (a 64-row half by 64 columns);
+// a thread issues every load of a chunk (`resid`, GELU' input, ACCUM `out`) before the chunk's first store, so it waits
+// on memory once per chunk.  `resid` may alias `out`: each element is read before it is written, by the same thread.
+// Two store back ends:
+//   staged (kStaged<EF>): a chunk's outputs go to shared memory as 64-row boxes of 128 B rows (64 bf16 or 32 fp32
+//     columns) in SWIZZLE_128B layout, so the fragment's st.shared of 8 consecutive rows hit 8 different 16-byte bank
+//     groups, and leave by TMA in whole lines (from the fragment, a warp's store covers 8 rows x 16 B).  The
+//     consumer's staging area holds NBUF chunks in a ring; thread 0 of the consumer commits one bulk group per chunk
+//     and, after the chunk's loads are issued and before the chunk is written, waits until the group that last read
+//     its buffer is done.  TMA clips rows >= M and columns >= N.
+//   registers (the weight gradients): st.global from the fragment; split-K slab s at rows [s*M, s*M + M) of `out`.
 constexpr int STG_BOX = 64 * 128;
 constexpr int STG_BYTES = 3 * STG_BOX;    // per consumer
 __device__ __forceinline__ uint32_t sw128(int r, int byte) {
@@ -224,24 +183,25 @@ __device__ __forceinline__ uint32_t sw128(int r, int byte) {
 }
 
 template <int BN, int EF>
-__device__ __forceinline__ void epilogue_tile_staged(const GemmEpilogue& ep, const CUtensorMap* tm_out,
-                                                     const CUtensorMap* tm_pre, float (&acc)[2][BN / 2],
-                                                     const float* s_bias, const float* s_gamma, uint8_t* stg,
-                                                     int& seq, int bar, int t, int m0, int n0, int M, int N, int r_in,
-                                                     int c_in) {
+__device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, const CUtensorMap* tm_out,
+                                              const CUtensorMap* tm_pre, float (&acc)[2][BN / 2], const float* s_bias,
+                                              const float* s_gamma, uint8_t* stg, int& seq, int bar, int t, int m0,
+                                              int n0, int M, int N, size_t slab_row0, int r_in, int c_in) {
+  constexpr bool STAGED = kStaged<EF>;
   constexpr bool F32 = (EF & EP_OUT_F32) != 0;
   constexpr int OUT_BOXES = F32 ? 2 : 1;
   constexpr int CHUNK = (OUT_BOXES + ((EF & EP_STORE_PRE) ? 1 : 0)) * STG_BOX;
   constexpr int NBUF = STG_BYTES / CHUNK;
   static_assert(NBUF >= 1, "a chunk must fit the staging area");
-  static_assert((EF & (EP_ACCUM | EP_SLABS)) == 0, "ACCUM and split-K slabs store from registers");
+  float* const out_f = reinterpret_cast<float*>(ep.out);
+  __nv_bfloat16* const out_h = reinterpret_cast<__nv_bfloat16*>(ep.out);
 #pragma unroll
   for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
     for (int cb = 0; cb < BN / 64; ++cb) {
       const int row0 = m0 + mh * 64, col0 = n0 + cb * 64;
       if (row0 >= M || col0 >= N) continue;   // uniform over the warpgroup
-      float2 xr[2][8];
+      float2 xr[2][8], xo[2][8];
       uint32_t xu[2][8];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -250,61 +210,62 @@ __device__ __forceinline__ void epilogue_tile_staged(const GemmEpilogue& ep, con
         for (int i = 0; i < 8; ++i) {
           const int n = col0 + 8 * i + c_in;
           if (row < (size_t)M && n < N) {
-            if constexpr ((EF & EP_RESID) != 0)
+            if (epi_has<EF>(ep, EP_RESID))
               xr[h][i] = *reinterpret_cast<const float2*>(ep.resid + row * ep.ld_resid + n);
-            if constexpr ((EF & EP_MUL_DGELU) != 0)
+            if (epi_has<EF>(ep, EP_MUL_DGELU))
               xu[h][i] = *reinterpret_cast<const uint32_t*>(ep.aux_in + row * ep.ld_aux + n);
+            if (epi_has<EF>(ep, EP_ACCUM))
+              xo[h][i] = *reinterpret_cast<const float2*>(out_f + (slab_row0 + row) * ep.ld_out + n);
           }
         }
       }
       uint8_t* const buf = stg + (seq % NBUF) * CHUNK;
-      if (t == 0) tma_store_wait_read<NBUF - 1>();   // the group that last read `buf` is done
-      named_bar_sync(bar, 128);
+      if constexpr (STAGED) {
+        if (t == 0) tma_store_wait_read<NBUF - 1>();   // the group that last read `buf` is done
+        named_bar_sync(bar, 128);
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = r_in + 8 * h;
+        const size_t row = (size_t)row0 + r;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const int cl = cb * 64 + 8 * i + c_in;   // column within the tile
-          float v0 = __fmul_rn(acc[mh][4 * (cl >> 3) + 2 * h], ep.alpha);
-          float v1 = __fmul_rn(acc[mh][4 * (cl >> 3) + 2 * h + 1], ep.alpha);
-          if constexpr ((EF & EP_BIAS) != 0) {
-            const float2 b = *reinterpret_cast<const float2*>(s_bias + cl);
-            v0 = __fadd_rn(v0, b.x); v1 = __fadd_rn(v1, b.y);
-          }
-          if constexpr ((EF & EP_STORE_PRE) != 0)
-            *reinterpret_cast<uint32_t*>(buf + OUT_BOXES * STG_BOX + sw128(r, 16 * i + 2 * c_in)) = pack_bf16(v0, v1);
-          if constexpr ((EF & EP_GELU) != 0) {
-            v0 = gelu_tanh_fast(v0); v1 = gelu_tanh_fast(v1);
-          }
-          if constexpr ((EF & EP_MUL_DGELU) != 0) {
-            const float2 u = unpack_bf16(xu[h][i]);
-            v0 = __fmul_rn(v0, gelu_grad_epi(u.x)); v1 = __fmul_rn(v1, gelu_grad_epi(u.y));
-          }
-          if constexpr ((EF & EP_GAMMA) != 0) {
-            const float2 g = *reinterpret_cast<const float2*>(s_gamma + cl);
-            v0 = __fmul_rn(v0, g.x); v1 = __fmul_rn(v1, g.y);
-          }
-          if constexpr ((EF & EP_RESID) != 0) {
-            v0 = __fadd_rn(v0, xr[h][i].x); v1 = __fadd_rn(v1, xr[h][i].y);
-          }
-          if constexpr (F32) {
-            *reinterpret_cast<float2*>(buf + (i >> 2) * STG_BOX + sw128(r, 32 * (i & 3) + 4 * c_in)) =
-                make_float2(v0, v1);
-          } else {
-            *reinterpret_cast<uint32_t*>(buf + sw128(r, 16 * i + 2 * c_in)) = pack_bf16(v0, v1);
+          const int n = n0 + cl;
+          const float2 b = epi_has<EF>(ep, EP_BIAS) ? *reinterpret_cast<const float2*>(s_bias + cl) : float2{};
+          const float2 g = epi_has<EF>(ep, EP_GAMMA) ? *reinterpret_cast<const float2*>(s_gamma + cl) : float2{};
+          const float2 u = epi_has<EF>(ep, EP_MUL_DGELU) ? unpack_bf16(xu[h][i]) : float2{};
+          float p0, p1;
+          const float v0 = epi_value<EF>(ep, acc[mh][4 * (cl >> 3) + 2 * h], b.x, u.x, g.x, xr[h][i].x, xo[h][i].x, p0);
+          const float v1 = epi_value<EF>(ep, acc[mh][4 * (cl >> 3) + 2 * h + 1], b.y, u.y, g.y, xr[h][i].y, xo[h][i].y,
+                                         p1);
+          if constexpr (STAGED) {
+            if (epi_has<EF>(ep, EP_STORE_PRE))
+              *reinterpret_cast<uint32_t*>(buf + OUT_BOXES * STG_BOX + sw128(r, 16 * i + 2 * c_in)) = pack_bf16(p0, p1);
+            if constexpr (F32) {
+              *reinterpret_cast<float2*>(buf + (i >> 2) * STG_BOX + sw128(r, 32 * (i & 3) + 4 * c_in)) =
+                  make_float2(v0, v1);
+            } else {
+              *reinterpret_cast<uint32_t*>(buf + sw128(r, 16 * i + 2 * c_in)) = pack_bf16(v0, v1);
+            }
+          } else if (row < (size_t)M && n < N) {
+            if (epi_has<EF>(ep, EP_STORE_PRE)) st_pair(ep.aux_out + row * ep.ld_aux + n, p0, p1, true, true);
+            if constexpr (F32) st_pair(out_f + (slab_row0 + row) * ep.ld_out + n, v0, v1, true, true);
+            else st_pair(out_h + (slab_row0 + row) * ep.ld_out + n, v0, v1, true, true);
           }
         }
       }
-      fence_proxy_async_smem();                // the writes above are visible to the TMA (async proxy)
-      named_bar_sync(bar, 128);
-      if (t == 0) {
-        tma_store_2d(tm_out, buf, col0, row0);
-        if (F32 && col0 + 32 < N) tma_store_2d(tm_out, buf + STG_BOX, col0 + 32, row0);
-        if constexpr ((EF & EP_STORE_PRE) != 0) tma_store_2d(tm_pre, buf + OUT_BOXES * STG_BOX, col0, row0);
-        tma_store_commit();
+      if constexpr (STAGED) {
+        fence_proxy_async_smem();                // the writes above are visible to the TMA (async proxy)
+        named_bar_sync(bar, 128);
+        if (t == 0) {
+          tma_store_2d(tm_out, buf, col0, row0);
+          if (F32 && col0 + 32 < N) tma_store_2d(tm_out, buf + STG_BOX, col0 + 32, row0);
+          if constexpr ((EF & EP_STORE_PRE) != 0) tma_store_2d(tm_pre, buf + OUT_BOXES * STG_BOX, col0, row0);
+          tma_store_commit();
+        }
+        ++seq;
       }
-      ++seq;
     }
 }
 
@@ -323,11 +284,6 @@ struct Cfg {
   static constexpr int SMEM_BYTES = (STAGED ? STG_OFF + 2 * STG_BYTES : VEC_END) + 1024;
   static_assert(SMEM_BYTES <= 227 * 1024, "over the opt-in shared-memory limit");
 };
-
-// The epilogue stores through shared memory: every fixed flag set but the weight gradients' (split-K slabs, ACCUM),
-// whose main loop runs over all tokens and so hides a register-store epilogue, and which keep the deeper ring.
-template <int EF>
-constexpr bool kStaged = EF != EPI_RUNTIME && (EF & (EP_SLABS | EP_ACCUM)) == 0;
 
 // work item = (tile, split): k-blocks [kb0, kb1)
 struct WorkRange { int m0, n0, kb0, kb1; };
@@ -486,28 +442,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         named_bar_sync(3 + cw, 128);           // bias / gamma of this tile are in shared memory
       }
       if (nkb <= 0) continue;                  // empty split-K slice: nothing to add
-      const size_t slab_row0 = (EF == EPI_RUNTIME ? (ep.flags & EP_SLABS) : (EF & EP_SLABS)) ? (size_t)(w % splits) * M : 0;
-      if constexpr (staged) {
-        epilogue_tile_staged<BN, EF>(ep, &tmO, &tmP, acc, s_bias, s_gamma, stg, stg_seq, 5 + cw, t, wr.m0, wr.n0, M, N,
-                                     r_in, c_in);
-      } else if constexpr (EF != EPI_RUNTIME) {
-        epilogue_tile<BN, EF>(ep, acc, s_bias, s_gamma, wr.m0, wr.n0, M, N, slab_row0, r_in, c_in);
+      const size_t slab_row0 = epi_has<EF>(ep, EP_SLABS) ? (size_t)(w % splits) * M : 0;
+      if constexpr (EF == EPI_RUNTIME) {
+        epilogue_tile_runtime<BN>(ep, acc, wr.m0, wr.n0, M, N, slab_row0, r_in, c_in);
       } else {
-        const bool fast = (ep.flags & EP_SLOW) == 0;
-#pragma unroll
-        for (int mh = 0; mh < 2; ++mh)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = wr.m0 + mh * 64 + r_in + 8 * h;
-            if (row >= M) continue;
-            const size_t orow = slab_row0 + row;
-#pragma unroll
-            for (int i = 0; i < BN / 8; ++i) {
-              const int n = wr.n0 + 8 * i + c_in;
-              if (n >= N) break;
-              epilogue_pair(ep, orow, n, N, acc[mh][4 * i + 2 * h], acc[mh][4 * i + 2 * h + 1], fast && n + 1 < N);
-            }
-          }
+        epilogue_tile<BN, EF>(ep, &tmO, &tmP, acc, s_bias, s_gamma, stg, stg_seq, 5 + cw, t, wr.m0, wr.n0, M, N,
+                              slab_row0, r_in, c_in);
       }
     }
     if (staged && t == 0) tma_store_wait_all();   // shared memory stays valid until the last store has read it
@@ -639,13 +579,15 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
       return set_error(D3_ERR_ARG, "gemm: SCATTER needs 1..8 ranks and 4-element aligned shard / offset / ld_out");
     if ((unsigned long long)ep.sc_off + (unsigned long long)(M - 1) * ep.ld_out + N > (unsigned long long)ep.sc_shard * ep.sc_world)
       return set_error(D3_ERR_ARG, "gemm: SCATTER output exceeds the sharded range");
-    ep.flags |= EP_ATOMIC;       // every contribution is an atomic add (other ranks add into the same slice)
   }
   if (splits > 1) {
     if (!plain_f32) return set_error(D3_ERR_ARG, "gemm: split-K needs a plain fp32 output");
     if (!(ep.flags & EP_ACCUM)) return set_error(D3_ERR_ARG, "gemm: split-K accumulates into out (set ACCUM, zero it first)");
     if (splits > num_k) splits = num_k;
   }
+  // every SCATTER contribution is an atomic add into the owners' shards (other ranks add into the same slice): `out`
+  // is neither read nor written
+  if (ep.flags & EP_SCATTER) ep.flags &= ~EP_ACCUM;
   // ---- epilogue fast-path eligibility
   const int out_elt = (ep.flags & EP_OUT_F32) ? 4 : 2;
   bool aligned = ((uintptr_t)ep.out % 16 == 0) && ((ep.ld_out * out_elt) % 16 == 0);
@@ -655,7 +597,6 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
   if (ep.flags & EP_STORE_PRE) aligned = aligned && ((uintptr_t)ep.aux_out % 16 == 0) && (ep.ld_aux % 8 == 0);
   if (ep.flags & EP_MUL_DGELU) aligned = aligned && ((uintptr_t)ep.aux_in % 16 == 0) && (ep.ld_aux % 8 == 0);
   if (!aligned) ep.flags |= EP_SLOW;
-  ep.flags |= EP_FAST_ACT;   // hardware tanh (rel. error 2^-11, below the bf16 rounding of the GEMM operands feeding it)
 
   CUtensorMap ta, tb;
   int rc = make_operand_map(&ta, A, M, K, lda, a_mn, BM);
