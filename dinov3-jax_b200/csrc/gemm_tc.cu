@@ -9,9 +9,14 @@
 // The epilogue fuses bias, tanh-GELU, GELU', LayerScale (gamma) and the residual add
 // (dinov3_jax/layers/block.py:198-199, dinov3_jax/layers/layer_scale.py:17-21).
 //
-// One kernel, 128 x {64,128} output tiles, 384 threads:
+// One kernel, 128 x {64,128} output tiles, 384 threads, launched in clusters of 2 CTAs that compute the tiles (m0, n0)
+// and (m0, n0 + BN) of a pair side by side, over the same k-blocks:
 //   warpgroup 0      TMA producer (one elected thread): A and B k-blocks of 64, tile after tile of this CTA's work
-//                    list, into one shared-memory ring;
+//                    list, into one shared-memory ring.  A is shared by the pair: each CTA loads one 64-row half and
+//                    multicasts it into both CTAs' ring, so a CTA reads 3/4 (BN = 128) or 2/3 (BN = 64) of the
+//                    operand bytes it consumes from L2.  A ring stage is written by both producers, so it is refilled
+//                    only after the consumers of both CTAs released it (empty barriers count 2 arrivals: one local,
+//                    one from the peer through its cluster address);
 //   warpgroups 1, 2  consumers in ping-pong: the CTA's tiles alternate between them, so one warpgroup's epilogue
 //                    runs under the other's main loop.  A tile is two m64nBNk16 wgmma chains (rows 0-63 / 64-127)
 //                    over SWIZZLE_128B operands, K-major or MN-major through the descriptor transpose bits.
@@ -285,16 +290,17 @@ struct Cfg {
   static_assert(SMEM_BYTES <= 227 * 1024, "over the opt-in shared-memory limit");
 };
 
-// work item = (tile, split): k-blocks [kb0, kb1)
+// work item = (m tile, pair of N tiles, split), walked by both CTAs of a cluster: CTA `rank` takes N tile
+// 2 * pair + rank (wholly beyond N when the pair is ragged), k-blocks [kb0, kb1)
 struct WorkRange { int m0, n0, kb0, kb1; };
 // Tiles are rasterised N-fastest: the CTAs resident at any moment cover a few M row-panels times all N tiles, so the
 // large activation operand streams from HBM once while the (small) weight operand stays L2-resident.
-__device__ __forceinline__ WorkRange work_item(int w, int num_n, int num_k, int splits, int tile_n) {
+__device__ __forceinline__ WorkRange work_item(int w, int rank, int num_pairs, int num_k, int splits, int tile_n) {
   const int tile = w / splits, sp = w % splits;
   const int per = (num_k + splits - 1) / splits;
   WorkRange r;
-  r.n0 = (tile % num_n) * tile_n;
-  r.m0 = (tile / num_n) * BM;
+  r.n0 = (2 * (tile % num_pairs) + rank) * tile_n;
+  r.m0 = (tile / num_pairs) * BM;
   r.kb0 = sp * per;
   r.kb1 = min(num_k, r.kb0 + per);
   return r;
@@ -333,6 +339,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   float* vecs = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + C::BAR_BYTES);
 
   const int wg = threadIdx.x >> 7;
+  const int rank = blockIdx.x & 1;                  // CTA within the cluster (cluster dims {2, 1, 1})
+  const int cluster = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
@@ -340,33 +348,33 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       tma_prefetch_desc(&tmO);
       if constexpr ((EF & EP_STORE_PRE) != 0) tma_prefetch_desc(&tmP);
     }
-    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
+    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_mbar_init();
   }
-  __syncthreads();
+  cluster_sync();   // both CTAs' barriers are initialised before either multicasts into or arrives on the other's
 
   const int num_m = (M + BM - 1) / BM;
-  const int num_n = (N + BN - 1) / BN;
+  const int num_pairs = ((N + BN - 1) / BN + 1) / 2;
   const int num_k = (K + BK - 1) / BK;
-  const int num_work = num_m * num_n * splits;
+  const int num_work = num_m * num_pairs * splits;
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
     if (threadIdx.x < 32 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-        const WorkRange wr = work_item(w, num_n, num_k, splits, BN);
+      for (int w = cluster; w < num_work; w += num_clusters) {
+        const WorkRange wr = work_item(w, rank, num_pairs, num_k, splits, BN);
         for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * C::STAGE_BYTES;
           uint8_t* sb = sa + C::A_BYTES;
+          // this CTA's 64-row half of A goes to both CTAs; the peer's half completes the other A_BYTES / 2
           mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
           if (A_MN) {
-#pragma unroll
-            for (int i = 0; i < BM / 64; ++i) tma_load_2d(&tmA, &full_bar[stage], sa + i * 8192, wr.m0 + i * 64, kb * BK);
+            tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, wr.m0 + rank * 64, kb * BK, 0b11);
           } else {
-            tma_load_2d(&tmA, &full_bar[stage], sa, kb * BK, wr.m0);
+            tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, kb * BK, wr.m0 + rank * 64, 0b11);
           }
           if (B_MN) {
 #pragma unroll
@@ -388,12 +396,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     float* const s_gamma = s_bias + BN;
     constexpr bool stage_vecs = EF != EPI_RUNTIME && (EF & (EP_BIAS | EP_GAMMA)) != 0;
     uint8_t* const stg = smem + C::STG_OFF + cw * STG_BYTES;   // output staging (staged epilogues only)
+    const uint32_t peer_empty = mapa_shared(smem_u32(empty_bar), rank ^ 1);   // the peer's empty barriers
     int stg_seq = 0;                           // chunks this consumer has staged
     int stage = 0;                             // position in the ring, counting the other consumer's k-blocks too
     uint32_t phase = 0;
     int j = 0;
-    for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++j) {
-      const WorkRange wr = work_item(w, num_n, num_k, splits, BN);
+    for (int w = cluster; w < num_work; w += num_clusters, ++j) {
+      const WorkRange wr = work_item(w, rank, num_pairs, num_k, splits, BN);
       const int nkb = wr.kb1 > wr.kb0 ? wr.kb1 - wr.kb0 : 0;
       if ((j & 1) != cw) {                     // the other consumer's tile: step over its fills
         stage += nkb;
@@ -427,16 +436,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         fence_regs(acc[1]);
         if (prev >= 0) {                       // the k-block before this one has been consumed: release its stage
           wgmma_wait<1>();
-          if (t == 0) mbar_arrive(&empty_bar[prev]);
+          if (t == 0) { mbar_arrive(&empty_bar[prev]); mbar_arrive_cluster(peer_empty + 8 * prev); }
         }
         prev = stage;
         if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
-      if (w + (int)gridDim.x < num_work) named_bar_arrive(1 + (cw ^ 1), 256);   // tile j+1 may start its main loop
+      if (w + num_clusters < num_work) named_bar_arrive(1 + (cw ^ 1), 256);   // tile j+1 may start its main loop
       wgmma_wait<0>();
       fence_regs(acc[0]);
       fence_regs(acc[1]);
-      if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
+      if (prev >= 0 && t == 0) { mbar_arrive(&empty_bar[prev]); mbar_arrive_cluster(peer_empty + 8 * prev); }
       if constexpr (stage_vecs) {
         cp_async_wait_all();
         named_bar_sync(3 + cw, 128);           // bias / gamma of this tile are in shared memory
@@ -452,6 +461,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     }
     if (staged && t == 0) tma_store_wait_all();   // shared memory stays valid until the last store has read it
   }
+  cluster_sync();   // neither CTA exits while the peer may still arrive on its barriers
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -474,11 +484,26 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilog
                   int splits, cudaStream_t stream) {
   using C = Cfg<BN, kStaged<EF>>;
   auto kern = gemm_kernel<BN, A_MN, B_MN, EF>;
-  static bool configured = false;
-  if (!configured) {
+  cudaLaunchAttribute attr{};
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 2;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = C::SMEM_BYTES;
+  cfg.stream = stream;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  // persistent grid: as many clusters as can be resident at once (GPCs need not hold an even number of free SMs)
+  static int max_clusters = 0;
+  if (max_clusters == 0) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
-    configured = true;
+    cfg.gridDim = dim3(2 * sm_count());
+    e = cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg);
+    if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+    if (max_clusters < 1) return set_error(D3_ERR_CUDA, "gemm: no 2-CTA cluster fits on the device");
   }
   // output maps of the staged epilogue: the logical [M, N] with the real leading dimension, so TMA clips ragged rows
   // and columns (gemm_bf16's alignment checks already meet TMA's 16-byte address and stride rules)
@@ -492,10 +517,10 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilog
       if (rc) return rc;
     }
   }
-  const int work = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * splits;
-  const int grid = work < sm_count() ? work : sm_count();
-  kern<<<grid, GEMM_THREADS, C::SMEM_BYTES, stream>>>(ta, tb, to, tp, ep, M, N, K, splits);
-  cudaError_t e = cudaPeekAtLastError();
+  const int work = ((M + BM - 1) / BM) * (((N + BN - 1) / BN + 1) / 2) * splits;   // work items: tile pairs
+  cfg.gridDim = dim3(2 * (work < max_clusters ? work : max_clusters));
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, to, tp, ep, M, N, K, splits);
+  if (e == cudaSuccess) e = cudaPeekAtLastError();
   if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
   count_launch();
   return D3_OK;
@@ -599,7 +624,7 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
   if (!aligned) ep.flags |= EP_SLOW;
 
   CUtensorMap ta, tb;
-  int rc = make_operand_map(&ta, A, M, K, lda, a_mn, BM);
+  int rc = make_operand_map(&ta, A, M, K, lda, a_mn, 64);   // A arrives as two 64-row halves, one per cluster CTA
   if (rc) return rc;
   rc = make_operand_map(&tb, B, N, K, ldb, b_mn, bn);
   if (rc) return rc;

@@ -82,7 +82,35 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+// Multicast tiled load: the box lands at the same shared-memory offset in every CTA of the cluster named in `cta_mask`,
+// and each of them completes its bytes on its own mbarrier at the offset of `bar`.
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
+      : "memory");
+}
 
+// ------------------------------------------------------------------ thread-block clusters
+// the shared::cluster address of the variable at shared::cta address `addr` in the cluster's CTA `rank`
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+// Arrive on an mbarrier of any CTA of the cluster (a shared::cluster address from mapa_shared).  The default (.cta)
+// release: what the arrive publishes is this thread's completed reads of a ring stage, which the peer's TMA issue
+// follows.  A .release.cluster arrive, which orders all of the thread's earlier memory accesses at cluster scope, made
+// the clustered GEMMs take 1.8x as long on H100.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
+// every thread of every CTA in the cluster (release / acquire)
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive;\n\tbarrier.cluster.wait;" ::: "memory");
+}
 
 // ------------------------------------------------------------------ TMA store (smem -> global) and per-warp TMA loads
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
