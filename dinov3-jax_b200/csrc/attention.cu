@@ -11,7 +11,7 @@
 // online softmax on the accumulator fragment, then O += P V with P handed to the tensor core straight from registers
 // (RS form: the accumulator fragment of S is the A-operand fragment of the PV product).
 //
-// Crops longer than the resident kernels hold (span > 448 forward, N > 384 backward; G = 1 there) take streamed kernels
+// Crops longer than the resident kernels hold (span > 448 forward, N > 256 backward; G = 1 there) take streamed kernels
 // with the same per-tile arithmetic: a producer warpgroup fills an mbarrier ring of 128-row K / V (or Q / dO) tiles that both
 // consumer warpgroups read, so shared memory no longer grows with N.  Any N up to ATTN_MAX_TOKENS.
 #include "ptx.cuh"
@@ -325,14 +325,11 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ O, const __n
 }
 
 // ------------------------------------------------------------------------------------------------ backward
-// One CTA per (head, crop group); span <= 384 (up to 3 query tiles x 3 key tiles of 128), two warpgroups of 64 rows.
-// Q and dO tiles stay resident; K / V come one 128-key tile at a time.  For a tile pair (kt, qt):
-//   S  = Q K^T, dP = dO V^T                                    (registers)
-//   P  = exp(S*scale - lse), dS = P * (dP - Delta) * scale
-// Phase 1 (kt outer, qt inner): P and dS go to shared memory as bf16 SWIZZLE_128B tiles [128 q x 128 keys], then
-//   dV[kt] += P^T dO, dK[kt] += dS^T Q      (A = P / dS read MN-major: each warpgroup owns 64 keys)
-// Phase 2 (qt outer, kt inner): S and dP are recomputed and dQ[qt] += dS K with dS straight from registers (RS form).
-// The recomputation costs two small products per tile pair and keeps every accumulator in registers.
+// For a 128-query x 128-key tile pair:
+//   S  = Q K^T, dP = dO V^T,  P = exp(S*scale - lse),  dS = P * (dP - Delta) * scale
+//   dV += P^T dO, dK += dS^T Q, dQ += dS K
+// Crop groups of span <= 256 take attn_bwd_fused_kernel (all of it in one pass); longer crops the streamed pair below,
+// which shares the helpers p_ds_tile / stash_p_ds / dkdv_mma / dq_mma.
 // inverse RoPE on the gradient: transpose of y = x*cos + rot_half(x)*sin (dinov3_jax/layers/attention.py:14-20); this
 // thread holds columns d = 8i + c2 + {0,1} of a row, i.e. both partners (d, d + 32) of every rotation pair it touches.
 __device__ __forceinline__ void store_grad_rows(float (&a)[32], const AttnShape& sh, int c, int row_base, int tile_row0,
@@ -462,22 +459,61 @@ __device__ __forceinline__ void dq_mma(float (&dq)[32], const float (&dp)[64], c
   fence_regs(dq);
 }
 
-__global__ void __launch_bounds__(256)
-attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
-                const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
-                const AttnShape sh) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int nQ = (sh.span + 127) / 128, nK = nQ;
-  uint8_t* sQ = smem;                          // [nQ][128 x 64]
-  uint8_t* sDO = sQ + nQ * 16384;              // [nQ][128 x 64]
-  uint8_t* sK = sDO + nQ * 16384;              // 16 KB (current key tile)
-  uint8_t* sV = sK + 16384;                    // 16 KB
-  uint8_t* sP = sV + 16384;                    // [2 chunks of 64 keys][128 q x 128 B] 32 KB
-  uint8_t* sDS = sP + 32768;                   // 32 KB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + 32768);
-  uint64_t* bar_q = bars;
-  uint64_t* bar_kv = bars + 1;
+// One CTA per (head, crop group) for span <= 256, two warpgroups.  At most two 128-row tiles: every Q / dO / K / V tile
+// stays resident, and one thread issues all their TMA loads at the start (one mbarrier per tile, so the first pair
+// starts as soon as it has landed and the rest arrives under it; a producer warpgroup would have nothing left to do).
+// dK, dV and dQ come out of one pass over the tile pairs (kt outer, qt inner), keys on the accumulator rows: warpgroup w
+// owns keys kt*128 + w*64 .. + 63 and, for each half of 64 query columns,
+//   S^T = K Q^T, dP^T = V dO^T                                 (SS, m64n64: registers)
+//   P^T = exp(S^T*scale - lse), dS^T = P^T * (dP^T - Delta) * scale   (LSE / Delta per query column, staged in smem)
+//   dV += P^T dO, dK += dS^T Q                                  (RS: the fragments of P^T / dS^T are the A operands)
+// and stashes its dS^T as bf16 (MN-major for the dQ product).  After a named barrier, warpgroup w computes
+//   dQ[qt rows w*64 ..] += dS K over all 128 keys of the tile  (SS, A = the stash read MN-major)
+// as one accumulation chain per query tile, no atomics.  The chains run over the key tiles in a fixed order, the one
+// the two-phase backward before this kernel used, so that training runs keep their bits: query tile 1 ascending (its
+// partial sum after key tile 0 waits in shared memory as fp32), query tile 0 from the last key tile down (the stash of
+// pair (0, 0) is kept and its products are issued after those of pair (1, 0)).
+// Five tile products per pair and one ex2 per score; 244 registers, no spills.  Shared memory at span 256: K/V 64 KB,
+// Q/dO 64 KB, two stashes 64 KB, dQ partial sum 32 KB, LSE / Delta 2 KB (one CTA per SM).
+
+// bytes of dynamic shared memory for n_t 128-row tiles (layout in attn_bwd_fused_kernel)
+__host__ __device__ constexpr int bwd_fused_smem(int n_t) {
+  return n_t * 32768 * 2 + 32768 + (n_t > 1 ? 2 * 32768 : 0) + n_t * 128 * 8 + 2 * n_t * 8;
+}
+
+// descriptor of a tile computed where it is used: loop-invariant descriptors (and their per-k-step offsets) would
+// otherwise be hoisted out of the tile loops and held in registers across the whole pass
+__device__ __forceinline__ uint64_t desc_here(const void* p, uint32_t lbo, uint32_t sbo) {
+  uint32_t a;
+  asm volatile("mov.b32 %0, %1;" : "=r"(a) : "r"(smem_u32(p)));
+  return gmma_desc_sw128(a, lbo, sbo);
+}
+
+// registers of the RS A fragments stay untouched until the wgmma reading them has completed
+__device__ __forceinline__ void fence_frag(uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) asm volatile("" : "+r"(a[i][e])::"memory");
+}
+
+__global__ void __launch_bounds__(256, 1)
+attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
+                      const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
+                      const AttnShape sh) {
+  // no round-up of the base as in the other kernels: span 256 leaves under 1 KB of the 227 KB opt-in, so the window's
+  // own 1 KB alignment (requested here) is what the SWIZZLE_128B tiles rely on
+  extern __shared__ __align__(1024) uint8_t smem_al[];
+  const int nT = (sh.span + 127) / 128;
+  uint8_t* sKV = smem_al;                       // [nT][K 16 KB | V 16 KB]
+  uint8_t* sQDO = sKV + nT * 32768;             // [nT][Q 16 KB | dO 16 KB]
+  uint8_t* sDS = sQDO + nT * 32768;             // dS^T of one tile pair: [2 chunks of 64 q][128 keys x 128 B]
+  uint8_t* sDS0 = sDS + 32768;                  // nT = 2: dS^T of pair (0, 0), kept until pair (1, 0)
+  float* sDQ = reinterpret_cast<float*>(sDS0 + 32768);   // nT = 2: dQ of query tile 1 after key tile 0, [2 wg][8][128][4]
+  float* sLSE = reinterpret_cast<float*>(sDS + (nT > 1 ? 3 * 32768 : 32768));   // [nT * 128] lse * log2(e) per query row
+  float* sDel = sLSE + nT * 128;                 // [nT * 128]
+  uint64_t* bar_kv = reinterpret_cast<uint64_t*>(sDel + nT * 128);
+  uint64_t* bar_q = bar_kv + nT;
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
@@ -487,74 +523,172 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmDO);
-    mbar_init(bar_q, 1);
-    mbar_init(bar_kv, 1);
+    for (int i = 0; i < 2 * nT; ++i) mbar_init(bar_kv + i, 1);
     fence_mbar_init();
   }
   __syncthreads();
   if (threadIdx.x < 32 && elect_one()) {
-    mbar_expect_tx(bar_q, nQ * 2 * 16384);
-    for (int qt = 0; qt < nQ; ++qt) {
-      tma_load_2d(&tmQKV, bar_q, sQ + qt * 16384, h * 64, row_base + qt * 128);
-      tma_load_2d(&tmDO, bar_q, sDO + qt * 16384, h * 64, row_base + qt * 128);
+    for (int i = 0; i < nT; ++i) {             // K/V 0, Q/dO 0, then the second tiles: the first pair starts early
+      mbar_expect_tx(bar_kv + i, 32768);
+      tma_load_2d(&tmQKV, bar_kv + i, sKV + i * 32768, sh.D + h * 64, row_base + i * 128);
+      tma_load_2d(&tmQKV, bar_kv + i, sKV + i * 32768 + 16384, 2 * sh.D + h * 64, row_base + i * 128);
+      mbar_expect_tx(bar_q + i, 32768);
+      tma_load_2d(&tmQKV, bar_q + i, sQDO + i * 32768, h * 64, row_base + i * 128);
+      tma_load_2d(&tmDO, bar_q + i, sQDO + i * 32768 + 16384, h * 64, row_base + i * 128);
     }
   }
-  uint32_t kv_phase = 0;
-  int kv_loaded = -1;
-  auto load_kv = [&](int kt) {       // every thread: K / V tile kt resident (the previous tile's readers are done)
-    if (kv_loaded == kt) return;
-    __syncthreads();
-    if (threadIdx.x < 32 && elect_one()) {
-      mbar_expect_tx(bar_kv, 2 * 16384);
-      tma_load_2d(&tmQKV, bar_kv, sK, sh.D + h * 64, row_base + kt * 128);
-      tma_load_2d(&tmQKV, bar_kv, sV, 2 * sh.D + h * 64, row_base + kt * 128);
-    }
-    mbar_wait(bar_kv, kv_phase);
-    kv_phase ^= 1;
-    kv_loaded = kt;
-  };
-  auto p_ds = [&](int qt, int kt, float (&s)[64], float (&dp)[64]) {
-    p_ds_tile(sh, LSE, Delta, c, h, qt * 128 + wg * 64, kt, sQ + qt * 16384 + wg * 8192, sDO + qt * 16384 + wg * 8192,
-              sK, sV, r_in, c2, s, dp);
-  };
+  for (int q = threadIdx.x; q < nT * 128; q += 256) {
+    const RowInfo ri = row_info(sh, c, q);
+    const size_t stat = ((size_t)(c * sh.G + ri.g) * sh.H + h) * sh.N + (q - ri.klo);
+    sLSE[q] = ri.ok ? LSE[stat] * LOG2E : 0.f;
+    sDel[q] = ri.ok ? Delta[stat] : 0.f;
+  }
+  __syncthreads();
 
-  mbar_wait(bar_q, 0);
-  // ---- phase 1: dK, dV of key tile kt (this warpgroup: keys kt*128 + wg*64 ..)
+  const float cs = sh.scale * LOG2E;
+  int pair = 0;
 #pragma unroll 1
-  for (int kt = 0; kt < nK; ++kt) {
-    load_kv(kt);
-    float dk[32], dv[32];
+  for (int kt = 0; kt < nT; ++kt) {
+    mbar_wait(bar_kv + kt, 0);
+    const uint8_t* sK = sKV + kt * 32768;
+    const uint8_t* sV = sK + 16384;
+    // valid query columns of this thread's two key rows: the key's own crop (none for keys outside the group)
+    int lo[2], hi[2];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
+    for (int hh = 0; hh < 2; ++hh) {
+      const RowInfo ri = row_info(sh, c, kt * 128 + wg * 64 + r_in + 8 * hh);
+      lo[hh] = ri.ok ? ri.klo : 0;
+      hi[hh] = ri.ok ? ri.khi : 0;
+    }
+    float dk[32], dv[32];
 #pragma unroll 1
-    for (int qt = 0; qt < nQ; ++qt) {
-      float s[64], dp[64];
-      p_ds(qt, kt, s, dp);
-      stash_p_ds(s, dp, sP, sDS, wg * 64 + r_in, c2);
-      fence_proxy_async_smem();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      __syncthreads();
-      dkdv_mma(dk, dv, sP, sDS, sDO + qt * 16384, sQ + qt * 16384, wg);
-      __syncthreads();            // both warpgroups are done reading sP / sDS before the next tile pair rewrites them
+    for (int qt = 0; qt < nT; ++qt, ++pair) {
+      mbar_wait(bar_q + qt, 0);
+      const uint8_t* sQt = sQDO + qt * 32768;
+      const uint8_t* sDOt = sQt + 16384;
+      const bool defer = nT == 2 && kt == 0 && qt == 0;   // dQ of query tile 0 starts with key tile 1
+      uint8_t* stash = defer ? sDS0 : sDS;
+      // the 128 query columns in two halves of 64: S^T / dP^T of one half (64 registers) at a time, so that the
+      // accumulators, the fragments of the half still being read by its RS products and the scores fit without spills
+      uint32_t pa[2][4][4], da[2][4][4];   // bf16 A fragments of P^T / dS^T (k-step kk: query columns 16 kk ..)
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        float s[32], dp[32];
+        {
+          const uint64_t kd = desc_here(sK + wg * 8192, 16, 1024);
+          const uint64_t vd = desc_here(sV + wg * 8192, 16, 1024);
+          const uint64_t qd = desc_here(sQt + hf * 8192, 16, 1024);
+          const uint64_t dod = desc_here(sDOt + hf * 8192, 16, 1024);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            wgmma_m64n64k16_ss<0, 0>(s, kd + 2 * k, qd + 2 * k, k > 0 ? 1u : 0u);
+            wgmma_m64n64k16_ss<0, 0>(dp, vd + 2 * k, dod + 2 * k, k > 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();        // also retires the first half's RS products
+          fence_regs(s);
+          fence_regs(dp);
+          if (hf == 1) { fence_frag(pa[0]); fence_frag(da[0]); }
+        }
+        const float* lse2 = sLSE + qt * 128 + hf * 64;
+        const float* del = sDel + qt * 128 + hf * 64;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int col = 8 * i + c2;
+          const float2 l2 = *reinterpret_cast<const float2*>(lse2 + col);
+          const float2 dl = *reinterpret_cast<const float2*>(del + col);
+          const int q = qt * 128 + hf * 64 + col;
+          float pv[4], dv4[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int hh = j >> 1, qq = q + (j & 1);
+            const bool ok = qq >= lo[hh] && qq < hi[hh];
+            const float p = ok ? ex2_approx(fmaf(s[4 * i + j], cs, -((j & 1) ? l2.y : l2.x))) : 0.f;
+            dv4[j] = ok ? (p * sh.scale) * (dp[4 * i + j] - ((j & 1) ? dl.y : dl.x)) : 0.f;
+            pv[j] = p;
+          }
+          pa[hf][i >> 1][2 * (i & 1)] = pack_bf16(pv[0], pv[1]);
+          pa[hf][i >> 1][2 * (i & 1) + 1] = pack_bf16(pv[2], pv[3]);
+          da[hf][i >> 1][2 * (i & 1)] = pack_bf16(dv4[0], dv4[1]);
+          da[hf][i >> 1][2 * (i & 1) + 1] = pack_bf16(dv4[2], dv4[3]);
+        }
+        // the dQ products of the previous pair (both warpgroups) have finished reading the stash (pairs 0 and 1 of
+        // nT = 2 write different stashes)
+        if (hf == 0 && pair > 1) named_bar_sync(1, 256);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {   // chunk hf of the stash holds query columns hf * 64 ..
+            const uint32_t off = hf * 16384 + sw128_offset(wg * 64 + r_in + 8 * hh, 8 * i + c2);
+            *reinterpret_cast<uint32_t*>(stash + off) = da[hf][i >> 1][2 * (i & 1) + hh];
+          }
+        {
+          const uint64_t dod = desc_here(sDOt, 8192, 1024);   // B MN-major: 16 query rows per k-step
+          const uint64_t qd = desc_here(sQt, 8192, 1024);
+          const uint32_t acc_on = (qt > 0 || hf > 0) ? 1u : 0u;
+          if (acc_on) { fence_regs(dk); fence_regs(dv); }
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            const int ks = 4 * hf + kk;
+            wgmma_m64n64k16_rs<1>(dv, pa[hf][kk], dod + 128 * ks, (acc_on || kk > 0) ? 1u : 0u);
+            wgmma_m64n64k16_rs<1>(dk, da[hf][kk], qd + 128 * ks, (acc_on || kk > 0) ? 1u : 0u);
+          }
+          wgmma_commit();
+        }
+      }
+      fence_proxy_async_smem();   // generic-proxy smem writes (the stash) -> visible to the tensor core (async proxy)
+      if (defer) {                // pair (1, 0) reads this stash; only the RS products remain to retire
+        wgmma_wait<0>();
+        fence_regs(dk);
+        fence_regs(dv);
+        fence_frag(pa[1]);
+        fence_frag(da[1]);
+        continue;
+      }
+      named_bar_sync(2, 256);     // both halves of dS^T are in the stash
+      const bool from_partial = nT == 2 && kt == 1 && qt == 1;
+      float dq[32];
+      float4* part = reinterpret_cast<float4*>(sDQ) + wg * 8 * 128 + t;
+      if (from_partial) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float4 v = part[j * 128];
+          dq[4 * j] = v.x; dq[4 * j + 1] = v.y; dq[4 * j + 2] = v.z; dq[4 * j + 3] = v.w;
+        }
+      }
+      {
+        const uint64_t sd = desc_here(sDS + wg * 16384, 16384, 1024);   // A MN-major: 16 keys per k-step
+        const uint64_t kbd = desc_here(sK, 8192, 1024);                 // B MN-major
+        fence_regs(dq);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk)
+          wgmma_m64n64k16_ss<1, 1>(dq, sd + 128 * kk, kbd + 128 * kk, (from_partial || kk > 0) ? 1u : 0u);
+        if (nT == 2 && kt == 1 && qt == 0) {   // then key tile 0, from the kept stash of pair (0, 0)
+          const uint64_t sd0 = desc_here(sDS0 + wg * 16384, 16384, 1024);
+          const uint64_t k0d = desc_here(sKV, 8192, 1024);
+#pragma unroll
+          for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_ss<1, 1>(dq, sd0 + 128 * kk, k0d + 128 * kk, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(dq);
+        fence_regs(dk);
+        fence_regs(dv);
+        fence_frag(pa[1]);
+        fence_frag(da[1]);
+      }
+      if (nT == 2 && kt == 0) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) part[j * 128] = make_float4(dq[4 * j], dq[4 * j + 1], dq[4 * j + 2], dq[4 * j + 3]);
+      } else {
+        store_grad_rows(dq, sh, c, row_base, qt * 128 + wg * 64, r_in, c2, h, 0, true, dQKV);
+      }
     }
     store_grad_rows(dk, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 1, true, dQKV);
     store_grad_rows(dv, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 2, false, dQKV);
-  }
-  // ---- phase 2: dQ of query tile qt (this warpgroup: rows qt*128 + wg*64 ..); the key tiles are walked in alternating
-  // directions so that each walk starts with the tile that is still resident
-#pragma unroll 1
-  for (int qt = 0; qt < nQ; ++qt) {
-    float dq[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) dq[i] = 0.f;
-#pragma unroll 1
-    for (int j = 0; j < nK; ++j) {
-      const int kt = (qt & 1) ? j : nK - 1 - j;
-      load_kv(kt);
-      float s[64], dp[64];
-      p_ds(qt, kt, s, dp);
-      dq_mma(dq, dp, sK);
-    }
-    store_grad_rows(dq, sh, c, row_base, qt * 128 + wg * 64, r_in, c2, h, 0, true, dQKV);
   }
   dbg_mark(1);
 }
@@ -716,7 +850,7 @@ static int make_map(CUtensorMap* map, const void* ptr, long rows, int cols, int 
 // is checked below.  It covers a 2 880^2 crop at patch 16 with 5 prefix tokens (32 405 tokens).
 constexpr int ATTN_MAX_TOKENS = 32768;
 constexpr int ATTN_FWD_RESIDENT_SPAN = 448;   // attn_fwd_kernel: Q and all of K / V of a crop group in shared memory
-constexpr int ATTN_BWD_RESIDENT_N = 384;      // attn_bwd_kernel: every Q / dO tile of a crop in shared memory
+constexpr int ATTN_BWD_RESIDENT_SPAN = 256;   // attn_bwd_fused_kernel: all Q / dO / K / V tiles of a crop group resident
 
 static int attn_shape(AttnShape* s, int n_crops, int N, int D, int H) {
   if (D != H * 64) return set_error(D3_ERR_ARG, "attention: head_dim must be 64");
@@ -791,7 +925,7 @@ int d3_attn_bwd(const void* qkv, const void* o, const void* d_o, const float* ls
   if (rc) return rc;
   if ((rope_sin == nullptr) != (rope_cos == nullptr)) return set_error(D3_ERR_ARG, "d3_attn_bwd: sin/cos tables");
   if (!delta_scratch) return set_error(D3_ERR_ARG, "d3_attn_bwd: delta scratch buffer");
-  const bool streamed = N > ATTN_BWD_RESIDENT_N;
+  const bool streamed = s.span > ATTN_BWD_RESIDENT_SPAN;
   dim3 sgrid;
   if (streamed && (rc = stream_grid(s, &sgrid))) return rc;
   s.sin_t = rope_sin; s.cos_t = rope_cos; s.prefix = rope_prefix;
@@ -821,11 +955,13 @@ int d3_attn_bwd(const void* qkv, const void* o, const void* d_o, const float* ls
     return D3_OK;
   }
   static bool cfg = false;
-  if (!cfg) { cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024); cfg = true; }
-  const int nq = (s.span + 127) / 128;
-  const int smem = 2 * nq * 16384 + 32768 + 65536 + 64 + 1024;
+  if (!cfg) {
+    cudaFuncSetAttribute(attn_bwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_fused_smem(2));
+    cfg = true;
+  }
   dim3 grid(H, (n_crops + s.G - 1) / s.G);
-  attn_bwd_kernel<<<grid, 256, smem, st>>>(tqkv, tdo, lse, delta_scratch, (__nv_bfloat16*)dqkv, s);
+  attn_bwd_fused_kernel<<<grid, 256, bwd_fused_smem((s.span + 127) / 128), st>>>(tqkv, tdo, lse, delta_scratch,
+                                                                                 (__nv_bfloat16*)dqkv, s);
   D3_CHECK_LAUNCH();
   return D3_OK;
 }

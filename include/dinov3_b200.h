@@ -136,7 +136,7 @@ int d3_rope(void* qkv_bf16, const float* sin_t /*[P,hd]*/, const float* cos_t, l
 
 /* ---- attention (layers/attention.py:116 nn.dot_product_attention; head_dim 64, any N up to 32768) ----------------- */
 /* N > 32768, or n_crops * N >= 2^31, returns D3_ERR_ARG before any CUDA call.  Crops of up to 448 tokens (forward) /
- * 384 tokens (backward) run on kernels that hold a whole crop in shared memory; longer ones on streamed kernels.   */
+ * 256 tokens (backward) run on kernels that hold a whole crop in shared memory; longer ones on streamed kernels.   */
 int d3_attn_fwd(const void* qkv_bf16 /*[n*N,3D] post-RoPE*/, void* o_bf16 /*[n*N,D]*/, float* lse /*[n,H,N] or NULL*/,
                 int n_crops, int N, int D, int H, void* stream);
 /* rope_sin / rope_cos ([P,64] fp32, or NULL): when given, the inverse rotation (transpose of layers/attention.py:19-20)

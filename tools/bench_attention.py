@@ -1,6 +1,6 @@
-"""Isolated timing of the attention kernels at the ViT-L/16 B=64 shapes of the headline step, then at the long crops
-of the high-resolution recipes (streamed kernels), all at ViT-L heads (CUDA events, 20 launches after 3 warm-ups, inputs
-larger than L2): python tools/bench_attention.py [fwd|bwd|all]."""
+"""Isolated timing of the attention kernels at the ViT-L/16 B=64 shapes of the headline step, the ViT-g/16 global crops
+(257 tokens, 24 heads), then the long crops of the high-resolution recipes (streamed kernels) at ViT-L heads (CUDA
+events, 20 launches after 3 warm-ups, inputs larger than L2): python tools/bench_attention.py [fwd|bwd|all]."""
 import os
 import subprocess
 import sys
@@ -12,7 +12,6 @@ from dinov3_jax import _native, ops
 
 _native.init(0)
 what = sys.argv[1] if len(sys.argv) > 1 else "all"
-H, D = 16, 1024
 bf = torch.bfloat16
 
 
@@ -40,10 +39,12 @@ def card():
 
 
 print(card())
-SHORT = (("global 128 crops x 197", 128, 197, True), ("local 512 crops x 37", 512, 37, True))
-LONG = (("512^2 16 crops x 1029", 16, 1029, True), ("768^2 16 crops x 2309", 16, 2309, True),
-        ("gram 1152^2 8 crops x 5189", 8, 5189, False))        # B = 8 global crops, 4 storage tokens
-for name, n, N, with_bwd in SHORT + LONG:
+SHORT = (("global 128 crops x 197", 128, 197, 16, True), ("local 512 crops x 37", 512, 37, 16, True),
+         ("ViT-g global 128 crops x 257", 128, 257, 24, True))
+LONG = (("512^2 16 crops x 1029", 16, 1029, 16, True), ("768^2 16 crops x 2309", 16, 2309, 16, True),
+        ("gram 1152^2 8 crops x 5189", 8, 5189, 16, False))        # B = 8 global crops, 4 storage tokens
+for name, n, N, H, with_bwd in SHORT + LONG:
+    D = 64 * H
     T = n * N
     qkv = torch.randn(T, 3 * D, device="cuda").to(bf)
     o = torch.empty(T, D, device="cuda", dtype=bf)
