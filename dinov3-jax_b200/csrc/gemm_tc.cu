@@ -10,7 +10,7 @@
 // (dinov3_jax/layers/block.py:198-199, dinov3_jax/layers/layer_scale.py:17-21).
 //
 // One kernel, 128 x {64,128} output tiles, 384 threads, launched in clusters of 2 CTAs that compute the tiles (m0, n0)
-// and (m0, n0 + BN) of a pair side by side, over the same k-blocks:
+// and (m0, n0 + BN) of a pair side by side, over the same k-blocks (128 x 256 tiles: see below):
 //   warpgroup 0      TMA producer (one elected thread): A and B k-blocks of 64, tile after tile of this CTA's work
 //                    list, into one shared-memory ring.  A is shared by the pair: each CTA loads one 64-row half and
 //                    multicasts it into both CTAs' ring, so a CTA reads 3/4 (BN = 128) or 2/3 (BN = 64) of the
@@ -24,6 +24,12 @@
 // consumer starts its main loop only after the other has passed its last full-barrier wait (named barriers 1 / 2), so
 // every fill of a stage is waited on by exactly one consumer, in order, and no wait can be two phases ahead (which the
 // phase parity could not tell apart).  The main loop of one tile so has the whole ring in flight.
+//
+// 128 x 256 tiles (BN = 256, only when forced by tile_n): both consumers share every tile, warpgroup 1 rows 0-63 and
+// warpgroup 2 rows 64-127, each one m64n256k16 chain; both wait on every full barrier and release every stage, locally
+// and on the peer (empty barriers count 4).  The cluster pairs tiles (m0, n0) and (m0 + 128, n0): each CTA loads its own
+// A and multicasts one 128-column half of B.  Each element keeps the k-blocks, k16 steps and split-K slices of BN = 128,
+// so the bits are the same.  The epilogue is not hidden under another main loop.
 //
 // The epilogue's arithmetic is one function, epi_value (one element, accumulator to stored value), under two tile
 // walkers.  The epilogue flags are a template parameter.  The flag sets one training step issues are compiled with
@@ -187,9 +193,11 @@ __device__ __forceinline__ uint32_t sw128(int r, int byte) {
   return r * 128 + ((((byte >> 4) ^ r) & 7) << 4) + (byte & 15);
 }
 
-template <int BN, int EF>
+// `acc` holds MH 64-row halves of BN columns: a whole 128-row tile (MH = 2) or, at BN = 256, the consumer's 64 rows
+// starting at m0 (MH = 1).
+template <int MH, int BN, int EF>
 __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, const CUtensorMap* tm_out,
-                                              const CUtensorMap* tm_pre, float (&acc)[2][BN / 2], const float* s_bias,
+                                              const CUtensorMap* tm_pre, float (&acc)[MH][BN / 2], const float* s_bias,
                                               const float* s_gamma, uint8_t* stg, int& seq, int bar, int t, int m0,
                                               int n0, int M, int N, size_t slab_row0, int r_in, int c_in) {
   constexpr bool STAGED = kStaged<EF>;
@@ -201,7 +209,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, const CUte
   float* const out_f = reinterpret_cast<float*>(ep.out);
   __nv_bfloat16* const out_h = reinterpret_cast<__nv_bfloat16*>(ep.out);
 #pragma unroll
-  for (int mh = 0; mh < 2; ++mh)
+  for (int mh = 0; mh < MH; ++mh)
 #pragma unroll
     for (int cb = 0; cb < BN / 64; ++cb) {
       const int row0 = m0 + mh * 64, col0 = n0 + cb * 64;
@@ -276,39 +284,54 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, const CUte
 
 // ---------------------------------------------------------------------------------------------------------------
 // STAGED: the epilogue stores through shared memory, which takes one ring stage's worth of space (227 KB in all)
+// WIDE (BN = 256): both consumers share each tile, so bias and gamma are staged once per tile
 template <int BN, bool STAGED>
 struct Cfg {
-  static constexpr int STAGES = (BN == 128 ? 6 : 8) - (STAGED ? 1 : 0);
+  static constexpr bool WIDE = BN == 256;
+  static constexpr int STAGES = (BN == 256 ? 4 : BN == 128 ? 6 : 8) - (STAGED ? 1 : 0);
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int BAR_BYTES = 256;                       // full and empty mbarriers
-  static constexpr int VEC_BYTES = 2 * 2 * BN * 4;            // per consumer: bias and gamma of its tile (fp32)
+  static constexpr int VEC_BYTES = (WIDE ? 1 : 2) * 2 * BN * 4;   // bias and gamma of a tile (fp32), per consumer
   static constexpr int VEC_END = STAGES * STAGE_BYTES + BAR_BYTES + VEC_BYTES;
   static constexpr int STG_OFF = (VEC_END + 1023) / 1024 * 1024;   // SWIZZLE_128B staging: 1024-byte aligned
   static constexpr int SMEM_BYTES = (STAGED ? STG_OFF + 2 * STG_BYTES : VEC_END) + 1024;
   static_assert(SMEM_BYTES <= 227 * 1024, "over the opt-in shared-memory limit");
 };
 
-// work item = (m tile, pair of N tiles, split), walked by both CTAs of a cluster: CTA `rank` takes N tile
-// 2 * pair + rank (wholly beyond N when the pair is ragged), k-blocks [kb0, kb1)
-struct WorkRange { int m0, n0, kb0, kb1; };
+// work item = (tile pair, split), walked by both CTAs of a cluster, k-blocks [kb0, kb1).  BN = 64 / 128: the pair is
+// (m tile, pair of N tiles) and CTA `rank` takes N tile 2 * pair + rank; BN = 256: the pair is (pair of M tiles, N tile)
+// and CTA `rank` takes M tile 2 * pair + rank.  The second tile of a ragged pair lies wholly beyond N or M.
+// `num_n`: N positions of the list (pairs of N tiles, or N tiles at BN = 256); `num_tiles`: tile pairs per split.
+struct WorkRange { int m0, n0, kb0, kb1, sp; };
 // Tiles are rasterised N-fastest: the CTAs resident at any moment cover a few M row-panels times all N tiles, so the
-// large activation operand streams from HBM once while the (small) weight operand stays L2-resident.
-__device__ __forceinline__ WorkRange work_item(int w, int rank, int num_pairs, int num_k, int splits, int tile_n) {
-  const int tile = w / splits, sp = w % splits;
+// large activation operand streams from HBM once while the (small) weight operand stays L2-resident.  Splits are the
+// slowest index: the items resident at once read the same k-range of both operands, which L2 holds for all of them
+// (split-fastest, every resident slice read its own k-range, and the weight gradients split over the tokens streamed
+// each from HBM).  The order items run in does not change their sums or the slab order.
+template <int BN>
+__device__ __forceinline__ WorkRange work_item(int w, int rank, int num_n, int num_tiles, int num_k, int splits) {
+  const int tile = w % num_tiles, sp = w / num_tiles;
   const int per = (num_k + splits - 1) / splits;
   WorkRange r;
-  r.n0 = (2 * (tile % num_pairs) + rank) * tile_n;
-  r.m0 = (tile / num_pairs) * BM;
+  if constexpr (BN == 256) {
+    r.n0 = (tile % num_n) * BN;
+    r.m0 = (2 * (tile / num_n) + rank) * BM;
+  } else {
+    r.n0 = (2 * (tile % num_n) + rank) * BN;
+    r.m0 = (tile / num_n) * BM;
+  }
   r.kb0 = sp * per;
   r.kb1 = min(num_k, r.kb0 + per);
+  r.sp = sp;
   return r;
 }
 
-template <int BN, int A_MN, int B_MN>
-__device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint32_t sa, uint32_t sb, bool first) {
-  // A rows 64-127 start 8 KB into the stage in both layouts (64 rows x 128 B, or the second 64-row box)
+// MH 64-row halves of A starting at `sa` (A rows 64-127 start 8 KB into the stage in both layouts: 64 rows x 128 B, or
+// the second 64-row box) times all BN columns of B, one wgmma chain per half
+template <int MH, int BN, int A_MN, int B_MN>
+__device__ __forceinline__ void mma_kblock(float (&acc)[MH][BN / 2], uint32_t sa, uint32_t sb, bool first) {
   const uint64_t bd = B_MN ? gmma_desc_sw128(sb, 8192, 1024) : gmma_desc_sw128(sb, 16, 1024);
   constexpr uint64_t a_adv = A_MN ? (2048 >> 4) : (32 >> 4);
   constexpr uint64_t b_adv = B_MN ? (2048 >> 4) : (32 >> 4);
@@ -316,9 +339,10 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint32_t sa,
   for (int k = 0; k < BK / 16; ++k) {
     const uint32_t sc = (first && k == 0) ? 0u : 1u;
 #pragma unroll
-    for (int mh = 0; mh < 2; ++mh) {
+    for (int mh = 0; mh < MH; ++mh) {
       const uint64_t ad = A_MN ? gmma_desc_sw128(sa + mh * 8192, 8192, 1024) : gmma_desc_sw128(sa + mh * 8192, 16, 1024);
-      if constexpr (BN == 128) wgmma_m64n128k16_ss<A_MN, B_MN>(acc[mh], ad + k * a_adv, bd + k * b_adv, sc);
+      if constexpr (BN == 256) wgmma_m64n256k16_ss<A_MN, B_MN>(acc[mh], ad + k * a_adv, bd + k * b_adv, sc);
+      else if constexpr (BN == 128) wgmma_m64n128k16_ss<A_MN, B_MN>(acc[mh], ad + k * a_adv, bd + k * b_adv, sc);
       else wgmma_m64n64k16_ss<A_MN, B_MN>(acc[mh], ad + k * a_adv, bd + k * b_adv, sc);
     }
   }
@@ -331,6 +355,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             int M, int N, int K, int splits) {
   constexpr bool staged = kStaged<EF>;   // tmO / tmP (out, pre-activation stash) are used only then
   using C = Cfg<BN, staged>;
+  constexpr bool WIDE = C::WIDE;
+  constexpr int MH = WIDE ? 1 : 2;       // 64-row halves of a tile one consumer computes
+  static_assert(!WIDE || EF != EPI_RUNTIME, "run-time flags run on the 128-wide tile");
   static_assert(2 * C::STAGES * 8 <= C::BAR_BYTES, "mbarriers overflow their slot");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -348,15 +375,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       tma_prefetch_desc(&tmO);
       if constexpr ((EF & EP_STORE_PRE) != 0) tma_prefetch_desc(&tmP);
     }
-    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+    // a stage is released by every consumer that reads it, in both CTAs
+    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], WIDE ? 4 : 2); }
     fence_mbar_init();
   }
   cluster_sync();   // both CTAs' barriers are initialised before either multicasts into or arrives on the other's
 
   const int num_m = (M + BM - 1) / BM;
-  const int num_pairs = ((N + BN - 1) / BN + 1) / 2;
+  const int num_n = WIDE ? (N + BN - 1) / BN : ((N + BN - 1) / BN + 1) / 2;
   const int num_k = (K + BK - 1) / BK;
-  const int num_work = num_m * num_pairs * splits;
+  const int num_tiles = (WIDE ? (num_m + 1) / 2 : num_m) * num_n;
+  const int num_work = num_tiles * splits;
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
@@ -364,23 +393,38 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       int stage = 0;
       uint32_t phase = 0;
       for (int w = cluster; w < num_work; w += num_clusters) {
-        const WorkRange wr = work_item(w, rank, num_pairs, num_k, splits, BN);
+        const WorkRange wr = work_item<BN>(w, rank, num_n, num_tiles, num_k, splits);
         for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * C::STAGE_BYTES;
           uint8_t* sb = sa + C::A_BYTES;
-          // this CTA's 64-row half of A goes to both CTAs; the peer's half completes the other A_BYTES / 2
+          // the shared operand: this CTA's half goes to both CTAs, the peer's half completes the stage's bytes
           mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-          if (A_MN) {
-            tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, wr.m0 + rank * 64, kb * BK, 0b11);
-          } else {
-            tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, kb * BK, wr.m0 + rank * 64, 0b11);
-          }
-          if (B_MN) {
+          if constexpr (WIDE) {            // own 128 rows of A (two 64-row boxes), 128-column half of B to both
 #pragma unroll
-            for (int i = 0; i < BN / 64; ++i) tma_load_2d(&tmB, &full_bar[stage], sb + i * 8192, wr.n0 + i * 64, kb * BK);
-          } else {
-            tma_load_2d(&tmB, &full_bar[stage], sb, kb * BK, wr.n0);
+            for (int i = 0; i < 2; ++i) {
+              if (A_MN) tma_load_2d(&tmA, &full_bar[stage], sa + i * 8192, wr.m0 + i * 64, kb * BK);
+              else tma_load_2d(&tmA, &full_bar[stage], sa + i * 8192, kb * BK, wr.m0 + i * 64);
+            }
+            if (B_MN) {
+#pragma unroll
+              for (int i = 2 * rank; i < 2 * rank + 2; ++i)
+                tma_load_2d_multicast(&tmB, &full_bar[stage], sb + i * 8192, wr.n0 + i * 64, kb * BK, 0b11);
+            } else {
+              tma_load_2d_multicast(&tmB, &full_bar[stage], sb + rank * 16384, kb * BK, wr.n0 + rank * 128, 0b11);
+            }
+          } else {                         // 64-row half of A to both, own B
+            if (A_MN) {
+              tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, wr.m0 + rank * 64, kb * BK, 0b11);
+            } else {
+              tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, kb * BK, wr.m0 + rank * 64, 0b11);
+            }
+            if (B_MN) {
+#pragma unroll
+              for (int i = 0; i < BN / 64; ++i) tma_load_2d(&tmB, &full_bar[stage], sb + i * 8192, wr.n0 + i * 64, kb * BK);
+            } else {
+              tma_load_2d(&tmB, &full_bar[stage], sb, kb * BK, wr.n0);
+            }
           }
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
@@ -388,13 +432,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     }
   } else {
     setmaxnreg_inc<232>();
-    const int cw = wg - 1;                     // consumer warpgroup: tiles j of this CTA with j % 2 == cw
+    // consumer warpgroup: in ping-pong, tiles j of this CTA with j % 2 == cw; WIDE, rows 64 cw .. 64 cw + 63 of every
+    // tile
+    const int cw = wg - 1;
     const int t = threadIdx.x & 127;
     const int r_in = 16 * (t >> 5) + ((t & 31) >> 2);
     const int c_in = 2 * (t & 3);
-    float* const s_bias = vecs + cw * 2 * BN;
+    float* const s_bias = vecs + (WIDE ? 0 : cw * 2 * BN);
     float* const s_gamma = s_bias + BN;
     constexpr bool stage_vecs = EF != EPI_RUNTIME && (EF & (EP_BIAS | EP_GAMMA)) != 0;
+    constexpr int VEC_THREADS = WIDE ? 256 : 128;   // the consumers that read s_bias / s_gamma
+    const int vt = WIDE ? threadIdx.x - 128 : t;
     uint8_t* const stg = smem + C::STG_OFF + cw * STG_BYTES;   // output staging (staged epilogues only)
     const uint32_t peer_empty = mapa_shared(smem_u32(empty_bar), rank ^ 1);   // the peer's empty barriers
     int stg_seq = 0;                           // chunks this consumer has staged
@@ -402,38 +450,38 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     uint32_t phase = 0;
     int j = 0;
     for (int w = cluster; w < num_work; w += num_clusters, ++j) {
-      const WorkRange wr = work_item(w, rank, num_pairs, num_k, splits, BN);
+      const WorkRange wr = work_item<BN>(w, rank, num_n, num_tiles, num_k, splits);
       const int nkb = wr.kb1 > wr.kb0 ? wr.kb1 - wr.kb0 : 0;
-      if ((j & 1) != cw) {                     // the other consumer's tile: step over its fills
+      if (!WIDE && (j & 1) != cw) {            // the other consumer's tile: step over its fills
         stage += nkb;
         phase ^= (stage / C::STAGES) & 1;
         stage %= C::STAGES;
         continue;
       }
       if constexpr (stage_vecs) {
-        named_bar_sync(3 + cw, 128);           // this consumer's previous epilogue has read its bias / gamma
-        if (t < BN && wr.n0 + t < N) {
-          if constexpr ((EF & EP_BIAS) != 0) cp_async_4(s_bias + t, ep.bias + wr.n0 + t);
-          if constexpr ((EF & EP_GAMMA) != 0) cp_async_4(s_gamma + t, ep.gamma + wr.n0 + t);
+        named_bar_sync(3 + cw * !WIDE, VEC_THREADS);   // the previous epilogue has read bias / gamma
+        if (vt < BN && wr.n0 + vt < N) {
+          if constexpr ((EF & EP_BIAS) != 0) cp_async_4(s_bias + vt, ep.bias + wr.n0 + vt);
+          if constexpr ((EF & EP_GAMMA) != 0) cp_async_4(s_gamma + vt, ep.gamma + wr.n0 + vt);
         }
       }
-      if (j > 0) named_bar_sync(1 + cw, 256);  // tile j-1's main loop has passed its last full-barrier wait
-      float acc[2][BN / 2];
+      if (!WIDE && j > 0) named_bar_sync(1 + cw, 256);   // tile j-1's main loop has passed its last full-barrier wait
+      float acc[MH][BN / 2];
 #pragma unroll
-      for (int mh = 0; mh < 2; ++mh)
+      for (int mh = 0; mh < MH; ++mh)
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[mh][i] = 0.f;
       int prev = -1;
       for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
-        fence_regs(acc[0]);
-        fence_regs(acc[1]);
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh) fence_regs(acc[mh]);
         wgmma_fence();
-        mma_kblock<BN, A_MN, B_MN>(acc, sa, sa + C::A_BYTES, kb == wr.kb0);
+        mma_kblock<MH, BN, A_MN, B_MN>(acc, sa + (WIDE ? cw * 8192 : 0), sa + C::A_BYTES, kb == wr.kb0);
         wgmma_commit();
-        fence_regs(acc[0]);
-        fence_regs(acc[1]);
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh) fence_regs(acc[mh]);
         if (prev >= 0) {                       // the k-block before this one has been consumed: release its stage
           wgmma_wait<1>();
           if (t == 0) { mbar_arrive(&empty_bar[prev]); mbar_arrive_cluster(peer_empty + 8 * prev); }
@@ -441,22 +489,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         prev = stage;
         if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
-      if (w + num_clusters < num_work) named_bar_arrive(1 + (cw ^ 1), 256);   // tile j+1 may start its main loop
+      if (!WIDE && w + num_clusters < num_work) named_bar_arrive(1 + (cw ^ 1), 256);   // tile j+1 may start its main loop
       wgmma_wait<0>();
-      fence_regs(acc[0]);
-      fence_regs(acc[1]);
+#pragma unroll
+      for (int mh = 0; mh < MH; ++mh) fence_regs(acc[mh]);
       if (prev >= 0 && t == 0) { mbar_arrive(&empty_bar[prev]); mbar_arrive_cluster(peer_empty + 8 * prev); }
       if constexpr (stage_vecs) {
         cp_async_wait_all();
-        named_bar_sync(3 + cw, 128);           // bias / gamma of this tile are in shared memory
+        named_bar_sync(3 + cw * !WIDE, VEC_THREADS);   // bias / gamma of this tile are in shared memory
       }
       if (nkb <= 0) continue;                  // empty split-K slice: nothing to add
-      const size_t slab_row0 = epi_has<EF>(ep, EP_SLABS) ? (size_t)(w % splits) * M : 0;
+      const size_t slab_row0 = epi_has<EF>(ep, EP_SLABS) ? (size_t)wr.sp * M : 0;
       if constexpr (EF == EPI_RUNTIME) {
         epilogue_tile_runtime<BN>(ep, acc, wr.m0, wr.n0, M, N, slab_row0, r_in, c_in);
       } else {
-        epilogue_tile<BN, EF>(ep, &tmO, &tmP, acc, s_bias, s_gamma, stg, stg_seq, 5 + cw, t, wr.m0, wr.n0, M, N,
-                              slab_row0, r_in, c_in);
+        epilogue_tile<MH, BN, EF>(ep, &tmO, &tmP, acc, s_bias, s_gamma, stg, stg_seq, 5 + cw, t,
+                                  wr.m0 + (WIDE ? cw * 64 : 0), wr.n0, M, N, slab_row0, r_in, c_in);
       }
     }
     if (staged && t == 0) tma_store_wait_all();   // shared memory stays valid until the last store has read it
@@ -517,7 +565,8 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilog
       if (rc) return rc;
     }
   }
-  const int work = ((M + BM - 1) / BM) * (((N + BN - 1) / BN + 1) / 2) * splits;   // work items: tile pairs
+  const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
+  const int work = (BN == 256 ? (num_m + 1) / 2 * num_n : num_m * ((num_n + 1) / 2)) * splits;   // tile pairs
   cfg.gridDim = dim3(2 * (work < max_clusters ? work : max_clusters));
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, to, tp, ep, M, N, K, splits);
   if (e == cudaSuccess) e = cudaPeekAtLastError();
@@ -553,13 +602,20 @@ static int dispatch(int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap
     D3_EPI(1, 1, EP_OUT_F32 | EP_ACCUM)
 #undef D3_EPI
   }
-  if (!a_mn && !b_mn) return launch<BN, 0, 0, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
-  if (!a_mn && b_mn) return launch<BN, 0, 1, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
-  if (a_mn && !b_mn) return launch<BN, 1, 0, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
-  return launch<BN, 1, 1, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
+  // Every other call (run-time flags: D3_EP_SCATTER, misaligned operands, odd N, other flag sets) runs on a 64- or
+  // 128-wide tile: the run-time-flag epilogue is not compiled at BN = 256, whose operand maps are those of BN = 128.
+  if constexpr (BN == 256) {
+    return dispatch<128>(a_mn, b_mn, ta, tb, ep, M, N, K, splits, s);
+  } else {
+    if (!a_mn && !b_mn) return launch<BN, 0, 0, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
+    if (!a_mn && b_mn) return launch<BN, 0, 1, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
+    if (a_mn && !b_mn) return launch<BN, 1, 0, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
+    return launch<BN, 1, 1, EPI_RUNTIME>(ta, tb, ep, M, N, K, splits, s);
+  }
 }
 
-// tile_n: 0 = auto; 64/128 force that tile width; 256 and 512 (wider tiles) are taken as 128.
+// tile_n: 0 = auto (256 for weight gradients, else 64 or 128); 64 / 128 / 256 force that tile width; 512 is taken as
+// 256, the widest tile.
 // split_k: 0 = auto (only when the epilogue is a plain fp32 accumulate-able output), >= 1 forced.
 int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K,
               GemmEpilogue ep, int tile_n, int split_k, cudaStream_t stream) {
@@ -568,8 +624,10 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
     return set_error(D3_ERR_ARG, "gemm: operands must be 16-byte aligned with ld % 8 == 0");
   const int sms = sm_count();
   const int num_k = (K + BK - 1) / BK;
-  // ---- tile choice: fewest waves of (tile width + fixed per-tile cost) over the SMs
-  int bn = tile_n >= 256 ? 128 : tile_n;
+  // ---- tile choice: fewest waves of (tile width + fixed per-tile cost) over the SMs.  BN = 256 is not a candidate
+  //      here: at every forward and input-gradient shape of a ViT-L step it measured slower than 128 (DESIGN.md
+  //      section 4); the weight gradients take it below, after their split count
+  int bn = tile_n >= 256 ? 256 : tile_n;
   if (tile_n == 0) {
     const int cand[2] = {128, 64};
     long best = -1;
@@ -588,7 +646,8 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
   if (split_k >= 1) {
     splits = split_k;
   } else if (plain_f32 && (ep.flags & EP_ACCUM)) {
-    const long units = (long)((M + BM - 1) / BM) * ((N + bn - 1) / bn);
+    const int unit_n = bn < 128 ? bn : 128;   // the tile widths before BN = 256 (its split counts and bits)
+    const long units = (long)((M + BM - 1) / BM) * ((N + unit_n - 1) / unit_n);
     if (units <= sms && num_k >= 16) {
       // fill the SMs; and keep every accumulation chain within 64 k-blocks: the tensor core's fp32 accumulation drifts
       // measurably (> 1e-5 relative) over longer chains, the fp32 reduction of the slices does not
@@ -598,6 +657,10 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
       if (splits < 1) splits = 1;
     }
   }
+  // weight gradients (both operands MN-major) run on the 128 x 256 tile: its M-paired clusters read a third fewer
+  // operand bytes from L2 per FLOP, and their main loops run over the tokens, so the epilogue it does not hide is a
+  // small part of a tile's time.  The split count above stays that of the narrower tile, and so do the bits.
+  if (tile_n == 0 && a_mn && b_mn) bn = 256;
   if (ep.flags & EP_SCATTER) {
     if (!plain_f32) return set_error(D3_ERR_ARG, "gemm: SCATTER needs a plain fp32 output");
     if (ep.sc_world < 1 || ep.sc_world > 8 || ep.sc_shard <= 0 || (ep.sc_shard % 4) || (ep.sc_off % 4) || (ep.ld_out % 4))
@@ -626,7 +689,7 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
   CUtensorMap ta, tb;
   int rc = make_operand_map(&ta, A, M, K, lda, a_mn, 64);   // A arrives as two 64-row halves, one per cluster CTA
   if (rc) return rc;
-  rc = make_operand_map(&tb, B, N, K, ldb, b_mn, bn);
+  rc = make_operand_map(&tb, B, N, K, ldb, b_mn, bn < 128 ? bn : 128);   // BN = 256: one 128-row half per cluster CTA
   if (rc) return rc;
   float* ws = nullptr;
   GemmEpilogue out_ep = ep;
@@ -638,6 +701,7 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
     ep.flags = (ep.flags & ~(EP_ACCUM | EP_SLOW)) | EP_SLABS | (N % 4 ? EP_SLOW : 0);
   }
   switch (bn) {
+    case 256: rc = dispatch<256>(a_mn, b_mn, ta, tb, ep, M, N, K, splits, stream); break;
     case 128: rc = dispatch<128>(a_mn, b_mn, ta, tb, ep, M, N, K, splits, stream); break;
     case 64: rc = dispatch<64>(a_mn, b_mn, ta, tb, ep, M, N, K, splits, stream); break;
     default: rc = set_error(D3_ERR_ARG, "gemm: bad tile N");

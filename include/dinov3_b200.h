@@ -73,7 +73,8 @@ typedef struct {
   long long sc_off;
   int sc_shard, sc_world;
 } d3_gemm_epilogue;
-/* tile_n : 0 = auto; 64 / 128 = 128-row tiles of that width; 256 and 512 (wider tiles) are taken as 128.
+/* tile_n : 0 = auto (256 when both operands are MN-major, else 64 or 128); 64 / 128 / 256 = 128-row tiles of that
+ *          width; 512 is taken as 256.
  * split_k: 0 = auto (used only for plain fp32 outputs with D3_EP_ACCUM, i.e. weight gradients: the slices' partial sums
  *          are added to `out`, which the caller zeroes or wants accumulated into, in slice order); >= 1 = forced.  */
 int d3_gemm_bf16(const void* A, int lda, int a_major, const void* B, int ldb, int b_major, int M, int N, int K,
