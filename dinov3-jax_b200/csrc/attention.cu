@@ -14,6 +14,9 @@
 // Crops longer than the resident kernels hold (span > 448 forward, N > 256 backward; G = 1 there) take streamed kernels
 // with the same per-tile arithmetic: a producer warpgroup fills an mbarrier ring of 128-row K / V (or Q / dO) tiles that both
 // consumer warpgroups read, so shared memory no longer grows with N.  Any N up to ATTN_MAX_TOKENS.
+//
+// head_dim 128 (vit_7b) has kernels of its own, after the head_dim 64 ones; d3_attn_fwd / d3_attn_bwd pick the family
+// from D / H.
 #include "ptx.cuh"
 #include <climits>
 #include <cstdlib>
@@ -60,10 +63,10 @@ __device__ __forceinline__ RowInfo row_info(const AttnShape& sh, int c, int q) {
 }
 
 // Online softmax of one block of 8*NI keys starting at key k0, on the S accumulator fragment (this thread: rows ri[0],
-// ri[1], columns k0 + 8i + c2 + {0,1}).  S becomes P; the running max m, sum l and the output accumulator o are rescaled.
-// Keys outside a row's [klo, khi) give exactly 0.
-template <int NI>
-__device__ __forceinline__ void online_softmax(float (&s)[4 * NI], float (&o)[32], float (&m)[2], float (&l)[2],
+// ri[1], columns k0 + 8i + c2 + {0,1}).  S becomes P; the running max m, sum l and the output accumulator o (NO = head_dim
+// / 2 registers) are rescaled.  Keys outside a row's [klo, khi) give exactly 0.
+template <int NI, int NO>
+__device__ __forceinline__ void online_softmax(float (&s)[4 * NI], float (&o)[NO], float (&m)[2], float (&l)[2],
                                                const RowInfo (&ri)[2], int k0, int c2, float cs) {
   const int kb0 = k0 + c2;
   const bool full = k0 >= max(ri[0].klo, ri[1].klo) && k0 + 8 * NI <= min(ri[0].khi, ri[1].khi);
@@ -94,12 +97,14 @@ __device__ __forceinline__ void online_softmax(float (&s)[4 * NI], float (&o)[32
       const float p = (full || (kk >= ri[hh].klo && kk < ri[hh].khi)) ? ex2_approx(fmaf(s[4 * i + j], cs, -ms[hh])) : 0.f;
       s[4 * i + j] = p;
       l[hh] += p;
-      if (i < 8) o[4 * i + j] *= corr[hh];
+      if (i < NO / 4) o[4 * i + j] *= corr[hh];
     }
 }
 
 // O = o / l as bf16 and the natural-log LSE of the scaled scores ([crop, head, token]) for this thread's two rows
-__device__ __forceinline__ void store_o_lse(const float (&o)[32], float (&l)[2], const float (&m)[2], const RowInfo (&ri)[2],
+// (head_dim = 2 * NO)
+template <int NO>
+__device__ __forceinline__ void store_o_lse(const float (&o)[NO], float (&l)[2], const float (&m)[2], const RowInfo (&ri)[2],
                                             const AttnShape& sh, int c, int h, int row_base, int wq0, int r_in, int c2,
                                             __nv_bfloat16* O, float* LSE) {
 #pragma unroll
@@ -109,9 +114,9 @@ __device__ __forceinline__ void store_o_lse(const float (&o)[32], float (&l)[2],
     const int q = wq0 + r_in + 8 * hh;
     if (!ri[hh].ok) continue;
     const float inv = 1.f / l[hh];
-    __nv_bfloat16* dst = O + (size_t)(row_base + q) * sh.D + h * 64 + c2;
+    __nv_bfloat16* dst = O + (size_t)(row_base + q) * sh.D + h * (2 * NO) + c2;
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
+    for (int i = 0; i < NO / 4; ++i)
       *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
     if (LSE && c2 == 0)
       LSE[((size_t)(c * sh.G + ri[hh].g) * sh.H + h) * sh.N + (q - ri[hh].klo)] = m[hh] * sh.scale + logf(l[hh]);
@@ -300,9 +305,12 @@ attn_fwd_stream_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
 }
 
 // Delta[c,h,q] = sum_d dO[q, h, d] * O[q, h, d]    (backward softmax term)
+template <int HD>
 __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ O, const __nv_bfloat16* __restrict__ dO,
                                   float* __restrict__ delta, long T, int N, int D, int H) {
-  // 8 threads per (row, head): one 16-byte load of O and of dO each, 3 shuffle steps inside the 8-lane group
+  // HD / 8 threads per (row, head): one 16-byte load of O and of dO each, log2(HD / 8) shuffle steps inside the group
+  constexpr int LANES = HD / 8;
+  static_assert(LANES == 8 || LANES == 16, "head_dim 64 or 128");
   const long g = blockIdx.x * (long)blockDim.x + threadIdx.x;
   const int per_row = D >> 3;
   const bool ok = g < T * per_row;
@@ -318,10 +326,11 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ O, const __n
     const float2 b0 = unpack_bf16(b.x), b1 = unpack_bf16(b.y), b2 = unpack_bf16(b.z), b3 = unpack_bf16(b.w);
     s = a0.x * b0.x + a0.y * b0.y + a1.x * b1.x + a1.y * b1.y + a2.x * b2.x + a2.y * b2.y + a3.x * b3.x + a3.y * b3.y;
   }
+  if (LANES == 16) s += __shfl_xor_sync(0xffffffffu, s, 8);
   s += __shfl_xor_sync(0xffffffffu, s, 4);
   s += __shfl_xor_sync(0xffffffffu, s, 2);
   s += __shfl_xor_sync(0xffffffffu, s, 1);
-  if (ok && (c8 & 7) == 0) delta[((row / N) * H + (c8 >> 3)) * N + (row % N)] = s;
+  if (ok && (c8 & (LANES - 1)) == 0) delta[((row / N) * H + (c8 >> (LANES == 16 ? 4 : 3))) * N + (row % N)] = s;
 }
 
 // ------------------------------------------------------------------------------------------------ backward
@@ -331,34 +340,37 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ O, const __n
 // Crop groups of span <= 256 take attn_bwd_fused_kernel (all of it in one pass); longer crops the streamed pair below,
 // which shares the helpers p_ds_tile / stash_p_ds / dkdv_mma / dq_mma.
 // inverse RoPE on the gradient: transpose of y = x*cos + rot_half(x)*sin (dinov3_jax/layers/attention.py:14-20); this
-// thread holds columns d = 8i + c2 + {0,1} of a row, i.e. both partners (d, d + 32) of every rotation pair it touches.
-__device__ __forceinline__ void store_grad_rows(float (&a)[32], const AttnShape& sh, int c, int row_base, int tile_row0,
+// thread holds columns d = 8i + c2 + {0,1} of a row, i.e. both partners (d, d + head_dim / 2) of every rotation pair it
+// touches.  head_dim = 2 * NA; the tables are [P, head_dim].
+template <int NA>
+__device__ __forceinline__ void store_grad_rows(float (&a)[NA], const AttnShape& sh, int c, int row_base, int tile_row0,
                                                 int r_in, int c2, int h, int third, bool rope, __nv_bfloat16* dQKV) {
+  constexpr int HD = 2 * NA;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int row = tile_row0 + r_in + 8 * hh;
     const RowInfo ri = row_info(sh, c, row);
     if (!ri.ok) continue;
     const int tok = row - ri.klo;
-    float v[16];
+    float v[NA / 2];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) { v[2 * i] = a[4 * i + 2 * hh]; v[2 * i + 1] = a[4 * i + 2 * hh + 1]; }
+    for (int i = 0; i < NA / 4; ++i) { v[2 * i] = a[4 * i + 2 * hh]; v[2 * i + 1] = a[4 * i + 2 * hh + 1]; }
     if (rope && sh.sin_t && tok >= sh.prefix) {
-      const float* sn = sh.sin_t + (size_t)(tok - sh.prefix) * 64;
-      const float* cn = sh.cos_t + (size_t)(tok - sh.prefix) * 64;
+      const float* sn = sh.sin_t + (size_t)(tok - sh.prefix) * HD;
+      const float* cn = sh.cos_t + (size_t)(tok - sh.prefix) * HD;
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+      for (int i = 0; i < NA / 8; ++i)
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
           const int d = 8 * i + c2 + j;
-          const float lo = v[2 * i + j], hi = v[2 * (i + 4) + j];
+          const float lo = v[2 * i + j], hi = v[2 * (i + NA / 8) + j];
           v[2 * i + j] = lo * cn[d] + hi * sn[d];
-          v[2 * (i + 4) + j] = hi * cn[d] - lo * sn[d];
+          v[2 * (i + NA / 8) + j] = hi * cn[d] - lo * sn[d];
         }
     }
-    __nv_bfloat16* dst = dQKV + (size_t)(row_base + row) * (3 * sh.D) + third * sh.D + h * 64 + c2;
+    __nv_bfloat16* dst = dQKV + (size_t)(row_base + row) * (3 * sh.D) + third * sh.D + h * HD + c2;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16(v[2 * i], v[2 * i + 1]);
+    for (int i = 0; i < NA / 4; ++i) *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16(v[2 * i], v[2 * i + 1]);
   }
 }
 
@@ -490,9 +502,10 @@ __device__ __forceinline__ uint64_t desc_here(const void* p, uint32_t lbo, uint3
 }
 
 // registers of the RS A fragments stay untouched until the wgmma reading them has completed
-__device__ __forceinline__ void fence_frag(uint32_t (&a)[4][4]) {
+template <int R>
+__device__ __forceinline__ void fence_frag(uint32_t (&a)[R][4]) {
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
+  for (int i = 0; i < R; ++i)
 #pragma unroll
     for (int e = 0; e < 4; ++e) asm volatile("" : "+r"(a[i][e])::"memory");
 }
@@ -837,6 +850,376 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_const
   store_grad_rows(dq, sh, c, row_base, wq0, r_in, c2, h, 0, true, dQKV);
 }
 
+// ------------------------------------------------------------------------------------------------ head_dim 128
+// ViT-7B (embed 4096, 32 heads).  A 128-row x 128-column bf16 tile is two 64-column SWIZZLE_128B chunks of 16 KB (one TMA
+// box each, chunk j at +16 KB): K-major operands walk 8 k16 steps, 4 per chunk; the MN-major B operands of the P V,
+// P^T dO, dS^T Q and dS K products span both chunks with N = 128 (LBO = 16 KB).  Three kernels serve every N up to
+// ATTN_MAX_TOKENS and every packing of attn_shape: one CTA owns a crop group of span = G * N rows, short crops keep the
+// block-diagonal mask of row_info.  Each has the streamed kernels' producer warpgroup and ring protocol, with
+// HD128_STAGES stages of two 32 KB tiles (K | V or Q | dO):
+//   forward  one CTA per (128-row query tile, head, crop group), Q resident.  Per 128-key tile and consumer warpgroup:
+//            S = Q K^T (m64n128), online softmax, O += P V (RS m64n128, 8 k-steps).  Scores and O: 64 + 64 registers.
+//   dK / dV  one CTA per (128-key tile, head, crop group), K / V resident, Q / dO stream.  Keys on the accumulator rows
+//            as in attn_bwd_fused_kernel; per 32 query columns: S^T = K Q^T and dP^T = V dO^T (m64n32), then
+//            dV += P^T dO and dK += dS^T Q (RS m64n128).  dK + dV take 128 registers, the scores 32.
+//   dQ       one CTA per (128-row query tile, head, crop group), Q / dO resident, K / V stream.  Per half of 64 keys:
+//            S and dP (m64n64), dQ += dS K (RS m64n128).
+// Every output row is written once by one CTA and every sum runs over the tiles in ascending order: no atomics, the
+// same bits on every run.  Shared memory: 32 KB (forward) or 64 KB (backward) resident + 2 x 64 KB ring + 1 KB alignment.
+constexpr int HD128_STAGES = 2;
+constexpr int HD128_FWD_SMEM = 32768 + HD128_STAGES * 65536 + (2 * HD128_STAGES + 1) * 8 + 1024;
+constexpr int HD128_BWD_SMEM = 65536 + HD128_STAGES * 65536 + (2 * HD128_STAGES + 1) * 8 + 1024;
+
+// K-major descriptor of k16 step k (0..7) of a 128-column tile whose first chunk (at the operand's first row) is p
+__device__ __forceinline__ uint64_t kdesc128(const uint8_t* p, int k) {
+  return gmma_desc_sw128(smem_u32(p + (k >> 2) * 16384), 16, 1024) + 2 * (k & 3);
+}
+
+// 128 rows x 128 columns starting at column `col`: two 64-column boxes
+__device__ __forceinline__ void tma_load_tile128(const CUtensorMap* m, uint64_t* bar, uint8_t* dst, int col, int row) {
+  tma_load_2d(m, bar, dst, col, row);
+  tma_load_2d(m, bar, dst + 16384, col + 64, row);
+}
+
+__device__ __forceinline__ uint8_t* smem_base_1024(uint8_t* raw) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
+}
+
+__global__ void __launch_bounds__(RING_THREADS, 1)
+attn_fwd_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ O, float* __restrict__ LSE,
+                      const AttnShape sh) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_base_1024(smem_raw);
+  // layout: [Q 32 KB][STAGES x (K 32 KB, V 32 KB)][full][empty][q barrier]
+  uint8_t* sQ = smem;
+  uint8_t* ring = smem + 32768;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + HD128_STAGES * 65536);
+  uint64_t* empty = full + HD128_STAGES;
+  uint64_t* bar_q = empty + HD128_STAGES;
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int qt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
+  const int q0 = qt * 128, row_base = c * sh.span, nkb = (sh.span + 127) >> 7;
+  const int n_wg = (q0 + 64 < sh.span) ? 2 : 1;   // consumer warpgroups with at least one query row in the group
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    for (int st = 0; st < HD128_STAGES; ++st) {
+      mbar_init(full + st, 1);
+      mbar_init(empty + st, 4 * n_wg);
+    }
+    mbar_init(bar_q, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 288 && elect_one()) {
+      mbar_expect_tx(bar_q, 32768);
+      tma_load_tile128(&tmQKV, bar_q, sQ, h * 128, row_base + q0);
+      for (int b = 0; b < nkb; ++b) {
+        const int st = b % HD128_STAGES, u = b / HD128_STAGES;
+        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
+        mbar_expect_tx(full + st, 65536);
+        tma_load_tile128(&tmQKV, full + st, ring + st * 65536, sh.D + h * 128, row_base + b * 128);
+        tma_load_tile128(&tmQKV, full + st, ring + st * 65536 + 32768, 2 * sh.D + h * 128, row_base + b * 128);
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int wq0 = q0 + wg * 64;
+  if (wq0 >= sh.span) return;                  // not counted by the empty barriers (n_wg)
+  mbar_wait(bar_q, 0);
+
+  const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
+  RowInfo ri[2];
+  ri[0] = row_info(sh, c, wq0 + r_in);
+  ri[1] = row_info(sh, c, wq0 + r_in + 8);
+  const float cs = sh.scale * LOG2E;
+  float m[2] = {-3.0e38f, -3.0e38f}, l[2] = {0.f, 0.f};
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+
+#pragma unroll 1
+  for (int b = 0; b < nkb; ++b) {
+    const int st = b % HD128_STAGES;
+    uint8_t* sK = ring + st * 65536;
+    mbar_wait(full + st, (b / HD128_STAGES) & 1);
+    float s[64];
+    fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      wgmma_m64n128k16_ss<0, 0>(s, kdesc128(sQ + wg * 8192, k), kdesc128(sK, k), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    online_softmax<16>(s, o, m, l, ri, b * 128, c2, cs);
+    uint32_t a[8][4];
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) a[kk][e] = pack_bf16(s[8 * kk + 2 * e], s[8 * kk + 2 * e + 1]);
+    const uint64_t vd = desc_here(sK + 32768, 16384, 1024);   // V MN-major: 16 keys per k-step, d chunks 16 KB apart
+    fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_m64n128k16_rs<1>(o, a[kk], vd + 128 * kk, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
+    if (lane_id() == 0) mbar_arrive(empty + st);   // this warp no longer reads the stage
+  }
+  store_o_lse(o, l, m, ri, sh, c, h, row_base, wq0, r_in, c2, O, LSE);
+}
+
+// lse * log2(e) and Delta of token row q of the crop group (0 for rows outside it)
+__device__ __forceinline__ void row_stats(const AttnShape& sh, const float* __restrict__ LSE, const float* __restrict__ Delta,
+                                          int c, int h, int q, float& lse2, float& dl) {
+  const RowInfo ri = row_info(sh, c, q);
+  const size_t stat = ((size_t)(c * sh.G + ri.g) * sh.H + h) * sh.N + (ri.ok ? q - ri.klo : 0);
+  lse2 = ri.ok ? LSE[stat] * LOG2E : 0.f;
+  dl = ri.ok ? Delta[stat] : 0.f;
+}
+
+__global__ void __launch_bounds__(RING_THREADS, 1)
+attn_bwd_dkdv_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
+                           const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
+                           const AttnShape sh) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_base_1024(smem_raw);
+  // layout: [K 32 KB][V 32 KB][STAGES x (Q 32 KB, dO 32 KB)][full][empty][kv barrier]
+  uint8_t* sK = smem;
+  uint8_t* sV = smem + 32768;
+  uint8_t* ring = smem + 65536;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + HD128_STAGES * 65536);
+  uint64_t* empty = full + HD128_STAGES;
+  uint64_t* bar_kv = empty + HD128_STAGES;
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
+  const int kt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
+  const int row_base = c * sh.span, nq = (sh.span + 127) >> 7;
+  const int n_wg = (kt * 128 + 64 < sh.span) ? 2 : 1;   // consumer warpgroups with at least one key row in the group
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    tma_prefetch_desc(&tmDO);
+    for (int st = 0; st < HD128_STAGES; ++st) {
+      mbar_init(full + st, 1);
+      mbar_init(empty + st, 4 * n_wg);
+    }
+    mbar_init(bar_kv, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 288 && elect_one()) {
+      mbar_expect_tx(bar_kv, 65536);
+      tma_load_tile128(&tmQKV, bar_kv, sK, sh.D + h * 128, row_base + kt * 128);
+      tma_load_tile128(&tmQKV, bar_kv, sV, 2 * sh.D + h * 128, row_base + kt * 128);
+      for (int qt = 0; qt < nq; ++qt) {
+        const int st = qt % HD128_STAGES, u = qt / HD128_STAGES;
+        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
+        mbar_expect_tx(full + st, 65536);
+        tma_load_tile128(&tmQKV, full + st, ring + st * 65536, h * 128, row_base + qt * 128);
+        tma_load_tile128(&tmDO, full + st, ring + st * 65536 + 32768, h * 128, row_base + qt * 128);
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int wk0 = kt * 128 + wg * 64;
+  if (wk0 >= sh.span) return;                  // not counted by the empty barriers (n_wg)
+  mbar_wait(bar_kv, 0);
+  // valid query columns of this thread's two key rows: the key's own crop (none for keys outside the group)
+  int lo[2], hi[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const RowInfo ri = row_info(sh, c, wk0 + r_in + 8 * hh);
+    lo[hh] = ri.ok ? ri.klo : 0;
+    hi[hh] = ri.ok ? ri.khi : 0;
+  }
+  const float cs = sh.scale * LOG2E;
+  float dk[64], dv[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
+#pragma unroll 1
+  for (int qt = 0; qt < nq; ++qt) {
+    const int st = qt % HD128_STAGES;
+    const uint8_t* sQt = ring + st * 65536;
+    const uint8_t* sDOt = sQt + 32768;
+    mbar_wait(full + st, (qt / HD128_STAGES) & 1);
+#pragma unroll 1
+    for (int qc = 0; qc < 4; ++qc) {   // 32 query columns at a time: with dK + dV resident, 64 would spill
+      float s[16], dp[16];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {   // S^T and dP^T are independent accumulator chains: interleave them
+        wgmma_m64n32k16_ss<0, 0>(s, kdesc128(sK + wg * 8192, k), kdesc128(sQt + qc * 4096, k), k > 0 ? 1u : 0u);
+        wgmma_m64n32k16_ss<0, 0>(dp, kdesc128(sV + wg * 8192, k), kdesc128(sDOt + qc * 4096, k), k > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+      fence_regs(dp);
+      uint32_t pa[2][4], da[2][4];    // bf16 A fragments of P^T / dS^T (k-step kk: query columns 16 kk ..)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int q = qt * 128 + qc * 32 + 8 * i + c2;
+        float l2[2], dl[2];
+        row_stats(sh, LSE, Delta, c, h, q, l2[0], dl[0]);
+        row_stats(sh, LSE, Delta, c, h, q + 1, l2[1], dl[1]);
+        float pv[4], dv4[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int hh = j >> 1, qq = q + (j & 1);
+          const bool ok = qq >= lo[hh] && qq < hi[hh];
+          const float p = ok ? ex2_approx(fmaf(s[4 * i + j], cs, -l2[j & 1])) : 0.f;
+          dv4[j] = ok ? (p * sh.scale) * (dp[4 * i + j] - dl[j & 1]) : 0.f;
+          pv[j] = p;
+        }
+        pa[i >> 1][2 * (i & 1)] = pack_bf16(pv[0], pv[1]);
+        pa[i >> 1][2 * (i & 1) + 1] = pack_bf16(pv[2], pv[3]);
+        da[i >> 1][2 * (i & 1)] = pack_bf16(dv4[0], dv4[1]);
+        da[i >> 1][2 * (i & 1) + 1] = pack_bf16(dv4[2], dv4[3]);
+      }
+      const uint64_t dod = desc_here(sDOt + qc * 4096, 16384, 1024);   // B MN-major: 16 query rows per k-step
+      const uint64_t qd = desc_here(sQt + qc * 4096, 16384, 1024);
+      fence_regs(dk);
+      fence_regs(dv);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 2; ++kk) {
+        wgmma_m64n128k16_rs<1>(dv, pa[kk], dod + 128 * kk, 1u);
+        wgmma_m64n128k16_rs<1>(dk, da[kk], qd + 128 * kk, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(dk);
+      fence_regs(dv);
+      fence_frag(pa);
+      fence_frag(da);
+    }
+    if (lane_id() == 0) mbar_arrive(empty + st);   // this warp no longer reads the stage
+  }
+  store_grad_rows(dk, sh, c, row_base, wk0, r_in, c2, h, 1, true, dQKV);
+  store_grad_rows(dv, sh, c, row_base, wk0, r_in, c2, h, 2, false, dQKV);
+}
+
+__global__ void __launch_bounds__(RING_THREADS, 1)
+attn_bwd_dq_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
+                         const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
+                         const AttnShape sh) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_base_1024(smem_raw);
+  // layout: [Q 32 KB][dO 32 KB][STAGES x (K 32 KB, V 32 KB)][full][empty][q barrier]
+  uint8_t* sQ = smem;
+  uint8_t* sDO = smem + 32768;
+  uint8_t* ring = smem + 65536;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + HD128_STAGES * 65536);
+  uint64_t* empty = full + HD128_STAGES;
+  uint64_t* bar_q = empty + HD128_STAGES;
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
+  const int qt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
+  const int q0 = qt * 128, row_base = c * sh.span, nk = (sh.span + 127) >> 7;
+  const int n_wg = (q0 + 64 < sh.span) ? 2 : 1;   // consumer warpgroups with at least one query row in the group
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    tma_prefetch_desc(&tmDO);
+    for (int st = 0; st < HD128_STAGES; ++st) {
+      mbar_init(full + st, 1);
+      mbar_init(empty + st, 4 * n_wg);
+    }
+    mbar_init(bar_q, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 288 && elect_one()) {
+      mbar_expect_tx(bar_q, 65536);
+      tma_load_tile128(&tmQKV, bar_q, sQ, h * 128, row_base + q0);
+      tma_load_tile128(&tmDO, bar_q, sDO, h * 128, row_base + q0);
+      for (int kt = 0; kt < nk; ++kt) {
+        const int st = kt % HD128_STAGES, u = kt / HD128_STAGES;
+        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
+        mbar_expect_tx(full + st, 65536);
+        tma_load_tile128(&tmQKV, full + st, ring + st * 65536, sh.D + h * 128, row_base + kt * 128);
+        tma_load_tile128(&tmQKV, full + st, ring + st * 65536 + 32768, 2 * sh.D + h * 128, row_base + kt * 128);
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int wq0 = q0 + wg * 64;
+  if (wq0 >= sh.span) return;                  // not counted by the empty barriers (n_wg)
+  mbar_wait(bar_q, 0);
+  float lse2[2], dl[2];
+  int lo[2], hi[2];                            // valid key columns of this thread's two query rows
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const RowInfo ri = row_info(sh, c, wq0 + r_in + 8 * hh);
+    row_stats(sh, LSE, Delta, c, h, wq0 + r_in + 8 * hh, lse2[hh], dl[hh]);
+    lo[hh] = ri.ok ? ri.klo : 0;
+    hi[hh] = ri.ok ? ri.khi : 0;
+  }
+  const float cs = sh.scale * LOG2E;
+  float dq[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) dq[i] = 0.f;
+#pragma unroll 1
+  for (int kt = 0; kt < nk; ++kt) {
+    const int st = kt % HD128_STAGES;
+    const uint8_t* sK = ring + st * 65536;
+    const uint8_t* sV = sK + 32768;
+    mbar_wait(full + st, (kt / HD128_STAGES) & 1);
+#pragma unroll 1
+    for (int hf = 0; hf < 2; ++hf) {
+      float s[32], dp[32];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        wgmma_m64n64k16_ss<0, 0>(s, kdesc128(sQ + wg * 8192, k), kdesc128(sK + hf * 8192, k), k > 0 ? 1u : 0u);
+        wgmma_m64n64k16_ss<0, 0>(dp, kdesc128(sDO + wg * 8192, k), kdesc128(sV + hf * 8192, k), k > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+      fence_regs(dp);
+      uint32_t da[4][4];              // bf16 A fragments of dS (k-step kk: keys 16 kk ..)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int key = kt * 128 + hf * 64 + 8 * i + c2;
+        float d4[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int hh = j >> 1, kk = key + (j & 1);
+          const bool ok = kk >= lo[hh] && kk < hi[hh];
+          const float p = ok ? ex2_approx(fmaf(s[4 * i + j], cs, -lse2[hh])) : 0.f;
+          d4[j] = ok ? (p * sh.scale) * (dp[4 * i + j] - dl[hh]) : 0.f;
+        }
+        da[i >> 1][2 * (i & 1)] = pack_bf16(d4[0], d4[1]);
+        da[i >> 1][2 * (i & 1) + 1] = pack_bf16(d4[2], d4[3]);
+      }
+      const uint64_t kd = desc_here(sK + hf * 8192, 16384, 1024);   // B MN-major: 16 keys per k-step
+      fence_regs(dq);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_m64n128k16_rs<1>(dq, da[kk], kd + 128 * kk, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(dq);
+      fence_frag(da);
+    }
+    if (lane_id() == 0) mbar_arrive(empty + st);   // this warp no longer reads the stage
+  }
+  store_grad_rows(dq, sh, c, row_base, wq0, r_in, c2, h, 0, true, dQKV);
+}
+
 static int make_map(CUtensorMap* map, const void* ptr, long rows, int cols, int ld, int box_rows) {
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
@@ -853,11 +1236,12 @@ constexpr int ATTN_FWD_RESIDENT_SPAN = 448;   // attn_fwd_kernel: Q and all of K
 constexpr int ATTN_BWD_RESIDENT_SPAN = 256;   // attn_bwd_fused_kernel: all Q / dO / K / V tiles of a crop group resident
 
 static int attn_shape(AttnShape* s, int n_crops, int N, int D, int H) {
-  if (D != H * 64) return set_error(D3_ERR_ARG, "attention: head_dim must be 64");
+  if (D != H * 64 && D != H * 128) return set_error(D3_ERR_ARG, "attention: head_dim must be 64 or 128");
   if (N <= 0 || n_crops <= 0) return set_error(D3_ERR_ARG, "attention: empty problem");
   if (N > ATTN_MAX_TOKENS) return set_error(D3_ERR_ARG, "attention: N > 32768 tokens per crop");
   if ((long)n_crops * N > INT_MAX) return set_error(D3_ERR_ARG, "attention: n_crops * N must be below 2^31 token rows");
-  s->N = N; s->D = D; s->H = H; s->scale = 0.125f; s->n_crops = n_crops;
+  s->N = N; s->D = D; s->H = H; s->n_crops = n_crops;
+  s->scale = (D == H * 64) ? 0.125f : 0.08838834764831845f;   // head_dim^-0.5
   s->sin_t = nullptr; s->cos_t = nullptr; s->prefix = 0;
   s->G = (N <= 64) ? (128 / N) : 1;                 // short crops: several per 128-row tile, block-diagonal mask
   if (s->G > n_crops) s->G = n_crops;
@@ -870,6 +1254,14 @@ static int attn_shape(AttnShape* s, int n_crops, int N, int D, int H) {
 static int stream_grid(const AttnShape& s, dim3* grid) {
   if (s.H > 65535 || s.n_crops > 65535) return set_error(D3_ERR_ARG, "attention: H and n_crops must be <= 65535 for long crops");
   *grid = dim3((s.N + 127) / 128, s.H, s.n_crops);
+  return D3_OK;
+}
+
+// grid of the head_dim 128 kernels: (128-row tiles of a crop group, head, crop group)
+static int hd128_grid(const AttnShape& s, dim3* grid) {
+  const int groups = (s.n_crops + s.G - 1) / s.G;
+  if (s.H > 65535 || groups > 65535) return set_error(D3_ERR_ARG, "attention: H and crop groups must be <= 65535 at head_dim 128");
+  *grid = dim3((s.span + 127) / 128, s.H, groups);
   return D3_OK;
 }
 
@@ -889,6 +1281,21 @@ int d3_attn_fwd(const void* qkv, void* o, float* lse, int n_crops, int N, int D,
   int rc = attn_shape(&s, n_crops, N, D, H);
   if (rc) return rc;
   const long T = (long)n_crops * N;
+  if (D == H * 128) {
+    dim3 grid;
+    if ((rc = hd128_grid(s, &grid))) return rc;
+    CUtensorMap tqkv;
+    if ((rc = make_map(&tqkv, qkv, T, 3 * D, 3 * D, 128))) return rc;
+    static bool cfg128 = false;
+    if (!cfg128) {
+      cudaFuncSetAttribute(attn_fwd_hd128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HD128_FWD_SMEM);
+      cfg128 = true;
+    }
+    attn_fwd_hd128_kernel<<<grid, RING_THREADS, HD128_FWD_SMEM, reinterpret_cast<cudaStream_t>(stream)>>>(
+        tqkv, (__nv_bfloat16*)o, lse, s);
+    D3_CHECK_LAUNCH();
+    return D3_OK;
+  }
   if (s.span > ATTN_FWD_RESIDENT_SPAN) {
     dim3 grid;
     if ((rc = stream_grid(s, &grid))) return rc;
@@ -925,19 +1332,41 @@ int d3_attn_bwd(const void* qkv, const void* o, const void* d_o, const float* ls
   if (rc) return rc;
   if ((rope_sin == nullptr) != (rope_cos == nullptr)) return set_error(D3_ERR_ARG, "d3_attn_bwd: sin/cos tables");
   if (!delta_scratch) return set_error(D3_ERR_ARG, "d3_attn_bwd: delta scratch buffer");
+  const bool hd128 = D == H * 128;
   const bool streamed = s.span > ATTN_BWD_RESIDENT_SPAN;
   dim3 sgrid;
-  if (streamed && (rc = stream_grid(s, &sgrid))) return rc;
+  if (hd128 && (rc = hd128_grid(s, &sgrid))) return rc;
+  if (!hd128 && streamed && (rc = stream_grid(s, &sgrid))) return rc;
   s.sin_t = rope_sin; s.cos_t = rope_cos; s.prefix = rope_prefix;
   const long T = (long)n_crops * N;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long threads = T * (D / 8);
-  attn_delta_kernel<<<(int)((threads + 255) / 256), 256, 0, st>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o,
-                                                                delta_scratch, T, N, D, H);
+  if (hd128)
+    attn_delta_kernel<128><<<(int)((threads + 255) / 256), 256, 0, st>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o,
+                                                                       delta_scratch, T, N, D, H);
+  else
+    attn_delta_kernel<64><<<(int)((threads + 255) / 256), 256, 0, st>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o,
+                                                                      delta_scratch, T, N, D, H);
   D3_CHECK_LAUNCH();
   CUtensorMap tqkv, tdo;
   if ((rc = make_map(&tqkv, qkv, T, 3 * D, 3 * D, 128))) return rc;
   if ((rc = make_map(&tdo, d_o, T, D, D, 128))) return rc;
+  if (hd128) {
+    static bool cfg128 = false;
+    if (!cfg128) {
+      cudaFuncSetAttribute(attn_bwd_dkdv_hd128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HD128_BWD_SMEM);
+      cudaFuncSetAttribute(attn_bwd_dq_hd128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HD128_BWD_SMEM);
+      cfg128 = true;
+    }
+    // key tiles and query tiles of a crop group are both (span + 127) / 128: one grid shape for the two kernels
+    attn_bwd_dkdv_hd128_kernel<<<sgrid, RING_THREADS, HD128_BWD_SMEM, st>>>(tqkv, tdo, lse, delta_scratch,
+                                                                             (__nv_bfloat16*)dqkv, s);
+    D3_CHECK_LAUNCH();
+    attn_bwd_dq_hd128_kernel<<<sgrid, RING_THREADS, HD128_BWD_SMEM, st>>>(tqkv, tdo, lse, delta_scratch,
+                                                                           (__nv_bfloat16*)dqkv, s);
+    D3_CHECK_LAUNCH();
+    return D3_OK;
+  }
   if (streamed) {
     const int smem_kv = 16384 * 2 + 32768 * 2 + DKDV_STAGES * 32768 + (2 * DKDV_STAGES + 1) * 8 + 1024;
     const int smem_q = 16384 * 2 + DQ_STAGES * 32768 + (2 * DQ_STAGES + 1) * 8 + 1024;

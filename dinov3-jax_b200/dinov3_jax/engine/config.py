@@ -14,7 +14,10 @@ ARCHS = {  # name -> (embed_dim, depth, heads)
     "vit_so400m": (1152, 27, 18),
     "vit_huge2": (1280, 32, 20),
     "vit_giant2": (1536, 40, 24),
+    "vit_7b": (4096, 40, 32),        # head_dim 128
 }
+# constructor defaults of a factory beyond the table (models/vision_transformer.py:400-408: vit_7b has ffn_ratio 3)
+ARCH_DEFAULTS = {"vit_7b": {"ffn_ratio": 3.0}}
 
 
 @dataclass(frozen=True)
@@ -100,7 +103,7 @@ class EngineConfig:
 
 def config_for(arch: str, **kw) -> EngineConfig:
     d, l, h = ARCHS[arch]
-    return replace(EngineConfig(embed_dim=d, depth=l, heads=h), **kw)
+    return replace(EngineConfig(embed_dim=d, depth=l, heads=h), **{**ARCH_DEFAULTS.get(arch, {}), **kw})
 
 
 def from_oracle_cfg(c) -> EngineConfig:
@@ -182,6 +185,13 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
     arch = cfg.student.arch
     if arch not in ARCHS:
         raise ValueError(f"unknown student.arch {arch!r}")
+    if arch == "vit_7b":
+        # the shipped 7B recipes set these; the engine's blocks always carry a qkv bias and one shared cls norm
+        if not g(cfg.student, "qkv_bias", True):
+            raise NotImplementedError("student.qkv_bias=false is not on the GPU path (every block has a qkv bias)")
+        for key in ("untie_cls_and_patch_norms", "untie_global_and_local_cls_norm"):
+            if g(cfg.student, key, False):
+                raise NotImplementedError(f"student.{key}=true is not on the GPU path (one final norm for every token)")
     if (cfg.dino.head_n_prototypes, cfg.dino.head_hidden_dim, cfg.dino.head_bottleneck_dim) != \
             (cfg.ibot.head_n_prototypes, cfg.ibot.head_hidden_dim, cfg.ibot.head_bottleneck_dim):
         raise NotImplementedError("dino and ibot heads must share their dimensions")

@@ -141,7 +141,11 @@ class Engine:
 
     def __init__(self, cfg: EngineConfig, B: int, device="cuda", max_masked: int | None = None, comm=None,
                  centering: str = "sinkhorn_knopp", center_momentum: float = 0.9, remat: bool = False):
-        assert cfg.head_dim == 64, "kernels are specialised for head_dim 64 (every BASELINE arch)"
+        assert cfg.head_dim in (64, 128), "attention kernels exist for head_dim 64 (ViT-S ... giant2) and 128 (vit_7b)"
+        if cfg.embed_dim > 1536:
+            raise NotImplementedError(f"embed_dim {cfg.embed_dim}: the LayerNorm backward (d3_layernorm_bwd_ls) takes rows of "
+                                      "at most 1536 columns, so training stops at ViT-giant2 width; vit_7b (4096) runs "
+                                      "forward through dinov3_jax.models.DinoVisionTransformer")
         assert centering in ("sinkhorn_knopp", "softmax")
         self.centering, self.center_momentum = centering, center_momentum
         # activation rematerialisation (train.checkpointing, ssl_default_config.yaml:88): only the block inputs X[i] of

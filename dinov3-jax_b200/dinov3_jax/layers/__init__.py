@@ -89,8 +89,8 @@ class SelfAttention:
                  attn_drop: float = 0.0, proj_drop: float = 0.0, mask_k_bias: bool = False):
         if mask_k_bias:
             raise NotImplementedError("mask_k_bias (LinearKMaskedBias fills its mask with NaN in the reference, attention.py:42)")
-        if dim != num_heads * 64:
-            raise NotImplementedError("head_dim must be 64")
+        if dim not in (num_heads * 64, num_heads * 128):
+            raise NotImplementedError("head_dim must be 64 or 128")
         self.dim, self.H = dim, num_heads
         self.wqkv = _w(params["qkv"]["kernel"])
         self.bqkv = _v(params["qkv"]["bias"]) if "bias" in params["qkv"] else torch.zeros(3 * dim, device=self.wqkv.device)
@@ -102,7 +102,7 @@ class SelfAttention:
         q2 = qkv.reshape(n * N, 3 * self.dim).contiguous()
         if rope is not None:
             sin, cos = rope
-            ops.rope(q2, sin, cos, N, N - sin.shape[0], self.dim, 64)
+            ops.rope(q2, sin, cos, N, N - sin.shape[0], self.dim, self.dim // self.H)
         o = torch.empty(n * N, self.dim, dtype=bf16, device=qkv.device)
         ops.attn_fwd(q2, o, None, n, N, self.dim, self.H)
         return o.view(n, N, self.dim)

@@ -17,12 +17,13 @@ def _factory(name):
 
 vit_small, vit_base, vit_large = _factory("vit_small"), _factory("vit_base"), _factory("vit_large")
 vit_so400m, vit_huge2, vit_giant2 = _factory("vit_so400m"), _factory("vit_huge2"), _factory("vit_giant2")
+vit_7b = _factory("vit_7b")            # head_dim 128, ffn_ratio 3
 
 
 def build_model(args, only_teacher: bool = False, img_size: int = 224):
     """models/__init__.py:17-55: returns (student, teacher, embed_dim) — here two (equal) static descriptions."""
     if args.arch not in ARCHS:
-        raise ValueError(f"unknown arch {args.arch!r} (ConvNeXt and vit_7b are not on the GPU path)")
+        raise ValueError(f"unknown arch {args.arch!r} (ConvNeXt is not on the GPU path)")
     cfg = config_for(args.arch, patch=args.patch_size)
     if only_teacher:
         return cfg, cfg.embed_dim

@@ -135,12 +135,13 @@ int d3_allreduce_peers(const float* const* peers /*host array [world]*/, int wor
 int d3_rope(void* qkv_bf16, const float* sin_t /*[P,hd]*/, const float* cos_t, long long T, int tokens_per_crop,
             int prefix, int D, int head_dim, int inverse, void* stream);
 
-/* ---- attention (layers/attention.py:116 nn.dot_product_attention; head_dim 64, any N up to 32768) ----------------- */
-/* N > 32768, or n_crops * N >= 2^31, returns D3_ERR_ARG before any CUDA call.  Crops of up to 448 tokens (forward) /
- * 256 tokens (backward) run on kernels that hold a whole crop in shared memory; longer ones on streamed kernels.   */
+/* ---- attention (layers/attention.py:116 nn.dot_product_attention; head_dim D/H = 64 or 128, any N up to 32768) ---- */
+/* N > 32768, n_crops * N >= 2^31 or another head_dim returns D3_ERR_ARG before any CUDA call.  Scale head_dim^-0.5.
+ * head_dim 64: crops of up to 448 tokens (forward) / 256 tokens (backward) run on kernels that hold a whole crop in
+ * shared memory, longer ones on streamed kernels.  head_dim 128 (vit_7b): streamed kernels at every N.             */
 int d3_attn_fwd(const void* qkv_bf16 /*[n*N,3D] post-RoPE*/, void* o_bf16 /*[n*N,D]*/, float* lse /*[n,H,N] or NULL*/,
                 int n_crops, int N, int D, int H, void* stream);
-/* rope_sin / rope_cos ([P,64] fp32, or NULL): when given, the inverse rotation (transpose of layers/attention.py:19-20)
+/* rope_sin / rope_cos ([P,head_dim] fp32, or NULL): when given, the inverse rotation (transpose of layers/attention.py:19-20)
  * is applied to dq / dk of tokens >= rope_prefix before they are stored, i.e. dqkv is the gradient w.r.t. the
  * pre-RoPE qkv projection output.                                                                                  */
 int d3_attn_bwd(const void* qkv_bf16, const void* o_bf16, const void* do_bf16, const float* lse,

@@ -6,6 +6,7 @@ Prints the card name and power limit, ms/step and global-crops/s (CUDA events ov
 usage: python tools/bench_hires_step.py [--steps 10] [--warmup 3] [--global-size 512] [--batch 8]"""
 import argparse
 import collections
+import dataclasses
 import os
 import subprocess
 import sys
@@ -33,6 +34,8 @@ def main():
     ap.add_argument("--global-size", type=int, default=512)
     ap.add_argument("--local-size", type=int, default=112)
     ap.add_argument("--arch", default="vit_large")
+    ap.add_argument("--depth", type=int, default=0, help="blocks (0: the arch's own depth)")
+    ap.add_argument("--prototypes", type=int, default=65536)
     args = ap.parse_args()
 
     from dinov3_jax import _native
@@ -40,7 +43,12 @@ def main():
     from dinov3_jax.engine.synth import init_reference_like, synthetic_batch
     _native.init(0)
     print(card(), flush=True)
-    cfg = config_for(args.arch, patch=16, global_size=args.global_size, local_size=args.local_size, n_storage=4)
+    # vit_7b runs its recipe's blocks (configs/train/dinov3_vit7b16_*.yaml): SwiGLU64, layernormbf16, mask_k_bias
+    recipe = dict(ffn_layer="swiglu", swiglu_align=64, ln_eps=1e-5, mask_k_bias=True) if args.arch == "vit_7b" else {}
+    cfg = config_for(args.arch, patch=16, global_size=args.global_size, local_size=args.local_size, n_storage=4,
+                     n_prototypes=args.prototypes, **recipe)
+    if args.depth:
+        cfg = dataclasses.replace(cfg, depth=args.depth)
     B = args.batch
     batch = synthetic_batch(cfg, B, seed=0, pin=True)
     eng = Engine(cfg, B, max_masked=max(int(batch["mask_indices_list"].shape[0]), 1))
@@ -61,7 +69,7 @@ def main():
     launches = _native.launch_count() / args.steps
     loss = eng.read_metrics()["total_loss"]
     ntok = lambda s: (s // 16) ** 2 + 1 + cfg.n_storage
-    print(f"{args.arch}/16, 2 x {args.global_size}^2 ({ntok(args.global_size)} tokens) + 8 x {args.local_size}^2 "
+    print(f"{args.arch}/16 ({cfg.depth} blocks, K = {cfg.n_prototypes}), 2 x {args.global_size}^2 ({ntok(args.global_size)} tokens) + 8 x {args.local_size}^2 "
           f"({ntok(args.local_size)} tokens), B = {B}: {ms:.2f} ms/step, {2 * B * 1e3 / ms:.1f} global-crops/s, "
           f"{launches:.0f} launches/step, loss {loss:.4f}", flush=True)
 
