@@ -1,22 +1,20 @@
-// Multi-head self-attention forward / backward on the Hopper tensor cores (wgmma) for the short ViT sequences of the
-// DINOv3 crops (N = 197 / 37 / 257 / 50 tokens, head_dim = 64): replaces flax `nn.dot_product_attention(q, k, v)` at
-// dinov3_jax/layers/attention.py:116 (softmax((q / sqrt(64)) k^T) v, no mask, no dropout) and its jax.grad.
+// Multi-head self-attention forward / backward on the Hopper tensor cores (wgmma): replaces flax
+// `nn.dot_product_attention(q, k, v)` at dinov3_jax/layers/attention.py:116 (softmax((q / sqrt(head_dim)) k^T) v, no mask,
+// no dropout) and its jax.grad, for head_dim 64 and 128 and any crop length up to ATTN_MAX_TOKENS.
 //
-// Short crops (N <= 64) are packed G per 128-row tile with a block-diagonal mask, so one CTA covers a "crop group" of
-// span = G * N token rows.  Operands come by TMA (SWIZZLE_128B) from the fused qkv buffer [T, 3D] (q | k | v thirds,
-// heads contiguous); every product is a warpgroup MMA with fp32 accumulators in registers.
+// Operands come by TMA (SWIZZLE_128B) from the fused qkv buffer [T, 3D] (q | k | v thirds, heads contiguous); every
+// product is a warpgroup MMA with fp32 accumulators in registers.  Short crops (N <= 64) are packed G per 128-row tile
+// with a block-diagonal mask, so one CTA covers a "crop group" of span = G * N token rows.
 //
-// Forward: one CTA per (q-tile of 128 rows, head, crop group), two warpgroups of 64 query rows each.  Q and the whole
-// key / value range of the group are staged once; each warpgroup walks the keys in blocks of 64: S = Q K^T (SS form),
-// online softmax on the accumulator fragment, then O += P V with P handed to the tensor core straight from registers
-// (RS form: the accumulator fragment of S is the A-operand fragment of the PV product).
-//
-// Crops longer than the resident kernels hold (span > 448 forward, N > 256 backward; G = 1 there) take streamed kernels
-// with the same per-tile arithmetic: a producer warpgroup fills an mbarrier ring of 128-row K / V (or Q / dO) tiles that both
-// consumer warpgroups read, so shared memory no longer grows with N.  Any N up to ATTN_MAX_TOKENS.
-//
-// head_dim 128 (vit_7b) has kernels of its own, after the head_dim 64 ones; d3_attn_fwd / d3_attn_bwd pick the family
-// from D / H.
+// Three kernel families; d3_attn_fwd / d3_attn_bwd pick one from D / H and the span:
+//   resident, head_dim 64   the DINOv3 crops (N = 197 / 37 / 257 / 50; span <= 448 forward, <= 256 backward):
+//                           attn_fwd_kernel and attn_bwd_fused_kernel keep every tile of the crop group in shared memory.
+//   streamed, head_dim 64   longer crops, G = 1: attn_fwd_stream_kernel, attn_bwd_dkdv_kernel, attn_bwd_dq_kernel.
+//   head_dim 128 (vit_7b)   any span: attn_fwd_hd128_kernel, attn_bwd_dkdv_hd128_kernel, attn_bwd_dq_hd128_kernel.
+// The streamed and head_dim 128 kernels share one TileRing: a producer warpgroup streams 128-row K / V (or Q / dO) tiles
+// through an mbarrier ring that both consumer warpgroups read, so shared memory does not grow with N.  All three
+// families run the same per-tile arithmetic: S = Q K^T, online softmax (forward) or P / dS from the saved LSE (backward),
+// with the score fragments handed to the next product straight from registers (RS form).
 #include "ptx.cuh"
 #include <climits>
 #include <cstdlib>
@@ -25,11 +23,10 @@
 namespace d3 {
 
 constexpr float LOG2E = 1.4426950408889634f;
+constexpr int SMEM_ALIGN = 1024;   // dynamic shared memory slack for smem_base_1024 (SWIZZLE_128B tiles are 1 KB aligned)
 
-__device__ long long* g_attn_dbg = nullptr;   // optional clock64() trace of CTA (0,0) (tools/attn_trace.py)
-__device__ __forceinline__ void dbg_mark(int slot) {
-  if (g_attn_dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (threadIdx.x == 0 || threadIdx.x == 200))
-    g_attn_dbg[slot * 2 + (threadIdx.x == 0 ? 0 : 1)] = clock64();
+__device__ __forceinline__ uint8_t* smem_base_1024(uint8_t* raw) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
 }
 
 struct AttnShape {
@@ -123,14 +120,19 @@ __device__ __forceinline__ void store_o_lse(const float (&o)[NO], float (&l)[2],
   }
 }
 
+// Resident forward: one CTA per (q-tile of 128 rows, head, crop group), two warpgroups of 64 query rows each.  Q and the
+// whole key / value range of the group are staged once; each warpgroup walks the keys in blocks of 64: S = Q K^T (SS
+// form), online softmax on the accumulator fragment, then O += P V with P handed to the tensor core straight from
+// registers (RS form: the accumulator fragment of S is the A-operand fragment of the PV product).
+// Shared memory: [Q 128 x 128 B][K nkb x 8 KB][V nkb x 8 KB][barrier].
+__host__ __device__ constexpr int fwd_smem(int nkb) { return SMEM_ALIGN + 16384 + 2 * nkb * 8192 + 8; }
+
 __global__ void __launch_bounds__(256)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                 __nv_bfloat16* __restrict__ O, float* __restrict__ LSE, const AttnShape sh) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // layout: [Q 128 x 128 B][K nkb x 8 KB][V nkb x 8 KB][barrier]
-  uint8_t* sQ = smem;
-  uint8_t* sK = smem + 16384;
+  uint8_t* sQ = smem_base_1024(smem_raw);
+  uint8_t* sK = sQ + 16384;
   uint8_t* sV = sK + sh.nkb * 8192;
   uint64_t* bar = reinterpret_cast<uint64_t*>(sV + sh.nkb * 8192);
 
@@ -138,7 +140,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int qt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
   const int q0 = qt * 128;
   const int row_base = c * sh.span;  // first token row of this CTA's crop group in [T, ...]
-  dbg_mark(0);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmKV);
@@ -201,30 +202,82 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     fence_regs(o);
   }
   store_o_lse(o, l, m, ri, sh, c, h, row_base, wq0, r_in, c2, O, LSE);
-  dbg_mark(1);
+}
+
+// ------------------------------------------------------------------------------------------------ tile ring
+// STAGES shared-memory stages of BYTES each, [STAGES x BYTES][full x STAGES][empty x STAGES], filled by TMA from one
+// producer thread and read by the consumer warps.  Full barriers count the TMA bytes; empty barriers one arrive per
+// consumer warp.  Tile j sits in stage j % STAGES and is that stage's use u = j / STAGES: consumers wait on full parity
+// u & 1, the producer waits on empty parity (u - 1) & 1 before every use u >= 1.
+template <int STAGES, int BYTES>
+struct TileRing {
+  static constexpr int SMEM = STAGES * BYTES + 2 * STAGES * 8;   // bytes from the base to end()
+  uint8_t* buf;
+  uint64_t* full;
+  uint64_t* empty;
+
+  __device__ __forceinline__ explicit TileRing(uint8_t* base)
+      : buf(base), full(reinterpret_cast<uint64_t*>(base + STAGES * BYTES)), empty(full + STAGES) {}
+  __device__ __forceinline__ uint64_t* end() const { return empty + STAGES; }
+  // one thread, before the fence_mbar_init / __syncthreads that publish the barriers
+  __device__ __forceinline__ void init(int consumer_warps) const {
+    for (int st = 0; st < STAGES; ++st) {
+      mbar_init(full + st, 1);
+      mbar_init(empty + st, consumer_warps);
+    }
+  }
+  // producer thread: tiles 0 .. n-1, load(bar, dst, j) issues the TMA loads of BYTES bytes of tile j into dst
+  template <class Load>
+  __device__ __forceinline__ void fill(int n, Load load) const {
+    for (int j = 0; j < n; ++j) {
+      const int st = j % STAGES, u = j / STAGES;
+      if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
+      mbar_expect_tx(full + st, BYTES);
+      load(full + st, buf + st * BYTES, j);
+    }
+  }
+  // consumer: the stage of tile j once it has landed
+  __device__ __forceinline__ uint8_t* wait(int j) const {
+    mbar_wait(full + j % STAGES, (j / STAGES) & 1);
+    return buf + (j % STAGES) * BYTES;
+  }
+  // consumer warp, converged: it no longer reads the stage of tile j
+  __device__ __forceinline__ void release(int j) const {
+    if (lane_id() == 0) mbar_arrive(empty + j % STAGES);
+  }
+};
+
+constexpr int FWD_STAGES = 4, DKDV_STAGES = 3, DQ_STAGES = 4, HD128_STAGES = 2;
+constexpr int RING_THREADS = 384;            // two consumer warpgroups + a producer warpgroup (registers: 232 / 40)
+
+// Role split of a ring kernel: warpgroup 2 hands its registers to the consumers and one of its threads runs `produce`
+// (the resident loads, then TileRing::fill); true there and in the rest of warpgroup 2, which return.  The consumer
+// warpgroups 0 and 1 take 232 registers each and get false.
+template <class Produce>
+__device__ __forceinline__ bool ring_producer(int wg, Produce produce) {
+  if (wg == 2) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 288 && elect_one()) produce();
+    return true;
+  }
+  setmaxnreg_inc<232>();
+  return false;
 }
 
 // ------------------------------------------------------------------------------------------------ streamed forward
-// One CTA per (128-row query tile, head, crop), G = 1, any N.  Warpgroup 2 is the producer (one warp issues the fills):
-// Q once, then every 128-key K / V
-// block through a ring of FWD_STAGES 32 KB stages (full barrier: TMA bytes; empty barrier: one arrive per consumer warp
-// that has rows in this crop).  Per block each consumer warpgroup runs S = Q K^T (m64n128), the resident kernel's online
-// softmax, and O += P V as 8 RS k-steps.  Block b sits in stage b % STAGES; its fill is use u = b / STAGES of the stage,
-// so consumers wait on full parity u & 1, and the producer waits on empty parity (u - 1) & 1 before fill u >= 1.
-constexpr int FWD_STAGES = 4, DKDV_STAGES = 3, DQ_STAGES = 4;
-constexpr int RING_THREADS = 384;            // two consumer warpgroups + a producer warpgroup (registers: 232 / 40)
+// One CTA per (128-row query tile, head, crop), G = 1, any N.  The producer loads Q once, then streams every 128-key
+// K | V block through the ring (the empty barriers count the consumer warps that have rows in this crop).  Per block each
+// consumer warpgroup runs S = Q K^T (m64n128), the resident kernel's online softmax, and O += P V as 8 RS k-steps.
+using FwdRing = TileRing<FWD_STAGES, 32768>;                            // K 16 KB | V 16 KB
+constexpr int FWD_STREAM_SMEM = SMEM_ALIGN + 16384 + FwdRing::SMEM + 8;   // [Q][ring][q barrier]
 
 __global__ void __launch_bounds__(RING_THREADS, 1)
 attn_fwd_stream_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ O, float* __restrict__ LSE,
                        const AttnShape sh) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // layout: [Q 128 x 128 B][STAGES x (K 16 KB, V 16 KB)][full][empty][q barrier]
-  uint8_t* sQ = smem;
-  uint8_t* ring = smem + 16384;
-  uint64_t* full = reinterpret_cast<uint64_t*>(ring + FWD_STAGES * 32768);
-  uint64_t* empty = full + FWD_STAGES;
-  uint64_t* bar_q = empty + FWD_STAGES;
+  uint8_t* sQ = smem_base_1024(smem_raw);
+  const FwdRing ring(sQ + 16384);
+  uint64_t* bar_q = ring.end();
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int qt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
@@ -232,30 +285,20 @@ attn_fwd_stream_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
   const int n_wg = (q0 + 64 < sh.N) ? 2 : 1;   // consumer warpgroups with at least one query row of the crop
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
-    for (int st = 0; st < FWD_STAGES; ++st) {
-      mbar_init(full + st, 1);
-      mbar_init(empty + st, 4 * n_wg);
-    }
+    ring.init(4 * n_wg);
     mbar_init(bar_q, 1);
     fence_mbar_init();
   }
   __syncthreads();
-  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
-    setmaxnreg_dec<40>();
-    if (threadIdx.x < 288 && elect_one()) {
-      mbar_expect_tx(bar_q, 16384);
-      tma_load_2d(&tmQKV, bar_q, sQ, h * 64, row_base + q0);
-      for (int b = 0; b < nkb; ++b) {
-        const int st = b % FWD_STAGES, u = b / FWD_STAGES;
-        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
-        mbar_expect_tx(full + st, 32768);
-        tma_load_2d(&tmQKV, full + st, ring + st * 32768, sh.D + h * 64, row_base + b * 128);
-        tma_load_2d(&tmQKV, full + st, ring + st * 32768 + 16384, 2 * sh.D + h * 64, row_base + b * 128);
-      }
-    }
+  if (ring_producer(wg, [&] {
+        mbar_expect_tx(bar_q, 16384);
+        tma_load_2d(&tmQKV, bar_q, sQ, h * 64, row_base + q0);
+        ring.fill(nkb, [&](uint64_t* bar, uint8_t* dst, int b) {
+          tma_load_2d(&tmQKV, bar, dst, sh.D + h * 64, row_base + b * 128);
+          tma_load_2d(&tmQKV, bar, dst + 16384, 2 * sh.D + h * 64, row_base + b * 128);
+        });
+      }))
     return;
-  }
-  setmaxnreg_inc<232>();
   const int wq0 = q0 + wg * 64;
   if (wq0 >= sh.N) return;                     // not counted by the empty barriers (n_wg)
   mbar_wait(bar_q, 0);
@@ -273,9 +316,7 @@ attn_fwd_stream_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
 
 #pragma unroll 1
   for (int b = 0; b < nkb; ++b) {
-    const int st = b % FWD_STAGES;
-    uint8_t* sK = ring + st * 32768;
-    mbar_wait(full + st, (b / FWD_STAGES) & 1);
+    const uint8_t* sK = ring.wait(b);
     float s[64];
     const uint64_t kd = gmma_desc_sw128(smem_u32(sK), 16, 1024);
     fence_regs(o);
@@ -299,7 +340,7 @@ attn_fwd_stream_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16*
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(o);
-    if (lane_id() == 0) mbar_arrive(empty + st);   // this warp no longer reads the stage
+    ring.release(b);
   }
   store_o_lse(o, l, m, ri, sh, c, h, row_base, wq0, r_in, c2, O, LSE);
 }
@@ -374,6 +415,15 @@ __device__ __forceinline__ void store_grad_rows(float (&a)[NA], const AttnShape&
   }
 }
 
+// lse * log2(e) and Delta of token row q of the crop group (0 for rows outside it)
+__device__ __forceinline__ void row_stats(const AttnShape& sh, const float* __restrict__ LSE, const float* __restrict__ Delta,
+                                          int c, int h, int q, float& lse2, float& dl) {
+  const RowInfo ri = row_info(sh, c, q);
+  const size_t stat = ((size_t)(c * sh.G + ri.g) * sh.H + h) * sh.N + (ri.ok ? q - ri.klo : 0);
+  lse2 = ri.ok ? LSE[stat] * LOG2E : 0.f;
+  dl = ri.ok ? Delta[stat] : 0.f;
+}
+
 // S and dP of one warpgroup's 64 query rows (first row q0 of the crop group, tiles sQw / sDOw: 64 rows x 128 B) against
 // the 128-key tile kt (sK, sV), turned into P (in s) and dS (in dp).  Keys outside a row's crop and rows outside the group
 // give exactly 0.
@@ -400,9 +450,8 @@ __device__ __forceinline__ void p_ds_tile(const AttnShape& sh, const float* __re
   for (int hh = 0; hh < 2; ++hh) {
     const int q = q0 + r_in + 8 * hh;
     const RowInfo ri = row_info(sh, c, q);
-    const size_t stat = ((size_t)(c * sh.G + ri.g) * sh.H + h) * sh.N + (ri.ok ? q - ri.klo : 0);
-    const float lse2 = ri.ok ? LSE[stat] * LOG2E : 0.f;
-    const float dl = ri.ok ? Delta[stat] : 0.f;
+    float lse2, dl;
+    row_stats(sh, LSE, Delta, c, h, q, lse2, dl);
     const int lo = ri.ok ? ri.klo - kt * 128 : 0, hi = ri.ok ? ri.khi - kt * 128 : 0;   // valid key columns
 #pragma unroll
     for (int i = 0; i < 16; ++i)
@@ -532,7 +581,6 @@ attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
   const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
   const int h = blockIdx.x, c = blockIdx.y;
   const int row_base = c * sh.span;
-  dbg_mark(0);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmDO);
@@ -550,7 +598,7 @@ attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
       tma_load_2d(&tmDO, bar_q + i, sQDO + i * 32768 + 16384, h * 64, row_base + i * 128);
     }
   }
-  for (int q = threadIdx.x; q < nT * 128; q += 256) {
+  for (int q = threadIdx.x; q < nT * 128; q += 256) {   // row_stats without its clamp of the index of rows outside the group
     const RowInfo ri = row_info(sh, c, q);
     const size_t stat = ((size_t)(c * sh.G + ri.g) * sh.H + h) * sh.N + (q - ri.klo);
     sLSE[q] = ri.ok ? LSE[stat] * LOG2E : 0.f;
@@ -703,7 +751,6 @@ attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
     store_grad_rows(dk, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 1, true, dQKV);
     store_grad_rows(dv, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 2, false, dQKV);
   }
-  dbg_mark(1);
 }
 
 // ------------------------------------------------------------------------------------------------ streamed backward
@@ -713,22 +760,23 @@ attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_co
 //            kernel's phase 1).
 //   dQ:      one CTA per (128-row query tile, head, crop).  Q / dO stay resident; K / V stream through a ring of DQ_STAGES
 //            stages.  Per key tile: p_ds_tile, dq_mma (the resident kernel's phase 2).
-// Warpgroup 2 is the producer; the ring protocol is the streamed forward's (tile j in stage j % STAGES, use u = j / STAGES:
-// consumers wait on full parity u & 1, the producer waits on empty parity (u - 1) & 1 before fill u >= 1).
+// Warpgroup 2 is the producer of the TileRing.
+using DkdvRing = TileRing<DKDV_STAGES, 32768>;                                  // Q 16 KB | dO 16 KB
+constexpr int DKDV_SMEM = SMEM_ALIGN + 2 * 16384 + 2 * 32768 + DkdvRing::SMEM + 8;   // [K][V][P][dS][ring][kv barrier]
+using DqRing = TileRing<DQ_STAGES, 32768>;                                      // K 16 KB | V 16 KB
+constexpr int DQ_SMEM = SMEM_ALIGN + 2 * 16384 + DqRing::SMEM + 8;                 // [Q][dO][ring][q barrier]
+
 __global__ void __launch_bounds__(RING_THREADS, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
                      const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
                      const AttnShape sh) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sK = smem;                          // 16 KB
+  uint8_t* sK = smem_base_1024(smem_raw);      // 16 KB
   uint8_t* sV = sK + 16384;                    // 16 KB
   uint8_t* sP = sV + 16384;                    // 32 KB
   uint8_t* sDS = sP + 32768;                   // 32 KB
-  uint8_t* ring = sDS + 32768;                 // STAGES x (Q 16 KB, dO 16 KB)
-  uint64_t* full = reinterpret_cast<uint64_t*>(ring + DKDV_STAGES * 32768);
-  uint64_t* empty = full + DKDV_STAGES;
-  uint64_t* bar_kv = empty + DKDV_STAGES;
+  const DkdvRing ring(sDS + 32768);
+  uint64_t* bar_kv = ring.end();
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
@@ -737,48 +785,36 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmDO);
-    for (int st = 0; st < DKDV_STAGES; ++st) {
-      mbar_init(full + st, 1);
-      mbar_init(empty + st, 8);                // both consumer warpgroups read every query tile
-    }
+    ring.init(8);                              // both consumer warpgroups read every query tile
     mbar_init(bar_kv, 1);
     fence_mbar_init();
   }
   __syncthreads();
-  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
-    setmaxnreg_dec<40>();
-    if (threadIdx.x < 288 && elect_one()) {
-      mbar_expect_tx(bar_kv, 32768);
-      tma_load_2d(&tmQKV, bar_kv, sK, sh.D + h * 64, row_base + kt * 128);
-      tma_load_2d(&tmQKV, bar_kv, sV, 2 * sh.D + h * 64, row_base + kt * 128);
-      for (int qt = 0; qt < nq; ++qt) {
-        const int st = qt % DKDV_STAGES, u = qt / DKDV_STAGES;
-        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
-        mbar_expect_tx(full + st, 32768);
-        tma_load_2d(&tmQKV, full + st, ring + st * 32768, h * 64, row_base + qt * 128);
-        tma_load_2d(&tmDO, full + st, ring + st * 32768 + 16384, h * 64, row_base + qt * 128);
-      }
-    }
+  if (ring_producer(wg, [&] {
+        mbar_expect_tx(bar_kv, 32768);
+        tma_load_2d(&tmQKV, bar_kv, sK, sh.D + h * 64, row_base + kt * 128);
+        tma_load_2d(&tmQKV, bar_kv, sV, 2 * sh.D + h * 64, row_base + kt * 128);
+        ring.fill(nq, [&](uint64_t* bar, uint8_t* dst, int qt) {
+          tma_load_2d(&tmQKV, bar, dst, h * 64, row_base + qt * 128);
+          tma_load_2d(&tmDO, bar, dst + 16384, h * 64, row_base + qt * 128);
+        });
+      }))
     return;
-  }
-  setmaxnreg_inc<232>();
   mbar_wait(bar_kv, 0);
   float dk[32], dv[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
 #pragma unroll 1
   for (int qt = 0; qt < nq; ++qt) {
-    const int st = qt % DKDV_STAGES;
-    const uint8_t* sQt = ring + st * 32768;
+    const uint8_t* sQt = ring.wait(qt);
     const uint8_t* sDOt = sQt + 16384;
-    mbar_wait(full + st, (qt / DKDV_STAGES) & 1);
     float s[64], dp[64];
     p_ds_tile(sh, LSE, Delta, c, h, qt * 128 + wg * 64, kt, sQt + wg * 8192, sDOt + wg * 8192, sK, sV, r_in, c2, s, dp);
     stash_p_ds(s, dp, sP, sDS, wg * 64 + r_in, c2);
     fence_proxy_async_smem();
     named_bar_sync(1, 256);                    // the consumer warpgroups only: P / dS of all 128 query rows are staged
     dkdv_mma(dk, dv, sP, sDS, sDOt, sQt, wg);
-    if (lane_id() == 0) mbar_arrive(empty + st);
+    ring.release(qt);
     named_bar_sync(1, 256);                    // both are done reading sP / sDS before the next tile rewrites them
   }
   store_grad_rows(dk, sh, c, row_base, kt * 128 + wg * 64, r_in, c2, h, 1, true, dQKV);
@@ -790,13 +826,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_const
                    const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
                    const AttnShape sh) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                          // 16 KB
+  uint8_t* sQ = smem_base_1024(smem_raw);      // 16 KB
   uint8_t* sDO = sQ + 16384;                   // 16 KB
-  uint8_t* ring = sDO + 16384;                 // STAGES x (K 16 KB, V 16 KB)
-  uint64_t* full = reinterpret_cast<uint64_t*>(ring + DQ_STAGES * 32768);
-  uint64_t* empty = full + DQ_STAGES;
-  uint64_t* bar_q = empty + DQ_STAGES;
+  const DqRing ring(sDO + 16384);
+  uint64_t* bar_q = ring.end();
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
@@ -806,31 +839,21 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_const
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmDO);
-    for (int st = 0; st < DQ_STAGES; ++st) {
-      mbar_init(full + st, 1);
-      mbar_init(empty + st, 4 * n_wg);
-    }
+    ring.init(4 * n_wg);
     mbar_init(bar_q, 1);
     fence_mbar_init();
   }
   __syncthreads();
-  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
-    setmaxnreg_dec<40>();
-    if (threadIdx.x < 288 && elect_one()) {
-      mbar_expect_tx(bar_q, 32768);
-      tma_load_2d(&tmQKV, bar_q, sQ, h * 64, row_base + q0);
-      tma_load_2d(&tmDO, bar_q, sDO, h * 64, row_base + q0);
-      for (int kt = 0; kt < nk; ++kt) {
-        const int st = kt % DQ_STAGES, u = kt / DQ_STAGES;
-        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
-        mbar_expect_tx(full + st, 32768);
-        tma_load_2d(&tmQKV, full + st, ring + st * 32768, sh.D + h * 64, row_base + kt * 128);
-        tma_load_2d(&tmQKV, full + st, ring + st * 32768 + 16384, 2 * sh.D + h * 64, row_base + kt * 128);
-      }
-    }
+  if (ring_producer(wg, [&] {
+        mbar_expect_tx(bar_q, 32768);
+        tma_load_2d(&tmQKV, bar_q, sQ, h * 64, row_base + q0);
+        tma_load_2d(&tmDO, bar_q, sDO, h * 64, row_base + q0);
+        ring.fill(nk, [&](uint64_t* bar, uint8_t* dst, int kt) {
+          tma_load_2d(&tmQKV, bar, dst, sh.D + h * 64, row_base + kt * 128);
+          tma_load_2d(&tmQKV, bar, dst + 16384, 2 * sh.D + h * 64, row_base + kt * 128);
+        });
+      }))
     return;
-  }
-  setmaxnreg_inc<232>();
   const int wq0 = q0 + wg * 64;
   if (wq0 >= sh.N) return;                     // not counted by the empty barriers (n_wg)
   mbar_wait(bar_q, 0);
@@ -839,13 +862,11 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_const
   for (int i = 0; i < 32; ++i) dq[i] = 0.f;
 #pragma unroll 1
   for (int kt = 0; kt < nk; ++kt) {
-    const int st = kt % DQ_STAGES;
-    const uint8_t* sK = ring + st * 32768;
-    mbar_wait(full + st, (kt / DQ_STAGES) & 1);
+    const uint8_t* sK = ring.wait(kt);
     float s[64], dp[64];
     p_ds_tile(sh, LSE, Delta, c, h, wq0, kt, sQ + wg * 8192, sDO + wg * 8192, sK, sK + 16384, r_in, c2, s, dp);
     dq_mma(dq, dp, sK);
-    if (lane_id() == 0) mbar_arrive(empty + st);
+    ring.release(kt);
   }
   store_grad_rows(dq, sh, c, row_base, wq0, r_in, c2, h, 0, true, dQKV);
 }
@@ -855,8 +876,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_const
 // box each, chunk j at +16 KB): K-major operands walk 8 k16 steps, 4 per chunk; the MN-major B operands of the P V,
 // P^T dO, dS^T Q and dS K products span both chunks with N = 128 (LBO = 16 KB).  Three kernels serve every N up to
 // ATTN_MAX_TOKENS and every packing of attn_shape: one CTA owns a crop group of span = G * N rows, short crops keep the
-// block-diagonal mask of row_info.  Each has the streamed kernels' producer warpgroup and ring protocol, with
-// HD128_STAGES stages of two 32 KB tiles (K | V or Q | dO):
+// block-diagonal mask of row_info.  Each has the streamed kernels' producer warpgroup and TileRing, with HD128_STAGES
+// stages of two 32 KB tiles (K | V or Q | dO):
 //   forward  one CTA per (128-row query tile, head, crop group), Q resident.  Per 128-key tile and consumer warpgroup:
 //            S = Q K^T (m64n128), online softmax, O += P V (RS m64n128, 8 k-steps).  Scores and O: 64 + 64 registers.
 //   dK / dV  one CTA per (128-key tile, head, crop group), K / V resident, Q / dO stream.  Keys on the accumulator rows
@@ -865,10 +886,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_const
 //   dQ       one CTA per (128-row query tile, head, crop group), Q / dO resident, K / V stream.  Per half of 64 keys:
 //            S and dP (m64n64), dQ += dS K (RS m64n128).
 // Every output row is written once by one CTA and every sum runs over the tiles in ascending order: no atomics, the
-// same bits on every run.  Shared memory: 32 KB (forward) or 64 KB (backward) resident + 2 x 64 KB ring + 1 KB alignment.
-constexpr int HD128_STAGES = 2;
-constexpr int HD128_FWD_SMEM = 32768 + HD128_STAGES * 65536 + (2 * HD128_STAGES + 1) * 8 + 1024;
-constexpr int HD128_BWD_SMEM = 65536 + HD128_STAGES * 65536 + (2 * HD128_STAGES + 1) * 8 + 1024;
+// same bits on every run.  Shared memory: 32 KB (forward) or 64 KB (backward) resident, the ring, its barrier.
+using Hd128Ring = TileRing<HD128_STAGES, 65536>;
+constexpr int HD128_FWD_SMEM = SMEM_ALIGN + 32768 + Hd128Ring::SMEM + 8;
+constexpr int HD128_BWD_SMEM = SMEM_ALIGN + 65536 + Hd128Ring::SMEM + 8;
 
 // K-major descriptor of k16 step k (0..7) of a 128-column tile whose first chunk (at the operand's first row) is p
 __device__ __forceinline__ uint64_t kdesc128(const uint8_t* p, int k) {
@@ -881,21 +902,13 @@ __device__ __forceinline__ void tma_load_tile128(const CUtensorMap* m, uint64_t*
   tma_load_2d(m, bar, dst + 16384, col + 64, row);
 }
 
-__device__ __forceinline__ uint8_t* smem_base_1024(uint8_t* raw) {
-  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
-}
-
 __global__ void __launch_bounds__(RING_THREADS, 1)
 attn_fwd_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* __restrict__ O, float* __restrict__ LSE,
                       const AttnShape sh) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_base_1024(smem_raw);
-  // layout: [Q 32 KB][STAGES x (K 32 KB, V 32 KB)][full][empty][q barrier]
-  uint8_t* sQ = smem;
-  uint8_t* ring = smem + 32768;
-  uint64_t* full = reinterpret_cast<uint64_t*>(ring + HD128_STAGES * 65536);
-  uint64_t* empty = full + HD128_STAGES;
-  uint64_t* bar_q = empty + HD128_STAGES;
+  uint8_t* sQ = smem_base_1024(smem_raw);      // [Q 32 KB][ring][q barrier]
+  const Hd128Ring ring(sQ + 32768);
+  uint64_t* bar_q = ring.end();
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int qt = blockIdx.x, h = blockIdx.y, c = blockIdx.z;
@@ -903,30 +916,20 @@ attn_fwd_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* 
   const int n_wg = (q0 + 64 < sh.span) ? 2 : 1;   // consumer warpgroups with at least one query row in the group
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
-    for (int st = 0; st < HD128_STAGES; ++st) {
-      mbar_init(full + st, 1);
-      mbar_init(empty + st, 4 * n_wg);
-    }
+    ring.init(4 * n_wg);
     mbar_init(bar_q, 1);
     fence_mbar_init();
   }
   __syncthreads();
-  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
-    setmaxnreg_dec<40>();
-    if (threadIdx.x < 288 && elect_one()) {
-      mbar_expect_tx(bar_q, 32768);
-      tma_load_tile128(&tmQKV, bar_q, sQ, h * 128, row_base + q0);
-      for (int b = 0; b < nkb; ++b) {
-        const int st = b % HD128_STAGES, u = b / HD128_STAGES;
-        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
-        mbar_expect_tx(full + st, 65536);
-        tma_load_tile128(&tmQKV, full + st, ring + st * 65536, sh.D + h * 128, row_base + b * 128);
-        tma_load_tile128(&tmQKV, full + st, ring + st * 65536 + 32768, 2 * sh.D + h * 128, row_base + b * 128);
-      }
-    }
+  if (ring_producer(wg, [&] {
+        mbar_expect_tx(bar_q, 32768);
+        tma_load_tile128(&tmQKV, bar_q, sQ, h * 128, row_base + q0);
+        ring.fill(nkb, [&](uint64_t* bar, uint8_t* dst, int b) {
+          tma_load_tile128(&tmQKV, bar, dst, sh.D + h * 128, row_base + b * 128);
+          tma_load_tile128(&tmQKV, bar, dst + 32768, 2 * sh.D + h * 128, row_base + b * 128);
+        });
+      }))
     return;
-  }
-  setmaxnreg_inc<232>();
   const int wq0 = q0 + wg * 64;
   if (wq0 >= sh.span) return;                  // not counted by the empty barriers (n_wg)
   mbar_wait(bar_q, 0);
@@ -943,9 +946,7 @@ attn_fwd_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* 
 
 #pragma unroll 1
   for (int b = 0; b < nkb; ++b) {
-    const int st = b % HD128_STAGES;
-    uint8_t* sK = ring + st * 65536;
-    mbar_wait(full + st, (b / HD128_STAGES) & 1);
+    const uint8_t* sK = ring.wait(b);
     float s[64];
     fence_regs(o);
     wgmma_fence();
@@ -969,18 +970,9 @@ attn_fwd_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16* 
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(o);
-    if (lane_id() == 0) mbar_arrive(empty + st);   // this warp no longer reads the stage
+    ring.release(b);
   }
   store_o_lse(o, l, m, ri, sh, c, h, row_base, wq0, r_in, c2, O, LSE);
-}
-
-// lse * log2(e) and Delta of token row q of the crop group (0 for rows outside it)
-__device__ __forceinline__ void row_stats(const AttnShape& sh, const float* __restrict__ LSE, const float* __restrict__ Delta,
-                                          int c, int h, int q, float& lse2, float& dl) {
-  const RowInfo ri = row_info(sh, c, q);
-  const size_t stat = ((size_t)(c * sh.G + ri.g) * sh.H + h) * sh.N + (ri.ok ? q - ri.klo : 0);
-  lse2 = ri.ok ? LSE[stat] * LOG2E : 0.f;
-  dl = ri.ok ? Delta[stat] : 0.f;
 }
 
 __global__ void __launch_bounds__(RING_THREADS, 1)
@@ -988,14 +980,10 @@ attn_bwd_dkdv_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __gr
                            const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
                            const AttnShape sh) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_base_1024(smem_raw);
-  // layout: [K 32 KB][V 32 KB][STAGES x (Q 32 KB, dO 32 KB)][full][empty][kv barrier]
-  uint8_t* sK = smem;
-  uint8_t* sV = smem + 32768;
-  uint8_t* ring = smem + 65536;
-  uint64_t* full = reinterpret_cast<uint64_t*>(ring + HD128_STAGES * 65536);
-  uint64_t* empty = full + HD128_STAGES;
-  uint64_t* bar_kv = empty + HD128_STAGES;
+  uint8_t* sK = smem_base_1024(smem_raw);      // [K 32 KB][V 32 KB][ring][kv barrier]
+  uint8_t* sV = sK + 32768;
+  const Hd128Ring ring(sK + 65536);
+  uint64_t* bar_kv = ring.end();
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
@@ -1005,31 +993,21 @@ attn_bwd_dkdv_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __gr
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmDO);
-    for (int st = 0; st < HD128_STAGES; ++st) {
-      mbar_init(full + st, 1);
-      mbar_init(empty + st, 4 * n_wg);
-    }
+    ring.init(4 * n_wg);
     mbar_init(bar_kv, 1);
     fence_mbar_init();
   }
   __syncthreads();
-  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
-    setmaxnreg_dec<40>();
-    if (threadIdx.x < 288 && elect_one()) {
-      mbar_expect_tx(bar_kv, 65536);
-      tma_load_tile128(&tmQKV, bar_kv, sK, sh.D + h * 128, row_base + kt * 128);
-      tma_load_tile128(&tmQKV, bar_kv, sV, 2 * sh.D + h * 128, row_base + kt * 128);
-      for (int qt = 0; qt < nq; ++qt) {
-        const int st = qt % HD128_STAGES, u = qt / HD128_STAGES;
-        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
-        mbar_expect_tx(full + st, 65536);
-        tma_load_tile128(&tmQKV, full + st, ring + st * 65536, h * 128, row_base + qt * 128);
-        tma_load_tile128(&tmDO, full + st, ring + st * 65536 + 32768, h * 128, row_base + qt * 128);
-      }
-    }
+  if (ring_producer(wg, [&] {
+        mbar_expect_tx(bar_kv, 65536);
+        tma_load_tile128(&tmQKV, bar_kv, sK, sh.D + h * 128, row_base + kt * 128);
+        tma_load_tile128(&tmQKV, bar_kv, sV, 2 * sh.D + h * 128, row_base + kt * 128);
+        ring.fill(nq, [&](uint64_t* bar, uint8_t* dst, int qt) {
+          tma_load_tile128(&tmQKV, bar, dst, h * 128, row_base + qt * 128);
+          tma_load_tile128(&tmDO, bar, dst + 32768, h * 128, row_base + qt * 128);
+        });
+      }))
     return;
-  }
-  setmaxnreg_inc<232>();
   const int wk0 = kt * 128 + wg * 64;
   if (wk0 >= sh.span) return;                  // not counted by the empty barriers (n_wg)
   mbar_wait(bar_kv, 0);
@@ -1047,10 +1025,8 @@ attn_bwd_dkdv_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __gr
   for (int i = 0; i < 64; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
 #pragma unroll 1
   for (int qt = 0; qt < nq; ++qt) {
-    const int st = qt % HD128_STAGES;
-    const uint8_t* sQt = ring + st * 65536;
+    const uint8_t* sQt = ring.wait(qt);
     const uint8_t* sDOt = sQt + 32768;
-    mbar_wait(full + st, (qt / HD128_STAGES) & 1);
 #pragma unroll 1
     for (int qc = 0; qc < 4; ++qc) {   // 32 query columns at a time: with dK + dV resident, 64 would spill
       float s[16], dp[16];
@@ -1102,7 +1078,7 @@ attn_bwd_dkdv_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __gr
       fence_frag(pa);
       fence_frag(da);
     }
-    if (lane_id() == 0) mbar_arrive(empty + st);   // this warp no longer reads the stage
+    ring.release(qt);
   }
   store_grad_rows(dk, sh, c, row_base, wk0, r_in, c2, h, 1, true, dQKV);
   store_grad_rows(dv, sh, c, row_base, wk0, r_in, c2, h, 2, false, dQKV);
@@ -1113,14 +1089,10 @@ attn_bwd_dq_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid
                          const float* __restrict__ LSE, const float* __restrict__ Delta, __nv_bfloat16* __restrict__ dQKV,
                          const AttnShape sh) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_base_1024(smem_raw);
-  // layout: [Q 32 KB][dO 32 KB][STAGES x (K 32 KB, V 32 KB)][full][empty][q barrier]
-  uint8_t* sQ = smem;
-  uint8_t* sDO = smem + 32768;
-  uint8_t* ring = smem + 65536;
-  uint64_t* full = reinterpret_cast<uint64_t*>(ring + HD128_STAGES * 65536);
-  uint64_t* empty = full + HD128_STAGES;
-  uint64_t* bar_q = empty + HD128_STAGES;
+  uint8_t* sQ = smem_base_1024(smem_raw);      // [Q 32 KB][dO 32 KB][ring][q barrier]
+  uint8_t* sDO = sQ + 32768;
+  const Hd128Ring ring(sQ + 65536);
+  uint64_t* bar_q = ring.end();
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int r_in = 16 * (t >> 5) + ((t & 31) >> 2), c2 = 2 * (t & 3);
@@ -1130,31 +1102,21 @@ attn_bwd_dq_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmDO);
-    for (int st = 0; st < HD128_STAGES; ++st) {
-      mbar_init(full + st, 1);
-      mbar_init(empty + st, 4 * n_wg);
-    }
+    ring.init(4 * n_wg);
     mbar_init(bar_q, 1);
     fence_mbar_init();
   }
   __syncthreads();
-  if (wg == 2) {                               // producer warpgroup: one warp issues the fills
-    setmaxnreg_dec<40>();
-    if (threadIdx.x < 288 && elect_one()) {
-      mbar_expect_tx(bar_q, 65536);
-      tma_load_tile128(&tmQKV, bar_q, sQ, h * 128, row_base + q0);
-      tma_load_tile128(&tmDO, bar_q, sDO, h * 128, row_base + q0);
-      for (int kt = 0; kt < nk; ++kt) {
-        const int st = kt % HD128_STAGES, u = kt / HD128_STAGES;
-        if (u > 0) mbar_wait(empty + st, (u - 1) & 1);
-        mbar_expect_tx(full + st, 65536);
-        tma_load_tile128(&tmQKV, full + st, ring + st * 65536, sh.D + h * 128, row_base + kt * 128);
-        tma_load_tile128(&tmQKV, full + st, ring + st * 65536 + 32768, 2 * sh.D + h * 128, row_base + kt * 128);
-      }
-    }
+  if (ring_producer(wg, [&] {
+        mbar_expect_tx(bar_q, 65536);
+        tma_load_tile128(&tmQKV, bar_q, sQ, h * 128, row_base + q0);
+        tma_load_tile128(&tmDO, bar_q, sDO, h * 128, row_base + q0);
+        ring.fill(nk, [&](uint64_t* bar, uint8_t* dst, int kt) {
+          tma_load_tile128(&tmQKV, bar, dst, sh.D + h * 128, row_base + kt * 128);
+          tma_load_tile128(&tmQKV, bar, dst + 32768, 2 * sh.D + h * 128, row_base + kt * 128);
+        });
+      }))
     return;
-  }
-  setmaxnreg_inc<232>();
   const int wq0 = q0 + wg * 64;
   if (wq0 >= sh.span) return;                  // not counted by the empty barriers (n_wg)
   mbar_wait(bar_q, 0);
@@ -1173,10 +1135,8 @@ attn_bwd_dq_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid
   for (int i = 0; i < 64; ++i) dq[i] = 0.f;
 #pragma unroll 1
   for (int kt = 0; kt < nk; ++kt) {
-    const int st = kt % HD128_STAGES;
-    const uint8_t* sK = ring + st * 65536;
+    const uint8_t* sK = ring.wait(kt);
     const uint8_t* sV = sK + 32768;
-    mbar_wait(full + st, (kt / HD128_STAGES) & 1);
 #pragma unroll 1
     for (int hf = 0; hf < 2; ++hf) {
       float s[32], dp[32];
@@ -1215,7 +1175,7 @@ attn_bwd_dq_hd128_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid
       fence_regs(dq);
       fence_frag(da);
     }
-    if (lane_id() == 0) mbar_arrive(empty + st);   // this warp no longer reads the stage
+    ring.release(kt);
   }
   store_grad_rows(dq, sh, c, row_base, wq0, r_in, c2, h, 0, true, dQKV);
 }
@@ -1250,18 +1210,22 @@ static int attn_shape(AttnShape* s, int n_crops, int N, int D, int H) {
   return D3_OK;
 }
 
-// grid of the streamed kernels: (128-row tiles, head, crop); G = 1 there
-static int stream_grid(const AttnShape& s, dim3* grid) {
-  if (s.H > 65535 || s.n_crops > 65535) return set_error(D3_ERR_ARG, "attention: H and n_crops must be <= 65535 for long crops");
-  *grid = dim3((s.N + 127) / 128, s.H, s.n_crops);
+// grid of every kernel that owns 128-row tiles of a crop group: (tiles of the span, head, crop group)
+static int tile_grid(const AttnShape& s, dim3* grid) {
+  const int groups = (s.n_crops + s.G - 1) / s.G;
+  if (s.H > 65535 || groups > 65535) return set_error(D3_ERR_ARG, "attention: H and crop groups must be <= 65535");
+  *grid = dim3((s.span + 127) / 128, s.H, groups);
   return D3_OK;
 }
 
-// grid of the head_dim 128 kernels: (128-row tiles of a crop group, head, crop group)
-static int hd128_grid(const AttnShape& s, dim3* grid) {
-  const int groups = (s.n_crops + s.G - 1) / s.G;
-  if (s.H > 65535 || groups > 65535) return set_error(D3_ERR_ARG, "attention: H and crop groups must be <= 65535 at head_dim 128");
-  *grid = dim3((s.span + 127) / 128, s.H, groups);
+// Launches `kernel` with `smem` bytes of dynamic shared memory.  The first launch of a kernel in the process raises its
+// opt-in limit to `smem_max`, the most any of its launches asks for.
+template <auto kernel, class... Args>
+static int launch(dim3 grid, int threads, int smem, int smem_max, cudaStream_t st, const Args&... args) {
+  static const cudaError_t cfg = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
+  (void)cfg;   // a failure shows at the launch
+  kernel<<<grid, threads, smem, st>>>(args...);
+  D3_CHECK_LAUNCH();
   return D3_OK;
 }
 
@@ -1271,57 +1235,25 @@ using namespace d3;
 
 extern "C" {
 
-int d3_debug_attn_trace(long long* buf /*device [64] or NULL*/) {
-  cudaError_t e = cudaMemcpyToSymbol(g_attn_dbg, &buf, sizeof(buf));
-  return e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
-}
-
 int d3_attn_fwd(const void* qkv, void* o, float* lse, int n_crops, int N, int D, int H, void* stream) {
   AttnShape s;
   int rc = attn_shape(&s, n_crops, N, D, H);
   if (rc) return rc;
+  dim3 grid;
+  if ((rc = tile_grid(s, &grid))) return rc;
   const long T = (long)n_crops * N;
-  if (D == H * 128) {
-    dim3 grid;
-    if ((rc = hd128_grid(s, &grid))) return rc;
-    CUtensorMap tqkv;
-    if ((rc = make_map(&tqkv, qkv, T, 3 * D, 3 * D, 128))) return rc;
-    static bool cfg128 = false;
-    if (!cfg128) {
-      cudaFuncSetAttribute(attn_fwd_hd128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HD128_FWD_SMEM);
-      cfg128 = true;
-    }
-    attn_fwd_hd128_kernel<<<grid, RING_THREADS, HD128_FWD_SMEM, reinterpret_cast<cudaStream_t>(stream)>>>(
-        tqkv, (__nv_bfloat16*)o, lse, s);
-    D3_CHECK_LAUNCH();
-    return D3_OK;
-  }
-  if (s.span > ATTN_FWD_RESIDENT_SPAN) {
-    dim3 grid;
-    if ((rc = stream_grid(s, &grid))) return rc;
-    CUtensorMap tqkv;
-    if ((rc = make_map(&tqkv, qkv, T, 3 * D, 3 * D, 128))) return rc;
-    const int smem = 16384 + FWD_STAGES * 32768 + (2 * FWD_STAGES + 1) * 8 + 1024;
-    static bool cfg_stream = false;
-    if (!cfg_stream) {
-      cudaFuncSetAttribute(attn_fwd_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-      cfg_stream = true;
-    }
-    attn_fwd_stream_kernel<<<grid, RING_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(tqkv, (__nv_bfloat16*)o,
-                                                                                                 lse, s);
-    D3_CHECK_LAUNCH();
-    return D3_OK;
-  }
-  CUtensorMap tq, tkv;
-  if ((rc = make_map(&tq, qkv, T, 3 * D, 3 * D, 128))) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  __nv_bfloat16* out = (__nv_bfloat16*)o;
+  CUtensorMap tqkv;
+  if ((rc = make_map(&tqkv, qkv, T, 3 * D, 3 * D, 128))) return rc;
+  if (D == H * 128)
+    return launch<attn_fwd_hd128_kernel>(grid, RING_THREADS, HD128_FWD_SMEM, HD128_FWD_SMEM, st, tqkv, out, lse, s);
+  if (s.span > ATTN_FWD_RESIDENT_SPAN)
+    return launch<attn_fwd_stream_kernel>(grid, RING_THREADS, FWD_STREAM_SMEM, FWD_STREAM_SMEM, st, tqkv, out, lse, s);
+  CUtensorMap tkv;
   if ((rc = make_map(&tkv, qkv, T, 3 * D, 3 * D, 64))) return rc;
-  const int smem = 16384 + 2 * s.nkb * 8192 + 64 + 1024;
-  static bool cfg = false;
-  if (!cfg) { cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); cfg = true; }
-  dim3 grid((s.span + 127) / 128, H, (n_crops + s.G - 1) / s.G);
-  attn_fwd_kernel<<<grid, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(tq, tkv, (__nv_bfloat16*)o, lse, s);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  return launch<attn_fwd_kernel>(grid, 256, fwd_smem(s.nkb), fwd_smem((ATTN_FWD_RESIDENT_SPAN + 63) / 64), st, tqkv, tkv,
+                                 out, lse, s);
 }
 
 int d3_attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta_scratch, void* dqkv,
@@ -1334,9 +1266,8 @@ int d3_attn_bwd(const void* qkv, const void* o, const void* d_o, const float* ls
   if (!delta_scratch) return set_error(D3_ERR_ARG, "d3_attn_bwd: delta scratch buffer");
   const bool hd128 = D == H * 128;
   const bool streamed = s.span > ATTN_BWD_RESIDENT_SPAN;
-  dim3 sgrid;
-  if (hd128 && (rc = hd128_grid(s, &sgrid))) return rc;
-  if (!hd128 && streamed && (rc = stream_grid(s, &sgrid))) return rc;
+  dim3 grid;   // ring kernels; key tiles and query tiles of a crop group are both (span + 127) / 128
+  if ((hd128 || streamed) && (rc = tile_grid(s, &grid))) return rc;
   s.sin_t = rope_sin; s.cos_t = rope_cos; s.prefix = rope_prefix;
   const long T = (long)n_crops * N;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -1351,48 +1282,23 @@ int d3_attn_bwd(const void* qkv, const void* o, const void* d_o, const float* ls
   CUtensorMap tqkv, tdo;
   if ((rc = make_map(&tqkv, qkv, T, 3 * D, 3 * D, 128))) return rc;
   if ((rc = make_map(&tdo, d_o, T, D, D, 128))) return rc;
+  __nv_bfloat16* dq = (__nv_bfloat16*)dqkv;
   if (hd128) {
-    static bool cfg128 = false;
-    if (!cfg128) {
-      cudaFuncSetAttribute(attn_bwd_dkdv_hd128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HD128_BWD_SMEM);
-      cudaFuncSetAttribute(attn_bwd_dq_hd128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HD128_BWD_SMEM);
-      cfg128 = true;
-    }
-    // key tiles and query tiles of a crop group are both (span + 127) / 128: one grid shape for the two kernels
-    attn_bwd_dkdv_hd128_kernel<<<sgrid, RING_THREADS, HD128_BWD_SMEM, st>>>(tqkv, tdo, lse, delta_scratch,
-                                                                             (__nv_bfloat16*)dqkv, s);
-    D3_CHECK_LAUNCH();
-    attn_bwd_dq_hd128_kernel<<<sgrid, RING_THREADS, HD128_BWD_SMEM, st>>>(tqkv, tdo, lse, delta_scratch,
-                                                                           (__nv_bfloat16*)dqkv, s);
-    D3_CHECK_LAUNCH();
-    return D3_OK;
+    if ((rc = launch<attn_bwd_dkdv_hd128_kernel>(grid, RING_THREADS, HD128_BWD_SMEM, HD128_BWD_SMEM, st, tqkv, tdo, lse,
+                                                 delta_scratch, dq, s)))
+      return rc;
+    return launch<attn_bwd_dq_hd128_kernel>(grid, RING_THREADS, HD128_BWD_SMEM, HD128_BWD_SMEM, st, tqkv, tdo, lse,
+                                            delta_scratch, dq, s);
   }
   if (streamed) {
-    const int smem_kv = 16384 * 2 + 32768 * 2 + DKDV_STAGES * 32768 + (2 * DKDV_STAGES + 1) * 8 + 1024;
-    const int smem_q = 16384 * 2 + DQ_STAGES * 32768 + (2 * DQ_STAGES + 1) * 8 + 1024;
-    static bool cfg_stream = false;
-    if (!cfg_stream) {
-      cudaFuncSetAttribute(attn_bwd_dkdv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_kv);
-      cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_q);
-      cfg_stream = true;
-    }
-    // key tiles and query tiles are both (N + 127) / 128: the same grid shape for the two kernels
-    attn_bwd_dkdv_kernel<<<sgrid, RING_THREADS, smem_kv, st>>>(tqkv, tdo, lse, delta_scratch, (__nv_bfloat16*)dqkv, s);
-    D3_CHECK_LAUNCH();
-    attn_bwd_dq_kernel<<<sgrid, RING_THREADS, smem_q, st>>>(tqkv, tdo, lse, delta_scratch, (__nv_bfloat16*)dqkv, s);
-    D3_CHECK_LAUNCH();
-    return D3_OK;
+    if ((rc = launch<attn_bwd_dkdv_kernel>(grid, RING_THREADS, DKDV_SMEM, DKDV_SMEM, st, tqkv, tdo, lse, delta_scratch, dq,
+                                           s)))
+      return rc;
+    return launch<attn_bwd_dq_kernel>(grid, RING_THREADS, DQ_SMEM, DQ_SMEM, st, tqkv, tdo, lse, delta_scratch, dq, s);
   }
-  static bool cfg = false;
-  if (!cfg) {
-    cudaFuncSetAttribute(attn_bwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_fused_smem(2));
-    cfg = true;
-  }
-  dim3 grid(H, (n_crops + s.G - 1) / s.G);
-  attn_bwd_fused_kernel<<<grid, 256, bwd_fused_smem((s.span + 127) / 128), st>>>(tqkv, tdo, lse, delta_scratch,
-                                                                                 (__nv_bfloat16*)dqkv, s);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  return launch<attn_bwd_fused_kernel>(dim3(H, (n_crops + s.G - 1) / s.G), 256, bwd_fused_smem((s.span + 127) / 128),
+                                       bwd_fused_smem(ATTN_BWD_RESIDENT_SPAN / 128), st, tqkv, tdo, lse, delta_scratch,
+                                       dq, s);
 }
 
 }  // extern "C"

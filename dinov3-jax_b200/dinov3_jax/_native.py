@@ -52,7 +52,6 @@ SIGNATURES = {
     "d3_ls_gamma_from_wgrad": [P, P, P, P, P, P, I, I, P],
     "d3_rope": [P, P, P, LL, I, I, I, I, I, P],
     "d3_attn_fwd": [P, P, P, I, I, I, I, P],
-    "d3_debug_attn_trace": [P],
     "d3_attn_bwd": [P, P, P, P, P, P, I, I, I, I, P, P, I, P],
     "d3_token_rows": [P, P, I, I, I, I, P],
     "d3_gather_rows": [P, P, P, P, I, I, P],

@@ -148,9 +148,6 @@ int d3_attn_bwd(const void* qkv_bf16, const void* o_bf16, const void* do_bf16, c
                 float* delta_scratch /*[n,H,N]*/, void* dqkv_bf16 /*[n*N,3D]*/, int n_crops, int N, int D, int H,
                 const float* rope_sin, const float* rope_cos, int rope_prefix, void* stream);
 
-/* diagnostics: when buf != NULL, CTA (0,0) of d3_attn_bwd writes clock64() marks (2 threads x 32 slots) into it */
-int d3_debug_attn_trace(long long* buf);
-
 /* ---- row gather / scatter (train/ssl_meta_arch.py:377,432 patch.reshape(-1,D)[mask_indices_list]; cls = token 0) --- */
 int d3_token_rows(const long long* mask_indices /*int64 [count] (mode 0)*/, int* rows /*int32 [count]*/, int count,
                   int P, int prefix /*tokens before the patches: 1 + n_storage_tokens*/,

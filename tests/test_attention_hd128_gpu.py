@@ -6,17 +6,13 @@ import dataclasses
 import pytest
 import torch
 
+from attention_helpers import BF16_TOL, attn_ref, bwd, fwd, rel
 from test_engine_gpu import HYPER, check, run_pair
 
 pytestmark = pytest.mark.gpu
 
 HD = 128
-BF16_TOL = 6e-3      # norm-wise relative error of a bf16-stored result (2^-9 per element)
 NS = [1, 37, 54, 64, 65, 128, 129, 197, 261, 449, 1029, 2309]
-
-
-def rel(a, b):
-    return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-30)).item()
 
 
 @pytest.fixture(autouse=True)
@@ -29,30 +25,6 @@ def n_crops(N):
     return 5 if N <= 64 else 3 if N <= 449 else 2 if N <= 1029 else 1
 
 
-def attn_ref(qkv, n, N, H):
-    q, k, v = qkv.float().reshape(n, N, 3, H, HD).permute(2, 0, 3, 1, 4)
-    s = (q @ k.transpose(-1, -2)) * HD ** -0.5
-    o = (torch.softmax(s, -1) @ v).permute(0, 2, 1, 3).reshape(n * N, H * HD)
-    return o, torch.logsumexp(s, -1)
-
-
-def fwd(qkv, n, N, H):
-    from dinov3_jax import ops
-    D = HD * H
-    o = torch.full((n * N, D), float("nan"), device="cuda", dtype=torch.bfloat16)
-    lse = torch.full((n, H, N), float("nan"), device="cuda")
-    ops.attn_fwd(qkv, o, lse, n, N, D, H)
-    return o, lse
-
-
-def bwd(qkv, o, do, lse, n, N, H, **rope):
-    from dinov3_jax import ops
-    D = HD * H
-    dqkv = torch.full((n * N, 3 * D), float("nan"), device="cuda", dtype=torch.bfloat16)
-    ops.attn_bwd(qkv, o, do, lse, torch.zeros(n, H, N, device="cuda"), dqkv, n, N, D, H, **rope)
-    return dqkv
-
-
 @pytest.mark.parametrize("H", [1, 2, 32])
 @pytest.mark.parametrize("N", NS)
 def test_hd128_forward_and_backward(N, H):
@@ -60,11 +32,11 @@ def test_hd128_forward_and_backward(N, H):
     qkv = torch.randn(n * N, 3 * D, device="cuda").to(torch.bfloat16)
     do = torch.randn(n * N, D, device="cuda").to(torch.bfloat16)
     x = qkv.float().requires_grad_(True)
-    ro, rl = attn_ref(x, n, N, H)
+    ro, rl = attn_ref(x, n, N, H, HD)
     ro.backward(do.float())
-    o, lse = fwd(qkv, n, N, H)
+    o, lse = fwd(qkv, n, N, H, HD)
     assert rel(o, ro.detach()) < BF16_TOL and rel(lse, rl.detach()) < 1e-5
-    dqkv = bwd(qkv, o, do, lse, n, N, H)
+    dqkv = bwd(qkv, o, do, lse, n, N, H, HD)
     # at N = 1 dq and dk are exactly zero (dP - Delta = 0): their error is measured against the scale of the whole dqkv
     floor = 1e-2 * x.grad.norm().item()
     for j in range(3):
@@ -84,14 +56,14 @@ def test_hd128_backward_fused_inverse_rope(Hp, prefix):
     assert sin.shape == (Hp * Hp, HD)
     qkv = torch.randn(n * N, 3 * D, device="cuda").to(torch.bfloat16)
     do = torch.randn(n * N, D, device="cuda").to(torch.bfloat16)
-    o, lse = fwd(qkv, n, N, H)
-    d1 = bwd(qkv, o, do, lse, n, N, H)
+    o, lse = fwd(qkv, n, N, H, HD)
+    d1 = bwd(qkv, o, do, lse, n, N, H, HD)
     ops.rope(d1, sin, cos, N, prefix, D, HD, inverse=True)
-    d2 = bwd(qkv, o, do, lse, n, N, H, rope_sin=sin, rope_cos=cos, rope_prefix=prefix)
+    d2 = bwd(qkv, o, do, lse, n, N, H, HD, rope_sin=sin, rope_cos=cos, rope_prefix=prefix)
     assert rel(d2, d1) < BF16_TOL          # d1 is rounded to bf16 twice, d2 once
     assert torch.equal(d2[:, 2 * D:], d1[:, 2 * D:])
     pre = torch.cat([torch.arange(c * N, c * N + prefix) for c in range(n)]).cuda()
-    assert torch.equal(d2[pre, :2 * D], bwd(qkv, o, do, lse, n, N, H)[pre, :2 * D])
+    assert torch.equal(d2[pre, :2 * D], bwd(qkv, o, do, lse, n, N, H, HD)[pre, :2 * D])
 
 
 def test_hd128_rope_forward_matches_oracle():
@@ -118,9 +90,9 @@ def test_hd128_attention_is_bit_reproducible(n, N, H):
     D = HD * H
     qkv = torch.randn(n * N, 3 * D, device="cuda").to(torch.bfloat16)
     do = torch.randn(n * N, D, device="cuda").to(torch.bfloat16)
-    (o1, l1), (o2, l2) = fwd(qkv, n, N, H), fwd(qkv, n, N, H)
+    (o1, l1), (o2, l2) = fwd(qkv, n, N, H, HD), fwd(qkv, n, N, H, HD)
     assert torch.equal(o1, o2) and torch.equal(l1, l2)
-    assert torch.equal(bwd(qkv, o1, do, l1, n, N, H), bwd(qkv, o1, do, l1, n, N, H))
+    assert torch.equal(bwd(qkv, o1, do, l1, n, N, H, HD), bwd(qkv, o1, do, l1, n, N, H, HD))
 
 
 def test_other_head_dims_are_refused():

@@ -6,44 +6,15 @@ import dataclasses
 import pytest
 import torch
 
+from attention_helpers import BF16_TOL, attn_ref, bwd, fwd, rel
 from test_engine_gpu import HYPER, check, run_pair
 
 pytestmark = pytest.mark.gpu
-
-BF16_TOL = 6e-3      # norm-wise relative error of a bf16-stored result (2^-9 per element)
-
-
-def rel(a, b):
-    return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-30)).item()
 
 
 @pytest.fixture(autouse=True)
 def _seed(native):
     torch.manual_seed(0)
-
-
-def attn_ref(qkv, n, N, D, H):
-    q, k, v = qkv.float().reshape(n, N, 3, H, 64).permute(2, 0, 3, 1, 4)
-    s = (q @ k.transpose(-1, -2)) * 0.125
-    o = (torch.softmax(s, -1) @ v).permute(0, 2, 1, 3).reshape(n * N, D)
-    return o, torch.logsumexp(s, -1)
-
-
-def fwd(qkv, n, N, H):
-    from dinov3_jax import ops
-    D = 64 * H
-    o = torch.full((n * N, D), float("nan"), device="cuda", dtype=torch.bfloat16)
-    lse = torch.full((n, H, N), float("nan"), device="cuda")
-    ops.attn_fwd(qkv, o, lse, n, N, D, H)
-    return o, lse
-
-
-def bwd(qkv, o, do, lse, n, N, H, **rope):
-    from dinov3_jax import ops
-    D = 64 * H
-    dqkv = torch.full((n * N, 3 * D), float("nan"), device="cuda", dtype=torch.bfloat16)
-    ops.attn_bwd(qkv, o, do, lse, torch.zeros(n, H, N, device="cuda"), dqkv, n, N, D, H, **rope)
-    return dqkv
 
 
 # (16, 1029, 16): 512^2 crops at patch 16 with 4 storage tokens, ViT-L heads; (1, 5189, 2): a 1 152^2 gram teacher crop
@@ -52,7 +23,7 @@ def bwd(qkv, o, do, lse, n, N, H, **rope):
 def test_long_attention_forward(n, N, H):
     qkv = torch.randn(n * N, 3 * 64 * H, device="cuda").to(torch.bfloat16)
     o, lse = fwd(qkv, n, N, H)
-    ro, rl = attn_ref(qkv, n, N, 64 * H, H)
+    ro, rl = attn_ref(qkv, n, N, H)
     assert rel(o, ro) < BF16_TOL and rel(lse, rl) < 1e-5
 
 
@@ -63,7 +34,7 @@ def test_long_attention_backward(n, N, H):
     qkv = torch.randn(n * N, 3 * D, device="cuda").to(torch.bfloat16)
     do = torch.randn(n * N, D, device="cuda").to(torch.bfloat16)
     x = qkv.float().requires_grad_(True)
-    attn_ref(x, n, N, D, H)[0].backward(do.float())
+    attn_ref(x, n, N, H)[0].backward(do.float())
     o, lse = fwd(qkv, n, N, H)
     dqkv = bwd(qkv, o, do, lse, n, N, H)
     for j in range(3):

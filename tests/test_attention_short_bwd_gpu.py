@@ -4,13 +4,9 @@ crops, the fused inverse RoPE with 5 prefix tokens, and bit-identical repeats (d
 import pytest
 import torch
 
+from attention_helpers import BF16_TOL, attn_ref, bwd, fwd, rel
+
 pytestmark = pytest.mark.gpu
-
-BF16_TOL = 6e-3      # norm-wise relative error of a bf16-stored result (2^-9 per element)
-
-
-def rel(a, b):
-    return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-30)).item()
 
 
 @pytest.fixture(autouse=True)
@@ -18,21 +14,9 @@ def _seed(native):
     torch.manual_seed(0)
 
 
-def attn_ref(qkv, n, N, D, H):
-    q, k, v = qkv.float().reshape(n, N, 3, H, 64).permute(2, 0, 3, 1, 4)
-    s = (q @ k.transpose(-1, -2)) * 0.125
-    return (torch.softmax(s, -1) @ v).permute(0, 2, 1, 3).reshape(n * N, D)
-
-
 def fwd_bwd(qkv, do, n, N, H, **rope):
-    from dinov3_jax import ops
-    D = 64 * H
-    o = torch.empty(n * N, D, device="cuda", dtype=torch.bfloat16)
-    lse = torch.zeros(n, H, N, device="cuda")
-    ops.attn_fwd(qkv, o, lse, n, N, D, H)
-    dqkv = torch.full((n * N, 3 * D), float("nan"), device="cuda", dtype=torch.bfloat16)
-    ops.attn_bwd(qkv, o, do, lse, torch.zeros(n, H, N, device="cuda"), dqkv, n, N, D, H, **rope)
-    return dqkv
+    o, lse = fwd(qkv, n, N, H)
+    return bwd(qkv, o, do, lse, n, N, H, **rope)
 
 
 def check_against_autograd(n, N, H):
@@ -40,7 +24,7 @@ def check_against_autograd(n, N, H):
     qkv = torch.randn(n * N, 3 * D, device="cuda").to(torch.bfloat16)
     do = torch.randn(n * N, D, device="cuda").to(torch.bfloat16)
     x = qkv.float().requires_grad_(True)
-    attn_ref(x, n, N, D, H).backward(do.float())
+    attn_ref(x, n, N, H)[0].backward(do.float())
     dqkv = fwd_bwd(qkv, do, n, N, H)
     if N == 1:    # softmax over one key: the q and k gradients are 0, only the bf16 rounding of O and dO remains
         assert dqkv[:, :2 * D].float().abs().max().item() < 1e-3

@@ -6,6 +6,8 @@ import numpy as np
 import pytest
 import torch
 
+from attention_helpers import attn_ref, bwd, fwd
+
 pytestmark = pytest.mark.gpu
 
 BF16_TOL = 6e-3      # norm-wise relative error of a bf16-stored result (2^-9 per element)
@@ -108,39 +110,25 @@ def test_gemm_rejects_bad_arguments():
 
 
 # --------------------------------------------------------------------------------------------------- attention
-def attn_ref(qkv, n, N, D, H):
-    q, k, v = qkv.float().reshape(n, N, 3, H, 64).permute(2, 0, 3, 1, 4)
-    s = (q @ k.transpose(-1, -2)) * 0.125
-    o = (torch.softmax(s, -1) @ v).permute(0, 2, 1, 3).reshape(n * N, D)
-    return o, torch.logsumexp(s, -1)
-
-
 @pytest.mark.parametrize("n,N,H", [(3, 197, 2), (5, 37, 2), (2, 128, 1), (2, 257, 1), (4, 50, 3), (1, 1, 1), (2, 17, 6),
                                    (2, 256, 1), (3, 200, 1), (7, 64, 1), (4, 65, 2), (3, 129, 1),
                                    (40, 197, 16), (130, 37, 16), (9, 201, 8)])
 def test_attention_forward(n, N, H):
-    from dinov3_jax import ops
-    D = 64 * H
-    qkv = torch.randn(n * N, 3 * D, device="cuda").to(torch.bfloat16)
-    o = torch.full((n * N, D), float("nan"), device="cuda", dtype=torch.bfloat16)
-    lse = torch.zeros(n, H, N, device="cuda")
-    ops.attn_fwd(qkv, o, lse, n, N, D, H)
-    ro, rl = attn_ref(qkv, n, N, D, H)
+    qkv = torch.randn(n * N, 3 * 64 * H, device="cuda").to(torch.bfloat16)
+    o, lse = fwd(qkv, n, N, H)
+    ro, rl = attn_ref(qkv, n, N, H)
     assert rel(o, ro) < BF16_TOL and rel(lse, rl) < 1e-5
 
 
 @pytest.mark.parametrize("n,N,H", [(2, 128, 1), (3, 197, 2), (5, 37, 2), (4, 50, 3), (2, 256, 1), (2, 17, 6), (2, 257, 2), (1, 384, 1), (3, 300, 1)])
 def test_attention_backward(n, N, H):
-    from dinov3_jax import ops
     D = 64 * H
     qkv = torch.randn(n * N, 3 * D, device="cuda").to(torch.bfloat16)
     do = torch.randn(n * N, D, device="cuda").to(torch.bfloat16)
     x = qkv.float().requires_grad_(True)
-    attn_ref(x, n, N, D, H)[0].backward(do.float())
-    o = torch.empty(n * N, D, device="cuda", dtype=torch.bfloat16); lse = torch.zeros(n, H, N, device="cuda")
-    ops.attn_fwd(qkv, o, lse, n, N, D, H)
-    dqkv = torch.full((n * N, 3 * D), float("nan"), device="cuda", dtype=torch.bfloat16)
-    ops.attn_bwd(qkv, o, do, lse, torch.zeros(n, H, N, device="cuda"), dqkv, n, N, D, H)
+    attn_ref(x, n, N, H)[0].backward(do.float())
+    o, lse = fwd(qkv, n, N, H)
+    dqkv = bwd(qkv, o, do, lse, n, N, H)
     for j in range(3):
         assert rel(dqkv[:, j * D:(j + 1) * D], x.grad[:, j * D:(j + 1) * D]) < 1e-2
 
@@ -154,13 +142,10 @@ def test_attention_backward_fused_inverse_rope():
     sin, cos = [t.cuda().contiguous() for t in rope_sincos(Hp, Hp, 64, 100.0, torch.float32)]
     qkv = torch.randn(n * N, 3 * D, device="cuda").to(torch.bfloat16)
     do = torch.randn(n * N, D, device="cuda").to(torch.bfloat16)
-    o = torch.empty(n * N, D, device="cuda", dtype=torch.bfloat16); lse = torch.zeros(n, H, N, device="cuda")
-    ops.attn_fwd(qkv, o, lse, n, N, D, H)
-    d1 = torch.empty(n * N, 3 * D, device="cuda", dtype=torch.bfloat16); d2 = torch.empty_like(d1)
-    delta = torch.zeros(n, H, N, device="cuda")
-    ops.attn_bwd(qkv, o, do, lse, delta, d1, n, N, D, H)
+    o, lse = fwd(qkv, n, N, H)
+    d1 = bwd(qkv, o, do, lse, n, N, H)
     ops.rope(d1, sin, cos, N, 1, D, 64, inverse=True)
-    ops.attn_bwd(qkv, o, do, lse, delta, d2, n, N, D, H, rope_sin=sin, rope_cos=cos, rope_prefix=1)
+    d2 = bwd(qkv, o, do, lse, n, N, H, rope_sin=sin, rope_cos=cos, rope_prefix=1)
     assert rel(d2, d1) < BF16_TOL          # d1 is rounded to bf16 twice, d2 once
     assert torch.equal(d2[:, 2 * D:], d1[:, 2 * D:])
 
