@@ -113,7 +113,7 @@ extern "C" {
 
 int d3_set_scatter_mode(int mode) { d3::set_scatter_mode(mode); return D3_OK; }
 
-int d3_abi_version(void) { return 5; }   // 2: d3_gemm_epilogue gained the sc_* scatter fields; 3: round-2 entry points (swiglu, ema, colmax, deterministic Sinkhorn sums, koleo rows, augmentation); 4: two entry points removed (the plain LayerNorm backward is d3_layernorm_bwd_ls without a tail; d3_sinkhorn_colsum is deterministic for every K); 5: d3_debug_attn_trace removed (the attention clock64() trace)
+int d3_abi_version(void) { return 6; }   // 2: d3_gemm_epilogue gained the sc_* scatter fields; 3: round-2 entry points (swiglu, ema, colmax, deterministic Sinkhorn sums, koleo rows, augmentation); 4: two entry points removed (the plain LayerNorm backward is d3_layernorm_bwd_ls without a tail; d3_sinkhorn_colsum is deterministic for every K); 5: d3_debug_attn_trace removed (the attention clock64() trace); 6: d3_koleo_fwd_bwd removed (it is d3_koleo_fwd_bwd_rows with row0 = 0, nrows = B)
 int d3_set_sm_limit(int n) {
   if (n < 0) return set_error(D3_ERR_ARG, "d3_set_sm_limit: n < 0");
   g_sm_limit = n;

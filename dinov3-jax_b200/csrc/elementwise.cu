@@ -6,17 +6,6 @@
 
 namespace d3 {
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
 // ------------------------------------------------------------------------------------------------ im2col
 // layers/patch_embed.py:38-51: conv with kernel == stride == p is a GEMM over flattened patches.
 // img bf16 [n, H, W, 3] -> out bf16 [n*Hp*Wp, p*p*3], k = (a*p + b)*3 + c  (kernel layout [p,p,3,D]).

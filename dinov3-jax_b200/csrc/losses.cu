@@ -8,42 +8,41 @@
 
 namespace d3 {
 
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float wmax(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
 // block reductions over 256 threads (8 warps)
 __device__ __forceinline__ float block_sum(float v, float* sh) {
-  v = wsum(v);
+  v = warp_sum(v);
   __syncthreads();
   if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
   __syncthreads();
   float t = (threadIdx.x < (blockDim.x >> 5)) ? sh[threadIdx.x] : 0.f;
-  if (threadIdx.x < 32) t = wsum(t);
+  if (threadIdx.x < 32) t = warp_sum(t);
   if (threadIdx.x == 0) sh[0] = t;
   __syncthreads();
   return sh[0];
 }
 __device__ __forceinline__ float block_max(float v, float* sh) {
-  v = wmax(v);
+  v = warp_max(v);
   __syncthreads();
   if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
   __syncthreads();
   float t = (threadIdx.x < (blockDim.x >> 5)) ? sh[threadIdx.x] : -CUDART_INF_F;
-  if (threadIdx.x < 32) t = wmax(t);
+  if (threadIdx.x < 32) t = warp_max(t);
   if (threadIdx.x == 0) sh[0] = t;
   __syncthreads();
   return sh[0];
 }
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
+// Elements 4g .. 4g+3 of a row of n floats.  VEC: one 128-bit load (the row is 16-byte aligned and n % 4 == 0).
+// Otherwise four scalar loads, and an element at or past n reads as `fill`, the neutral value of the reduction it
+// enters, so that both instances walk the same four-column groups.
+template <bool VEC, class I>
+__device__ __forceinline__ float4 load4(const float* __restrict__ row, I g, I n, float fill) {
+  if constexpr (VEC) {
+    return reinterpret_cast<const float4*>(row)[g];
+  } else {
+    const I k = 4 * g;
+    return make_float4(k < n ? row[k] : fill, k + 1 < n ? row[k + 1] : fill, k + 2 < n ? row[k + 2] : fill,
+                       k + 3 < n ? row[k + 3] : fill);
+  }
 }
 // 1/s for a Sinkhorn column sum; a column whose terms all underflowed (s == 0) contributes nothing instead of 0/0
 __device__ __forceinline__ float rcp_pos(float s) { return s > 0.f ? __fdividef(1.f, s) : 0.f; }
@@ -61,24 +60,24 @@ __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
 // largest term at 1, so a prototype far below the batch maximum keeps its Sinkhorn mass 1/K like in the reference
 // instead of underflowing to 0/0 (a single global shift loses columns more than ~3.5 below the maximum at temp 0.04).
 // The row step's E^T a (K floats) is what the reference psums over "dp" (:53 / ibot :99).
-__global__ void absmax_kernel(const float* __restrict__ L, long n, float* __restrict__ out) {
+// absmax, colmax, sk_rowsum and the cross-entropy take four columns per thread.  VEC reads them with 128-bit loads,
+// used when K % 4 == 0 and the rows are 16-byte aligned (every recipe: K = 65536); otherwise the same walk reads them
+// with scalar loads (load4).
+// n4 = ceil(n / 4) groups of four elements
+template <bool VEC>
+__global__ void absmax_kernel(const float* __restrict__ L, long n4, float* __restrict__ out, long n) {
   __shared__ float sh[32];
   float m = -CUDART_INF_F;
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) m = fmaxf(m, L[i]);
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
+    const float4 v = load4<VEC>(L, i, n, -CUDART_INF_F);
+    m = fmaxf(fmaxf(m, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
+  }
   m = block_max(m, sh);
   if (threadIdx.x == 0) atomic_max_float(out, m);
 }
-// cm[k] = max(cm[k], max_b L[b,k])   (cm pre-set to -inf; atomics across row slabs)
+// cm[k] = max(cm[k], max_b L[b,k])   (cm pre-set to -inf; atomics across row slabs), four columns per thread
+template <bool VEC>
 __global__ void colmax_kernel(const float* __restrict__ L, float* __restrict__ cm, int R, int K) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  const int slab = (R + gridDim.y - 1) / gridDim.y;
-  const int r0 = blockIdx.y * slab, r1 = min(R, r0 + slab);
-  if (k >= K || r0 >= r1) return;
-  float m = -CUDART_INF_F;
-  for (int b = r0; b < r1; ++b) m = fmaxf(m, L[(long)b * K + k]);
-  atomic_max_float(&cm[k], m);
-}
-__global__ void colmax_vec_kernel(const float* __restrict__ L, float* __restrict__ cm, int R, int K) {
   const int k = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   const int slab = (R + gridDim.y - 1) / gridDim.y;
   const int r0 = blockIdx.y * slab, r1 = min(R, r0 + slab);
@@ -86,33 +85,84 @@ __global__ void colmax_vec_kernel(const float* __restrict__ L, float* __restrict
   float4 m = make_float4(-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F);
 #pragma unroll 4
   for (int b = r0; b < r1; ++b) {
-    const float4 v = *reinterpret_cast<const float4*>(L + (long)b * K + k);
+    const float4 v = load4<VEC>(L + (long)b * K + k, 0, K - k, -CUDART_INF_F);   // row b from column k on
     m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
   }
-  atomic_max_float(&cm[k], m.x); atomic_max_float(&cm[k + 1], m.y);
-  atomic_max_float(&cm[k + 2], m.z); atomic_max_float(&cm[k + 3], m.w);
+  const float mv[4] = {m.x, m.y, m.z, m.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if constexpr (!VEC) if (k + j >= K) break;
+    atomic_max_float(&cm[k + j], mv[j]);
+  }
+}
+// Sinkhorn column sums, part[slab][k] = sum over the row slab of E[b,k] * a[b]  (a == nullptr -> a = 1); slab_combine
+// then adds the slabs in a fixed order.  Float atomics here would perturb s[k] in the last bit from run to run, which
+// flips a few bf16 roundings of the iBOT d(logits) and grows to ~3e-3 in the embedding gradients through the bf16
+// backward chain (tools/check_determinism.py); with the slabs the whole dX chain of a step is bit-reproducible.
+// VEC: four columns per thread with 128-bit loads (K % 4 == 0, 16-byte aligned L and mx); otherwise one column.
+template <bool VEC>
+__global__ void sk_colsum_part_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
+                                      const float* __restrict__ a, float* __restrict__ part, int R, int K) {
+  const int k = (blockIdx.x * blockDim.x + threadIdx.x) * (VEC ? 4 : 1);
+  const int slab = (R + gridDim.y - 1) / gridDim.y;
+  const int r0 = blockIdx.y * slab, r1 = min(R, r0 + slab);
+  if (k >= K) return;
+  const float c = inv_temp * 1.4426950408889634f;
+  if constexpr (VEC) {
+    const float4 m4 = *reinterpret_cast<const float4*>(mx + k);
+    const float4 mc = make_float4(m4.x * c, m4.y * c, m4.z * c, m4.w * c);
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 4
+    for (int b = r0; b < r1; ++b) {
+      const float4 v = *reinterpret_cast<const float4*>(L + (long)b * K + k);
+      const float w = a ? a[b] : 1.f;
+      acc.x += exp2f(v.x * c - mc.x) * w; acc.y += exp2f(v.y * c - mc.y) * w;
+      acc.z += exp2f(v.z * c - mc.z) * w; acc.w += exp2f(v.w * c - mc.w) * w;
+    }
+    *reinterpret_cast<float4*>(part + (long)blockIdx.y * K + k) = acc;
+  } else {
+    const float mc = mx[k] * c;
+    float acc = 0.f;
+#pragma unroll 4
+    for (int b = r0; b < r1; ++b) acc += exp2f(L[(long)b * K + k] * c - mc) * (a ? a[b] : 1.f);
+    part[(long)blockIdx.y * K + k] = acc;
+  }
 }
 // a[b] = 1 / (Btot * sum_k E[b,k] * r[k]),  r[k] = 1/(K*s[k])
+template <bool VEC>
 __global__ void sk_rowsum_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
                                  const float* __restrict__ s, const float* __restrict__ btot, float* __restrict__ a,
                                  int R, int K) {
   __shared__ float sh[32];
   const int b = blockIdx.x;
+  const float c = inv_temp * 1.4426950408889634f;
+  const float* Lb = L + (long)b * K;
   float acc = 0.f;
-  for (int k = threadIdx.x; k < K; k += blockDim.x)
-    acc += __expf((L[(long)b * K + k] - mx[k]) * inv_temp) * rcp_pos((float)K * s[k]);
-  acc = block_sum(acc, sh);
+#pragma unroll 4
+  for (int k = threadIdx.x; k < (VEC ? K / 4 : (K + 3) / 4); k += blockDim.x) {
+    // past the row E = 2^-inf = 0 and r = rcp_pos(0) = 0
+    const float4 v = load4<VEC>(Lb, k, K, -CUDART_INF_F), sv = load4<VEC>(s, k, K, 0.f), mv = load4<VEC>(mx, k, K, 0.f);
+    acc += exp2f((v.x - mv.x) * c) * rcp_pos(sv.x) + exp2f((v.y - mv.y) * c) * rcp_pos(sv.y) +
+           exp2f((v.z - mv.z) * c) * rcp_pos(sv.z) + exp2f((v.w - mv.w) * c) * rcp_pos(sv.w);
+  }
+  acc = block_sum(acc, sh) / (float)K;
   if (threadIdx.x == 0) a[b] = acc > 0.f ? 1.f / (*btot * acc) : 0.f;
 }
-// materialise teacher probabilities (tests / optional consumers): Q[b,k] = Btot * E * r[k] * a[b]
+// Q[b,k] for teacher logit t = L[b,k], shift m = mx[k], ct = log2(e) / temp, r = rcp_pos(s[k]) and
+// coef = Btot * a[b] / K.  The cross-entropy and sk_probs_kernel both evaluate it here, so the Q a test materialises
+// is the Q behind dS.  It takes r rather than s so that the cross-entropy computes r once for both teacher rows.
+__device__ __forceinline__ float teacher_prob(float t, float m, float ct, float r, float coef) {
+  return coef * exp2f((t - m) * ct) * r;
+}
+// materialise teacher probabilities (tests / optional consumers)
 __global__ void sk_probs_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
                                 const float* __restrict__ s, const float* __restrict__ a,
                                 const float* __restrict__ btot, float* __restrict__ Q, int R, int K) {
   const long n = (long)R * K;
-  const float bt = *btot;
+  const float bt = *btot, ct = inv_temp * 1.4426950408889634f, invK = 1.f / (float)K;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     const int b = (int)(i / K), k = (int)(i % K);
-    Q[i] = bt * __expf((L[i] - mx[k]) * inv_temp) * rcp_pos((float)K * s[k]) * a[b];
+    Q[i] = teacher_prob(L[i], mx[k], ct, rcp_pos(s[k]), bt * a[b] * invK);
   }
 }
 
@@ -152,7 +202,9 @@ __global__ void center_update_kernel(float* __restrict__ center, const float* __
 // rows p in {t0[i], t1[i]} (-1 = none), Q_p from the Sinkhorn scalings above.
 // row_loss[i] = wm[i] * loss_i (added to metric[slot[i]] by metric_rows_kernel) ;  dS[i,k] = wg[i]/ts * (npairs * softmax[k] - sum_p Q_p[k])   (bf16)
 // (dino_clstoken_loss.py:66-89; ibot_patch_loss.py:13-14,55-67; weights per train/ssl_meta_arch.py:480-525)
-__global__ void __launch_bounds__(256)
+// The second pass re-reads the student row from L2.
+template <bool VEC>
+__global__ void __launch_bounds__(512)
 ce_fwd_bwd_kernel(const float* __restrict__ S, float inv_ts, const float* __restrict__ Lt,
                   const float* __restrict__ mx, float inv_tt, const float* __restrict__ s_t,
                   const float* __restrict__ a_t, const float* __restrict__ btot, const int* __restrict__ t0,
@@ -160,127 +212,15 @@ ce_fwd_bwd_kernel(const float* __restrict__ S, float inv_ts, const float* __rest
                   const int* __restrict__ slot, float* __restrict__ row_loss, __nv_bfloat16* __restrict__ dS, int K) {
   __shared__ float sh[32];
   const int i = blockIdx.x;
-  const float* Si = S + (long)i * K;
-  // online max / sum-exp
-  float m = -CUDART_INF_F, z = 0.f;
-  for (int k = threadIdx.x; k < K; k += blockDim.x) {
-    const float v = Si[k] * inv_ts;
-    if (v > m) { z = z * __expf(m - v) + 1.f; m = v; }
-    else z += __expf(v - m);
-  }
-  const float gm = block_max(m, sh);
-  z = block_sum(z * __expf(m - gm), sh);
-  const float lse = gm + logf(z);
-  const int p0 = t0[i], p1 = t1[i];
-  const float np = (p0 >= 0 ? 1.f : 0.f) + (p1 >= 0 ? 1.f : 0.f);
-  const float bt = s_t ? *btot : 1.f;
-  const float c0 = (s_t && p0 >= 0) ? bt * a_t[p0] : 0.f;
-  const float c1 = (s_t && p1 >= 0) ? bt * a_t[p1] : 0.f;
-  const float* L0 = Lt + (long)(p0 >= 0 ? p0 : 0) * K;
-  const float* L1 = Lt + (long)(p1 >= 0 ? p1 : 0) * K;
-  const float g = wg[i] * inv_ts;
-  float loss = 0.f;
-  for (int k = threadIdx.x; k < K; k += blockDim.x) {
-    const float lsm = Si[k] * inv_ts - lse;
-    float q = 0.f;
-    if (s_t) {
-      const float rk = rcp_pos((float)K * s_t[k]), mt = mx[k];
-      if (p0 >= 0) q += c0 * __expf((L0[k] - mt) * inv_tt) * rk;
-      if (p1 >= 0) q += c1 * __expf((L1[k] - mt) * inv_tt) * rk;
-    } else {          // teacher rows are already probabilities
-      if (p0 >= 0) q += L0[k];
-      if (p1 >= 0) q += L1[k];
-    }
-    loss -= q * lsm;
-    if (dS) dS[(long)i * K + k] = __float2bfloat16(g * (np * __expf(lsm) - q));
-  }
-  loss = block_sum(loss, sh);
-  if (threadIdx.x == 0) row_loss[i] = wm[i] * loss;
-}
-
-
-// ---- 128-bit versions used when K % 4 == 0 and the rows are 16-byte aligned (every recipe: K = 65536) --------------
-__global__ void absmax_vec_kernel(const float4* __restrict__ L, long n4, float* __restrict__ out) {
-  __shared__ float sh[32];
-  float m = -CUDART_INF_F;
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
-    const float4 v = L[i];
-    m = fmaxf(fmaxf(m, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
-  }
-  m = block_max(m, sh);
-  if (threadIdx.x == 0) atomic_max_float(out, m);
-}
-// Sinkhorn column sums, part[slab][k] = sum over the row slab of E[b,k] * a[b]  (a == nullptr -> a = 1); slab_combine
-// then adds the slabs in a fixed order.  Float atomics here would perturb s[k] in the last bit from run to run, which
-// flips a few bf16 roundings of the iBOT d(logits) and grows to ~3e-3 in the embedding gradients through the bf16
-// backward chain (tools/check_determinism.py); with the slabs the whole dX chain of a step is bit-reproducible.
-// VEC: four columns per thread with 128-bit loads (K % 4 == 0, 16-byte aligned L and mx); otherwise one column.
-template <bool VEC>
-__global__ void sk_colsum_part_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
-                                      const float* __restrict__ a, float* __restrict__ part, int R, int K) {
-  const int k = (blockIdx.x * blockDim.x + threadIdx.x) * (VEC ? 4 : 1);
-  const int slab = (R + gridDim.y - 1) / gridDim.y;
-  const int r0 = blockIdx.y * slab, r1 = min(R, r0 + slab);
-  if (k >= K) return;
-  const float c = inv_temp * 1.4426950408889634f;
-  if constexpr (VEC) {
-    const float4 m4 = *reinterpret_cast<const float4*>(mx + k);
-    const float4 mc = make_float4(m4.x * c, m4.y * c, m4.z * c, m4.w * c);
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 4
-    for (int b = r0; b < r1; ++b) {
-      const float4 v = *reinterpret_cast<const float4*>(L + (long)b * K + k);
-      const float w = a ? a[b] : 1.f;
-      acc.x += exp2f(v.x * c - mc.x) * w; acc.y += exp2f(v.y * c - mc.y) * w;
-      acc.z += exp2f(v.z * c - mc.z) * w; acc.w += exp2f(v.w * c - mc.w) * w;
-    }
-    *reinterpret_cast<float4*>(part + (long)blockIdx.y * K + k) = acc;
-  } else {
-    const float mc = mx[k] * c;
-    float acc = 0.f;
-#pragma unroll 4
-    for (int b = r0; b < r1; ++b) acc += exp2f(L[(long)b * K + k] * c - mc) * (a ? a[b] : 1.f);
-    part[(long)blockIdx.y * K + k] = acc;
-  }
-}
-__global__ void sk_rowsum_vec_kernel(const float* __restrict__ L, const float* __restrict__ mx, float inv_temp,
-                                     const float* __restrict__ s, const float* __restrict__ btot, float* __restrict__ a,
-                                     int R, int K) {
-  __shared__ float sh[32];
-  const int b = blockIdx.x;
-  const float c = inv_temp * 1.4426950408889634f;
-  const float4* Lb = reinterpret_cast<const float4*>(L + (long)b * K);
-  const float4* s4 = reinterpret_cast<const float4*>(s);
-  const float4* m4 = reinterpret_cast<const float4*>(mx);
-  float acc = 0.f;
-#pragma unroll 4
-  for (int k = threadIdx.x; k < K / 4; k += blockDim.x) {
-    const float4 v = Lb[k], sv = s4[k], mv = m4[k];
-    acc += exp2f((v.x - mv.x) * c) * rcp_pos(sv.x) + exp2f((v.y - mv.y) * c) * rcp_pos(sv.y) +
-           exp2f((v.z - mv.z) * c) * rcp_pos(sv.z) + exp2f((v.w - mv.w) * c) * rcp_pos(sv.w);
-  }
-  acc = block_sum(acc, sh) / (float)K;
-  if (threadIdx.x == 0) a[b] = acc > 0.f ? 1.f / (*btot * acc) : 0.f;
-}
-
-// vectorised cross-entropy: same contract as ce_fwd_bwd_kernel; the second pass re-reads the student row from L2
-__global__ void __launch_bounds__(512)
-ce_fwd_bwd_vec_kernel(const float* __restrict__ S, float inv_ts, const float* __restrict__ Lt,
-                      const float* __restrict__ mx, float inv_tt, const float* __restrict__ s_t,
-                      const float* __restrict__ a_t, const float* __restrict__ btot, const int* __restrict__ t0,
-                      const int* __restrict__ t1, const float* __restrict__ wm, const float* __restrict__ wg,
-                      const int* __restrict__ slot, float* __restrict__ row_loss, __nv_bfloat16* __restrict__ dS, int K) {
-  __shared__ float sh[32];
-  const int i = blockIdx.x;
-  const int K4 = K >> 2;
+  const int K4 = VEC ? K >> 2 : (K + 3) >> 2;
   const float LOG2E = 1.4426950408889634f;
-  const float4* Si = reinterpret_cast<const float4*>(S + (long)i * K);
+  const float* Si = S + (long)i * K;
   const float cs = inv_ts * LOG2E;
-  // online max / sum of 2^(cs * s) per thread, one float4 at a time
+  // online max / sum of 2^(cs * s) per thread, one float4 at a time (a column past the row adds 2^-inf = 0)
   float m = -CUDART_INF_F, z = 0.f;
 #pragma unroll 2
   for (int k = threadIdx.x; k < K4; k += blockDim.x) {
-    const float4 v = Si[k];
+    const float4 v = load4<VEC>(Si, k, K, -CUDART_INF_F);
     const float m4 = fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)) * cs;
     if (m4 > m) { z *= exp2f(m - m4); m = m4; }
     z += exp2f(v.x * cs - m) + exp2f(v.y * cs - m) + exp2f(v.z * cs - m) + exp2f(v.w * cs - m);
@@ -293,46 +233,60 @@ ce_fwd_bwd_vec_kernel(const float* __restrict__ S, float inv_ts, const float* __
   const float ct = inv_tt * LOG2E;
   const float bt = s_t ? *btot : 1.f;
   const float invK = 1.f / (float)K;
-  const float4* mx4 = reinterpret_cast<const float4*>(mx);
   const float c0 = (s_t && p0 >= 0) ? bt * a_t[p0] * invK : 0.f;
   const float c1 = (s_t && p1 >= 0) ? bt * a_t[p1] * invK : 0.f;
-  const float4* L0 = reinterpret_cast<const float4*>(Lt + (long)(p0 >= 0 ? p0 : 0) * K);
-  const float4* L1 = reinterpret_cast<const float4*>(Lt + (long)(p1 >= 0 ? p1 : 0) * K);
-  const float4* st4 = reinterpret_cast<const float4*>(s_t);
+  const float* L0 = Lt + (long)(p0 >= 0 ? p0 : 0) * K;
+  const float* L1 = Lt + (long)(p1 >= 0 ? p1 : 0) * K;
   const float g = wg[i] * inv_ts;
   const float LN2 = 0.6931471805599453f;
-  uint2* dSi = dS ? reinterpret_cast<uint2*>(dS + (long)i * K) : nullptr;
+  __nv_bfloat16* dSi = dS ? dS + (long)i * K : nullptr;
   float loss = 0.f;
 #pragma unroll 2
   for (int k = threadIdx.x; k < K4; k += blockDim.x) {
-    const float4 v = Si[k];
-    const float l2[4] = {v.x * cs - lse2, v.y * cs - lse2, v.z * cs - lse2, v.w * cs - lse2};   // log2 softmax
+    const float4 v = load4<VEC>(Si, k, K, -CUDART_INF_F);
+    float l2[4] = {v.x * cs - lse2, v.y * cs - lse2, v.z * cs - lse2, v.w * cs - lse2};   // log2 softmax
     float q[4] = {0.f, 0.f, 0.f, 0.f};
     if (s_t) {
-      const float4 sv = st4[k], mv = mx4[k];
+      const float4 sv = load4<VEC>(s_t, k, K, 0.f), mv = load4<VEC>(mx, k, K, 0.f);
       const float r[4] = {rcp_pos(sv.x), rcp_pos(sv.y), rcp_pos(sv.z), rcp_pos(sv.w)};
       if (p0 >= 0) {
-        const float4 t = L0[k];
-        q[0] += c0 * exp2f((t.x - mv.x) * ct) * r[0]; q[1] += c0 * exp2f((t.y - mv.y) * ct) * r[1];
-        q[2] += c0 * exp2f((t.z - mv.z) * ct) * r[2]; q[3] += c0 * exp2f((t.w - mv.w) * ct) * r[3];
+        const float4 t = load4<VEC>(L0, k, K, 0.f);
+        q[0] += teacher_prob(t.x, mv.x, ct, r[0], c0); q[1] += teacher_prob(t.y, mv.y, ct, r[1], c0);
+        q[2] += teacher_prob(t.z, mv.z, ct, r[2], c0); q[3] += teacher_prob(t.w, mv.w, ct, r[3], c0);
       }
       if (p1 >= 0) {
-        const float4 t = L1[k];
-        q[0] += c1 * exp2f((t.x - mv.x) * ct) * r[0]; q[1] += c1 * exp2f((t.y - mv.y) * ct) * r[1];
-        q[2] += c1 * exp2f((t.z - mv.z) * ct) * r[2]; q[3] += c1 * exp2f((t.w - mv.w) * ct) * r[3];
+        const float4 t = load4<VEC>(L1, k, K, 0.f);
+        q[0] += teacher_prob(t.x, mv.x, ct, r[0], c1); q[1] += teacher_prob(t.y, mv.y, ct, r[1], c1);
+        q[2] += teacher_prob(t.z, mv.z, ct, r[2], c1); q[3] += teacher_prob(t.w, mv.w, ct, r[3], c1);
       }
-    } else {
-      if (p0 >= 0) { const float4 t = L0[k]; q[0] += t.x; q[1] += t.y; q[2] += t.z; q[3] += t.w; }
-      if (p1 >= 0) { const float4 t = L1[k]; q[0] += t.x; q[1] += t.y; q[2] += t.z; q[3] += t.w; }
+    } else {          // teacher rows are already probabilities
+      if (p0 >= 0) { const float4 t = load4<VEC>(L0, k, K, 0.f); q[0] += t.x; q[1] += t.y; q[2] += t.z; q[3] += t.w; }
+      if (p1 >= 0) { const float4 t = load4<VEC>(L1, k, K, 0.f); q[0] += t.x; q[1] += t.y; q[2] += t.z; q[3] += t.w; }
+    }
+    if constexpr (!VEC) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (4 * k + j >= K) { q[j] = 0.f; l2[j] = 0.f; }   // past the row: no loss term (not 0 * -inf), no dS below
     }
     loss -= (q[0] * l2[0] + q[1] * l2[1] + q[2] * l2[2] + q[3] * l2[3]) * LN2;
-    if (dSi)
-      dSi[k] = make_uint2(pack2(g * (np * exp2f(l2[0]) - q[0]), g * (np * exp2f(l2[1]) - q[1])),
-                          pack2(g * (np * exp2f(l2[2]) - q[2]), g * (np * exp2f(l2[3]) - q[3])));
+    if (dSi) {
+      const float d[4] = {g * (np * exp2f(l2[0]) - q[0]), g * (np * exp2f(l2[1]) - q[1]),
+                          g * (np * exp2f(l2[2]) - q[2]), g * (np * exp2f(l2[3]) - q[3])};
+      if constexpr (VEC) {
+        reinterpret_cast<uint2*>(dSi)[k] = make_uint2(pack_bf16(d[0], d[1]), pack_bf16(d[2], d[3]));
+      } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (4 * k + j < K) dSi[4 * k + j] = __float2bfloat16(d[j]);
+      }
+    }
   }
   loss = block_sum(loss, sh);
   if (threadIdx.x == 0) row_loss[i] = wm[i] * loss;
 }
+// Instantiated here, not implicitly at the end of the file: where a kernel sits in the module changes the code NVVM
+// makes of it.  Emitted last, this instance compiles to other loop code (1024 SASS instructions instead of 1064).
+template __global__ decltype(ce_fwd_bwd_kernel<true>) ce_fwd_bwd_kernel<true>;
 
 // ------------------------------------------------------------------------------------------------ KoLeo
 // loss/koleo_loss.py:16-35:  xn = x/(||x||+eps); nn(i) = argmax_{j!=i} xn_i.xn_j; L = -mean_i log(||xn_i - xn_nn(i)|| + 2 eps)
@@ -471,24 +425,18 @@ extern "C" {
 
 int d3_absmax(const float* L, long long n, float* out /* pre-set to -inf */, void* stream) {
   if (n <= 0) return D3_OK;
-  if (n % 4 == 0 && (uintptr_t)L % 16 == 0)
-    absmax_vec_kernel<<<(int)min((n / 4 + 1023) / 1024, (long long)sm_count() * 8), 256, 0, STREAM(stream)>>>(
-        reinterpret_cast<const float4*>(L), n / 4, out);
-  else
-    absmax_kernel<<<(int)min((n + 1023) / 1024, (long long)sm_count() * 8), 256, 0, STREAM(stream)>>>(L, n, out);
+  const long long n4 = (n + 3) / 4;
+  const auto kernel = n % 4 == 0 && (uintptr_t)L % 16 == 0 ? absmax_kernel<true> : absmax_kernel<false>;
+  kernel<<<(int)min((n4 + 1023) / 1024, (long long)sm_count() * 8), 256, 0, STREAM(stream)>>>(L, n4, out, n);
   D3_CHECK_LAUNCH();
   return D3_OK;
 }
 int d3_colmax(const float* L, float* cm /* [K] pre-set to -inf */, int R, int K, void* stream) {
   if (R <= 0) return D3_OK;
-  if (K % 4 == 0 && (uintptr_t)L % 16 == 0) {
-    const int cx = (K / 4 + 127) / 128;
-    dim3 grid(cx, max(1, min(R / 8, max(1, sm_count() * 8 / cx))));
-    colmax_vec_kernel<<<grid, 128, 0, STREAM(stream)>>>(L, cm, R, K);
-  } else {
-    dim3 grid((K + 255) / 256, max(1, min(R / 8, 64)));
-    colmax_kernel<<<grid, 256, 0, STREAM(stream)>>>(L, cm, R, K);
-  }
+  const int cx = ((K + 3) / 4 + 127) / 128;
+  const dim3 grid(cx, max(1, min(R / 8, max(1, sm_count() * 8 / cx))));
+  const auto kernel = K % 4 == 0 && (uintptr_t)L % 16 == 0 ? colmax_kernel<true> : colmax_kernel<false>;
+  kernel<<<grid, 128, 0, STREAM(stream)>>>(L, cm, R, K);
   D3_CHECK_LAUNCH();
   return D3_OK;
 }
@@ -513,10 +461,9 @@ int d3_sinkhorn_colsum(const float* L, const float* mx, float temp, const float*
 int d3_sinkhorn_rowsum(const float* L, const float* mx, float temp, const float* s, const float* btot, float* a, int R,
                        int K, void* stream) {
   if (R <= 0) return D3_OK;
-  if (K % 4 == 0 && ((uintptr_t)L | (uintptr_t)s | (uintptr_t)mx) % 16 == 0)
-    sk_rowsum_vec_kernel<<<R, 256, 0, STREAM(stream)>>>(L, mx, 1.f / temp, s, btot, a, R, K);
-  else
-    sk_rowsum_kernel<<<R, 256, 0, STREAM(stream)>>>(L, mx, 1.f / temp, s, btot, a, R, K);
+  const auto kernel = K % 4 == 0 && ((uintptr_t)L | (uintptr_t)s | (uintptr_t)mx) % 16 == 0 ? sk_rowsum_kernel<true>
+                                                                                             : sk_rowsum_kernel<false>;
+  kernel<<<R, 256, 0, STREAM(stream)>>>(L, mx, 1.f / temp, s, btot, a, R, K);
   D3_CHECK_LAUNCH();
   return D3_OK;
 }
@@ -597,12 +544,11 @@ int d3_ce_fwd_bwd(const float* S, float student_temp, const float* Lt, const flo
   cudaStream_t st = STREAM(stream);
   float* rows = slab_workspace(Rs, st);
   if (!rows) return D3_ERR_CUDA;
-  if (K % 4 == 0 && ((uintptr_t)S | (uintptr_t)Lt | (uintptr_t)s_t | (uintptr_t)dS | (uintptr_t)mx) % 16 == 0)
-    ce_fwd_bwd_vec_kernel<<<Rs, 512, 0, st>>>(S, 1.f / student_temp, Lt, mx, 1.f / teacher_temp, s_t, a_t, btot,
-                                             t0, t1, wm, wg, slot, rows, (__nv_bfloat16*)dS, K);
-  else
-    ce_fwd_bwd_kernel<<<Rs, 256, 0, st>>>(S, 1.f / student_temp, Lt, mx, 1.f / teacher_temp, s_t, a_t, btot, t0,
-                                         t1, wm, wg, slot, rows, (__nv_bfloat16*)dS, K);
+  const auto kernel =
+      K % 4 == 0 && ((uintptr_t)S | (uintptr_t)Lt | (uintptr_t)s_t | (uintptr_t)dS | (uintptr_t)mx) % 16 == 0
+          ? ce_fwd_bwd_kernel<true> : ce_fwd_bwd_kernel<false>;
+  kernel<<<Rs, 512, 0, st>>>(S, 1.f / student_temp, Lt, mx, 1.f / teacher_temp, s_t, a_t, btot, t0, t1, wm, wg, slot,
+                             rows, (__nv_bfloat16*)dS, K);
   cudaError_t e = cudaPeekAtLastError();
   if (e != cudaSuccess) { slab_release(rows, st); return set_error(D3_ERR_CUDA, cudaGetErrorString(e)); }
   count_launch();
@@ -643,21 +589,6 @@ int d3_gram_diff(const float* Ss, const float* St, void* G_bf16, long long n_ele
   if (!rc) { count_launch(); rc = slab_combine(ws, blocks, 1, 1, 1, loss, 1, st); }
   slab_release(ws, st);
   return rc;
-}
-
-int d3_koleo_fwd_bwd(const float* x, float* xn_scratch, float* nrm_scratch, int* nn_scratch, float* coef_scratch,
-                     float* metric, float* dx, int B, int D, float eps, float w_metric, float w_grad, void* stream) {
-  if (B <= 1) return D3_OK;
-  cudaStream_t st = STREAM(stream);
-  float* rows = slab_workspace(B, st);
-  if (!rows) return D3_ERR_CUDA;
-  koleo_norm_kernel<<<B, 256, 0, st>>>(x, xn_scratch, nrm_scratch, D, eps);
-  koleo_nn_kernel<<<B, 256, 0, st>>>(xn_scratch, nn_scratch, coef_scratch, rows, B, D, eps, w_metric, w_grad, 0, B);
-  koleo_bwd_kernel<<<B, 256, D * sizeof(float), st>>>(x, xn_scratch, nrm_scratch, nn_scratch, coef_scratch, dx, B, D, eps);
-  cudaError_t e = cudaPeekAtLastError();
-  if (e != cudaSuccess) { slab_release(rows, st); return set_error(D3_ERR_CUDA, cudaGetErrorString(e)); }
-  count_launch(3);
-  return add_row_losses(rows, nullptr, B, metric, st);
 }
 
 }  // extern "C"

@@ -263,5 +263,16 @@ __device__ __forceinline__ float2 unpack_bf16(uint32_t u) {
   __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&u);
   return __bfloat1622float2(v);
 }
+// butterfly reductions: every lane of the (converged) warp gets the result
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
 
 }  // namespace d3

@@ -73,7 +73,6 @@ SIGNATURES = {
     "d3_ce_fwd_bwd": [P, F, P, P, F, P, P, P, P, P, P, P, P, P, P, I, I, P],
     "d3_gram_diff": [P, P, P, LL, I, F, P, I, I, P],
     "d3_resize_tokens_bicubic": [P, P, I, I, I, I, I, I, I, P],
-    "d3_koleo_fwd_bwd": [P, P, P, P, P, P, P, I, I, F, F, F, P],
     "d3_koleo_fwd_bwd_rows": [P, P, P, P, P, P, P, I, I, I, I, F, F, F, P],
     "d3_aug_resized_crop": [P, I, I, I, P, I, P, I, P],
     "d3_aug_color": [P, P, I, I, P, P],

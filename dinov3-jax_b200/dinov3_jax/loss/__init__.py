@@ -169,9 +169,9 @@ class KoLeoLossDistributed:
         self.comm.all_gather(allx, x)
         n = world * B
         met, dx = torch.zeros(1, device=dev), torch.zeros(n, D, device=dev)
-        ops.koleo_fwd_bwd_rows(allx, torch.empty(n, D, device=dev), torch.empty(n, device=dev),
-                               torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, device=dev), met, dx,
-                               rank * B, B, 1.0, 0.0, eps)
+        ops.koleo_fwd_bwd(allx, torch.empty(n, D, device=dev), torch.empty(n, device=dev),
+                          torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, device=dev), met, dx, 1.0, 0.0,
+                          eps, row0=rank * B, nrows=B)
         return met[0]
 
 

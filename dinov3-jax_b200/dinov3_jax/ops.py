@@ -290,17 +290,11 @@ def ce_fwd_bwd(S, student_temp, Lt, mx, teacher_temp, s_t, a_t, btot, t0, t1, wm
             "d3_ce_fwd_bwd")
 
 
-def koleo_fwd_bwd(x, xn, nrm, nn, coef, metric, dx, w_metric, w_grad, eps=1e-8):
+def koleo_fwd_bwd(x, xn, nrm, nn, coef, metric, dx, w_metric, w_grad, eps=1e-8, row0=0, nrows=None):
+    """KoLeo over the rows of x, with the loss terms restricted to rows [row0, row0+nrows) (default: all rows)."""
     B, D = x.shape
     assert x.dtype == f32 and nn.dtype == torch.int32
-    N.check(N.init().d3_koleo_fwd_bwd(_p(x), _p(xn), _p(nrm), _p(nn), _p(coef), _p(metric), _p(dx), B, D, eps,
-                                      w_metric, w_grad, _s()), "d3_koleo_fwd_bwd")
-
-
-def koleo_fwd_bwd_rows(x, xn, nrm, nn, coef, metric, dx, row0, nrows, w_metric, w_grad, eps=1e-8):
-    """KoLeo with the loss terms restricted to rows [row0, row0+nrows) of the (all-gathered) matrix x."""
-    B, D = x.shape
-    assert x.dtype == f32 and nn.dtype == torch.int32
+    nrows = B if nrows is None else nrows
     N.check(N.init().d3_koleo_fwd_bwd_rows(_p(x), _p(xn), _p(nrm), _p(nn), _p(coef), _p(metric), _p(dx), B, D, int(row0),
                                            int(nrows), eps, w_metric, w_grad, _s()), "d3_koleo_fwd_bwd_rows")
 

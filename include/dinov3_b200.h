@@ -225,16 +225,14 @@ int d3_gram_diff(const float* Ss, const float* St, void* G_bf16, long long n_ele
 int d3_resize_tokens_bicubic(const float* src, float* dst, int n, int Hs, int Ws, int Hd, int Wd, int D, int antialias,
                              void* stream);
 
-/* ---- KoLeo (loss/koleo_loss.py:16-35), forward + backward: metric += w_metric * loss; dx += w_grad * dloss/dx ------ */
-int d3_koleo_fwd_bwd(const float* x /*[B,D]*/, float* xn_scratch /*[B,D]*/, float* nrm_scratch /*[B]*/,
-                     int* nn_scratch /*[B]*/, float* coef_scratch /*[B]*/, float* metric, float* dx /*[B,D] +=*/, int B,
-                     int D, float eps, float w_metric, float w_grad, void* stream);
-/* KoLeoLossDistributed (loss/koleo_loss.py:39-70): x holds the all-gathered rows of every rank; only the local rows
- * [row0, row0+nrows) contribute loss terms (mean over nrows), neighbours are searched over all B rows; dx gets the
- * gradient for all B rows (the caller reduce-scatters the other ranks' parts).                                     */
-int d3_koleo_fwd_bwd_rows(const float* x /*[B,D]*/, float* xn_scratch, float* nrm_scratch, int* nn_scratch,
-                          float* coef_scratch, float* metric, float* dx /*[B,D] +=*/, int B, int D, int row0, int nrows,
-                          float eps, float w_metric, float w_grad, void* stream);
+/* ---- KoLeo (loss/koleo_loss.py:16-35), forward + backward: metric += w_metric * loss; dx += w_grad * dloss/dx ------
+ * Only the rows [row0, row0+nrows) contribute loss terms (mean over nrows); neighbours are searched over all B rows.
+ * row0 = 0, nrows = B is KoLeoLoss.  A sub-range is KoLeoLossDistributed (loss/koleo_loss.py:39-70): x holds the
+ * all-gathered rows of every rank, and dx gets the gradient for all B rows (the caller reduce-scatters the other ranks'
+ * parts).                                                                                                          */
+int d3_koleo_fwd_bwd_rows(const float* x /*[B,D]*/, float* xn_scratch /*[B,D]*/, float* nrm_scratch /*[B]*/,
+                          int* nn_scratch /*[B]*/, float* coef_scratch /*[B]*/, float* metric, float* dx /*[B,D] +=*/,
+                          int B, int D, int row0, int nrows, float eps, float w_metric, float w_grad, void* stream);
 
 /* ---- optimiser (train/train.py:516-541 clip, :95-106,562-563 optax.adamw; train/ssl_meta_arch.py:650-652 EMA) -------
  * flat fp32 buffers; segs = array of {int64 start; float lr_mult, wd_mult; int is_last_layer, pad} sorted by start.  */

@@ -381,6 +381,52 @@ def _sinkhorn_ce_koleo_vs_oracle(K):
     assert abs(met.item() - lk.item()) < 1e-5 and rel(dx, xr.grad) < 1e-4
 
 
+def _off16(t):
+    """A copy of t stored one float (4 bytes) past a 16-byte boundary."""
+    e = 4 // t.element_size()
+    buf = torch.empty(t.numel() + e, dtype=t.dtype, device=t.device)
+    assert buf.data_ptr() % 16 == 0
+    out = buf[e:].view(t.shape)
+    out.copy_(t)
+    return out
+
+
+def test_sinkhorn_ce_misaligned_rows_match_aligned():
+    """Buffers one float past a 16-byte boundary take the scalar-load instances of absmax, colmax, the Sinkhorn sums
+    and the cross-entropy.  At K = 4096 they walk the same four-column groups as the 128-bit instances with the same
+    arithmetic, so they must agree with the aligned run."""
+    from dinov3_jax import ops
+    R, K, temp = 24, 4096, 0.05
+    L0 = torch.randn(R, K, device="cuda") * 0.3
+    S0 = torch.randn(R, K, device="cuda") * 0.5
+    t0 = torch.arange(R, dtype=torch.int32, device="cuda")
+    t1 = torch.where(t0 % 3 == 0, -1, (t0 + 5) % R).to(torch.int32)      # one or two teacher rows per student row
+    wm, wg = torch.rand(R, device="cuda"), torch.rand(R, device="cuda")
+    slot = (t0 % 2).to(torch.int32)
+    btot = torch.tensor([float(R)], device="cuda")
+
+    def run(place):
+        L, S = place(L0), place(S0)
+        gmx = place(torch.full((1,), float("-inf"), device="cuda")); ops.absmax(L, gmx)
+        mx = place(torch.full((K,), float("-inf"), device="cuda")); ops.colmax(L, mx)
+        s, a, av = place(torch.zeros(K, device="cuda")), None, place(torch.empty(R, device="cuda"))
+        for _ in range(3):
+            s.zero_(); ops.sinkhorn_colsum(L, mx, temp, a, s); ops.sinkhorn_rowsum(L, mx, temp, s, btot, av); a = av
+        Q = place(torch.empty(R, K, device="cuda")); ops.sinkhorn_probs(L, mx, temp, s, a, btot, Q)
+        metric = torch.zeros(2, device="cuda"); dS = place(torch.empty(R, K, device="cuda", dtype=torch.bfloat16))
+        ops.ce_fwd_bwd(S, 0.1, L, mx, temp, s, a, btot, t0, t1, wm, wg, slot, metric, dS)
+        # teacher rows that are already probabilities (s_t == NULL)
+        metric_p = torch.zeros(2, device="cuda"); dS_p = place(torch.empty(R, K, device="cuda", dtype=torch.bfloat16))
+        ops.ce_fwd_bwd(S, 0.1, Q, None, 1.0, None, None, None, t0, t1, wm, wg, slot, metric_p, dS_p)
+        return dict(absmax=gmx, colmax=mx, s=s, a=a, Q=Q, metric=metric, dS=dS, metric_p=metric_p, dS_p=dS_p)
+
+    ref = run(lambda t: t.clone())
+    mis = run(_off16)
+    assert ref["dS"].data_ptr() % 16 == 0 and mis["dS"].data_ptr() % 16 == 4
+    differ = {k: rel(mis[k], ref[k]) for k in ref if not torch.equal(ref[k], mis[k])}
+    assert not differ, differ
+
+
 def test_adamw_ema_clip_matches_optax_formula():
     from dinov3_jax import ops
     n = 4096 * 3 + 64
