@@ -85,61 +85,49 @@ __global__ void assemble_tokens_bwd_kernel(const float* __restrict__ dX, const u
 // ------------------------------------------------------------------------------------------------ LayerNorm
 // models/vision_transformer.py:40 (flax nn.LayerNorm, eps 1e-6, biased variance E[x^2]-E[x]^2, fp32 stats).
 // One warp per row; x fp32 [T, D]; y bf16 or fp32.
+// columns 4e..4e+3 of the row yr: (v - mean) rstd scale + bias
 template <typename OutT>
-__global__ void layernorm_fwd_kernel(const float* __restrict__ x, const float* __restrict__ scale,
-                                     const float* __restrict__ bias, OutT* __restrict__ y, float* __restrict__ mean_out,
-                                     float* __restrict__ rstd_out, int T, int D, float eps) {
-  const int warps = blockDim.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int D4 = D >> 2;
-  for (long row = (long)blockIdx.x * warps + (threadIdx.x >> 5); row < T; row += (long)gridDim.x * warps) {
-    const float4* xr = reinterpret_cast<const float4*>(x + row * (long)D);
-    float s = 0.f, s2 = 0.f;
-    for (int e = lane; e < D4; e += 32) {
-      float4 v = xr[e];
-      s += v.x + v.y + v.z + v.w;
-      s2 += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
-    }
-    s = warp_sum(s);
-    s2 = warp_sum(s2);
-    const float mean = s / D;
-    const float var = fmaxf(s2 / D - mean * mean, 0.f);
-    const float rstd = rsqrtf(var + eps);
-    if (lane == 0 && mean_out) { mean_out[row] = mean; rstd_out[row] = rstd; }
-    for (int e = lane; e < D4; e += 32) {
-      float4 v = xr[e];
-      float4 g = reinterpret_cast<const float4*>(scale)[e];
-      float4 b = reinterpret_cast<const float4*>(bias)[e];
-      float o0 = (v.x - mean) * rstd * g.x + b.x, o1 = (v.y - mean) * rstd * g.y + b.y;
-      float o2 = (v.z - mean) * rstd * g.z + b.z, o3 = (v.w - mean) * rstd * g.w + b.w;
-      if constexpr (sizeof(OutT) == 2) {
-        reinterpret_cast<uint2*>(y + row * (long)D)[e] = make_uint2(pack_bf16(o0, o1), pack_bf16(o2, o3));
-      } else {
-        reinterpret_cast<float4*>(y + row * (long)D)[e] = make_float4(o0, o1, o2, o3);
-      }
-    }
+__device__ __forceinline__ void ln_store4(OutT* yr, int e, const float4& v, const float* scale, const float* bias, float mean,
+                                          float rstd) {
+  const float4 g = reinterpret_cast<const float4*>(scale)[e];
+  const float4 b = reinterpret_cast<const float4*>(bias)[e];
+  const float o0 = (v.x - mean) * rstd * g.x + b.x, o1 = (v.y - mean) * rstd * g.y + b.y;
+  const float o2 = (v.z - mean) * rstd * g.z + b.z, o3 = (v.w - mean) * rstd * g.w + b.w;
+  if constexpr (sizeof(OutT) == 2) {
+    reinterpret_cast<uint2*>(yr)[e] = make_uint2(pack_bf16(o0, o1), pack_bf16(o2, o3));
+  } else {
+    reinterpret_cast<float4*>(yr)[e] = make_float4(o0, o1, o2, o3);
   }
 }
 
-
-// D = 128 * VPL known at compile time: the row stays in registers between the statistics and the normalisation (one
-// read of x), all VPL 16-byte loads of a lane are in flight together.
+// VPL > 0: D = 128 * VPL known at compile time; the row stays in registers between the statistics and the
+// normalisation (one read of x), all VPL 16-byte loads of a lane are in flight together.  VPL == 0: any D % 4 == 0
+// (`width` is read only then), x read twice.
 template <int VPL, typename OutT>
 __global__ void __launch_bounds__(256)
-layernorm_fwd_reg_kernel(const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ bias,
-                         OutT* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int T, float eps) {
-  constexpr int D = VPL * 128;
+layernorm_fwd_kernel(const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ bias,
+                     OutT* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int T, float eps,
+                     int width) {
+  const int D = VPL > 0 ? VPL * 128 : width;
   const int warps = blockDim.x >> 5, lane = threadIdx.x & 31;
   for (long row = (long)blockIdx.x * warps + (threadIdx.x >> 5); row < T; row += (long)gridDim.x * warps) {
     const float4* xr = reinterpret_cast<const float4*>(x + row * (long)D);
-    float4 v[VPL];
-#pragma unroll
-    for (int k = 0; k < VPL; ++k) v[k] = xr[k * 32 + lane];
+    float4 v[VPL > 0 ? VPL : 1];
     float s = 0.f, s2 = 0.f;
+    if constexpr (VPL > 0) {
 #pragma unroll
-    for (int k = 0; k < VPL; ++k) {
-      s += v[k].x + v[k].y + v[k].z + v[k].w;
-      s2 += v[k].x * v[k].x + v[k].y * v[k].y + v[k].z * v[k].z + v[k].w * v[k].w;
+      for (int k = 0; k < VPL; ++k) v[k] = xr[k * 32 + lane];
+#pragma unroll
+      for (int k = 0; k < VPL; ++k) {
+        s += v[k].x + v[k].y + v[k].z + v[k].w;
+        s2 += v[k].x * v[k].x + v[k].y * v[k].y + v[k].z * v[k].z + v[k].w * v[k].w;
+      }
+    } else {
+      for (int e = lane; e < D / 4; e += 32) {
+        const float4 w = xr[e];
+        s += w.x + w.y + w.z + w.w;
+        s2 += w.x * w.x + w.y * w.y + w.z * w.z + w.w * w.w;
+      }
     }
     s = warp_sum(s);
     s2 = warp_sum(s2);
@@ -147,20 +135,70 @@ layernorm_fwd_reg_kernel(const float* __restrict__ x, const float* __restrict__ 
     const float var = fmaxf(s2 * (1.f / D) - mean * mean, 0.f);
     const float rstd = rsqrtf(var + eps);
     if (lane == 0 && mean_out) { mean_out[row] = mean; rstd_out[row] = rstd; }
+    if constexpr (VPL > 0) {
 #pragma unroll
-    for (int k = 0; k < VPL; ++k) {
-      const int e = k * 32 + lane;
-      const float4 g = reinterpret_cast<const float4*>(scale)[e];
-      const float4 b = reinterpret_cast<const float4*>(bias)[e];
-      const float o0 = (v[k].x - mean) * rstd * g.x + b.x, o1 = (v[k].y - mean) * rstd * g.y + b.y;
-      const float o2 = (v[k].z - mean) * rstd * g.z + b.z, o3 = (v[k].w - mean) * rstd * g.w + b.w;
-      if constexpr (sizeof(OutT) == 2) {
-        reinterpret_cast<uint2*>(y + row * (long)D)[e] = make_uint2(pack_bf16(o0, o1), pack_bf16(o2, o3));
-      } else {
-        reinterpret_cast<float4*>(y + row * (long)D)[e] = make_float4(o0, o1, o2, o3);
-      }
+      for (int k = 0; k < VPL; ++k) ln_store4(y + row * (long)D, k * 32 + lane, v[k], scale, bias, mean, rstd);
+    } else {
+      for (int e = lane; e < D / 4; e += 32) ln_store4(y + row * (long)D, e, xr[e], scale, bias, mean, rstd);
     }
   }
+}
+
+// The per-element steps of the LayerNorm backward and of the LayerScale/GELU tail.  ln_bwd_ls_kernel and
+// ls_act_bwd_kernel call these helpers; ln_bwd_ring_kernel spells out the same expressions inline, because calling
+// them changes its register allocation and instruction order.
+
+// 4 consecutive elements as fp32 (p: 8-byte aligned bf16 or 16-byte aligned fp32)
+template <typename T>
+__device__ __forceinline__ void load4(const T* p, float (&v)[4]) {
+  if constexpr (sizeof(T) == 2) {
+    const uint2 u = *reinterpret_cast<const uint2*>(p);
+    const float2 v0 = unpack_bf16(u.x), v1 = unpack_bf16(u.y);
+    v[0] = v0.x; v[1] = v0.y; v[2] = v1.x; v[3] = v1.y;
+  } else {
+    const float4 f = *reinterpret_cast<const float4*>(p);
+    v[0] = f.x; v[1] = f.y; v[2] = f.z; v[3] = f.w;
+  }
+}
+
+// LayerNorm input gradient of 4 columns of a row with rstd rs, from gs = dy * scale and xh = x̂, with a = mean(gs),
+// b = mean(gs x̂):  o = rs (gs - a - x̂ b)  (+ the residual-stream gradient at `add`, 16-byte aligned, if `has_add`)
+__device__ __forceinline__ void ln_dx4(float (&o)[4], const float (&gs)[4], const float (&xh)[4], float a, float b,
+                                       float rs, bool has_add, const float* add) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) o[j] = rs * (gs[j] - a - xh[j] * b);
+  if (has_add) {
+    const float4 r4 = *reinterpret_cast<const float4*>(add);
+    o[0] += r4.x; o[1] += r4.y; o[2] += r4.z; o[3] += r4.w;
+  }
+}
+
+// LayerScale / activation backward of 4 columns of x_out = x_in + gamma * act(u), given o = dx_out: returns the packed
+// du = bf16(o gamma act'(u)), adds o act(u) to the dgamma partials `dg` and the rounded du, the values the weight-
+// gradient GEMM sees, to the dbias partials `db`.  act = tanh-GELU with the hardware tanh (the forward's GEMM epilogue
+// computed act(u) with it) if `gelu`, else identity.  u: 4 bf16 (8-byte aligned), read only if `has_u`; without it
+// act = identity and `dg` is untouched.
+__device__ __forceinline__ uint2 ls_tail4(const float (&o)[4], const float (&gm)[4], bool has_u,
+                                          const __nv_bfloat16* u, bool gelu, float (&dg)[4], float (&db)[4]) {
+  float d[4];
+  if (has_u) {
+    float uv[4];
+    load4(u, uv);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float act = gelu ? gelu_tanh_fast(uv[j]) : uv[j];
+      const float dact = gelu ? gelu_tanh_grad_fast(uv[j]) : 1.f;
+      d[j] = o[j] * gm[j] * dact;
+      dg[j] += o[j] * act;
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) d[j] = o[j] * gm[j];
+  }
+  const uint32_t p0 = pack_bf16(d[0], d[1]), p1 = pack_bf16(d[2], d[3]);
+  const float2 r0 = unpack_bf16(p0), r1 = unpack_bf16(p1);
+  db[0] += r0.x; db[1] += r0.y; db[2] += r1.x; db[3] += r1.y;
+  return make_uint2(p0, p1);
 }
 
 // LayerNorm backward fused with the LayerScale/GELU backward of the branch that *feeds on* its result.
@@ -207,17 +245,9 @@ ln_bwd_ls_kernel(const InT* __restrict__ dy, const float* __restrict__ x, const 
     for (int c = 0; c < NC; ++c) {
       const int col = (c * 128 + t) * 4;
       if (col < D) {
-        const float4 xv = *reinterpret_cast<const float4*>(x + row * (long)D + col);
-        float g[4];
-        if constexpr (sizeof(InT) == 2) {
-          const uint2 u = *reinterpret_cast<const uint2*>(dy + row * (long)D + col);
-          const float2 g0 = unpack_bf16(u.x), g1 = unpack_bf16(u.y);
-          g[0] = g0.x; g[1] = g0.y; g[2] = g1.x; g[3] = g1.y;
-        } else {
-          const float4 gv = *reinterpret_cast<const float4*>(dy + row * (long)D + col);
-          g[0] = gv.x; g[1] = gv.y; g[2] = gv.z; g[3] = gv.w;
-        }
-        const float xs[4] = {xv.x, xv.y, xv.z, xv.w};
+        float xs[4], g[4];
+        load4(x + row * (long)D + col, xs);
+        load4(dy + row * (long)D + col, g);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           xh[c][j] = (xs[j] - mu) * rs;
@@ -242,37 +272,13 @@ ln_bwd_ls_kernel(const InT* __restrict__ dy, const float* __restrict__ x, const 
     for (int c = 0; c < NC; ++c) {
       const int col = (c * 128 + t) * 4;
       if (col < D) {
+        const long off = row * (long)D + col;
         float o[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) o[j] = rs * (gs[c][j] - a - xh[c][j] * b);
-        if (dx_add) {
-          const float4 r4 = *reinterpret_cast<const float4*>(dx_add + row * (long)D + col);
-          o[0] += r4.x; o[1] += r4.y; o[2] += r4.z; o[3] += r4.w;
-        }
-        *reinterpret_cast<float4*>(dx + row * (long)D + col) = make_float4(o[0], o[1], o[2], o[3]);
-        if (tail) {
-          float d[4];
-          if (ls_u) {
-            const uint2 uu = *reinterpret_cast<const uint2*>(ls_u + row * (long)D + col);
-            const float2 u0 = unpack_bf16(uu.x), u1 = unpack_bf16(uu.y);
-            const float uv[4] = {u0.x, u0.y, u1.x, u1.y};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float act = ls_gelu ? gelu_tanh(uv[j]) : uv[j];
-              const float dact = ls_gelu ? gelu_tanh_grad(uv[j]) : 1.f;
-              d[j] = o[j] * gm[c][j] * dact;
-              tdg[c][j] += o[j] * act;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) d[j] = o[j] * gm[c][j];
-          }
-          const uint32_t p0 = pack_bf16(d[0], d[1]), p1 = pack_bf16(d[2], d[3]);
-          // dbias is the column sum of the values the wgrad GEMM sees (the bf16-rounded du)
-          const float2 r0 = unpack_bf16(p0), r1 = unpack_bf16(p1);
-          tdb[c][0] += r0.x; tdb[c][1] += r0.y; tdb[c][2] += r1.x; tdb[c][3] += r1.y;
-          *reinterpret_cast<uint2*>(ls_du + row * (long)D + col) = make_uint2(p0, p1);
-        }
+        ln_dx4(o, gs[c], xh[c], a, b, rs, dx_add != nullptr, dx_add ? dx_add + off : nullptr);
+        *reinterpret_cast<float4*>(dx + off) = make_float4(o[0], o[1], o[2], o[3]);
+        if (tail)
+          *reinterpret_cast<uint2*>(ls_du + off) =
+              ls_tail4(o, gm[c], ls_u != nullptr, ls_u ? ls_u + off : nullptr, ls_gelu, tdg[c], tdb[c]);
       }
     }
   }
@@ -324,6 +330,7 @@ ln_bwd_ls_kernel(const InT* __restrict__ dy, const float* __restrict__ x, const 
 // (dscale, dbias, ls_dgamma, ls_dbias) for their columns in registers until the end.
 constexpr int LNR_MAX_STAGES = 16;
 constexpr int LNR_CONSUMERS = 7;     // + 1 producer warp = 8 warps: two per SM sub-partition, so 255 registers stay available
+constexpr int LNR_SMEM_BUDGET = 200 * 1024;   // dynamic shared memory: barriers, scale | gamma, the ring
 
 __device__ __forceinline__ void bulk_load_1d(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -512,14 +519,12 @@ __global__ void ls_gamma_from_wgrad_kernel(const __nv_bfloat16* __restrict__ W, 
   const int slab = (K + gridDim.y - 1) / gridDim.y;
   const int r0 = blockIdx.y * slab, r1 = min(K, r0 + slab);
   float s0 = 0.f, s1 = 0.f;
-  if (col + 1 < N) {
+  if (col < N) {   // N is even
     for (int i = r0 + wy; i < r1; i += 8) {
       const float2 w = unpack_bf16(*reinterpret_cast<const uint32_t*>(W + (long)i * N + col));
       const float2 g = *reinterpret_cast<const float2*>(dW + (long)i * N + col);
       s0 += w.x * g.x; s1 += w.y * g.y;
     }
-  } else if (col < N) {
-    for (int i = r0 + wy; i < r1; i += 8) s0 += __bfloat162float(W[(long)i * N + col]) * dW[(long)i * N + col];
   }
   acc[wy][lane * 2] = s0; acc[wy][lane * 2 + 1] = s1;
   __syncthreads();
@@ -662,55 +667,37 @@ __global__ void l2norm_bwd_kernel(const __nv_bfloat16* __restrict__ g, const flo
 }
 
 // ------------------------------------------------------------------------------------------------ LayerScale / GELU bwd
-// block output x_out = x_in + gamma * act(u),  act = gelu_tanh (use_gelu) or identity   (layers/block.py:198-199)
-// given dX fp32 [T,D] and the bf16 stash u: du bf16 = dX*gamma*act'(u); dgamma += colsum(dX*act(u)); dbias += colsum(du)
+// block output x_out = x_in + gamma * act(u),  act = tanh-GELU (use_gelu) or identity   (layers/block.py:198-199)
+// given dX fp32 [T,D] and the bf16 stash u: du bf16 = dX*gamma*act'(u); dgamma += colsum(dX*act(u)); dbias += colsum(du).
+// The same ls_tail4 as the LayerNorm backward's fused tail, on 4 columns per thread; grid.y = row slabs.
 __global__ void ls_act_bwd_kernel(const float* __restrict__ dX, const __nv_bfloat16* __restrict__ u,
                                   const float* __restrict__ gamma, __nv_bfloat16* __restrict__ du,
                                   float* __restrict__ ws, int T, int D, int use_gelu) {
-  const int col = blockIdx.x * blockDim.x + threadIdx.x;
+  const int col = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   const long slab = ((long)T + gridDim.y - 1) / gridDim.y;
   const long r0 = blockIdx.y * slab, r1 = min((long)T, r0 + slab);
   if (col >= D) return;
-  const float gm = gamma[col];
-  float ag = 0.f, ab = 0.f;
+  float gm[4], ag[4] = {0.f, 0.f, 0.f, 0.f}, ab[4] = {0.f, 0.f, 0.f, 0.f};
+  load4(gamma + col, gm);
   for (long r = r0; r < r1; ++r) {
-    const float g = dX[r * D + col];
-    const float uu = __bfloat162float(u[r * D + col]);
-    const float act = use_gelu ? gelu_tanh(uu) : uu;
-    const float dact = use_gelu ? gelu_tanh_grad(uu) : 1.f;
-    const float d = g * gm * dact;
-    ag += g * act;
-    ab += d;
-    du[r * D + col] = __float2bfloat16(d);
+    float o[4];
+    load4(dX + r * D + col, o);
+    *reinterpret_cast<uint2*>(du + r * D + col) = ls_tail4(o, gm, true, u + r * D + col, use_gelu, ag, ab);
   }
-  ws[(long)blockIdx.y * 2 * D + col] = ag;        // row slab's share of [dgamma | dbias]
-  ws[(long)blockIdx.y * 2 * D + D + col] = ab;
-}
-
-// ws[slab][n] = sum over the row slab of x[t, n]   (bias gradients; the slabs are added in order).  x bf16 [T, N]
-__global__ void colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ ws, long T, int N, int ld) {
-  const int col = (blockIdx.x * blockDim.x + threadIdx.x) * 2;
-  const long slab = (T + gridDim.y - 1) / gridDim.y;
-  const long r0 = blockIdx.y * slab, r1 = min(T, r0 + slab);
-  if (col >= N) return;
-  float a0 = 0.f, a1 = 0.f;
-  if (col + 1 < N) {
-    for (long r = r0; r < r1; ++r) {
-      float2 v = unpack_bf16(*reinterpret_cast<const uint32_t*>(x + r * ld + col));
-      a0 += v.x; a1 += v.y;
-    }
-    ws[(long)blockIdx.y * N + col] = a0;
-    ws[(long)blockIdx.y * N + col + 1] = a1;
-  } else {
-    for (long r = r0; r < r1; ++r) a0 += __bfloat162float(x[r * ld + col]);
-    ws[(long)blockIdx.y * N + col] = a0;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    ws[(long)blockIdx.y * 2 * D + col + j] = ag[j];        // row slab's share of [dgamma | dbias]
+    ws[(long)blockIdx.y * 2 * D + D + col + j] = ab[j];
   }
 }
 
-
-// 128-bit version: a thread owns 8 adjacent columns; blockDim = (32, 8): 8 row phases per CTA, reduced in shared memory
+// ws[slab][n] = sum over the row slab of x[t, n]   (bias gradients; the slabs are added in order).  x bf16 [T, N], row
+// stride ld.  blockDim = (32, 8): a thread owns 8 adjacent columns and one of 8 row phases, reduced in shared memory.
+// VEC: 16-byte loads (N % 8 == 0, ld % 8 == 0, x 16-byte aligned); otherwise scalar loads of the columns < N, over the
+// same walk, so the sums do not depend on the layout.
+template <bool VEC>
 __global__ void __launch_bounds__(256)
-colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ ws, long T, int N, int ld) {
+colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ ws, long T, int N, int ld) {
   __shared__ float red[8][32][9];
   const int col = (blockIdx.x * 32 + threadIdx.x) * 8;
   const long slab = (T + gridDim.y - 1) / gridDim.y;
@@ -719,9 +706,15 @@ colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ 
   if (col < N) {
 #pragma unroll 4
     for (long r = r0 + threadIdx.y; r < r1; r += 8) {
-      const uint4 v = *reinterpret_cast<const uint4*>(x + r * ld + col);
-      const float2 f0 = unpack_bf16(v.x), f1 = unpack_bf16(v.y), f2 = unpack_bf16(v.z), f3 = unpack_bf16(v.w);
-      a[0] += f0.x; a[1] += f0.y; a[2] += f1.x; a[3] += f1.y; a[4] += f2.x; a[5] += f2.y; a[6] += f3.x; a[7] += f3.y;
+      if constexpr (VEC) {
+        const uint4 v = *reinterpret_cast<const uint4*>(x + r * ld + col);
+        const float2 f0 = unpack_bf16(v.x), f1 = unpack_bf16(v.y), f2 = unpack_bf16(v.z), f3 = unpack_bf16(v.w);
+        a[0] += f0.x; a[1] += f0.y; a[2] += f1.x; a[3] += f1.y; a[4] += f2.x; a[5] += f2.y; a[6] += f3.x; a[7] += f3.y;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (col + j < N) a[j] += __bfloat162float(x[r * ld + col + j]);
+      }
     }
   }
 #pragma unroll
@@ -914,82 +907,97 @@ __global__ void allreduce_peers_kernel(PeerCPtrs peers, int world, float* __rest
 using namespace d3;
 #define STREAM(s) reinterpret_cast<cudaStream_t>(s)
 
-// adds the CTAs' [dscale | dbias | ls_dgamma | ls_dbias] slabs of the LayerNorm backward kernels to the destinations
-// (nullptr: skipped; a quantity a kernel did not compute adds zeros) and releases the workspace
-static int combine_ln_slabs(float* ws, int slabs, int D, float* dscale, float* dbias, float* ls_dgamma, float* ls_dbias,
-                            cudaStream_t st) {
-  float* dst[4] = {dscale, dbias, ls_dgamma, ls_dbias};
-  int rc = D3_OK;
-  for (int q = 0; q < 4 && !rc; ++q) rc = slab_combine(ws + (long)q * D, slabs, 4LL * D, 1, D, dst[q], D, st);
+// d3_layernorm_bwd_ls's operands
+struct LnBwd {
+  const void* dy;
+  const float *x, *mean, *rstd, *scale, *dx_add;
+  float *dx, *dscale, *dbias;
+  int T, D;
+  const float* ls_gamma;
+  const void* ls_u;
+  int ls_gelu;
+  void* ls_du;
+  float *ls_dgamma, *ls_dbias;
+};
+
+// Launches a LayerNorm backward kernel instance (dy of type InT) over `grid` CTAs, each writing one
+// [dscale | dbias | ls_dgamma | ls_dbias] workspace slab, and adds the slabs to the outputs (nullptr: skipped; a
+// quantity the kernel did not compute adds zeros).  `arg` is the kernel's int after T: D (ln_bwd_ls_kernel) or the
+// ring's stage count (ln_bwd_ring_kernel).
+template <typename InT, typename Kernel>
+static int launch_ln_bwd(Kernel kernel, const LnBwd& a, int grid, int threads, size_t smem, int arg, cudaStream_t st) {
+  float* ws = slab_workspace((size_t)grid * 4 * a.D, st);
+  if (!ws) return D3_ERR_CUDA;
+  kernel<<<grid, threads, smem, st>>>((const InT*)a.dy, a.x, a.mean, a.rstd, a.scale, a.dx_add, a.dx, a.dscale, a.dbias, a.T,
+                                      arg, a.ls_gamma, (const __nv_bfloat16*)a.ls_u, a.ls_gelu, (__nv_bfloat16*)a.ls_du,
+                                      a.ls_dgamma, a.ls_dbias, ws);
+  cudaError_t e = cudaPeekAtLastError();
+  int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
+  if (!rc) count_launch();
+  float* dst[4] = {a.dscale, a.dbias, a.ls_dgamma, a.ls_dbias};
+  for (int q = 0; q < 4 && !rc; ++q) rc = slab_combine(ws + (long)q * a.D, grid, 4LL * a.D, 1, a.D, dst[q], a.D, st);
   slab_release(ws, st);
   return rc;
 }
 
-template <int NC>
-static int launch_ln_bwd_ls(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
-                             const float* scale, const float* dx_add, float* dx, float* dscale, float* dbias, int T, int D,
-                             const float* ls_gamma, const void* ls_u, int ls_gelu, void* ls_du, float* ls_dgamma,
-                             float* ls_dbias, cudaStream_t st) {
-  const size_t smem = (size_t)4 * D * sizeof(float);
-  static int occ_bf16 = 0, occ_f32 = 0;
-  if (!occ_bf16) {
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_bf16, ln_bwd_ls_kernel<NC, __nv_bfloat16>, 256, smem);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_f32, ln_bwd_ls_kernel<NC, float>, 256, smem);
-    occ_bf16 = max(occ_bf16, 1); occ_f32 = max(occ_f32, 1);
+template <int NC, typename InT>
+static int launch_ln_bwd_ls(const LnBwd& a, cudaStream_t st) {
+  const size_t smem = (size_t)4 * a.D * sizeof(float);
+  static int occ = 0;
+  if (!occ) {
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ln_bwd_ls_kernel<NC, InT>, 256, smem);
+    occ = max(occ, 1);
   }
-  const int blocks = min((T + 1) / 2, sm_count() * (dy_is_f32 ? occ_f32 : occ_bf16));
-  float* ws = slab_workspace((size_t)blocks * 4 * D, st);
-  if (!ws) return D3_ERR_CUDA;
-  if (dy_is_f32) {
-    ln_bwd_ls_kernel<NC, float><<<blocks, 256, smem, st>>>((const float*)dy, x, mean, rstd, scale, dx_add, dx, dscale, dbias,
-        T, D, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias, ws);
-  } else {
-    ln_bwd_ls_kernel<NC, __nv_bfloat16><<<blocks, 256, smem, st>>>((const __nv_bfloat16*)dy, x, mean, rstd, scale, dx_add, dx,
-        dscale, dbias, T, D, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias, ws);
-  }
-  cudaError_t e = cudaPeekAtLastError();
-  if (e != cudaSuccess) { slab_release(ws, st); return set_error(D3_ERR_CUDA, cudaGetErrorString(e)); }
-  count_launch();
-  return combine_ln_slabs(ws, blocks, D, dscale, dbias, ls_dgamma, ls_dbias, st);
+  const int blocks = min((a.T + 1) / 2, sm_count() * occ);
+  return launch_ln_bwd<InT>(ln_bwd_ls_kernel<NC, InT>, a, blocks, 256, smem, a.D, st);
 }
 
-
-// 1: shape not served by the ring kernel; otherwise D3_OK or an error
-template <int VPL>
-static int launch_ln_bwd_ring(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
-                               const float* scale, const float* dx_add, float* dx, float* dscale, float* dbias, int T,
-                               const float* ls_gamma, const void* ls_u, int ls_gelu, void* ls_du, float* ls_dgamma,
-                               float* ls_dbias, cudaStream_t st) {
+template <int VPL, typename InT>
+static int launch_ln_bwd_ring(const LnBwd& a, cudaStream_t st) {
   constexpr int D = VPL * 128;
-  const size_t stageB = (size_t)D * 4 + (dx_add ? D * 4 : 0) + (size_t)D * (dy_is_f32 ? 4 : 2) + ((ls_gamma && ls_u) ? D * 2 : 0);
-  const size_t fixed = 256 + 2 * D * sizeof(float);
-  const size_t budget = 200 * 1024;
-  int stages = (int)min((size_t)LNR_MAX_STAGES, (budget - fixed) / stageB);
+  constexpr size_t fixed = 256 + 2 * D * sizeof(float);
+  constexpr size_t max_stageB = (size_t)D * (4 + 4 + 4 + 2);      // x | dx_add | fp32 dy | u
+  static_assert((LNR_SMEM_BUDGET - fixed) / max_stageB >= LNR_CONSUMERS, "the ring holds a stage per consumer warp");
+  const size_t stageB = (size_t)D * 4 + (a.dx_add ? D * 4 : 0) + (size_t)D * sizeof(InT) + ((a.ls_gamma && a.ls_u) ? D * 2 : 0);
+  int stages = (int)min((size_t)LNR_MAX_STAGES, (LNR_SMEM_BUDGET - fixed) / stageB);
   // A multiple of the consumer count: then every use of a ring stage is handled by the same consumer warp, in order, so
   // a warp can never start waiting for use u of a stage before use u-1 has completed (an mbarrier parity wait that is
   // two phases ahead would return immediately).
   stages = stages / LNR_CONSUMERS * LNR_CONSUMERS;
-  if (stages < LNR_CONSUMERS) return 1;
   const size_t need = max(stageB * stages, (size_t)LNR_CONSUMERS * D * sizeof(float));    // ring doubles as the reduction slabs
-  const size_t smem = fixed + need;
-  static bool cfg_b = false, cfg_f = false;
-  const int grid = min(T, sm_count());
-  const int threads = 32 * (LNR_CONSUMERS + 1);
-  float* ws = slab_workspace((size_t)grid * 4 * D, st);
-  if (!ws) return D3_ERR_CUDA;
-  if (dy_is_f32) {
-    if (!cfg_f) { cudaFuncSetAttribute(ln_bwd_ring_kernel<VPL, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024); cfg_f = true; }
-    ln_bwd_ring_kernel<VPL, float><<<grid, threads, smem, st>>>((const float*)dy, x, mean, rstd, scale, dx_add, dx, dscale,
-        dbias, T, stages, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias, ws);
-  } else {
-    if (!cfg_b) { cudaFuncSetAttribute(ln_bwd_ring_kernel<VPL, __nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024); cfg_b = true; }
-    ln_bwd_ring_kernel<VPL, __nv_bfloat16><<<grid, threads, smem, st>>>((const __nv_bfloat16*)dy, x, mean, rstd, scale, dx_add,
-        dx, dscale, dbias, T, stages, ls_gamma, (const __nv_bfloat16*)ls_u, ls_gelu, (__nv_bfloat16*)ls_du, ls_dgamma, ls_dbias, ws);
+  static const cudaError_t cfg = cudaFuncSetAttribute(ln_bwd_ring_kernel<VPL, InT>,
+                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, LNR_SMEM_BUDGET);
+  (void)cfg;   // a failure shows at the launch
+  return launch_ln_bwd<InT>(ln_bwd_ring_kernel<VPL, InT>, a, min(a.T, sm_count()), 32 * (LNR_CONSUMERS + 1), fixed + need,
+                            stages, st);
+}
+
+// the ring for the widths it is instantiated for, ln_bwd_ls_kernel for every other
+template <typename InT>
+static int launch_ln_bwd(const LnBwd& a, cudaStream_t st) {
+  switch (a.D) {
+    case 128: return launch_ln_bwd_ring<1, InT>(a, st);
+    case 256: return launch_ln_bwd_ring<2, InT>(a, st);
+    case 384: return launch_ln_bwd_ring<3, InT>(a, st);
+    case 512: return launch_ln_bwd_ring<4, InT>(a, st);
+    case 768: return launch_ln_bwd_ring<6, InT>(a, st);
+    case 1024: return launch_ln_bwd_ring<8, InT>(a, st);
+    default: break;
   }
-  cudaError_t e = cudaPeekAtLastError();
-  if (e != cudaSuccess) { slab_release(ws, st); return set_error(D3_ERR_CUDA, cudaGetErrorString(e)); }
-  count_launch();
-  return combine_ln_slabs(ws, grid, D, dscale, dbias, ls_dgamma, ls_dbias, st);
+  const int nc = (a.D + 511) / 512;
+  return nc == 1 ? launch_ln_bwd_ls<1, InT>(a, st) : nc == 2 ? launch_ln_bwd_ls<2, InT>(a, st) : launch_ln_bwd_ls<3, InT>(a, st);
+}
+
+template <int VPL>
+static int launch_ln_fwd(const float* x, const float* scale, const float* bias, void* y, int y_is_f32, float* mean,
+                         float* rstd, int T, int D, float eps, cudaStream_t st) {
+  const int blocks = min((T + 7) / 8, sm_count() * 8);
+  if (y_is_f32)
+    layernorm_fwd_kernel<VPL, float><<<blocks, 256, 0, st>>>(x, scale, bias, (float*)y, mean, rstd, T, eps, D);
+  else
+    layernorm_fwd_kernel<VPL, __nv_bfloat16><<<blocks, 256, 0, st>>>(x, scale, bias, (__nv_bfloat16*)y, mean, rstd, T, eps, D);
+  D3_CHECK_LAUNCH();
+  return D3_OK;
 }
 
 
@@ -1040,28 +1048,19 @@ int d3_assemble_tokens_bwd(const float* dX, const unsigned char* masks, void* dT
 int d3_layernorm_fwd(const float* x, const float* scale, const float* bias, void* y, int y_is_f32, float* mean,
                      float* rstd, int T, int D, float eps, void* stream) {
   if (D % 4) return set_error(D3_ERR_ARG, "d3_layernorm_fwd: D % 4");
-  int blocks = min((T + 7) / 8, sm_count() * 8);
-  if (D % 128 == 0 && D / 128 <= 12 && ((uintptr_t)x | (uintptr_t)y | (uintptr_t)scale | (uintptr_t)bias) % 16 == 0) {
-#define LN_FWD_REG(V)                                                                                                   \
-  case V:                                                                                                               \
-    if (y_is_f32) layernorm_fwd_reg_kernel<V, float><<<blocks, 256, 0, STREAM(stream)>>>(x, scale, bias, (float*)y, mean, rstd, T, eps); \
-    else layernorm_fwd_reg_kernel<V, __nv_bfloat16><<<blocks, 256, 0, STREAM(stream)>>>(x, scale, bias, (__nv_bfloat16*)y, mean, rstd, T, eps); \
-    break;
-    bool done = true;
-    switch (D / 128) {
-      LN_FWD_REG(1) LN_FWD_REG(2) LN_FWD_REG(3) LN_FWD_REG(4) LN_FWD_REG(6) LN_FWD_REG(8) LN_FWD_REG(12)
-      default: done = false;
-    }
-#undef LN_FWD_REG
-    if (done) { D3_CHECK_LAUNCH(); return D3_OK; }
+  if (((uintptr_t)x | (uintptr_t)scale | (uintptr_t)bias) % 16 || (uintptr_t)y % (y_is_f32 ? 16 : 8))
+    return set_error(D3_ERR_ARG, "d3_layernorm_fwd: x, scale, bias and fp32 y must be 16-byte aligned, bf16 y 8-byte");
+  cudaStream_t st = STREAM(stream);
+  switch (D) {
+    case 128: return launch_ln_fwd<1>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
+    case 256: return launch_ln_fwd<2>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
+    case 384: return launch_ln_fwd<3>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
+    case 512: return launch_ln_fwd<4>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
+    case 768: return launch_ln_fwd<6>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
+    case 1024: return launch_ln_fwd<8>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
+    case 1536: return launch_ln_fwd<12>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
+    default: return launch_ln_fwd<0>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
   }
-  if (y_is_f32)
-    layernorm_fwd_kernel<float><<<blocks, 256, 0, STREAM(stream)>>>(x, scale, bias, (float*)y, mean, rstd, T, D, eps);
-  else
-    layernorm_fwd_kernel<__nv_bfloat16><<<blocks, 256, 0, STREAM(stream)>>>(x, scale, bias, (__nv_bfloat16*)y, mean,
-                                                                          rstd, T, D, eps);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
 }
 
 int d3_layernorm_bwd_ls(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,
@@ -1071,34 +1070,12 @@ int d3_layernorm_bwd_ls(const void* dy, int dy_is_f32, const float* x, const flo
   if (T <= 0) return D3_OK;
   if (D % 4 != 0 || D > 1536) return set_error(D3_ERR_ARG, "d3_layernorm_bwd_ls: D must be a multiple of 4 and <= 1536");
   if (ls_gamma && !ls_du) return set_error(D3_ERR_ARG, "d3_layernorm_bwd_ls: ls_du required with ls_gamma");
+  // 16-byte loads of every row operand and parameter vector, and the ring's bulk copies of whole rows
   if (((uintptr_t)dy | (uintptr_t)x | (uintptr_t)dx | (uintptr_t)scale | (uintptr_t)dx_add | (uintptr_t)ls_gamma |
-       (uintptr_t)ls_u | (uintptr_t)ls_du) % 8 != 0 || ((uintptr_t)x | (uintptr_t)dx | (uintptr_t)dx_add) % 16 != 0)
-    return set_error(D3_ERR_ARG, "d3_layernorm_bwd_ls: misaligned buffer");
-  cudaStream_t st = STREAM(stream);
-  const bool ring_ok = ((uintptr_t)dy | (uintptr_t)x | (uintptr_t)dx | (uintptr_t)dx_add | (uintptr_t)ls_u | (uintptr_t)ls_du) % 16 == 0;
-#define LN_RING_ARGS dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, ls_gamma, ls_u, ls_gelu, ls_du, ls_dgamma, ls_dbias, st
-  if (ring_ok && D % 128 == 0 && D / 128 <= 8) {
-    int rc = 1;
-    switch (D / 128) {
-      case 1: rc = launch_ln_bwd_ring<1>(LN_RING_ARGS); break;
-      case 2: rc = launch_ln_bwd_ring<2>(LN_RING_ARGS); break;
-      case 3: rc = launch_ln_bwd_ring<3>(LN_RING_ARGS); break;
-      case 4: rc = launch_ln_bwd_ring<4>(LN_RING_ARGS); break;
-      case 6: rc = launch_ln_bwd_ring<6>(LN_RING_ARGS); break;
-      case 8: rc = launch_ln_bwd_ring<8>(LN_RING_ARGS); break;
-      default: break;
-    }
-    if (rc != 1) return rc;
-  }
-#undef LN_RING_ARGS
-  const int nc = (D + 511) / 512;
-#define LN_LS_ARGS dy, dy_is_f32, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, D, ls_gamma, ls_u, ls_gelu, ls_du, ls_dgamma, ls_dbias, st
-  int rc;
-  if (nc == 1) rc = launch_ln_bwd_ls<1>(LN_LS_ARGS);
-  else if (nc == 2) rc = launch_ln_bwd_ls<2>(LN_LS_ARGS);
-  else rc = launch_ln_bwd_ls<3>(LN_LS_ARGS);
-#undef LN_LS_ARGS
-  return rc;
+       (uintptr_t)ls_u | (uintptr_t)ls_du) % 16 != 0)
+    return set_error(D3_ERR_ARG, "d3_layernorm_bwd_ls: misaligned buffer (all must be 16-byte aligned)");
+  const LnBwd a{dy, x, mean, rstd, scale, dx_add, dx, dscale, dbias, T, D, ls_gamma, ls_u, ls_gelu, ls_du, ls_dgamma, ls_dbias};
+  return dy_is_f32 ? launch_ln_bwd<float>(a, STREAM(stream)) : launch_ln_bwd<__nv_bfloat16>(a, STREAM(stream));
 }
 
 int d3_ls_gamma_from_wgrad(const void* W, const float* dW, const float* bias, const float* dbias, const float* gamma,
@@ -1219,7 +1196,9 @@ int d3_l2norm_bwd(const void* g, const float* u, const float* nrm, void* du, int
 
 int d3_ls_act_bwd(const float* dX, const void* u, const float* gamma, void* du, float* dgamma, float* dbias, int T,
                   int D, int use_gelu, void* stream) {
-  dim3 grid((D + 127) / 128, min(256, max(1, T / 64)));
+  if (D % 4 || ((uintptr_t)dX | (uintptr_t)gamma) % 16 || ((uintptr_t)u | (uintptr_t)du) % 8)
+    return set_error(D3_ERR_ARG, "d3_ls_act_bwd: D % 4, dX and gamma 16-byte aligned, u and du 8-byte aligned");
+  dim3 grid((D / 4 + 127) / 128, min(256, max(1, T / 64)));
   cudaStream_t st = STREAM(stream);
   float* ws = slab_workspace((size_t)grid.y * 2 * D, st);
   if (!ws) return D3_ERR_CUDA;
@@ -1237,21 +1216,15 @@ int d3_ls_act_bwd(const float* dX, const void* u, const float* gamma, void* du, 
 
 int d3_colsum_bf16(const void* x, float* out, long long T, int N, int ld, void* stream) {
   if (T <= 0) return D3_OK;
-  if (ld % 2) return set_error(D3_ERR_ARG, "d3_colsum_bf16: ld % 2");
   cudaStream_t st = STREAM(stream);
-  const bool vec = N % 8 == 0 && ld % 8 == 0 && (uintptr_t)x % 16 == 0 && T >= 64;
-  dim3 grid;
-  if (vec) {
-    grid.x = (N / 8 + 31) / 32;
-    grid.y = (int)max(1LL, min(T / 32, (long long)(sm_count() * 8 + grid.x - 1) / grid.x));
-  } else {
-    grid = dim3((N / 2 + 127) / 128 + ((N / 2) % 128 == 0 && N % 2 ? 1 : 0), (int)min(256LL, max(1LL, T / 64)));
-    if (((N + 1) / 2 + 127) / 128 > (int)grid.x) grid.x = ((N + 1) / 2 + 127) / 128;
-  }
+  dim3 grid((N + 255) / 256);
+  grid.y = (int)max(1LL, min(T / 32, (long long)(sm_count() * 8 + grid.x - 1) / grid.x));
   float* ws = slab_workspace((size_t)grid.y * N, st);
   if (!ws) return D3_ERR_CUDA;
-  if (vec) colsum_bf16_vec_kernel<<<grid, dim3(32, 8), 0, st>>>((const __nv_bfloat16*)x, ws, T, N, ld);
-  else colsum_bf16_kernel<<<grid, 128, 0, st>>>((const __nv_bfloat16*)x, ws, T, N, ld);
+  if (N % 8 == 0 && ld % 8 == 0 && (uintptr_t)x % 16 == 0)
+    colsum_bf16_kernel<true><<<grid, dim3(32, 8), 0, st>>>((const __nv_bfloat16*)x, ws, T, N, ld);
+  else
+    colsum_bf16_kernel<false><<<grid, dim3(32, 8), 0, st>>>((const __nv_bfloat16*)x, ws, T, N, ld);
   cudaError_t e = cudaPeekAtLastError();
   int rc = e == cudaSuccess ? D3_OK : set_error(D3_ERR_CUDA, cudaGetErrorString(e));
   if (!rc) { count_launch(); rc = slab_combine(ws, grid.y, N, 1, N, out, N, st); }

@@ -227,7 +227,8 @@ __device__ __forceinline__ float tanh_approx(float x) {
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// tanh-GELU with the hardware tanh (rel. error ~2^-11): used where the result is stored as bf16 anyway
+// tanh-GELU 0.5 u (1 + tanh(sqrt(2/pi) (u + 0.044715 u^3))) (flax.linen.gelu(approximate=True)) and its derivative,
+// with the hardware tanh (rel. error ~2^-11): used where the result is stored as bf16 anyway
 __device__ __forceinline__ float gelu_tanh_fast(float u) {
   const float t = tanh_approx(u * (0.7978845608028654f + 0.0356774081363001f * u * u));
   const float h = 0.5f * u;
@@ -242,19 +243,6 @@ __device__ __forceinline__ float gelu_tanh_grad_fast(float u) {
 
 
 // ------------------------------------------------------------------ math helpers
-__device__ __forceinline__ float gelu_tanh(float u) {
-  // 0.5 u (1 + tanh(sqrt(2/pi)(u + 0.044715 u^3)))  -- flax.linen.gelu(approximate=True)
-  float z = 0.7978845608028654f * (u + 0.044715f * u * u * u);
-  float t = 1.0f - 2.0f / (__expf(2.0f * z) + 1.0f);
-  return 0.5f * u * (1.0f + t);
-}
-__device__ __forceinline__ float gelu_tanh_grad(float u) {
-  float u2 = u * u;
-  float z = 0.7978845608028654f * (u + 0.044715f * u * u2);
-  float t = 1.0f - 2.0f / (__expf(2.0f * z) + 1.0f);
-  float dz = 0.7978845608028654f * (1.0f + 3.0f * 0.044715f * u2);
-  return 0.5f * (1.0f + t) + 0.5f * u * (1.0f - t * t) * dz;
-}
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&v);

@@ -92,7 +92,9 @@ int d3_assemble_tokens_bwd(const float* dX, const unsigned char* masks, void* dT
                            float* dcls /*[D] +=*/, float* dstorage /*[R,D] += or NULL*/, float* dmask_token /*[D] +=*/,
                            int n, int P, int R, int D, void* stream);
 
-/* ---- LayerNorm (models/vision_transformer.py:40: eps 1e-6, biased variance E[x^2]-E[x]^2, fp32 statistics) ------- */
+/* ---- LayerNorm (models/vision_transformer.py:40: eps 1e-6, biased variance E[x^2]-E[x]^2, fp32 statistics) -------
+ * D % 4 == 0.  Alignment (else D3_ERR_ARG): d3_layernorm_fwd: x, scale, bias and an fp32 y 16 bytes, a bf16 y 8 bytes;
+ * d3_layernorm_bwd_ls: every row operand and parameter vector (dy, x, scale, dx_add, dx, ls_gamma, ls_u, ls_du) 16 bytes. */
 int d3_layernorm_fwd(const float* x /*[T,D]*/, const float* scale, const float* bias, void* y, int y_is_f32,
                      float* mean /*[T] or NULL*/, float* rstd, int T, int D, float eps, void* stream);
 /* LayerNorm backward: dx = LN'(dy) (+ dx_add), dscale += colsum(dy * xhat), dbias += colsum(dy); with ls_gamma == NULL
@@ -163,7 +165,9 @@ int d3_l2norm_bwd(const void* g_bf16, const float* u, const float* nrm, void* du
 
 /* ---- backward helpers ----------------------------------------------------------------------------------------------
  * d3_ls_act_bwd: x_out = x_in + gamma * act(u) (layers/block.py:198-199): du = dX*gamma*act'(u) (bf16),
- * dgamma += colsum(dX*act(u)), dbias += colsum(du).  d3_colsum_bf16: bias gradients.                                 */
+ * dgamma += colsum(dX*act(u)), dbias += colsum(bf16 du), the same arithmetic as the tail of d3_layernorm_bwd_ls;
+ * D % 4 == 0, dX and gamma 16-byte, u and du 8-byte aligned.  d3_colsum_bf16: bias gradients, any N, ld and
+ * alignment, the same sums whatever the layout.                                                                      */
 int d3_ls_act_bwd(const float* dX /*[T,D]*/, const void* u_bf16, const float* gamma, void* du_bf16, float* dgamma,
                   float* dbias, int T, int D, int use_gelu, void* stream);
 int d3_colsum_bf16(const void* x_bf16 /*[T,N], row stride ld*/, float* out /*[N] +=*/, long long T, int N, int ld,

@@ -341,9 +341,10 @@ def test_step_with_mask_k_bias():
 
 def test_activation_remat_equals_stashing():
     """train.checkpointing (ssl_default_config.yaml:88): recomputing each student block in the backward gives the same
-    loss and, to the bf16 level, the same gradients as keeping its activations: the recomputing path takes the
-    LayerScale / GELU backward of the MLP branch from the stand-alone kernel (exact tanh) instead of the tail fused into
-    the LayerNorm backward (hardware tanh.approx, 2^-11), everything else is identical."""
+    loss and the same gradients as keeping its activations.  The recomputing path takes the LayerScale / GELU backward
+    of the MLP branch from the stand-alone kernel instead of the tail fused into the LayerNorm backward; both compute du
+    with the same arithmetic, so every gradient is bit-identical except the two column sums that kernel forms in
+    another order (ls2/gamma and the fc2 bias), which agree to 1e-5."""
     from dinov3_jax.engine import Engine, from_oracle_cfg
     from oracle import tiny_cfg
     from oracle.batch import synthetic_batch
@@ -363,10 +364,13 @@ def test_activation_remat_equals_stashing():
         eng.optimizer_step(HYPER["lr"], HYPER["wd"], HYPER["last_layer_lr"], HYPER["momentum"])
         out.append((eng.read_metrics()["total_loss"], g))
     (la, ga), (lb, gb) = out
-    assert abs(la - lb) <= 1e-6 * abs(la)
-    num = sum(float(((ga[k] - gb[k]) ** 2).sum()) for k in ga)
-    den = sum(float((ga[k] ** 2).sum()) for k in ga)
-    assert (num / den) ** 0.5 < 5e-3
+    assert la == lb
+    assert ga.keys() == gb.keys()
+    for k in ga:
+        if k.endswith("/ls2/gamma") or k.endswith("/mlp/Dense_1/bias"):
+            assert float((ga[k] - gb[k]).norm() / ga[k].norm()) < 1e-5, k
+        else:
+            assert torch.equal(ga[k], gb[k]), k
 
 
 # --------------------------------------------------------------------------------------------------- Gram anchoring (8f.2)

@@ -45,6 +45,13 @@ cs = torch.zeros(3 * D, device=dev); q = torch.randn(T, 3 * D, device=dev).to(bf
 timeit("colsum_bf16 [T,3D]", lambda: ops.colsum_bf16(q, cs), TD * 3 * 2)
 h = torch.randn(T, 4 * D, device=dev).to(bf); cs4 = torch.zeros(4 * D, device=dev)
 timeit("colsum_bf16 [T,4D]", lambda: ops.colsum_bf16(h, cs4), TD * 4 * 2)
+# layouts the 16-byte loads cannot take (scalar loads): a width not a multiple of 8, rows 2 elements past a 16-byte
+# boundary, and a short matrix
+r = torch.randn(T, 1004, device=dev).to(bf); csr = torch.zeros(1004, device=dev)
+timeit("colsum_bf16 [T,1004]", lambda: ops.colsum_bf16(r, csr), T * 1004 * 2)
+qs = torch.empty(TD * 3 + 8, device=dev, dtype=bf)[2:2 + TD * 3].view(T, 3 * D); qs.copy_(q)
+timeit("colsum_bf16 [T,3D] unaligned", lambda: ops.colsum_bf16(qs, cs), TD * 3 * 2)
+timeit("colsum_bf16 [37,3D]", lambda: ops.colsum_bf16(q[:37], cs), 37 * D * 3 * 2)
 
 # ---- head / loss kernels at the iBOT shape (M = 3771 masked tokens, K = 65536 prototypes)
 if len(sys.argv) <= 2:
