@@ -12,6 +12,8 @@
 #include "ptx.cuh"
 #include "d3_internal.h"
 
+#include <type_traits>
+
 namespace d3 {
 
 // one record per output crop (host-filled, 64 bytes)
@@ -37,7 +39,11 @@ __device__ __forceinline__ float cubic_aa(float x) {           // Keys cubic, a 
 // Same definition as torch's _upsample_bicubic2d_aa (align_corners = False): per axis, scale = in/out,
 // support = 2 * max(scale, 1), taps j in [floor(center - support + 0.5), ...), weight cubic((j + 0.5 - center) / max(scale, 1)),
 // normalised; taps are clipped to the crop box.
-__global__ void aug_resized_crop_kernel(const uint8_t* __restrict__ src, int H, int W, const AugCrop* __restrict__ crops,
+// T = uint8_t reads a decoded image (/255); T = float reads an fp32 [0,1] image (the colour-jittered source of
+// share_color_jitter, or a base crop resized to the global / gram size).  CLAMP = false is the Resize of a normalised
+// tensor, which torchvision does not clamp.
+template <typename T, bool CLAMP>
+__global__ void aug_resized_crop_kernel(const T* __restrict__ src, int H, int W, const AugCrop* __restrict__ crops,
                                         float* __restrict__ out, int S) {
   const int n = blockIdx.z;
   const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y * blockDim.y + threadIdx.y;
@@ -53,11 +59,11 @@ __global__ void aug_resized_crop_kernel(const uint8_t* __restrict__ src, int H, 
   float wxs = 0.f, wys = 0.f;
   for (int x = xmin; x < xmax; ++x) wxs += cubic_aa((x - cx + 0.5f) * isx);
   for (int y = ymin; y < ymax; ++y) wys += cubic_aa((y - cy + 0.5f) * isy);
-  const uint8_t* base = src + ((size_t)c.img * H + c.y0) * W * 3 + (size_t)c.x0 * 3;
+  const T* base = src + ((size_t)c.img * H + c.y0) * W * 3 + (size_t)c.x0 * 3;
   float r = 0.f, g = 0.f, b = 0.f;
   for (int y = ymin; y < ymax; ++y) {
     const float wy = cubic_aa((y - cy + 0.5f) * isy);
-    const uint8_t* row = base + (size_t)y * W * 3;
+    const T* row = base + (size_t)y * W * 3;
     float rr = 0.f, gg = 0.f, bb = 0.f;
     for (int x = xmin; x < xmax; ++x) {
       const float wx = cubic_aa((x - cx + 0.5f) * isx);
@@ -65,10 +71,14 @@ __global__ void aug_resized_crop_kernel(const uint8_t* __restrict__ src, int H, 
     }
     r += wy * rr; g += wy * gg; b += wy * bb;
   }
-  const float norm = 1.f / (255.f * wxs * wys);
+  const float norm = 1.f / ((std::is_same_v<T, uint8_t> ? 255.f : 1.f) * wxs * wys);
   float* o = out + (((size_t)n * S + oy) * S + ox) * 3;
-  // bicubic overshoots are clamped like a uint8 image would (PIL result is uint8)
-  o[0] = fminf(fmaxf(r * norm, 0.f), 1.f); o[1] = fminf(fmaxf(g * norm, 0.f), 1.f); o[2] = fminf(fmaxf(b * norm, 0.f), 1.f);
+  if constexpr (CLAMP) {
+    // bicubic overshoots are clamped like a uint8 image would (PIL result is uint8)
+    o[0] = fminf(fmaxf(r * norm, 0.f), 1.f); o[1] = fminf(fmaxf(g * norm, 0.f), 1.f); o[2] = fminf(fmaxf(b * norm, 0.f), 1.f);
+  } else {
+    o[0] = r * norm; o[1] = g * norm; o[2] = b * norm;
+  }
 }
 
 // torchvision _rgb_to_grayscale_image weights
@@ -116,11 +126,13 @@ __device__ __forceinline__ void jitter_op(int op, const AugCrop& c, float mean_g
 // Pass A: the jitter ops that come BEFORE contrast in this crop's order, plus the sum of the gray values of the result
 // (contrast blends with the mean gray of the image it is applied to).  Pass B: contrast and what follows, then
 // RandomGrayscale.  A crop without jitter / without a pending contrast simply passes through pass A untouched.
+// SQUARE: x holds S x S crops; otherwise S is the pixel count of each image (whole H x W sources).
+template <bool SQUARE>
 __global__ void aug_color_a_kernel(float* __restrict__ x, const AugCrop* __restrict__ crops, float* __restrict__ gray_sum,
                                    int S) {
   const int n = blockIdx.y;
   const AugCrop c = crops[n];
-  const int npix = S * S;
+  const int npix = SQUARE ? S * S : S;
   float local = 0.f;
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
     float* px = x + ((size_t)n * npix + p) * 3;
@@ -134,11 +146,12 @@ __global__ void aug_color_a_kernel(float* __restrict__ x, const AugCrop* __restr
   for (int o = 16; o > 0; o >>= 1) local += __shfl_xor_sync(0xffffffffu, local, o);
   if ((threadIdx.x & 31) == 0) atomicAdd(&gray_sum[n], local);
 }
+template <bool SQUARE>
 __global__ void aug_color_b_kernel(float* __restrict__ x, const AugCrop* __restrict__ crops,
                                    const float* __restrict__ gray_sum, int S) {
   const int n = blockIdx.y;
   const AugCrop c = crops[n];
-  const int npix = S * S;
+  const int npix = SQUARE ? S * S : S;
   const float mean_gray = gray_sum[n] / npix;
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
     float* px = x + ((size_t)n * npix + p) * 3;
@@ -152,6 +165,16 @@ __global__ void aug_color_b_kernel(float* __restrict__ x, const AugCrop* __restr
     px[0] = r; px[1] = g; px[2] = b;
   }
 }
+
+// torchvision _get_gaussian_kernel1d(9, sigma) taps, unnormalised; returns their sum
+__device__ __forceinline__ float blur_taps(float sigma, float (&w)[9]) {
+  float ws = 0.f;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) { const float d = (float)(k - 4) / sigma; w[k] = __expf(-0.5f * d * d); ws += w[k]; }
+  return ws;
+}
+// reflect padding (no edge repeat) of index t into [0, S), S >= 5
+__device__ __forceinline__ int reflect(int t, int S) { return t < 0 ? -t : (t >= S ? 2 * S - 2 - t : t); }
 
 // separable 9-tap Gaussian (torchvision gaussian_blur: kernel_size 9, reflect padding), one axis per launch
 __global__ void aug_blur_kernel(const float* __restrict__ x, float* __restrict__ y, const AugBlur* __restrict__ blur, int S,
@@ -167,20 +190,22 @@ __global__ void aug_blur_kernel(const float* __restrict__ x, float* __restrict__
     yo[0] = p[0]; yo[1] = p[1]; yo[2] = p[2];
     return;
   }
-  float w[9], ws = 0.f;
-#pragma unroll
-  for (int k = 0; k < 9; ++k) { const float d = (float)(k - 4) / sigma; w[k] = __expf(-0.5f * d * d); ws += w[k]; }
+  float w[9];
+  const float ws = blur_taps(sigma, w);
   float r = 0.f, g = 0.f, b = 0.f;
 #pragma unroll
   for (int k = 0; k < 9; ++k) {
     int t = (vertical ? oy : ox) + k - 4;
-    t = t < 0 ? -t : (t >= S ? 2 * S - 2 - t : t);           // reflect (no edge repeat), S >= 5
+    t = t < 0 ? -t : (t >= S ? 2 * S - 2 - t : t);           // reflect(); written out, the kernel keeps its schedule
     const float* p = xi + (vertical ? ((size_t)t * S + ox) : ((size_t)oy * S + t)) * 3;
     r += w[k] * p[0]; g += w[k] * p[1]; b += w[k] * p[2];
   }
   const float inv = 1.f / ws;
   yo[0] = r * inv; yo[1] = g * inv; yo[2] = b * inv;
 }
+
+// RandomSolarize(threshold 128): pixels >= 128/255 inverted
+__device__ __forceinline__ float solarize(float v) { return v >= 128.f / 255.f ? 1.f - v : v; }
 
 // RandomSolarize (pixels >= 128/255 inverted), Normalize(mean, std), cast to bf16 NHWC
 __global__ void aug_finish_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out,
@@ -189,14 +214,98 @@ __global__ void aug_finish_kernel(const float* __restrict__ x, __nv_bfloat16* __
   const int n = blockIdx.y;
   const int sol = crops[n].solarize;
   const int npix = S * S;
-  const float thr = 128.f / 255.f;
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
     const float* px = x + ((size_t)n * npix + p) * 3;
     float r = px[0], g = px[1], b = px[2];
-    if (sol) { r = r >= thr ? 1.f - r : r; g = g >= thr ? 1.f - g : g; b = b >= thr ? 1.f - b : b; }
+    if (sol) { r = solarize(r); g = solarize(g); b = solarize(b); }
     __nv_bfloat16* o = out + ((size_t)n * npix + p) * 3;
     o[0] = __float2bfloat16((r - m0) * is0); o[1] = __float2bfloat16((g - m1) * is1); o[2] = __float2bfloat16((b - m2) * is2);
   }
+}
+
+// RandomSolarize in place, for crops that are resized after their distortions (gram crops with distortions: the
+// reference normalises, then resizes; Resize commutes with Normalize but not with Solarize)
+__global__ void aug_solarize_kernel(float* __restrict__ x, const AugCrop* __restrict__ crops, int S) {
+  const int n = blockIdx.y;
+  if (!crops[n].solarize) return;
+  const int npix = S * S;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
+    float* px = x + ((size_t)n * npix + p) * 3;
+    px[0] = solarize(px[0]); px[1] = solarize(px[1]); px[2] = solarize(px[2]);
+  }
+}
+
+// uint8 [n, npix, 3] -> fp32 [0, 1] copy (share_color_jitter transforms the whole source image before any crop)
+__global__ void aug_u8_to_f32_kernel(const uint8_t* __restrict__ src, float* __restrict__ x, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    x[i] = src[i] * (1.f / 255.f);
+}
+
+// Local crops cut from a global base crop (local_crops_subset_of_global_crops): the reference jitters and blurs the
+// WHOLE M x M base, then slices an L x L window at (y0, x0).  Per window record (img = base index):
+//  gray   pass A of aug_color over the whole base without writing it: the contrast mean of the whole image;
+//  gather the window plus a 4-pixel halo, reflected at the base's border, through the full jitter and grayscale;
+//  blur   valid-mode 9-tap Gaussian over the halo (what the whole-image blur gives inside the window).
+__global__ void aug_window_gray_kernel(const float* __restrict__ base, int M, const AugCrop* __restrict__ crops,
+                                       float* __restrict__ gray_sum) {
+  const int n = blockIdx.y;
+  const AugCrop c = crops[n];
+  if (c.order[0] < 0) return;                                // no jitter: the mean is never read
+  const int npix = M * M;
+  const float* xi = base + (size_t)c.img * npix * 3;
+  float local = 0.f;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
+    const float* px = xi + (size_t)p * 3;
+    float r = px[0], g = px[1], b = px[2];
+    for (int k = 0; k < 4 && c.order[k] != 1; ++k) jitter_op(c.order[k], c, 0.f, r, g, b);
+    local += gray_of(r, g, b);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) local += __shfl_xor_sync(0xffffffffu, local, o);
+  if ((threadIdx.x & 31) == 0) atomicAdd(&gray_sum[n], local);
+}
+__global__ void aug_window_gather_kernel(const float* __restrict__ base, int M, const AugCrop* __restrict__ crops,
+                                         const float* __restrict__ gray_sum, float* __restrict__ win, int L) {
+  const int n = blockIdx.z, E = L + 8;
+  const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y * blockDim.y + threadIdx.y;
+  if (ox >= E || oy >= E) return;
+  const AugCrop c = crops[n];
+  const int sx = reflect(c.x0 - 4 + ox, M), sy = reflect(c.y0 - 4 + oy, M);
+  const float* px = base + (((size_t)c.img * M + sy) * M + sx) * 3;
+  float r = px[0], g = px[1], b = px[2];
+  if (c.order[0] >= 0) {
+    const float mean_gray = gray_sum[n] / (M * M);
+    for (int k = 0; k < 4; ++k) jitter_op(c.order[k], c, mean_gray, r, g, b);
+  }
+  if (c.gray) { const float y = gray_of(r, g, b); r = g = b = y; }
+  float* o = win + (((size_t)n * E + oy) * E + ox) * 3;
+  o[0] = r; o[1] = g; o[2] = b;
+}
+// x [n, Hin, Win, 3] -> y [n, Hin, Win - 8, 3] (horizontal) or [n, Hin - 8, Win, 3] (vertical)
+__global__ void aug_blur_valid_kernel(const float* __restrict__ x, float* __restrict__ y, const AugBlur* __restrict__ blur,
+                                      int Hin, int Win, int vertical) {
+  const int n = blockIdx.z;
+  const int Ho = vertical ? Hin - 8 : Hin, Wo = vertical ? Win : Win - 8;
+  const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y * blockDim.y + threadIdx.y;
+  if (ox >= Wo || oy >= Ho) return;
+  const float sigma = blur[n].sigma;
+  const float* xi = x + (size_t)n * Hin * Win * 3;
+  float* yo = y + (((size_t)n * Ho + oy) * Wo + ox) * 3;
+  if (sigma <= 0.f) {
+    const float* p = xi + (vertical ? ((size_t)(oy + 4) * Win + ox) : ((size_t)oy * Win + ox + 4)) * 3;
+    yo[0] = p[0]; yo[1] = p[1]; yo[2] = p[2];
+    return;
+  }
+  float w[9];
+  const float ws = blur_taps(sigma, w);
+  float r = 0.f, g = 0.f, b = 0.f;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    const float* p = xi + (vertical ? ((size_t)(oy + k) * Win + ox) : ((size_t)oy * Win + ox + k)) * 3;
+    r += w[k] * p[0]; g += w[k] * p[1]; b += w[k] * p[2];
+  }
+  const float inv = 1.f / ws;
+  yo[0] = r * inv; yo[1] = g * inv; yo[2] = b * inv;
 }
 
 }  // namespace d3
@@ -211,7 +320,7 @@ int d3_aug_resized_crop(const void* src_u8, int n_img, int H, int W, const void*
   if (n_crops <= 0) return D3_OK;
   if (S < 5 || H <= 0 || W <= 0 || n_img <= 0) return set_error(D3_ERR_ARG, "d3_aug_resized_crop: bad geometry");
   dim3 block(32, 8), grid((S + 31) / 32, (S + 7) / 8, n_crops);
-  aug_resized_crop_kernel<<<grid, block, 0, STREAM(stream)>>>((const uint8_t*)src_u8, H, W, (const AugCrop*)crops, out, S);
+  aug_resized_crop_kernel<uint8_t, true><<<grid, block, 0, STREAM(stream)>>>((const uint8_t*)src_u8, H, W, (const AugCrop*)crops, out, S);
   D3_CHECK_LAUNCH();
   return D3_OK;
 }
@@ -219,8 +328,8 @@ int d3_aug_resized_crop(const void* src_u8, int n_img, int H, int W, const void*
 int d3_aug_color(float* x, const void* crops, int n_crops, int S, float* gray_sum /* [n_crops] zeroed */, void* stream) {
   if (n_crops <= 0) return D3_OK;
   dim3 grid(min((S * S + 255) / 256, 64), n_crops);
-  aug_color_a_kernel<<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)crops, gray_sum, S);
-  aug_color_b_kernel<<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)crops, gray_sum, S);
+  aug_color_a_kernel<true><<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)crops, gray_sum, S);
+  aug_color_b_kernel<true><<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)crops, gray_sum, S);
   D3_CHECK_LAUNCH();
   count_launch(1);
   return D3_OK;
@@ -244,6 +353,61 @@ int d3_aug_finish(const float* x, void* out_bf16, const void* crops, int n_crops
   aug_finish_kernel<<<grid, 256, 0, STREAM(stream)>>>(x, (__nv_bfloat16*)out_bf16, (const AugCrop*)crops, S, mean3[0], mean3[1],
                                                      mean3[2], 1.f / std3[0], 1.f / std3[1], 1.f / std3[2]);
   D3_CHECK_LAUNCH();
+  return D3_OK;
+}
+
+int d3_aug_resized_crop_f32(const float* src, int n_img, int H, int W, const void* crops, int n_crops, float* out, int S,
+                            int clamp, void* stream) {
+  if (n_crops <= 0) return D3_OK;
+  if (S < 5 || H <= 0 || W <= 0 || n_img <= 0) return set_error(D3_ERR_ARG, "d3_aug_resized_crop_f32: bad geometry");
+  dim3 block(32, 8), grid((S + 31) / 32, (S + 7) / 8, n_crops);
+  if (clamp)
+    aug_resized_crop_kernel<float, true><<<grid, block, 0, STREAM(stream)>>>(src, H, W, (const AugCrop*)crops, out, S);
+  else
+    aug_resized_crop_kernel<float, false><<<grid, block, 0, STREAM(stream)>>>(src, H, W, (const AugCrop*)crops, out, S);
+  D3_CHECK_LAUNCH();
+  return D3_OK;
+}
+
+int d3_aug_color_images(const void* src_u8, int n_img, int H, int W, const void* recs, float* x, float* gray_sum,
+                        void* stream) {
+  if (n_img <= 0) return D3_OK;
+  if (H <= 0 || W <= 0) return set_error(D3_ERR_ARG, "d3_aug_color_images: bad geometry");
+  const long long n = (long long)n_img * H * W * 3;
+  aug_u8_to_f32_kernel<<<(int)std::min<long long>((n + 255) / 256, 4096), 256, 0, STREAM(stream)>>>(
+      (const uint8_t*)src_u8, x, n);
+  dim3 grid(min((H * W + 255) / 256, 64), n_img);
+  aug_color_a_kernel<false><<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)recs, gray_sum, H * W);
+  aug_color_b_kernel<false><<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)recs, gray_sum, H * W);
+  D3_CHECK_LAUNCH();
+  count_launch(2);
+  return D3_OK;
+}
+
+int d3_aug_solarize(float* x, const void* crops, int n_crops, int S, void* stream) {
+  if (n_crops <= 0) return D3_OK;
+  dim3 grid(min((S * S + 255) / 256, 64), n_crops);
+  aug_solarize_kernel<<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)crops, S);
+  D3_CHECK_LAUNCH();
+  return D3_OK;
+}
+
+int d3_aug_local_windows(const float* base, int n_base, int M, const void* crops, const void* blur, int n_crops, int L,
+                         float* win, float* tmp, float* y, float* gray_sum, void* stream) {
+  if (n_crops <= 0) return D3_OK;
+  if (M < 5 || L < 1 || L > M || n_base <= 0) return set_error(D3_ERR_ARG, "d3_aug_local_windows: bad geometry");
+  const int E = L + 8;
+  aug_window_gray_kernel<<<dim3(min((M * M + 255) / 256, 64), n_crops), 256, 0, STREAM(stream)>>>(
+      base, M, (const AugCrop*)crops, gray_sum);
+  dim3 block(32, 8);
+  aug_window_gather_kernel<<<dim3((E + 31) / 32, (E + 7) / 8, n_crops), block, 0, STREAM(stream)>>>(
+      base, M, (const AugCrop*)crops, gray_sum, win, L);
+  aug_blur_valid_kernel<<<dim3((L + 31) / 32, (E + 7) / 8, n_crops), block, 0, STREAM(stream)>>>(
+      win, tmp, (const AugBlur*)blur, E, E, 0);
+  aug_blur_valid_kernel<<<dim3((L + 31) / 32, (L + 7) / 8, n_crops), block, 0, STREAM(stream)>>>(
+      tmp, y, (const AugBlur*)blur, E, L, 1);
+  D3_CHECK_LAUNCH();
+  count_launch(3);
   return D3_OK;
 }
 

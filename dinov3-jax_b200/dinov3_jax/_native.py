@@ -78,6 +78,10 @@ SIGNATURES = {
     "d3_aug_color": [P, P, I, I, P, P],
     "d3_aug_blur": [P, P, P, P, I, I, P],
     "d3_aug_finish": [P, P, P, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P],
+    "d3_aug_resized_crop_f32": [P, I, I, I, P, I, P, I, I, P],
+    "d3_aug_color_images": [P, I, I, I, P, P, P, P],
+    "d3_aug_solarize": [P, P, I, I, P],
+    "d3_aug_local_windows": [P, I, I, P, P, I, I, P, P, P, P, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

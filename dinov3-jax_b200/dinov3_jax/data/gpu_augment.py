@@ -16,6 +16,19 @@ on the host (a few dozen scalars per image, numpy), following torchvision's samp
   RandomSolarize(threshold 128)  p = 0.2, second global crop only
   ToTensor + Normalize(mean, std)
 
+The other options of the reference constructor follow data/augmentations.py:70-230:
+
+  gram_teacher_crops_size        the global "base" crops are taken at max(global, gram) and resized (bicubic,
+                                 antialias) to both sizes; with gram_teacher_no_distortions the global crop is resized
+                                 before its distortions and the gram crop is the undistorted base, otherwise both are
+                                 resized from the distorted base.  Batch key `collated_gram_teacher_crops`, crop-major.
+  local_crops_subset_of_global_crops
+                                 local crop c is a local x local window of base crop 1 (c < n/2) or 2, at offsets
+                                 randint(0, (global - local) // patch) * patch, after the local jitter and blur of the
+                                 WHOLE base; it inherits the base's flip
+  share_color_jitter             one ColorJitter + RandomGrayscale per source image, before any crop; no per-crop jitter
+  teacher_no_color_jitter        only fills `global_crops_teacher`, which the collate never reads: no effect on the batch
+
 The kernels (csrc/augment.cu) are deterministic functions of those parameters and are tested against torchvision's
 float implementations.  `GpuBatchPipeline` adds the iBOT block masks (host `MaskingGenerator`, as in the reference's
 collate) and yields the batch dict `Engine.set_batch` consumes.
@@ -68,12 +81,24 @@ class GpuDataAugmentationDINO:
                  teacher_no_color_jitter=False, local_crops_subset_of_global_crops=False, patch_size=16,
                  share_color_jitter=False, horizontal_flips=True, mean=IMAGENET_DEFAULT_MEAN, std=IMAGENET_DEFAULT_STD,
                  seed: int = 0, out_dtype=torch.bfloat16):
-        if gram_teacher_crops_size is not None or local_crops_subset_of_global_crops or share_color_jitter or teacher_no_color_jitter:
-            raise NotImplementedError("gram-teacher crops / local-subset crops / shared or teacher-free colour jitter are not "
-                                      "on the GPU augmentation path (the reference defaults are)")
         assert out_dtype == torch.bfloat16, "the kernels emit bf16 (compute_precision.param_dtype: bf16)"
+        if isinstance(gram_teacher_crops_size, (list, tuple)):
+            raise NotImplementedError("a list of gram_teacher_crops_size values (multi-resolution crops): build one "
+                                      "augmentation per resolution")
         self.global_scale, self.local_scale = tuple(global_crops_scale), tuple(local_crops_scale)
         self.n_local, self.gs, self.ls = int(local_crops_number), int(global_crops_size), int(local_crops_size)
+        if local_crops_subset_of_global_crops:
+            if self.n_local % 2:
+                raise ValueError(f"local_crops_subset_of_global_crops needs an even local_crops_number, got {self.n_local} "
+                                 "(half of the local crops come from each global crop)")
+            if (self.gs - self.ls) // patch_size < 1:
+                raise ValueError(f"local_crops_subset_of_global_crops: (global_crops_size - local_crops_size) // patch_size "
+                                 f"= ({self.gs} - {self.ls}) // {patch_size} leaves no offset to draw")
+        self.gram = None if gram_teacher_crops_size is None else int(gram_teacher_crops_size)
+        self.gram_no_distortions = bool(gram_teacher_no_distortions)
+        self.subset, self.patch = bool(local_crops_subset_of_global_crops), int(patch_size)
+        self.share_color_jitter = bool(share_color_jitter)
+        self.base_size = max(self.gs, self.gram or 0)    # augmentations.py:73: global and gram crops come from one base
         self.flip_p = 0.5 if horizontal_flips else 0.0
         self.mean = (C.c_float * 3)(*[float(v) for v in mean])
         self.std = (C.c_float * 3)(*[float(v) for v in std])
@@ -81,9 +106,22 @@ class GpuDataAugmentationDINO:
         self._scratch = {}
 
     # ---- host: random parameters ----------------------------------------------------------------------------------
+    def _color(self, rec, i):
+        """RandomApply([ColorJitter], p=0.8) + RandomGrayscale(p=0.2) into record i."""
+        rng = self.rng
+        if rng.random() < 0.8:
+            rec["order"][i] = rng.permutation(4)
+            rec["fb"][i], rec["fc"][i] = rng.uniform(0.6, 1.4), rng.uniform(0.6, 1.4)
+            rec["fs"][i], rec["fh"][i] = rng.uniform(0.8, 1.2), rng.uniform(-0.1, 0.1)
+        else:
+            rec["order"][i] = -1
+        rec["gray"][i] = int(rng.random() < 0.2)
+
     def sample(self, B: int, H: int, W: int):
         """Crop records (crop-major: crop index outer, image inner, like the collate's stacking) and blur sigmas for the
-        2 global and n_local local crop sets."""
+        2 global and n_local local crop sets.  The global records' boxes are the base crops at `base_size`.  With
+        local_crops_subset_of_global_crops a local record is a window: img = its base crop's row in the global records,
+        (y0, x0) = (rx, ry), w = h = local size, no flip of its own."""
         rng = self.rng
         g = np.zeros(2 * B, dtype=CROP_DTYPE)
         l = np.zeros(self.n_local * B, dtype=CROP_DTYPE)
@@ -94,23 +132,40 @@ class GpuDataAugmentationDINO:
             y0, x0, h, w = _resized_crop_params(rng, H, W, scale)
             rec["img"][i], rec["x0"][i], rec["y0"][i], rec["w"][i], rec["h"][i] = img, x0, y0, w, h
             rec["flip"][i] = int(rng.random() < self.flip_p)
-            if rng.random() < 0.8:                              # RandomApply([ColorJitter], p=0.8)
-                rec["order"][i] = rng.permutation(4)
-                rec["fb"][i], rec["fc"][i] = rng.uniform(0.6, 1.4), rng.uniform(0.6, 1.4)
-                rec["fs"][i], rec["fh"][i] = rng.uniform(0.8, 1.2), rng.uniform(-0.1, 0.1)
+            if self.share_color_jitter:
+                rec["order"][i] = -1                            # the source image was jittered instead
             else:
-                rec["order"][i] = -1
-            rec["gray"][i] = int(rng.random() < 0.2)            # RandomGrayscale(p=0.2)
+                self._color(rec, i)
             sig[i] = rng.uniform(0.1, 2.0) if rng.random() < blur_apply_p else 0.0
             rec["solarize"][i] = int(rng.random() < solarize_p)
+
+        def fill_window(i, base):
+            l["img"][i], l["w"][i], l["h"][i] = base, self.ls, self.ls
+            if self.share_color_jitter:
+                l["order"][i] = -1
+            else:
+                self._color(l, i)
+            lb[i] = rng.uniform(0.1, 2.0) if rng.random() < 0.5 else 0.0
+            l["y0"][i], l["x0"][i] = rng.integers(0, (self.gs - self.ls) // self.patch, 2) * self.patch   # rx (row), ry
 
         for b in range(B):
             # reference GaussianBlur(p=...) applies the blur with probability 1 - p (data/transforms.py:30-33)
             fill(g, 0 * B + b, b, self.global_scale, 1.0 - 1.0, 0.0, gb)          # global_transfo1: GaussianBlur(p=1.0)
             fill(g, 1 * B + b, b, self.global_scale, 1.0 - 0.1, 0.2, gb)          # global_transfo2: GaussianBlur(p=0.1), Solarize(0.2)
             for c in range(self.n_local):
-                fill(l, c * B + b, b, self.local_scale, 1.0 - 0.5, 0.0, lb)       # local_transfo: GaussianBlur(p=0.5)
+                if self.subset:                                 # crops 0 .. n/2-1 from base 1, the rest from base 2
+                    fill_window(c * B + b, (0 if c < self.n_local // 2 else 1) * B + b)
+                else:
+                    fill(l, c * B + b, b, self.local_scale, 1.0 - 0.5, 0.0, lb)   # local_transfo: GaussianBlur(p=0.5)
         return (g, gb), (l, lb)
+
+    def sample_source_jitter(self, B: int) -> np.ndarray:
+        """share_color_jitter: one ColorJitter + RandomGrayscale record per source image (img = b)."""
+        s = np.zeros(B, dtype=CROP_DTYPE)
+        s["img"] = np.arange(B)
+        for b in range(B):
+            self._color(s, b)
+        return s
 
     # ---- device: kernels ----------------------------------------------------------------------------------------------
     def _buf(self, key, shape, dtype, device):
@@ -120,32 +175,122 @@ class GpuDataAugmentationDINO:
             self._scratch[key] = t
         return t
 
-    def apply(self, images_u8: torch.Tensor, crops: np.ndarray, sigmas: np.ndarray, S: int) -> torch.Tensor:
-        """images_u8 [B,H,W,3] uint8 on the GPU; returns [n_crops, S, S, 3] bf16 (normalised)."""
-        assert images_u8.dtype == torch.uint8 and images_u8.is_cuda and images_u8.is_contiguous() and images_u8.shape[-1] == 3
+    @staticmethod
+    def _dev(records: np.ndarray, dev):
+        return torch.from_numpy(records.view(np.uint8).reshape(-1).copy()).to(dev, non_blocking=True)
+
+    def _crop(self, src: torch.Tensor, d_crops, n: int, S: int, key, clamp: bool = True) -> torch.Tensor:
+        """[n, S, S, 3] fp32 resized crops of src (uint8 images, or fp32 [0,1] images)."""
         lib = N.init()
-        dev = images_u8.device
-        B, H, W, _ = images_u8.shape
-        n = crops.shape[0]
-        d_crops = torch.from_numpy(crops.view(np.uint8).reshape(-1).copy()).to(dev, non_blocking=True)
+        B, H, W, _ = src.shape
+        x = self._buf((key, S), (n, S, S, 3), torch.float32, src.device)
+        if src.dtype == torch.uint8:
+            N.check(lib.d3_aug_resized_crop(N.ptr(src), B, H, W, N.ptr(d_crops), n, N.ptr(x), S, N.stream_ptr()),
+                    "d3_aug_resized_crop")
+        else:
+            N.check(lib.d3_aug_resized_crop_f32(N.ptr(src), B, H, W, N.ptr(d_crops), n, N.ptr(x), S, int(clamp),
+                                                N.stream_ptr()), "d3_aug_resized_crop_f32")
+        return x
+
+    def _resize(self, x: torch.Tensor, S: int, key, clamp: bool) -> torch.Tensor:
+        """Resize(S, bicubic) of every [M, M] image of x; the identity when M == S."""
+        n, M = x.shape[0], x.shape[1]
+        if M == S:
+            return x
+        return self._crop(x, self._dev(self._whole(n, M), x.device), n, S, key, clamp)
+
+    @staticmethod
+    def _whole(n: int, M: int) -> np.ndarray:
+        """Records of the whole [M, M] image i with no flip, jitter, grayscale or solarize."""
+        r = np.zeros(n, dtype=CROP_DTYPE)
+        r["img"], r["w"], r["h"], r["order"] = np.arange(n), M, M, -1
+        return r
+
+    def _finish(self, x: torch.Tensor, d_crops) -> torch.Tensor:
+        n, S = x.shape[0], x.shape[1]
+        out = torch.empty(n, S, S, 3, dtype=torch.bfloat16, device=x.device)
+        N.check(N.init().d3_aug_finish(N.ptr(x), N.ptr(out), N.ptr(d_crops), n, S, self.mean, self.std, N.stream_ptr()),
+                "d3_aug_finish")
+        return out
+
+    def _distort(self, x: torch.Tensor, d_crops, sigmas: np.ndarray, finish: bool = True) -> torch.Tensor:
+        """ColorJitter + RandomGrayscale (in place on x), GaussianBlur, then Solarize + Normalize -> bf16 when `finish`;
+        otherwise the blurred fp32 crops."""
+        lib = N.init()
+        n, S = x.shape[0], x.shape[1]
+        dev = x.device
         d_sig = torch.from_numpy(sigmas.astype(np.float32)).to(dev, non_blocking=True)
-        x = self._buf(("x", S), (n, S, S, 3), torch.float32, dev)
         t1 = self._buf(("t1", S), (n, S, S, 3), torch.float32, dev)
         t2 = self._buf(("t2", S), (n, S, S, 3), torch.float32, dev)
         gsum = torch.zeros(n, dtype=torch.float32, device=dev)
-        out = torch.empty(n, S, S, 3, dtype=torch.bfloat16, device=dev)
         s = N.stream_ptr()
-        N.check(lib.d3_aug_resized_crop(N.ptr(images_u8), B, H, W, N.ptr(d_crops), n, N.ptr(x), S, s), "d3_aug_resized_crop")
         N.check(lib.d3_aug_color(N.ptr(x), N.ptr(d_crops), n, S, N.ptr(gsum), s), "d3_aug_color")
         N.check(lib.d3_aug_blur(N.ptr(x), N.ptr(t1), N.ptr(t2), N.ptr(d_sig), n, S, s), "d3_aug_blur")
-        N.check(lib.d3_aug_finish(N.ptr(t2), N.ptr(out), N.ptr(d_crops), n, S, self.mean, self.std, s), "d3_aug_finish")
-        return out
+        return self._finish(t2, d_crops) if finish else t2
+
+    def apply(self, images_u8: torch.Tensor, crops: np.ndarray, sigmas: np.ndarray, S: int) -> torch.Tensor:
+        """images_u8 [B,H,W,3] uint8 on the GPU (or the fp32 jittered sources of share_color_jitter); returns
+        [n_crops, S, S, 3] bf16 (normalised)."""
+        assert images_u8.dtype in (torch.uint8, torch.float32) and images_u8.is_cuda and images_u8.is_contiguous() \
+            and images_u8.shape[-1] == 3
+        d_crops = self._dev(crops, images_u8.device)
+        return self._distort(self._crop(images_u8, d_crops, crops.shape[0], S, "x"), d_crops, sigmas)
+
+    def jitter_sources(self, images_u8: torch.Tensor, recs: np.ndarray) -> torch.Tensor:
+        """share_color_jitter: fp32 [B,H,W,3] copy of the sources, each jittered with its record."""
+        B, H, W, _ = images_u8.shape
+        dev = images_u8.device
+        x = self._buf(("src", H, W), (B, H, W, 3), torch.float32, dev)
+        gsum = torch.zeros(B, dtype=torch.float32, device=dev)
+        d_recs = self._dev(recs, dev)
+        N.check(N.init().d3_aug_color_images(N.ptr(images_u8), B, H, W, N.ptr(d_recs), N.ptr(x), N.ptr(gsum),
+                                             N.stream_ptr()), "d3_aug_color_images")
+        return x
+
+    def local_windows(self, base: torch.Tensor, crops: np.ndarray, sigmas: np.ndarray) -> torch.Tensor:
+        """local_crops_subset_of_global_crops: [n_crops, L, L, 3] bf16 windows of the fp32 base crops [n_base, M, M, 3],
+        each cut after its own jitter and blur of the whole base."""
+        n_base, M = base.shape[0], base.shape[1]
+        n, L = crops.shape[0], self.ls
+        assert (crops["img"] < n_base).all() and (crops["x0"] + L <= M).all() and (crops["y0"] + L <= M).all()
+        dev = base.device
+        d_crops = self._dev(crops, dev)
+        d_sig = torch.from_numpy(sigmas.astype(np.float32)).to(dev, non_blocking=True)
+        win = self._buf(("win", L), (n, L + 8, L + 8, 3), torch.float32, dev)
+        tmp = self._buf(("wtmp", L), (n, L + 8, L, 3), torch.float32, dev)
+        y = self._buf(("wy", L), (n, L, L, 3), torch.float32, dev)
+        gsum = torch.zeros(n, dtype=torch.float32, device=dev)
+        N.check(N.init().d3_aug_local_windows(N.ptr(base), n_base, M, N.ptr(d_crops), N.ptr(d_sig), n, L, N.ptr(win),
+                                              N.ptr(tmp), N.ptr(y), N.ptr(gsum), N.stream_ptr()), "d3_aug_local_windows")
+        return self._finish(y, d_crops)
 
     def __call__(self, images_u8: torch.Tensor) -> dict:
         B, H, W, _ = images_u8.shape
+        src = images_u8
+        if self.share_color_jitter:
+            src = self.jitter_sources(images_u8, self.sample_source_jitter(B))
         (g, gb), (l, lb) = self.sample(B, H, W)
-        return {"collated_global_crops": self.apply(images_u8, g, gb, self.gs),
-                "collated_local_crops": self.apply(images_u8, l, lb, self.ls)}
+        if self.gram is None and not self.subset:
+            return {"collated_global_crops": self.apply(src, g, gb, self.gs),
+                    "collated_local_crops": self.apply(src, l, lb, self.ls)}
+        # base crops at max(global, gram); what reads the undistorted base runs before the jitter works in place on it
+        dev = images_u8.device
+        d_g = self._dev(g, dev)
+        base = self._crop(src, d_g, 2 * B, self.base_size, "base")
+        out = {"collated_local_crops": self.local_windows(base, l, lb) if self.subset else self.apply(src, l, lb, self.ls)}
+        if self.gram is None:
+            out["collated_global_crops"] = self._distort(base, d_g, gb)
+        elif self.gram_no_distortions:                        # augmentations.py:98-101, :200-201
+            d_whole = self._dev(self._whole(2 * B, self.base_size), dev)
+            out["collated_gram_teacher_crops"] = self._finish(self._resize(base, self.gram, "gram", True), d_whole)
+            out["collated_global_crops"] = self._distort(self._resize(base, self.gs, "x", True), d_g, gb)
+        else:                                                 # :105-108, :202-204: resize the distorted, normalised base
+            y = self._distort(base, d_g, gb, finish=False)
+            N.check(N.init().d3_aug_solarize(N.ptr(y), N.ptr(d_g), 2 * B, self.base_size, N.stream_ptr()), "d3_aug_solarize")
+            d_whole = self._dev(self._whole(2 * B, self.base_size), dev)
+            out["collated_global_crops"] = self._finish(self._resize(y, self.gs, "x", False), d_whole)
+            out["collated_gram_teacher_crops"] = self._finish(self._resize(y, self.gram, "gram", False), d_whole)
+        return out
 
 
 class GpuBatchPipeline:
@@ -156,6 +301,10 @@ class GpuBatchPipeline:
         c = config.crops
         self.aug = GpuDataAugmentationDINO(c.global_crops_scale, c.local_crops_scale, c.local_crops_number,
                                            global_crops_size=c.global_crops_size, local_crops_size=c.local_crops_size,
+                                           gram_teacher_crops_size=c.get("gram_teacher_crops_size", None),
+                                           gram_teacher_no_distortions=c.get("gram_teacher_no_distortions", False),
+                                           local_crops_subset_of_global_crops=c.get("localcrops_subset_of_globalcrops", False),
+                                           share_color_jitter=c.get("share_color_jitter", False),
                                            horizontal_flips=c.get("horizontal_flips", True),
                                            mean=c.get("rgb_mean", IMAGENET_DEFAULT_MEAN), std=c.get("rgb_std", IMAGENET_DEFAULT_STD),
                                            patch_size=config.student.patch_size, seed=seed)

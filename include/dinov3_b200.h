@@ -265,6 +265,25 @@ int d3_aug_blur(const float* x, float* tmp, float* y, const void* blur /*device 
                 int n_crops, int S, void* stream);                                          /* GaussianBlur(9, sigma) */
 int d3_aug_finish(const float* x, void* out_bf16 /*[n_crops,S,S,3]*/, const void* crops, int n_crops, int S,
                   const float* mean3 /*host*/, const float* std3 /*host*/, void* stream);     /* Solarize(128) + Normalize + bf16 */
+/* The remaining DataAugmentationDINO options (augmentations.py:70-230):
+ *  - share_color_jitter (:156-175): ColorJitter + RandomGrayscale of each whole [H, W] source image, one record per image
+ *    (img = image index); x = the jittered fp32 copy, which d3_aug_resized_crop_f32 (clamp 1) then crops.
+ *  - gram_teacher_crops_size (:70-113, :197-205): the global "base" crops are taken at max(global, gram) and resized to
+ *    the global and gram sizes with d3_aug_resized_crop_f32 over the whole base (x0 = y0 = 0, w = h = base size).
+ *    Before the distortions (gram_teacher_no_distortions) the Resize acts on a PIL image: clamp 1.  After them the
+ *    reference resizes the normalised tensor: clamp 0, run after d3_aug_solarize and before d3_aug_finish (Resize
+ *    commutes with Normalize, not with Solarize), and d3_aug_finish is given records with solarize = 0.
+ *  - local_crops_subset_of_global_crops (:208-223): each local crop is the L x L window at (y0, x0) = (rx, ry) of its
+ *    whole base crop (img = base index in [n_base, M, M, 3]) after the base's own jitter and 9-tap blur; y = the
+ *    un-normalised window for d3_aug_finish.  Scratch: win [n_crops, L+8, L+8, 3], tmp [n_crops, L+8, L, 3].         */
+int d3_aug_resized_crop_f32(const float* src /*[n_img,H,W,3] in [0,1]*/, int n_img, int H, int W, const void* crops,
+                            int n_crops, float* out /*[n_crops,S,S,3]*/, int S, int clamp, void* stream);
+int d3_aug_color_images(const void* src_u8 /*[n_img,H,W,3]*/, int n_img, int H, int W, const void* recs /*[n_img]*/,
+                        float* x /*[n_img,H,W,3]*/, float* gray_sum /*[n_img] zeroed*/, void* stream);
+int d3_aug_solarize(float* x /*[n_crops,S,S,3] in place*/, const void* crops, int n_crops, int S, void* stream);
+int d3_aug_local_windows(const float* base /*[n_base,M,M,3]*/, int n_base, int M, const void* crops, const void* blur,
+                         int n_crops, int L, float* win, float* tmp, float* y /*[n_crops,L,L,3]*/,
+                         float* gray_sum /*[n_crops] zeroed*/, void* stream);
 
 #ifdef __cplusplus
 }
