@@ -31,9 +31,14 @@ class EngineConfig:
     local_size: int = 96
     n_global: int = 2
     n_local: int = 8
-    n_prototypes: int = 65536
+    n_prototypes: int = 65536        # the DINO head's sizes (dino.head_*)
     head_hidden: int = 2048
     head_bottleneck: int = 256
+    # the iBOT head's sizes (ibot.head_*); None: the same as the DINO head.  No concrete defaults on purpose: then
+    # config_for(..., n_prototypes=4096) would still build a 65 536-prototype iBOT head
+    ibot_n_prototypes: int | None = None
+    ibot_head_hidden: int | None = None
+    ibot_head_bottleneck: int | None = None
     layerscale: float = 1e-5
     rope_base: float = 100.0
     student_temp: float = 0.1
@@ -88,6 +93,16 @@ class EngineConfig:
     def ffn_width(self) -> int:
         """Columns of the FFN's hidden activation h (what fc2 / w3 contracts over)."""
         return self.swiglu_hidden if self.ffn_layer == "swiglu" else self.hidden
+
+    def head_dims(self, module: str) -> tuple:
+        """(hidden, bottleneck, prototypes) of "dino_head" or "ibot_head" (layers/dino_head.py)."""
+        if module == "dino_head":
+            return self.head_hidden, self.head_bottleneck, self.n_prototypes
+        if module == "ibot_head":
+            own = lambda v, dino: dino if v is None else v
+            return (own(self.ibot_head_hidden, self.head_hidden), own(self.ibot_head_bottleneck, self.head_bottleneck),
+                    own(self.ibot_n_prototypes, self.n_prototypes))
+        raise ValueError(f"no head named {module!r} (dino_head | ibot_head)")
 
     def patches(self, size: int) -> int:
         return (size // self.patch) ** 2
@@ -192,9 +207,11 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
         for key in ("untie_cls_and_patch_norms", "untie_global_and_local_cls_norm"):
             if g(cfg.student, key, False):
                 raise NotImplementedError(f"student.{key}=true is not on the GPU path (one final norm for every token)")
-    if (cfg.dino.head_n_prototypes, cfg.dino.head_hidden_dim, cfg.dino.head_bottleneck_dim) != \
-            (cfg.ibot.head_n_prototypes, cfg.ibot.head_hidden_dim, cfg.ibot.head_bottleneck_dim):
-        raise NotImplementedError("dino and ibot heads must share their dimensions")
+    # an ibot_* field is set only where the iBOT head differs, so equal heads map to the same EngineConfig as ever
+    ibot_kw = {field: int(getattr(cfg.ibot, key)) for field, key in (("ibot_n_prototypes", "head_n_prototypes"),
+                                                                     ("ibot_head_hidden", "head_hidden_dim"),
+                                                                     ("ibot_head_bottleneck", "head_bottleneck_dim"))
+               if getattr(cfg.ibot, key) != getattr(cfg.dino, key)}
     return config_for(
         arch, patch=cfg.student.patch_size, ffn_ratio=cfg.student.ffn_ratio, global_size=cfg.crops.global_crops_size,
         local_size=cfg.crops.local_crops_size, n_local=cfg.crops.local_crops_number,
@@ -209,4 +226,4 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
         n_storage=int(cfg.student.n_storage_tokens), ln_eps=1e-5 if cfg.student.norm_layer == "layernormbf16" else 1e-6,
         ffn_layer=ffn_table[cfg.student.ffn_layer][0], swiglu_align=ffn_table[cfg.student.ffn_layer][1],
         mask_k_bias=bool(cfg.student.get("mask_k_bias", False)),
-        mlp_second_act=ffn_table[cfg.student.ffn_layer][0] == "mlp", **gram_kw)
+        mlp_second_act=ffn_table[cfg.student.ffn_layer][0] == "mlp", **ibot_kw, **gram_kw)

@@ -96,8 +96,9 @@ class Stream:
 
 
 class HeadBufs:
-    def __init__(self, cfg: EngineConfig, R: int, device, stash: bool):
-        D, Hh, Bn, K = cfg.embed_dim, cfg.head_hidden, cfg.head_bottleneck, cfg.n_prototypes
+    def __init__(self, cfg: EngineConfig, module: str, R: int, device, stash: bool):
+        D = cfg.embed_dim
+        Hh, Bn, K = cfg.head_dims(module)
         e = lambda *shape, dt=bf16: torch.empty(*shape, dtype=dt, device=device)
         self.R = R
         self.A0 = e(R, D)
@@ -116,18 +117,21 @@ class HeadBufs:
 
 class SinkhornBufs:
     """`mx`, `s`, `btot` may be views into buffers shared by the DINO and iBOT heads (`joint`): the cross-rank
-    reductions of the two Sinkhorn normalisations then travel in ONE all-reduce per stage (Engine._sinkhorn_pair)."""
+    reductions of the two Sinkhorn normalisations then travel in ONE all-reduce per stage (Engine._sinkhorn_pair).
+    The head's K prototypes sit at [off, off + K) of the joint buffers, its row total at slot `slot` after them."""
 
-    def __init__(self, R: int, K: int, device, joint=None, slot: int = 0):
+    def __init__(self, R: int, K: int, device, joint=None, off: int = 0, slot: int = 0):
+        self.K, self.off = K, off
         if joint is None:
             self.mx = torch.empty(K, dtype=f32, device=device)  # per-prototype shift (column maxima / global max)
             self.s = torch.empty(K, dtype=f32, device=device)
             self.btot = torch.empty(1, dtype=f32, device=device)
         else:
-            mx2, s2 = joint                                      # [2K], [2K + 4]: sums of both heads, then the two row totals
-            self.mx = mx2[slot * K:(slot + 1) * K]
-            self.s = s2[slot * K:(slot + 1) * K]
-            self.btot = s2[2 * K + slot:2 * K + slot + 1]
+            mx2, s2 = joint              # [K_d + K_i], [K_d + K_i + 4]: sums of both heads, then the two row totals
+            Ks = mx2.numel()
+            self.mx = mx2[off:off + K]
+            self.s = s2[off:off + K]
+            self.btot = s2[Ks + slot:Ks + slot + 1]
         self.gmx = torch.empty(1, dtype=f32, device=device)
         self.a = torch.empty(R, dtype=f32, device=device)
 
@@ -177,23 +181,25 @@ class Engine:
             max_masked = sum(int(P * (cfg.mask_ratio[0] + (cfg.mask_ratio[1] - cfg.mask_ratio[0]) * (i + 1) /
                                       max(n_masked_crops, 1))) for i in range(n_masked_crops)) + 8
         self.max_masked = max(int(max_masked), 1)
-        K, D = cfg.n_prototypes, cfg.embed_dim
+        D = cfg.embed_dim
+        Kd, Ki = cfg.head_dims("dino_head")[2], cfg.head_dims("ibot_head")[2]
+        Ks = Kd + Ki
         self.Rc = ng + nl                         # student dino-head rows: concat(g_cls, l_cls)
-        self.h_s_dino = HeadBufs(cfg, self.Rc, dev, stash=True)
-        self.h_s_ibot = HeadBufs(cfg, self.max_masked, dev, stash=True)
-        self.h_t_dino = HeadBufs(cfg, ng, dev, stash=False)
-        self.h_t_ibot = HeadBufs(cfg, self.max_masked, dev, stash=False)
-        self.sk_mx2 = torch.empty(2 * K, dtype=f32, device=dev)
-        self.sk_s2 = torch.zeros(2 * K + 4, dtype=f32, device=dev)
+        self.h_s_dino = HeadBufs(cfg, "dino_head", self.Rc, dev, stash=True)
+        self.h_s_ibot = HeadBufs(cfg, "ibot_head", self.max_masked, dev, stash=True)
+        self.h_t_dino = HeadBufs(cfg, "dino_head", ng, dev, stash=False)
+        self.h_t_ibot = HeadBufs(cfg, "ibot_head", self.max_masked, dev, stash=False)
+        self.sk_mx2 = torch.empty(Ks, dtype=f32, device=dev)
+        self.sk_s2 = torch.zeros(Ks + 4, dtype=f32, device=dev)
         self.sk_btot_local = torch.zeros(4, dtype=f32, device=dev)
         # small cross-rank reductions (Sinkhorn vectors, gradient norms) over NVLink peer memory when the runtime has it
-        self._ar_stage = self.fsdp.setup_small_allreduce(2 * K + 2 * (2 * K + 4) + 4) if comm is not None else None
-        self.sk_dino = SinkhornBufs(ng, K, dev, joint=(self.sk_mx2, self.sk_s2), slot=0)
-        self.sk_ibot = SinkhornBufs(self.max_masked, K, dev, joint=(self.sk_mx2, self.sk_s2), slot=1)
+        self._ar_stage = self.fsdp.setup_small_allreduce(Ks + 2 * (Ks + 4) + 4) if comm is not None else None
+        self.sk_dino = SinkhornBufs(ng, Kd, dev, joint=(self.sk_mx2, self.sk_s2), off=0, slot=0)
+        self.sk_ibot = SinkhornBufs(self.max_masked, Ki, dev, joint=(self.sk_mx2, self.sk_s2), off=Kd, slot=1)
         # centers of the optional softmax-centering path ("state" collection of the reference: dino_clstoken_loss.py:19-22)
-        self.center_dino = torch.zeros(K, dtype=f32, device=dev)
-        self.center_ibot = torch.zeros(K, dtype=f32, device=dev)
-        self._colsum = torch.zeros(K, dtype=f32, device=dev)
+        self.center_dino = torch.zeros(Kd, dtype=f32, device=dev)
+        self.center_ibot = torch.zeros(Ki, dtype=f32, device=dev)
+        self._colsum = torch.zeros(max(Kd, Ki), dtype=f32, device=dev)      # column sums of one head at a time
         i32 = torch.int32
         self.rows_masked_t = torch.empty(self.max_masked, dtype=i32, device=dev)
         self.rows_cls_t = torch.empty(ng, dtype=i32, device=dev)
@@ -537,8 +543,8 @@ class Engine:
         column maxima of the two heads share one all-reduce(max), and each iteration's column sums — with the two row
         totals B riding in the same buffer — one all-reduce(sum): 4 collectives per step instead of 10 (each is latency,
         not bandwidth: 2 x 256 KB).  With NVLink peer memory available the all-reduce is d3_allreduce_peers on inputs
-        staged in symmetric memory (FsdpRuntime.small_allreduce), otherwise NCCL."""
-        K = self.cfg.n_prototypes
+        staged in symmetric memory (FsdpRuntime.small_allreduce), otherwise NCCL.  Ks = K_d + K_i prototypes."""
+        Ks = self.sk_mx2.numel()
         heads = [(0, self.sk_dino, self.h_t_dino.logits[:R_d], R_d)]
         if R_i:
             heads.append((1, self.sk_ibot, self.h_t_ibot.logits[:R_i], R_i))
@@ -546,26 +552,26 @@ class Engine:
             self.sk_btot_local[0:1].fill_(float(R_d))
             self.sk_btot_local[1:2].fill_(float(R_i))
             self._sk_rows = (R_d, R_i)
-        stage = self._ar_stage                                   # symmetric staging: [mx 2K | s 2K+4 | s 2K+4 | sumsq 4]
-        mx_in = stage[:2 * K] if stage is not None else self.sk_mx2
+        stage = self._ar_stage                                   # symmetric staging: [mx Ks | s Ks+4 | s Ks+4 | sumsq 4]
+        mx_in = stage[:Ks] if stage is not None else self.sk_mx2
         mx_in.fill_(float("-inf"))
         for slot, sk, L, R in heads:
-            ops.colmax(L, mx_in[slot * K:(slot + 1) * K])
+            ops.colmax(L, mx_in[sk.off:sk.off + sk.K])
         if stage is not None:
-            self.fsdp.small_allreduce(0, 2 * K, self.sk_mx2, "max")
+            self.fsdp.small_allreduce(0, Ks, self.sk_mx2, "max")
         elif self.comm is not None:
             self.comm.all_reduce_max(self.sk_mx2)
         a = [None, None]
         for it in range(n_iter):
             # staged inputs alternate between two buffers: a peer may still be reading the previous iteration's
-            off = 2 * K + (it & 1) * (2 * K + 4)
-            s_in = stage[off:off + 2 * K + 4] if stage is not None else self.sk_s2
+            off = Ks + (it & 1) * (Ks + 4)
+            s_in = stage[off:off + Ks + 4] if stage is not None else self.sk_s2
             s_in.zero_()
-            s_in[2 * K:].copy_(self.sk_btot_local)
+            s_in[Ks:].copy_(self.sk_btot_local)
             for slot, sk, L, R in heads:
-                ops.sinkhorn_colsum(L, sk.mx, temp, a[slot], s_in[slot * K:(slot + 1) * K])
+                ops.sinkhorn_colsum(L, sk.mx, temp, a[slot], s_in[sk.off:sk.off + sk.K])
             if stage is not None:
-                self.fsdp.small_allreduce(off, 2 * K + 4, self.sk_s2, "sum")   # psum of the row sums (:53 / ibot :99), of B
+                self.fsdp.small_allreduce(off, Ks + 4, self.sk_s2, "sum")   # psum of the row sums (:53 / ibot :99), of B
             elif self.comm is not None:
                 self.comm.all_reduce_sum(self.sk_s2)
             for slot, sk, L, R in heads:
@@ -576,17 +582,18 @@ class Engine:
         """softmax((x - center)/temp) after the center EMA update (loss/dino_clstoken_loss.py:24-33,91-95), expressed
         through the same (mx, s, a, btot) scalings the cross-entropy kernel consumes."""
         L = logits[:R]
+        colsum = self._colsum[:sk.K]
         sk.gmx.fill_(float("-inf"))
         sk.btot.fill_(float(rows_local))
         ops.absmax(L, sk.gmx)
-        self._colsum.zero_()
-        ops.colsum_f32(L, self._colsum)
+        colsum.zero_()
+        ops.colsum_f32(L, colsum)
         if self.comm is not None:
             self.comm.all_reduce_max(sk.gmx)
             self.comm.all_reduce_sum(sk.btot)
-            self.comm.all_reduce_sum(self._colsum)        # pmean of the local centers over "dp" (:93)
+            self.comm.all_reduce_sum(colsum)              # pmean of the local centers over "dp" (:93)
         sk.mx.copy_(sk.gmx.expand_as(sk.mx))              # one global shift for every prototype (device-side broadcast)
-        ops.center_update(center, self._colsum, sk.btot, self.center_momentum, temp, sk.s)
+        ops.center_update(center, colsum, sk.btot, self.center_momentum, temp, sk.s)
         ops.sinkhorn_rowsum(L, sk.mx, temp, sk.s, sk.btot, sk.a[:R])
 
     # ------------------------------------------------------------------------------------------------ backward pieces
@@ -774,7 +781,7 @@ class Engine:
 
     def forward_backward(self, teacher_temp: float):
         cfg, B, M = self.cfg, self.B, self.M
-        D, K = cfg.embed_dim, cfg.n_prototypes
+        D = cfg.embed_dim
         ng = cfg.n_global * B
         self.metrics.zero_()
         for st in self.params.mods.values():
@@ -878,8 +885,8 @@ class Engine:
         # global gradient norm per module (SURVEY A4): sum over ranks of the shards' squares; the modules' scalars are
         # views of one buffer, so the cross-rank sum is one reduction
         if self._ar_stage is not None:
-            K = cfg.n_prototypes
-            off = 2 * K + 2 * (2 * K + 4)
+            Ks = self.sk_mx2.numel()                          # after the Sinkhorn ranges of _sinkhorn_pair
+            off = Ks + 2 * (Ks + 4)
             sq_in = self._ar_stage[off:off + 4]
             sq_in.zero_()
             for i, st in enumerate(self.params.mods.values()):

@@ -51,9 +51,10 @@ def backbone_spec(cfg: EngineConfig):
     return spec
 
 
-def head_spec(cfg: EngineConfig):
-    """layers/dino_head.py:15-43,65-74."""
-    D, Hh, Bn, K = cfg.embed_dim, cfg.head_hidden, cfg.head_bottleneck, cfg.n_prototypes
+def head_spec(cfg: EngineConfig, module: str = "dino_head"):
+    """layers/dino_head.py:15-43,65-74, at the sizes of `module` ("dino_head" | "ibot_head")."""
+    D = cfg.embed_dim
+    Hh, Bn, K = cfg.head_dims(module)
     return [("mlp/layers_0/kernel", (D, Hh), "mat"), ("mlp/layers_0/bias", (Hh,), "vec"),
             ("mlp/layers_2/kernel", (Hh, Hh), "mat"), ("mlp/layers_2/bias", (Hh,), "vec"),
             ("mlp/layers_4/kernel", (Hh, Bn), "mat"), ("mlp/layers_4/bias", (Bn,), "vec"),
@@ -218,8 +219,8 @@ class ParamStore:
         self.cfg = cfg
         self.mods = {
             "backbone": ModuleStore("backbone", backbone_spec(cfg), cfg, device, world, rank),
-            "dino_head": ModuleStore("dino_head", head_spec(cfg), cfg, device, world, rank),
-            "ibot_head": ModuleStore("ibot_head", head_spec(cfg), cfg, device, world, rank),
+            "dino_head": ModuleStore("dino_head", head_spec(cfg, "dino_head"), cfg, device, world, rank),
+            "ibot_head": ModuleStore("ibot_head", head_spec(cfg, "ibot_head"), cfg, device, world, rank),
         }
         self.runtime = None     # set by the engine (fsdp.runtime.FsdpRuntime)
 

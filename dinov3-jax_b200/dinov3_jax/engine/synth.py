@@ -66,8 +66,8 @@ def reference_like_params(cfg: EngineConfig, seed: int = 0) -> dict:
             out[f"teacher_{module}/{name}"] = t.clone()
 
     fill("backbone", backbone_spec(cfg))
-    fill("dino_head", head_spec(cfg))
-    fill("ibot_head", head_spec(cfg))
+    fill("dino_head", head_spec(cfg, "dino_head"))
+    fill("ibot_head", head_spec(cfg, "ibot_head"))
     return out
 
 

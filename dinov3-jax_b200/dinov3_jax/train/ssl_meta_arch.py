@@ -92,8 +92,9 @@ class SSLMetaArch:
         """name -> (lr_multiplier, wd_multiplier, is_last_layer) for every student tensor (:577-598 / param_groups.py)."""
         from ..engine.params import backbone_spec, head_spec
         out = {}
-        for module, spec in (("backbone", backbone_spec(self.engine_config)), ("dino_head", head_spec(self.engine_config)),
-                             ("ibot_head", head_spec(self.engine_config))):
+        for module, spec in (("backbone", backbone_spec(self.engine_config)),
+                             ("dino_head", head_spec(self.engine_config, "dino_head")),
+                             ("ibot_head", head_spec(self.engine_config, "ibot_head"))):
             for name, _, _ in spec:
                 out[f"student_{module}/{name}"] = lr_wd_multipliers(module, name, self.engine_config)
         return out

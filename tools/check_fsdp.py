@@ -23,9 +23,16 @@ def main():
     cfg = tiny_cfg(layerscale=0.5)
     B = 2
     P = init_params(cfg, 0, perturb=0.05)
+    ecfg = from_oracle_cfg(cfg)
+    if "--distinct-heads" in sys.argv:      # an iBOT head with its own sizes (the oracle reads them from the parameters)
+        import dataclasses
+        K, Hh, Bn = 136, 96, 48
+        Pi = init_params(dataclasses.replace(cfg, n_prototypes=K, head_hidden=Hh, head_bottleneck=Bn), 1, perturb=0.05)
+        P.update({k: v for k, v in Pi.items() if "_ibot_head/" in k})
+        ecfg = dataclasses.replace(ecfg, ibot_n_prototypes=K, ibot_head_hidden=Hh, ibot_head_bottleneck=Bn)
     batches = [synthetic_batch(cfg, B, seed=r) for r in range(world)]
     hyper = dict(lr=1e-3, wd=0.04, last_layer_lr=5e-4, momentum=0.99, teacher_temp=0.05)
-    eng = Engine(from_oracle_cfg(cfg), B, device=f"cuda:{lr_}", max_masked=max(int(b["mask_indices_list"].shape[0]) for b in batches), comm=Comm())
+    eng = Engine(ecfg, B, device=f"cuda:{lr_}", max_masked=max(int(b["mask_indices_list"].shape[0]) for b in batches), comm=Comm())
     eng.params.load_reference_tree(P)
     if rank == 0:
         print("gradient reduce-scatter path:", "push over NVLink peer memory (GEMM epilogue + d3_scatter_add_peers)" if eng.fsdp.push else "NCCL reduce_scatter", flush=True)
