@@ -2,7 +2,6 @@
 #include <algorithm>
 #include <atomic>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include "d3_internal.h"
 
@@ -20,11 +19,7 @@ int set_error(int code, const char* msg) {
   snprintf(g_err, sizeof(g_err), "%s", msg ? msg : "");
   return code;
 }
-static int g_sm_limit = 0;
-int sm_count() {
-  const int n = g_sm_count > 0 ? g_sm_count : 132;
-  return (g_sm_limit > 0 && g_sm_limit < n) ? g_sm_limit : n;
-}
+int sm_count() { return g_sm_count > 0 ? g_sm_count : 132; }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
 int encode_tensor_map_2d_bf16(CUtensorMap* map, const void* ptr, const cuuint64_t dims[2],
@@ -98,27 +93,11 @@ int slab_combine(const float* ws, int slabs, long long stride, long long rows, i
 
 }  // namespace d3
 
-static int g_scatter_mode = -1;
-namespace d3 {
-int scatter_mode() {
-  if (g_scatter_mode < 0) { const char* e = getenv("D3_FSDP_PUSH_SYS"); g_scatter_mode = (e && e[0] == '1') ? 1 : 0; }
-  return g_scatter_mode;
-}
-void set_scatter_mode(int mode) { g_scatter_mode = mode ? 1 : 0; }
-}  // namespace d3
-
 using namespace d3;
 
 extern "C" {
 
-int d3_set_scatter_mode(int mode) { d3::set_scatter_mode(mode); return D3_OK; }
-
-int d3_abi_version(void) { return 6; }   // 2: d3_gemm_epilogue gained the sc_* scatter fields; 3: round-2 entry points (swiglu, ema, colmax, deterministic Sinkhorn sums, koleo rows, augmentation); 4: two entry points removed (the plain LayerNorm backward is d3_layernorm_bwd_ls without a tail; d3_sinkhorn_colsum is deterministic for every K); 5: d3_debug_attn_trace removed (the attention clock64() trace); 6: d3_koleo_fwd_bwd removed (it is d3_koleo_fwd_bwd_rows with row0 = 0, nrows = B)
-int d3_set_sm_limit(int n) {
-  if (n < 0) return set_error(D3_ERR_ARG, "d3_set_sm_limit: n < 0");
-  g_sm_limit = n;
-  return D3_OK;
-}
+int d3_abi_version(void) { return 7; }   // 2: d3_gemm_epilogue gained the sc_* scatter fields; 3: round-2 entry points (swiglu, ema, colmax, deterministic Sinkhorn sums, koleo rows, augmentation); 4: two entry points removed (the plain LayerNorm backward is d3_layernorm_bwd_ls without a tail; d3_sinkhorn_colsum is deterministic for every K); 5: d3_debug_attn_trace removed (the attention clock64() trace); 6: d3_koleo_fwd_bwd removed (it is d3_koleo_fwd_bwd_rows with row0 = 0, nrows = B); 7: the scatter-mode and SM-limit setters removed (the peer push is always one device-scope vector red; the persistent grids always cover every SM)
 const char* d3_last_error(void) { return g_err; }
 long long d3_launch_count(void) { return g_launches.load(); }
 void d3_reset_launch_count(void) { g_launches.store(0); }
@@ -143,7 +122,6 @@ int d3_init(int device) {
       cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
     }
   }
-  if (const char* e = getenv("D3_GEMM_SMS")) g_sm_limit = atoi(e);
   if (!g_encode) {
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult q;
@@ -167,7 +145,7 @@ int d3_gemm_bf16(const void* A, int lda, int a_major, const void* B, int ldb, in
   g.out = ep->out; g.ld_out = ep->ld_out; g.ld_aux = ep->ld_aux; g.ld_resid = ep->ld_resid;
   g.flags = ep->flags & 0x1FF; g.alpha = ep->alpha;
   for (int i = 0; i < 8; ++i) g.sc_peer[i] = ep->sc_peer[i];
-  g.sc_off = ep->sc_off; g.sc_shard = ep->sc_shard; g.sc_world = ep->sc_world; g.sc_sys = scatter_mode();
+  g.sc_off = ep->sc_off; g.sc_shard = ep->sc_shard; g.sc_world = ep->sc_world;
   if (g.flags & EP_SCATTER)
     for (int i = 0; i < g.sc_world && i < 8; ++i)
       if (!g.sc_peer[i]) return set_error(D3_ERR_ARG, "scatter flag without peer pointers");

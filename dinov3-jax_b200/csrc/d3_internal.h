@@ -39,12 +39,9 @@ struct GemmEpilogue {
   float* sc_peer[8];
   long long sc_off;
   int sc_shard, sc_world;
-  int sc_sys;      // 1: scalar system-scope atomics (atomicAdd_system) instead of one device-scope vector red
 };
 
 int set_error(int code, const char* msg);
-int scatter_mode();            // 0: one vector device-scope red per float4 (default); 1: four scalar system-scope atomics
-void set_scatter_mode(int mode);
 int sm_count();
 void count_launch(int n = 1);
 int encode_tensor_map_2d_bf16(CUtensorMap* map, const void* ptr, const cuuint64_t dims[2],

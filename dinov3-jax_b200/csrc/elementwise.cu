@@ -797,18 +797,13 @@ __global__ void swiglu_bwd_kernel(const __nv_bfloat16* __restrict__ x12, const _
 // fsdp/utils.py:61-64,108): element g of src (g = off + i) is added, scaled by alpha, into rank g / shard's slice.
 struct PeerPtrs { float* p[8]; };
 __global__ void scatter_add_peers_kernel(const float* __restrict__ src, long n4, PeerPtrs peers, unsigned long long off,
-                                         unsigned shard, float alpha, int sys_scope) {
+                                         unsigned shard, float alpha) {
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
     const float4 v = reinterpret_cast<const float4*>(src)[i];
     const unsigned long long g = off + (unsigned long long)i * 4;
     const unsigned r = (unsigned)(g / shard);
     float* dst = peers.p[r] + (g - (unsigned long long)r * shard);
-    if (sys_scope) {
-      atomicAdd_system(dst, v.x * alpha); atomicAdd_system(dst + 1, v.y * alpha);
-      atomicAdd_system(dst + 2, v.z * alpha); atomicAdd_system(dst + 3, v.w * alpha);
-    } else {
-      atomicAdd(reinterpret_cast<float4*>(dst), make_float4(v.x * alpha, v.y * alpha, v.z * alpha, v.w * alpha));
-    }
+    atomicAdd(reinterpret_cast<float4*>(dst), make_float4(v.x * alpha, v.y * alpha, v.z * alpha, v.w * alpha));
   }
 }
 
@@ -1104,8 +1099,7 @@ int d3_scatter_add_peers(const float* src, long long n, float* const* peers /*ho
   for (int i = 0; i < 8; ++i) pp.p[i] = i < world ? peers[i] : nullptr;
   const long n4 = n / 4;
   const int blocks = (int)min((n4 + 255) / 256, (long)sm_count() * 4);
-  scatter_add_peers_kernel<<<blocks, 256, 0, STREAM(stream)>>>(src, n4, pp, (unsigned long long)off, (unsigned)shard, alpha,
-                                                              scatter_mode());
+  scatter_add_peers_kernel<<<blocks, 256, 0, STREAM(stream)>>>(src, n4, pp, (unsigned long long)off, (unsigned)shard, alpha);
   D3_CHECK_LAUNCH();
   return D3_OK;
 }

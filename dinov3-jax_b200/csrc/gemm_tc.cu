@@ -158,13 +158,8 @@ __device__ __forceinline__ void epilogue_tile_runtime(const GemmEpilogue& ep, fl
           const unsigned long long shard = (unsigned long long)ep.sc_shard;
           const unsigned r = (unsigned)(g_idx / shard);   // a pair never straddles two owners (shard % 4 == 0)
           float* const dst = ep.sc_peer[r] + (g_idx - r * shard);
-          if (!two) {
-            atomicAdd(dst, v0);
-          } else if (ep.sc_sys) {
-            atomicAdd_system(dst, v0); atomicAdd_system(dst + 1, v1);
-          } else {
-            atomicAdd(reinterpret_cast<float2*>(dst), make_float2(v0, v1));
-          }
+          if (!two) atomicAdd(dst, v0);
+          else atomicAdd(reinterpret_cast<float2*>(dst), make_float2(v0, v1));
           continue;
         }
         if (epi_has<EPI_RUNTIME>(ep, EP_STORE_PRE)) st_pair(ep.aux_out + row * ep.ld_aux + n, p0, p1, vec, two);

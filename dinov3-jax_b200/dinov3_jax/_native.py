@@ -39,11 +39,9 @@ P, I, LL, F = C.c_void_p, C.c_int, C.c_longlong, C.c_float
 # name -> argtypes, mirrors include/dinov3_b200.h (tests/test_abi.py checks every declared symbol is exported)
 SIGNATURES = {
     "d3_init": [I],
-    "d3_set_sm_limit": [I],
     "d3_gemm_bf16": [P, I, I, P, I, I, I, I, I, C.POINTER(GemmEpilogue), I, I, P],
     "d3_scatter_add_peers": [P, LL, P, I, LL, I, F, P],
     "d3_allreduce_peers": [P, I, P, LL, I, P],
-    "d3_set_scatter_mode": [I],
     "d3_im2col": [P, P, I, I, I, I, I, P],
     "d3_assemble_tokens": [P, P, P, P, P, P, I, I, I, I, P],
     "d3_assemble_tokens_bwd": [P, P, P, P, P, P, I, I, I, I, P],

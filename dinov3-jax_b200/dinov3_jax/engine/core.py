@@ -223,7 +223,7 @@ class Engine:
         # they read (dU2, dU1, dP, dQKV) are double-buffered by block parity; events order reuse.
         # (with remat the weight-gradient GEMMs read the single scratch set that the next block's recompute overwrites,
         # so they stay on the main stream)
-        self.wgrad_overlap = os.environ.get("D3_WGRAD_STREAM", "1") != "0" and not self.remat
+        self.wgrad_overlap = not self.remat
         nbuf = 2 if self.wgrad_overlap else 1
         self.dU2, self.dP = [e(T, D) for _ in range(nbuf)], [e(T, D) for _ in range(nbuf)]
         self.dU1 = [e(T, 2 * Hd if self.swiglu else Hd) for _ in range(nbuf)]       # swiglu: [dx1 | dx2]
@@ -666,7 +666,7 @@ class Engine:
         # added into the owning rank's gradient shard over NVLink); the rest of the unit is pushed in grads_ready
         big = ("mlp/w3/kernel", "mlp/w1/kernel", "mlp/w2/kernel", "attn/qkv/kernel") if self.swiglu else \
               ("mlp/Dense_1/kernel", "mlp/Dense_0/kernel", "attn/qkv/kernel")
-        fused = big if (self.fsdp.push and self.fsdp.push_gemm) else ()
+        fused = big if self.fsdp.push else ()
         inv_world = 1.0 / self.fsdp.world
 
         def wgrad(slot, a, b, name):

@@ -1,5 +1,11 @@
-"""FSDP runtime: NCCL all-gather of each unit's parameters before use and reduce-scatter (mean) of its gradients after
-its backward, issued on a side stream so they overlap the neighbouring unit's compute.
+"""FSDP runtime: all-gather of each unit's parameters before use and reduce-scatter (mean) of its gradients after its
+backward, issued on a side stream so they overlap the neighbouring unit's compute.
+
+With NCCL and more than one rank both go through NVLink peer memory (torch symmetric memory): the bf16 matrices are
+gathered by copy-engine copies out of the peers' shards, and every rank adds its gradients straight into the owners'
+fp32 shards (the weight-gradient GEMM epilogue for the big matrices, d3_scatter_add_peers for the rest), fenced by a
+symmetric-memory barrier.  NCCL all_gather / reduce_scatter is the fallback: on gloo (the CPU tests), where symmetric
+memory is unavailable, and with D3_FSDP_PUSH=0.  The small vector ranges always take one all-gather per module.
 
 Replaces `gather_params` / `fwd_gather_bwd_pmean_scatter` / `sync_grads` of the reference (dinov3_jax/fsdp/utils.py:
 56-110), which lower to per-leaf jax.lax.all_gather / psum_scatter / pmean inside the jitted step.  torch.distributed
@@ -68,29 +74,20 @@ class FsdpRuntime:
         self._pending = {}       # (module, unit, teacher) -> [works]
         self._grad_works = []
         import os
-        self._debug = int(os.environ.get("D3_FSDP_DEBUG", "0"))   # diagnostics only: 1 = skip gathers, 2 = skip reduce-scatters
         # Gradient reduce-scatter without NCCL: every rank ADDS its contribution straight into the owner's gradient
         # shard through NVLink peer mappings (torch symmetric memory provides the mappings) — from the weight-gradient
         # GEMM's epilogue for the big matrices (ops.gemm(scatter=...)), from d3_scatter_add_peers for the rest.
         self.push = False
-        self.push_gemm = os.environ.get("D3_FSDP_PUSH_GEMM", "1") != "0"     # 0: only the stand-alone push kernel
-        # parameter all-gather of the bf16 matrices through the copy engines (peer-mapped shards) instead of NCCL kernels
-        # that take SMs from the persistent GEMM grids; D3_FSDP_DMA_GATHER=0 keeps NCCL
-        self.dma_gather = os.environ.get("D3_FSDP_DMA_GATHER", "1") != "0"
         self._peer_views = {}
         self._peer_ptrs = {}
         # vector regions (LN / bias / LayerScale: ~1 MB per module): ONE all-gather per (module, teacher|student) and one
         # permutation kernel at step start instead of one NCCL kernel per unit — ~50 fewer NCCL launches co-running
-        # with (and taking SMs from) the teacher pass's persistent GEMMs.  D3_FSDP_VEC_BULK=0: per-unit gathers.
-        self.vec_bulk = os.environ.get("D3_FSDP_VEC_BULK", "1") != "0"
-        self._fence_barrier = os.environ.get("D3_FSDP_FENCE_BARRIER", "1") != "0"   # 0: NCCL all-reduce as the push fence
-        self._push_side = os.environ.get("D3_FSDP_PUSH_SIDE", "1") != "0"          # 0: stand-alone pushes on the compute stream
+        # with (and taking SMs from) the teacher pass's persistent GEMMs.
         self._vec_perm = {}
         self._vec_tmp = {}
-        # Default: on at every world size (tools/check_fsdp_push.py compares the pushed shards with the NCCL
-        # reduce-scatter).  D3_FSDP_PUSH=0 selects the NCCL reduce-scatter.
-        want = os.environ.get("D3_FSDP_PUSH", "auto")
-        if self.cuda and self.world > 1 and comm.backend == "nccl" and want in ("1", "auto"):
+        # On at every world size.  D3_FSDP_PUSH=0 selects the NCCL reduce-scatter and all-gather
+        # (tools/check_fsdp_push.py compares the pushed shards with the NCCL reduce-scatter).
+        if self.cuda and self.world > 1 and comm.backend == "nccl" and os.environ.get("D3_FSDP_PUSH", "1") != "0":
             self._setup_push()
 
     def _setup_push(self):
@@ -103,9 +100,10 @@ class FsdpRuntime:
                 st.grad_shard = shard
                 self._peer_ptrs[name] = [int(p) for p in hdl.buffer_ptrs]
                 st._symm_handle = hdl
-                if self.dma_gather and st.bf16_shard.numel():
+                if st.bf16_shard.numel():
                     # bf16 matrix shards (student + teacher) in peer-mapped memory: the parameter all-gather becomes
-                    # plain device-to-device copies out of the peers' shards (copy engines, no SM, no NCCL kernel)
+                    # plain device-to-device copies out of the peers' shards (copy engines, no SM, no NCCL kernel
+                    # taking SMs from the persistent GEMM grids)
                     hs = {}
                     for attr in ("bf16_shard", "t_bf16_shard"):
                         old = getattr(st, attr)
@@ -125,9 +123,8 @@ class FsdpRuntime:
 
     def setup_small_allreduce(self, n_floats: int):
         """Symmetric-memory staging buffer for small all-reduces over peer mappings (d3_allreduce_peers); None when the
-        peer-memory path is not active (the caller then uses NCCL).  D3_FSDP_SMALL_AR=0 keeps NCCL."""
-        import os
-        if not self.push or os.environ.get("D3_FSDP_SMALL_AR", "1") == "0":
+        peer-memory path is not active (the caller then uses NCCL)."""
+        if not self.push:
             return None
         import torch.distributed._symmetric_memory as symm_mem
         dev = next(iter(self.stores.values())).grad_shard.device
@@ -200,7 +197,7 @@ class FsdpRuntime:
             sa, sb = L.shard_range(unit, "mat")
             src = (st.t_bf16_shard if teacher else st.bf16_shard)[sa:sb]
             dst = (st.t_bf16 if teacher else st.bf16)[ma:mb]
-            if self.push and self.dma_gather and hasattr(st, "_symm_param_handles"):
+            if self.push:
                 # tiled all-gather (fsdp/utils.py:66) as world copies: slice r of the unit comes from rank r's shard
                 n = sb - sa
                 views = self._shard_views(module, st, teacher)
@@ -212,13 +209,8 @@ class FsdpRuntime:
             else:
                 works.append(self.comm.all_gather(dst, src, async_op=True))
         va, vb = unit.vec
-        if vb > va and self.vec_bulk:
+        if vb > va:
             works.append(self._vec_done[(module, teacher)])
-        elif vb > va:
-            sa, sb = L.shard_range(unit, "vec")
-            src = (st.t_master if teacher else st.master)[sa:sb]
-            dst = (st.t_vecs if teacher else st.vecs)[va - L.n_mat: vb - L.n_mat]
-            works.append(self.comm.all_gather(dst, src, async_op=True))
         self._pending[(module, unit.name, teacher)] = works
 
     def _gather_vecs(self, module: str, teacher: bool):
@@ -266,26 +258,23 @@ class FsdpRuntime:
     def prefetch(self, items):
         """items: iterable of (module, unit, teacher) in use order.  All gathers are queued on the side stream at once:
         NCCL executes them back to back while the compute stream works through earlier units."""
-        if self.world == 1 or (self._debug & 1):
+        if self.world == 1:
             return
         items = list(items)
         self._vec_done = {}
 
         def vecs_first():
-            if self.vec_bulk:
-                for module, teacher in dict.fromkeys((m, t) for m, _, t in items):
-                    self._vec_done[(module, teacher)] = self._gather_vecs(module, teacher)
+            for module, teacher in dict.fromkeys((m, t) for m, _, t in items):
+                self._vec_done[(module, teacher)] = self._gather_vecs(module, teacher)
         if self.side is not None:
             self.side.wait_stream(torch.cuda.current_stream())   # parameters come from the previous optimizer step
             with torch.cuda.stream(self.side):
-                if self.push and self.dma_gather:
+                if self.push:
                     # the copies below read the PEERS' shards: every rank's optimizer step must have finished.  (The
                     # opposite hazard - a peer's next optimizer step overwriting a shard still being copied - is closed
-                    # by the fence all-reduce of finish_grads: a rank reaches it only after its backward, i.e. after all
+                    # by the fence barrier of finish_grads: a rank reaches it only after its backward, i.e. after all
                     # of its gathers of this step were consumed.)
-                    st0 = next(iter(self.stores.values()))
-                    if hasattr(st0, "_symm_handle"):
-                        st0._symm_handle.barrier(0)
+                    next(iter(self.stores.values()))._symm_handle.barrier(0)
                 vecs_first()
                 for module, unit, teacher in items:
                     self._issue_gather(module, unit, teacher)
@@ -306,7 +295,7 @@ class FsdpRuntime:
     def grads_ready(self, module: str, unit_name: str, also_after=None, scattered=()):
         """Called right after the kernels of this unit's backward were enqueued: reduce-scatter (mean) its gradient
         ranges into the rank's gradient shard, on the side stream."""
-        if self.world == 1 or (self._debug & 2):
+        if self.world == 1:
             return
         st = self.stores[module]
         L = st.layout
@@ -315,15 +304,11 @@ class FsdpRuntime:
             # the stand-alone pushes (proj matrices, vectors, heads, embed: 0.84 ms per ViT-L step at 2 ranks in the
             # kernel timeline) only feed the optimizer: they run on the side stream, off the backward's critical path;
             # finish_grads() joins it before the fence
-            cur = torch.cuda.current_stream()
-            ps = self.side if (self.side is not None and self._push_side) else cur
-            if ps is not cur:
-                ps.wait_stream(cur)
+            self.side.wait_stream(torch.cuda.current_stream())
             if also_after is not None:
-                ps.wait_event(also_after)
-            with torch.cuda.stream(ps):
+                self.side.wait_event(also_after)
+            with torch.cuda.stream(self.side):
                 self._push_ranges(module, unit, tuple(scattered))
-            self._pushed_on_side = ps is not cur
             return
 
         def issue():
@@ -350,20 +335,10 @@ class FsdpRuntime:
             w.wait()
         self._grad_works = []
         if self.push:
-            if getattr(self, "_pushed_on_side", False):
-                torch.cuda.current_stream().wait_stream(self.side)
-                self._pushed_on_side = False
-            # every rank's pushes are complete once its stream reaches this collective; the all-reduce completes on a
-            # rank only after all ranks have joined, so afterwards every contribution has landed in the local shard
-            # (a symmetric-memory barrier on this stream has the same property at a fraction of an all-reduce's latency)
-            st0 = next(iter(self.stores.values()))
-            if self._fence_barrier and hasattr(st0, "_symm_handle"):
-                st0._symm_handle.barrier(1)
-                return
-            self._fence = getattr(self, "_fence", None)
-            if self._fence is None:
-                self._fence = torch.zeros(1, device=st0.grad_shard.device)
-            self.comm.all_reduce_sum(self._fence)
+            torch.cuda.current_stream().wait_stream(self.side)
+            # every rank's pushes are complete once its stream reaches this barrier; the barrier completes on a rank
+            # only after all ranks have reached it, so afterwards every contribution has landed in the local shard
+            next(iter(self.stores.values()))._symm_handle.barrier(1)
 
     # ------------------------------------------------------------------------------------------ utilities
     def gather_full(self, module: str, what: str, teacher: bool = False) -> torch.Tensor:

@@ -29,9 +29,6 @@ typedef enum {
 int d3_init(int device);                /* bind to device, cache SM count, resolve cuTensorMapEncodeTiled */
 const char* d3_last_error(void);
 int d3_abi_version(void);
-/* Cap the grid of the persistent kernels (GEMMs) to n SMs (0 = all).  Multi-GPU runs leave a few SMs to the NCCL
- * kernels of the FSDP all-gather / reduce-scatter so they run under the GEMMs instead of between them.              */
-int d3_set_sm_limit(int n);
 long long d3_launch_count(void);        /* kernels launched by this library since the last reset (bench: gpu_launches) */
 void d3_reset_launch_count(void);
 
@@ -118,9 +115,6 @@ int d3_ls_gamma_from_wgrad(const void* W_bf16, const float* dW, const float* bia
  * adds alpha * src[i] into the rank owning flat index off + i of a range split into `world` slices of `shard` elements;
  * peers[r] = rank r's zero-initialised slice (a pointer valid in THIS process: NVLink peer mapping, peers[rank] local).
  * The caller orders the step with a cross-rank barrier before the slices are consumed.                               */
-/* 0 (default): one device-scope vector red per float4; 1: four scalar system-scope atomics (also env D3_FSDP_PUSH_SYS=1).
- * Applies to D3_EP_SCATTER and d3_scatter_add_peers.                                                                   */
-int d3_set_scatter_mode(int mode);
 int d3_scatter_add_peers(const float* src, long long n, float* const* peers /*host array [world]*/, int world,
                          long long off, int shard, float alpha, void* stream);
 

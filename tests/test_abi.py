@@ -28,13 +28,14 @@ def test_python_signature_table_matches_header():
     assert declared == bound, (declared - bound, bound - declared)
 
 
-def test_abi_version_6_and_error_string():
-    """Version 6: the plain KoLeo is d3_koleo_fwd_bwd_rows over all rows.  Version 5: the attention debug trace
+def test_abi_version_7_and_error_string():
+    """Version 7: the scatter-mode and SM-limit setters are gone (the peer push has one form, the persistent grids use
+    every SM).  Version 6: the plain KoLeo is d3_koleo_fwd_bwd_rows over all rows.  Version 5: the attention debug trace
     (d3_debug_attn_trace) is gone.  Version 4: the plain LayerNorm backward and the atomic-free Sinkhorn sums have no
     entry points of their own."""
     from dinov3_jax import _native
     lib = _native.lib()
-    assert lib.d3_abi_version() == 6
+    assert lib.d3_abi_version() == 7
     assert isinstance(lib.d3_last_error(), bytes)
 
 

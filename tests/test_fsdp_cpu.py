@@ -116,8 +116,8 @@ def _worker(rank, world, port, ret):
         dist.destroy_process_group()
 
 
-def _runtime_worker(rank, world, port, ret, bulk):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), D3_FSDP_VEC_BULK="1" if bulk else "0")
+def _runtime_worker(rank, world, port, ret):
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
         from dinov3_jax.engine.params import ModuleStore, backbone_spec
@@ -144,13 +144,12 @@ def _runtime_worker(rank, world, port, ret, bulk):
         dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("bulk", [True, False])
-def test_gloo_world2_runtime_prefetch_fills_the_compute_buffers(bulk):
-    """FsdpRuntime.prefetch / acquire: per-unit matrix gathers + (bulk: one all-gather and a permutation per module |
-    per-unit) vector gathers reproduce the single-GPU buffers for student and teacher."""
+def test_gloo_world2_runtime_prefetch_fills_the_compute_buffers():
+    """FsdpRuntime.prefetch / acquire: per-unit matrix gathers + one vector all-gather and a permutation per module
+    reproduce the single-GPU buffers for student and teacher."""
     world = 2
     ret = mp.Manager().dict()
-    mp.spawn(_runtime_worker, args=(world, _free_port(), ret, bulk), nprocs=world, join=True)
+    mp.spawn(_runtime_worker, args=(world, _free_port(), ret), nprocs=world, join=True)
     assert all(ret[r] for r in range(world))
 
 

@@ -557,13 +557,11 @@ def test_sums_are_bit_reproducible(case):
 
 
 # --------------------------------------------------------------------------------------------------- fused reduce-scatter
-@pytest.mark.parametrize("mode", [0, 1])
 @pytest.mark.parametrize("M,N,K,world", [(512, 768, 4096, 2), (1024, 1024, 8192, 4), (296, 264, 2048, 8)])
-def test_gemm_scatter_epilogue_and_peer_push(M, N, K, world, mode):
+def test_gemm_scatter_epilogue_and_peer_push(M, N, K, world):
     """D3_EP_SCATTER: the weight-gradient tile is added into the slice owner's buffer (here `world` local buffers stand
     in for the peers' NVLink mappings); d3_scatter_add_peers does the same for a flat range.  Two "ranks" contribute."""
-    from dinov3_jax import _native, ops
-    _native.lib().d3_set_scatter_mode(mode)          # 0: vector device-scope red, 1: scalar system-scope atomics
+    from dinov3_jax import ops
     total = ((M * N + 8 * world - 1) // (8 * world)) * 8 * world + 64 * world     # tensor sits at offset 64 in the range
     shard = total // world
     shards = [torch.zeros(shard, device="cuda") for _ in range(world)]
@@ -582,7 +580,6 @@ def test_gemm_scatter_epilogue_and_peer_push(M, N, K, world, mode):
     src = torch.randn(8 * world * 5, device="cuda")
     ops.scatter_add_peers(src, peers, 8 * world, shard, 0.25)
     ref[8 * world: 8 * world + src.numel()] += 0.25 * src
-    _native.lib().d3_set_scatter_mode(0)
     assert rel(torch.cat(shards), ref) < 2e-3
 
 

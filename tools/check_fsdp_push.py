@@ -41,7 +41,7 @@ def main():
         grads[mi] = {k: v.float().cpu() for k, v in eng.params.export_reference_tree("grad").items()}
         loss = eng.read_metrics()["total_loss"]
         if rank == 0:
-            print(f"[{mode}] world={world} loss {loss:.6f} scatter_mode={os.environ.get('D3_FSDP_PUSH_SYS', '0')}", flush=True)
+            print(f"[{mode}] world={world} loss {loss:.6f}", flush=True)
         del eng
         torch.cuda.empty_cache()
         dist.barrier()

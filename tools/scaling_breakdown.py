@@ -5,8 +5,8 @@ Run once as `python tools/scaling_breakdown.py` (1 GPU) and once under torchrun 
   * the step's phases (events at the phase boundaries of the real, two-stream step),
   * a single-stream instrumented step: every tensor-core GEMM launch timed, grouped by (kind, shape, scatter epilogue),
   * the time the compute stream spends WAITING for parameter gathers (acquire) — measured as the difference between the
-    phase with and without the gathers queued (N > 1 only; D3_FSDP_DEBUG_NOGATHER is not needed: we time acquire waits
-    through events recorded before / after each wait).
+    phase with and without the gathers queued (N > 1 only; acquire waits are timed through events recorded before /
+    after each wait).
 """
 import os, sys, time
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -141,8 +141,7 @@ for p, sc in zip(prof, scat_seen + [False] * (len(prof) - len(scat_seen))):
     g = groups.setdefault(key, [0, 0.0, 0.0])
     g[0] += 1; g[1] += p[2].elapsed_time(p[3]); g[2] += p[1]
 if rank == 0:
-    print(f"== {arch} B={B}/GPU world={world} push={getattr(eng.fsdp, 'push', None) if world > 1 else None} "
-          f"dma_gather={getattr(eng.fsdp, 'dma_gather', None) if world > 1 else None}")
+    print(f"== {arch} B={B}/GPU world={world} push={getattr(eng.fsdp, 'push', None) if world > 1 else None}")
     print(f"step {step_ms:.2f} ms   (single-stream instrumented step {single_ms:.2f} ms)")
     for k, v in phases.items():
         print(f"  phase {k:34s} {v:8.2f} ms")
