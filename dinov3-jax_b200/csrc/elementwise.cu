@@ -85,6 +85,19 @@ __global__ void assemble_tokens_bwd_kernel(const float* __restrict__ dX, const u
 // ------------------------------------------------------------------------------------------------ LayerNorm
 // models/vision_transformer.py:40 (flax nn.LayerNorm, eps 1e-6, biased variance E[x^2]-E[x]^2, fp32 stats).
 // One warp per row; x fp32 [T, D]; y bf16 or fp32.
+// Every LayerNorm forward (layernorm_fwd_kernel, ln_tokens_out_kernel) goes through ln_row_stats and ln_store4, so a
+// row normalised by either gets the same bits.
+
+// 4 values stored at columns 4e..4e+3 of the row yr (bf16: round to nearest even)
+template <typename OutT>
+__device__ __forceinline__ void store4(OutT* yr, int e, float o0, float o1, float o2, float o3) {
+  if constexpr (sizeof(OutT) == 2) {
+    reinterpret_cast<uint2*>(yr)[e] = make_uint2(pack_bf16(o0, o1), pack_bf16(o2, o3));
+  } else {
+    reinterpret_cast<float4*>(yr)[e] = make_float4(o0, o1, o2, o3);
+  }
+}
+
 // columns 4e..4e+3 of the row yr: (v - mean) rstd scale + bias
 template <typename OutT>
 __device__ __forceinline__ void ln_store4(OutT* yr, int e, const float4& v, const float* scale, const float* bias, float mean,
@@ -93,16 +106,55 @@ __device__ __forceinline__ void ln_store4(OutT* yr, int e, const float4& v, cons
   const float4 b = reinterpret_cast<const float4*>(bias)[e];
   const float o0 = (v.x - mean) * rstd * g.x + b.x, o1 = (v.y - mean) * rstd * g.y + b.y;
   const float o2 = (v.z - mean) * rstd * g.z + b.z, o3 = (v.w - mean) * rstd * g.w + b.w;
-  if constexpr (sizeof(OutT) == 2) {
-    reinterpret_cast<uint2*>(yr)[e] = make_uint2(pack_bf16(o0, o1), pack_bf16(o2, o3));
+  store4(yr, e, o0, o1, o2, o3);
+}
+
+// Mean and rstd of the row xr ([D] fp32, 16-byte aligned), computed by one warp: lane l sums the float4 columns
+// l, l + 32, ... in that order, then a butterfly.  VPL > 0: D = 128 * VPL known at compile time; the row is left in v
+// (lane l holds float4 columns k * 32 + l), all VPL 16-byte loads of a lane in flight together.  VPL == 0: any
+// D % 4 == 0 (`width` is read only then), v unused.
+template <int VPL>
+__device__ __forceinline__ void ln_row_stats(const float4* __restrict__ xr, int lane, int width, float eps,
+                                             float4 (&v)[VPL > 0 ? VPL : 1], float& mean, float& rstd) {
+  const int D = VPL > 0 ? VPL * 128 : width;
+  float s = 0.f, s2 = 0.f;
+  if constexpr (VPL > 0) {
+#pragma unroll
+    for (int k = 0; k < VPL; ++k) v[k] = xr[k * 32 + lane];
+#pragma unroll
+    for (int k = 0; k < VPL; ++k) {
+      s += v[k].x + v[k].y + v[k].z + v[k].w;
+      s2 += v[k].x * v[k].x + v[k].y * v[k].y + v[k].z * v[k].z + v[k].w * v[k].w;
+    }
   } else {
-    reinterpret_cast<float4*>(yr)[e] = make_float4(o0, o1, o2, o3);
+    for (int e = lane; e < D / 4; e += 32) {
+      const float4 w = xr[e];
+      s += w.x + w.y + w.z + w.w;
+      s2 += w.x * w.x + w.y * w.y + w.z * w.z + w.w * w.w;
+    }
+  }
+  s = warp_sum(s);
+  s2 = warp_sum(s2);
+  mean = s * (1.f / D);
+  const float var = fmaxf(s2 * (1.f / D) - mean * mean, 0.f);
+  rstd = rsqrtf(var + eps);
+}
+
+// the whole row xr normalised into yr (one warp; v and mean / rstd from ln_row_stats<VPL>)
+template <int VPL, typename OutT>
+__device__ __forceinline__ void ln_store_row(OutT* yr, const float4* __restrict__ xr, int lane, int D,
+                                             const float4 (&v)[VPL > 0 ? VPL : 1], const float* scale, const float* bias,
+                                             float mean, float rstd) {
+  if constexpr (VPL > 0) {
+#pragma unroll
+    for (int k = 0; k < VPL; ++k) ln_store4(yr, k * 32 + lane, v[k], scale, bias, mean, rstd);
+  } else {
+    for (int e = lane; e < D / 4; e += 32) ln_store4(yr, e, xr[e], scale, bias, mean, rstd);
   }
 }
 
-// VPL > 0: D = 128 * VPL known at compile time; the row stays in registers between the statistics and the
-// normalisation (one read of x), all VPL 16-byte loads of a lane are in flight together.  VPL == 0: any D % 4 == 0
-// (`width` is read only then), x read twice.
+// VPL > 0: the row stays in registers between the statistics and the normalisation (one read of x).  VPL == 0: x read
+// twice.
 template <int VPL, typename OutT>
 __global__ void __launch_bounds__(256)
 layernorm_fwd_kernel(const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ bias,
@@ -113,34 +165,108 @@ layernorm_fwd_kernel(const float* __restrict__ x, const float* __restrict__ scal
   for (long row = (long)blockIdx.x * warps + (threadIdx.x >> 5); row < T; row += (long)gridDim.x * warps) {
     const float4* xr = reinterpret_cast<const float4*>(x + row * (long)D);
     float4 v[VPL > 0 ? VPL : 1];
-    float s = 0.f, s2 = 0.f;
-    if constexpr (VPL > 0) {
-#pragma unroll
-      for (int k = 0; k < VPL; ++k) v[k] = xr[k * 32 + lane];
-#pragma unroll
-      for (int k = 0; k < VPL; ++k) {
-        s += v[k].x + v[k].y + v[k].z + v[k].w;
-        s2 += v[k].x * v[k].x + v[k].y * v[k].y + v[k].z * v[k].z + v[k].w * v[k].w;
-      }
-    } else {
-      for (int e = lane; e < D / 4; e += 32) {
-        const float4 w = xr[e];
-        s += w.x + w.y + w.z + w.w;
-        s2 += w.x * w.x + w.y * w.y + w.z * w.z + w.w * w.w;
-      }
-    }
-    s = warp_sum(s);
-    s2 = warp_sum(s2);
-    const float mean = s * (1.f / D);
-    const float var = fmaxf(s2 * (1.f / D) - mean * mean, 0.f);
-    const float rstd = rsqrtf(var + eps);
+    float mean, rstd;
+    ln_row_stats<VPL>(xr, lane, D, eps, v, mean, rstd);
     if (lane == 0 && mean_out) { mean_out[row] = mean; rstd_out[row] = rstd; }
-    if constexpr (VPL > 0) {
-#pragma unroll
-      for (int k = 0; k < VPL; ++k) ln_store4(y + row * (long)D, k * 32 + lane, v[k], scale, bias, mean, rstd);
-    } else {
-      for (int e = lane; e < D / 4; e += 32) ln_store4(y + row * (long)D, e, xr[e], scale, bias, mean, rstd);
+    ln_store_row<VPL>(y + row * (long)D, xr, lane, D, v, scale, bias, mean, rstd);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ block output -> features
+// models/vision_transformer.py:280-313 (get_intermediate_layers): one block output X [n, N = 1 + R + P, D] fp32 ->
+// cls [n, D], storage [n, R, D] and the patches, channels-last [n, P, D] or channels-first [n, D, Hp, Wp], each row
+// LayerNorm-ed with (pre_scale, pre_bias) for the 1 + R prefix rows and (scale, bias) for the patch rows, or only
+// converted when scale is null.
+struct TokensOut {
+  const float *X, *scale, *bias, *pre_scale, *pre_bias;
+  void *cls, *storage, *patches;
+  int n, N, R, P, D;
+  float eps;
+  int tp;                // channels-first: patch rows per tile (8 or 16 .. 64)
+  int tiles_per_img;     // ceil(P / tp)
+  int vec_bytes;         // channels-first: bytes per store along a channel plane (16, 8, 4 or 2)
+};
+
+constexpr int TOK_WARPS = 8;
+constexpr int TOK_PAD = 4;       // elements after each staged row: keeps rows 16-byte aligned, spreads the column reads
+
+// row t of image b (one warp) -> its output row, LayerNorm-ed or converted
+template <int VPL, typename OutT>
+__device__ __forceinline__ void tokens_out_row(const TokensOut& a, int b, int t, OutT* dst, int lane) {
+  const int D = a.D;
+  const float4* xr = reinterpret_cast<const float4*>(a.X + ((long)b * a.N + t) * D);
+  const bool prefix = t <= a.R;
+  const float* g = prefix ? a.pre_scale : a.scale;
+  const float* bb = prefix ? a.pre_bias : a.bias;
+  if (g) {
+    float4 v[VPL > 0 ? VPL : 1];
+    float mean, rstd;
+    ln_row_stats<VPL>(xr, lane, D, a.eps, v, mean, rstd);
+    ln_store_row<VPL>(dst, xr, lane, D, v, g, bb, mean, rstd);
+  } else {
+    for (int e = lane; e < D / 4; e += 32) {
+      const float4 w = xr[e];
+      store4(dst, e, w.x, w.y, w.z, w.w);
     }
+  }
+}
+
+template <typename OutT>
+__device__ __forceinline__ OutT* tokens_out_dst(const TokensOut& a, int b, int t) {
+  const long D = a.D;
+  if (t == 0) return (OutT*)a.cls + b * D;
+  if (t <= a.R) return (OutT*)a.storage + ((long)b * a.R + t - 1) * D;
+  return (OutT*)a.patches + ((long)b * a.P + t - 1 - a.R) * D;
+}
+
+// `vb` bytes of channel plane `dst` from the staged column src[0], src[ld], ... (vb / sizeof(OutT) rows)
+template <typename OutT>
+__device__ __forceinline__ void store_column_run(OutT* dst, const OutT* src, int ld, int vb) {
+  if constexpr (sizeof(OutT) == 4) {
+    if (vb == 16) *reinterpret_cast<float4*>(dst) = make_float4(src[0], src[ld], src[2 * ld], src[3 * ld]);
+    else if (vb == 8) *reinterpret_cast<float2*>(dst) = make_float2(src[0], src[ld]);
+    else *dst = src[0];
+  } else {
+    const unsigned short* s = reinterpret_cast<const unsigned short*>(src);
+    auto pair = [&](int i) { return (uint32_t)s[i * ld] | ((uint32_t)s[(i + 1) * ld] << 16); };
+    if (vb == 16) *reinterpret_cast<uint4*>(dst) = make_uint4(pair(0), pair(2), pair(4), pair(6));
+    else if (vb == 8) *reinterpret_cast<uint2*>(dst) = make_uint2(pair(0), pair(2));
+    else if (vb == 4) *reinterpret_cast<uint32_t*>(dst) = pair(0);
+    else *reinterpret_cast<unsigned short*>(dst) = s[0];
+  }
+}
+
+// CF = false: one warp per row of all n * N rows (grid-stride).
+// CF = true: CTAs [0, n * tiles_per_img) each take tp patch rows of one image: every warp normalises whole rows into a
+// shared-memory tile [tp][D + TOK_PAD] (x read once), then the CTA writes the tile out channel by channel, a run of
+// vec_bytes along Hp*Wp per thread, consecutive threads on consecutive runs of the same plane.  The CTAs after them take
+// the n * (1 + R) prefix rows, one warp per row.
+template <int VPL, typename OutT, bool CF>
+__global__ void __launch_bounds__(32 * TOK_WARPS, 2)
+ln_tokens_out_kernel(const TokensOut a) {
+  extern __shared__ __align__(16) unsigned char tok_smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_tiles = CF ? a.n * a.tiles_per_img : 0;
+  if (CF && (int)blockIdx.x < n_tiles) {
+    OutT* tile = reinterpret_cast<OutT*>(tok_smem);
+    const int ld = a.D + TOK_PAD;
+    const int b = blockIdx.x / a.tiles_per_img, p0 = blockIdx.x % a.tiles_per_img * a.tp;
+    const int rows = min(a.tp, a.P - p0);
+    for (int r = warp; r < rows; r += TOK_WARPS) tokens_out_row<VPL>(a, b, 1 + a.R + p0 + r, tile + (long)r * ld, lane);
+    __syncthreads();
+    const int w = a.vec_bytes / (int)sizeof(OutT), runs = a.tp / w;
+    OutT* plane0 = (OutT*)a.patches + (long)b * a.D * a.P + p0;
+    for (int i = threadIdx.x; i < a.D * runs; i += blockDim.x) {
+      const int c = i / runs, p = i % runs * w;
+      if (p < rows) store_column_run(plane0 + (long)c * a.P + p, tile + (long)p * ld + c, ld, a.vec_bytes);
+    }
+    return;
+  }
+  const int per_img = CF ? 1 + a.R : a.N;
+  const long total = (long)a.n * per_img;
+  for (long r = (long)(blockIdx.x - n_tiles) * TOK_WARPS + warp; r < total; r += (long)(gridDim.x - n_tiles) * TOK_WARPS) {
+    const int b = (int)(r / per_img), t = (int)(r % per_img);
+    tokens_out_row<VPL>(a, b, t, tokens_out_dst<OutT>(a, b, t), lane);
   }
 }
 
@@ -995,6 +1121,50 @@ static int launch_ln_fwd(const float* x, const float* scale, const float* bias, 
   return D3_OK;
 }
 
+constexpr size_t TOK_SMEM_MAX = 227 * 1024;
+constexpr size_t TOK_SMEM_TARGET = 113 * 1024;       // two tiles per SM
+
+template <int VPL, typename OutT>
+static int launch_tokens_out(TokensOut a, int channels_first, cudaStream_t st) {
+  if (!channels_first) {
+    const long rows = (long)a.n * a.N;
+    const int blocks = (int)min((rows + TOK_WARPS - 1) / TOK_WARPS, (long)sm_count() * 8);
+    ln_tokens_out_kernel<VPL, OutT, false><<<blocks, 32 * TOK_WARPS, 0, st>>>(a);
+    D3_CHECK_LAUNCH();
+    return D3_OK;
+  }
+  const size_t row_bytes = (size_t)(a.D + TOK_PAD) * sizeof(OutT);
+  // at least 32 bytes (one DRAM sector) of a channel plane per tile, 64 rows where two tiles fit on an SM
+  a.tp = 64;
+  while (a.tp > 32 / (int)sizeof(OutT) && a.tp * row_bytes > TOK_SMEM_TARGET) a.tp /= 2;
+  const size_t smem = a.tp * row_bytes;
+  if (smem > TOK_SMEM_MAX) return set_error(D3_ERR_ARG, "d3_layernorm_tokens_out: D too large for the channels-first tile");
+  a.tiles_per_img = (a.P + a.tp - 1) / a.tp;
+  static const cudaError_t cfg = cudaFuncSetAttribute(ln_tokens_out_kernel<VPL, OutT, true>,
+                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TOK_SMEM_MAX);
+  (void)cfg;   // a failure shows at the launch
+  const long prefix_rows = (long)a.n * (1 + a.R);
+  const long blocks = (long)a.n * a.tiles_per_img + (prefix_rows + TOK_WARPS - 1) / TOK_WARPS;
+  ln_tokens_out_kernel<VPL, OutT, true><<<(unsigned)blocks, 32 * TOK_WARPS, smem, st>>>(a);
+  D3_CHECK_LAUNCH();
+  return D3_OK;
+}
+
+template <typename OutT>
+static int launch_tokens_out(const TokensOut& a, int channels_first, cudaStream_t st) {
+  if (!a.scale) return launch_tokens_out<0, OutT>(a, channels_first, st);    // no statistics: plain copy / conversion
+  switch (a.D) {      // the widths d3_layernorm_fwd specialises, so that each row takes the same instructions
+    case 128: return launch_tokens_out<1, OutT>(a, channels_first, st);
+    case 256: return launch_tokens_out<2, OutT>(a, channels_first, st);
+    case 384: return launch_tokens_out<3, OutT>(a, channels_first, st);
+    case 512: return launch_tokens_out<4, OutT>(a, channels_first, st);
+    case 768: return launch_tokens_out<6, OutT>(a, channels_first, st);
+    case 1024: return launch_tokens_out<8, OutT>(a, channels_first, st);
+    case 1536: return launch_tokens_out<12, OutT>(a, channels_first, st);
+    default: return launch_tokens_out<0, OutT>(a, channels_first, st);
+  }
+}
+
 
 extern "C" {
 
@@ -1056,6 +1226,32 @@ int d3_layernorm_fwd(const float* x, const float* scale, const float* bias, void
     case 1536: return launch_ln_fwd<12>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
     default: return launch_ln_fwd<0>(x, scale, bias, y, y_is_f32, mean, rstd, T, D, eps, st);
   }
+}
+
+int d3_layernorm_tokens_out(const float* X, const float* scale, const float* bias, const float* pre_scale,
+                            const float* pre_bias, float eps, int n, int N, int R, int Hp, int Wp, int D, void* cls,
+                            void* storage, void* patches, int out_f32, int channels_first, void* stream) {
+  if (!X || !cls || !patches || (R > 0 && !storage)) return set_error(D3_ERR_ARG, "d3_layernorm_tokens_out: null pointer");
+  if (!scale != !bias || !pre_scale != !pre_bias || !scale != !pre_scale)
+    return set_error(D3_ERR_ARG, "d3_layernorm_tokens_out: scale, bias, pre_scale and pre_bias are all given (norm) or all null");
+  if (n < 0 || R < 0 || Hp < 1 || Wp < 1 || D < 4 || D % 4)
+    return set_error(D3_ERR_ARG, "d3_layernorm_tokens_out: need n >= 0, R >= 0, Hp, Wp >= 1, D a positive multiple of 4");
+  if ((long long)N != 1LL + R + (long long)Hp * Wp) return set_error(D3_ERR_ARG, "d3_layernorm_tokens_out: N != 1 + R + Hp*Wp");
+  if ((long long)n * N * D >= (1LL << 40)) return set_error(D3_ERR_ARG, "d3_layernorm_tokens_out: X too large");
+  const uintptr_t out_align = out_f32 ? 16 : 8;
+  if (((uintptr_t)X | (uintptr_t)scale | (uintptr_t)bias | (uintptr_t)pre_scale | (uintptr_t)pre_bias) % 16 ||
+      ((uintptr_t)cls | (uintptr_t)storage | (channels_first ? 0 : (uintptr_t)patches)) % out_align ||
+      (uintptr_t)patches % (out_f32 ? 4 : 2))
+    return set_error(D3_ERR_ARG, "d3_layernorm_tokens_out: X and the norm vectors must be 16-byte aligned, cls, storage and "
+                                 "channels-last patches 16-byte (fp32) / 8-byte (bf16), channels-first patches element-aligned");
+  if (n == 0) return D3_OK;
+  TokensOut a{X, scale, bias, pre_scale, pre_bias, cls, storage, patches, n, N, R, Hp * Wp, D, eps, 0, 0, 0};
+  // widest store whose size divides both a channel plane's byte stride and the plane base (odd grids: narrower)
+  const int es = out_f32 ? 4 : 2;
+  a.vec_bytes = 16;
+  while (a.vec_bytes > es && (((long)a.P * es) % a.vec_bytes || (uintptr_t)patches % a.vec_bytes)) a.vec_bytes /= 2;
+  cudaStream_t st = STREAM(stream);
+  return out_f32 ? launch_tokens_out<float>(a, channels_first, st) : launch_tokens_out<__nv_bfloat16>(a, channels_first, st);
 }
 
 int d3_layernorm_bwd_ls(const void* dy, int dy_is_f32, const float* x, const float* mean, const float* rstd,

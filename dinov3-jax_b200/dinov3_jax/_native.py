@@ -46,6 +46,7 @@ SIGNATURES = {
     "d3_assemble_tokens": [P, P, P, P, P, P, I, I, I, I, P],
     "d3_assemble_tokens_bwd": [P, P, P, P, P, P, I, I, I, I, P],
     "d3_layernorm_fwd": [P, P, P, P, I, P, P, I, I, F, P],
+    "d3_layernorm_tokens_out": [P, P, P, P, P, F, I, I, I, I, I, I, P, P, P, I, I, P],
     "d3_layernorm_bwd_ls": [P, I, P, P, P, P, P, P, P, P, I, I, P, P, I, P, P, P, P],
     "d3_ls_gamma_from_wgrad": [P, P, P, P, P, P, I, I, P],
     "d3_rope": [P, P, P, LL, I, I, I, I, I, P],

@@ -81,19 +81,71 @@ class Mlp:
         ops.gemm(h, self.w2, y, b_mn=True, bias=self.b2, gelu=True)
         return y.view(*shp[:-1], self.w2.shape[1])
 
+    def residual(self, z, xmid, gamma):
+        """xmid + gamma * mlp(z) (z bf16 [T, D], xmid fp32 [T, D]): LayerScale and residual in the second GEMM's epilogue."""
+        h = torch.empty(z.shape[0], self.w1.shape[1], dtype=bf16, device=z.device)
+        ops.gemm(z, self.w1, h, b_mn=True, bias=self.b1, gelu=True)
+        out = torch.empty_like(xmid)
+        ops.gemm(h, self.w2, out, b_mn=True, bias=self.b2, gelu=True, gamma=gamma, resid=xmid)
+        return out
+
+
+class SwiGLUFFN:
+    """layers/ffn_layers.py:52-76: w3(silu(w1 x) * w2 x), hidden width int(2/3 hidden_features) rounded up to align_to.
+    The engine's kernels (engine/core.py): the w1 and w2 GEMMs write the two halves of one [T, 2 Hs] buffer, then
+    d3_swiglu_fwd, then the w3 GEMM."""
+
+    def __init__(self, params: dict, hidden_features=None, out_features=None, act_layer=None, drop: float = 0.0,
+                 use_bias: bool = True, align_to: int = 8):
+        self.w1, self.w2, self.w3 = (_w(params[k]["kernel"]) for k in ("w1", "w2", "w3"))
+        Hs = self.w1.shape[1]
+        if hidden_features is not None:
+            d = int(hidden_features * 2 / 3)
+            assert Hs == d + (-d % align_to), f"w1 has {Hs} columns, SwiGLUFFN({hidden_features}, align_to={align_to}) " \
+                                              f"has {d + (-d % align_to)}"
+        if Hs % 8:
+            raise NotImplementedError("SwiGLU hidden width must be a multiple of 8 (align_to 8 / 32 / 64 / 128 all give one)")
+        zero = lambda k: torch.zeros(k, dtype=f32, device=self.w1.device)
+        bias = lambda k, w: _v(params[k]["bias"]) if use_bias and "bias" in params[k] else zero(w.shape[1])
+        self.b1, self.b2, self.b3 = bias("w1", self.w1), bias("w2", self.w2), bias("w3", self.w3)
+        self.Hs = Hs
+
+    def _hidden(self, z):
+        T, Hs = z.shape[0], self.Hs
+        x12 = torch.empty(T, 2 * Hs, dtype=bf16, device=z.device)
+        ops.gemm(z, self.w1, x12[:, :Hs], b_mn=True, bias=self.b1)
+        ops.gemm(z, self.w2, x12[:, Hs:], b_mn=True, bias=self.b2)
+        h = torch.empty(T, Hs, dtype=bf16, device=z.device)
+        ops.swiglu_fwd(x12, h)
+        return h
+
+    def __call__(self, x):
+        shp = x.shape
+        h = self._hidden(x.reshape(-1, shp[-1]).to(bf16).contiguous())
+        y = torch.empty(h.shape[0], self.w3.shape[1], dtype=f32, device=x.device)
+        ops.gemm(h, self.w3, y, b_mn=True, bias=self.b3)
+        return y.view(*shp[:-1], self.w3.shape[1])
+
+    def residual(self, z, xmid, gamma):
+        """xmid + gamma * ffn(z): LayerScale and residual in the w3 GEMM's epilogue."""
+        out = torch.empty_like(xmid)
+        ops.gemm(self._hidden(z), self.w3, out, b_mn=True, bias=self.b3, gamma=gamma, resid=xmid)
+        return out
+
 
 class SelfAttention:
     """layers/attention.py:49-118: fused qkv Dense -> RoPE on q,k (prefix tokens skipped) -> attention -> proj."""
 
     def __init__(self, params: dict, dim: int, num_heads: int = 8, qkv_bias: bool = False, proj_bias: bool = True,
                  attn_drop: float = 0.0, proj_drop: float = 0.0, mask_k_bias: bool = False):
-        if mask_k_bias:
-            raise NotImplementedError("mask_k_bias (LinearKMaskedBias fills its mask with NaN in the reference, attention.py:42)")
         if dim not in (num_heads * 64, num_heads * 128):
             raise NotImplementedError("head_dim must be 64 or 128")
         self.dim, self.H = dim, num_heads
         self.wqkv = _w(params["qkv"]["kernel"])
         self.bqkv = _v(params["qkv"]["bias"]) if "bias" in params["qkv"] else torch.zeros(3 * dim, device=self.wqkv.device)
+        if mask_k_bias:      # the engine's meaning (upstream DINOv3 LinearKMaskedBias): the k third of the bias is zero
+            self.bqkv = self.bqkv.clone()
+            self.bqkv[dim:2 * dim] = 0
         self.wp, self.bp = _w(params["proj"]["kernel"]), _v(params["proj"]["bias"])
 
     def compute_attention(self, qkv, attn_bias=None, rope=None, deterministic=True):
@@ -121,11 +173,20 @@ class SelfAttention:
 class SelfAttentionBlock:
     """layers/block.py:22-214, deterministic branch :195-201: x + ls1(attn(norm1 x)); x + ls2(mlp(norm2 x))."""
 
+    FFN_ALIGN = {"swiglu": 8, "swiglu32": 32, "swiglu64": 64, "swiglu128": 128}     # models/vision_transformer.py:30-36
+
     def __init__(self, params: dict, dim: int, num_heads: int, ffn_ratio: float = 4.0, qkv_bias: bool = True,
-                 proj_bias: bool = True, ffn_bias: bool = True, init_values=None, eps: float = 1e-6, **unused):
+                 proj_bias: bool = True, ffn_bias: bool = True, init_values=None, eps: float = 1e-6,
+                 ffn_layer: str = "mlp", mask_k_bias: bool = False, **unused):
         self.dim, self.H, self.eps = dim, num_heads, eps
-        self.attn = SelfAttention(params["attn"], dim, num_heads, qkv_bias=qkv_bias)
-        self.mlp = Mlp(params["mlp"])
+        self.attn = SelfAttention(params["attn"], dim, num_heads, qkv_bias=qkv_bias, mask_k_bias=mask_k_bias)
+        if ffn_layer == "mlp":
+            self.mlp = Mlp(params["mlp"])
+        elif ffn_layer in self.FFN_ALIGN:
+            self.mlp = SwiGLUFFN(params["mlp"], hidden_features=int(dim * ffn_ratio), out_features=dim, use_bias=ffn_bias,
+                                 align_to=self.FFN_ALIGN[ffn_layer])
+        else:
+            raise NotImplementedError(f"ffn_layer {ffn_layer!r}: mlp | swiglu | swiglu32 | swiglu64 | swiglu128")
         self.n1 = (_v(params["norm1"]["scale"]), _v(params["norm1"]["bias"]))
         self.n2 = (_v(params["norm2"]["scale"]), _v(params["norm2"]["bias"]))
         self.g1, self.g2 = _v(params["ls1"]["gamma"]), _v(params["ls2"]["gamma"])
@@ -142,11 +203,7 @@ class SelfAttentionBlock:
         ops.gemm(o, self.attn.wp, xmid, b_mn=True, bias=self.attn.bp, gamma=self.g1, resid=X)
         z = torch.empty(n * N, D, dtype=bf16, device=x.device)
         ops.layernorm_fwd(xmid, self.n2[0], self.n2[1], z, eps=self.eps)
-        h = torch.empty(n * N, self.mlp.w1.shape[1], dtype=bf16, device=x.device)
-        ops.gemm(z, self.mlp.w1, h, b_mn=True, bias=self.mlp.b1, gelu=True)
-        out = torch.empty_like(X)
-        ops.gemm(h, self.mlp.w2, out, b_mn=True, bias=self.mlp.b2, gelu=True, gamma=self.g2, resid=xmid)
-        return out.view(n, N, D)
+        return self.mlp.residual(z, xmid, self.g2).view(n, N, D)
 
 
 class DINOHead:
@@ -182,4 +239,4 @@ class DINOHead:
         return logits
 
 
-__all__ = ["RopePositionEmbedding", "LayerScale", "PatchEmbed", "Mlp", "SelfAttention", "SelfAttentionBlock", "DINOHead"]
+__all__ = ["RopePositionEmbedding", "LayerScale", "PatchEmbed", "Mlp", "SwiGLUFFN", "SelfAttention", "SelfAttentionBlock", "DINOHead"]

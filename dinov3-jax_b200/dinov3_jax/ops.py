@@ -124,6 +124,28 @@ def layernorm_fwd(x, scale, bias, y, mean=None, rstd=None, eps=1e-6):
     return y
 
 
+def layernorm_tokens_out(X, cls, storage, patches, Hp, Wp, norm=None, pre_norm=None, eps=1e-6, channels_first=False):
+    """One block output X [n, 1+R+Hp*Wp, D] fp32 -> cls [n, D], storage [n, R, D] (None when R == 0) and patches
+    ([n, Hp*Wp, D], or [n, D, Hp, Wp] with channels_first), all fp32 or all bf16 (d3_layernorm_tokens_out).
+    norm / pre_norm: (scale, bias) for the patch rows / the 1+R prefix rows (pre_norm None: the same norm); norm None:
+    copied / converted only."""
+    n, Ntok, D = X.shape
+    R = Ntok - 1 - Hp * Wp
+    out_dtype = cls.dtype
+    assert X.dtype == f32 and X.is_contiguous() and out_dtype in (f32, bf16)
+    assert cls.shape == (n, D) and patches.shape == ((n, D, Hp, Wp) if channels_first else (n, Hp * Wp, D))
+    assert storage is None if R == 0 else storage.shape == (n, R, D)
+    for t in (cls, storage, patches):
+        assert t is None or (t.dtype == out_dtype and t.is_contiguous())
+    pre_norm = norm if pre_norm is None else pre_norm
+    sc, bi = norm if norm is not None else (None, None)
+    psc, pbi = pre_norm if norm is not None else (None, None)
+    N.check(N.init().d3_layernorm_tokens_out(_p(X), _p(sc), _p(bi), _p(psc), _p(pbi), float(eps), n, Ntok, R, Hp, Wp, D,
+                                             _p(cls), _p(storage), _p(patches), int(out_dtype == f32), int(channels_first),
+                                             _s()), "d3_layernorm_tokens_out")
+    return cls, storage, patches
+
+
 def layernorm_bwd_ls(dy, x, mean, rstd, scale, dx, dx_add=None, dscale=None, dbias=None, *, ls_gamma=None, ls_u=None,
                      ls_gelu=False, ls_du=None, ls_dgamma=None, ls_dbias=None):
     """LayerNorm backward + the LayerScale/activation backward of the branch upstream (d3_layernorm_bwd_ls)."""

@@ -94,6 +94,18 @@ int d3_assemble_tokens_bwd(const float* dX, const unsigned char* masks, void* dT
  * d3_layernorm_bwd_ls: every row operand and parameter vector (dy, x, scale, dx_add, dx, ls_gamma, ls_u, ls_du) 16 bytes. */
 int d3_layernorm_fwd(const float* x /*[T,D]*/, const float* scale, const float* bias, void* y, int y_is_f32,
                      float* mean /*[T] or NULL*/, float* rstd, int T, int D, float eps, void* stream);
+/* One block output -> the dense features of models/vision_transformer.py:280-313 (get_intermediate_layers), one launch:
+ * X fp32 [n, N, D] with N = 1 + R + Hp*Wp (cls, R storage tokens, patches) -> cls [n, D], storage [n, R, D] (NULL when
+ * R == 0) and patches, channels-last [n, Hp*Wp, D] (channels_first = 0) or channels-first [n, D, Hp, Wp] (reshape=True),
+ * all three fp32 (out_f32 = 1) or bf16 (round to nearest even).  Each row is LayerNorm-ed with the statistics and
+ * arithmetic of d3_layernorm_fwd (the same bits as d3_layernorm_fwd on that row): the 1 + R prefix rows with
+ * (pre_scale, pre_bias), the patch rows with (scale, bias); pass the same pointers for tied norms and four NULLs for
+ * norm=False (values only copied / converted).  Any D % 4 == 0; channels-first stores are 16 bytes wide where a channel
+ * plane's byte stride and base allow it, narrower otherwise.  Alignment (else D3_ERR_ARG): X and the norm vectors 16
+ * bytes; cls, storage and channels-last patches 16 (fp32) / 8 (bf16) bytes; channels-first patches one element.      */
+int d3_layernorm_tokens_out(const float* X, const float* scale, const float* bias, const float* pre_scale,
+                            const float* pre_bias, float eps, int n, int N, int R, int Hp, int Wp, int D, void* cls,
+                            void* storage, void* patches, int out_f32, int channels_first, void* stream);
 /* LayerNorm backward: dx = LN'(dy) (+ dx_add), dscale += colsum(dy * xhat), dbias += colsum(dy); with ls_gamma == NULL
  * that is all it does (the plain LayerNorm backward).  With ls_gamma it is fused with the LayerScale (+GELU) backward
  * of the branch upstream of it (layers/block.py:198-199 x_out = x_in + gamma * act(u); layers/layer_scale.py:17-21):
