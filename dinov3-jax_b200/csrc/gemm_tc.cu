@@ -578,7 +578,8 @@ static int dispatch(int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap
     const int f = ep.flags & EPI_FLAGS;
 #define D3_EPI(A, B, F) \
     if (a_mn == A && b_mn == B && f == (F)) return launch<BN, A, B, (F)>(ta, tb, ep, M, N, K, splits, s);
-    // forward: qkv, patch embedding and head layers, fc1, proj, fc2, prototype logits
+    // forward: qkv, patch embedding and head layers, fc1, proj, fc2, prototype logits; qkv without a bias (vit_7b)
+    D3_EPI(0, 1, 0)
     D3_EPI(0, 1, EP_BIAS)
     D3_EPI(0, 1, EP_BIAS | EP_OUT_F32)
     D3_EPI(0, 1, EP_BIAS | EP_GELU)

@@ -48,6 +48,7 @@ DEFAULTS = {
               "scaling_rule": "sqrt_wrt_1024", "patch_embed_lr_mult": 0.2, "dino_head_wd_multiplier": 1.0,
               "layerwise_decay": 0.9, "multi_tensor_optim": True, "adamw_beta1": 0.9, "adamw_beta2": 0.999},
     "checkpointing": {"period": 3750, "max_to_keep": 3},
+    "distillation": {"enabled": False, "full_cfg_path": "", "checkpoint_path": ""},   # ssl_default_config.yaml:130-133
 }
 
 

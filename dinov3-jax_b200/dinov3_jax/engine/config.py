@@ -18,6 +18,9 @@ ARCHS = {  # name -> (embed_dim, depth, heads)
 }
 # constructor defaults of a factory beyond the table (models/vision_transformer.py:400-408: vit_7b has ffn_ratio 3)
 ARCH_DEFAULTS = {"vit_7b": {"ffn_ratio": 3.0}}
+# student.ffn_layer -> (EngineConfig.ffn_layer, swiglu_align)   models/vision_transformer.py:30-36
+FFN_LAYERS = {"mlp": ("mlp", 8), "swiglu": ("swiglu", 8), "swiglu32": ("swiglu", 32), "swiglu64": ("swiglu", 64),
+              "swiglu128": ("swiglu", 128)}
 
 
 @dataclass(frozen=True)
@@ -52,6 +55,7 @@ class EngineConfig:
     ffn_layer: str = "mlp"           # "mlp" | "swiglu" (layers/ffn_layers.py:52-76; SURVEY 8f.1: the 7B recipe uses swiglu64)
     swiglu_align: int = 8            # swiglu / swiglu32 / swiglu64 / swiglu128 (models/vision_transformer.py:30-36)
     mask_k_bias: bool = False        # student.mask_k_bias: the k third of the qkv bias is masked to zero (upstream DINOv3)
+    qkv_bias: bool = True            # student.qkv_bias; false only for a frozen distillation teacher (the 7B recipes)
     layerwise_decay: float = 0.9
     patch_embed_lr_mult: float = 0.2
     dino_head_wd_multiplier: float = 1.0
@@ -136,8 +140,7 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
         raise NotImplementedError("ibot.separate_head must be true (ssl_meta_arch.py:48)")
     if cfg.crops.local_crops_number <= 0:
         raise ValueError("crops.local_crops_number must be > 0 (ssl_meta_arch.py:47)")
-    ffn_table = {"mlp": ("mlp", 8), "swiglu": ("swiglu", 8), "swiglu32": ("swiglu", 32), "swiglu64": ("swiglu", 64),
-                 "swiglu128": ("swiglu", 128)}                      # models/vision_transformer.py:30-36
+    ffn_table = FFN_LAYERS
     if cfg.student.ffn_layer not in ffn_table or cfg.student.norm_layer not in ("layernorm", "layernormbf16"):
         raise NotImplementedError("ffn_layer must be mlp | swiglu[32|64|128] and norm_layer layernorm | layernormbf16 "
                                   "(RMSNorm is not on the GPU path, SURVEY 8f)")
@@ -227,3 +230,56 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
         ffn_layer=ffn_table[cfg.student.ffn_layer][0], swiglu_align=ffn_table[cfg.student.ffn_layer][1],
         mask_k_bias=bool(cfg.student.get("mask_k_bias", False)),
         mlp_second_act=ffn_table[cfg.student.ffn_layer][0] == "mlp", **ibot_kw, **gram_kw)
+
+
+def distill_config_from_reference_cfg(cfg) -> EngineConfig | None:
+    """The frozen teacher of `distillation.enabled` (train/ssl_meta_arch.py:257-286), or None without distillation.
+
+    `distillation.full_cfg_path` is merged over the defaults like any run configuration, and its `student.*` block is
+    read the way `build_model_from_cfg(only_teacher=True)` reads it; the heads take its `dino.*` / `ibot.*` sizes.  The
+    teacher config's optim / schedules / crops / train blocks are ignored: the teacher is frozen and sees the student's
+    global crops."""
+    g = lambda node, key, default: node.get(key, default) if hasattr(node, "get") else getattr(node, key, default)
+    dist = g(cfg, "distillation", None)
+    if dist is None or not g(dist, "enabled", False):
+        return None
+    if cfg.gram.use_loss:
+        raise NotImplementedError("distillation together with gram.use_loss is not on the GPU path")
+    from ..configs.config import DinoV3SetupArgs, get_cfg_from_args
+    path = str(g(dist, "full_cfg_path", "") or "")
+    if not path:
+        raise ValueError("distillation.enabled needs distillation.full_cfg_path (the teacher's config)")
+    t = get_cfg_from_args(DinoV3SetupArgs(config_file=path))
+    # the reference's asserts (train/ssl_meta_arch.py:264-267)
+    if not t.ibot.separate_head:
+        raise ValueError("the distillation teacher needs ibot.separate_head: true (ssl_meta_arch.py:264)")
+    if t.ibot.head_n_prototypes != cfg.ibot.head_n_prototypes or t.dino.head_n_prototypes != cfg.dino.head_n_prototypes:
+        raise ValueError("the distillation teacher's dino / ibot head_n_prototypes must equal the student's "
+                         "(ssl_meta_arch.py:265-266)")
+    if t.student.patch_size != cfg.student.patch_size:
+        raise ValueError("the distillation teacher's patch_size must equal the student's (ssl_meta_arch.py:267)")
+    s = t.student
+    if s.arch not in ARCHS:
+        raise ValueError(f"unknown teacher student.arch {s.arch!r}")
+    if s.ffn_layer not in FFN_LAYERS or s.norm_layer not in ("layernorm", "layernormbf16"):
+        raise NotImplementedError("teacher ffn_layer must be mlp | swiglu[32|64|128] and norm_layer layernorm | layernormbf16")
+    if g(s, "untie_cls_and_patch_norms", False):
+        raise NotImplementedError("teacher student.untie_cls_and_patch_norms=true is not on the GPU path")
+    if not g(s, "proj_bias", True) or not g(s, "ffn_bias", True):
+        raise NotImplementedError("teacher student.proj_bias / ffn_bias = false is not on the GPU path")
+    if int(g(t.dino, "head_nlayers", 3)) != 3 or int(g(t.ibot, "head_nlayers", 3)) != 3:
+        raise NotImplementedError("teacher head_nlayers != 3 is not on the GPU path")
+    # untie_global_and_local_cls_norm is accepted: local_cls_norm applies only to local crops, which the teacher never
+    # sees (models/vision_transformer.py:224-226)
+    ibot_kw = {field: int(getattr(t.ibot, key)) for field, key in (("ibot_n_prototypes", "head_n_prototypes"),
+                                                                   ("ibot_head_hidden", "head_hidden_dim"),
+                                                                   ("ibot_head_bottleneck", "head_bottleneck_dim"))
+               if getattr(t.ibot, key) != getattr(t.dino, key)}
+    return config_for(
+        s.arch, patch=s.patch_size, ffn_ratio=s.ffn_ratio, global_size=cfg.crops.global_crops_size,
+        local_size=cfg.crops.local_crops_size, n_local=cfg.crops.local_crops_number,
+        n_prototypes=t.dino.head_n_prototypes, head_hidden=t.dino.head_hidden_dim, head_bottleneck=t.dino.head_bottleneck_dim,
+        layerscale=s.layerscale, rope_base=s.pos_embed_rope_base, n_storage=int(s.n_storage_tokens),
+        ln_eps=1e-5 if s.norm_layer == "layernormbf16" else 1e-6, ffn_layer=FFN_LAYERS[s.ffn_layer][0],
+        swiglu_align=FFN_LAYERS[s.ffn_layer][1], mask_k_bias=bool(g(s, "mask_k_bias", False)),
+        qkv_bias=bool(g(s, "qkv_bias", True)), mlp_second_act=FFN_LAYERS[s.ffn_layer][0] == "mlp", **ibot_kw)

@@ -16,7 +16,7 @@ import torch
 
 from .. import ops
 from .config import EngineConfig
-from .params import ParamStore
+from .params import FrozenStore, ParamStore, backbone_spec, head_spec
 
 f32, bf16 = torch.float32, torch.bfloat16
 
@@ -136,6 +136,19 @@ class SinkhornBufs:
         self.a = torch.empty(R, dtype=f32, device=device)
 
 
+class Net:
+    """What one forward pass reads: a model's configuration and its weights.  `mods` maps "backbone" / "dino_head" /
+    "ibot_head" to stores with w(name, teacher) / vec(name, teacher); `teacher` selects the EMA copy of a ParamStore.
+    `fsdp` gathers a unit before it is read; None when the weights are resident (a FrozenStore)."""
+
+    def __init__(self, cfg: EngineConfig, mods: dict, teacher: bool, fsdp=None):
+        self.cfg, self.mods, self.teacher, self.fsdp = cfg, mods, teacher, fsdp
+
+    def acquire(self, module: str, unit: str):
+        if self.fsdp is not None:
+            self.fsdp.acquire(module, unit, self.teacher)
+
+
 class Engine:
     """One rank's training engine: parameters, buffers and the step.
 
@@ -144,8 +157,26 @@ class Engine:
     """
 
     def __init__(self, cfg: EngineConfig, B: int, device="cuda", max_masked: int | None = None, comm=None,
-                 centering: str = "sinkhorn_knopp", center_momentum: float = 0.9, remat: bool = False):
-        assert cfg.head_dim in (64, 128), "attention kernels exist for head_dim 64 (ViT-S ... giant2) and 128 (vit_7b)"
+                 centering: str = "sinkhorn_knopp", center_momentum: float = 0.9, remat: bool = False,
+                 distill: EngineConfig | None = None):
+        """`distill`: the configuration of a frozen teacher of another architecture (distillation.enabled,
+        train/ssl_meta_arch.py:257-286).  It replaces the EMA teacher in the forward; the EMA of the student is still
+        kept in the teacher_* buffers.  Its weights come from `distill_teacher_load`."""
+        for c in (cfg, distill):
+            if c is not None:
+                assert c.head_dim in (64, 128), "attention kernels exist for head_dim 64 (ViT-S ... giant2) and 128 (vit_7b)"
+        if not cfg.qkv_bias:
+            raise NotImplementedError("a trained model without a qkv bias: qkv_bias=false is supported for a frozen "
+                                      "distillation teacher only")
+        if distill is not None:
+            if comm is not None:
+                raise NotImplementedError("distillation on more than one GPU")
+            if cfg.gram_use_loss:
+                raise NotImplementedError("distillation together with Gram anchoring")
+            if (distill.patch, distill.n_prototypes, distill.head_dims("ibot_head")[2]) != \
+                    (cfg.patch, cfg.n_prototypes, cfg.head_dims("ibot_head")[2]):
+                raise ValueError("the distillation teacher needs the student's patch size and prototype counts "
+                                 "(train/ssl_meta_arch.py:264-267)")
         if cfg.embed_dim > 1536:
             raise NotImplementedError(f"embed_dim {cfg.embed_dim}: the LayerNorm backward (d3_layernorm_bwd_ls) takes rows of "
                                       "at most 1536 columns, so training stops at ViT-giant2 width; vit_7b (4096) runs "
@@ -168,12 +199,22 @@ class Engine:
         from ..fsdp.runtime import FsdpRuntime
         self.fsdp = FsdpRuntime(comm, self.params.mods, dev)
         self.params.runtime = self.fsdp
+        self.distill = distill
+        self.student_net = Net(cfg, self.params.mods, False, self.fsdp)
+        self.ema_net = Net(cfg, self.params.mods, True, self.fsdp)
+        if distill is None:
+            self.t_net = self.ema_net
+        else:
+            self.t_net = Net(distill, {"backbone": FrozenStore(backbone_spec(distill), dev),
+                                       "dino_head": FrozenStore(head_spec(distill, "dino_head"), dev),
+                                       "ibot_head": FrozenStore(head_spec(distill, "ibot_head"), dev)}, True)
+        tcfg = self.t_net.cfg
         ng, nl = cfg.n_global * B, cfg.n_local * B
-        # teacher stream: global crops only; student stream: global then local rows
-        self.t_sets = [CropSet(cfg, ng, cfg.global_size, 0, dev)]
+        # teacher stream: global crops only (at the teacher's width); student stream: global then local rows
+        self.t_sets = [CropSet(tcfg, ng, cfg.global_size, 0, dev)]
         self.s_sets = [CropSet(cfg, ng, cfg.global_size, 0, dev)]
         self.s_sets.append(CropSet(cfg, nl, cfg.local_size, self.s_sets[0].T, dev))
-        self.teacher = Stream(cfg, self.t_sets, dev, stash=False)
+        self.teacher = Stream(tcfg, self.t_sets, dev, stash=False)
         self.student = Stream(cfg, self.s_sets, dev, stash=True, remat=self.remat)
         P = self.s_sets[0].P
         if max_masked is None:
@@ -187,8 +228,8 @@ class Engine:
         self.Rc = ng + nl                         # student dino-head rows: concat(g_cls, l_cls)
         self.h_s_dino = HeadBufs(cfg, "dino_head", self.Rc, dev, stash=True)
         self.h_s_ibot = HeadBufs(cfg, "ibot_head", self.max_masked, dev, stash=True)
-        self.h_t_dino = HeadBufs(cfg, "dino_head", ng, dev, stash=False)
-        self.h_t_ibot = HeadBufs(cfg, "ibot_head", self.max_masked, dev, stash=False)
+        self.h_t_dino = HeadBufs(tcfg, "dino_head", ng, dev, stash=False)
+        self.h_t_ibot = HeadBufs(tcfg, "ibot_head", self.max_masked, dev, stash=False)
         self.sk_mx2 = torch.empty(Ks, dtype=f32, device=dev)
         self.sk_s2 = torch.zeros(Ks + 4, dtype=f32, device=dev)
         self.sk_btot_local = torch.zeros(4, dtype=f32, device=dev)
@@ -202,6 +243,8 @@ class Engine:
         self._colsum = torch.zeros(max(Kd, Ki), dtype=f32, device=dev)      # column sums of one head at a time
         i32 = torch.int32
         self.rows_masked_t = torch.empty(self.max_masked, dtype=i32, device=dev)
+        # the masked patches' rows in the teacher stream (another prefix when a distillation teacher has other storage tokens)
+        self.rows_masked_tt = self.rows_masked_t if distill is None else torch.empty(self.max_masked, dtype=i32, device=dev)
         self.rows_cls_t = torch.empty(ng, dtype=i32, device=dev)
         self.rows_cls_s = torch.empty(self.Rc, dtype=i32, device=dev)
         self.cls_f32 = torch.empty(self.Rc, D, dtype=f32, device=dev)     # student cls rows (fp32) for KoLeo
@@ -249,6 +292,23 @@ class Engine:
         self.masks_u8 = torch.zeros(ng, P, dtype=torch.uint8, device=dev)
         self.mask_idx = torch.zeros(self.max_masked, dtype=torch.int64, device=dev)
         self.M = 0
+
+    # ------------------------------------------------------------------------------------------------ distillation
+    def distill_teacher_load(self, tree: dict):
+        """Weights of the frozen distillation teacher: {"backbone", "dino_head", "ibot_head"} trees (nested dicts or
+        flat '/'-joined names) with the reference's names and layouts, e.g. the teacher_* subtrees of a checkpoint.
+        `attn/qkv/bias` is expected exactly when the teacher has a qkv bias."""
+        if self.distill is None:
+            raise ValueError("distill_teacher_load: the engine was built without a distillation teacher")
+        from ..checkpointer import flat_from_tree
+        for m in ("dino_head", "ibot_head"):
+            if m not in tree:
+                raise ValueError(f"distillation teacher without its {m}: the teacher's DINO and iBOT heads produce the "
+                                 "targets, so backbone weights alone (e.g. torch-hub weights) cannot drive distillation")
+        if "backbone" not in tree:
+            raise ValueError("distillation teacher without its backbone")
+        for m, store in self.t_net.mods.items():
+            store.load(flat_from_tree(tree[m]), self.distill.mask_k_bias)
 
     # ------------------------------------------------------------------------------------------------ Gram anchoring
     def _init_gram(self):
@@ -379,7 +439,7 @@ class Engine:
             keep = (bb.t_bf16, bb.t_vecs)
             bb.t_bf16, bb.t_vecs = bb.g_bf16, bb.g_vecs
             try:
-                self._backbone_fwd(self.gram_stream if hi else T_, [self.gram_img if hi else self.g_img], [None], teacher=True)
+                self._backbone_fwd(self.ema_net, self.gram_stream if hi else T_, [self.gram_img if hi else self.g_img], [None])
             finally:
                 bb.t_bf16, bb.t_vecs = keep
             if hi:
@@ -425,7 +485,7 @@ class Engine:
     # ------------------------------------------------------------------------------------------------ static tables
     def _build_rows(self):
         sg, sl = self.s_sets
-        ops.token_rows(None, self.rows_cls_t, self.t_sets[0].n, self.t_sets[0].P, 1, prefix=self.cfg.prefix)
+        ops.token_rows(None, self.rows_cls_t, self.t_sets[0].n, self.t_sets[0].P, 1, prefix=self.t_net.cfg.prefix)
         # student cls rows: global crops then local crops (local rows offset by the global part)
         rows_g = torch.arange(sg.n, dtype=torch.int32) * sg.N
         rows_l = torch.arange(sl.n, dtype=torch.int32) * sl.N + sl.row0
@@ -466,9 +526,9 @@ class Engine:
                         torch.full((Mx,), 3, dtype=torch.int32, device=dev))
 
     # ------------------------------------------------------------------------------------------------ forward pieces
-    def _embed(self, st: Stream, images, masks_list, teacher: bool):
-        cfg, bb = self.cfg, self.params.mods["backbone"]
-        self.fsdp.acquire("backbone", "embed", teacher)
+    def _embed(self, net: Net, st: Stream, images, masks_list):
+        cfg, bb, teacher = net.cfg, net.mods["backbone"], net.teacher
+        net.acquire("backbone", "embed")
         X0 = st.x_in(0)
         Wpe = bb.w("patch_embed/proj/kernel", teacher)
         for cs, img, masks in zip(st.sets, images, masks_list):
@@ -478,10 +538,10 @@ class Engine:
                                 X0[cs.row0: cs.row0 + cs.T], cs.n, cs.P, cfg.embed_dim,
                                 storage=bb.vec("storage_tokens", teacher) if cfg.n_storage else None)
 
-    def _block_fwd(self, st: Stream, i: int, teacher: bool):
-        cfg, bb = self.cfg, self.params.mods["backbone"]
+    def _block_fwd(self, net: Net, st: Stream, i: int):
+        cfg, bb, teacher = net.cfg, net.mods["backbone"], net.teacher
         D, H = cfg.embed_dim, cfg.heads
-        self.fsdp.acquire("backbone", f"blocks_{i}", teacher)
+        net.acquire("backbone", f"blocks_{i}")
         p = f"blocks_{i}/"
         v = lambda n: bb.vec(p + n, teacher)
         w = lambda n: bb.w(p + n, teacher)
@@ -489,7 +549,7 @@ class Engine:
         Y, QKV, O, Z, Hh = st.b(st.Y, i), st.b(st.QKV, i), st.b(st.O, i), st.b(st.Z, i), st.b(st.Hh, i)
         stats = st.b(st.stats, i) if st.stash else [None] * 4
         ops.layernorm_fwd(X, v("norm1/scale"), v("norm1/bias"), Y, stats[0], stats[1], cfg.ln_eps)
-        ops.gemm(Y, w("attn/qkv/kernel"), QKV, b_mn=True, bias=v("attn/qkv/bias"))
+        ops.gemm(Y, w("attn/qkv/kernel"), QKV, b_mn=True, bias=v("attn/qkv/bias") if cfg.qkv_bias else None)
         lses = st.b(st.LSE, i)
         for cs, lse in zip(st.sets, lses):
             q = QKV[cs.row0: cs.row0 + cs.T]
@@ -512,22 +572,22 @@ class Engine:
         ops.gemm(Hh, w("mlp/Dense_1/kernel"), Xo, b_mn=True, bias=v("mlp/Dense_1/bias"), gelu=cfg.mlp_second_act,
                  store_pre=st.b(st.U2, i) if st.stash else None, gamma=v("ls2/gamma"), resid=Xmid)
 
-    def _backbone_fwd(self, st: Stream, images, masks_list, teacher: bool):
-        cfg, bb = self.cfg, self.params.mods["backbone"]
-        self._embed(st, images, masks_list, teacher)
+    def _backbone_fwd(self, net: Net, st: Stream, images, masks_list):
+        cfg, bb, teacher = net.cfg, net.mods["backbone"], net.teacher
+        self._embed(net, st, images, masks_list)
         for i in range(cfg.depth):
-            self._block_fwd(st, i, teacher)
+            self._block_fwd(net, st, i)
         XL = st.x_in(cfg.depth)
-        self.fsdp.acquire("backbone", "norm", teacher)
+        net.acquire("backbone", "norm")
         fs = st.fstats if st.stash else [None, None]
         ops.layernorm_fwd(XL, bb.vec("norm/scale", teacher), bb.vec("norm/bias", teacher), st.Xn, fs[0], fs[1], cfg.ln_eps)
 
-    def _head_fwd(self, hb: HeadBufs, module: str, R: int, teacher: bool, stash: bool):
-        hd = self.params.mods[module]
+    def _head_fwd(self, net: Net, hb: HeadBufs, module: str, R: int, stash: bool):
+        hd, teacher = net.mods[module], net.teacher
         w = lambda n: hd.w(n, teacher)
         v = lambda n: hd.vec(n, teacher)
         r = lambda t: t[:R]
-        self.fsdp.acquire(module, "head", teacher)
+        net.acquire(module, "head")
         if R == 0:
             return
         ops.gemm(r(hb.A0), w("mlp/layers_0/kernel"), r(hb.H1), b_mn=True, bias=v("mlp/layers_0/bias"), gelu=True,
@@ -647,7 +707,7 @@ class Engine:
             # recompute this block's forward from its stashed input (writes the scratch activations, statistics, LSE and
             # x_out again), then the LayerScale / activation backward of its MLP branch, which the stashing path gets
             # for free from the LayerNorm backward of the block above (_ls_tail)
-            self._block_fwd(st, i, teacher=False)
+            self._block_fwd(self.student_net, st, i)
             t = self._ls_tail(i)
             ops.ls_act_bwd(dX, t["ls_u"], t["ls_gamma"], t["ls_du"], t["ls_dgamma"], t["ls_dbias"], t["ls_gelu"])
 
@@ -744,7 +804,7 @@ class Engine:
         """(module, unit, teacher) in the order the step uses them: teacher pass, then student pass (student parameters
         stay gathered for the backward: SHARD_GRAD_OP, ssl_default_config.yaml:19)."""
         items = []
-        for teacher in (True, False):
+        for teacher in ((False,) if self.distill is not None else (True, False)):   # a distillation teacher is resident
             bb = self.params.mods["backbone"].layout
             items += [("backbone", u, teacher) for u in bb.units]
             for m in (("dino_head", "ibot_head") if teacher else ("dino_head", "ibot_head")):
@@ -769,6 +829,8 @@ class Engine:
         assert self.M <= self.max_masked, f"M={self.M} exceeds max_masked={self.max_masked}"
         self.mask_idx[: self.M].copy_(idx, non_blocking=True)
         ops.token_rows(self.mask_idx, self.rows_masked_t, self.M, self.s_sets[0].P, 0, prefix=self.cfg.prefix)
+        if self.distill is not None:
+            ops.token_rows(self.mask_idx, self.rows_masked_tt, self.M, self.s_sets[0].P, 0, prefix=self.distill.prefix)
         if self.cfg.gram_use_loss and self.cfg.gram_tokens_used != "all":
             # gram.tokens_used (train/ssl_meta_arch.py:221-223; upstream: student_patches[masks] / [~masks])
             n_all = self.gram_rows_all.numel()
@@ -778,6 +840,23 @@ class Engine:
                 # stable sort of the mask bits: unmasked patch positions first, in order (no host sync, count known)
                 order = torch.argsort(self.masks_u8.reshape(-1).to(torch.int16), stable=True)[: n_all - self.M]
                 self.gram_rows, self.gram_n = self.gram_rows_all[order].contiguous(), n_all - self.M
+
+    def teacher_pass(self, teacher_temp: float):
+        """Teacher forward over the global crops, its heads and the centering of its logits (train/ssl_meta_arch.py:366-402)."""
+        ng, M, T_ = self.cfg.n_global * self.B, self.M, self.teacher
+        Dt = self.t_net.cfg.embed_dim
+        self._backbone_fwd(self.t_net, T_, [self.g_img], [None])
+        ops.gather_rows(T_.Xn, self.rows_cls_t, ng, Dt, dst_bf16=self.h_t_dino.A0)
+        ops.gather_rows(T_.Xn, self.rows_masked_tt, M, Dt, dst_bf16=self.h_t_ibot.A0)
+        self._head_fwd(self.t_net, self.h_t_dino, "dino_head", ng, stash=False)
+        self._head_fwd(self.t_net, self.h_t_ibot, "ibot_head", M, stash=False)
+        if self.centering == "sinkhorn_knopp":
+            self._sinkhorn_pair(ng, M, teacher_temp)
+        else:
+            self._softmax_center(self.sk_dino, self.center_dino, self.h_t_dino.logits, ng, teacher_temp, ng)
+            self._softmax_center(self.sk_ibot, self.center_ibot, self.h_t_ibot.logits, M, teacher_temp, M)
+        if self.cfg.gram_use_loss:
+            self._gram_teacher_targets()
 
     def forward_backward(self, teacher_temp: float):
         cfg, B, M = self.cfg, self.B, self.M
@@ -790,40 +869,27 @@ class Engine:
         self.fsdp.prefetch(self._gather_schedule())
         # ---- teacher (train/ssl_meta_arch.py:366-402).  It shares nothing with the student pass until the losses, so
         # it runs on its own stream: the HBM-bound kernels of one pass overlap the tensor-bound kernels of the other.
-        T_ = self.teacher
-
-        def teacher_pass():
-            self._backbone_fwd(T_, [self.g_img], [None], teacher=True)
-            ops.gather_rows(T_.Xn, self.rows_cls_t, ng, D, dst_bf16=self.h_t_dino.A0)
-            ops.gather_rows(T_.Xn, self.rows_masked_t, M, D, dst_bf16=self.h_t_ibot.A0)
-            self._head_fwd(self.h_t_dino, "dino_head", ng, teacher=True, stash=False)
-            self._head_fwd(self.h_t_ibot, "ibot_head", M, teacher=True, stash=False)
-            if self.centering == "sinkhorn_knopp":
-                self._sinkhorn_pair(ng, M, teacher_temp)
-            else:
-                self._softmax_center(self.sk_dino, self.center_dino, self.h_t_dino.logits, ng, teacher_temp, ng)
-                self._softmax_center(self.sk_ibot, self.center_ibot, self.h_t_ibot.logits, M, teacher_temp, M)
-            if cfg.gram_use_loss:
-                self._gram_teacher_targets()
-
         if self.fwd_overlap:
             main = torch.cuda.current_stream()
             self._ev_fwd[0].record(main)
             self.tstream.wait_event(self._ev_fwd[0])          # batch, zeroed metrics, parameters of the last update
             with torch.cuda.stream(self.tstream):
-                teacher_pass()
+                self.teacher_pass(teacher_temp)
                 self._ev_fwd[1].record(self.tstream)
         else:
-            teacher_pass()
+            self.teacher_pass(teacher_temp)
         # ---- student (train/ssl_meta_arch.py:406-460)
         S_ = self.student
-        self._backbone_fwd(S_, [self.g_img, self.l_img], [self.masks_u8, None], teacher=False)
+        # a distilling student's global crops get no mask tokens (train/ssl_meta_arch.py:416); the iBOT loss is still
+        # taken at the masked positions
+        g_masks = self.masks_u8 if self.distill is None else None
+        self._backbone_fwd(self.student_net, S_, [self.g_img, self.l_img], [g_masks, None])
         ops.gather_rows(S_.Xn, self.rows_cls_s, self.Rc, D, dst_bf16=self.h_s_dino.A0, dst_f32=self.cls_f32)
         ops.gather_rows(S_.Xn, self.rows_masked_t, M, D, dst_bf16=self.h_s_ibot.A0)
         if self.gram_active:
             self._gram_features(S_.Xn, self.gram_fs, self.gram_xs, self.gram_nrm_s)
-        self._head_fwd(self.h_s_dino, "dino_head", self.Rc, teacher=False, stash=True)
-        self._head_fwd(self.h_s_ibot, "ibot_head", M, teacher=False, stash=True)
+        self._head_fwd(self.student_net, self.h_s_dino, "dino_head", self.Rc, stash=True)
+        self._head_fwd(self.student_net, self.h_s_ibot, "ibot_head", M, stash=True)
         # ---- losses + d(logits) (train/ssl_meta_arch.py:463-525)
         if self.fwd_overlap:
             torch.cuda.current_stream().wait_event(self._ev_fwd[1])      # teacher targets ready
@@ -865,7 +931,7 @@ class Engine:
         # ---- backward: token assembly + patch embedding
         dX0 = self.dX[cur]
         first = True
-        for cs, masks, dTok in zip(S_.sets, [self.masks_u8, None], self.dTok):
+        for cs, masks, dTok in zip(S_.sets, [g_masks, None], self.dTok):
             ops.assemble_tokens_bwd(dX0[cs.row0: cs.row0 + cs.T], masks, dTok, bb.gv("cls_token"),
                                     bb.gv("mask_token"), cs.n, cs.P, D,
                                     dstorage=bb.gv("storage_tokens") if cfg.n_storage else None)

@@ -34,8 +34,10 @@ def backbone_spec(cfg: EngineConfig):
     for i in range(cfg.depth):
         b = f"blocks_{i}/"
         spec += [(b + "norm1/scale", (D,), "vec"), (b + "norm1/bias", (D,), "vec"),
-                 (b + "attn/qkv/kernel", (D, 3 * D), "mat"), (b + "attn/qkv/bias", (3 * D,), "vec"),
-                 (b + "attn/proj/kernel", (D, D), "mat"), (b + "attn/proj/bias", (D,), "vec"),
+                 (b + "attn/qkv/kernel", (D, 3 * D), "mat")]
+        if cfg.qkv_bias:
+            spec += [(b + "attn/qkv/bias", (3 * D,), "vec")]
+        spec += [(b + "attn/proj/kernel", (D, D), "mat"), (b + "attn/proj/bias", (D,), "vec"),
                  (b + "ls1/gamma", (D,), "vec"),
                  (b + "norm2/scale", (D,), "vec"), (b + "norm2/bias", (D,), "vec")]
         if cfg.ffn_layer == "swiglu":                                 # layers/ffn_layers.py:62-69
@@ -87,6 +89,65 @@ def _round_up(x: int, a: int) -> int:
     return (x + a - 1) // a * a
 
 
+def flat_layout(spec):
+    """(offsets, shapes, kinds, padded sizes, n_mat, n) of `spec` in one flat buffer: matrices first, then vectors."""
+    offsets, shapes, kinds, padded = {}, {}, {}, {}
+    off = n_mat = 0
+    for kind in ("mat", "vec"):
+        for name, shape, k in spec:
+            if k != kind:
+                continue
+            offsets[name], shapes[name], kinds[name] = off, tuple(shape), k
+            padded[name] = _round_up(int(np.prod(shape)), ALIGN)
+            off += padded[name]
+        if kind == "mat":
+            n_mat = off
+    return offsets, shapes, kinds, padded, n_mat, off
+
+
+def _flat_view(flat, offset, shape, as2d):
+    v = flat[offset:offset + int(np.prod(shape))]
+    return v.view(-1, shape[-1]) if as2d else v.view(shape)
+
+
+class FrozenStore:
+    """A module that only runs forward (the frozen distillation teacher): the bf16 matrix region and the fp32 vector
+    region of `spec`'s layout, with no master, optimiser state or gradient.  `w` / `vec` take the `teacher` argument
+    of ModuleStore's and ignore it, so the forward pieces read either store."""
+
+    def __init__(self, spec, device):
+        self.offsets, self.shapes, _, _, self.n_mat, self.n = flat_layout(spec)
+        self.bf16 = torch.zeros(self.n_mat, dtype=torch.bfloat16, device=device)
+        self.vecs = torch.zeros(self.n - self.n_mat, dtype=torch.float32, device=device)
+
+    def w(self, name, teacher=True):
+        return _flat_view(self.bf16, self.offsets[name], self.shapes[name], True)
+
+    def vec(self, name, teacher=True):
+        return _flat_view(self.vecs, self.offsets[name] - self.n_mat, self.shapes[name], False).reshape(-1)
+
+    def load(self, tensors: dict, mask_k_bias: bool):
+        """tensors: name -> array (reference layout).  Matrices are rounded to bf16 one tensor at a time (d3_cast_f32_bf16,
+        the rounding of ModuleStore.refresh_bf16), so no fp32 copy of the whole module is held on the device."""
+        missing = [n for n in self.offsets if n not in tensors]
+        extra = [n for n in tensors if n not in self.offsets]
+        if missing or extra:
+            raise KeyError(f"teacher tensors do not match the configuration: missing {missing[:4]}, unexpected {extra[:4]}")
+        dev = self.bf16.device
+        for name, off in self.offsets.items():
+            src = torch.as_tensor(tensors[name]).to(device=dev, dtype=torch.float32).reshape(-1).contiguous()
+            if src.numel() != int(np.prod(self.shapes[name])):
+                raise ValueError(f"teacher tensor {name}: {src.numel()} elements, expected shape {self.shapes[name]}")
+            if off < self.n_mat:
+                ops.cast_f32_bf16(src, self.bf16[off:off + src.numel()])
+            else:
+                dst = self.vecs[off - self.n_mat:off - self.n_mat + src.numel()]
+                dst.copy_(src)
+                if mask_k_bias and name.endswith("attn/qkv/bias"):
+                    third = src.numel() // 3
+                    dst[third:2 * third].zero_()
+
+
 class ModuleStore:
     """Flat buffers of one top-level module on one rank.
 
@@ -100,20 +161,7 @@ class ModuleStore:
         from ..fsdp.layout import ShardLayout
         self.module, self.spec, self.cfg = module, spec, cfg
         self.world, self.rank = world, rank
-        self.offsets, self.shapes, self.kinds, padded = {}, {}, {}, {}
-        off = 0
-        for kind in ("mat", "vec"):
-            for name, shape, k in spec:
-                if k != kind:
-                    continue
-                self.offsets[name] = off
-                self.shapes[name] = tuple(shape)
-                self.kinds[name] = k
-                padded[name] = _round_up(int(np.prod(shape)), ALIGN)
-                off += padded[name]
-            if kind == "mat":
-                self.n_mat = off
-        self.n = off
+        self.offsets, self.shapes, self.kinds, padded, self.n_mat, self.n = flat_layout(spec)
         names_in_order = [name for name, _, _ in spec]
         self.layout = L = ShardLayout(module, names_in_order, self.offsets, padded, self.kinds, self.n_mat, self.n, world)
         f32, bf16 = torch.float32, torch.bfloat16

@@ -6,7 +6,7 @@ configuration and builds the GPU step executor.  The top-level parameter keys (`
 """
 from __future__ import annotations
 
-from ..engine import Engine, config_from_reference_cfg
+from ..engine import Engine, config_from_reference_cfg, distill_config_from_reference_cfg
 from ..engine.params import lr_wd_multipliers
 
 
@@ -16,6 +16,9 @@ class SSLMetaArch:
     def __init__(self, config):
         self.config = config
         self.engine_config = config_from_reference_cfg(config)       # raises on options the reference asserts on (:47-51)
+        # distillation.enabled (:257-286): the frozen teacher's configuration, None without distillation
+        self.distill_config = distill_config_from_reference_cfg(config)
+        self.is_distillation_enabled = self.distill_config is not None
         self.n_local_crops = config.crops.local_crops_number
         self.embed_dim = self.engine_config.embed_dim
         self.dino_out_dim = config.dino.head_n_prototypes
@@ -47,8 +50,20 @@ class SSLMetaArch:
         # train.checkpointing (ssl_default_config.yaml:88-89): activation rematerialisation of the student blocks
         remat = bool(self.config.train.get("checkpointing", False) or self.config.train.get("checkpointing_full", False))
         self.engine = Engine(self.engine_config, self.config.train.batch_size_per_gpu, device=device,
-                             max_masked=max_masked, comm=comm, remat=remat)
+                             max_masked=max_masked, comm=comm, remat=remat, distill=self.distill_config)
+        if self.distill_config is not None:
+            self.load_distillation_teacher(self.config.distillation.checkpoint_path)
         return self.engine
+
+    def load_distillation_teacher(self, checkpoint_path):
+        """The frozen teacher from a directory written by `checkpointer.save_checkpoint`: its teacher_* subtrees, the
+        EMA teacher of the run being distilled.  It is not part of the training state, so every build (a resume
+        included) loads it again."""
+        from ..checkpointer import load_checkpoint
+        if not checkpoint_path:
+            raise ValueError("distillation.enabled needs distillation.checkpoint_path (a save_checkpoint directory)")
+        params = load_checkpoint(checkpoint_path)["model_params"]
+        self.engine.distill_teacher_load({m: params[f"teacher_{m}"] for m in self.PARAM_MODULES if f"teacher_{m}" in params})
 
     def __call__(self, data, *, teacher_temp=0, iteration=0, deterministic=True, init_phase=False):
         """Forward + backward of one batch (the reference returns (loss, metrics) and lets jax.grad differentiate it,
