@@ -143,7 +143,7 @@ int d3_gemm_bf16(const void* A, int lda, int a_major, const void* B, int ldb, in
   g.aux_in = reinterpret_cast<const __nv_bfloat16*>(ep->aux_in);
   g.aux_out = reinterpret_cast<__nv_bfloat16*>(ep->aux_out);
   g.out = ep->out; g.ld_out = ep->ld_out; g.ld_aux = ep->ld_aux; g.ld_resid = ep->ld_resid;
-  g.flags = ep->flags & 0x1FF; g.alpha = ep->alpha;
+  g.flags = ep->flags & 0x3FF; g.alpha = ep->alpha;
   for (int i = 0; i < 8; ++i) g.sc_peer[i] = ep->sc_peer[i];
   g.sc_off = ep->sc_off; g.sc_shard = ep->sc_shard; g.sc_world = ep->sc_world;
   if (g.flags & EP_SCATTER)

@@ -19,6 +19,7 @@ enum : int {
   EP_OUT_F32 = D3_EP_OUT_F32,
   EP_ACCUM = D3_EP_ACCUM,
   EP_SCATTER = D3_EP_SCATTER,
+  EP_GELU_ERF = D3_EP_GELU_ERF,
   EP_SLOW = 1 << 30,      // internal: force the bounds-checked scalar epilogue
   EP_SLABS = 1 << 27,     // internal: split-K slice s stores its partial tile at rows [s*M, s*M + M) of `out`
 };

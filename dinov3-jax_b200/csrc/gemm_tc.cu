@@ -7,7 +7,8 @@
 //   dinov3_jax/layers/attention.py:63-65,94,101   dinov3_jax/layers/ffn_layers.py:36-47
 //   dinov3_jax/layers/patch_embed.py:38-51        dinov3_jax/layers/dino_head.py:20-43,65-85
 // The epilogue fuses bias, tanh-GELU, GELU', LayerScale (gamma) and the residual add
-// (dinov3_jax/layers/block.py:198-199, dinov3_jax/layers/layer_scale.py:17-21).
+// (dinov3_jax/layers/block.py:198-199, dinov3_jax/layers/layer_scale.py:17-21), and the exact (erf) GELU of the
+// ConvNeXt block's first pointwise layer (dinov3_jax/models/convnext.py:70-72).
 //
 // One kernel, 128 x {64,128} output tiles, 384 threads, launched in clusters of 2 CTAs that compute the tiles (m0, n0)
 // and (m0, n0 + BN) of a pair side by side, over the same k-blocks (128 x 256 tiles: see below):
@@ -56,7 +57,7 @@ constexpr int GEMM_THREADS = 384;
 // a fixed flag set gives the bits of the run-time flags.
 constexpr int EPI_RUNTIME = -1;
 constexpr int EPI_FLAGS = EP_BIAS | EP_GELU | EP_STORE_PRE | EP_MUL_DGELU | EP_GAMMA | EP_RESID | EP_OUT_F32 | EP_ACCUM |
-                          EP_SLABS;
+                          EP_SLABS | EP_GELU_ERF;
 
 // The epilogue stores through shared memory: every fixed flag set but the weight gradients' (split-K slabs, ACCUM),
 // whose main loop runs over all tokens and so hides a register-store epilogue, and which keep the deeper ring.
@@ -79,9 +80,15 @@ __device__ __forceinline__ float gelu_grad_epi(float u) {
   return fmaf(__fmul_rn(__fmul_rn(0.5f, u), fmaf(-t, t, 1.0f)), dz, __fmul_rn(0.5f, __fadd_rn(1.0f, t)));
 }
 
-// alpha, bias, GELU, GELU' (of the bf16 pre-activation u), gamma, residual, accumulate (old: the fp32 `out`), in this
-// order; the operands of flags that are not set are ignored.  `pre` receives the value before the activation
-// (EP_STORE_PRE).  GELU and GELU' use the hardware tanh (rel. error 2^-11, below the bf16 rounding of the GEMM operands).
+// the exact GELU 0.5 u (1 + erf(u / sqrt 2)) (torch nn.GELU(), the ConvNeXt block), each step rounded on its own
+__device__ __forceinline__ float gelu_erf_epi(float u) {
+  return __fmul_rn(__fmul_rn(0.5f, u), __fadd_rn(1.0f, erff(__fmul_rn(u, 0.70710678118654752f))));
+}
+
+// alpha, bias, GELU (tanh or erf), GELU' (of the bf16 pre-activation u), gamma, residual, accumulate (old: the fp32
+// `out`), in this order; the operands of flags that are not set are ignored.  `pre` receives the value before the
+// activation (EP_STORE_PRE).  The tanh-GELU and GELU' use the hardware tanh (rel. error 2^-11, below the bf16 rounding
+// of the GEMM operands).
 template <int EF>
 __device__ __forceinline__ float epi_value(const GemmEpilogue& ep, float acc, float bias, float u, float gamma,
                                            float resid, float old, float& pre) {
@@ -89,6 +96,7 @@ __device__ __forceinline__ float epi_value(const GemmEpilogue& ep, float acc, fl
   if (epi_has<EF>(ep, EP_BIAS)) v = __fadd_rn(v, bias);
   pre = v;
   if (epi_has<EF>(ep, EP_GELU)) v = gelu_tanh_fast(v);
+  if (epi_has<EF>(ep, EP_GELU_ERF)) v = gelu_erf_epi(v);
   if (epi_has<EF>(ep, EP_MUL_DGELU)) v = __fmul_rn(v, gelu_grad_epi(u));
   if (epi_has<EF>(ep, EP_GAMMA)) v = __fmul_rn(v, gamma);
   if (epi_has<EF>(ep, EP_RESID)) v = __fadd_rn(v, resid);
@@ -589,6 +597,8 @@ static int dispatch(int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap
     D3_EPI(0, 1, EP_BIAS | EP_GELU | EP_GAMMA | EP_RESID | EP_OUT_F32)
     D3_EPI(0, 1, EP_BIAS | EP_GELU | EP_STORE_PRE | EP_GAMMA | EP_RESID | EP_OUT_F32)
     D3_EPI(0, 1, EP_OUT_F32)
+    // ConvNeXt pwconv1 (the exact GELU); its pwconv2 is the bias + gamma + residual instance above
+    D3_EPI(0, 1, EP_BIAS | EP_GELU_ERF)
     // input gradients
     D3_EPI(0, 0, 0)
     D3_EPI(0, 0, EP_MUL_DGELU)
@@ -637,7 +647,7 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
   // ---- split-K: only for plain fp32 outputs (weight gradients) accumulated into (EP_ACCUM); every slice stores its
   //      partial tile into a workspace and the slices are added to out in slice order (reproducible bit for bit)
   const bool plain_f32 = (ep.flags & EP_OUT_F32) && !(ep.flags & (EP_BIAS | EP_GELU | EP_STORE_PRE | EP_MUL_DGELU |
-                                                                  EP_GAMMA | EP_RESID));
+                                                                  EP_GAMMA | EP_RESID | EP_GELU_ERF));
   int splits = 1;
   if (split_k >= 1) {
     splits = split_k;

@@ -19,7 +19,7 @@ LIB_PATH = PKG_ROOT / "libdinov3_b200.so"
 
 # epilogue flags (include/dinov3_b200.h)
 EP_BIAS, EP_GELU, EP_STORE_PRE, EP_MUL_DGELU, EP_GAMMA, EP_RESID, EP_OUT_F32, EP_ACCUM = 1, 2, 4, 8, 16, 32, 64, 128
-EP_SCATTER = 256
+EP_SCATTER, EP_GELU_ERF = 256, 512
 
 
 class NativeError(RuntimeError):
@@ -72,6 +72,10 @@ SIGNATURES = {
     "d3_ce_fwd_bwd": [P, F, P, P, F, P, P, P, P, P, P, P, P, P, P, I, I, P],
     "d3_gram_diff": [P, P, P, LL, I, F, P, I, I, P],
     "d3_resize_tokens_bicubic": [P, P, I, I, I, I, I, I, I, P],
+    "d3_dwconv7_layernorm": [P, P, P, P, P, F, P, I, I, I, I, P],
+    "d3_layernorm_patchify2": [P, P, P, F, P, I, I, I, I, P],
+    "d3_pool_tokens": [P, P, I, I, I, I, I, P],
+    "d3_resize_tokens_bilinear_aa": [P, P, I, I, I, I, I, I, I, P],
     "d3_koleo_fwd_bwd_rows": [P, P, P, P, P, P, P, I, I, I, I, F, F, F, P],
     "d3_aug_resized_crop": [P, I, I, I, P, I, P, I, P],
     "d3_aug_color": [P, P, I, I, P, P],

@@ -284,7 +284,48 @@ def to_torch_hub_state_dict(backbone_tree: dict) -> dict:
     return out
 
 
+def convert_convnext_torch_hub_state_dict(state_dict: dict) -> dict:
+    """Meta's PyTorch DINOv3 ConvNeXt state dict -> the reference's ConvNeXt params tree (models/convnext.py:155-206).
+
+    `downsample_layers.i.j.` -> `downsample_layers_i/layers_j/`, `stages.i.j.` -> `stages_i/layers_j/`.  Conv weights
+    [O, I, kh, kw] -> HWIO `kernel` (the depthwise [C, 1, 7, 7] -> [7, 7, 1, C]); Linear `weight` [out, in] -> `kernel`
+    [in, out]; the blocks' and downsampling layers' LayerNorms keep `weight` / `bias` (the reference's own LayerNorm), the
+    final `norm.weight` becomes `scale` (flax nn.LayerNorm).  `norms.3.*`, upstream's alias of the final norm, is dropped."""
+    params = {}
+    for tk, v in state_dict.items():
+        if tk.startswith("norms."):
+            continue
+        v = v.detach().cpu() if torch.is_tensor(v) else torch.as_tensor(v)
+        parts = tk.split(".")
+        if parts[-1] == "weight" and v.dim() >= 2:
+            parts[-1] = "kernel"
+            v = v.permute(2, 3, 1, 0) if v.dim() == 4 else v.t()
+        elif parts == ["norm", "weight"]:
+            parts[-1] = "scale"
+        jk = re.sub(r"^(downsample_layers|stages)\.(\d+)\.(\d+)\.", r"\1_\2/layers_\3/", ".".join(parts))
+        params[jk.replace(".", "/")] = v.contiguous()
+    return tree_from_flat(params)
+
+
+def to_convnext_torch_hub_state_dict(tree: dict) -> dict:
+    """Inverse of convert_convnext_torch_hub_state_dict, with upstream's `norms.3.*` alias of the final norm, so the
+    result loads strictly into upstream's module."""
+    out = {}
+    for k, v in flat_from_tree(tree).items():
+        parts = k.split("/")
+        if parts[-1] == "kernel":
+            parts[-1] = "weight"
+            v = v.permute(3, 2, 0, 1) if v.dim() == 4 else v.t()
+        elif parts[-1] == "scale":
+            parts[-1] = "weight"
+        tk = re.sub(r"^(downsample_layers|stages)_(\d+)\.layers_(\d+)\.", r"\1.\2.\3.", ".".join(parts))
+        out[tk] = v.contiguous()
+    for name in ("weight", "bias"):
+        out[f"norms.3.{name}"] = out[f"norm.{name}"].clone()
+    return out
+
+
 __all__ = ["CheckpointRetentionPolicy", "cleanup_checkpoint", "find_all_checkpoints", "find_latest_checkpoint",
            "keep_checkpoint_copy", "keep_last_n_checkpoints", "load_checkpoint", "save_checkpoint", "engine_state",
            "load_engine_state", "tree_from_flat", "flat_from_tree", "convert_torch_hub_state_dict",
-           "to_torch_hub_state_dict"]
+           "to_torch_hub_state_dict", "convert_convnext_torch_hub_state_dict", "to_convnext_torch_hub_state_dict"]

@@ -5,6 +5,7 @@ from __future__ import annotations
 from dataclasses import replace
 
 from ..engine.config import ARCHS, EngineConfig, config_for, config_from_reference_cfg
+from .convnext import ConvNeXt, convnext_sizes, get_convnext_arch
 from .vision_transformer import DinoVisionTransformer
 
 

@@ -24,13 +24,15 @@ def _ld(t: torch.Tensor) -> int:
 
 
 def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False,
-         bias: torch.Tensor | None = None, gelu: bool = False, store_pre: torch.Tensor | None = None,
+         bias: torch.Tensor | None = None, gelu: bool = False, gelu_erf: bool = False,
+         store_pre: torch.Tensor | None = None,
          dgelu_of: torch.Tensor | None = None, gamma: torch.Tensor | None = None,
          resid: torch.Tensor | None = None, accum: bool = False, alpha: float = 1.0, tile_n: int = 0,
          split_k: int = 0, scatter=None) -> torch.Tensor:
     """out[M,N] = epilogue(alpha * A.B) on the wgmma tensor cores (d3_gemm_bf16).
 
     A is [M,K] (a_mn=False) or stored transposed [K,M] (a_mn=True); B is [N,K] (b_mn=False) or [K,N] (b_mn=True).
+    gelu: the tanh-GELU of the ViT MLP; gelu_erf: the exact GELU (torch nn.GELU()) of the ConvNeXt block.
     """
     l = N.init()
     assert A.dtype == bf16 and B.dtype == bf16
@@ -48,6 +50,8 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, a_mn: bool = Fa
         flags |= N.EP_BIAS; ep.bias = bias.data_ptr()
     if gelu:
         flags |= N.EP_GELU
+    if gelu_erf:
+        flags |= N.EP_GELU_ERF
     if store_pre is not None:
         assert store_pre.dtype == bf16 and store_pre.shape == out.shape
         flags |= N.EP_STORE_PRE; ep.aux_out = store_pre.data_ptr(); ep.ld_aux = _ld(store_pre)
@@ -182,6 +186,49 @@ def resize_tokens_bicubic(src, dst, n, Hs, Ws, Hd, Wd, D, antialias: bool):
     assert src.numel() == n * Hs * Ws * D and dst.numel() == n * Hd * Wd * D
     N.check(N.init().d3_resize_tokens_bicubic(_p(src), _p(dst), n, Hs, Ws, Hd, Wd, D, int(bool(antialias)), _s()),
             "d3_resize_tokens_bicubic")
+
+
+def dwconv7_layernorm(X, w, wb, scale, bias, Y, eps=1e-6):
+    """ConvNeXt block head: Y bf16 [n*H*W, C] = LayerNorm(dwconv7x7(X) + wb) per pixel; X fp32 [n, H, W, C], w fp32
+    [49, C] (tap-major), zero padding 3 (d3_dwconv7_layernorm)."""
+    n, H, W, Cc = X.shape
+    assert X.dtype == f32 and X.is_contiguous() and Y.dtype == bf16 and Y.is_contiguous() and Y.shape == (n * H * W, Cc)
+    assert w.dtype == f32 and w.is_contiguous() and w.shape == (49, Cc)
+    N.check(N.init().d3_dwconv7_layernorm(_p(X), _p(w), _p(wb), _p(scale), _p(bias), float(eps), _p(Y), n, H, W, Cc, _s()),
+            "d3_dwconv7_layernorm")
+    return Y
+
+
+def layernorm_patchify2(X, scale, bias, Y, eps=1e-6):
+    """ConvNeXt downsampling: Y bf16 [n*H/2*W/2, 4C], column (kh*2 + kw)*C + c = LayerNorm(X[b, 2i+kh, 2j+kw])[c]
+    (d3_layernorm_patchify2), the operand of the 2x2 stride-2 conv GEMM."""
+    n, H, W, Cc = X.shape
+    assert X.dtype == f32 and X.is_contiguous() and Y.dtype == bf16 and Y.is_contiguous()
+    assert Y.shape == (n * (H // 2) * (W // 2), 4 * Cc)
+    N.check(N.init().d3_layernorm_patchify2(_p(X), _p(scale), _p(bias), float(eps), _p(Y), n, H, W, Cc, _s()),
+            "d3_layernorm_patchify2")
+    return Y
+
+
+def pool_tokens(X, out, copy_tokens: bool = True):
+    """out fp32 [n, rows, C]: row 0 = mean over the P rows of X [n, P, C] (fixed summation order); copy_tokens (rows ==
+    1 + P): rows 1..P = X (d3_pool_tokens)."""
+    n, P, Cc = X.shape
+    assert X.dtype == f32 and X.is_contiguous() and out.dtype == f32 and out.is_contiguous()
+    assert out.dim() == 3 and out.shape[0] == n and out.shape[2] == Cc
+    N.check(N.init().d3_pool_tokens(_p(X), _p(out), n, P, Cc, out.shape[1], int(bool(copy_tokens)), _s()), "d3_pool_tokens")
+    return out
+
+
+def resize_tokens_bilinear_aa(src, dst, Hd, Wd, prefix: int = 0):
+    """fp32 maps src [n, Hs, Ws, C] -> rows prefix .. prefix + Hd*Wd - 1 of dst [n, prefix + Hd*Wd, C]: torch's
+    F.interpolate(mode="bilinear", antialias=True) (d3_resize_tokens_bilinear_aa)."""
+    n, Hs, Ws, Cc = src.shape
+    assert src.dtype == f32 and dst.dtype == f32 and src.is_contiguous() and dst.is_contiguous()
+    assert dst.shape == (n, prefix + Hd * Wd, Cc)
+    N.check(N.init().d3_resize_tokens_bilinear_aa(_p(src), _p(dst), n, Hs, Ws, Hd, Wd, Cc, int(prefix), _s()),
+            "d3_resize_tokens_bilinear_aa")
+    return dst
 
 
 def allreduce_peers(peers, out, n, op="sum"):

@@ -38,8 +38,9 @@ void d3_reset_launch_count(void);
  *   b_major = 0: B stored [N][K] (row stride ldb)      b_major = 1: B stored [K][N]   (reference kernel layout [in,out])
  * Replaces nn.Dense / nn.Conv(stride=kernel) at layers/attention.py:63-65,94,101, layers/ffn_layers.py:36-47,
  * layers/patch_embed.py:38-51, layers/dino_head.py:20-43,65-85, and their jax.grad transposes (train/train.py:504-513).
- * Epilogue order: +bias -> [store bf16 pre-activation] -> [tanh-GELU] -> [* GELU'(aux_in)] -> [* gamma] -> [+ resid]
- *                 -> [+= out] -> store (bf16 or fp32).   (layers/block.py:198-199, layers/layer_scale.py:17-21)     */
+ * Epilogue order: +bias -> [store bf16 pre-activation] -> [tanh-GELU] -> [erf-GELU] -> [* GELU'(aux_in)] -> [* gamma]
+ *                 -> [+ resid] -> [+= out] -> store (bf16 or fp32).   (layers/block.py:198-199, layers/layer_scale.py:17-21,
+ *                 the ConvNeXt block's pwconv1 -> nn.GELU(), models/convnext.py:70-72)                               */
 enum {
   D3_EP_BIAS = 1,       /* v += bias[n]                       (fp32 [N]) */
   D3_EP_GELU = 2,       /* v = gelu_tanh(v)                   flax nn.gelu, approximate=True */
@@ -50,6 +51,7 @@ enum {
   D3_EP_OUT_F32 = 64,   /* out is fp32 (default bf16) */
   D3_EP_ACCUM = 128,    /* out += v (fp32 out only; weight-gradient accumulation over crop sets) */
   D3_EP_SCATTER = 256, /* add the result into peer-mapped shard slices (see d3_gemm_epilogue.sc_*) */
+  D3_EP_GELU_ERF = 512, /* v = 0.5 v (1 + erf(v / sqrt 2))  exact GELU (torch nn.GELU()), forward only */
 };
 typedef struct {
   const float* bias;
@@ -234,6 +236,32 @@ int d3_gram_diff(const float* Ss, const float* St, void* G_bf16, long long n_ele
  * [n, Hs, Ws, D] -> [n, Hd, Wd, D], torch's upsample_bicubic2d (antialias 0) / _upsample_bicubic2d_aa (1) arithmetic. */
 int d3_resize_tokens_bicubic(const float* src, float* dst, int n, int Hs, int Ws, int Hd, int Wd, int D, int antialias,
                              void* stream);
+
+/* ---- ConvNeXt backbone (models/convnext.py:45-335, upstream DINOv3's ConvNeXt; forward only) -----------------------
+ * A block is d3_dwconv7_layernorm -> d3_gemm_bf16 (pwconv1, D3_EP_BIAS | D3_EP_GELU_ERF, bf16 out) -> d3_gemm_bf16
+ * (pwconv2, D3_EP_BIAS | D3_EP_GAMMA | D3_EP_RESID | D3_EP_OUT_F32 into the residual stream).  The stem is d3_im2col
+ * (p = 4) + d3_gemm_bf16 + d3_layernorm_fwd; a downsampling layer is d3_layernorm_patchify2 + d3_gemm_bf16 (K = 4C).
+ * Every LayerNorm here has the statistics and arithmetic of d3_layernorm_fwd (the same bits on each pixel's row).
+ * d3_dwconv7_layernorm: Y = LayerNorm(dwconv7x7(X) + wb) per pixel; X fp32 NHWC [n, H, W, C] (zero padding 3 at every
+ * border, any H, W >= 1), w fp32 [49, C] tap-major (the HWIO kernel [7, 7, 1, C]), Y bf16 [n*H*W, C].  C % 8 == 0,
+ * C <= 1536.  Alignment: X, Y, scale, bias 16 bytes.                                                                */
+int d3_dwconv7_layernorm(const float* X, const float* w, const float* wb, const float* scale, const float* bias, float eps,
+                         void* Y_bf16, int n, int H, int W, int C, void* stream);
+/* Y bf16 [n * H/2 * W/2, 4C]: row (b, i, j), column (kh * 2 + kw) * C + c = LayerNorm(X[b, 2i + kh, 2j + kw])[c], the
+ * operand of the 2x2 stride-2 conv GEMM (HWIO kernel viewed as [4C, C']).  Even H, W; C % 4 == 0; X, scale, bias
+ * 16-byte, Y 8-byte aligned.                                                                                        */
+int d3_layernorm_patchify2(const float* X, const float* scale, const float* bias, float eps, void* Y_bf16, int n, int H,
+                           int W, int C, void* stream);
+/* out fp32 [n, rows, C]: row 0 of image b = mean over the P rows of X[b] ([n, P, C] fp32), summed in a fixed order (the
+ * same bits every run); copy_tokens (rows == 1 + P): rows 1..P = X[b].  Otherwise rows 1.. are left untouched (for
+ * d3_resize_tokens_bilinear_aa).  The result is the X of d3_layernorm_tokens_out with R = 0.  C % 4 == 0, 16-byte
+ * aligned.                                                                                                          */
+int d3_pool_tokens(const float* X, float* out, int n, int P, int C, int rows, int copy_tokens, void* stream);
+/* fp32 maps [n, Hs, Ws, C] -> rows prefix .. prefix + Hd*Wd - 1 of each image's [prefix + Hd*Wd, C] block of dst:
+ * torch F.interpolate(mode="bilinear", antialias=True, align_corners=False) arithmetic (models/convnext.py:256-261).
+ * Down-scaling factors up to 7; C % 4 == 0; 16-byte aligned.                                                        */
+int d3_resize_tokens_bilinear_aa(const float* src, float* dst, int n, int Hs, int Ws, int Hd, int Wd, int C, int prefix,
+                                 void* stream);
 
 /* ---- KoLeo (loss/koleo_loss.py:16-35), forward + backward: metric += w_metric * loss; dx += w_grad * dloss/dx ------
  * Only the rows [row0, row0+nrows) contribute loss terms (mean over nrows); neighbours are searched over all B rows.
