@@ -202,17 +202,17 @@ def engine_state(engine) -> dict:
     (count, mu, nu) over the student modules (train/train.py:95-106).  Under FSDP every rank calls this (collective
     all-gathers of the shards); rank 0 writes."""
     flat = {k: v.cpu() for k, v in engine.params.export_reference_tree("param").items()}
-    bb = engine.params.mods["backbone"]
-    if getattr(engine, "gram_active", False) and hasattr(bb, "g_bf16"):
+    gram = getattr(engine, "gram_net", None) if getattr(engine, "gram_active", False) else None
+    if gram is not None:
         # frozen gram teacher (gram.use_loss with its own backbone, SURVEY 8f.2; full copies on every rank): without it a
         # resumed run would train without the Gram term until the next scheduled refresh
-        full = torch.cat([bb.g_bf16.float(), bb.g_vecs])
-        flat.update({f"gram_backbone/{k}": v.cpu() for k, v in bb.export_full(full).items()})
+        full = torch.cat([gram.mods["backbone"].bf16.float(), gram.mods["backbone"].vecs])
+        flat.update({f"gram_backbone/{k}": v.cpu() for k, v in engine.params.mods["backbone"].export_full(full).items()})
     params = tree_from_flat(flat)
     mu = tree_from_flat({k: v.cpu() for k, v in engine.params.export_reference_tree("m").items()})
     nu = tree_from_flat({k: v.cpu() for k, v in engine.params.export_reference_tree("v").items()})
     opt = {"count": int(engine.step_count), "mu": mu, "nu": nu}
-    if getattr(engine, "gram_active", False) and hasattr(bb, "g_bf16"):
+    if gram is not None:
         opt["gram_updates"] = int(engine.gram_updates)
     if getattr(engine, "centering", "sinkhorn_knopp") != "sinkhorn_knopp":
         # "state" collection of the optional softmax-centering path (loss/dino_clstoken_loss.py:19-22)

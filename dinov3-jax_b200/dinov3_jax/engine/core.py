@@ -16,103 +16,11 @@ import torch
 
 from .. import ops
 from .config import EngineConfig
+from .forward import CropSet, HeadBufs, Net, Stream, backbone_fwd, block_fwd, head_fwd
+from .forward import rope_tables  # noqa: F401  (engine.core.rope_tables stays importable for existing callers)
 from .params import FrozenStore, ParamStore, backbone_spec, head_spec
 
 f32, bf16 = torch.float32, torch.bfloat16
-
-
-def rope_tables(Hp: int, Wp: int, head_dim: int, base: float, device):
-    """sin / cos [Hp*Wp, head_dim] fp32 — layers/rope_position_encoding.py:36-40,64-73,117-123 (normalize 'separate').
-    Host-side table construction (a few KB, once per crop size); the rotation itself is d3_rope."""
-    dt = torch.float64
-    periods = base ** (2.0 * torch.arange(head_dim // 4, dtype=dt) / (head_dim // 2))
-    ch = torch.arange(0.5, Hp, dtype=dt) / Hp
-    cw = torch.arange(0.5, Wp, dtype=dt) / Wp
-    coords = torch.stack(torch.meshgrid(ch, cw, indexing="ij"), dim=-1).reshape(-1, 2)
-    coords = 2.0 * coords - 1.0
-    ang = 2 * math.pi * coords[:, :, None] / periods[None, None, :]
-    ang = ang.reshape(ang.shape[0], -1)
-    ang = torch.cat([ang, ang], dim=-1)
-    # the reference computes the tables in fp32 (SURVEY A8); fp64 -> fp32 rounding differs by < 1 ulp
-    return (torch.sin(ang).to(f32).to(device).contiguous(), torch.cos(ang).to(f32).to(device).contiguous())
-
-
-class CropSet:
-    """Static geometry of one crop resolution inside a token stream."""
-
-    def __init__(self, cfg: EngineConfig, n_crops: int, size: int, row0: int, device):
-        self.n = n_crops
-        self.size = size
-        self.Hp = size // cfg.patch
-        self.P = self.Hp * self.Hp
-        self.N = self.P + cfg.prefix
-        self.T = n_crops * self.N
-        self.row0 = row0
-        self.sin, self.cos = rope_tables(self.Hp, self.Hp, cfg.head_dim, cfg.rope_base, device)
-        kdim = cfg.patch * cfg.patch * 3
-        kpad = (kdim + 7) // 8 * 8             # TMA needs 16-byte row strides (patch 14: 588 -> 592, padding zeroed)
-        self.patches = torch.empty(n_crops * self.P, kpad, dtype=bf16, device=device)[:, :kdim]
-        self.tok = torch.empty(n_crops * self.P, cfg.embed_dim, dtype=f32, device=device)
-        self.lse = None
-
-
-class Stream:
-    """Activation buffers of one network pass over a list of crop sets (teacher: global only; student: global+local)."""
-
-    def __init__(self, cfg: EngineConfig, sets, device, stash: bool, remat: bool = False):
-        D, Hd, L = cfg.embed_dim, cfg.ffn_width, cfg.depth
-        swiglu = cfg.ffn_layer == "swiglu"
-        self.sets = sets
-        self.T = sum(s.T for s in sets)
-        T = self.T
-        self.stash = stash                    # keep what the backward needs
-        self.per_block = stash and not remat  # ... for every block (False: one scratch set, blocks are recomputed)
-        nb = L if self.per_block else 1
-        e = lambda *shape, dt=bf16: torch.empty(*shape, dtype=dt, device=device)
-        self.X = [e(T, D, dt=f32) for _ in range(L + 1)] if stash else [e(T, D, dt=f32), e(T, D, dt=f32)]
-        self.Xmid = [e(T, D, dt=f32) for _ in range(nb)]
-        self.Y = [e(T, D) for _ in range(nb)]
-        self.QKV = [e(T, 3 * D) for _ in range(nb)]
-        self.O = [e(T, D) for _ in range(nb)]
-        self.Z = [e(T, D) for _ in range(nb)]
-        self.Hh = [e(T, Hd) for _ in range(nb)]
-        self.Xn = e(T, D, dt=f32)
-        self.X12 = e(T, 2 * Hd) if (swiglu and not stash) else None       # teacher pass: [x1 | x2] scratch
-        self.LSE = [[e(s.n, cfg.heads, s.N, dt=f32) for s in sets] for _ in range(nb)]
-        if stash:
-            self.U1 = [e(T, 2 * Hd if swiglu else Hd) for _ in range(nb)]   # mlp: u1; swiglu: [x1 | x2]
-            self.U2 = [e(T, D) for _ in range(nb)]
-            self.stats = [[e(T, dt=f32) for _ in range(4)] for _ in range(nb)]   # mean1, rstd1, mean2, rstd2
-            self.fstats = [e(T, dt=f32), e(T, dt=f32)]
-
-    def x_in(self, i):
-        return self.X[i] if self.stash else self.X[i % 2]
-
-    def x_out(self, i):
-        return self.X[i + 1] if self.stash else self.X[(i + 1) % 2]
-
-    def b(self, lst, i):
-        return lst[i] if self.per_block else lst[0]
-
-
-class HeadBufs:
-    def __init__(self, cfg: EngineConfig, module: str, R: int, device, stash: bool):
-        D = cfg.embed_dim
-        Hh, Bn, K = cfg.head_dims(module)
-        e = lambda *shape, dt=bf16: torch.empty(*shape, dtype=dt, device=device)
-        self.R = R
-        self.A0 = e(R, D)
-        self.H1, self.H2 = e(R, Hh), e(R, Hh)
-        self.U3 = e(R, Bn, dt=f32)
-        self.nrm = e(R, dt=f32)
-        self.Yn = e(R, Bn)
-        self.logits = e(R, K, dt=f32)
-        if stash:
-            self.Ua, self.Ub = e(R, Hh), e(R, Hh)
-            self.dS = e(R, K)
-            self.dYn, self.dU3 = e(R, Bn), e(R, Bn)
-            self.dUb, self.dUa = e(R, Hh), e(R, Hh)
-            self.dA0 = e(R, D, dt=f32)
 
 
 class SinkhornBufs:
@@ -134,19 +42,6 @@ class SinkhornBufs:
             self.btot = s2[Ks + slot:Ks + slot + 1]
         self.gmx = torch.empty(1, dtype=f32, device=device)
         self.a = torch.empty(R, dtype=f32, device=device)
-
-
-class Net:
-    """What one forward pass reads: a model's configuration and its weights.  `mods` maps "backbone" / "dino_head" /
-    "ibot_head" to stores with w(name, teacher) / vec(name, teacher); `teacher` selects the EMA copy of a ParamStore.
-    `fsdp` gathers a unit before it is read; None when the weights are resident (a FrozenStore)."""
-
-    def __init__(self, cfg: EngineConfig, mods: dict, teacher: bool, fsdp=None):
-        self.cfg, self.mods, self.teacher, self.fsdp = cfg, mods, teacher, fsdp
-
-    def acquire(self, module: str, unit: str):
-        if self.fsdp is not None:
-            self.fsdp.acquire(module, unit, self.teacher)
 
 
 class Engine:
@@ -201,9 +96,8 @@ class Engine:
         self.params.runtime = self.fsdp
         self.distill = distill
         self.student_net = Net(cfg, self.params.mods, False, self.fsdp)
-        self.ema_net = Net(cfg, self.params.mods, True, self.fsdp)
         if distill is None:
-            self.t_net = self.ema_net
+            self.t_net = Net(cfg, self.params.mods, True, self.fsdp)
         else:
             self.t_net = Net(distill, {"backbone": FrozenStore(backbone_spec(distill), dev),
                                        "dino_head": FrozenStore(head_spec(distill, "dino_head"), dev),
@@ -211,9 +105,10 @@ class Engine:
         tcfg = self.t_net.cfg
         ng, nl = cfg.n_global * B, cfg.n_local * B
         # teacher stream: global crops only (at the teacher's width); student stream: global then local rows
-        self.t_sets = [CropSet(tcfg, ng, cfg.global_size, 0, dev)]
-        self.s_sets = [CropSet(cfg, ng, cfg.global_size, 0, dev)]
-        self.s_sets.append(CropSet(cfg, nl, cfg.local_size, self.s_sets[0].T, dev))
+        gp, lp = cfg.global_size // cfg.patch, cfg.local_size // cfg.patch
+        self.t_sets = [CropSet(tcfg, ng, gp, gp, 0, dev)]
+        self.s_sets = [CropSet(cfg, ng, gp, gp, 0, dev)]
+        self.s_sets.append(CropSet(cfg, nl, lp, lp, self.s_sets[0].T, dev))
         self.teacher = Stream(tcfg, self.t_sets, dev, stash=False)
         self.student = Stream(cfg, self.s_sets, dev, stash=True, remat=self.remat)
         P = self.s_sets[0].P
@@ -322,7 +217,7 @@ class Engine:
         self._gram_w = float(cfg.gram_loss_weight)
         self._gram_snapshot_pending = False
         self.gram_updates = 0
-        self.gram_stream, self.gram_img = None, None
+        self.gram_stream, self.gram_img, self.gram_net = None, None, None
         if not cfg.gram_use_loss:
             return
         assert cfg.gram_tokens_used in ("all", "masked", "unmasked")         # train/ssl_meta_arch.py:221
@@ -349,16 +244,15 @@ class Engine:
         if cfg.gram_ema_teacher:
             self.gram_active = True
         else:
-            bb = self.params.mods["backbone"]
-            bb.g_bf16 = torch.zeros_like(bb.t_bf16)                          # frozen full copies on every rank
-            bb.g_vecs = torch.zeros(bb.n - bb.n_mat, dtype=f32, device=dev)
+            # frozen full copy on every rank, in the backbone's flat layout (the snapshot copies the EMA teacher's)
+            self.gram_net = Net(cfg, {"backbone": FrozenStore(backbone_spec(cfg), dev)}, True)
             gs = cfg.gram_teacher_size
             if gs is not None and gs != cfg.global_size and cfg.gram_tokens_used != "all":
                 raise NotImplementedError("gram.tokens_used masked | unmasked with a gram teacher at its own resolution")
             if gs is not None and gs != cfg.global_size:
                 # the gram teacher sees its own (larger) crops: a third token stream at that resolution; its patch tokens are
                 # resized to the student's grid before the similarity matrices (upstream get_gram_teacher_output)
-                self.g_sets = [CropSet(cfg, sg.n, gs, 0, dev)]
+                self.g_sets = [CropSet(cfg, sg.n, gs // cfg.patch, gs // cfg.patch, 0, dev)]
                 self.gram_stream = Stream(cfg, self.g_sets, dev, stash=False)
                 gp = self.g_sets[0]
                 self.gram_rows_hi = (torch.arange(gp.n, dtype=torch.int32)[:, None] * gp.N + cfg.prefix
@@ -375,15 +269,8 @@ class Engine:
         """Gram teacher weights from a checkpoint: `tensors` maps the backbone's tensor names (reference layout, e.g.
         'blocks_0/attn/qkv/kernel', as in export_reference_tree without the 'teacher_backbone/' prefix) to arrays."""
         assert self.cfg.gram_use_loss and not self.cfg.gram_ema_teacher
-        bb = self.params.mods["backbone"]
-        full = torch.zeros(bb.n, dtype=f32, device=self.device)
-        for name in bb.offsets:
-            bb._view(full, name).copy_(torch.as_tensor(tensors[name]).to(device=self.device, dtype=f32).reshape(bb.shapes[name]))
-            if self.cfg.mask_k_bias and name.endswith("attn/qkv/bias"):
-                third = bb.shapes[name][0] // 3
-                bb._view(full, name)[third:2 * third].zero_()
-        ops.cast_f32_bf16(full[:bb.n_mat].contiguous(), bb.g_bf16)
-        bb.g_vecs.copy_(full[bb.n_mat:])
+        store = self.gram_net.mods["backbone"]
+        store.load({name: tensors[name] for name in store.offsets}, self.cfg.mask_k_bias)
         self.gram_active = True
 
     def gram_schedule(self, iteration: int):
@@ -422,10 +309,10 @@ class Engine:
         """Called at the end of the teacher pass (the EMA teacher's outputs have been gathered into the head buffers)."""
         cfg, T_ = self.cfg, self.teacher
         if not cfg.gram_ema_teacher:
-            bb = self.params.mods["backbone"]
             if self._gram_snapshot_pending:
-                bb.g_bf16.copy_(bb.t_bf16)
-                bb.g_vecs.copy_(bb.t_vecs)
+                bb, g = self.params.mods["backbone"], self.gram_net.mods["backbone"]
+                g.bf16.copy_(bb.t_bf16)
+                g.vecs.copy_(bb.t_vecs)
                 self._gram_snapshot_pending = False
                 self.gram_active = True
             if not self.gram_active:
@@ -436,16 +323,11 @@ class Engine:
             if hi and self.gram_img is None:
                 raise ValueError("no gram teacher crops in the data, have you set cfg.crops.gram_teacher_crops_size? "
                                  "(train/ssl_meta_arch.py:310-313)")
-            keep = (bb.t_bf16, bb.t_vecs)
-            bb.t_bf16, bb.t_vecs = bb.g_bf16, bb.g_vecs
-            try:
-                self._backbone_fwd(self.ema_net, self.gram_stream if hi else T_, [self.gram_img if hi else self.g_img], [None])
-            finally:
-                bb.t_bf16, bb.t_vecs = keep
+            backbone_fwd(self.gram_net, self.gram_stream if hi else T_, [self.gram_img if hi else self.g_img], [None])
             if hi:
                 gp, sg, D = self.g_sets[0], self.s_sets[0], cfg.embed_dim
                 ops.gather_rows(self.gram_stream.Xn, self.gram_rows_hi, gp.n * gp.P, D, dst_f32=self.gram_hi)
-                ops.resize_tokens_bicubic(self.gram_hi, self.gram_ft[:sg.n * sg.P], gp.n, gp.Hp, gp.Hp, sg.Hp, sg.Hp, D,
+                ops.resize_tokens_bicubic(self.gram_hi, self.gram_ft[:sg.n * sg.P], gp.n, gp.Hp, gp.Wp, sg.Hp, sg.Wp, D,
                                           cfg.gram_resize_antialias)
                 n = self.gram_n                       # all patch tokens (a multiple of 8 is not guaranteed: pad with zero rows)
                 npad = (n + 7) // 8 * 8
@@ -524,79 +406,6 @@ class Engine:
         self.ce_ibot = (torch.arange(Mx, dtype=torch.int32, device=dev), torch.full((Mx,), -1, dtype=torch.int32, device=dev),
                         torch.full((Mx,), 1.0 / n_rows, device=dev), torch.full((Mx,), cfg.ibot_loss_weight / n_rows, device=dev),
                         torch.full((Mx,), 3, dtype=torch.int32, device=dev))
-
-    # ------------------------------------------------------------------------------------------------ forward pieces
-    def _embed(self, net: Net, st: Stream, images, masks_list):
-        cfg, bb, teacher = net.cfg, net.mods["backbone"], net.teacher
-        net.acquire("backbone", "embed")
-        X0 = st.x_in(0)
-        Wpe = bb.w("patch_embed/proj/kernel", teacher)
-        for cs, img, masks in zip(st.sets, images, masks_list):
-            ops.im2col(img, cs.patches, cfg.patch)
-            ops.gemm(cs.patches, Wpe, cs.tok, b_mn=True, bias=bb.vec("patch_embed/proj/bias", teacher))
-            ops.assemble_tokens(cs.tok, bb.vec("cls_token", teacher), bb.vec("mask_token", teacher), masks,
-                                X0[cs.row0: cs.row0 + cs.T], cs.n, cs.P, cfg.embed_dim,
-                                storage=bb.vec("storage_tokens", teacher) if cfg.n_storage else None)
-
-    def _block_fwd(self, net: Net, st: Stream, i: int):
-        cfg, bb, teacher = net.cfg, net.mods["backbone"], net.teacher
-        D, H = cfg.embed_dim, cfg.heads
-        net.acquire("backbone", f"blocks_{i}")
-        p = f"blocks_{i}/"
-        v = lambda n: bb.vec(p + n, teacher)
-        w = lambda n: bb.w(p + n, teacher)
-        X, Xmid, Xo = st.x_in(i), st.b(st.Xmid, i), st.x_out(i)
-        Y, QKV, O, Z, Hh = st.b(st.Y, i), st.b(st.QKV, i), st.b(st.O, i), st.b(st.Z, i), st.b(st.Hh, i)
-        stats = st.b(st.stats, i) if st.stash else [None] * 4
-        ops.layernorm_fwd(X, v("norm1/scale"), v("norm1/bias"), Y, stats[0], stats[1], cfg.ln_eps)
-        ops.gemm(Y, w("attn/qkv/kernel"), QKV, b_mn=True, bias=v("attn/qkv/bias") if cfg.qkv_bias else None)
-        lses = st.b(st.LSE, i)
-        for cs, lse in zip(st.sets, lses):
-            q = QKV[cs.row0: cs.row0 + cs.T]
-            ops.rope(q, cs.sin, cs.cos, cs.N, cfg.prefix, D, cfg.head_dim)
-            ops.attn_fwd(q, O[cs.row0: cs.row0 + cs.T], lse if st.stash else None, cs.n, cs.N, D, H)
-        ops.gemm(O, w("attn/proj/kernel"), Xmid, b_mn=True, bias=v("attn/proj/bias"), gamma=v("ls1/gamma"), resid=X)
-        ops.layernorm_fwd(Xmid, v("norm2/scale"), v("norm2/bias"), Z, stats[2], stats[3], cfg.ln_eps)
-        if cfg.ffn_layer == "swiglu":
-            # SwiGLUFFN (layers/ffn_layers.py:71-76): h = silu(z W1 + b1) * (z W2 + b2); x_out = x_mid + g2 * (h W3 + b3)
-            Hs = cfg.swiglu_hidden
-            X12 = st.b(st.U1, i) if st.stash else st.X12
-            ops.gemm(Z, w("mlp/w1/kernel"), X12[:, :Hs], b_mn=True, bias=v("mlp/w1/bias"))
-            ops.gemm(Z, w("mlp/w2/kernel"), X12[:, Hs:], b_mn=True, bias=v("mlp/w2/bias"))
-            ops.swiglu_fwd(X12, Hh)
-            ops.gemm(Hh, w("mlp/w3/kernel"), Xo, b_mn=True, bias=v("mlp/w3/bias"),
-                     store_pre=st.b(st.U2, i) if st.stash else None, gamma=v("ls2/gamma"), resid=Xmid)
-            return
-        ops.gemm(Z, w("mlp/Dense_0/kernel"), Hh, b_mn=True, bias=v("mlp/Dense_0/bias"), gelu=True,
-                 store_pre=st.b(st.U1, i) if st.stash else None)
-        ops.gemm(Hh, w("mlp/Dense_1/kernel"), Xo, b_mn=True, bias=v("mlp/Dense_1/bias"), gelu=cfg.mlp_second_act,
-                 store_pre=st.b(st.U2, i) if st.stash else None, gamma=v("ls2/gamma"), resid=Xmid)
-
-    def _backbone_fwd(self, net: Net, st: Stream, images, masks_list):
-        cfg, bb, teacher = net.cfg, net.mods["backbone"], net.teacher
-        self._embed(net, st, images, masks_list)
-        for i in range(cfg.depth):
-            self._block_fwd(net, st, i)
-        XL = st.x_in(cfg.depth)
-        net.acquire("backbone", "norm")
-        fs = st.fstats if st.stash else [None, None]
-        ops.layernorm_fwd(XL, bb.vec("norm/scale", teacher), bb.vec("norm/bias", teacher), st.Xn, fs[0], fs[1], cfg.ln_eps)
-
-    def _head_fwd(self, net: Net, hb: HeadBufs, module: str, R: int, stash: bool):
-        hd, teacher = net.mods[module], net.teacher
-        w = lambda n: hd.w(n, teacher)
-        v = lambda n: hd.vec(n, teacher)
-        r = lambda t: t[:R]
-        net.acquire(module, "head")
-        if R == 0:
-            return
-        ops.gemm(r(hb.A0), w("mlp/layers_0/kernel"), r(hb.H1), b_mn=True, bias=v("mlp/layers_0/bias"), gelu=True,
-                 store_pre=r(hb.Ua) if stash else None)
-        ops.gemm(r(hb.H1), w("mlp/layers_2/kernel"), r(hb.H2), b_mn=True, bias=v("mlp/layers_2/bias"), gelu=True,
-                 store_pre=r(hb.Ub) if stash else None)
-        ops.gemm(r(hb.H2), w("mlp/layers_4/kernel"), r(hb.U3), b_mn=True, bias=v("mlp/layers_4/bias"))
-        ops.l2norm_fwd(r(hb.U3), r(hb.Yn), r(hb.nrm), 1e-12)
-        ops.gemm(r(hb.Yn), w("last_layer/kernel"), r(hb.logits), b_mn=True)
 
     def _sinkhorn_pair(self, R_d: int, R_i: int, temp: float, n_iter: int = 3):
         """Both heads' Sinkhorn-Knopp normalisations (DINO cls logits, iBOT masked-patch logits) in lock step: the
@@ -707,7 +516,7 @@ class Engine:
             # recompute this block's forward from its stashed input (writes the scratch activations, statistics, LSE and
             # x_out again), then the LayerScale / activation backward of its MLP branch, which the stashing path gets
             # for free from the LayerNorm backward of the block above (_ls_tail)
-            self._block_fwd(self.student_net, st, i)
+            block_fwd(self.student_net, st, i)
             t = self._ls_tail(i)
             ops.ls_act_bwd(dX, t["ls_u"], t["ls_gamma"], t["ls_du"], t["ls_dgamma"], t["ls_dbias"], t["ls_gelu"])
 
@@ -845,11 +654,11 @@ class Engine:
         """Teacher forward over the global crops, its heads and the centering of its logits (train/ssl_meta_arch.py:366-402)."""
         ng, M, T_ = self.cfg.n_global * self.B, self.M, self.teacher
         Dt = self.t_net.cfg.embed_dim
-        self._backbone_fwd(self.t_net, T_, [self.g_img], [None])
+        backbone_fwd(self.t_net, T_, [self.g_img], [None])
         ops.gather_rows(T_.Xn, self.rows_cls_t, ng, Dt, dst_bf16=self.h_t_dino.A0)
         ops.gather_rows(T_.Xn, self.rows_masked_tt, M, Dt, dst_bf16=self.h_t_ibot.A0)
-        self._head_fwd(self.t_net, self.h_t_dino, "dino_head", ng, stash=False)
-        self._head_fwd(self.t_net, self.h_t_ibot, "ibot_head", M, stash=False)
+        head_fwd(self.t_net, self.h_t_dino, "dino_head", ng, stash=False)
+        head_fwd(self.t_net, self.h_t_ibot, "ibot_head", M, stash=False)
         if self.centering == "sinkhorn_knopp":
             self._sinkhorn_pair(ng, M, teacher_temp)
         else:
@@ -883,13 +692,13 @@ class Engine:
         # a distilling student's global crops get no mask tokens (train/ssl_meta_arch.py:416); the iBOT loss is still
         # taken at the masked positions
         g_masks = self.masks_u8 if self.distill is None else None
-        self._backbone_fwd(self.student_net, S_, [self.g_img, self.l_img], [g_masks, None])
+        backbone_fwd(self.student_net, S_, [self.g_img, self.l_img], [g_masks, None])
         ops.gather_rows(S_.Xn, self.rows_cls_s, self.Rc, D, dst_bf16=self.h_s_dino.A0, dst_f32=self.cls_f32)
         ops.gather_rows(S_.Xn, self.rows_masked_t, M, D, dst_bf16=self.h_s_ibot.A0)
         if self.gram_active:
             self._gram_features(S_.Xn, self.gram_fs, self.gram_xs, self.gram_nrm_s)
-        self._head_fwd(self.student_net, self.h_s_dino, "dino_head", self.Rc, stash=True)
-        self._head_fwd(self.student_net, self.h_s_ibot, "ibot_head", M, stash=True)
+        head_fwd(self.student_net, self.h_s_dino, "dino_head", self.Rc, stash=True)
+        head_fwd(self.student_net, self.h_s_ibot, "ibot_head", M, stash=True)
         # ---- losses + d(logits) (train/ssl_meta_arch.py:463-525)
         if self.fwd_overlap:
             torch.cuda.current_stream().wait_event(self._ev_fwd[1])      # teacher targets ready

@@ -26,31 +26,36 @@ SEG_DTYPE = np.dtype([("start", "<i8"), ("lr_mult", "<f4"), ("wd_mult", "<f4"), 
 
 def backbone_spec(cfg: EngineConfig):
     """(name, shape, kind) in creation order — models/vision_transformer.py:86-171."""
-    D, p, Hd = cfg.embed_dim, cfg.patch, cfg.hidden
+    D, p = cfg.embed_dim, cfg.patch
     spec = [("patch_embed/proj/kernel", (p, p, 3, D), "mat"), ("patch_embed/proj/bias", (D,), "vec"),
             ("cls_token", (1, 1, D), "vec"), ("mask_token", (1, D), "vec")]
     if cfg.n_storage:
         spec.insert(3, ("storage_tokens", (1, cfg.n_storage, D), "vec"))
     for i in range(cfg.depth):
-        b = f"blocks_{i}/"
-        spec += [(b + "norm1/scale", (D,), "vec"), (b + "norm1/bias", (D,), "vec"),
-                 (b + "attn/qkv/kernel", (D, 3 * D), "mat")]
-        if cfg.qkv_bias:
-            spec += [(b + "attn/qkv/bias", (3 * D,), "vec")]
-        spec += [(b + "attn/proj/kernel", (D, D), "mat"), (b + "attn/proj/bias", (D,), "vec"),
-                 (b + "ls1/gamma", (D,), "vec"),
-                 (b + "norm2/scale", (D,), "vec"), (b + "norm2/bias", (D,), "vec")]
-        if cfg.ffn_layer == "swiglu":                                 # layers/ffn_layers.py:62-69
-            Hs = cfg.swiglu_hidden
-            spec += [(b + "mlp/w1/kernel", (D, Hs), "mat"), (b + "mlp/w1/bias", (Hs,), "vec"),
-                     (b + "mlp/w2/kernel", (D, Hs), "mat"), (b + "mlp/w2/bias", (Hs,), "vec"),
-                     (b + "mlp/w3/kernel", (Hs, D), "mat"), (b + "mlp/w3/bias", (D,), "vec")]
-        else:
-            spec += [(b + "mlp/Dense_0/kernel", (D, Hd), "mat"), (b + "mlp/Dense_0/bias", (Hd,), "vec"),
-                     (b + "mlp/Dense_1/kernel", (Hd, D), "mat"), (b + "mlp/Dense_1/bias", (D,), "vec")]
-        spec += [(b + "ls2/gamma", (D,), "vec")]
+        spec += block_spec(cfg, i)
     spec += [("norm/scale", (D,), "vec"), ("norm/bias", (D,), "vec")]
     return spec
+
+
+def block_spec(cfg: EngineConfig, i: int):
+    """(name, shape, kind) of block i — layers/block.py:22-214."""
+    D, Hd = cfg.embed_dim, cfg.hidden
+    b = f"blocks_{i}/"
+    spec = [(b + "norm1/scale", (D,), "vec"), (b + "norm1/bias", (D,), "vec"), (b + "attn/qkv/kernel", (D, 3 * D), "mat")]
+    if cfg.qkv_bias:
+        spec += [(b + "attn/qkv/bias", (3 * D,), "vec")]
+    spec += [(b + "attn/proj/kernel", (D, D), "mat"), (b + "attn/proj/bias", (D,), "vec"),
+             (b + "ls1/gamma", (D,), "vec"),
+             (b + "norm2/scale", (D,), "vec"), (b + "norm2/bias", (D,), "vec")]
+    if cfg.ffn_layer == "swiglu":                                 # layers/ffn_layers.py:62-69
+        Hs = cfg.swiglu_hidden
+        spec += [(b + "mlp/w1/kernel", (D, Hs), "mat"), (b + "mlp/w1/bias", (Hs,), "vec"),
+                 (b + "mlp/w2/kernel", (D, Hs), "mat"), (b + "mlp/w2/bias", (Hs,), "vec"),
+                 (b + "mlp/w3/kernel", (Hs, D), "mat"), (b + "mlp/w3/bias", (D,), "vec")]
+    else:
+        spec += [(b + "mlp/Dense_0/kernel", (D, Hd), "mat"), (b + "mlp/Dense_0/bias", (Hd,), "vec"),
+                 (b + "mlp/Dense_1/kernel", (Hd, D), "mat"), (b + "mlp/Dense_1/bias", (D,), "vec")]
+    return spec + [(b + "ls2/gamma", (D,), "vec")]
 
 
 def head_spec(cfg: EngineConfig, module: str = "dino_head"):

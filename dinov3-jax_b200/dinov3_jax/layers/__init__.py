@@ -1,14 +1,21 @@
 """Layer objects with the reference's names and constructor fields (dinov3_jax/layers/*.py), forward pass on CUDA
 tensors through the CUDA kernels.  Parameters are passed as a dict with the reference's leaf names and layouts
 (Dense `kernel` [in, out], `bias`; LayerNorm `scale`, `bias`; LayerScale `gamma`).  These are inference-style
-wrappers for unit-level use and tests; the training engine fuses the same kernels block-wise (engine/core.py).
+wrappers for unit-level use and tests.  `SelfAttentionBlock` and `DINOHead` run the training engine's forward pieces
+(engine/forward.py: `block_fwd`, `head_fwd`) on frozen weights; `PatchEmbed`, `SelfAttention`, `Mlp`, `SwiGLUFFN` and
+`LayerScale` launch the kernels of one layer on their own.
 """
 from __future__ import annotations
+
+from dataclasses import replace
 
 import torch
 
 from .. import ops
-from ..engine.core import rope_tables
+from ..checkpointer import flat_from_tree
+from ..engine.config import FFN_LAYERS, EngineConfig
+from ..engine.forward import CropSet, HeadBufs, Net, Stream, block_fwd, head_fwd, rope_tables
+from ..engine.params import FrozenStore, block_spec, head_spec
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -19,6 +26,33 @@ def _w(p):   # matrix -> bf16 [in, out]
 
 def _v(p):
     return p.to(f32).reshape(-1).contiguous()
+
+
+def vit_config(flat: dict, dim: int, num_heads: int, ffn_ratio: float, eps: float, ffn_layer: str, mask_k_bias: bool,
+               **kw) -> EngineConfig:
+    """The EngineConfig of a ViT block / backbone from the reference's constructor arguments.  A tree `flat` without
+    qkv biases runs without them, whatever the qkv_bias argument says."""
+    if dim not in (num_heads * 64, num_heads * 128):
+        raise NotImplementedError("head_dim must be 64 or 128")
+    if ffn_layer not in FFN_LAYERS:
+        raise NotImplementedError(f"ffn_layer {ffn_layer!r}: mlp | swiglu | swiglu32 | swiglu64 | swiglu128")
+    ffn, align = FFN_LAYERS[ffn_layer]
+    return EngineConfig(embed_dim=dim, heads=num_heads, ffn_ratio=ffn_ratio, ln_eps=eps, ffn_layer=ffn, swiglu_align=align,
+                        mask_k_bias=mask_k_bias, qkv_bias="blocks_0/attn/qkv/bias" in flat, **kw)
+
+
+def frozen_store(spec, flat: dict, mask_k_bias: bool, device, ffn_bias: bool = True) -> FrozenStore:
+    """A FrozenStore of `spec` loaded from `flat` ('/'-joined reference names, any float dtype).  Names outside the spec
+    are ignored; a SwiGLU bias is a zero vector where the tree has none or `ffn_bias` is off (SwiGLUFFN's use_bias)."""
+    tensors = {}
+    for name, shape, _ in spec:
+        if name.endswith(("mlp/w1/bias", "mlp/w2/bias", "mlp/w3/bias")) and (not ffn_bias or name not in flat):
+            tensors[name] = torch.zeros(shape)
+        elif name in flat:
+            tensors[name] = flat[name]
+    store = FrozenStore(spec, device)
+    store.load(tensors, mask_k_bias)
+    return store
 
 
 class RopePositionEmbedding:
@@ -81,18 +115,10 @@ class Mlp:
         ops.gemm(h, self.w2, y, b_mn=True, bias=self.b2, gelu=True)
         return y.view(*shp[:-1], self.w2.shape[1])
 
-    def residual(self, z, xmid, gamma):
-        """xmid + gamma * mlp(z) (z bf16 [T, D], xmid fp32 [T, D]): LayerScale and residual in the second GEMM's epilogue."""
-        h = torch.empty(z.shape[0], self.w1.shape[1], dtype=bf16, device=z.device)
-        ops.gemm(z, self.w1, h, b_mn=True, bias=self.b1, gelu=True)
-        out = torch.empty_like(xmid)
-        ops.gemm(h, self.w2, out, b_mn=True, bias=self.b2, gelu=True, gamma=gamma, resid=xmid)
-        return out
-
 
 class SwiGLUFFN:
     """layers/ffn_layers.py:52-76: w3(silu(w1 x) * w2 x), hidden width int(2/3 hidden_features) rounded up to align_to.
-    The engine's kernels (engine/core.py): the w1 and w2 GEMMs write the two halves of one [T, 2 Hs] buffer, then
+    The engine's kernels (engine/forward.py): the w1 and w2 GEMMs write the two halves of one [T, 2 Hs] buffer, then
     d3_swiglu_fwd, then the w3 GEMM."""
 
     def __init__(self, params: dict, hidden_features=None, out_features=None, act_layer=None, drop: float = 0.0,
@@ -110,27 +136,18 @@ class SwiGLUFFN:
         self.b1, self.b2, self.b3 = bias("w1", self.w1), bias("w2", self.w2), bias("w3", self.w3)
         self.Hs = Hs
 
-    def _hidden(self, z):
+    def __call__(self, x):
+        shp = x.shape
+        z = x.reshape(-1, shp[-1]).to(bf16).contiguous()
         T, Hs = z.shape[0], self.Hs
         x12 = torch.empty(T, 2 * Hs, dtype=bf16, device=z.device)
         ops.gemm(z, self.w1, x12[:, :Hs], b_mn=True, bias=self.b1)
         ops.gemm(z, self.w2, x12[:, Hs:], b_mn=True, bias=self.b2)
         h = torch.empty(T, Hs, dtype=bf16, device=z.device)
         ops.swiglu_fwd(x12, h)
-        return h
-
-    def __call__(self, x):
-        shp = x.shape
-        h = self._hidden(x.reshape(-1, shp[-1]).to(bf16).contiguous())
-        y = torch.empty(h.shape[0], self.w3.shape[1], dtype=f32, device=x.device)
+        y = torch.empty(T, self.w3.shape[1], dtype=f32, device=x.device)
         ops.gemm(h, self.w3, y, b_mn=True, bias=self.b3)
         return y.view(*shp[:-1], self.w3.shape[1])
-
-    def residual(self, z, xmid, gamma):
-        """xmid + gamma * ffn(z): LayerScale and residual in the w3 GEMM's epilogue."""
-        out = torch.empty_like(xmid)
-        ops.gemm(self._hidden(z), self.w3, out, b_mn=True, bias=self.b3, gamma=gamma, resid=xmid)
-        return out
 
 
 class SelfAttention:
@@ -171,72 +188,51 @@ class SelfAttention:
 
 
 class SelfAttentionBlock:
-    """layers/block.py:22-214, deterministic branch :195-201: x + ls1(attn(norm1 x)); x + ls2(mlp(norm2 x))."""
-
-    FFN_ALIGN = {"swiglu": 8, "swiglu32": 32, "swiglu64": 64, "swiglu128": 128}     # models/vision_transformer.py:30-36
+    """layers/block.py:22-214, deterministic branch :195-201: x + ls1(attn(norm1 x)); x + ls2(mlp(norm2 x)), as
+    engine.forward.block_fwd on a one-block FrozenStore."""
 
     def __init__(self, params: dict, dim: int, num_heads: int, ffn_ratio: float = 4.0, qkv_bias: bool = True,
                  proj_bias: bool = True, ffn_bias: bool = True, init_values=None, eps: float = 1e-6,
                  ffn_layer: str = "mlp", mask_k_bias: bool = False, **unused):
-        self.dim, self.H, self.eps = dim, num_heads, eps
-        self.attn = SelfAttention(params["attn"], dim, num_heads, qkv_bias=qkv_bias, mask_k_bias=mask_k_bias)
-        if ffn_layer == "mlp":
-            self.mlp = Mlp(params["mlp"])
-        elif ffn_layer in self.FFN_ALIGN:
-            self.mlp = SwiGLUFFN(params["mlp"], hidden_features=int(dim * ffn_ratio), out_features=dim, use_bias=ffn_bias,
-                                 align_to=self.FFN_ALIGN[ffn_layer])
-        else:
-            raise NotImplementedError(f"ffn_layer {ffn_layer!r}: mlp | swiglu | swiglu32 | swiglu64 | swiglu128")
-        self.n1 = (_v(params["norm1"]["scale"]), _v(params["norm1"]["bias"]))
-        self.n2 = (_v(params["norm2"]["scale"]), _v(params["norm2"]["bias"]))
-        self.g1, self.g2 = _v(params["ls1"]["gamma"]), _v(params["ls2"]["gamma"])
+        flat = {"blocks_0/" + k: v for k, v in flat_from_tree(params).items()}
+        self.cfg = vit_config(flat, dim, num_heads, ffn_ratio, eps, ffn_layer, mask_k_bias, depth=1)
+        self.store = frozen_store(block_spec(self.cfg, 0), flat, mask_k_bias, flat["blocks_0/attn/qkv/kernel"].device, ffn_bias)
 
     def __call__(self, x, rope=None, deterministic=True):
+        """x [n, N, D]; rope: (sin, cos) of the last P tokens, or None: identity tables (cos 1, sin 0), unrotated bits."""
         n, N, D = x.shape
-        X = x.reshape(n * N, D).to(f32).contiguous()
-        y = torch.empty(n * N, D, dtype=bf16, device=x.device)
-        ops.layernorm_fwd(X, self.n1[0], self.n1[1], y, eps=self.eps)
-        qkv = torch.empty(n * N, 3 * D, dtype=bf16, device=x.device)
-        ops.gemm(y, self.attn.wqkv, qkv, b_mn=True, bias=self.attn.bqkv)
-        o = self.attn.compute_attention(qkv.view(n, N, 3 * D), rope=rope).reshape(n * N, D)
-        xmid = torch.empty_like(X)
-        ops.gemm(o, self.attn.wp, xmid, b_mn=True, bias=self.attn.bp, gamma=self.g1, resid=X)
-        z = torch.empty(n * N, D, dtype=bf16, device=x.device)
-        ops.layernorm_fwd(xmid, self.n2[0], self.n2[1], z, eps=self.eps)
-        return self.mlp.residual(z, xmid, self.g2).view(n, N, D)
+        if rope is None:
+            rope = (torch.zeros(N - 1, self.cfg.head_dim, device=x.device), torch.ones(N - 1, self.cfg.head_dim, device=x.device))
+        P = rope[0].shape[0]
+        cfg = replace(self.cfg, n_storage=N - P - 1)          # the N - P tokens in front are not rotated
+        st = Stream(cfg, [CropSet(cfg, n, P, 1, 0, x.device, rope=rope)], x.device, stash=False)
+        st.x_in(0).copy_(x.reshape(n * N, D))
+        block_fwd(Net(cfg, {"backbone": self.store}, True), st, 0)
+        return st.x_out(0).view(n, N, D)
 
 
 class DINOHead:
-    """layers/dino_head.py:46-85: MLP(GELU) -> x / (||x|| + 1e-12) -> bias-free prototype layer."""
+    """layers/dino_head.py:46-85: MLP(GELU) -> x / (||x|| + 1e-12) -> bias-free prototype layer, as
+    engine.forward.head_fwd on a FrozenStore."""
 
     def __init__(self, params: dict, in_dim: int, out_dim: int, use_bn: bool = False, nlayers: int = 3,
                  hidden_dim: int = 2048, bottleneck_dim: int = 256, mlp_bias: bool = True):
         if use_bn or nlayers != 3:
             raise NotImplementedError("DINOHead on the GPU path: nlayers=3, no batch norm (reference defaults)")
-        m = params["mlp"]
-        self.w = [_w(m[f"layers_{i}"]["kernel"]) for i in (0, 2, 4)]
-        self.b = [_v(m[f"layers_{i}"]["bias"]) for i in (0, 2, 4)]
-        self.wl = _w(params["last_layer"]["kernel"])
+        flat = flat_from_tree(params)
+        self.cfg = EngineConfig(embed_dim=in_dim, n_prototypes=out_dim, head_hidden=hidden_dim, head_bottleneck=bottleneck_dim)
+        self.net = Net(self.cfg, {"dino_head": frozen_store(head_spec(self.cfg), flat, False, flat["last_layer/kernel"].device)}, True)
 
     def __call__(self, x, no_last_layer=False, only_last_layer=False):
         R = x.shape[0]
-        dev = x.device
-        if not only_last_layer:
-            a = x.to(bf16).contiguous()
-            h1 = torch.empty(R, self.w[0].shape[1], dtype=bf16, device=dev)
-            ops.gemm(a, self.w[0], h1, b_mn=True, bias=self.b[0], gelu=True)
-            h2 = torch.empty(R, self.w[1].shape[1], dtype=bf16, device=dev)
-            ops.gemm(h1, self.w[1], h2, b_mn=True, bias=self.b[1], gelu=True)
-            u = torch.empty(R, self.w[2].shape[1], dtype=f32, device=dev)
-            ops.gemm(h2, self.w[2], u, b_mn=True, bias=self.b[2])
-            yn = torch.empty(R, u.shape[1], dtype=bf16, device=dev)
-            ops.l2norm_fwd(u, yn, torch.empty(R, dtype=f32, device=dev), 1e-12)
-            x = yn
-        if no_last_layer:
-            return x
-        logits = torch.empty(R, self.wl.shape[1], dtype=f32, device=dev)
-        ops.gemm(x.to(bf16).contiguous(), self.wl, logits, b_mn=True)
-        return logits
+        if only_last_layer:
+            logits = torch.empty(R, self.cfg.n_prototypes, dtype=f32, device=x.device)
+            ops.gemm(x.to(bf16).contiguous(), self.net.mods["dino_head"].w("last_layer/kernel"), logits, b_mn=True)
+            return logits
+        hb = HeadBufs(self.cfg, "dino_head", R, x.device, stash=False)
+        hb.A0.copy_(x)
+        head_fwd(self.net, hb, "dino_head", R, stash=False)
+        return hb.Yn if no_last_layer else hb.logits
 
 
 __all__ = ["RopePositionEmbedding", "LayerScale", "PatchEmbed", "Mlp", "SwiGLUFFN", "SelfAttention", "SelfAttentionBlock", "DINOHead"]

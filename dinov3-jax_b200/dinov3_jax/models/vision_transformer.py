@@ -1,17 +1,22 @@
 """`DinoVisionTransformer` with the reference's constructor fields and call signature
 (dinov3_jax/models/vision_transformer.py:55-321), forward pass through the CUDA kernels.
 
-This is the feature-extraction entry point (`model(x)` / `model([global, local], masks=[m, None], is_training=True)`);
-training goes through engine/core.py, which runs the same kernels on packed multi-crop streams with the stash the
-backward needs.  Parameters arrive as the reference's nested dict (`cls_token`, `mask_token`, `patch_embed/proj`,
-`blocks_i/...`, `norm`), any float dtype, CUDA or CPU.
+This is the feature-extraction entry point (`model(x)` / `model([global, local], masks=[m, None], is_training=True)`).
+The weights live in one FrozenStore in the training engine's flat backbone layout, and the forward runs the engine's
+own pieces (engine/forward.py: `embed`, `block_fwd`, `backbone_fwd`) on one token stream per input, so a feature
+and a training teacher pass launch the same kernels on the same bits.  Parameters arrive as the reference's nested dict
+(`cls_token`, `mask_token`, `patch_embed/proj`, `blocks_i/...`, `norm`), any float dtype, CUDA or CPU; weights go
+through fp32 on their way to bf16, as every engine load does.
 """
 from __future__ import annotations
 
 import torch
 
 from .. import ops
-from ..layers import PatchEmbed, RopePositionEmbedding, SelfAttentionBlock
+from ..checkpointer import flat_from_tree
+from ..engine.forward import CropSet, Net, Stream, backbone_fwd, block_fwd, embed
+from ..engine.params import backbone_spec
+from ..layers import RopePositionEmbedding, frozen_store, vit_config
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -40,67 +45,55 @@ class DinoVisionTransformer:
                  untie_global_and_local_cls_norm: bool = False, device="cuda"):
         if norm_layer not in ("layernorm", "layernormbf16"):
             raise NotImplementedError("GPU path: norm_layer layernorm | layernormbf16")
-        if ffn_layer != "mlp" and ffn_layer not in SelfAttentionBlock.FFN_ALIGN:
-            raise NotImplementedError(f"ffn_layer {ffn_layer!r}: mlp | swiglu | swiglu32 | swiglu64 | swiglu128")
-        self.eps = 1e-5 if norm_layer == "layernormbf16" else 1e-6        # models/vision_transformer.py:38-42
-        self.n_storage_tokens = n_storage_tokens
         if drop_path_rate:
             raise NotImplementedError("stochastic depth is not on the GPU path (reference default 0 is asserted upstream)")
-        dev = torch.device(device)
-        to = lambda t: torch.as_tensor(t).to(dev)
-        mv = lambda tree: {k: (mv(v) if isinstance(v, dict) else to(v)) for k, v in tree.items()}
-        params = mv(params)
-        self.patch_size, self.embed_dim, self.n_blocks, self.num_heads = patch_size, embed_dim, n_blocks, num_heads
-        self.patch_embed = PatchEmbed(params["patch_embed"], img_size=img_size, patch_size=patch_size, in_chans=in_chans,
-                                      embed_dim=embed_dim)
-        self.cls_token = params["cls_token"].to(f32).reshape(-1).contiguous()
-        self.mask_token = params["mask_token"].to(f32).reshape(-1).contiguous()
-        self.storage_tokens = params["storage_tokens"].to(f32).reshape(-1).contiguous() if n_storage_tokens else None
         self.rope_embed = RopePositionEmbedding(embed_dim=embed_dim, num_heads=num_heads, base=pos_embed_rope_base,
                                                 min_period=pos_embed_rope_min_period, max_period=pos_embed_rope_max_period,
                                                 normalize_coords=pos_embed_rope_normalize_coords)
-        self.blocks = [SelfAttentionBlock(params[f"blocks_{i}"], dim=embed_dim, num_heads=num_heads, ffn_ratio=ffn_ratio,
-                                          qkv_bias=qkv_bias, proj_bias=proj_bias, ffn_bias=ffn_bias, eps=self.eps,
-                                          ffn_layer=ffn_layer, mask_k_bias=mask_k_bias)
-                       for i in range(n_blocks)]
-        ln = lambda p: (p["scale"].to(f32).reshape(-1).contiguous(), p["bias"].to(f32).reshape(-1).contiguous())
-        self.norm = ln(params["norm"])
+        dev = torch.device(device)
+        flat = {k: torch.as_tensor(v) for k, v in flat_from_tree(params).items()}
+        eps = 1e-5 if norm_layer == "layernormbf16" else 1e-6        # models/vision_transformer.py:38-42
+        self.cfg = vit_config(flat, embed_dim, num_heads, ffn_ratio, eps, ffn_layer, mask_k_bias, depth=n_blocks,
+                              patch=patch_size, rope_base=pos_embed_rope_base, n_storage=n_storage_tokens)
+        self.net = Net(self.cfg, {"backbone": frozen_store(backbone_spec(self.cfg), flat, mask_k_bias, dev, ffn_bias)}, True)
+        self.patch_size, self.embed_dim, self.n_blocks, self.num_heads = patch_size, embed_dim, n_blocks, num_heads
+        self.n_storage_tokens, self.eps = n_storage_tokens, eps
+        self.norm = (self.net.mods["backbone"].vec("norm/scale"), self.net.mods["backbone"].vec("norm/bias"))
+        ln = lambda name: tuple(flat[f"{name}/{k}"].to(device=dev, dtype=f32).reshape(-1).contiguous() for k in ("scale", "bias"))
         # :156-164.  local_cls_norm is only read by the training branch (:225), so it is loaded and never applied here.
-        self.cls_norm = ln(params["cls_norm"]) if untie_cls_and_patch_norms else None
-        self.local_cls_norm = ln(params["local_cls_norm"]) if untie_global_and_local_cls_norm else None
+        self.cls_norm = ln("cls_norm") if untie_cls_and_patch_norms else None
+        self.local_cls_norm = ln("local_cls_norm") if untie_global_and_local_cls_norm else None
         self.device = dev
 
-    # models/vision_transformer.py:173-203
-    def prepare_tokens_with_masks(self, x, masks=None):
+    def _stream(self, x, masks=None):
+        """One input batch -> (its bf16 NHWC images, uint8 masks or None, a token stream of one crop set)."""
         x = torch.as_tensor(x).to(self.device)
-        tok = self.patch_embed(x)
-        n, Hp, Wp, D = tok.shape
-        X = torch.empty(n, 1 + self.n_storage_tokens + Hp * Wp, D, dtype=f32, device=self.device)
-        m8 = None if masks is None else torch.as_tensor(masks).to(self.device).reshape(n, Hp * Wp).to(torch.uint8).contiguous()
-        ops.assemble_tokens(tok.view(n * Hp * Wp, D), self.cls_token, self.mask_token, m8, X, n, Hp * Wp, D,
-                            storage=self.storage_tokens)
-        return X, (Hp, Wp)
+        n, H, W, _ = x.shape
+        p = self.patch_size
+        if H % p or W % p:
+            raise AssertionError(f"Input image height {H} / width {W} is not a multiple of patch size {p}")   # layers/patch_embed.py:48-49
+        cs = CropSet(self.cfg, n, H // p, W // p, 0, self.device)
+        m8 = None if masks is None else torch.as_tensor(masks).to(self.device).reshape(n, cs.P).to(torch.uint8).contiguous()
+        return x.to(bf16).contiguous(), m8, Stream(self.cfg, [cs], self.device, stash=False)
 
     # models/vision_transformer.py:205-247
     def forward_features_list(self, x_list, masks_list):
         out = []
+        L, D, R = self.cfg.depth, self.embed_dim, self.n_storage_tokens
         for x, masks in zip(x_list, masks_list):
-            X, (Hp, Wp) = self.prepare_tokens_with_masks(x, masks)
-            rope = self.rope_embed(H=Hp, W=Wp, device=self.device)
-            for blk in self.blocks:
-                X = blk(X, rope=rope)
-            n, N, D = X.shape
-            R = self.n_storage_tokens
-            if self.cls_norm is not None:       # :224-232: the 1 + R prefix rows take cls_norm
-                cls, storage, patches = self._tokens_out(X, Hp, Wp, True, False, f32)
-                out.append({"x_norm_clstoken": cls, "x_storage_tokens": storage, "x_norm_patchtokens": patches,
-                            "x_prenorm": X, "masks": masks})
-                continue
-            Y = torch.empty(n * N, D, dtype=f32, device=self.device)
-            ops.layernorm_fwd(X.view(n * N, D), self.norm[0], self.norm[1], Y, eps=self.eps)
-            Y = Y.view(n, N, D)
-            out.append({"x_norm_clstoken": Y[:, 0], "x_storage_tokens": Y[:, 1:1 + R], "x_norm_patchtokens": Y[:, 1 + R:],
-                        "x_prenorm": X, "masks": masks})
+            img, m8, st = self._stream(x, masks)
+            cs = st.sets[0]
+            if self.cls_norm is None:
+                backbone_fwd(self.net, st, [img], [m8])
+                Y = st.Xn.view(cs.n, cs.N, D)
+                cls, storage, patches = Y[:, 0], Y[:, 1:1 + R], Y[:, 1 + R:]
+            else:       # :224-232: the 1 + R prefix rows take cls_norm, so no LayerNorm runs over every token
+                embed(self.net, st, [img], [m8])
+                for i in range(L):
+                    block_fwd(self.net, st, i)
+                cls, storage, patches = self._tokens_out(st.x_in(L).view(cs.n, cs.N, D), cs.Hp, cs.Wp, True, False, f32)
+            out.append({"x_norm_clstoken": cls, "x_storage_tokens": storage, "x_norm_patchtokens": patches,
+                        "x_prenorm": st.x_in(L).view(cs.n, cs.N, D), "masks": masks})
         return out
 
     def _tokens_out(self, X, Hp, Wp, norm: bool, reshape: bool, out_dtype):
@@ -129,15 +122,16 @@ class DinoVisionTransformer:
         [B, D] and / or the storage tokens [B, R, D] when asked for.  out_dtype: torch.float32 or torch.bfloat16."""
         if out_dtype not in (f32, bf16):
             raise ValueError("out_dtype must be torch.float32 or torch.bfloat16")
-        X, (Hp, Wp) = self.prepare_tokens_with_masks(x)
-        L = len(self.blocks)
+        img, _, st = self._stream(x)
+        cs, L = st.sets[0], self.cfg.depth
         take = range(L - n, L) if isinstance(n, int) else [int(i) for i in n]
-        rope = self.rope_embed(H=Hp, W=Wp, device=self.device)
+        embed(self.net, st, [img], [None])
         outputs = []
-        for i, blk in enumerate(self.blocks[:max(take, default=-1) + 1]):     # later blocks feed no selected output
-            X = blk(X, rope=rope)
+        for i in range(min(max(take, default=-1) + 1, L)):     # later blocks feed no selected output
+            block_fwd(self.net, st, i)
             if i in take:
-                outputs.append(self._tokens_out(X, Hp, Wp, norm, reshape, out_dtype))
+                outputs.append(self._tokens_out(st.x_out(i).view(cs.n, cs.N, self.embed_dim), cs.Hp, cs.Wp, norm, reshape,
+                                                out_dtype))
         assert len(outputs) == len(take), f"only {len(outputs)} / {len(take)} blocks found"
         return pack_intermediate_layers(outputs, return_class_token, return_extra_tokens)
 

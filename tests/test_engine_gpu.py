@@ -447,8 +447,9 @@ def test_checkpoint_keeps_the_frozen_gram_teacher(tmp_path):
     ck = load_checkpoint(tmp_path / "0", abstract_model_params=engine_state(b)[0], strict_loading=False)
     load_engine_state(b, ck["model_params"], ck["optimizer_state"])
     assert b.gram_active
-    bba, bbb = a.params.mods["backbone"], b.params.mods["backbone"]
-    assert torch.equal(bba.g_bf16, bbb.g_bf16) and torch.equal(bba.g_vecs, bbb.g_vecs)
+    ga, gb = a.gram_net.mods["backbone"], b.gram_net.mods["backbone"]
+    assert torch.equal(ga.bf16, gb.bf16) and torch.equal(ga.vecs, gb.vecs)
+    assert ga.bf16.float().abs().sum() > 0            # a snapshot was taken, not the zero-initialised store
     for e in (a, b):
         e.train_step(batch, iteration=1, **HYPER)
     ma, mb = a.read_metrics(), b.read_metrics()

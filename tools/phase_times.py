@@ -19,14 +19,16 @@ for _ in range(3): eng.train_step(None, **hyper)
 marks = []
 def mark(name):
     e = torch.cuda.Event(enable_timing=True); e.record(); marks.append((name, e))
-orig = {k: getattr(eng, k) for k in ("_backbone_fwd", "_head_fwd", "_sinkhorn_pair", "_head_bwd", "_block_bwd", "optimizer_step")}
+import dinov3_jax.engine.core as core      # the forward pieces are module functions the engine calls by name
+owner = {"backbone_fwd": core, "head_fwd": core, "_sinkhorn_pair": eng, "_head_bwd": eng, "_block_bwd": eng, "optimizer_step": eng}
+orig = {k: getattr(o, k) for k, o in owner.items()}
 def wrap(name, label_fn):
     f = orig[name]
     def g(*a, **k):
         r = f(*a, **k); mark(label_fn(*a, **k)); return r
-    setattr(eng, name, g)
-wrap("_backbone_fwd", lambda st, imgs, masks, teacher: "backbone fwd teacher" if teacher else "backbone fwd student")
-wrap("_head_fwd", lambda hb, module, R, teacher, stash: f"heads fwd {'teacher' if teacher else 'student'}")
+    setattr(owner[name], name, g)
+wrap("backbone_fwd", lambda net, *a: f"backbone fwd {'teacher' if net.teacher else 'student'}")
+wrap("head_fwd", lambda net, *a, **k: f"heads fwd {'teacher' if net.teacher else 'student'}")
 wrap("_sinkhorn_pair", lambda *a, **k: "sinkhorn")
 wrap("_head_bwd", lambda *a, **k: "heads bwd (+CE, before)")
 wrap("_block_bwd", lambda i, *a: "blocks bwd")

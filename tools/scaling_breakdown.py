@@ -57,15 +57,16 @@ step_ms = e0.elapsed_time(e1) / 6
 marks = []
 def mark(name):
     e = torch.cuda.Event(enable_timing=True); e.record(); marks.append((name, e))
-names = ("_backbone_fwd", "_head_fwd", "_sinkhorn_pair", "_head_bwd", "_block_bwd", "optimizer_step")
-orig = {k: getattr(eng, k) for k in names}
+import dinov3_jax.engine.core as core      # the forward pieces are module functions the engine calls by name
+owner = {"backbone_fwd": core, "head_fwd": core, "_sinkhorn_pair": eng, "_head_bwd": eng, "_block_bwd": eng, "optimizer_step": eng}
+orig = {k: getattr(o, k) for k, o in owner.items()}
 def wrap(name, label_fn):
     f = orig[name]
     def g(*a, **k):
         r = f(*a, **k); mark(label_fn(*a, **k)); return r
-    setattr(eng, name, g)
-wrap("_backbone_fwd", lambda st, imgs, masks, teacher: "backbone fwd teacher" if teacher else "backbone fwd student")
-wrap("_head_fwd", lambda hb, module, R, teacher, stash: f"heads fwd {'teacher' if teacher else 'student'}")
+    setattr(owner[name], name, g)
+wrap("backbone_fwd", lambda net, *a: f"backbone fwd {'teacher' if net.teacher else 'student'}")
+wrap("head_fwd", lambda net, *a, **k: f"heads fwd {'teacher' if net.teacher else 'student'}")
 wrap("_sinkhorn_pair", lambda *a, **k: "sinkhorn")
 wrap("_head_bwd", lambda *a, **k: "heads bwd (+CE, KoLeo before)")
 wrap("_block_bwd", lambda i, *a: "blocks bwd")
@@ -100,8 +101,8 @@ for rep in range(3):
     agg["TOTAL"] = marks[0][1].elapsed_time(marks[-1][1])
     phase_runs.append(agg)
     wait_runs.append([(n, x.elapsed_time(y)) for n, x, y in waits])
-for k in names:
-    setattr(eng, k, orig[k])
+for k, o in owner.items():
+    setattr(o, k, orig[k])
 if world > 1:
     eng.fsdp.acquire, eng.fsdp.finish_grads = _acq, _fin
 phases = {k: sorted(r[k] for r in phase_runs)[1] for k in phase_runs[0]}     # median of 3
@@ -120,7 +121,6 @@ def gemm_tagged(*a, **k):
         scat_seen.append(k.get("scatter") is not None)
     return r
 ops.gemm = gemm_tagged
-import dinov3_jax.engine.core as core
 if hasattr(core, "ops"):
     core.ops.gemm = gemm_tagged
 barrier()
