@@ -37,6 +37,25 @@ int encode_tensor_map_2d_bf16(CUtensorMap* map, const void* ptr, const cuuint64_
   return D3_OK;
 }
 
+int encode_tensor_map_2d_u8(CUtensorMap* map, const void* ptr, cuuint64_t cols, cuuint64_t rows, cuuint64_t ld_bytes,
+                            cuuint32_t box_cols, cuuint32_t box_rows) {
+  if (!g_encode) return set_error(D3_ERR_CUDA, "d3_init() was not called (cuTensorMapEncodeTiled unresolved)");
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {ld_bytes};
+  cuuint32_t box[2] = {box_cols, box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    char buf[160];
+    snprintf(buf, sizeof(buf), "cuTensorMapEncodeTiled(e4m3) failed (%d): dims=(%llu,%llu) stride=%llu", (int)r,
+             (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)ld_bytes);
+    return set_error(D3_ERR_CUDA, buf);
+  }
+  return D3_OK;
+}
+
 int encode_tensor_map_2d(CUtensorMap* map, const void* ptr, int elt_bytes, cuuint64_t cols, cuuint64_t rows,
                          cuuint64_t row_stride_bytes, cuuint32_t box_cols, cuuint32_t box_rows, int swizzle_bytes) {
   if (!g_encode) return set_error(D3_ERR_CUDA, "d3_init() was not called (cuTensorMapEncodeTiled unresolved)");
@@ -132,13 +151,9 @@ int d3_init(int device) {
   return D3_OK;
 }
 
-int d3_gemm_bf16(const void* A, int lda, int a_major, const void* B, int ldb, int b_major, int M, int N, int K,
-                 const d3_gemm_epilogue* ep, int tile_n, int split_k, void* stream) {
-  if (!A || !B || !ep || !ep->out) return set_error(D3_ERR_ARG, "d3_gemm_bf16: null pointer");
-  if (tile_n != 0 && tile_n != 64 && tile_n != 128 && tile_n != 256 && tile_n != 512) return set_error(D3_ERR_ARG, "tile_n");
-  if (split_k < 0) return set_error(D3_ERR_ARG, "split_k");
+// the public epilogue description -> the kernels' GemmEpilogue, with the flag / pointer checks both GEMM entry points make
+static int epilogue_from_abi(const d3_gemm_epilogue* ep, GemmEpilogue& g) {
   if ((ep->flags & D3_EP_ACCUM) && !(ep->flags & D3_EP_OUT_F32)) return set_error(D3_ERR_ARG, "ACCUM needs fp32 out");
-  GemmEpilogue g;
   g.bias = ep->bias; g.gamma = ep->gamma; g.resid = ep->resid;
   g.aux_in = reinterpret_cast<const __nv_bfloat16*>(ep->aux_in);
   g.aux_out = reinterpret_cast<__nv_bfloat16*>(ep->aux_out);
@@ -154,7 +169,27 @@ int d3_gemm_bf16(const void* A, int lda, int a_major, const void* B, int ldb, in
   if ((g.flags & EP_RESID) && !g.resid) return set_error(D3_ERR_ARG, "resid flag without pointer");
   if ((g.flags & EP_STORE_PRE) && !g.aux_out) return set_error(D3_ERR_ARG, "store_pre flag without pointer");
   if ((g.flags & EP_MUL_DGELU) && !g.aux_in) return set_error(D3_ERR_ARG, "mul_dgelu flag without pointer");
+  return D3_OK;
+}
+
+int d3_gemm_bf16(const void* A, int lda, int a_major, const void* B, int ldb, int b_major, int M, int N, int K,
+                 const d3_gemm_epilogue* ep, int tile_n, int split_k, void* stream) {
+  if (!A || !B || !ep || !ep->out) return set_error(D3_ERR_ARG, "d3_gemm_bf16: null pointer");
+  if (tile_n != 0 && tile_n != 64 && tile_n != 128 && tile_n != 256 && tile_n != 512) return set_error(D3_ERR_ARG, "tile_n");
+  if (split_k < 0) return set_error(D3_ERR_ARG, "split_k");
+  GemmEpilogue g;
+  const int rc = epilogue_from_abi(ep, g);
+  if (rc) return rc;
   return gemm_bf16(A, lda, a_major, B, ldb, b_major, M, N, K, g, tile_n, split_k, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int d3_gemm_e4m3(const void* A_u8, int lda, const float* sa, const void* B_u8, int ldb, const float* sb, int M, int N,
+                 int K, const d3_gemm_epilogue* ep, void* stream) {
+  if (!A_u8 || !B_u8 || !sa || !sb || !ep || !ep->out) return set_error(D3_ERR_ARG, "d3_gemm_e4m3: null pointer");
+  GemmEpilogue g;
+  const int rc = epilogue_from_abi(ep, g);
+  if (rc) return rc;
+  return gemm_e4m3(A_u8, lda, sa, B_u8, ldb, sb, M, N, K, g, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

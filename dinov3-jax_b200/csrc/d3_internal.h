@@ -50,6 +50,9 @@ int encode_tensor_map_2d_bf16(CUtensorMap* map, const void* ptr, const cuuint64_
 // generic 2-D map: elt_bytes 2 (bf16) or 4 (fp32); swizzle_bytes 0 / 64 / 128
 int encode_tensor_map_2d(CUtensorMap* map, const void* ptr, int elt_bytes, cuuint64_t cols, cuuint64_t rows,
                          cuuint64_t row_stride_bytes, cuuint32_t box_cols, cuuint32_t box_rows, int swizzle_bytes);
+// e4m3 (uint8) operand map: `cols` bytes per row, SWIZZLE_128B, boxes of box_cols x box_rows
+int encode_tensor_map_2d_u8(CUtensorMap* map, const void* ptr, cuuint64_t cols, cuuint64_t rows, cuuint64_t ld_bytes,
+                            cuuint32_t box_cols, cuuint32_t box_rows);
 
 // Deterministic reductions.  A kernel that would add one partial per (slab, element) into a destination with a float
 // atomic (whose order, and so whose rounding, changes from run to run) writes it into slab s of a zeroed, stream-ordered
@@ -62,6 +65,8 @@ int slab_combine(const float* ws, int slabs, long long stride, long long rows, i
 
 int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K,
               GemmEpilogue ep, int tile_n, int split_k, cudaStream_t stream);
+int gemm_e4m3(const void* A, int lda, const float* sa, const void* B, int ldb, const float* sb, int M, int N, int K,
+              GemmEpilogue ep, cudaStream_t stream);
 
 #define D3_CHECK_LAUNCH()                                               \
   do {                                                                  \

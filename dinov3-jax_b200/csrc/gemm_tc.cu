@@ -351,11 +351,45 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[MH][BN / 2], uint32_t sa
   }
 }
 
-template <int BN, int A_MN, int B_MN, int EF>
+// E4M3 (both operands K-major): a 128-element k-block of 128-byte rows has the same SWIZZLE_128B layout as a bf16
+// k-block of 64; a k32 step advances 32 bytes.  This is half of it, k32 steps 2 h and 2 h + 1, chained from zero: the
+// caller promotes the sum into the fp32 accumulator.
+template <int MH, int BN>
+__device__ __forceinline__ void mma_khalf_e4m3(float (&acc)[MH][BN / 2], uint32_t sa, uint32_t sb, int h) {
+  static_assert(BN == 64, "the e4m3 GEMM runs 128 x 64 tiles");
+  const uint64_t bd = gmma_desc_sw128(sb, 16, 1024);
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+#pragma unroll
+    for (int mh = 0; mh < MH; ++mh) {
+      const uint64_t ad = gmma_desc_sw128(sa + mh * 8192, 16, 1024);
+      wgmma_m64n64k32_e4m3(acc[mh], ad + (2 * h + k) * (32 >> 4), bd + (2 * h + k) * (32 >> 4), k == 0 ? 0u : 1u);
+    }
+  }
+}
+
+template <int MH, int BN>
+__device__ __forceinline__ void add_acc(float (&acc)[MH][BN / 2], const float (&part)[MH][BN / 2]) {
+#pragma unroll
+  for (int mh = 0; mh < MH; ++mh)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[mh][i] = __fadd_rn(acc[mh][i], part[mh][i]);
+}
+
+// E4M3 = true: A [M, K] and B [N, K] are e4m3 bytes (K-major), sa [M] / sb [N] their power-of-two row scales.  Every 64
+// k-elements (half a k-block) the tensor core's sum goes into a zeroed temporary that is added to the fp32 accumulator
+// once it completes (two-level FP8 accumulation: the tensor core's FP8 sums keep fewer bits than fp32; promoting every
+// 128 left 6.8e-4 relative error at K = 4096 on all-positive operands).  The add waits for the wgmma: a second
+// temporary to overlap them would take the consumer past the 168 registers a thread of a 384-thread CTA is compiled
+// for, and reading one while the other is in flight serializes the wgmma (C7514).
+// The accumulator is multiplied by sa[m] sb[n] (exact: powers of two) before the epilogue.
+template <int BN, int A_MN, int B_MN, int EF, bool E4M3 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmP, const GemmEpilogue ep,
-            int M, int N, int K, int splits) {
+            int M, int N, int K, int splits, const float* scale_a, const float* scale_b) {
+  static_assert(!E4M3 || (BN == 64 && !A_MN && !B_MN), "e4m3: 128 x 64 tiles, both operands K-major");
+  constexpr int KB = E4M3 ? 128 : BK;    // elements per k-block (128 bytes per row either way)
   constexpr bool staged = kStaged<EF>;   // tmO / tmP (out, pre-activation stash) are used only then
   using C = Cfg<BN, staged>;
   constexpr bool WIDE = C::WIDE;
@@ -386,7 +420,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
   const int num_m = (M + BM - 1) / BM;
   const int num_n = WIDE ? (N + BN - 1) / BN : ((N + BN - 1) / BN + 1) / 2;
-  const int num_k = (K + BK - 1) / BK;
+  const int num_k = (K + KB - 1) / KB;
   const int num_tiles = (WIDE ? (num_m + 1) / 2 : num_m) * num_n;
   const int num_work = num_tiles * splits;
 
@@ -406,27 +440,27 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           if constexpr (WIDE) {            // own 128 rows of A (two 64-row boxes), 128-column half of B to both
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
-              if (A_MN) tma_load_2d(&tmA, &full_bar[stage], sa + i * 8192, wr.m0 + i * 64, kb * BK);
-              else tma_load_2d(&tmA, &full_bar[stage], sa + i * 8192, kb * BK, wr.m0 + i * 64);
+              if (A_MN) tma_load_2d(&tmA, &full_bar[stage], sa + i * 8192, wr.m0 + i * 64, kb * KB);
+              else tma_load_2d(&tmA, &full_bar[stage], sa + i * 8192, kb * KB, wr.m0 + i * 64);
             }
             if (B_MN) {
 #pragma unroll
               for (int i = 2 * rank; i < 2 * rank + 2; ++i)
-                tma_load_2d_multicast(&tmB, &full_bar[stage], sb + i * 8192, wr.n0 + i * 64, kb * BK, 0b11);
+                tma_load_2d_multicast(&tmB, &full_bar[stage], sb + i * 8192, wr.n0 + i * 64, kb * KB, 0b11);
             } else {
-              tma_load_2d_multicast(&tmB, &full_bar[stage], sb + rank * 16384, kb * BK, wr.n0 + rank * 128, 0b11);
+              tma_load_2d_multicast(&tmB, &full_bar[stage], sb + rank * 16384, kb * KB, wr.n0 + rank * 128, 0b11);
             }
           } else {                         // 64-row half of A to both, own B
             if (A_MN) {
-              tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, wr.m0 + rank * 64, kb * BK, 0b11);
+              tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, wr.m0 + rank * 64, kb * KB, 0b11);
             } else {
-              tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, kb * BK, wr.m0 + rank * 64, 0b11);
+              tma_load_2d_multicast(&tmA, &full_bar[stage], sa + rank * 8192, kb * KB, wr.m0 + rank * 64, 0b11);
             }
             if (B_MN) {
 #pragma unroll
-              for (int i = 0; i < BN / 64; ++i) tma_load_2d(&tmB, &full_bar[stage], sb + i * 8192, wr.n0 + i * 64, kb * BK);
+              for (int i = 0; i < BN / 64; ++i) tma_load_2d(&tmB, &full_bar[stage], sb + i * 8192, wr.n0 + i * 64, kb * KB);
             } else {
-              tma_load_2d(&tmB, &full_bar[stage], sb, kb * BK, wr.n0);
+              tma_load_2d(&tmB, &full_bar[stage], sb, kb * KB, wr.n0);
             }
           }
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
@@ -474,29 +508,67 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       for (int mh = 0; mh < MH; ++mh)
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[mh][i] = 0.f;
-      int prev = -1;
-      for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
+      if constexpr (E4M3) {
+        float part[MH][BN / 2];
+        for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
 #pragma unroll
-        for (int mh = 0; mh < MH; ++mh) fence_regs(acc[mh]);
-        wgmma_fence();
-        mma_kblock<MH, BN, A_MN, B_MN>(acc, sa + (WIDE ? cw * 8192 : 0), sa + C::A_BYTES, kb == wr.kb0);
-        wgmma_commit();
+          for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int mh = 0; mh < MH; ++mh) fence_regs(acc[mh]);
-        if (prev >= 0) {                       // the k-block before this one has been consumed: release its stage
-          wgmma_wait<1>();
-          if (t == 0) { mbar_arrive(&empty_bar[prev]); mbar_arrive_cluster(peer_empty + 8 * prev); }
+            for (int mh = 0; mh < MH; ++mh) fence_regs(part[mh]);
+            wgmma_fence();
+            mma_khalf_e4m3<MH, BN>(part, sa, sa + C::A_BYTES, h);
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int mh = 0; mh < MH; ++mh) fence_regs(part[mh]);
+            if (h == 1 && t == 0) { mbar_arrive(&empty_bar[stage]); mbar_arrive_cluster(peer_empty + 8 * stage); }
+            add_acc<MH, BN>(acc, part);
+          }
+          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
-        prev = stage;
-        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (!WIDE && w + num_clusters < num_work) named_bar_arrive(1 + (cw ^ 1), 256);   // tile j+1 may start its main loop
-      wgmma_wait<0>();
+        if (!WIDE && w + num_clusters < num_work) named_bar_arrive(1 + (cw ^ 1), 256);   // tile j+1 may start its main loop
+        // dequantise: rows r_in, r_in + 8 of each 64-row half, columns 8 i + c_in, + 1
 #pragma unroll
-      for (int mh = 0; mh < MH; ++mh) fence_regs(acc[mh]);
-      if (prev >= 0 && t == 0) { mbar_arrive(&empty_bar[prev]); mbar_arrive_cluster(peer_empty + 8 * prev); }
+        for (int mh = 0; mh < MH; ++mh)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = wr.m0 + mh * 64 + r_in + 8 * h;
+            const float s_row = row < M ? scale_a[row] : 0.f;
+#pragma unroll
+            for (int i = 0; i < BN / 8; ++i) {
+              const int n = wr.n0 + 8 * i + c_in;
+              const float s0 = n < N ? scale_b[n] : 0.f, s1 = n + 1 < N ? scale_b[n + 1] : 0.f;
+              acc[mh][4 * i + 2 * h] = __fmul_rn(__fmul_rn(acc[mh][4 * i + 2 * h], s_row), s0);
+              acc[mh][4 * i + 2 * h + 1] = __fmul_rn(__fmul_rn(acc[mh][4 * i + 2 * h + 1], s_row), s1);
+            }
+          }
+      } else {
+        int prev = -1;
+        for (int kb = wr.kb0; kb < wr.kb1; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
+#pragma unroll
+          for (int mh = 0; mh < MH; ++mh) fence_regs(acc[mh]);
+          wgmma_fence();
+          mma_kblock<MH, BN, A_MN, B_MN>(acc, sa + (WIDE ? cw * 8192 : 0), sa + C::A_BYTES, kb == wr.kb0);
+          wgmma_commit();
+#pragma unroll
+          for (int mh = 0; mh < MH; ++mh) fence_regs(acc[mh]);
+          if (prev >= 0) {                       // the k-block before this one has been consumed: release its stage
+            wgmma_wait<1>();
+            if (t == 0) { mbar_arrive(&empty_bar[prev]); mbar_arrive_cluster(peer_empty + 8 * prev); }
+          }
+          prev = stage;
+          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        }
+        if (!WIDE && w + num_clusters < num_work) named_bar_arrive(1 + (cw ^ 1), 256);   // tile j+1 may start its main loop
+        wgmma_wait<0>();
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh) fence_regs(acc[mh]);
+        if (prev >= 0 && t == 0) { mbar_arrive(&empty_bar[prev]); mbar_arrive_cluster(peer_empty + 8 * prev); }
+      }
       if constexpr (stage_vecs) {
         cp_async_wait_all();
         named_bar_sync(3 + cw * !WIDE, VEC_THREADS);   // bias / gamma of this tile are in shared memory
@@ -530,11 +602,11 @@ static int make_operand_map(CUtensorMap* map, const void* ptr, int mn, int k, in
   return encode_tensor_map_2d_bf16(map, ptr, dims, strides, box, estr);
 }
 
-template <int BN, int A_MN, int B_MN, int EF>
+template <int BN, int A_MN, int B_MN, int EF, bool E4M3 = false>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M, int N, int K,
-                  int splits, cudaStream_t stream) {
+                  int splits, cudaStream_t stream, const float* scale_a = nullptr, const float* scale_b = nullptr) {
   using C = Cfg<BN, kStaged<EF>>;
-  auto kern = gemm_kernel<BN, A_MN, B_MN, EF>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EF, E4M3>;
   cudaLaunchAttribute attr{};
   attr.id = cudaLaunchAttributeClusterDimension;
   attr.val.clusterDim.x = 2;
@@ -571,7 +643,7 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilog
   const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
   const int work = (BN == 256 ? (num_m + 1) / 2 * num_n : num_m * ((num_n + 1) / 2)) * splits;   // tile pairs
   cfg.gridDim = dim3(2 * (work < max_clusters ? work : max_clusters));
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, to, tp, ep, M, N, K, splits);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, to, tp, ep, M, N, K, splits, scale_a, scale_b);
   if (e == cudaSuccess) e = cudaPeekAtLastError();
   if (e != cudaSuccess) return set_error(D3_ERR_CUDA, cudaGetErrorString(e));
   count_launch();
@@ -717,6 +789,57 @@ int gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn
     slab_release(ws, stream);
   }
   return rc;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// E4M3: out = epilogue(alpha * (A B^T) * sa[m] * sb[n]), A [M, K] and B [N, K] e4m3 bytes, K-major (FP8 wgmma has no
+// transpose bits), on 128 x 64 tiles: two m64n64 chains and their two promotion temporaries fit a consumer's registers,
+// two m64n128 chains would not.  No split-K and no scatter: the block linears' forward and input-gradient GEMMs.
+static int dispatch_e4m3(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int M, int N, int K,
+                         const float* sa, const float* sb, cudaStream_t s) {
+  if (!(ep.flags & EP_SLOW) && N % 2 == 0) {
+    const int f = ep.flags & EPI_FLAGS;
+#define D3_EPI(F) \
+    if (f == (F)) return launch<64, 0, 0, (F), true>(ta, tb, ep, M, N, K, 1, s, sa, sb);
+    // forward: qkv (with and without a bias), fc1 / w1 / w2, proj, fc2 / w3 (with and without the stash)
+    D3_EPI(0)
+    D3_EPI(EP_BIAS)
+    D3_EPI(EP_BIAS | EP_GELU)
+    D3_EPI(EP_BIAS | EP_GELU | EP_STORE_PRE)
+    D3_EPI(EP_BIAS | EP_GAMMA | EP_RESID | EP_OUT_F32)
+    D3_EPI(EP_BIAS | EP_STORE_PRE | EP_GAMMA | EP_RESID | EP_OUT_F32)
+    D3_EPI(EP_BIAS | EP_GELU | EP_GAMMA | EP_RESID | EP_OUT_F32)
+    D3_EPI(EP_BIAS | EP_GELU | EP_STORE_PRE | EP_GAMMA | EP_RESID | EP_OUT_F32)
+    // input gradients: dQKV / dP Wᵀ, fc2's through GELU', swiglu's fp32 dz = dx1 W1ᵀ + dx2 W2ᵀ
+    D3_EPI(EP_MUL_DGELU)
+    D3_EPI(EP_OUT_F32)
+    D3_EPI(EP_OUT_F32 | EP_ACCUM)
+#undef D3_EPI
+  }
+  return launch<64, 0, 0, EPI_RUNTIME, true>(ta, tb, ep, M, N, K, 1, s, sa, sb);
+}
+
+int gemm_e4m3(const void* A, int lda, const float* sa, const void* B, int ldb, const float* sb, int M, int N, int K,
+              GemmEpilogue ep, cudaStream_t stream) {
+  if (M <= 0 || N <= 0 || K <= 0) return set_error(D3_ERR_ARG, "gemm_e4m3: empty problem");
+  if (K % 16) return set_error(D3_ERR_ARG, "gemm_e4m3: K must be a multiple of 16");
+  if ((lda % 16) || (ldb % 16) || (reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(B) & 15))
+    return set_error(D3_ERR_ARG, "gemm_e4m3: operands must be 16-byte aligned with ld % 16 == 0");
+  if (ep.flags & (EP_SCATTER | EP_GELU_ERF)) return set_error(D3_ERR_ARG, "gemm_e4m3: SCATTER / GELU_ERF not supported");
+  const int out_elt = (ep.flags & EP_OUT_F32) ? 4 : 2;
+  bool aligned = ((uintptr_t)ep.out % 16 == 0) && ((ep.ld_out * out_elt) % 16 == 0);
+  if (ep.flags & EP_BIAS) aligned = aligned && ((uintptr_t)ep.bias % 16 == 0);
+  if (ep.flags & EP_GAMMA) aligned = aligned && ((uintptr_t)ep.gamma % 16 == 0);
+  if (ep.flags & EP_RESID) aligned = aligned && ((uintptr_t)ep.resid % 16 == 0) && (ep.ld_resid % 4 == 0);
+  if (ep.flags & EP_STORE_PRE) aligned = aligned && ((uintptr_t)ep.aux_out % 16 == 0) && (ep.ld_aux % 8 == 0);
+  if (ep.flags & EP_MUL_DGELU) aligned = aligned && ((uintptr_t)ep.aux_in % 16 == 0) && (ep.ld_aux % 8 == 0);
+  if (!aligned) ep.flags |= EP_SLOW;
+  CUtensorMap ta, tb;
+  int rc = encode_tensor_map_2d_u8(&ta, A, K, M, lda, 128, 64);   // A: one 64-row half per cluster CTA
+  if (rc) return rc;
+  rc = encode_tensor_map_2d_u8(&tb, B, K, N, ldb, 128, 64);
+  if (rc) return rc;
+  return dispatch_e4m3(ta, tb, ep, M, N, K, sa, sb, stream);
 }
 
 }  // namespace d3

@@ -40,6 +40,9 @@ P, I, LL, F = C.c_void_p, C.c_int, C.c_longlong, C.c_float
 SIGNATURES = {
     "d3_init": [I],
     "d3_gemm_bf16": [P, I, I, P, I, I, I, I, I, C.POINTER(GemmEpilogue), I, I, P],
+    "d3_quant_rows_e4m3": [P, I, I, I, P, I, P, P],
+    "d3_quant_cols_e4m3_t": [P, I, I, I, P, I, P, P],
+    "d3_gemm_e4m3": [P, I, P, P, I, P, I, I, I, C.POINTER(GemmEpilogue), P],
     "d3_scatter_add_peers": [P, LL, P, I, LL, I, F, P],
     "d3_allreduce_peers": [P, I, P, LL, I, P],
     "d3_im2col": [P, P, I, I, I, I, I, P],

@@ -16,7 +16,7 @@ import torch
 
 from .. import ops
 from .config import EngineConfig
-from .forward import CropSet, HeadBufs, Net, Stream, backbone_fwd, block_fwd, head_fwd
+from .forward import CropSet, HeadBufs, Net, Stream, backbone_fwd, block_fwd, dgrad, head_fwd
 from .forward import rope_tables  # noqa: F401  (engine.core.rope_tables stays importable for existing callers)
 from .params import FrozenStore, ParamStore, backbone_spec, head_spec
 
@@ -53,10 +53,13 @@ class Engine:
 
     def __init__(self, cfg: EngineConfig, B: int, device="cuda", max_masked: int | None = None, comm=None,
                  centering: str = "sinkhorn_knopp", center_momentum: float = 0.9, remat: bool = False,
-                 distill: EngineConfig | None = None):
+                 distill: EngineConfig | None = None, fp8: bool = False):
         """`distill`: the configuration of a frozen teacher of another architecture (distillation.enabled,
         train/ssl_meta_arch.py:257-286).  It replaces the EMA teacher in the forward; the EMA of the student is still
-        kept in the teacher_* buffers.  Its weights come from `distill_teacher_load`."""
+        kept in the teacher_* buffers.  Its weights come from `distill_teacher_load`.
+        `fp8` (student.fp8_enabled, fp8_filter: blocks): the block linears (qkv, proj, fc1 / fc2 or w1 / w2 / w3) of
+        every backbone the step runs compute their forward and input gradients in e4m3 with row-wise power-of-two
+        scales (d3_gemm_e4m3); their weight gradients stay bf16.  The heads, patch embedding and attention stay bf16."""
         for c in (cfg, distill):
             if c is not None:
                 assert c.head_dim in (64, 128), "attention kernels exist for head_dim 64 (ViT-S ... giant2) and 128 (vit_7b)"
@@ -76,6 +79,12 @@ class Engine:
             raise NotImplementedError(f"embed_dim {cfg.embed_dim}: the LayerNorm backward (d3_layernorm_bwd_ls) takes rows of "
                                       "at most 1536 columns, so training stops at ViT-giant2 width; vit_7b (4096) runs "
                                       "forward through dinov3_jax.models.DinoVisionTransformer")
+        if fp8:
+            for c in (cfg, distill):
+                if c is not None and (c.embed_dim % 16 or c.ffn_width % 16):
+                    raise NotImplementedError(f"fp8: the e4m3 GEMM contracts over multiples of 16; embed_dim "
+                                              f"{c.embed_dim} / ffn width {c.ffn_width} is not")
+        self.fp8 = bool(fp8)
         assert centering in ("sinkhorn_knopp", "softmax")
         self.centering, self.center_momentum = centering, center_momentum
         # activation rematerialisation (train.checkpointing, ssl_default_config.yaml:88): only the block inputs X[i] of
@@ -95,13 +104,13 @@ class Engine:
         self.fsdp = FsdpRuntime(comm, self.params.mods, dev)
         self.params.runtime = self.fsdp
         self.distill = distill
-        self.student_net = Net(cfg, self.params.mods, False, self.fsdp)
+        self.student_net = Net(cfg, self.params.mods, False, self.fsdp, fp8=self.fp8)
         if distill is None:
-            self.t_net = Net(cfg, self.params.mods, True, self.fsdp)
+            self.t_net = Net(cfg, self.params.mods, True, self.fsdp, fp8=self.fp8)
         else:
             self.t_net = Net(distill, {"backbone": FrozenStore(backbone_spec(distill), dev),
                                        "dino_head": FrozenStore(head_spec(distill, "dino_head"), dev),
-                                       "ibot_head": FrozenStore(head_spec(distill, "ibot_head"), dev)}, True)
+                                       "ibot_head": FrozenStore(head_spec(distill, "ibot_head"), dev)}, True, fp8=self.fp8)
         tcfg = self.t_net.cfg
         ng, nl = cfg.n_global * B, cfg.n_local * B
         # teacher stream: global crops only (at the teacher's width); student stream: global then local rows
@@ -110,7 +119,7 @@ class Engine:
         self.s_sets = [CropSet(cfg, ng, gp, gp, 0, dev)]
         self.s_sets.append(CropSet(cfg, nl, lp, lp, self.s_sets[0].T, dev))
         self.teacher = Stream(tcfg, self.t_sets, dev, stash=False)
-        self.student = Stream(cfg, self.s_sets, dev, stash=True, remat=self.remat)
+        self.student = Stream(cfg, self.s_sets, dev, stash=True, remat=self.remat, fp8=self.fp8)
         P = self.s_sets[0].P
         if max_masked is None:
             n_masked_crops = int(ng * cfg.mask_probability)
@@ -245,7 +254,7 @@ class Engine:
             self.gram_active = True
         else:
             # frozen full copy on every rank, in the backbone's flat layout (the snapshot copies the EMA teacher's)
-            self.gram_net = Net(cfg, {"backbone": FrozenStore(backbone_spec(cfg), dev)}, True)
+            self.gram_net = Net(cfg, {"backbone": FrozenStore(backbone_spec(cfg), dev)}, True, fp8=self.fp8)
             gs = cfg.gram_teacher_size
             if gs is not None and gs != cfg.global_size and cfg.gram_tokens_used != "all":
                 raise NotImplementedError("gram.tokens_used masked | unmasked with a gram teacher at its own resolution")
@@ -512,6 +521,7 @@ class Engine:
         par = (i & 1) if self.wgrad_overlap else 0
         dU2, dU1, dP, dQKV = self.dU2[par], self.dU1[par], self.dP[par], self.dQKV[par]
         main = torch.cuda.current_stream()
+        dg = lambda dy, n, out, **ep: dgrad(self.student_net, dy, w(n), out, **ep)   # bf16 or e4m3 (fp8)
         if self.remat:
             # recompute this block's forward from its stashed input (writes the scratch activations, statistics, LSE and
             # x_out again), then the LayerScale / activation backward of its MLP branch, which the stashing path gets
@@ -548,34 +558,36 @@ class Engine:
             Hs = cfg.swiglu_hidden
             X12, dX12 = st.b(st.U1, i), dU1
             wgrad(0, st.b(st.Hh, i), dU2, "mlp/w3/kernel")                                           # dW3 = h^T dU2
-            ops.gemm(dU2, w("mlp/w3/kernel"), self.dH)                                         # dh = dU2 W3^T
+            dg(dU2, "mlp/w3/kernel", self.dH)                                                  # dh = dU2 W3^T
             ops.swiglu_bwd(X12, self.dH, dX12)                                                 # [dx1 | dx2]
             wgrad(1, st.b(st.Z, i), dX12[:, :Hs], "mlp/w1/kernel")                                   # dW1 = z^T dx1
             wgrad(1, st.b(st.Z, i), dX12[:, Hs:], "mlp/w2/kernel")                                   # dW2 = z^T dx2
             on_wstream(1, lambda: (ops.colsum_bf16(dX12[:, :Hs], gv("mlp/w1/bias")), ops.colsum_bf16(dX12[:, Hs:], gv("mlp/w2/bias"))))
-            ops.gemm(dX12[:, :Hs], w("mlp/w1/kernel"), self.dZ32)                              # dz = dx1 W1^T + dx2 W2^T (fp32)
-            ops.gemm(dX12[:, Hs:], w("mlp/w2/kernel"), self.dZ32, accum=True)
+            dg(dX12[:, :Hs], "mlp/w1/kernel", self.dZ32)                                       # dz = dx1 W1^T + dx2 W2^T (fp32)
+            dg(dX12[:, Hs:], "mlp/w2/kernel", self.dZ32, accum=True)
             dZ = self.dZ32
         else:
             wgrad(0, st.b(st.Hh, i), dU2, "mlp/Dense_1/kernel")                                      # dW2 = h^T dU2
-            ops.gemm(dU2, w("mlp/Dense_1/kernel"), dU1, dgelu_of=st.b(st.U1, i))                     # dU1 = (dU2 W2^T) * gelu'(u1)
+            dg(dU2, "mlp/Dense_1/kernel", dU1, dgelu_of=st.b(st.U1, i))                              # dU1 = (dU2 W2^T) * gelu'(u1)
             wgrad(1, st.b(st.Z, i), dU1, "mlp/Dense_0/kernel")                                       # dW1 = z^T dU1
             # bias gradients are column sums that only feed the optimizer: they ride on the weight-gradient stream
             on_wstream(1, lambda: ops.colsum_bf16(dU1, gv("mlp/Dense_0/bias")))
-            ops.gemm(dU1, w("mlp/Dense_0/kernel"), self.dZ)                                    # dZ = dU1 W1^T
+            dg(dU1, "mlp/Dense_0/kernel", self.dZ)                                             # dZ = dU1 W1^T
             dZ = self.dZ
-        # LN2 backward; its tail is the attention branch's LayerScale: x_mid = x_in + g1 * (o Wp + bp), dP = dXmid * g1
+        # LN2 backward; its tail is the attention branch's LayerScale: x_mid = x_in + g1 * p, p = o Wp + bp, dP = dXmid * g1.
+        # With fp8, p is not o Wp + bp in high precision, so dg1 = colsum(dXmid * p) comes from the stashed p.
+        ls1 = dict(ls_u=st.b(st.Pa, i), ls_dgamma=gv("ls1/gamma")) if self.fp8 else {}
         ops.layernorm_bwd_ls(dZ, st.b(st.Xmid, i), m2, r2, v("norm2/scale"), self.dXmid, dx_add=dX,
                              dscale=gv("norm2/scale"), dbias=gv("norm2/bias"),
-                             ls_gamma=v("ls1/gamma"), ls_du=dP, ls_dbias=gv("attn/proj/bias"))
+                             ls_gamma=v("ls1/gamma"), ls_du=dP, ls_dbias=gv("attn/proj/bias"), **ls1)
 
         def proj_wgrad():
             ops.gemm(st.b(st.O, i), dP, gw("attn/proj/kernel"), a_mn=True, b_mn=True, accum=True)    # dWp = o^T dP
-            # dg1 from dWp / dbp (no stash of the projection output needed)
-            ops.ls_gamma_from_wgrad(w("attn/proj/kernel"), gw("attn/proj/kernel"), v("attn/proj/bias"),
-                                    gv("attn/proj/bias"), v("ls1/gamma"), gv("ls1/gamma"))
+            if not self.fp8:   # dg1 from dWp / dbp (no stash of the projection output needed)
+                ops.ls_gamma_from_wgrad(w("attn/proj/kernel"), gw("attn/proj/kernel"), v("attn/proj/bias"),
+                                        gv("attn/proj/bias"), v("ls1/gamma"), gv("ls1/gamma"))
         on_wstream(2, proj_wgrad)
-        ops.gemm(dP, w("attn/proj/kernel"), self.dO)                                           # dO = dP Wp^T
+        dg(dP, "attn/proj/kernel", self.dO)                                                    # dO = dP Wp^T
         for cs, lse, delta in zip(st.sets, st.b(st.LSE, i), self.delta):
             sl = slice(cs.row0, cs.row0 + cs.T)
             # gradient w.r.t. the pre-RoPE projection: the inverse rotation is fused into the kernel's store stage
@@ -591,7 +603,7 @@ class Engine:
             else:
                 ops.colsum_bf16(dQKV, gv("attn/qkv/bias"))
         on_wstream(3, qkv_bias_grad)
-        ops.gemm(dQKV, w("attn/qkv/kernel"), self.dY)                                          # dY = dQKV Wqkv^T
+        dg(dQKV, "attn/qkv/kernel", self.dY)                                                   # dY = dQKV Wqkv^T
         tail = self._ls_tail(i - 1) if (i > 0 and not self.remat) else {}
         ops.layernorm_bwd_ls(self.dY, st.X[i], m1, r1, v("norm1/scale"), dXprev, dx_add=self.dXmid,
                              dscale=gv("norm1/scale"), dbias=gv("norm1/bias"), **tail)

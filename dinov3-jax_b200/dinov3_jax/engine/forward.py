@@ -9,7 +9,7 @@ import torch
 from .. import ops
 from .config import EngineConfig
 
-f32, bf16 = torch.float32, torch.bfloat16
+f32, bf16, u8 = torch.float32, torch.bfloat16, torch.uint8
 
 
 def rope_tables(Hp: int, Wp: int, head_dim: int, base: float, device):
@@ -47,7 +47,7 @@ class CropSet:
 class Stream:
     """Activation buffers of one network pass over a list of crop sets (teacher: global only; student: global+local)."""
 
-    def __init__(self, cfg: EngineConfig, sets, device, stash: bool, remat: bool = False):
+    def __init__(self, cfg: EngineConfig, sets, device, stash: bool, remat: bool = False, fp8: bool = False):
         D, Hd, L = cfg.embed_dim, cfg.ffn_width, cfg.depth
         swiglu = cfg.ffn_layer == "swiglu"
         self.sets = sets
@@ -64,11 +64,14 @@ class Stream:
         self.Z = [e(T, D) for _ in range(nb)]
         self.Hh = [e(T, Hd) for _ in range(nb)]
         self.Xn = e(T, D, dt=f32) if stash else self.X[(L + 1) % 2]   # no stash: the buffer block L-1 read from
+        self.Pa = None
         self.X12 = e(T, 2 * Hd) if (swiglu and not stash) else None       # teacher pass: [x1 | x2] scratch
         self.LSE = [[e(s.n, cfg.heads, s.N, dt=f32) for s in sets] for _ in range(nb)]
         if stash:
             self.U1 = [e(T, 2 * Hd if swiglu else Hd) for _ in range(nb)]   # mlp: u1; swiglu: [x1 | x2]
             self.U2 = [e(T, D) for _ in range(nb)]
+            # FP8: the attention projection before LayerScale 1, whose gradient the backward takes from it
+            self.Pa = [e(T, D) for _ in range(nb)] if fp8 else None
             self.stats = [[e(T, dt=f32) for _ in range(4)] for _ in range(nb)]   # mean1, rstd1, mean2, rstd2
             self.fstats = [e(T, dt=f32), e(T, dt=f32)]
 
@@ -104,14 +107,53 @@ class HeadBufs:
 class Net:
     """What one forward pass reads: a model's configuration and its weights.  `mods` maps "backbone" / "dino_head" /
     "ibot_head" to stores with w(name, teacher) / vec(name, teacher); `teacher` selects the EMA copy of a ParamStore.
-    `fsdp` gathers a unit before it is read; None when the weights are resident (a FrozenStore)."""
+    `fsdp` gathers a unit before it is read; None when the weights are resident (a FrozenStore).
+    `fp8`: the block linears run in e4m3 (`linear`, `dgrad`) on scratch that belongs to this Net, so passes on other
+    streams do not share it."""
 
-    def __init__(self, cfg: EngineConfig, mods: dict, teacher: bool, fsdp=None):
+    def __init__(self, cfg: EngineConfig, mods: dict, teacher: bool, fsdp=None, fp8: bool = False):
         self.cfg, self.mods, self.teacher, self.fsdp = cfg, mods, teacher, fsdp
+        self.fp8 = bool(fp8)
+        self._scratch = {}
 
     def acquire(self, module: str, unit: str):
         if self.fsdp is not None:
             self.fsdp.acquire(module, unit, self.teacher)
+
+    def scratch(self, key: str, shape, dtype, device):
+        """A [shape] view of this Net's buffer `key`, grown when a call needs more (stream order keeps reuse safe)."""
+        n = math.prod(shape)
+        b = self._scratch.get(key)
+        if b is None or b.numel() < n:
+            b = self._scratch[key] = torch.empty(n, dtype=dtype, device=device)
+        return b[:n].view(*shape)
+
+
+def _e4m3_rows(net: Net, which: str, x):
+    """x (bf16 [R, C] view) quantized per row into net's scratch `which`: (e4m3 [R, C], fp32 scales [R])."""
+    R, C = x.shape
+    return ops.quant_rows(x, net.scratch("q" + which, (R, C), u8, x.device), net.scratch("s" + which, (R,), f32, x.device))
+
+
+def linear(net: Net, x, W, out, **ep):
+    """out = epilogue(x W) of a block linear (W [in, out]): the bf16 GEMM, or with net.fp8 x per token row and W per
+    output column in e4m3 (W^T, K-major) on d3_gemm_e4m3.  `ep`: the epilogue arguments of ops.gemm."""
+    if not net.fp8:
+        return ops.gemm(x, W, out, b_mn=True, **ep)
+    qx, sx = _e4m3_rows(net, "a", x)
+    K, Nn = W.shape
+    qw, sw = ops.quant_cols_t(W, net.scratch("qb", (Nn, K), u8, W.device), net.scratch("sb", (Nn,), f32, W.device))
+    return ops.gemm_e4m3(qx, sx, qw, sw, out, **ep)
+
+
+def dgrad(net: Net, dy, W, out, **ep):
+    """out = epilogue(dy W^T), the input gradient of a block linear: bf16, or with net.fp8 the bf16 dy and W both per
+    row in e4m3 (both K-major as they are stored, no transpose)."""
+    if not net.fp8:
+        return ops.gemm(dy, W, out, **ep)
+    qd, sd = _e4m3_rows(net, "a", dy)
+    qw, sw = _e4m3_rows(net, "b", W)
+    return ops.gemm_e4m3(qd, sd, qw, sw, out, **ep)
 
 
 def embed(net: Net, st: Stream, images, masks_list):
@@ -136,33 +178,33 @@ def block_fwd(net: Net, st: Stream, i: int):
     net.acquire("backbone", f"blocks_{i}")
     p = f"blocks_{i}/"
     v = lambda n: bb.vec(p + n, teacher)
-    w = lambda n: bb.w(p + n, teacher)
+    lin = lambda x, n, out, **ep: linear(net, x, bb.w(p + n, teacher), out, **ep)
     X, Xmid, Xo = st.x_in(i), st.b(st.Xmid, i), st.x_out(i)
     Y, QKV, O, Z, Hh = st.b(st.Y, i), st.b(st.QKV, i), st.b(st.O, i), st.b(st.Z, i), st.b(st.Hh, i)
     stats = st.b(st.stats, i) if st.stash else [None] * 4
     ops.layernorm_fwd(X, v("norm1/scale"), v("norm1/bias"), Y, stats[0], stats[1], cfg.ln_eps)
-    ops.gemm(Y, w("attn/qkv/kernel"), QKV, b_mn=True, bias=v("attn/qkv/bias") if cfg.qkv_bias else None)
+    lin(Y, "attn/qkv/kernel", QKV, bias=v("attn/qkv/bias") if cfg.qkv_bias else None)
     lses = st.b(st.LSE, i)
     for cs, lse in zip(st.sets, lses):
         q = QKV[cs.row0: cs.row0 + cs.T]
         ops.rope(q, cs.sin, cs.cos, cs.N, cfg.prefix, D, cfg.head_dim)
         ops.attn_fwd(q, O[cs.row0: cs.row0 + cs.T], lse if st.stash else None, cs.n, cs.N, D, H)
-    ops.gemm(O, w("attn/proj/kernel"), Xmid, b_mn=True, bias=v("attn/proj/bias"), gamma=v("ls1/gamma"), resid=X)
+    lin(O, "attn/proj/kernel", Xmid, bias=v("attn/proj/bias"), gamma=v("ls1/gamma"), resid=X,
+        store_pre=st.b(st.Pa, i) if st.Pa is not None else None)
     ops.layernorm_fwd(Xmid, v("norm2/scale"), v("norm2/bias"), Z, stats[2], stats[3], cfg.ln_eps)
     if cfg.ffn_layer == "swiglu":
         # SwiGLUFFN (layers/ffn_layers.py:71-76): h = silu(z W1 + b1) * (z W2 + b2); x_out = x_mid + g2 * (h W3 + b3)
         Hs = cfg.swiglu_hidden
         X12 = st.b(st.U1, i) if st.stash else st.X12
-        ops.gemm(Z, w("mlp/w1/kernel"), X12[:, :Hs], b_mn=True, bias=v("mlp/w1/bias"))
-        ops.gemm(Z, w("mlp/w2/kernel"), X12[:, Hs:], b_mn=True, bias=v("mlp/w2/bias"))
+        lin(Z, "mlp/w1/kernel", X12[:, :Hs], bias=v("mlp/w1/bias"))
+        lin(Z, "mlp/w2/kernel", X12[:, Hs:], bias=v("mlp/w2/bias"))
         ops.swiglu_fwd(X12, Hh)
-        ops.gemm(Hh, w("mlp/w3/kernel"), Xo, b_mn=True, bias=v("mlp/w3/bias"),
-                 store_pre=st.b(st.U2, i) if st.stash else None, gamma=v("ls2/gamma"), resid=Xmid)
+        lin(Hh, "mlp/w3/kernel", Xo, bias=v("mlp/w3/bias"), store_pre=st.b(st.U2, i) if st.stash else None,
+            gamma=v("ls2/gamma"), resid=Xmid)
         return
-    ops.gemm(Z, w("mlp/Dense_0/kernel"), Hh, b_mn=True, bias=v("mlp/Dense_0/bias"), gelu=True,
-             store_pre=st.b(st.U1, i) if st.stash else None)
-    ops.gemm(Hh, w("mlp/Dense_1/kernel"), Xo, b_mn=True, bias=v("mlp/Dense_1/bias"), gelu=cfg.mlp_second_act,
-             store_pre=st.b(st.U2, i) if st.stash else None, gamma=v("ls2/gamma"), resid=Xmid)
+    lin(Z, "mlp/Dense_0/kernel", Hh, bias=v("mlp/Dense_0/bias"), gelu=True, store_pre=st.b(st.U1, i) if st.stash else None)
+    lin(Hh, "mlp/Dense_1/kernel", Xo, bias=v("mlp/Dense_1/bias"), gelu=cfg.mlp_second_act,
+        store_pre=st.b(st.U2, i) if st.stash else None, gamma=v("ls2/gamma"), resid=Xmid)
 
 
 def backbone_fwd(net: Net, st: Stream, images, masks_list):

@@ -23,23 +23,8 @@ def _ld(t: torch.Tensor) -> int:
     return t.stride(0)
 
 
-def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False,
-         bias: torch.Tensor | None = None, gelu: bool = False, gelu_erf: bool = False,
-         store_pre: torch.Tensor | None = None,
-         dgelu_of: torch.Tensor | None = None, gamma: torch.Tensor | None = None,
-         resid: torch.Tensor | None = None, accum: bool = False, alpha: float = 1.0, tile_n: int = 0,
-         split_k: int = 0, scatter=None) -> torch.Tensor:
-    """out[M,N] = epilogue(alpha * A.B) on the wgmma tensor cores (d3_gemm_bf16).
-
-    A is [M,K] (a_mn=False) or stored transposed [K,M] (a_mn=True); B is [N,K] (b_mn=False) or [K,N] (b_mn=True).
-    gelu: the tanh-GELU of the ViT MLP; gelu_erf: the exact GELU (torch nn.GELU()) of the ConvNeXt block.
-    """
-    l = N.init()
-    assert A.dtype == bf16 and B.dtype == bf16
-    M, K = (A.shape[1], A.shape[0]) if a_mn else (A.shape[0], A.shape[1])
-    Nn, Kb = (B.shape[1], B.shape[0]) if b_mn else (B.shape[0], B.shape[1])
-    assert K == Kb, f"contraction mismatch {K} vs {Kb}"
-    assert out.shape[0] == M and out.shape[1] == Nn and out.dtype in (bf16, f32)
+def _epilogue(out, Nn, bias, gelu, gelu_erf, store_pre, dgelu_of, gamma, resid, accum, alpha, scatter):
+    """The d3_gemm_epilogue of a call writing `out` [M, Nn], with the flags its arguments select."""
     flags = 0
     ep = N.GemmEpilogue()
     ep.out = out.data_ptr(); ep.ld_out = _ld(out)
@@ -77,6 +62,27 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, a_mn: bool = Fa
         ep.sc_off, ep.sc_shard, ep.sc_world = int(sc_off), int(sc_shard), len(peers)
     ep.flags = flags
     ep.alpha = float(alpha)
+    return ep
+
+
+def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False,
+         bias: torch.Tensor | None = None, gelu: bool = False, gelu_erf: bool = False,
+         store_pre: torch.Tensor | None = None,
+         dgelu_of: torch.Tensor | None = None, gamma: torch.Tensor | None = None,
+         resid: torch.Tensor | None = None, accum: bool = False, alpha: float = 1.0, tile_n: int = 0,
+         split_k: int = 0, scatter=None) -> torch.Tensor:
+    """out[M,N] = epilogue(alpha * A.B) on the wgmma tensor cores (d3_gemm_bf16).
+
+    A is [M,K] (a_mn=False) or stored transposed [K,M] (a_mn=True); B is [N,K] (b_mn=False) or [K,N] (b_mn=True).
+    gelu: the tanh-GELU of the ViT MLP; gelu_erf: the exact GELU (torch nn.GELU()) of the ConvNeXt block.
+    """
+    l = N.init()
+    assert A.dtype == bf16 and B.dtype == bf16
+    M, K = (A.shape[1], A.shape[0]) if a_mn else (A.shape[0], A.shape[1])
+    Nn, Kb = (B.shape[1], B.shape[0]) if b_mn else (B.shape[0], B.shape[1])
+    assert K == Kb, f"contraction mismatch {K} vs {Kb}"
+    assert out.shape[0] == M and out.shape[1] == Nn and out.dtype in (bf16, f32)
+    ep = _epilogue(out, Nn, bias, gelu, gelu_erf, store_pre, dgelu_of, gamma, resid, accum, alpha, scatter)
     if PROFILE is not None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -85,6 +91,58 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, a_mn: bool = Fa
     if PROFILE is not None:
         e1.record()
         PROFILE.append(("gemm", 2.0 * M * Nn * K, e0, e1, (M, Nn, K, int(a_mn), int(b_mn))))
+    return out
+
+
+def quant_rows(x: torch.Tensor, q: torch.Tensor, scale: torch.Tensor):
+    """q[r] = e4m3(x[r] / scale[r]) (d3_quant_rows_e4m3): x a bf16 [R, C] view with unit inner stride, q uint8 [R, >= C]
+    (its first C columns written), scale fp32 [R] receives each row's power-of-two scale."""
+    l = N.init()
+    R, Cc = x.shape
+    assert x.dtype == bf16 and q.dtype == torch.uint8 and scale.dtype == f32 and scale.is_contiguous()
+    assert q.shape[0] == R and q.shape[1] >= Cc and scale.numel() == R
+    N.check(l.d3_quant_rows_e4m3(N.ptr(x), _ld(x), R, Cc, N.ptr(q), _ld(q), N.ptr(scale), N.stream_ptr()),
+            "d3_quant_rows_e4m3")
+    return q, scale
+
+
+def quant_cols_t(W: torch.Tensor, qt: torch.Tensor, scale: torch.Tensor):
+    """qt[c] = e4m3(W[:, c] / scale[c]) (d3_quant_cols_e4m3_t): W a bf16 [R, C] view, qt uint8 [C, >= R] (W^T, per
+    column of W), scale fp32 [C]."""
+    l = N.init()
+    R, Cc = W.shape
+    assert W.dtype == bf16 and qt.dtype == torch.uint8 and scale.dtype == f32 and scale.is_contiguous()
+    assert qt.shape[0] == Cc and qt.shape[1] >= R and scale.numel() == Cc
+    N.check(l.d3_quant_cols_e4m3_t(N.ptr(W), _ld(W), R, Cc, N.ptr(qt), _ld(qt), N.ptr(scale), N.stream_ptr()),
+            "d3_quant_cols_e4m3_t")
+    return qt, scale
+
+
+def gemm_e4m3(A: torch.Tensor, sa: torch.Tensor, B: torch.Tensor, sb: torch.Tensor, out: torch.Tensor, *,
+              bias: torch.Tensor | None = None, gelu: bool = False, store_pre: torch.Tensor | None = None,
+              dgelu_of: torch.Tensor | None = None, gamma: torch.Tensor | None = None,
+              resid: torch.Tensor | None = None, accum: bool = False, alpha: float = 1.0) -> torch.Tensor:
+    """out[M,N] = epilogue(alpha * (A B^T) * sa[m] * sb[n]) on the FP8 tensor cores (d3_gemm_e4m3).
+
+    A uint8 e4m3 [M, K] and B uint8 e4m3 [N, K] (both K-major: quant_rows / quant_cols_t outputs), sa / sb their fp32
+    row scales; the epilogue arguments are those of `gemm`.
+    """
+    l = N.init()
+    assert A.dtype == torch.uint8 and B.dtype == torch.uint8 and sa.dtype == f32 and sb.dtype == f32
+    M, K = A.shape
+    Nn, Kb = B.shape
+    assert K == Kb, f"contraction mismatch {K} vs {Kb}"
+    assert sa.numel() == M and sb.numel() == Nn and sa.is_contiguous() and sb.is_contiguous()
+    assert out.shape[0] == M and out.shape[1] == Nn and out.dtype in (bf16, f32)
+    ep = _epilogue(out, Nn, bias, gelu, False, store_pre, dgelu_of, gamma, resid, accum, alpha, None)
+    if PROFILE is not None:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    N.check(l.d3_gemm_e4m3(N.ptr(A), _ld(A), N.ptr(sa), N.ptr(B), _ld(B), N.ptr(sb), M, Nn, K, C.byref(ep),
+                           N.stream_ptr()), "d3_gemm_e4m3")
+    if PROFILE is not None:
+        e1.record()
+        PROFILE.append(("gemm_e4m3", 2.0 * M * Nn * K, e0, e1, (M, Nn, K, 0, 0)))
     return out
 
 

@@ -9,6 +9,21 @@ from __future__ import annotations
 from ..engine import Engine, config_from_reference_cfg, distill_config_from_reference_cfg
 from ..engine.params import lr_wd_multipliers
 
+FP8_FILTERS = ("blocks",)
+
+
+def fp8_from_config(config) -> bool:
+    """student.fp8_enabled / student.fp8_filter (ssl_default_config.yaml:121-122): whether the engine runs the block
+    linears in FP8.  "blocks" (qkv, proj and the MLP linears of every block) is the only filter there is."""
+    st = config.student
+    if not bool(st.get("fp8_enabled", False)):
+        return False
+    flt = st.get("fp8_filter", "blocks")
+    if flt not in FP8_FILTERS:
+        raise NotImplementedError(f"student.fp8_filter={flt!r}: FP8 runs only the block linears (fp8_filter: blocks = "
+                                  "attn.qkv, attn.proj and mlp fc1 / fc2 or w1 / w2 / w3 of every block)")
+    return True
+
 
 class SSLMetaArch:
     PARAM_MODULES = ("backbone", "dino_head", "ibot_head")
@@ -19,6 +34,7 @@ class SSLMetaArch:
         # distillation.enabled (:257-286): the frozen teacher's configuration, None without distillation
         self.distill_config = distill_config_from_reference_cfg(config)
         self.is_distillation_enabled = self.distill_config is not None
+        self.fp8 = fp8_from_config(config)                           # student.fp8_enabled, fp8_filter: blocks
         self.n_local_crops = config.crops.local_crops_number
         self.embed_dim = self.engine_config.embed_dim
         self.dino_out_dim = config.dino.head_n_prototypes
@@ -50,7 +66,8 @@ class SSLMetaArch:
         # train.checkpointing (ssl_default_config.yaml:88-89): activation rematerialisation of the student blocks
         remat = bool(self.config.train.get("checkpointing", False) or self.config.train.get("checkpointing_full", False))
         self.engine = Engine(self.engine_config, self.config.train.batch_size_per_gpu, device=device,
-                             max_masked=max_masked, comm=comm, remat=remat, distill=self.distill_config)
+                             max_masked=max_masked, comm=comm, remat=remat, distill=self.distill_config,
+                             fp8=self.fp8)
         if self.distill_config is not None:
             self.load_distillation_teacher(self.config.distillation.checkpoint_path)
         return self.engine

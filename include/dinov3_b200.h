@@ -79,6 +79,23 @@ typedef struct {
 int d3_gemm_bf16(const void* A, int lda, int a_major, const void* B, int ldb, int b_major, int M, int N, int K,
                  const d3_gemm_epilogue* ep, int tile_n, int split_k, void* stream);
 
+/* ---- FP8 (e4m3) block linears: row-wise power-of-two scales -----------------------------------------------------
+ * d3_quant_rows_e4m3: dst[r, c] = e4m3(src[r, c] / scale[r]) for a bf16 [R, C] view (row stride ld elements), with
+ *   scale[r] = 2^e, e the smallest integer with max_c |src[r, c]| <= 448 * 2^e over the row's finite elements (1 for a
+ *   row with none but zeros).  Round to nearest even; x / 2^e is exact and never exceeds 448.  A non-finite element
+ *   becomes the e4m3 NaN.  The same bits on every run.
+ * d3_quant_cols_e4m3_t: the same per column of a bf16 W [R = in, C = out], written transposed: dst [C, R] e4m3 (row
+ *   stride ld_dst bytes), scale [C].
+ * d3_gemm_e4m3: out = epilogue(alpha * sum_k A[m, k] B[n, k] * sa[m] * sb[n]) with A [M, K] and B [N, K] e4m3, both
+ *   K-major (row strides lda / ldb bytes, multiples of 16, 16-byte aligned; K % 16 == 0), the tensor core's
+ *   sum of every 64 k-elements added into the fp32 accumulator on its own.  Every epilogue flag but SCATTER and GELU_ERF; no split-K.  */
+int d3_quant_rows_e4m3(const void* src_bf16, int ld, int R, int C, void* dst_u8, int ld_dst, float* scale,
+                       void* stream);
+int d3_quant_cols_e4m3_t(const void* src_bf16, int ld, int R, int C, void* dst_u8, int ld_dst, float* scale,
+                         void* stream);
+int d3_gemm_e4m3(const void* A_u8, int lda, const float* sa, const void* B_u8, int ldb, const float* sb, int M, int N,
+                 int K, const d3_gemm_epilogue* ep, void* stream);
+
 /* ---- patch embedding / token assembly ---------------------------------------------------------------------------
  * layers/patch_embed.py:38-51: the stride==kernel conv is im2col + GEMM (d3_gemm_bf16 with the kernel viewed as
  * [p*p*3, D]); models/vision_transformer.py:173-203: where(mask, mask_token, x), prepend cls.                        */
