@@ -202,18 +202,12 @@ def engine_state(engine) -> dict:
     (count, mu, nu) over the student modules (train/train.py:95-106).  Under FSDP every rank calls this (collective
     all-gathers of the shards); rank 0 writes."""
     flat = {k: v.cpu() for k, v in engine.params.export_reference_tree("param").items()}
-    gram = getattr(engine, "gram_net", None) if getattr(engine, "gram_active", False) else None
-    if gram is not None:
-        # frozen gram teacher (gram.use_loss with its own backbone, SURVEY 8f.2; full copies on every rank): without it a
-        # resumed run would train without the Gram term until the next scheduled refresh
-        full = torch.cat([gram.mods["backbone"].bf16.float(), gram.mods["backbone"].vecs])
-        flat.update({f"gram_backbone/{k}": v.cpu() for k, v in engine.params.mods["backbone"].export_full(full).items()})
+    gram_params, gram_opt = engine.gram_state()
+    flat.update(gram_params)              # the frozen gram teacher (SURVEY 8f.2)
     params = tree_from_flat(flat)
     mu = tree_from_flat({k: v.cpu() for k, v in engine.params.export_reference_tree("m").items()})
     nu = tree_from_flat({k: v.cpu() for k, v in engine.params.export_reference_tree("v").items()})
-    opt = {"count": int(engine.step_count), "mu": mu, "nu": nu}
-    if gram is not None:
-        opt["gram_updates"] = int(engine.gram_updates)
+    opt = {"count": int(engine.step_count), "mu": mu, "nu": nu, **gram_opt}
     if getattr(engine, "centering", "sinkhorn_knopp") != "sinkhorn_knopp":
         # "state" collection of the optional softmax-centering path (loss/dino_clstoken_loss.py:19-22)
         opt["centers"] = {"dino": engine.center_dino.cpu(), "ibot": engine.center_ibot.cpu()}
@@ -223,11 +217,7 @@ def engine_state(engine) -> dict:
 def load_engine_state(engine, params: dict, optimizer_state: dict | None = None):
     flat = flat_from_tree(params)
     engine.params.load_reference_tree(flat)
-    gram = {k[len("gram_backbone/"):]: v for k, v in flat.items() if k.startswith("gram_backbone/")}
-    if gram and getattr(engine.cfg, "gram_use_loss", False) and not engine.cfg.gram_ema_teacher:
-        engine.gram_teacher_load(gram)
-        if optimizer_state is not None and "gram_updates" in optimizer_state:
-            engine.gram_updates = int(optimizer_state["gram_updates"])
+    engine.gram_load_state(flat, optimizer_state)
     if optimizer_state is not None:
         engine.step_count = int(optimizer_state["count"])
         engine.params.load_optimizer_tree(flat_from_tree(optimizer_state["mu"]), flat_from_tree(optimizer_state["nu"]))

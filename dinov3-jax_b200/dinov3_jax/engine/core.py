@@ -18,30 +18,11 @@ from .. import ops
 from .config import EngineConfig
 from .forward import CropSet, HeadBufs, Net, Stream, backbone_fwd, block_fwd, dgrad, head_fwd
 from .forward import rope_tables  # noqa: F401  (engine.core.rope_tables stays importable for existing callers)
+from .gram import GramAnchor
+from .losses import SinkhornBufs, SmallReduce, sinkhorn, softmax_center
 from .params import FrozenStore, ParamStore, backbone_spec, head_spec
 
 f32, bf16 = torch.float32, torch.bfloat16
-
-
-class SinkhornBufs:
-    """`mx`, `s`, `btot` may be views into buffers shared by the DINO and iBOT heads (`joint`): the cross-rank
-    reductions of the two Sinkhorn normalisations then travel in ONE all-reduce per stage (Engine._sinkhorn_pair).
-    The head's K prototypes sit at [off, off + K) of the joint buffers, its row total at slot `slot` after them."""
-
-    def __init__(self, R: int, K: int, device, joint=None, off: int = 0, slot: int = 0):
-        self.K, self.off = K, off
-        if joint is None:
-            self.mx = torch.empty(K, dtype=f32, device=device)  # per-prototype shift (column maxima / global max)
-            self.s = torch.empty(K, dtype=f32, device=device)
-            self.btot = torch.empty(1, dtype=f32, device=device)
-        else:
-            mx2, s2 = joint              # [K_d + K_i], [K_d + K_i + 4]: sums of both heads, then the two row totals
-            Ks = mx2.numel()
-            self.mx = mx2[off:off + K]
-            self.s = s2[off:off + K]
-            self.btot = s2[Ks + slot:Ks + slot + 1]
-        self.gmx = torch.empty(1, dtype=f32, device=device)
-        self.a = torch.empty(R, dtype=f32, device=device)
 
 
 class Engine:
@@ -134,17 +115,14 @@ class Engine:
         self.h_s_ibot = HeadBufs(cfg, "ibot_head", self.max_masked, dev, stash=True)
         self.h_t_dino = HeadBufs(tcfg, "dino_head", ng, dev, stash=False)
         self.h_t_ibot = HeadBufs(tcfg, "ibot_head", self.max_masked, dev, stash=False)
-        self.sk_mx2 = torch.empty(Ks, dtype=f32, device=dev)
-        self.sk_s2 = torch.zeros(Ks + 4, dtype=f32, device=dev)
-        self.sk_btot_local = torch.zeros(4, dtype=f32, device=dev)
-        # small cross-rank reductions (Sinkhorn vectors, gradient norms) over NVLink peer memory when the runtime has it
-        self._ar_stage = self.fsdp.setup_small_allreduce(Ks + 2 * (Ks + 4) + 4) if comm is not None else None
-        self.sk_dino = SinkhornBufs(ng, Kd, dev, joint=(self.sk_mx2, self.sk_s2), off=0, slot=0)
-        self.sk_ibot = SinkhornBufs(self.max_masked, Ki, dev, joint=(self.sk_mx2, self.sk_s2), off=Kd, slot=1)
+        # each Sinkhorn stage reduces both heads at once (4 collectives per step instead of 10): [K_d | K_i] in sk_mx2
+        self.sk_dino, self.sk_ibot = SinkhornBufs.joint([(ng, Kd), (self.max_masked, Ki)], dev)
+        self.sk_mx2 = self.sk_dino.shared["mx"]
+        self.reduce = SmallReduce(comm, {"max": Ks, "sum0": Ks + 4, "sum1": Ks + 4, "sumsq": len(self.params.mods)},
+                                  peer=self.fsdp.push, device=dev)
         # centers of the optional softmax-centering path ("state" collection of the reference: dino_clstoken_loss.py:19-22)
         self.center_dino = torch.zeros(Kd, dtype=f32, device=dev)
         self.center_ibot = torch.zeros(Ki, dtype=f32, device=dev)
-        self._colsum = torch.zeros(max(Kd, Ki), dtype=f32, device=dev)      # column sums of one head at a time
         i32 = torch.int32
         self.rows_masked_t = torch.empty(self.max_masked, dtype=i32, device=dev)
         # the masked patches' rows in the teacher stream (another prefix when a distillation teacher has other storage tokens)
@@ -192,7 +170,9 @@ class Engine:
         self._build_ce_tables()
         self._build_rows()
         self.step_count = 0
-        self._init_gram()
+        self._gram = g = GramAnchor(cfg, self.s_sets[0], dev, self.fp8) if cfg.gram_use_loss else None
+        self.gram_net = g.net if g is not None else None                  # the frozen gram teacher (None: EMA teacher)
+        self.g_sets = g.stream.sets if g is not None and g.stream is not None else None   # its own-resolution crops
         self.masks_u8 = torch.zeros(ng, P, dtype=torch.uint8, device=dev)
         self.mask_idx = torch.zeros(self.max_masked, dtype=torch.int64, device=dev)
         self.M = 0
@@ -215,163 +195,23 @@ class Engine:
             store.load(flat_from_tree(tree[m]), self.distill.mask_k_bias)
 
     # ------------------------------------------------------------------------------------------------ Gram anchoring
-    def _init_gram(self):
-        """Buffers of the Gram-anchoring term (SURVEY 8f.2; loss/gram_loss.py:13-50, train/ssl_meta_arch.py:165-254,527-541):
-        MSE between the patch-similarity matrices of the student's and a gram teacher's global-crop patch tokens, over
-        the rank's whole local batch (gram.img_level: false).  The gram teacher is the EMA teacher itself
-        (gram.ema_teacher: true) or a frozen snapshot of it (`gram_teacher_load_from_ema`, scheduled by `gram_schedule`)
-        run through the teacher path at the global-crop resolution."""
-        cfg, dev = self.cfg, self.device
-        self.gram_active = False
-        self._gram_w = float(cfg.gram_loss_weight)
-        self._gram_snapshot_pending = False
-        self.gram_updates = 0
-        self.gram_stream, self.gram_img, self.gram_net = None, None, None
-        if not cfg.gram_use_loss:
-            return
-        assert cfg.gram_tokens_used in ("all", "masked", "unmasked")         # train/ssl_meta_arch.py:221
-        if cfg.gram_tokens_used != "all" and cfg.gram_img_level:
-            raise ValueError("gram.tokens_used masked | unmasked needs gram.img_level: false (train/ssl_meta_arch.py:222-223)")
-        sg = self.s_sets[0]
-        D = cfg.embed_dim
-        n = sg.n * sg.P
-        rows = (torch.arange(sg.n, dtype=torch.int32)[:, None] * sg.N + cfg.prefix
-                + torch.arange(sg.P, dtype=torch.int32)[None, :]).reshape(-1)
-        self.gram_rows_all = rows.to(dev)                                    # token row of every global-crop patch
-        self.gram_rows = self.gram_rows_all                                  # rows in use: all | masked | unmasked (set_batch)
-        self.gram_n = n                                                      # live row count; buffers hold the maximum
-        self.gram_block = sg.P if cfg.gram_img_level else 0                  # per-image Gram matrices: diagonal blocks
-        e = lambda *shape, dt: torch.empty(*shape, dtype=dt, device=dev)
-        npad = (n + 7) // 8 * 8
-        self.gram_fs, self.gram_ft = e(npad, D, dt=f32), e(npad, D, dt=f32)  # gathered final-norm patch tokens
-        self.gram_xs, self.gram_xt = e(npad, D, dt=bf16), e(npad, D, dt=bf16)  # (normalised) GEMM operands
-        self.gram_nrm_s, self.gram_nrm_t = e(npad, dt=f32), e(npad, dt=f32)
-        self.gram_Ss, self.gram_St = e(npad * npad, dt=f32), e(npad * npad, dt=f32)
-        self.gram_G = e(npad * npad, dt=bf16)
-        self.gram_dX, self.gram_dF = e(npad, D, dt=bf16), e(npad, D, dt=bf16)
-        self.gram_mode = ops.GRAM_MODES[(bool(cfg.gram_remove_neg), bool(cfg.gram_remove_only_teacher_neg))]
-        if cfg.gram_ema_teacher:
-            self.gram_active = True
-        else:
-            # frozen full copy on every rank, in the backbone's flat layout (the snapshot copies the EMA teacher's)
-            self.gram_net = Net(cfg, {"backbone": FrozenStore(backbone_spec(cfg), dev)}, True, fp8=self.fp8)
-            gs = cfg.gram_teacher_size
-            if gs is not None and gs != cfg.global_size and cfg.gram_tokens_used != "all":
-                raise NotImplementedError("gram.tokens_used masked | unmasked with a gram teacher at its own resolution")
-            if gs is not None and gs != cfg.global_size:
-                # the gram teacher sees its own (larger) crops: a third token stream at that resolution; its patch tokens are
-                # resized to the student's grid before the similarity matrices (upstream get_gram_teacher_output)
-                self.g_sets = [CropSet(cfg, sg.n, gs // cfg.patch, gs // cfg.patch, 0, dev)]
-                self.gram_stream = Stream(cfg, self.g_sets, dev, stash=False)
-                gp = self.g_sets[0]
-                self.gram_rows_hi = (torch.arange(gp.n, dtype=torch.int32)[:, None] * gp.N + cfg.prefix
-                                     + torch.arange(gp.P, dtype=torch.int32)[None, :]).reshape(-1).to(dev)
-                self.gram_hi = e(gp.n * gp.P, D, dt=f32)
-
-    def gram_teacher_load_from_ema(self):
-        """The gram teacher becomes a frozen copy of the current EMA teacher.  The copy is taken inside the next step,
-        right after the EMA teacher's forward, when its gathered full-size buffers are valid on every rank."""
-        assert self.cfg.gram_use_loss and not self.cfg.gram_ema_teacher
-        self._gram_snapshot_pending = True
+    @property
+    def gram_active(self) -> bool:
+        return self._gram is not None and self._gram.active
 
     def gram_teacher_load(self, tensors: dict):
-        """Gram teacher weights from a checkpoint: `tensors` maps the backbone's tensor names (reference layout, e.g.
-        'blocks_0/attn/qkv/kernel', as in export_reference_tree without the 'teacher_backbone/' prefix) to arrays."""
-        assert self.cfg.gram_use_loss and not self.cfg.gram_ema_teacher
-        store = self.gram_net.mods["backbone"]
-        store.load({name: tensors[name] for name in store.offsets}, self.cfg.mask_k_bias)
-        self.gram_active = True
+        self._gram.teacher_load(tensors)
 
     def gram_schedule(self, iteration: int):
-        """When the gram teacher is refreshed (upstream DINOv3 train loop; the reference's loop has no such code):
-        loaded from the EMA teacher at gram.it_load_ema_teacher, then, with gram.rep_update, every
-        gram.update_frequency iterations from gram.it_first_update on, at most gram.max_updates times."""
-        cfg = self.cfg
-        if not cfg.gram_use_loss or cfg.gram_ema_teacher:
-            return
-        if iteration == cfg.gram_it_load_ema_teacher:
-            self.gram_teacher_load_from_ema()
-        elif (cfg.gram_rep_update and self.gram_active and iteration >= cfg.gram_it_first_update
-              and (iteration + 1) % cfg.gram_update_frequency == 0
-              and (cfg.gram_max_updates is None or self.gram_updates < cfg.gram_max_updates)):
-            self.gram_teacher_load_from_ema()
-            self.gram_updates += 1
+        if self._gram is not None:
+            self._gram.schedule(iteration)
 
-    def _gram_features(self, Xn, feats, x_bf16, nrm):
-        """The selected global-crop patch tokens of a final-norm output -> the Gram operands (L2-normalised rows).  The row
-        count is padded to the kernels' 8-row granule with zero rows (zero similarity on both sides: no contribution)."""
-        n, D = self.gram_n, self.cfg.embed_dim
-        if n == 0:
-            return
-        npad = (n + 7) // 8 * 8
-        if self.cfg.gram_normalized:
-            ops.gather_rows(Xn, self.gram_rows, n, D, dst_f32=feats)
-            if npad > n:
-                feats[n:npad].zero_()
-            ops.l2norm_fwd(feats[:npad], x_bf16[:npad], nrm[:npad], 1e-12)
-        else:
-            ops.gather_rows(Xn, self.gram_rows, n, D, dst_bf16=x_bf16)
-            if npad > n:
-                x_bf16[n:npad].zero_()
+    def gram_state(self) -> tuple:
+        return self._gram.state() if self._gram is not None else ({}, {})
 
-    def _gram_teacher_targets(self):
-        """Called at the end of the teacher pass (the EMA teacher's outputs have been gathered into the head buffers)."""
-        cfg, T_ = self.cfg, self.teacher
-        if not cfg.gram_ema_teacher:
-            if self._gram_snapshot_pending:
-                bb, g = self.params.mods["backbone"], self.gram_net.mods["backbone"]
-                g.bf16.copy_(bb.t_bf16)
-                g.vecs.copy_(bb.t_vecs)
-                self._gram_snapshot_pending = False
-                self.gram_active = True
-            if not self.gram_active:
-                return
-            # the same kernels (and, at the global-crop resolution, the same buffers) as the EMA teacher's pass, reading
-            # the frozen weights
-            hi = self.gram_stream is not None
-            if hi and self.gram_img is None:
-                raise ValueError("no gram teacher crops in the data, have you set cfg.crops.gram_teacher_crops_size? "
-                                 "(train/ssl_meta_arch.py:310-313)")
-            backbone_fwd(self.gram_net, self.gram_stream if hi else T_, [self.gram_img if hi else self.g_img], [None])
-            if hi:
-                gp, sg, D = self.g_sets[0], self.s_sets[0], cfg.embed_dim
-                ops.gather_rows(self.gram_stream.Xn, self.gram_rows_hi, gp.n * gp.P, D, dst_f32=self.gram_hi)
-                ops.resize_tokens_bicubic(self.gram_hi, self.gram_ft[:sg.n * sg.P], gp.n, gp.Hp, gp.Wp, sg.Hp, sg.Wp, D,
-                                          cfg.gram_resize_antialias)
-                n = self.gram_n                       # all patch tokens (a multiple of 8 is not guaranteed: pad with zero rows)
-                npad = (n + 7) // 8 * 8
-                if npad > n:
-                    self.gram_ft[n:npad].zero_()
-                if cfg.gram_normalized:
-                    ops.l2norm_fwd(self.gram_ft[:npad], self.gram_xt[:npad], self.gram_nrm_t[:npad], 1e-12)
-                else:
-                    ops.cast_f32_bf16(self.gram_ft[:npad].reshape(-1), self.gram_xt[:npad].reshape(-1))
-                return
-        self._gram_features(T_.Xn, self.gram_ft, self.gram_xt, self.gram_nrm_t)
-
-    def _gram_loss_bwd(self, dXn):
-        """loss/gram_loss.py:38-50 on the tensor cores: St = Xt Xt^T, Ss = Xs Xs^T, elementwise negative removal + squared
-        difference (d3_gram_diff; per-image blocks only with gram.img_level), dXs = (4 w / count) G Xs (G symmetric), back
-        through the row normalisation, added to the gradient of the student's final-norm output."""
-        n, D = self.gram_n, self.cfg.embed_dim
-        if n == 0:
-            return
-        npad = (n + 7) // 8 * 8
-        count = float(n) * float(self.gram_block) if self.gram_block else float(n) * float(n)   # entries under the mean
-        inv = 1.0 / count
-        xs, xt = self.gram_xs[:npad], self.gram_xt[:npad]
-        Ss, St = self.gram_Ss[:npad * npad].view(npad, npad), self.gram_St[:npad * npad].view(npad, npad)
-        G = self.gram_G[:npad * npad].view(npad, npad)
-        ops.gemm(xt, xt, St)
-        ops.gemm(xs, xs, Ss)
-        ops.gram_diff(Ss, St, G, self.gram_mode, inv, self.metrics[4:5], block=self.gram_block)
-        ops.gemm(G, xs, self.gram_dX[:npad], b_mn=True, alpha=4.0 * self._gram_w * inv)
-        if self.cfg.gram_normalized:
-            ops.l2norm_bwd(self.gram_dX[:npad], self.gram_fs[:npad], self.gram_nrm_s[:npad], self.gram_dF[:npad])
-            src = self.gram_dF
-        else:
-            src = self.gram_dX
-        ops.scatter_add_rows(src, self.gram_rows, dXn, n, D)
+    def gram_load_state(self, flat: dict, optimizer_state: dict | None):
+        if self._gram is not None:
+            self._gram.load_state(flat, optimizer_state)
 
     # ------------------------------------------------------------------------------------------------ static tables
     def _build_rows(self):
@@ -415,64 +255,6 @@ class Engine:
         self.ce_ibot = (torch.arange(Mx, dtype=torch.int32, device=dev), torch.full((Mx,), -1, dtype=torch.int32, device=dev),
                         torch.full((Mx,), 1.0 / n_rows, device=dev), torch.full((Mx,), cfg.ibot_loss_weight / n_rows, device=dev),
                         torch.full((Mx,), 3, dtype=torch.int32, device=dev))
-
-    def _sinkhorn_pair(self, R_d: int, R_i: int, temp: float, n_iter: int = 3):
-        """Both heads' Sinkhorn-Knopp normalisations (DINO cls logits, iBOT masked-patch logits) in lock step: the
-        column maxima of the two heads share one all-reduce(max), and each iteration's column sums — with the two row
-        totals B riding in the same buffer — one all-reduce(sum): 4 collectives per step instead of 10 (each is latency,
-        not bandwidth: 2 x 256 KB).  With NVLink peer memory available the all-reduce is d3_allreduce_peers on inputs
-        staged in symmetric memory (FsdpRuntime.small_allreduce), otherwise NCCL.  Ks = K_d + K_i prototypes."""
-        Ks = self.sk_mx2.numel()
-        heads = [(0, self.sk_dino, self.h_t_dino.logits[:R_d], R_d)]
-        if R_i:
-            heads.append((1, self.sk_ibot, self.h_t_ibot.logits[:R_i], R_i))
-        if getattr(self, "_sk_rows", None) != (R_d, R_i):       # local row counts: device copy refreshed when M changes
-            self.sk_btot_local[0:1].fill_(float(R_d))
-            self.sk_btot_local[1:2].fill_(float(R_i))
-            self._sk_rows = (R_d, R_i)
-        stage = self._ar_stage                                   # symmetric staging: [mx Ks | s Ks+4 | s Ks+4 | sumsq 4]
-        mx_in = stage[:Ks] if stage is not None else self.sk_mx2
-        mx_in.fill_(float("-inf"))
-        for slot, sk, L, R in heads:
-            ops.colmax(L, mx_in[sk.off:sk.off + sk.K])
-        if stage is not None:
-            self.fsdp.small_allreduce(0, Ks, self.sk_mx2, "max")
-        elif self.comm is not None:
-            self.comm.all_reduce_max(self.sk_mx2)
-        a = [None, None]
-        for it in range(n_iter):
-            # staged inputs alternate between two buffers: a peer may still be reading the previous iteration's
-            off = Ks + (it & 1) * (Ks + 4)
-            s_in = stage[off:off + Ks + 4] if stage is not None else self.sk_s2
-            s_in.zero_()
-            s_in[Ks:].copy_(self.sk_btot_local)
-            for slot, sk, L, R in heads:
-                ops.sinkhorn_colsum(L, sk.mx, temp, a[slot], s_in[sk.off:sk.off + sk.K])
-            if stage is not None:
-                self.fsdp.small_allreduce(off, Ks + 4, self.sk_s2, "sum")   # psum of the row sums (:53 / ibot :99), of B
-            elif self.comm is not None:
-                self.comm.all_reduce_sum(self.sk_s2)
-            for slot, sk, L, R in heads:
-                ops.sinkhorn_rowsum(L, sk.mx, temp, sk.s, sk.btot, sk.a[:R])
-                a[slot] = sk.a[:R]
-
-    def _softmax_center(self, sk: SinkhornBufs, center, logits, R: int, temp: float, rows_local: float):
-        """softmax((x - center)/temp) after the center EMA update (loss/dino_clstoken_loss.py:24-33,91-95), expressed
-        through the same (mx, s, a, btot) scalings the cross-entropy kernel consumes."""
-        L = logits[:R]
-        colsum = self._colsum[:sk.K]
-        sk.gmx.fill_(float("-inf"))
-        sk.btot.fill_(float(rows_local))
-        ops.absmax(L, sk.gmx)
-        colsum.zero_()
-        ops.colsum_f32(L, colsum)
-        if self.comm is not None:
-            self.comm.all_reduce_max(sk.gmx)
-            self.comm.all_reduce_sum(sk.btot)
-            self.comm.all_reduce_sum(colsum)              # pmean of the local centers over "dp" (:93)
-        sk.mx.copy_(sk.gmx.expand_as(sk.mx))              # one global shift for every prototype (device-side broadcast)
-        ops.center_update(center, colsum, sk.btot, self.center_momentum, temp, sk.s)
-        ops.sinkhorn_rowsum(L, sk.mx, temp, sk.s, sk.btot, sk.a[:R])
 
     # ------------------------------------------------------------------------------------------------ backward pieces
     def _head_bwd(self, hb: HeadBufs, module: str, R: int):
@@ -641,8 +423,6 @@ class Engine:
         to = lambda t, dt=None: t.to(device=dev, dtype=dt, non_blocking=True)
         self.g_img = to(batch["collated_global_crops"], bf16).contiguous()
         self.l_img = to(batch["collated_local_crops"], bf16).contiguous()
-        if self.gram_stream is not None and batch.get("collated_gram_teacher_crops", None) is not None:
-            self.gram_img = to(batch["collated_gram_teacher_crops"], bf16).contiguous()
         masks = batch["collated_masks"]
         self.masks_u8.copy_(masks.to(torch.uint8) if masks.dtype != torch.uint8 else masks, non_blocking=True)
         idx = batch["mask_indices_list"]
@@ -652,15 +432,8 @@ class Engine:
         ops.token_rows(self.mask_idx, self.rows_masked_t, self.M, self.s_sets[0].P, 0, prefix=self.cfg.prefix)
         if self.distill is not None:
             ops.token_rows(self.mask_idx, self.rows_masked_tt, self.M, self.s_sets[0].P, 0, prefix=self.distill.prefix)
-        if self.cfg.gram_use_loss and self.cfg.gram_tokens_used != "all":
-            # gram.tokens_used (train/ssl_meta_arch.py:221-223; upstream: student_patches[masks] / [~masks])
-            n_all = self.gram_rows_all.numel()
-            if self.cfg.gram_tokens_used == "masked":
-                self.gram_rows, self.gram_n = self.rows_masked_t, self.M
-            else:
-                # stable sort of the mask bits: unmasked patch positions first, in order (no host sync, count known)
-                order = torch.argsort(self.masks_u8.reshape(-1).to(torch.int16), stable=True)[: n_all - self.M]
-                self.gram_rows, self.gram_n = self.gram_rows_all[order].contiguous(), n_all - self.M
+        if self._gram is not None:
+            self._gram.set_batch(batch, self.rows_masked_t, self.M, self.masks_u8)
 
     def teacher_pass(self, teacher_temp: float):
         """Teacher forward over the global crops, its heads and the centering of its logits (train/ssl_meta_arch.py:366-402)."""
@@ -671,13 +444,14 @@ class Engine:
         ops.gather_rows(T_.Xn, self.rows_masked_tt, M, Dt, dst_bf16=self.h_t_ibot.A0)
         head_fwd(self.t_net, self.h_t_dino, "dino_head", ng, stash=False)
         head_fwd(self.t_net, self.h_t_ibot, "ibot_head", M, stash=False)
+        heads = [(self.h_t_dino.logits[:ng], self.sk_dino), (self.h_t_ibot.logits[:M], self.sk_ibot)]
         if self.centering == "sinkhorn_knopp":
-            self._sinkhorn_pair(ng, M, teacher_temp)
+            sinkhorn(heads, teacher_temp, 3, self.reduce)
         else:
-            self._softmax_center(self.sk_dino, self.center_dino, self.h_t_dino.logits, ng, teacher_temp, ng)
-            self._softmax_center(self.sk_ibot, self.center_ibot, self.h_t_ibot.logits, M, teacher_temp, M)
-        if self.cfg.gram_use_loss:
-            self._gram_teacher_targets()
+            for (L, sk), center in zip(heads, (self.center_dino, self.center_ibot)):
+                softmax_center(L, sk, center, teacher_temp, self.center_momentum, self.reduce)
+        if self._gram is not None:
+            self._gram.teacher_targets(T_, self.g_img, self.params.mods["backbone"])
 
     def forward_backward(self, teacher_temp: float):
         cfg, B, M = self.cfg, self.B, self.M
@@ -701,14 +475,15 @@ class Engine:
             self.teacher_pass(teacher_temp)
         # ---- student (train/ssl_meta_arch.py:406-460)
         S_ = self.student
+        gram = self._gram if self.gram_active else None
         # a distilling student's global crops get no mask tokens (train/ssl_meta_arch.py:416); the iBOT loss is still
         # taken at the masked positions
         g_masks = self.masks_u8 if self.distill is None else None
         backbone_fwd(self.student_net, S_, [self.g_img, self.l_img], [g_masks, None])
         ops.gather_rows(S_.Xn, self.rows_cls_s, self.Rc, D, dst_bf16=self.h_s_dino.A0, dst_f32=self.cls_f32)
         ops.gather_rows(S_.Xn, self.rows_masked_t, M, D, dst_bf16=self.h_s_ibot.A0)
-        if self.gram_active:
-            self._gram_features(S_.Xn, self.gram_fs, self.gram_xs, self.gram_nrm_s)
+        if gram is not None:
+            gram.features(S_.Xn, student=True)
         head_fwd(self.student_net, self.h_s_dino, "dino_head", self.Rc, stash=True)
         head_fwd(self.student_net, self.h_s_ibot, "ibot_head", M, stash=True)
         # ---- losses + d(logits) (train/ssl_meta_arch.py:463-525)
@@ -737,8 +512,8 @@ class Engine:
         dXn.zero_()
         ops.scatter_add_rows(self.h_s_dino.dA0, self.rows_cls_s, dXn, self.Rc, D)
         ops.scatter_add_rows(self.h_s_ibot.dA0, self.rows_masked_t, dXn, M, D)
-        if self.gram_active:
-            self._gram_loss_bwd(dXn)
+        if gram is not None:
+            gram.loss_bwd(dXn, self.metrics)
         bb = self.params.mods["backbone"]
         dXL = self.dX[1]
         ops.layernorm_bwd_ls(dXn, S_.X[cfg.depth], S_.fstats[0], S_.fstats[1], bb.vec("norm/scale"), dXL,
@@ -771,19 +546,12 @@ class Engine:
         self.fsdp.finish_grads()
         # global gradient norm per module (SURVEY A4): sum over ranks of the shards' squares; the modules' scalars are
         # views of one buffer, so the cross-rank sum is one reduction
-        if self._ar_stage is not None:
-            Ks = self.sk_mx2.numel()                          # after the Sinkhorn ranges of _sinkhorn_pair
-            off = Ks + 2 * (Ks + 4)
-            sq_in = self._ar_stage[off:off + 4]
-            sq_in.zero_()
-            for i, st in enumerate(self.params.mods.values()):
-                ops.sumsq(st.grad_shard, sq_in[i:i + 1])
-            self.fsdp.small_allreduce(off, len(self.params.mods), self._sumsq_all, "sum")
-        else:
-            for st in self.params.mods.values():
-                ops.sumsq(st.grad_shard, st.sumsq)
-            if self.comm is not None:
-                self.comm.all_reduce_sum(self._sumsq_all)
+        sq_in = self.reduce.input("sumsq", self._sumsq_all)
+        if self.reduce.stage is not None:
+            sq_in.zero_()                 # d3_sumsq adds; the engine's own buffer was zeroed with the gradients
+        for i, st in enumerate(self.params.mods.values()):
+            ops.sumsq(st.grad_shard, sq_in[i:i + 1])
+        self.reduce(self._sumsq_all, "sum", "sumsq")
         for st in self.params.mods.values():
             ops.adamw_ema(st.master, st.grad_shard, st.m, st.v, st.t_master, st.bf16_shard, st.t_bf16_shard,
                           st.layout.n_mat_shard, st.segs, st.nseg, st.sumsq, float(cfg.clip_grad or 0.0), lr,
@@ -799,10 +567,9 @@ class Engine:
                    momentum: float, gram_loss_weight: float | None = None, iteration: int | None = None):
         if batch is not None:
             self.set_batch(batch)
-        if self.cfg.gram_use_loss:
-            if gram_loss_weight is not None:       # gram.loss_weight_schedule[iteration] (train/ssl_meta_arch.py:534-537)
-                self._gram_w = float(gram_loss_weight)
-            self.gram_schedule(self.step_count if iteration is None else int(iteration))
+        if gram_loss_weight is not None and self._gram is not None:   # gram.loss_weight_schedule[iteration] (:534-537)
+            self._gram.weight = float(gram_loss_weight)
+        self.gram_schedule(self.step_count if iteration is None else int(iteration))
         self.forward_backward(teacher_temp)
         self.optimizer_step(lr, wd, last_layer_lr, momentum)
 
@@ -823,9 +590,8 @@ class Engine:
                 + cfg.koleo_loss_weight * ng * m[2] + cfg.ibot_loss_weight * m[3])
         out = {"dino_local_crops_loss": m[0], "dino_local_loss_weight": 1.0, "dino_global_crops_loss": m[1],
                "koleo_loss": m[2], "ibot_loss": m[3], "local_batch_size": float(self.B)}
-        if self.gram_active:                       # train/ssl_meta_arch.py:538-541
-            loss += self._gram_w * m[4]
-            out["gram_loss"], out["gram_loss_weight"] = m[4], self._gram_w
+        if self.gram_active:
+            loss += self._gram.read(m, out)
         out["total_loss"] = loss
         for name, st in self.params.mods.items():
             out[f"student_{name}_grad_norm"] = math.sqrt(max(st.sumsq.item(), 0.0))

@@ -152,6 +152,11 @@ class FrozenStore:
                     third = src.numel() // 3
                     dst[third:2 * third].zero_()
 
+    def export(self) -> dict:
+        """name -> fp32 tensor (reference layout) of every weight: the inverse of `load`, matrices as stored in bf16."""
+        full = torch.cat([self.bf16.float(), self.vecs])
+        return {name: _flat_view(full, off, self.shapes[name], False).clone() for name, off in self.offsets.items()}
+
 
 class ModuleStore:
     """Flat buffers of one top-level module on one rank.

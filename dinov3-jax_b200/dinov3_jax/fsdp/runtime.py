@@ -121,30 +121,6 @@ class FsdpRuntime:
             warnings.warn(f"symmetric-memory gradient push disabled ({type(e).__name__}: {e}); using NCCL reduce-scatter")
             self.push = False
 
-    def setup_small_allreduce(self, n_floats: int):
-        """Symmetric-memory staging buffer for small all-reduces over peer mappings (d3_allreduce_peers); None when the
-        peer-memory path is not active (the caller then uses NCCL)."""
-        if not self.push:
-            return None
-        import torch.distributed._symmetric_memory as symm_mem
-        dev = next(iter(self.stores.values())).grad_shard.device
-        buf = symm_mem.empty(n_floats, dtype=torch.float32, device=dev)
-        hdl = symm_mem.rendezvous(buf, self.comm.group)
-        buf.zero_()
-        torch.cuda.synchronize()
-        torch.distributed.barrier(group=self.comm.group)
-        self._ar = (buf, hdl, [int(p) for p in hdl.buffer_ptrs])
-        return buf
-
-    def small_allreduce(self, off: int, n: int, out: torch.Tensor, op: str):
-        """out[:n] = reduce over ranks of stage[off:off+n] (every rank gets identical bits).  One symmetric-memory barrier
-        (all ranks have written their inputs; also: all ranks have finished the reads of every EARLIER reduction, which
-        is what allows a staging range to be rewritten two calls later) + one pull kernel."""
-        from .. import ops
-        buf, hdl, ptrs = self._ar
-        hdl.barrier(2)
-        ops.allreduce_peers([p + 4 * off for p in ptrs], out, n, op)
-
     def scatter_spec(self, module: str, unit_name: str, tensor: str):
         """(peer pointers at this unit's shard slice, offset of the tensor inside the unit's matrix range, shard length)
         for ops.gemm(scatter=...), or None when gradients go through NCCL."""

@@ -5,60 +5,23 @@ from __future__ import annotations
 import torch
 
 from .. import ops
+from ..engine.gram import operands, pad8, similarity_diff
+from ..engine.losses import SinkhornBufs, SmallReduce, sinkhorn, softmax_center
 
 f32 = torch.float32
 
 
-def _sinkhorn(teacher_output: torch.Tensor, teacher_temp: float, btot_local: float, n_iterations: int = 3, comm=None):
+def _teacher(teacher_output, owner=None):
+    """fp32 logits and one head's normalisation buffers; `owner`'s center ("state" collection) is created on first use."""
     L = teacher_output.to(f32).contiguous()
-    R, K = L.shape
-    dev = L.device
-    mx = torch.full((K,), float("-inf"), device=dev)      # per-prototype shift (cancels exactly, see csrc/losses.cu)
-    btot = torch.tensor([float(btot_local)], device=dev)
-    ops.colmax(L, mx)
-    if comm is not None:
-        comm.all_reduce_max(mx)
-        comm.all_reduce_sum(btot)
-    s, a_buf, a = torch.zeros(K, device=dev), torch.empty(R, device=dev), None
-    for _ in range(n_iterations):
-        s.zero_()
-        ops.sinkhorn_colsum(L, mx, teacher_temp, a, s)
-        if comm is not None:
-            comm.all_reduce_sum(s)
-        ops.sinkhorn_rowsum(L, mx, teacher_temp, s, btot, a_buf)
-        a = a_buf
-    Q = torch.empty(R, K, device=dev)
-    ops.sinkhorn_probs(L, mx, teacher_temp, s, a, btot, Q)
-    return Q
+    if owner is not None and owner.center is None:
+        owner.center = torch.zeros(L.shape[1], device=L.device)
+    return L, SinkhornBufs.joint([L.shape], L.device)[0]
 
 
-def _softmax_center(obj, teacher_output, teacher_temp: float, update: bool, probs: bool = True):
-    L = teacher_output.to(f32).contiguous()
-    R, K = L.shape
-    dev = L.device
-    if obj.center is None:
-        obj.center = torch.zeros(K, device=dev)
-    gmx = torch.full((1,), float("-inf"), device=dev)
-    rows = torch.tensor([float(R)], device=dev)
-    ops.absmax(L, gmx)
-    colsum = torch.zeros(K, device=dev)
-    if update:
-        ops.colsum_f32(L, colsum)
-    if obj.comm is not None:
-        obj.comm.all_reduce_max(gmx)
-        obj.comm.all_reduce_sum(rows)
-        if update:
-            obj.comm.all_reduce_sum(colsum)
-    s = torch.empty(K, device=dev)
-    # momentum 1.0 leaves the center untouched and only produces s[k] = exp((center[k] - max center)/temp)/K
-    ops.center_update(obj.center, colsum, rows, obj.center_momentum if update else 1.0, teacher_temp, s)
-    if not probs:
-        return None
-    mx = gmx.expand(K).contiguous()
-    a = torch.empty(R, device=dev)
-    ops.sinkhorn_rowsum(L, mx, teacher_temp, s, rows, a)
-    Q = torch.empty(R, K, device=dev)
-    ops.sinkhorn_probs(L, mx, teacher_temp, s, a, rows, Q)
+def _probs(L, sk: SinkhornBufs, teacher_temp: float):
+    Q = torch.empty_like(L)
+    ops.sinkhorn_probs(L, sk.mx, teacher_temp, sk.s, sk.a, sk.btot, Q)
     return Q
 
 
@@ -81,18 +44,20 @@ class DINOLoss:
         self.center = None          # "state" collection of the reference (:19-22): [1, K] zeros, created on first use
 
     def sinkhorn_knopp_teacher(self, teacher_output, teacher_temp, n_iterations=3, init_phase=False):
-        world = 1 if (self.comm is None or init_phase) else self.comm.world
-        return _sinkhorn(teacher_output, float(teacher_temp), teacher_output.shape[0], n_iterations,
-                         None if init_phase else self.comm)
+        L, sk = _teacher(teacher_output)
+        sinkhorn([(L, sk)], float(teacher_temp), n_iterations, SmallReduce(None if init_phase else self.comm))
+        return _probs(L, sk, float(teacher_temp))
 
     def softmax_center_teacher(self, teacher_output, teacher_temp, update_centers=True):
-        """loss/dino_clstoken_loss.py:24-33: (optionally) apply_center_update first, then softmax((x - center)/temp).
-        Same kernels as the engine's optional centering path (engine/core.py::_softmax_center)."""
-        return _softmax_center(self, teacher_output, float(teacher_temp), update_centers)
+        """loss/dino_clstoken_loss.py:24-33: (optionally) apply_center_update first, then softmax((x - center)/temp)."""
+        L, sk = _teacher(teacher_output, self)
+        softmax_center(L, sk, self.center, float(teacher_temp), self.center_momentum, SmallReduce(self.comm), update_centers)
+        return _probs(L, sk, float(teacher_temp))
 
     def apply_center_update(self, teacher_output):
         """:91-95: center <- m*center + (1-m)*pmean(mean_rows(teacher_output))."""
-        _softmax_center(self, teacher_output, 1.0, True, probs=False)
+        L, sk = _teacher(teacher_output, self)
+        softmax_center(L, sk, self.center, 1.0, self.center_momentum, SmallReduce(self.comm), probs=False)
 
     def __call__(self, student_logits, teacher_probs, ignore_diagonal=False):
         S, B, K = student_logits.shape
@@ -120,11 +85,13 @@ class iBOTPatchLoss:
 
     def softmax_center_teacher(self, teacher_patch_tokens, teacher_temp, update_centers=True):
         """loss/ibot_patch_loss.py:28-36 (same arithmetic as DINOLoss.softmax_center_teacher, rows = masked patches)."""
-        return _softmax_center(self, teacher_patch_tokens, float(teacher_temp), update_centers)
+        return DINOLoss.softmax_center_teacher(self, teacher_patch_tokens, teacher_temp, update_centers)
 
     def sinkhorn_knopp_teacher(self, teacher_output, teacher_temp, n_masked_patches_tensor, n_iterations=3, init_phase=False):
-        return _sinkhorn(teacher_output, float(teacher_temp), float(n_masked_patches_tensor.sum()), n_iterations,
-                         None if init_phase else self.comm)
+        L, sk = _teacher(teacher_output)
+        sinkhorn([(L, sk)], float(teacher_temp), n_iterations, SmallReduce(None if init_phase else self.comm),
+                 rows=(float(n_masked_patches_tensor.sum()),))
+        return _probs(L, sk, float(teacher_temp))
 
     def forward_masked(self, student_patch_tokens_masked, teacher_patch_tokens_masked, student_masks_flat,
                        n_masked_patches=None, masks_weight=None):
@@ -180,7 +147,7 @@ class GramLoss:
     features.  The value is computed with the library: row normalisation (d3_l2norm_fwd), similarity matrices on the
     tensor cores (d3_gemm_bf16, bf16 operands / fp32 accumulate), negative removal + squared difference (d3_gram_diff).
     `img_level=True` takes the diagonal (per-image) blocks of the batch's similarity matrix.  The training engine uses the same kernels with the
-    backward fused in (engine/core.py:_gram_loss_bwd)."""
+    backward fused in (engine/gram.py:GramAnchor.loss_bwd)."""
 
     def __init__(self, apply_norm: bool = True, img_level: bool = True, remove_neg: bool = True,
                  remove_only_teacher_neg: bool = False):
@@ -190,22 +157,14 @@ class GramLoss:
 
     def _one(self, s: torch.Tensor, t: torch.Tensor, acc: torch.Tensor, inv: float, block: int = 0):
         n, D = s.shape
-        pn, pd = (0 if block else -n % 8), -D % 8             # kernels work in 8-element granules; zero padding adds nothing
-        if pn or pd:
-            s, t = torch.nn.functional.pad(s, (0, pd, 0, pn)), torch.nn.functional.pad(t, (0, pd, 0, pn))
-        s, t = s.to(f32).contiguous(), t.to(f32).contiguous()
-        m = s.shape[0]
-        xs, xt = torch.empty_like(s, dtype=torch.bfloat16), torch.empty_like(t, dtype=torch.bfloat16)
-        if self.apply_norm:
-            nrm = torch.empty(m, dtype=f32, device=s.device)
-            ops.l2norm_fwd(s, xs, nrm, 1e-12)
-            ops.l2norm_fwd(t, xt, nrm, 1e-12)
-        else:
-            xs.copy_(s); xt.copy_(t)
-        Ss, St = torch.empty(m, m, dtype=f32, device=s.device), torch.empty(m, m, dtype=f32, device=s.device)
-        ops.gemm(xs, xs, Ss)
-        ops.gemm(xt, xt, St)
-        ops.gram_diff(Ss, St, None, ops.GRAM_MODES[(self.remove_neg, self.remove_only_teacher_neg)], inv, acc, block=block)
+        pd = -D % 8                                           # kernels work in 8-column granules; zero columns add nothing
+        npad = pad8(n)
+        e = lambda *shape, dt=f32: torch.empty(*shape, dtype=dt, device=s.device)
+        xs, xt, nrm = e(npad, D + pd, dt=torch.bfloat16), e(npad, D + pd, dt=torch.bfloat16), e(npad)
+        for f, x in ((s, xs), (t, xt)):
+            operands(torch.nn.functional.pad(f.to(f32), (0, pd, 0, npad - n)).contiguous(), x, nrm, n, self.apply_norm)
+        similarity_diff(xs, xt, e(npad, npad), e(npad, npad), None,
+                        ops.GRAM_MODES[(self.remove_neg, self.remove_only_teacher_neg)], inv, acc, block=block)
 
     def __call__(self, output_feats: torch.Tensor, target_feats: torch.Tensor, img_level: bool = True) -> torch.Tensor:
         acc = torch.zeros(1, dtype=f32, device=output_feats.device)

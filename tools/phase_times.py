@@ -20,7 +20,7 @@ marks = []
 def mark(name):
     e = torch.cuda.Event(enable_timing=True); e.record(); marks.append((name, e))
 import dinov3_jax.engine.core as core      # the forward pieces are module functions the engine calls by name
-owner = {"backbone_fwd": core, "head_fwd": core, "_sinkhorn_pair": eng, "_head_bwd": eng, "_block_bwd": eng, "optimizer_step": eng}
+owner = {"backbone_fwd": core, "head_fwd": core, "sinkhorn": core, "_head_bwd": eng, "_block_bwd": eng, "optimizer_step": eng}
 orig = {k: getattr(o, k) for k, o in owner.items()}
 def wrap(name, label_fn):
     f = orig[name]
@@ -29,7 +29,7 @@ def wrap(name, label_fn):
     setattr(owner[name], name, g)
 wrap("backbone_fwd", lambda net, *a: f"backbone fwd {'teacher' if net.teacher else 'student'}")
 wrap("head_fwd", lambda net, *a, **k: f"heads fwd {'teacher' if net.teacher else 'student'}")
-wrap("_sinkhorn_pair", lambda *a, **k: "sinkhorn")
+wrap("sinkhorn", lambda *a, **k: "sinkhorn")
 wrap("_head_bwd", lambda *a, **k: "heads bwd (+CE, before)")
 wrap("_block_bwd", lambda i, *a: "blocks bwd")
 wrap("optimizer_step", lambda *a, **k: "optimizer (sumsq+adamw+ema)")
