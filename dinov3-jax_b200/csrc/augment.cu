@@ -11,6 +11,7 @@
 // reproduced).
 #include "ptx.cuh"
 #include "d3_internal.h"
+#include "resample.cuh"
 
 #include <type_traits>
 
@@ -27,13 +28,6 @@ struct AugCrop {
   int solarize;            // RandomSolarize applied (threshold 128/255)
 };
 struct AugBlur { float sigma; };   // <= 0: no blur
-
-__device__ __forceinline__ float cubic_aa(float x) {           // Keys cubic, a = -0.5 (PIL / torch antialias bicubic)
-  x = fabsf(x);
-  if (x < 1.f) return ((1.5f * x - 2.5f) * x) * x + 1.f;
-  if (x < 2.f) return ((-0.5f * x + 2.5f) * x - 4.f) * x + 2.f;
-  return 0.f;
-}
 
 // out[n, S, S, 3] (fp32, [0,1]) = antialiased bicubic resize of src[img, y0:y0+h, x0:x0+w] (+ horizontal flip).
 // Same definition as torch's _upsample_bicubic2d_aa (align_corners = False): per axis, scale = in/out,
@@ -54,19 +48,17 @@ __global__ void aug_resized_crop_kernel(const T* __restrict__ src, int H, int W,
   const float isx = 1.f / fmaxf(scx, 1.f), isy = 1.f / fmaxf(scy, 1.f);
   const float supx = 2.f * fmaxf(scx, 1.f), supy = 2.f * fmaxf(scy, 1.f);
   const float cx = scx * (sx_out + 0.5f), cy = scy * (oy + 0.5f);
-  const int xmin = max((int)(cx - supx + 0.5f), 0), xmax = min((int)(cx + supx + 0.5f), c.w);
-  const int ymin = max((int)(cy - supy + 0.5f), 0), ymax = min((int)(cy + supy + 0.5f), c.h);
-  float wxs = 0.f, wys = 0.f;
-  for (int x = xmin; x < xmax; ++x) wxs += cubic_aa((x - cx + 0.5f) * isx);
-  for (int y = ymin; y < ymax; ++y) wys += cubic_aa((y - cy + 0.5f) * isy);
+  int xmin, xmax, ymin, ymax;
+  const float wxs = aa_window(cx, supx, isx, c.w, c.w, xmin, xmax);
+  const float wys = aa_window(cy, supy, isy, c.h, c.h, ymin, ymax);
   const T* base = src + ((size_t)c.img * H + c.y0) * W * 3 + (size_t)c.x0 * 3;
   float r = 0.f, g = 0.f, b = 0.f;
   for (int y = ymin; y < ymax; ++y) {
-    const float wy = cubic_aa((y - cy + 0.5f) * isy);
+    const float wy = cubic_aa<float>((y - cy + 0.5f) * isy);
     const T* row = base + (size_t)y * W * 3;
     float rr = 0.f, gg = 0.f, bb = 0.f;
     for (int x = xmin; x < xmax; ++x) {
-      const float wx = cubic_aa((x - cx + 0.5f) * isx);
+      const float wx = cubic_aa<float>((x - cx + 0.5f) * isx);
       rr += wx * row[3 * x]; gg += wx * row[3 * x + 1]; bb += wx * row[3 * x + 2];
     }
     r += wy * rr; g += wy * gg; b += wy * bb;

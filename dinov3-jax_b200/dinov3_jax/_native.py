@@ -88,6 +88,10 @@ SIGNATURES = {
     "d3_aug_color_images": [P, I, I, I, P, P, P, P],
     "d3_aug_solarize": [P, P, I, I, P],
     "d3_aug_local_windows": [P, I, I, P, P, I, I, P, P, P, P, P],
+    "d3_eval_resize_crop": [P, P, I, I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, I, P],
+    "d3_knn_normalize": [P, I, I, I, P, P, I, P],
+    "d3_topk_merge": [P, LL, I, I, I, P, P, I, I, I, P],
+    "d3_knn_vote": [P, P, I, I, P, I, C.POINTER(C.c_int), I, F, I, P, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

@@ -49,6 +49,12 @@ DEFAULTS = {
               "layerwise_decay": 0.9, "multi_tensor_optim": True, "adamw_beta1": 0.9, "adamw_beta2": 0.999},
     "checkpointing": {"period": 3750, "max_to_keep": 3},
     "distillation": {"enabled": False, "full_cfg_path": "", "checkpoint_path": ""},   # ssl_default_config.yaml:130-133
+    # k-NN evaluation of the teacher backbone (train.do_test); empty dataset paths: nothing is evaluated.
+    # `config_files` (the reference's list of evaluation configs) is accepted and not read.
+    "evaluation": {"eval_period_iterations": 12500, "config_files": [],
+                   "knn": {"train_dataset_path": "", "val_dataset_path": "", "nb_knn": [10, 20, 100, 200],
+                           "temperature": 0.07, "batch_size": 256, "resize_size": 256, "crop_size": 224,
+                           "num_workers": 8}},
 }
 
 

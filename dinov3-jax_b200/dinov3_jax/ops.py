@@ -6,6 +6,7 @@ current CUDA stream, and raises NativeError on a non-zero status.  No function h
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import torch
 
@@ -454,3 +455,72 @@ def adamw_ema(p, g, m, v, teacher, p_bf16, t_bf16, n_bf16, segs, nseg, sumsq_t, 
     N.check(N.init().d3_adamw_ema(_p(p), _p(g), _p(m), _p(v), _p(teacher), _p(p_bf16), _p(t_bf16), n_bf16, _p(segs),
                                   nseg, n, _p(sumsq_t), max_norm, lr, last_layer_lr, wd, b1, b2, eps, step, momentum,
                                   _s()), "d3_adamw_ema")
+
+
+# ------------------------------------------------------------------------------------------------------ k-NN evaluation
+def eval_max_taps(sizes, resize: int) -> int:
+    """The filter taps of the widest window d3_eval_resize_crop meets over images of (H, W) `sizes`: torch's
+    2 * ceil(support) + 1 with support = 2 * max(input / resized, 1), over both axes of every image."""
+    taps = 5
+    for H, W in sizes:
+        short, long = min(H, W), max(H, W)
+        new_long = int(resize * long / short)
+        for i, o in ((short, resize), (long, new_long)):
+            s = i / o
+            taps = max(taps, 2 * int(math.ceil(2.0 * s if s >= 1.0 else 2.0)) + 1)
+    return taps
+
+
+def eval_resize_crop(src: torch.Tensor, desc: torch.Tensor, out: torch.Tensor, *, resize: int, max_taps: int,
+                     mean=None, std=None) -> torch.Tensor:
+    """Resize(resize, bicubic, antialias) + CenterCrop of n packed uint8 HWC images (d3_eval_resize_crop).
+
+    src uint8 (flat), desc int64 [n, 3] = (byte offset, H, W) on the device, out [n, crop, crop, 3]: bf16 normalised
+    with mean / std (3 floats each), or uint8 (the crop itself, mean / std not used)."""
+    n, S = out.shape[0], out.shape[1]
+    assert src.dtype == torch.uint8 and src.is_contiguous() and desc.dtype == torch.int64 and desc.is_contiguous()
+    assert desc.shape == (n, 3) and out.shape == (n, S, S, 3) and out.is_contiguous() and out.dtype in (bf16, torch.uint8)
+    u8 = out.dtype == torch.uint8
+    m = (C.c_float * 3)(*([0.0] * 3 if u8 else [float(v) for v in mean]))
+    s = (C.c_float * 3)(*([1.0] * 3 if u8 else [float(v) for v in std]))
+    N.check(N.init().d3_eval_resize_crop(_p(src), _p(desc), n, int(resize), S, int(max_taps), m, s, _p(out), int(u8),
+                                         _s()), "d3_eval_resize_crop")
+    return out
+
+
+def knn_normalize(x: torch.Tensor, y_f32: torch.Tensor | None = None, y_bf16: torch.Tensor | None = None):
+    """Rows of x (fp32 [R, D], unit inner stride) / max(||row||, 1e-12) into y_f32 and / or y_bf16 ([>= R, ld >= D],
+    the same row stride when both are given) (d3_knn_normalize)."""
+    R, D = x.shape
+    assert x.dtype == f32 and (y_f32 is not None or y_bf16 is not None)
+    assert y_f32 is None or (y_f32.dtype == f32 and y_f32.shape[0] >= R and y_f32.shape[1] >= D)
+    assert y_bf16 is None or (y_bf16.dtype == bf16 and y_bf16.shape[0] >= R and y_bf16.shape[1] >= D)
+    lds = {_ld(t) for t in (y_f32, y_bf16) if t is not None}
+    assert len(lds) == 1, "y_f32 and y_bf16 need the same row stride"
+    N.check(N.init().d3_knn_normalize(_p(x), _ld(x), R, D, _p(y_f32), _p(y_bf16), lds.pop(), _s()), "d3_knn_normalize")
+
+
+def topk_merge(sims: torch.Tensor, top_sim: torch.Tensor, top_idx: torch.Tensor, *, offset: int, valid: int | None = None,
+               fresh: bool = False):
+    """Merge the similarity chunk sims (fp32 [Q, >= valid], bank indices offset + column) into the running sorted top-k
+    top_sim fp32 / top_idx int32 [Q, k] (d3_topk_merge).  fresh: the running lists start empty."""
+    Q = sims.shape[0]
+    valid = sims.shape[1] if valid is None else int(valid)
+    assert sims.dtype == f32 and top_sim.dtype == f32 and top_idx.dtype == torch.int32
+    assert top_sim.shape == top_idx.shape and top_sim.shape[0] == Q and _ld(top_sim) == _ld(top_idx)
+    N.check(N.init().d3_topk_merge(_p(sims), _ld(sims), Q, valid, int(offset), _p(top_sim), _p(top_idx), _ld(top_sim),
+                                   top_sim.shape[1], int(bool(fresh)), _s()), "d3_topk_merge")
+
+
+def knn_vote(top_sim: torch.Tensor, top_idx: torch.Tensor, labels: torch.Tensor, nb_knn, temperature: float,
+             num_classes: int, preds: torch.Tensor) -> torch.Tensor:
+    """preds int32 [Q, len(nb_knn), 5]: the 5 best classes of the softmax(sims[:k] / T)-weighted vote of each query's k
+    first neighbours, for every k of nb_knn (d3_knn_vote)."""
+    Q = top_sim.shape[0]
+    nk = len(nb_knn)
+    assert top_sim.dtype == f32 and top_idx.dtype == torch.int32 and labels.dtype == torch.int32 and labels.is_contiguous()
+    assert preds.dtype == torch.int32 and preds.shape == (Q, nk, 5) and preds.is_contiguous()
+    ks = (C.c_int * nk)(*[int(k) for k in nb_knn])
+    N.check(N.init().d3_knn_vote(_p(top_sim), _p(top_idx), _ld(top_sim), Q, _p(labels), labels.numel(), ks, nk,
+                                 float(temperature), int(num_classes), _p(preds), _s()), "d3_knn_vote")
+    return preds

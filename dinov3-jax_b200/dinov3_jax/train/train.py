@@ -224,6 +224,75 @@ def build_data_loader_from_cfg(config, model, start_iter: int = 0):
                             collate_fn=collate_fn)
 
 
+def _knn_cfg(config) -> dict:
+    """The `evaluation.knn` block, or {} when it names no train / val dataset (then nothing is evaluated)."""
+    ev = config.get("evaluation", None) or {}
+    knn = dict(ev.get("knn", None) or {})
+    return knn if knn.get("train_dataset_path") and knn.get("val_dataset_path") else {}
+
+
+def eval_backbone(config, weights):
+    """The frozen backbone k-NN evaluates, with the architecture of the run's `student.*` config (the depth is the
+    number of blocks in the weights).  `weights`: a DinoVisionTransformer (returned as is); a `save_checkpoint`
+    directory (its `teacher_backbone`); a torch-hub `.pth` state dict; or a live Engine / SSLMetaArch (its EMA teacher,
+    through `engine_state`, which is collective under FSDP: every rank calls this)."""
+    from ..checkpointer import convert_torch_hub_state_dict, engine_state, flat_from_tree, load_checkpoint
+    from ..engine.config import config_from_reference_cfg
+    from ..models import DinoVisionTransformer
+    if isinstance(weights, DinoVisionTransformer):
+        return weights
+    engine = getattr(weights, "engine", None) if isinstance(weights, SSLMetaArch) else weights
+    if hasattr(engine, "params") and hasattr(engine, "train_step"):
+        tree = engine_state(engine)[0]["teacher_backbone"]
+        device = engine.device
+    else:
+        path = str(weights)
+        if os.path.isdir(path):
+            tree = load_checkpoint(path)["model_params"]["teacher_backbone"]
+        elif path.endswith(".pth"):
+            tree = convert_torch_hub_state_dict(torch.load(path, map_location="cpu", weights_only=True))[0]
+        else:
+            raise FileNotFoundError(f"{path}: not a checkpoint directory or a .pth state dict")
+        device = f"cuda:{int(os.environ.get('LOCAL_RANK', '0'))}"
+    ec, st = config_from_reference_cfg(config), config.student
+    depth = sum(1 for k in tree if str(k).startswith("blocks_"))
+    ffn = st.ffn_layer
+    return DinoVisionTransformer(tree, patch_size=ec.patch, pos_embed_rope_base=ec.rope_base, embed_dim=ec.embed_dim,
+                                 n_blocks=depth, num_heads=ec.heads, ffn_ratio=ec.ffn_ratio, norm_layer=st.norm_layer,
+                                 ffn_layer=ffn, n_storage_tokens=ec.n_storage, mask_k_bias=ec.mask_k_bias,
+                                 device=device)
+
+
+def do_test(config, model, header):
+    """k-NN evaluation of the teacher backbone of `model` (see `eval_backbone`) on the `evaluation.knn` datasets; rank 0
+    writes <output_dir>/eval/<header>/results_knn.json and returns {k: {"top1", "top5"}} ({} on other ranks).  Without
+    configured datasets it logs one line and returns {}."""
+    import json
+    from .. import distributed
+    knn = _knn_cfg(config)
+    if not knn:
+        if distributed.is_main_process():
+            print(f"do_test({header}): no evaluation.knn train / val dataset configured, nothing evaluated", flush=True)
+        return {}
+    backbone = eval_backbone(config, model)            # collective for a live engine under FSDP
+    if not distributed.is_main_process():
+        return {}
+    from ..eval import eval_knn, make_eval_dataset
+    c = config.crops
+    results = eval_knn(backbone, make_eval_dataset(knn["train_dataset_path"]), make_eval_dataset(knn["val_dataset_path"]),
+                       nb_knn=knn.get("nb_knn", (10, 20, 100, 200)), temperature=float(knn.get("temperature", 0.07)),
+                       batch_size=int(knn.get("batch_size", 256)), resize_size=int(knn.get("resize_size", 256)),
+                       crop_size=int(knn.get("crop_size", 224)), num_workers=int(knn.get("num_workers", 8)),
+                       rgb_mean=c.get("rgb_mean", (0.485, 0.456, 0.406)), rgb_std=c.get("rgb_std", (0.229, 0.224, 0.225)))
+    out_dir = os.path.join(getattr(config.train, "output_dir", None) or ".", "eval", header)
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "results_knn.json"), "w") as f:
+        json.dump({str(k): v for k, v in results.items()}, f, indent=1)
+    print(f"do_test({header}): " + ", ".join(f"{k}-NN top-1 {v['top1']:.2f} top-5 {v['top5']:.2f}"
+                                             for k, v in results.items()), flush=True)
+    return results
+
+
 def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None, max_iters: int = 0,
              print_freq: int = 10):
     """train/train.py:319-713.  `data_loader` (optional) yields the reference's collate dicts; by default it is built
@@ -265,6 +334,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
         for _ in range(start_iter):
             next(it_loader)
     meters, nan_streak, t0 = {}, 0, time.time()
+    ev = config.get("evaluation", None) or {}
+    eval_period = int(ev.get("eval_period_iterations", 0) or 0) if _knn_cfg(config) else 0
     for it in range(start_iter, n_iters):
         try:
             data = next(it_loader)
@@ -280,6 +351,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
                 keep_last_n_checkpoints(ckpt_dir, ck_cfg.max_to_keep)
                 if "keep_every" in ck_cfg and (it + 1) % int(ck_cfg.keep_every) == 0:
                     keep_checkpoint_copy(os.path.join(ckpt_dir, str(it)))
+        if eval_period > 0 and (it + 1) % eval_period == 0:          # train/train.py:689-692
+            do_test(config, engine, f"training_{it}")
         if it % print_freq == 0 or it == n_iters - 1:
             m = engine.read_metrics()                  # the only device->host sync of the loop
             if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
@@ -307,6 +380,22 @@ def main(argv=None):
     import random
     import numpy as np
     random.seed(args.seed); np.random.seed(args.seed); torch.manual_seed(args.seed)   # setup_job(seed=args.seed), :281
+    if args.eval not in ("", "knn"):
+        raise NotImplementedError(f"--eval {args.eval!r}: the k-NN evaluation (--eval knn, or empty) is the only one")
+    if args.eval_only:                                 # train/train.py:304-311
+        import json
+        from ..checkpointer import find_latest_checkpoint
+        weights = args.eval_pretrained_weights
+        if not weights:
+            weights = find_latest_checkpoint(os.path.join(config.train.output_dir, "ckpt"))
+        if not weights:
+            raise FileNotFoundError("--eval-only needs --eval-pretrained-weights (a checkpoint directory or a torch-hub "
+                                    f".pth) or a checkpoint under {os.path.join(config.train.output_dir, 'ckpt')}")
+        it = 0
+        if os.path.isdir(str(weights)):
+            stored = json.loads(open(os.path.join(str(weights), "manifest.json")).read())["iteration"]
+            it = int(stored) + 1 if str(stored).lstrip("-").isdigit() else 0
+        return do_test(config, str(weights), f"manual_{it}")
     model = SSLMetaArch(config)
     return do_train(config, model, resume=not args.no_resume, max_iters=args.max_iters, print_freq=args.print_freq)
 

@@ -336,6 +336,29 @@ int d3_aug_local_windows(const float* base /*[n_base,M,M,3]*/, int n_base, int M
                          int n_crops, int L, float* win, float* tmp, float* y /*[n_crops,L,L,3]*/,
                          float* gray_sum /*[n_crops] zeroed*/, void* stream);
 
+/* ---- k-NN evaluation (the DINO / DINOv2 / DINOv3 k-NN protocol on the teacher's normalised class token) ---------
+ * The similarities of a query tile with a bank chunk are d3_gemm_bf16 (fp32 out) of L2-normalised bf16 rows; these
+ * entry points are the rest of the search and the vote.  Every one is deterministic (the same bits on every run).
+ * d3_eval_resize_crop: n uint8 HWC images of any sizes packed in one buffer, desc[3i .. 3i+2] = (byte offset, H, W)
+ *   (device, int64).  torchvision Resize(resize, BICUBIC, antialias=True) on the short side (long side
+ *   int(resize * long / short)) with torch's uint8 arithmetic, then CenterCrop(crop); only the crop is computed.  out:
+ *   bf16 NHWC [n, crop, crop, 3] = (u8 / 255 - mean) / std, or (out_u8) the uint8 crop.  max_taps >= 2 ceil(2 max(s, 1))
+ *   + 1 over both axes of every image, s = input / resized length (the filter taps of the widest window).
+ * d3_knn_normalize: y = x / max(||x||, 1e-12) per row (F.normalize), into y_f32 and / or y_bf16 (both NULL: error).
+ * d3_topk_merge: per query row q, the running top-k (top_sim fp32 / top_idx int32 [Q, ldk], sorted by similarity desc,
+ *   index asc; fresh = 1: start from an empty list) merged with sims[q, 0:valid] (bank indices offset + column) into
+ *   the new sorted top-k.  1 <= k <= 1024; chunks must come in increasing offset; empty slots are (-inf, -1).
+ * d3_knn_vote: per query and per k in nb_knn (host, <= 16 entries, each <= ldk): weights softmax(sims[:k] / T) (fp32,
+ *   max subtracted), class scores (labels[top_idx]) summed in neighbour order, the 5 best classes (score desc, class
+ *   asc) into preds int32 [Q, n_k, 5].  num_classes <= 32768.                                                        */
+int d3_eval_resize_crop(const void* src_u8, const long long* desc, int n, int resize, int crop, int max_taps,
+                        const float* mean3 /*host*/, const float* std3 /*host*/, void* out, int out_u8, void* stream);
+int d3_knn_normalize(const float* x, int ldx, int R, int D, float* y_f32, void* y_bf16, int ldy, void* stream);
+int d3_topk_merge(const float* sims, long long lds, int Q, int valid, int offset, float* top_sim, int* top_idx, int ldk,
+                  int k, int fresh, void* stream);
+int d3_knn_vote(const float* top_sim, const int* top_idx, int ldk, int Q, const int* bank_labels, int n_bank,
+                const int* nb_knn /*host*/, int n_k, float temperature, int num_classes, int* preds, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
