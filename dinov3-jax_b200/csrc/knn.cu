@@ -1,5 +1,5 @@
 // k-NN evaluation of a frozen backbone (the DINO / DINOv2 / DINOv3 k-NN protocol): the eval transform of a batch of
-// decoded images of any size, the L2 normalisation of the features, the running top-k merge over chunks of
+// decoded images of any size (and, with the same kernel, the linear probe's RandomResizedCrop + flip train crop), the L2 normalisation of the features, the running top-k merge over chunks of
 // similarities, and the softmax-weighted class vote.  The similarities themselves are d3_gemm_bf16 with an fp32
 // output (queries . bank_chunk^T); nothing here multiplies matrices.
 //
@@ -11,6 +11,7 @@
 #include "resample.cuh"
 
 #include <math.h>
+#include <stdio.h>
 
 namespace d3 {
 
@@ -84,10 +85,21 @@ __device__ void eval_axis_table(const EvalAxis& a, int in, int crop, int prec, i
   }
 }
 
+// One resampled axis of the window a crop reads: source positions [src0, src0 + axis.in) of the image feed output
+// positions [0, crop) of the resized axis from `first` on (mirrored when flip).
+struct CropAxis {
+  EvalAxis a;
+  int in, src0, flip;
+};
+
+// The eval transform (boxes == nullptr: Resize(resize) of the whole image + CenterCrop(crop)) and the train crop
+// (boxes[5n .. 5n+4] = (top, left, height, width, flip): crop the box, resize it to crop x crop, mirror when flip).
+// Both take their int16 weights from eval_axis_wmax / eval_precision / eval_axis_table, so the two share torch's uint8
+// arithmetic bit for bit.
 template <bool U8>
 __global__ void __launch_bounds__(EV_THREADS) eval_resize_crop_kernel(
-    const uint8_t* __restrict__ src, const long long* __restrict__ desc, int resize, int crop, int max_taps,
-    float m0, float m1, float m2, float s0, float s1, float s2, void* __restrict__ out) {
+    const uint8_t* __restrict__ src, const long long* __restrict__ desc, const int* __restrict__ boxes, int resize,
+    int crop, int max_taps, float m0, float m1, float m2, float s0, float s1, float s2, void* __restrict__ out) {
   extern __shared__ __align__(16) unsigned char ev_smem[];
   __shared__ double red[EV_THREADS / 32];
   int* lo_x = reinterpret_cast<int*>(ev_smem);
@@ -97,33 +109,43 @@ __global__ void __launch_bounds__(EV_THREADS) eval_resize_crop_kernel(
   const int n = blockIdx.y;
   const long long off = desc[3 * n];
   const int H = (int)desc[3 * n + 1], W = (int)desc[3 * n + 2];
-  // torchvision _compute_resized_output_size and center_crop (offsets rounded half to even, like Python's round)
-  const int shorter = min(H, W), longer = max(H, W);
-  const int new_long = (int)((double)((long long)resize * longer) / (double)shorter);
-  const int oh = W <= H ? new_long : resize, ow = W <= H ? resize : new_long;
-  const EvalAxis ax = eval_axis(W, ow, (int)rint((ow - crop) / 2.0));
-  const EvalAxis ay = eval_axis(H, oh, (int)rint((oh - crop) / 2.0));
-  const int px = eval_precision(eval_axis_wmax(ax, W, red));
-  const int py = eval_precision(eval_axis_wmax(ay, H, red));
-  eval_axis_table(ax, W, crop, px, max_taps, lo_x, w_x);
-  eval_axis_table(ay, H, crop, py, max_taps, lo_y, w_y);
+  CropAxis cx, cy;
+  if (boxes) {
+    const int* bx = boxes + 5 * n;
+    cy = {eval_axis(bx[2], crop, 0), bx[2], bx[0], 0};
+    cx = {eval_axis(bx[3], crop, 0), bx[3], bx[1], bx[4]};
+  } else {
+    // torchvision _compute_resized_output_size and center_crop (offsets rounded half to even, like Python's round)
+    const int shorter = min(H, W), longer = max(H, W);
+    const int new_long = (int)((double)((long long)resize * longer) / (double)shorter);
+    const int oh = W <= H ? new_long : resize, ow = W <= H ? resize : new_long;
+    cx = {eval_axis(W, ow, (int)rint((ow - crop) / 2.0)), W, 0, 0};
+    cy = {eval_axis(H, oh, (int)rint((oh - crop) / 2.0)), H, 0, 0};
+  }
+  const EvalAxis& ax = cx.a;
+  const EvalAxis& ay = cy.a;
+  const int px = eval_precision(eval_axis_wmax(ax, cx.in, red));
+  const int py = eval_precision(eval_axis_wmax(ay, cy.in, red));
+  eval_axis_table(ax, cx.in, crop, px, max_taps, lo_x, w_x);
+  eval_axis_table(ay, cy.in, crop, py, max_taps, lo_y, w_y);
   __syncthreads();
   const int tx = min(ax.taps, max_taps), ty = min(ay.taps, max_taps);
-  const uint8_t* img = src + off;
+  const uint8_t* img = src + off + ((size_t)cy.src0 * W + cx.src0) * 3;
   const int row0 = blockIdx.x * EV_ROWS, rows = min(EV_ROWS, crop - row0);
   const int hx = px > 0 ? 1 << (px - 1) : 0, hy = py > 0 ? 1 << (py - 1) : 0;
   for (int p = threadIdx.x; p < rows * crop; p += blockDim.x) {
     const int oy = row0 + p / crop, ox = p % crop;
+    const int sx = cx.flip ? crop - 1 - ox : ox;
     const short* wy = w_y + (size_t)oy * max_taps;
-    const short* wx = w_x + (size_t)ox * max_taps;
-    const int y0 = lo_y[oy], x0 = lo_x[ox];
+    const short* wx = w_x + (size_t)sx * max_taps;
+    const int y0 = lo_y[oy], x0 = lo_x[sx];
     int ar = hy, ag = hy, ab = hy;
     for (int j = 0; j < ty; ++j) {
       const int wv = wy[j];
-      if (wv == 0 || y0 + j >= H) continue;
+      if (wv == 0 || y0 + j >= cy.in) continue;
       const uint8_t* row = img + ((size_t)(y0 + j) * W + x0) * 3;
       int hr = hx, hg = hx, hb = hx;
-      for (int i = 0; i < tx && x0 + i < W; ++i) {
+      for (int i = 0; i < tx && x0 + i < cx.in; ++i) {
         const int w = wx[i];
         hr += w * row[3 * i]; hg += w * row[3 * i + 1]; hb += w * row[3 * i + 2];
       }
@@ -440,31 +462,53 @@ using namespace d3;
 
 extern "C" {
 
-int d3_eval_resize_crop(const void* src_u8, const long long* desc, int n, int resize, int crop, int max_taps,
-                        const float* mean3, const float* std3, void* out, int out_u8, void* stream) {
-  if (n <= 0) return D3_OK;
-  if (crop < 1 || resize < crop || max_taps < 1 || !src_u8 || !desc || !out)
-    return set_error(D3_ERR_ARG, "d3_eval_resize_crop: need 1 <= crop <= resize, max_taps >= 1");
+static int crop_error(int code, const char* who, const char* what) {
+  char msg[160];
+  snprintf(msg, sizeof(msg), "%s: %s", who, what);
+  return set_error(code, msg);
+}
+
+static int launch_resize_crop(const char* who, const void* src_u8, const long long* desc, const int* boxes, int n,
+                              int resize, int crop, int max_taps, const float* mean3, const float* std3, void* out,
+                              int out_u8, void* stream) {
   const size_t smem = (size_t)2 * crop * sizeof(int) + (size_t)2 * crop * max_taps * sizeof(short);
   constexpr int SMEM_MAX = 200 * 1024;
-  if (smem > SMEM_MAX) return set_error(D3_ERR_ARG, "d3_eval_resize_crop: crop * max_taps too large (downscale > ~100x)");
-  if (!out_u8 && (!mean3 || !std3)) return set_error(D3_ERR_ARG, "d3_eval_resize_crop: mean / std needed for bf16 output");
+  if (smem > SMEM_MAX) return crop_error(D3_ERR_ARG, who, "crop * max_taps too large (downscale > ~100x)");
+  if (!out_u8 && (!mean3 || !std3)) return crop_error(D3_ERR_ARG, who, "mean / std needed for bf16 output");
   static const cudaError_t c0 =
       cudaFuncSetAttribute(eval_resize_crop_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
   static const cudaError_t c1 =
       cudaFuncSetAttribute(eval_resize_crop_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
-  if (c0 != cudaSuccess || c1 != cudaSuccess) return set_error(D3_ERR_CUDA, "d3_eval_resize_crop: smem attribute");
+  if (c0 != cudaSuccess || c1 != cudaSuccess) return crop_error(D3_ERR_CUDA, who, "smem attribute");
   const dim3 grid((crop + EV_ROWS - 1) / EV_ROWS, n);
   const float m[3] = {out_u8 ? 0.f : mean3[0], out_u8 ? 0.f : mean3[1], out_u8 ? 0.f : mean3[2]};
   const float s[3] = {out_u8 ? 1.f : std3[0], out_u8 ? 1.f : std3[1], out_u8 ? 1.f : std3[2]};
   if (out_u8)
     eval_resize_crop_kernel<true><<<grid, EV_THREADS, smem, STREAM(stream)>>>(
-        (const uint8_t*)src_u8, desc, resize, crop, max_taps, m[0], m[1], m[2], s[0], s[1], s[2], out);
+        (const uint8_t*)src_u8, desc, boxes, resize, crop, max_taps, m[0], m[1], m[2], s[0], s[1], s[2], out);
   else
     eval_resize_crop_kernel<false><<<grid, EV_THREADS, smem, STREAM(stream)>>>(
-        (const uint8_t*)src_u8, desc, resize, crop, max_taps, m[0], m[1], m[2], s[0], s[1], s[2], out);
+        (const uint8_t*)src_u8, desc, boxes, resize, crop, max_taps, m[0], m[1], m[2], s[0], s[1], s[2], out);
   D3_CHECK_LAUNCH();
   return D3_OK;
+}
+
+int d3_eval_resize_crop(const void* src_u8, const long long* desc, int n, int resize, int crop, int max_taps,
+                        const float* mean3, const float* std3, void* out, int out_u8, void* stream) {
+  if (n <= 0) return D3_OK;
+  if (crop < 1 || resize < crop || max_taps < 1 || !src_u8 || !desc || !out)
+    return set_error(D3_ERR_ARG, "d3_eval_resize_crop: need 1 <= crop <= resize, max_taps >= 1");
+  return launch_resize_crop("d3_eval_resize_crop", src_u8, desc, nullptr, n, resize, crop, max_taps, mean3, std3, out,
+                            out_u8, stream);
+}
+
+int d3_train_resized_crop(const void* src_u8, const long long* desc, const int* boxes, int n, int crop, int max_taps,
+                          const float* mean3, const float* std3, void* out, int out_u8, void* stream) {
+  if (n <= 0) return D3_OK;
+  if (crop < 1 || max_taps < 1 || !src_u8 || !desc || !boxes || !out)
+    return set_error(D3_ERR_ARG, "d3_train_resized_crop: need crop >= 1, max_taps >= 1 and non-null buffers");
+  return launch_resize_crop("d3_train_resized_crop", src_u8, desc, boxes, n, 0, crop, max_taps, mean3, std3, out,
+                            out_u8, stream);
 }
 
 int d3_knn_normalize(const float* x, int ldx, int R, int D, float* y_f32, void* y_bf16, int ldy, void* stream) {

@@ -1,6 +1,7 @@
 // Optimiser kernels on flat fp32 parameter shards: squared-norm reduction (for the per-submodule clip,
 // dinov3_jax/train/train.py:516-541) and a fused clip + AdamW (optax.adamw semantics, train/train.py:95-106,562-563)
-// + teacher EMA (train/ssl_meta_arch.py:650-652) + bf16 re-cast of the compute copies.
+// + teacher EMA (train/ssl_meta_arch.py:650-652) + bf16 re-cast of the compute copies; and the SGD-momentum update of
+// the linear-probe classifiers.
 #include <cmath>
 #include "ptx.cuh"
 #include "d3_internal.h"
@@ -100,6 +101,30 @@ __global__ void ema_kernel(float* __restrict__ teacher, const float* __restrict_
   if (i4 < n_bf16) *reinterpret_cast<uint2*>(t_bf16 + i4) = make_uint2(pack_bf16(t.x, t.y), pack_bf16(t.z, t.w));
 }
 
+// torch.optim.SGD(momentum, dampening = 0, nesterov = False, weight_decay = 0) on a [rows, cols] fp32 matrix whose
+// rows come in groups of Cp per classifier: buf = first ? g : momentum * buf + g (torch's mul_ then add_, two
+// roundings), p = p - lr * buf with lr = lr_base[(i / cols) / Cp] * lr_scale; the bf16 copy the next forward GEMM reads
+// is written alongside.  Four elements per thread (n % 4 == 0).
+__global__ void sgd_momentum_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                    __nv_bfloat16* __restrict__ p_bf16, long n, int cols, const float* __restrict__ lr,
+                                    int Cp, float lr_scale, float momentum, int first) {
+  const long i4 = (blockIdx.x * (long)blockDim.x + threadIdx.x) * 4;
+  if (i4 >= n) return;
+  float pv[4], gv[4], mv[4];
+  *reinterpret_cast<float4*>(pv) = *reinterpret_cast<const float4*>(p + i4);
+  *reinterpret_cast<float4*>(gv) = *reinterpret_cast<const float4*>(g + i4);
+  if (!first) *reinterpret_cast<float4*>(mv) = *reinterpret_cast<const float4*>(m + i4);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float l = lr[(i4 + j) / cols / Cp] * lr_scale;
+    mv[j] = first ? gv[j] : __fadd_rn(__fmul_rn(mv[j], momentum), gv[j]);
+    pv[j] = fmaf(-l, mv[j], pv[j]);
+  }
+  *reinterpret_cast<float4*>(p + i4) = *reinterpret_cast<float4*>(pv);
+  *reinterpret_cast<float4*>(m + i4) = *reinterpret_cast<float4*>(mv);
+  if (p_bf16) *reinterpret_cast<uint2*>(p_bf16 + i4) = make_uint2(pack_bf16(pv[0], pv[1]), pack_bf16(pv[2], pv[3]));
+}
+
 }  // namespace d3
 
 using namespace d3;
@@ -142,6 +167,19 @@ int d3_ema(float* teacher, const float* student, void* t_bf16, long long n_bf16,
   if (n % 4 || n_bf16 % 4) return set_error(D3_ERR_ARG, "d3_ema: n, n_bf16 must be multiples of 4");
   ema_kernel<<<(int)((n / 4 + 255) / 256), 256, 0, STREAM(stream)>>>(teacher, student, (__nv_bfloat16*)t_bf16, n_bf16, n,
                                                                   momentum);
+  D3_CHECK_LAUNCH();
+  return D3_OK;
+}
+
+int d3_sgd_momentum(float* p, const float* g, float* m, void* p_bf16, long long rows, int cols, const float* lr, int Cp,
+                    float lr_scale, float momentum, int first, void* stream) {
+  if (rows <= 0) return D3_OK;
+  const long long n = rows * cols;
+  if (!p || !g || !m || !lr || cols < 1 || Cp < 1 || n % 4 || ((uintptr_t)p | (uintptr_t)g | (uintptr_t)m) % 16 ||
+      (uintptr_t)p_bf16 % 8)
+    return set_error(D3_ERR_ARG, "d3_sgd_momentum: need rows * cols % 4 == 0, p, g, m 16-byte and p_bf16 8-byte aligned");
+  sgd_momentum_kernel<<<(int)((n / 4 + 255) / 256), 256, 0, STREAM(stream)>>>(
+      p, g, m, (__nv_bfloat16*)p_bf16, n, cols, lr, Cp, lr_scale, momentum, first ? 1 : 0);
   D3_CHECK_LAUNCH();
   return D3_OK;
 }

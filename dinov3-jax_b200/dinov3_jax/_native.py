@@ -92,9 +92,13 @@ SIGNATURES = {
     "d3_knn_normalize": [P, I, I, I, P, P, I, P],
     "d3_topk_merge": [P, LL, I, I, I, P, P, I, I, I, P],
     "d3_knn_vote": [P, P, I, I, P, I, C.POINTER(C.c_int), I, F, I, P, P],
+    "d3_train_resized_crop": [P, P, P, I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, I, P],
+    "d3_linear_inputs": [C.POINTER(C.c_void_p), I, I, I, P, I, P],
+    "d3_linear_xent_fwd_bwd": [P, I, P, I, I, I, I, P, P, I, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],
+    "d3_sgd_momentum": [P, P, P, P, LL, I, P, I, F, F, I, P],
 }
 NO_ARG_SYMBOLS = ["d3_last_error", "d3_abi_version", "d3_launch_count", "d3_reset_launch_count"]
 

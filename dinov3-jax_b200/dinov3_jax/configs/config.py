@@ -49,12 +49,18 @@ DEFAULTS = {
               "layerwise_decay": 0.9, "multi_tensor_optim": True, "adamw_beta1": 0.9, "adamw_beta2": 0.999},
     "checkpointing": {"period": 3750, "max_to_keep": 3},
     "distillation": {"enabled": False, "full_cfg_path": "", "checkpoint_path": ""},   # ssl_default_config.yaml:130-133
-    # k-NN evaluation of the teacher backbone (train.do_test); empty dataset paths: nothing is evaluated.
-    # `config_files` (the reference's list of evaluation configs) is accepted and not read.
+    # k-NN (train.do_test) and linear-probe (train.do_linear_eval) evaluations of the teacher backbone; empty dataset
+    # paths: nothing is evaluated.  `config_files` (the reference's list of evaluation configs) is accepted and not read.
     "evaluation": {"eval_period_iterations": 12500, "config_files": [],
                    "knn": {"train_dataset_path": "", "val_dataset_path": "", "nb_knn": [10, 20, 100, 200],
                            "temperature": 0.07, "batch_size": 256, "resize_size": 256, "crop_size": 224,
-                           "num_workers": 8}},
+                           "num_workers": 8},
+                   "linear": {"train_dataset_path": "", "val_dataset_path": "", "epochs": 10, "epoch_length": 1250,
+                              "batch_size": 128,
+                              "learning_rates": [1e-5, 2e-5, 5e-5, 1e-4, 2e-4, 5e-4, 1e-3, 2e-3, 5e-3, 1e-2, 2e-2,
+                                                 5e-2, 0.1],
+                              "n_last_blocks_list": [1, 4], "avgpools": [False, True], "crop_size": 224,
+                              "resize_size": 256, "num_workers": 8, "seed": 0}},
 }
 
 

@@ -524,3 +524,72 @@ def knn_vote(top_sim: torch.Tensor, top_idx: torch.Tensor, labels: torch.Tensor,
     N.check(N.init().d3_knn_vote(_p(top_sim), _p(top_idx), _ld(top_sim), Q, _p(labels), labels.numel(), ks, nk,
                                  float(temperature), int(num_classes), _p(preds), _s()), "d3_knn_vote")
     return preds
+
+
+# ------------------------------------------------------------------------------------------------- linear probe
+def train_max_taps(boxes, crop: int) -> int:
+    """The filter taps of the widest window d3_train_resized_crop meets for crop boxes (top, left, height, width, ...)
+    resized to crop x crop: torch's 2 * ceil(support) + 1 with support = 2 * max(box / crop, 1), over both axes."""
+    taps = 5
+    for b in boxes:
+        for length in (int(b[2]), int(b[3])):
+            s = length / crop
+            taps = max(taps, 2 * int(math.ceil(2.0 * s if s >= 1.0 else 2.0)) + 1)
+    return taps
+
+
+def train_resized_crop(src: torch.Tensor, desc: torch.Tensor, boxes: torch.Tensor, out: torch.Tensor, *, max_taps: int,
+                       mean=None, std=None) -> torch.Tensor:
+    """torchvision resized_crop(top, left, height, width -> crop x crop, bicubic, antialias) + hflip of n packed uint8
+    HWC images (d3_train_resized_crop).
+
+    src uint8 (flat), desc int64 [n, 3] = (byte offset, H, W) and boxes int32 [n, 5] = (top, left, height, width, flip)
+    on the device; out [n, crop, crop, 3]: bf16 normalised with mean / std, or uint8."""
+    n, S = out.shape[0], out.shape[1]
+    assert src.dtype == torch.uint8 and src.is_contiguous() and desc.dtype == torch.int64 and desc.is_contiguous()
+    assert boxes.dtype == torch.int32 and boxes.is_contiguous() and boxes.shape == (n, 5) and desc.shape == (n, 3)
+    assert out.shape == (n, S, S, 3) and out.is_contiguous() and out.dtype in (bf16, torch.uint8)
+    u8 = out.dtype == torch.uint8
+    m = (C.c_float * 3)(*([0.0] * 3 if u8 else [float(v) for v in mean]))
+    s = (C.c_float * 3)(*([1.0] * 3 if u8 else [float(v) for v in std]))
+    N.check(N.init().d3_train_resized_crop(_p(src), _p(desc), _p(boxes), n, S, int(max_taps), m, s, _p(out), int(u8),
+                                           _s()), "d3_train_resized_crop")
+    return out
+
+
+def linear_inputs(srcs, out: torch.Tensor) -> torch.Tensor:
+    """out[:, s*D:(s+1)*D] = bf16(srcs[s]) for fp32 [B, D] contiguous sources, in one launch (d3_linear_inputs).  out:
+    bf16 [>= B, >= len(srcs) * D] with unit inner stride."""
+    B, D = srcs[0].shape
+    for t in srcs:
+        assert t.dtype == f32 and t.is_contiguous() and t.shape == (B, D)
+    assert out.dtype == bf16 and out.shape[0] >= B and out.shape[1] >= len(srcs) * D
+    ptrs = (C.c_void_p * len(srcs))(*[t.data_ptr() for t in srcs])
+    N.check(N.init().d3_linear_inputs(ptrs, len(srcs), B, D, _p(out), _ld(out), _s()), "d3_linear_inputs")
+    return out
+
+
+def linear_xent_fwd_bwd(logits: torch.Tensor, labels: torch.Tensor, num_classes: int, Cp: int, loss: torch.Tensor,
+                        dz: torch.Tensor):
+    """Cross-entropy of G = loss.numel() classifiers against hard labels (d3_linear_xent_fwd_bwd): logits fp32 [B, >=
+    G * Cp] (classifier g in columns g*Cp .. g*Cp + num_classes), labels int32 [B]; loss fp32 [G] = batch means, dz
+    bf16 [>= B, >= G * Cp] = (softmax - onehot) / B with zero padding columns."""
+    B = logits.shape[0]
+    G = loss.numel()
+    assert logits.dtype == f32 and labels.dtype == torch.int32 and labels.is_contiguous() and labels.numel() == B
+    assert loss.dtype == f32 and loss.is_contiguous() and dz.dtype == bf16 and dz.shape[0] >= B
+    N.check(N.init().d3_linear_xent_fwd_bwd(_p(logits), _ld(logits), _p(labels), B, G, int(num_classes), int(Cp), _p(loss),
+                                            _p(dz), _ld(dz), _s()), "d3_linear_xent_fwd_bwd")
+
+
+def sgd_momentum(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, p_bf16: torch.Tensor | None, lr: torch.Tensor, Cp: int,
+                 *, lr_scale: float = 1.0, momentum: float = 0.9, first: bool = False):
+    """torch SGD(momentum) on fp32 [rows, cols] (or [rows]) p / g / m with lr[row // Cp] * lr_scale per row, the bf16
+    copy of p into p_bf16 (d3_sgd_momentum).  first: the momentum buffer starts as the gradient."""
+    rows, cols = (p.shape[0], 1) if p.dim() == 1 else tuple(p.shape)
+    for t in (p, g, m):
+        assert t.dtype == f32 and t.is_contiguous() and t.shape == p.shape
+    assert lr.dtype == f32 and lr.is_contiguous() and lr.numel() * Cp >= rows
+    assert p_bf16 is None or (p_bf16.dtype == bf16 and p_bf16.is_contiguous() and p_bf16.shape == p.shape)
+    N.check(N.init().d3_sgd_momentum(_p(p), _p(g), _p(m), _p(p_bf16), rows, cols, _p(lr), int(Cp), float(lr_scale),
+                                     float(momentum), int(bool(first)), _s()), "d3_sgd_momentum")

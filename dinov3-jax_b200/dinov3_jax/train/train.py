@@ -231,6 +231,13 @@ def _knn_cfg(config) -> dict:
     return knn if knn.get("train_dataset_path") and knn.get("val_dataset_path") else {}
 
 
+def _linear_cfg(config) -> dict:
+    """The `evaluation.linear` block, or {} when it names no train / val dataset (then nothing is evaluated)."""
+    ev = config.get("evaluation", None) or {}
+    linear = dict(ev.get("linear", None) or {})
+    return linear if linear.get("train_dataset_path") and linear.get("val_dataset_path") else {}
+
+
 def eval_backbone(config, weights):
     """The frozen backbone k-NN evaluates, with the architecture of the run's `student.*` config (the depth is the
     number of blocks in the weights).  `weights`: a DinoVisionTransformer (returned as is); a `save_checkpoint`
@@ -293,6 +300,38 @@ def do_test(config, model, header):
     return results
 
 
+def do_linear_eval(config, model, header):
+    """Linear-probe evaluation of the teacher backbone of `model` (see `eval_backbone`) on the `evaluation.linear`
+    datasets; rank 0 writes <output_dir>/eval/<header>/results_linear.json and returns {classifier name: {"top1",
+    "top5"}, "best_classifier": {"name", "top1", "top5"}} ({} on other ranks).  Without configured datasets it logs one
+    line and returns {}."""
+    import json
+    from .. import distributed
+    linear = _linear_cfg(config)
+    if not linear:
+        if distributed.is_main_process():
+            print(f"do_linear_eval({header}): no evaluation.linear train / val dataset configured, nothing evaluated",
+                  flush=True)
+        return {}
+    backbone = eval_backbone(config, model)            # collective for a live engine under FSDP
+    if not distributed.is_main_process():
+        return {}
+    from ..eval import eval_linear, make_eval_dataset
+    c = config.crops
+    kw = {k: linear[k] for k in ("epochs", "epoch_length", "batch_size", "learning_rates", "n_last_blocks_list",
+                                 "avgpools", "crop_size", "resize_size", "num_workers", "seed") if k in linear}
+    results = eval_linear(backbone, make_eval_dataset(linear["train_dataset_path"]),
+                          make_eval_dataset(linear["val_dataset_path"]), rgb_mean=c.get("rgb_mean", (0.485, 0.456, 0.406)),
+                          rgb_std=c.get("rgb_std", (0.229, 0.224, 0.225)), **kw)
+    out_dir = os.path.join(getattr(config.train, "output_dir", None) or ".", "eval", header)
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "results_linear.json"), "w") as f:
+        json.dump(results, f, indent=1)
+    best = results["best_classifier"]
+    print(f"do_linear_eval({header}): best {best['name']} top-1 {best['top1']:.2f} top-5 {best['top5']:.2f}", flush=True)
+    return results
+
+
 def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None, max_iters: int = 0,
              print_freq: int = 10):
     """train/train.py:319-713.  `data_loader` (optional) yields the reference's collate dicts; by default it is built
@@ -335,7 +374,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
             next(it_loader)
     meters, nan_streak, t0 = {}, 0, time.time()
     ev = config.get("evaluation", None) or {}
-    eval_period = int(ev.get("eval_period_iterations", 0) or 0) if _knn_cfg(config) else 0
+    knn_on, linear_on = bool(_knn_cfg(config)), bool(_linear_cfg(config))
+    eval_period = int(ev.get("eval_period_iterations", 0) or 0) if knn_on or linear_on else 0
     for it in range(start_iter, n_iters):
         try:
             data = next(it_loader)
@@ -352,7 +392,10 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
                 if "keep_every" in ck_cfg and (it + 1) % int(ck_cfg.keep_every) == 0:
                     keep_checkpoint_copy(os.path.join(ckpt_dir, str(it)))
         if eval_period > 0 and (it + 1) % eval_period == 0:          # train/train.py:689-692
-            do_test(config, engine, f"training_{it}")
+            if knn_on:
+                do_test(config, engine, f"training_{it}")
+            if linear_on:
+                do_linear_eval(config, engine, f"training_{it}")
         if it % print_freq == 0 or it == n_iters - 1:
             m = engine.read_metrics()                  # the only device->host sync of the loop
             if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
@@ -380,8 +423,9 @@ def main(argv=None):
     import random
     import numpy as np
     random.seed(args.seed); np.random.seed(args.seed); torch.manual_seed(args.seed)   # setup_job(seed=args.seed), :281
-    if args.eval not in ("", "knn"):
-        raise NotImplementedError(f"--eval {args.eval!r}: the k-NN evaluation (--eval knn, or empty) is the only one")
+    if args.eval not in ("", "knn", "linear"):
+        raise NotImplementedError(f"--eval {args.eval!r}: the evaluations are k-NN (--eval knn, or empty) and the linear "
+                                  "probe (--eval linear)")
     if args.eval_only:                                 # train/train.py:304-311
         import json
         from ..checkpointer import find_latest_checkpoint
@@ -395,6 +439,8 @@ def main(argv=None):
         if os.path.isdir(str(weights)):
             stored = json.loads(open(os.path.join(str(weights), "manifest.json")).read())["iteration"]
             it = int(stored) + 1 if str(stored).lstrip("-").isdigit() else 0
+        if args.eval == "linear":
+            return do_linear_eval(config, str(weights), f"manual_{it}")
         return do_test(config, str(weights), f"manual_{it}")
     model = SSLMetaArch(config)
     return do_train(config, model, resume=not args.no_resume, max_iters=args.max_iters, print_freq=args.print_freq)

@@ -359,6 +359,33 @@ int d3_topk_merge(const float* sims, long long lds, int Q, int valid, int offset
 int d3_knn_vote(const float* top_sim, const int* top_idx, int ldk, int Q, const int* bank_labels, int n_bank,
                 const int* nb_knn /*host*/, int n_k, float temperature, int num_classes, int* preds, void* stream);
 
+/* ---- linear-probe evaluation (the DINOv2 / DINOv3 linear protocol: many linear classifiers on frozen features) ------
+ * Every entry point is deterministic.  The logits are d3_gemm_bf16 (fp32 out, bias epilogue) of one column window of
+ * the input rows per classifier group, the weight gradients d3_gemm_bf16 of dZ^T and the same window, the bias
+ * gradients d3_colsum_bf16 of dZ.
+ * d3_train_resized_crop: torchvision RandomResizedCrop's resized_crop + RandomHorizontalFlip of n packed uint8 images
+ *   (desc as d3_eval_resize_crop): boxes int32 [n, 5] (device) = (top, left, height, width, flip); the box is resized
+ *   to crop x crop with torch's uint8 bicubic antialias arithmetic (the int16 weights of d3_eval_resize_crop), then
+ *   mirrored when flip != 0.  out: bf16 NHWC (u8 / 255 - mean) / std, or (out_u8) uint8.  max_taps >= 2 ceil(2
+ *   max(box / crop, 1)) + 1 over both axes of every box.
+ * d3_linear_inputs: out[b, s * D + c] = bf16(srcs[s][b * D + c]) for the n_src fp32 [B, D] sources (host array of
+ *   device pointers, 16-byte aligned, n_src <= 32): [cls of the last n blocks | patch mean] in one row of stride ld_out.
+ * d3_linear_xent_fwd_bwd: logits fp32 [B, ld >= G * Cp], classifier g in columns [g * Cp, g * Cp + C) (the padding
+ *   columns are not read); labels int32 [B] in [0, C).  loss fp32 [G] = batch-mean cross-entropy per classifier (rows
+ *   summed in order); dz bf16 [B, ld_dz] = (softmax - onehot) / B, 0 in the padding columns.  2 <= C <= 32768,
+ *   Cp % 8 == 0.
+ * d3_sgd_momentum: torch SGD(momentum, dampening 0, weight_decay 0) on fp32 p / g / m [rows, cols]: m = first ? g :
+ *   momentum * m + g; p -= lr[(row) / Cp] * lr_scale * m (lr device fp32, one per classifier of Cp rows); p_bf16
+ *   (optional) receives the bf16 copy of p.  rows * cols % 4 == 0.                                                    */
+int d3_train_resized_crop(const void* src_u8, const long long* desc, const int* boxes, int n, int crop, int max_taps,
+                          const float* mean3 /*host*/, const float* std3 /*host*/, void* out, int out_u8, void* stream);
+int d3_linear_inputs(const float* const* srcs /*host*/, int n_src, int B, int D, void* out_bf16, int ld_out,
+                     void* stream);
+int d3_linear_xent_fwd_bwd(const float* logits, int ld, const int* labels, int B, int G, int C, int Cp, float* loss,
+                           void* dz_bf16, int ld_dz, void* stream);
+int d3_sgd_momentum(float* p, const float* g, float* m, void* p_bf16, long long rows, int cols, const float* lr, int Cp,
+                    float lr_scale, float momentum, int first, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
