@@ -197,6 +197,16 @@ def test_token_rows_gather_scatter_bit_exact():
     ops.gather_rows(src, rows, 0, D, gb, gf)      # empty gather is a no-op
 
 
+@pytest.mark.parametrize("n", [100003 * 4, 100003 * 4 + 3])
+def test_cast_f32_bf16_bit_exact(n):
+    """d3_cast_f32_bf16 (the bf16 compute copy of the weights) rounds as torch does, in the 4-wide body and the tail."""
+    from dinov3_jax import ops
+    src = torch.randn(n, device="cuda")
+    dst = torch.empty(n, device="cuda", dtype=torch.bfloat16)
+    ops.cast_f32_bf16(src, dst)
+    assert torch.equal(dst, src.to(torch.bfloat16))
+
+
 # --------------------------------------------------------------------------------------------------- normalisation / rope
 @pytest.mark.parametrize("T,D", [(1000, 384), (333, 1024), (7, 128), (2051, 768), (100, 256), (300, 1536), (64, 192)])
 def test_layernorm_forward_and_plain_backward(T, D):

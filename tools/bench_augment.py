@@ -3,13 +3,13 @@ events around each call), for the default options at the ViT-L sizes, each furth
 sizes, and the 7B gram-anchoring recipe's sizes (dinov3_vit7b16_gram_anchor.yaml).  Prints the card and its power limit
 with the numbers."""
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "dinov3-jax_b200"))
 import torch
 
 from dinov3_jax.data.gpu_augment import GpuDataAugmentationDINO
+from gpu_timing import card, cuda_ms_each
 
 VITL = dict(global_crops_size=224, local_crops_size=96)
 CASES = [   # name, images per batch, source H x W, options
@@ -27,29 +27,14 @@ CASES = [   # name, images per batch, source H x W, options
 
 def main(iters: int = 20, warmup: int = 3):
     assert torch.cuda.is_available(), "bench_augment measures on the GPU"
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        power = "unknown"
-    print(f"{torch.cuda.get_device_name(0)}, power limit {power}")
+    print(card())
     g = torch.Generator(device="cuda").manual_seed(0)
     for name, B, (H, W), opts in CASES:
         kw = dict(VITL)
         kw.update(opts)
         aug = GpuDataAugmentationDINO((0.32, 1.0), (0.05, 0.32), 8, seed=0, **kw)
         imgs = torch.randint(0, 256, (B, H, W, 3), generator=g, device="cuda", dtype=torch.uint8)
-        for _ in range(warmup):
-            aug(imgs)
-        ts = []
-        for _ in range(iters):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            aug(imgs)
-            e1.record()
-            torch.cuda.synchronize()
-            ts.append(e0.elapsed_time(e1))
-        ts.sort()
+        ts = sorted(cuda_ms_each(lambda: aug(imgs), iters, warmup))
         print(f"  B={B:3d} src {H}x{W}  {name:78s} {ts[len(ts) // 2]:8.2f} ms/batch (median of {iters}, "
               f"min {ts[0]:.2f})")
 

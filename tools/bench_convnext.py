@@ -12,7 +12,6 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -22,20 +21,9 @@ for p in (os.path.join(ROOT, "dinov3-jax_b200"), ROOT, os.path.join(ROOT, "tests
     if p not in sys.path:
         sys.path.insert(0, p)
 
+from gpu_timing import card, cuda_ms  # noqa: E402
+
 HBM_TBS = 3.35     # H100 SXM HBM3 peak
-
-
-def _time(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps
 
 
 def _rel(a, b):
@@ -45,16 +33,6 @@ def _rel(a, b):
 def _hf_state_dict(sd):
     from test_convnext_cpu import _hf_state_dict
     return _hf_state_dict(sd)
-
-
-def device_info():
-    name = torch.cuda.get_device_name(0)
-    try:
-        limit = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        limit = "not measured"
-    return {"gpu": name, "power_limit": limit or "not measured"}
 
 
 def bench_model(size, res, B, steps, warmup):
@@ -76,13 +54,13 @@ def bench_model(size, res, B, steps, warmup):
         with torch.autocast("cuda", dtype=torch.bfloat16):
             ref_bf = hf(pixel_values=xc).last_hidden_state
         mine = torch.cat([ff["x_norm_clstoken"][:, None], ff["x_norm_patchtokens"]], dim=1)
-        t_ours = _time(lambda: ours.forward_features(x), steps, warmup)
-        t_fp32 = _time(lambda: hf(pixel_values=xc), steps, warmup)
+        t_ours = cuda_ms(lambda: ours.forward_features(x), steps, warmup)
+        t_fp32 = cuda_ms(lambda: hf(pixel_values=xc), steps, warmup)
 
         def hf_bf16():
             with torch.autocast("cuda", dtype=torch.bfloat16):
                 hf(pixel_values=xc)
-        t_bf16 = _time(hf_bf16, steps, warmup)
+        t_bf16 = cuda_ms(hf_bf16, steps, warmup)
     del hf
     torch.cuda.empty_cache()
     return {"kind": "model", "size": size, "res": res, "batch": B, "ours_ms": round(t_ours, 3),
@@ -98,7 +76,7 @@ def bench_dwconv(C, H, W, n, steps, warmup):
     w, wb = torch.randn(49, C, device="cuda") / 7, torch.randn(C, device="cuda")
     sc, bi = torch.ones(C, device="cuda"), torch.zeros(C, device="cuda")
     Y = torch.empty(n * H * W, C, dtype=torch.bfloat16, device="cuda")
-    t = _time(lambda: ops.dwconv7_layernorm(X, w, wb, sc, bi, Y), steps, warmup)
+    t = cuda_ms(lambda: ops.dwconv7_layernorm(X, w, wb, sc, bi, Y), steps, warmup)
     nbytes = X.numel() * 4 + Y.numel() * 2
     tbs = nbytes / (t * 1e-3) / 1e12
     return {"kind": "dwconv7_layernorm", "n": n, "H": H, "W": W, "C": C, "us": round(t * 1e3, 2),
@@ -118,7 +96,7 @@ def main():
     _native.init(0)
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
-    rows = [dict(kind="device", **device_info())]
+    rows = [dict(kind="device", **card())]
     print(json.dumps(rows[0]), flush=True)
     from dinov3_jax.models import convnext_sizes
     for res in [int(r) for r in a.res.split(",")]:

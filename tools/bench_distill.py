@@ -19,10 +19,10 @@ import os
 import sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200")); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.dirname(__file__))
+sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200")); sys.path.insert(0, ROOT)
 import torch
 
-from bench_hires_step import card
+from gpu_timing import card, cuda_ms
 
 HEADS = dict(n_prototypes=262144, head_hidden=8192, head_bottleneck=512, ibot_n_prototypes=98304, ibot_head_hidden=4096,
              ibot_head_bottleneck=384)
@@ -70,25 +70,12 @@ def build(B):
     return eng
 
 
-def event_ms(fn, n):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / n
-
-
 def step(B, steps, warmup):
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats()
     eng = build(B)
-    for _ in range(warmup):
-        eng.train_step(None, **HYPER)
-    torch.cuda.synchronize()
-    ms = event_ms(lambda: eng.train_step(None, **HYPER), steps)
-    t_ms = event_ms(lambda: eng.teacher_pass(HYPER["teacher_temp"]), steps)
+    ms = cuda_ms(lambda: eng.train_step(None, **HYPER), steps, warmup)
+    t_ms = cuda_ms(lambda: eng.teacher_pass(HYPER["teacher_temp"]), steps, 0)     # the train steps ran the teacher pass
     m = eng.read_metrics()
     peak = torch.cuda.max_memory_allocated()
     T = eng.teacher.T
@@ -117,11 +104,10 @@ def gemms(T, iters, rounds=2):
     }
     for fn, _, _ in shapes.values():
         fn()
-    torch.cuda.synchronize()
     out = {k: [] for k in shapes}
     for _ in range(rounds):
         for k, (fn, N, K) in shapes.items():
-            ms = event_ms(fn, iters)
+            ms = cuda_ms(fn, iters, 0)     # every shape ran once above, so the rounds alternate warm shapes
             out[k].append(2.0 * T * N * K / (ms * 1e-3) / 1e12)
     return out
 

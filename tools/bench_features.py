@@ -9,7 +9,6 @@ after a warm-up of every shape.
 """
 import argparse
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "dinov3-jax_b200"))
@@ -17,6 +16,7 @@ import torch
 
 from dinov3_jax import _native, ops
 from dinov3_jax.models import DinoVisionTransformer
+from gpu_timing import card, cuda_ms, cuda_ms_each
 
 f32, bf16 = torch.float32, torch.bfloat16
 HBM_BYTES_PER_S = 3.35e12                 # H100 SXM data sheet
@@ -27,11 +27,6 @@ CONFIGS = {   # name: (embed_dim, blocks, heads, ffn_layer, ffn_ratio, mask_k_bi
 }
 SIZES = {224: 64, 512: 16, 1024: 4}
 R, PATCH = 4, 16
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[torch.cuda.current_device()] if q.returncode == 0 else "nvidia-smi unavailable"
 
 
 def random_tree(D, L, ffn, ratio, g):
@@ -83,15 +78,6 @@ def hf_features(model, x_nchw, n=4):
     return feats
 
 
-def timed(fn, sync=True):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1)
-
-
 def kernel_time(B, N, D, Hp, Wp, out_dtype, channels_first, iters=20):
     """Median d3_layernorm_tokens_out time over `iters` launches, L2 flushed before each; returns (ms, bytes)."""
     X = torch.randn(B, N, D, device="cuda")
@@ -100,12 +86,7 @@ def kernel_time(B, N, D, Hp, Wp, out_dtype, channels_first, iters=20):
     pt = torch.empty(*((B, D, Hp, Wp) if channels_first else (B, Hp * Wp, D)), dtype=out_dtype, device="cuda")
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     call = lambda: ops.layernorm_tokens_out(X, cls, st, pt, Hp, Wp, norm=(sc, bi), eps=1e-5, channels_first=channels_first)
-    call()
-    ts = []
-    for _ in range(iters):
-        flush.zero_()
-        ts.append(timed(call))
-    ts.sort()
+    ts = sorted(cuda_ms_each(call, iters, 1, before=flush.zero_))
     nbytes = B * N * D * (4 + out_dtype.itemsize) + 4 * D * 4
     return ts[len(ts) // 2], nbytes
 
@@ -148,10 +129,10 @@ def main():
                     theirs(); torch.cuda.synchronize()
                     peak_hf = torch.cuda.max_memory_allocated() - base
                 t_ours, t_hf = [], []
-                for _ in range(args.iters):         # alternate the two
-                    t_ours.append(timed(ours))
+                for _ in range(args.iters):         # alternate the two, one call each; both were warmed up above
+                    t_ours.append(cuda_ms(ours, 1, 0))
                     if theirs is not None:
-                        t_hf.append(timed(theirs))
+                        t_hf.append(cuda_ms(theirs, 1, 0))
             med = lambda ts: sorted(ts)[len(ts) // 2]
             line = (f"  {size:4d}^2 B={B:2d}: ours {med(t_ours):8.2f} ms  {B / med(t_ours) * 1e3:8.1f} img/s  "
                     f"peak +{peak_ours / 2**20:7.0f} MiB over the weights")

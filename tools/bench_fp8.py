@@ -9,18 +9,19 @@ Prints one JSON line per measurement (and writes them to --out when given; nothi
   quant      GB/s of the quantizers (bytes read + written, from the shapes).
   step       ms per train_step of Engine(fp8=False) and Engine(fp8=True), ViT-L/16 B = 64, alternated `--runs` times
              (`--runs 0` skips it).
-Each record carries the card's name, its power limit and the SM clock read in the same process.
+Each record carries the card's name, its power limit and its maximum SM clock, read in the same process.
 """
 from __future__ import annotations
 
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
 import torch
+
+from gpu_timing import card, cuda_ms
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200"))
@@ -28,29 +29,10 @@ sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200"))
 RECORDS = []
 
 
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
-    f = [x.strip() for x in r.stdout.strip().splitlines()[torch.cuda.current_device()].split(",")] if r.returncode == 0 else []
-    return dict(zip(("gpu", "power_limit", "sm_clock", "sm_clock_max"), f)) if f else {"gpu": torch.cuda.get_device_name()}
-
-
 def emit(rec):
     rec.update(card())
     RECORDS.append(rec)
     print(json.dumps(rec), flush=True)
-
-
-def timed(fn, iters):
-    fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
 
 
 def bench_gemm(M, K, N, site, iters):
@@ -70,7 +52,7 @@ def bench_gemm(M, K, N, site, iters):
     flops = 2.0 * M * N * K
     for kind, bf, f8 in (("forward", lambda: ops.gemm(x, W, y, b_mn=True), lambda: ops.gemm_e4m3(qx, sx, qwt, swt, y)),
                          ("input_grad", lambda: ops.gemm(dy, W, dx), lambda: ops.gemm_e4m3(qdy, sdy, qw, sw, dx))):
-        t_bf, t_f8 = timed(bf, iters), timed(f8, iters)
+        t_bf, t_f8 = cuda_ms(bf, iters, 1), cuda_ms(f8, iters, 1)
         emit({"what": "gemm", "site": site, "kind": kind, "M": M, "K": K if kind == "forward" else N,
               "N": N if kind == "forward" else K, "bf16_tflops": round(flops / t_bf / 1e9, 1),
               "e4m3_tflops": round(flops / t_f8 / 1e9, 1), "bf16_ms": round(t_bf, 4), "e4m3_ms": round(t_f8, 4)})
@@ -83,13 +65,13 @@ def bench_quant(iters):
     for R, C in ((44160, 1024), (44160, 4096)):
         x = torch.randn(R, C, device=dev).to(torch.bfloat16)
         q, s = torch.empty(R, C, dtype=u8, device=dev), torch.empty(R, dtype=f32, device=dev)
-        t = timed(lambda: ops.quant_rows(x, q, s), iters)
+        t = cuda_ms(lambda: ops.quant_rows(x, q, s), iters, 1)
         emit({"what": "quant", "kernel": "quant_rows", "R": R, "C": C, "ms": round(t, 4),
               "GB/s": round(R * C * 3 / t / 1e6, 1)})
     for R, C in ((1024, 4096), (4096, 1024), (4096, 12288)):
         W = torch.randn(R, C, device=dev).to(torch.bfloat16)
         q, s = torch.empty(C, R, dtype=u8, device=dev), torch.empty(C, dtype=f32, device=dev)
-        t = timed(lambda: ops.quant_cols_t(W, q, s), iters)
+        t = cuda_ms(lambda: ops.quant_cols_t(W, q, s), iters, 1)
         emit({"what": "quant", "kernel": "quant_cols_t", "R": R, "C": C, "ms": round(t, 4),
               "GB/s": round(R * C * 3 / t / 1e6, 1)})
 

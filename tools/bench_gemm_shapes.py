@@ -1,33 +1,16 @@
 """GPU microbench: every GEMM call shape of one ViT-L/16 B=64 training step, with its real epilogue, timed in isolation."""
-import os, statistics, subprocess, sys
+import os, statistics, sys
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200"))
 import torch
 from dinov3_jax import ops
 
+from gpu_timing import card, cuda_ms
+
 dev = "cuda"
 bf, f32 = torch.bfloat16, torch.float32
 D, Hd = 1024, 4096
 Tt, Ts = 25216, 44160
-
-
-def card():
-    """Card name and power limit, read in the same run as the numbers they belong to."""
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ""
-    return q or f"{torch.cuda.get_device_name(0)}, power limit not read"
-
-
-def timeit(fn, iters=8):
-    for _ in range(3): fn()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(iters): fn()
-    e.record(); torch.cuda.synchronize()
-    return s.elapsed_time(e) / iters
 
 
 def cases():
@@ -68,7 +51,7 @@ def run(widths, batches, only=None):
     for _ in range(batches):
         for name, _, fn in cs:
             for w in widths:
-                ms[(name, w)].append(timeit(lambda: fn(w)))
+                ms[(name, w)].append(cuda_ms(lambda: fn(w), 8, 3))
     med = {k: statistics.median(v) for k, v in ms.items()}
     print(f"  {'shape':44s}" + "".join(f" {'auto' if w == 0 else w:>21}" for w in widths))
     tot = {w: [0.0, 0] for w in widths}

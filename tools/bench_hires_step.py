@@ -8,22 +8,13 @@ import argparse
 import collections
 import dataclasses
 import os
-import subprocess
 import sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200")); sys.path.insert(0, ROOT)
 import torch
 
-
-def card():
-    """Card name and power limit, read in the same run as the numbers they belong to."""
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ""
-    return q or f"{torch.cuda.get_device_name(0)}, power limit not read"
+from gpu_timing import card, cuda_ms
 
 
 def main():
@@ -57,15 +48,8 @@ def main():
     eng.set_batch(batch)
     for _ in range(args.warmup):
         eng.train_step(None, **hyper)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     _native.reset_launch_count()
-    e0.record()
-    for _ in range(args.steps):
-        eng.train_step(None, **hyper)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / args.steps
+    ms = cuda_ms(lambda: eng.train_step(None, **hyper), args.steps, 0)     # warmed up above, before the count restarts
     launches = _native.launch_count() / args.steps
     loss = eng.read_metrics()["total_loss"]
     ntok = lambda s: (s // 16) ** 2 + 1 + cfg.n_storage

@@ -13,7 +13,6 @@ Prints the card and its power limit with the numbers.   python tools/bench_knn.p
 """
 import argparse
 import os
-import subprocess
 import sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -22,29 +21,9 @@ import torch
 
 from dinov3_jax import ops
 from dinov3_jax.eval import KnnClassifier
+from gpu_timing import card, cuda_ms
 
 bf16, f32 = torch.bfloat16, torch.float32
-
-
-def card():
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        power = "unknown"
-    return f"{torch.cuda.get_device_name(0)}, power limit {power}"
-
-
-def timed(fn, iters, warmup=2):
-    for _ in range(warmup):
-        fn()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
 
 
 def clustered(n, centers, g, spread=4.0):
@@ -93,7 +72,7 @@ def bench_search(Q, N, D, k, C, chunk, tile):
     topk_ms = sum(e[1].elapsed_time(e[2]) for e in rec)
     nb = [10, 20, 100, 200]
     preds = torch.empty(Q, len(nb), 5, dtype=torch.int32, device="cuda")
-    vote_ms = timed(lambda: ops.knn_vote(top_s, top_i, clf.labels, nb, 0.07, C, preds), 3)
+    vote_ms = cuda_ms(lambda: ops.knn_vote(top_s, top_i, clf.labels, nb, 0.07, C, preds), 3, 2)
     acc = {k_: 100.0 * (preds[:, j, 0] == yva).float().mean().item() for j, k_ in enumerate(nb)}
     flops = 2.0 * Q * rows * D
     sim_bytes = 2 * 4.0 * Q * rows
@@ -151,8 +130,8 @@ def bench_transform(batch=256, iters=10):
     flat, desc = flat.cuda(), desc.cuda()
     out = torch.empty(batch, 224, 224, 3, dtype=bf16, device="cuda")
     taps = ops.eval_max_taps([(375, 500)], 256)
-    ms = timed(lambda: ops.eval_resize_crop(flat, desc, out, resize=256, max_taps=taps, mean=(0.485, 0.456, 0.406),
-                                            std=(0.229, 0.224, 0.225)), iters)
+    ms = cuda_ms(lambda: ops.eval_resize_crop(flat, desc, out, resize=256, max_taps=taps, mean=(0.485, 0.456, 0.406),
+                                              std=(0.229, 0.224, 0.225)), iters, 2)
     print(f"eval transform 500x375 -> 256 -> 224^2: {ms:.3f} ms per batch of {batch}, {batch / ms * 1e3:,.0f} images/s")
 
 
@@ -165,7 +144,7 @@ def bench_extract(batch=256, iters=5):
     model = DinoVisionTransformer(tree_from_flat(init_backbone(cfg, torch.Generator().manual_seed(0))), embed_dim=1024,
                                   n_blocks=24, num_heads=16)
     x = torch.randn(batch, 224, 224, 3, device="cuda").to(bf16)
-    ms = timed(lambda: model(x), iters)
+    ms = cuda_ms(lambda: model(x), iters, 2)
     print(f"ViT-L/16 class tokens at 224^2: {ms:.1f} ms per batch of {batch}, {batch / ms * 1e3:,.0f} images/s "
           f"(1 331 167 images: {1331167 / batch * ms / 1e3 / 60:.1f} min)")
 

@@ -17,7 +17,6 @@ Prints the card and its power limit with the numbers.   python tools/bench_linea
 """
 import argparse
 import os
-import subprocess
 import sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -26,30 +25,10 @@ import torch
 
 from dinov3_jax import ops
 from dinov3_jax.eval.linear import LinearClassifiers, sample_train_boxes, write_linear_inputs
+from gpu_timing import card, cuda_ms
 
 bf16, f32 = torch.bfloat16, torch.float32
 B, C, D, S = 128, 1000, 1024, 224
-
-
-def card():
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        power = "unknown"
-    return f"{torch.cuda.get_device_name(0)}, power limit {power}"
-
-
-def timed(fn, iters, warmup=2):
-    for _ in range(warmup):
-        fn()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
 
 
 def bench_crop(iters):
@@ -61,8 +40,8 @@ def bench_crop(iters):
     taps = ops.train_max_taps(boxes.tolist(), S)
     flat, desc, bx = flat.cuda(), desc.cuda(), boxes.cuda()
     out = torch.empty(B, S, S, 3, dtype=bf16, device="cuda")
-    ms = timed(lambda: ops.train_resized_crop(flat, desc, bx, out, max_taps=taps, mean=(0.485, 0.456, 0.406),
-                                              std=(0.229, 0.224, 0.225)), iters)
+    ms = cuda_ms(lambda: ops.train_resized_crop(flat, desc, bx, out, max_taps=taps, mean=(0.485, 0.456, 0.406),
+                                                std=(0.229, 0.224, 0.225)), iters, 2)
     print(f"train crop 500x375 -> RandomResizedCrop 224^2 + flip: {ms:.3f} ms per batch of {B}, "
           f"{B / ms * 1e3:,.0f} images/s")
     return out
@@ -76,7 +55,7 @@ def bench_features(images, out, iters):
     cfg = ModelCfg(embed_dim=D, depth=24, heads=16)
     model = DinoVisionTransformer(tree_from_flat(init_backbone(cfg, torch.Generator().manual_seed(0))), embed_dim=D,
                                   n_blocks=24, num_heads=16)
-    ms = timed(lambda: write_linear_inputs(model, images, 4, out), iters)
+    ms = cuda_ms(lambda: write_linear_inputs(model, images, 4, out), iters, 2)
     print(f"ViT-L/16 features (last 4 blocks' class tokens + patch mean) at 224^2: {ms:.1f} ms per batch of {B}, "
           f"{B / ms * 1e3:,.0f} images/s")
     return ms
@@ -140,8 +119,8 @@ def bench_heads(iters):
     print("weights after 6 steps, max relative L2 difference to the torch fp32 module per window: " +
           ", ".join(f"{k}: {v:.2e}" for k, v in worst.items()) +
           f" ({'within' if max(worst.values()) <= 1e-3 else 'ABOVE'} 1e-3)")
-    ms = timed(ours, iters)
-    ms_t = timed(theirs, iters)
+    ms = cuda_ms(ours, iters, 2)
+    ms_t = cuda_ms(theirs, iters, 2)
     fl = head_flops(clf)
     print(f"head work (52 classifiers, {C} classes, B = {B}): {ms:.2f} ms per step "
           f"({fl / 1e9:.1f} GFLOP of GEMMs, {fl / ms / 1e9:.0f} TFLOP/s over the whole step); torch baseline "

@@ -18,10 +18,10 @@ import os
 import sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200")); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.dirname(__file__))
+sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200")); sys.path.insert(0, ROOT)
 import torch
 
-from bench_hires_step import card
+from gpu_timing import card, cuda_ms
 
 HEADS = {"shared": {}, "dinov3": dict(n_prototypes=262144, head_hidden=8192, head_bottleneck=512, ibot_n_prototypes=98304,
                                       ibot_head_hidden=4096, ibot_head_bottleneck=384)}
@@ -41,20 +41,11 @@ def build(name, B):
     return cfg, eng
 
 
-def timed(name, B, steps, warmup):
+def step_ms(name, B, steps, warmup):
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats()
     cfg, eng = build(name, B)
-    for _ in range(warmup):
-        eng.train_step(None, **HYPER)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        eng.train_step(None, **HYPER)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
+    ms = cuda_ms(lambda: eng.train_step(None, **HYPER), steps, warmup)
     m = eng.read_metrics()
     peak = torch.cuda.max_memory_allocated()
     del eng
@@ -116,7 +107,7 @@ def main():
         return
     for rnd in range(args.rounds):
         for name in HEADS:
-            ms, peak, m = timed(name, B, args.steps, args.warmup)
+            ms, peak, m = step_ms(name, B, args.steps, args.warmup)
             print(f"round {rnd} {name:7s} B = {B}: {ms:.2f} ms/step, max_memory_allocated {peak / 2**30:.2f} GiB, "
                   f"dino_local {m['dino_local_crops_loss']:.3f}, ibot {m['ibot_loss']:.3f}", flush=True)
 

@@ -9,22 +9,13 @@ usage: python tools/step_kernel_times.py [--steps 3] [--warmup 3] [--batch 64] [
 import argparse
 import collections
 import os
-import subprocess
 import sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, os.path.join(ROOT, "dinov3-jax_b200"))
 import torch  # noqa: E402
 
-
-def card():
-    """Card name and power limit, read in the same run as the numbers they belong to."""
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ""
-    return q or f"{torch.cuda.get_device_name(0)}, power limit not read"
+from gpu_timing import card, cuda_ms  # noqa: E402
 
 
 def kernel_name(key):
@@ -69,15 +60,9 @@ def main():
     print(card())
 
     # ---- every kernel of `steps` steps
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     acts = [torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]
     with torch.profiler.profile(activities=acts) as prof:
-        e0.record()
-        for _ in range(args.steps):
-            eng.train_step(None, **hyper)
-        e1.record()
-        torch.cuda.synchronize()
-    step_ms = e0.elapsed_time(e1) / args.steps
+        step_ms = cuda_ms(lambda: eng.train_step(None, **hyper), args.steps, 0)     # warmed up above, unprofiled
     t_us, n = collections.Counter(), collections.Counter()
     for ev in prof.key_averages():
         if ev.device_type != torch.autograd.DeviceType.CUDA:
