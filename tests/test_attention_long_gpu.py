@@ -1,4 +1,4 @@
-"""-m gpu: attention on crops longer than the resident kernels hold (forward span > 448, backward N > 384), served by the
+"""-m gpu: attention on crops longer than the resident kernels hold (forward span > 448, backward span > 256), served by the
 streamed kernels: against PyTorch fp32 / autograd, with the fused inverse RoPE, bit-reproducible, and through the
 module forward and full training steps at high resolution against the oracle."""
 import dataclasses
