@@ -167,6 +167,85 @@ __global__ void __launch_bounds__(EV_THREADS) eval_resize_crop_kernel(
   }
 }
 
+// The segmentation probe's image and label crops (one kernel for both, from the same box).  Image n (desc as above) is
+// resized to (rh, rw) = boxes[6n], boxes[6n + 1] with the arithmetic above (the whole image is the source window), and
+// the out_h x out_w window at (top, left) = boxes[6n + 2], boxes[6n + 3] of the resized image is written; the part of
+// the window inside the resized image (vh x vw) is mirrored within its own width when flip = boxes[6n + 4], and the
+// rest (bottom / right) is 0 in the image (after normalisation) and 255 in the labels.  Labels: torch's 'nearest'
+// (src = min(floor(dst * in / out), in - 1)) from a uint8 map of the image's size at lab_src + desc offset / 3.
+template <bool U8>
+__global__ void __launch_bounds__(EV_THREADS) seg_crop_kernel(
+    const uint8_t* __restrict__ src, const long long* __restrict__ desc, const uint8_t* __restrict__ lab_src,
+    const int* __restrict__ boxes, int out_h, int out_w, int max_taps, float m0, float m1, float m2, float s0, float s1,
+    float s2, void* __restrict__ out, uint8_t* __restrict__ lab_out) {
+  extern __shared__ __align__(16) unsigned char ev_smem[];
+  __shared__ double red[EV_THREADS / 32];
+  int* lo_x = reinterpret_cast<int*>(ev_smem);
+  int* lo_y = lo_x + out_w;
+  short* w_x = reinterpret_cast<short*>(lo_y + out_h);
+  short* w_y = w_x + (size_t)out_w * max_taps;
+  const int n = blockIdx.y;
+  const long long off = desc[3 * n];
+  const int H = (int)desc[3 * n + 1], W = (int)desc[3 * n + 2];
+  const int* bx = boxes + 6 * n;
+  const int rh = bx[0], rw = bx[1], top = bx[2], left = bx[3], flip = bx[4];
+  const EvalAxis ax = eval_axis(W, rw, left), ay = eval_axis(H, rh, top);
+  const int px = eval_precision(eval_axis_wmax(ax, W, red));
+  const int py = eval_precision(eval_axis_wmax(ay, H, red));
+  eval_axis_table(ax, W, out_w, px, max_taps, lo_x, w_x);
+  eval_axis_table(ay, H, out_h, py, max_taps, lo_y, w_y);
+  __syncthreads();
+  const int tx = min(ax.taps, max_taps), ty = min(ay.taps, max_taps);
+  const int vh = min(out_h, rh - top), vw = min(out_w, rw - left);
+  const float nsy = (float)H / (float)rh, nsx = (float)W / (float)rw;
+  const uint8_t* img = src + off;
+  const int row0 = blockIdx.x * EV_ROWS, rows = min(EV_ROWS, out_h - row0);
+  const int hx = px > 0 ? 1 << (px - 1) : 0, hy = py > 0 ? 1 << (py - 1) : 0;
+  for (int p = threadIdx.x; p < rows * out_w; p += blockDim.x) {
+    const int oy = row0 + p / out_w, ox = p % out_w;
+    const size_t o = ((size_t)n * out_h + oy) * out_w + ox;
+    const bool inside = oy < vh && ox < vw;
+    int r = 0, g = 0, b = 0;
+    if (inside) {
+      const int sx = flip ? vw - 1 - ox : ox;
+      const short* wy = w_y + (size_t)oy * max_taps;
+      const short* wx = w_x + (size_t)sx * max_taps;
+      const int y0 = lo_y[oy], x0 = lo_x[sx];
+      int ar = hy, ag = hy, ab = hy;
+      for (int j = 0; j < ty; ++j) {
+        const int wv = wy[j];
+        if (wv == 0 || y0 + j >= H) continue;
+        const uint8_t* row = img + ((size_t)(y0 + j) * W + x0) * 3;
+        int hr = hx, hg = hx, hb = hx;
+        for (int i = 0; i < tx && x0 + i < W; ++i) {
+          const int w = wx[i];
+          hr += w * row[3 * i]; hg += w * row[3 * i + 1]; hb += w * row[3 * i + 2];
+        }
+        ar += wv * min(max(hr >> px, 0), 255);
+        ag += wv * min(max(hg >> px, 0), 255);
+        ab += wv * min(max(hb >> px, 0), 255);
+      }
+      r = min(max(ar >> py, 0), 255); g = min(max(ag >> py, 0), 255); b = min(max(ab >> py, 0), 255);
+      if (lab_out) {
+        const int ly = min((int)floorf((float)(top + oy) * nsy), H - 1);
+        const int lx = min((int)floorf((float)(left + sx) * nsx), W - 1);
+        lab_out[o] = lab_src[off / 3 + (size_t)ly * W + lx];
+      }
+    } else if (lab_out) {
+      lab_out[o] = 255;
+    }
+    if constexpr (U8) {
+      uint8_t* y = reinterpret_cast<uint8_t*>(out) + 3 * o;
+      y[0] = (uint8_t)r; y[1] = (uint8_t)g; y[2] = (uint8_t)b;
+    } else {
+      __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(out) + 3 * o;
+      y[0] = __float2bfloat16(inside ? (r / 255.f - m0) / s0 : 0.f);
+      y[1] = __float2bfloat16(inside ? (g / 255.f - m1) / s1 : 0.f);
+      y[2] = __float2bfloat16(inside ? (b / 255.f - m2) / s2 : 0.f);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------- L2 normalisation
 // y = x / max(||x||, 1e-12) per row (F.normalize), one warp per row, lanes strided then a butterfly: the same bits on
 // every run.  Writes fp32 and / or bf16.
@@ -509,6 +588,36 @@ int d3_train_resized_crop(const void* src_u8, const long long* desc, const int* 
     return set_error(D3_ERR_ARG, "d3_train_resized_crop: need crop >= 1, max_taps >= 1 and non-null buffers");
   return launch_resize_crop("d3_train_resized_crop", src_u8, desc, boxes, n, 0, crop, max_taps, mean3, std3, out,
                             out_u8, stream);
+}
+
+int d3_seg_crop(const void* src_u8, const long long* desc, const void* labels_u8, const int* boxes, int n, int out_h,
+                int out_w, int max_taps, const float* mean3, const float* std3, void* out, int out_u8, void* label_out,
+                void* stream) {
+  if (n <= 0) return D3_OK;
+  if (out_h < 1 || out_w < 1 || max_taps < 1 || !src_u8 || !desc || !boxes || !out || (label_out && !labels_u8))
+    return set_error(D3_ERR_ARG, "d3_seg_crop: need out_h, out_w, max_taps >= 1, non-null buffers (labels with label_out)");
+  const size_t smem = (size_t)(out_h + out_w) * sizeof(int) + (size_t)(out_h + out_w) * max_taps * sizeof(short);
+  constexpr int SMEM_MAX = 200 * 1024;
+  if (smem > SMEM_MAX) return set_error(D3_ERR_ARG, "d3_seg_crop: (out_h + out_w) * max_taps too large");
+  if (!out_u8 && (!mean3 || !std3)) return set_error(D3_ERR_ARG, "d3_seg_crop: mean / std needed for bf16 output");
+  static const cudaError_t c0 =
+      cudaFuncSetAttribute(seg_crop_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
+  static const cudaError_t c1 =
+      cudaFuncSetAttribute(seg_crop_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
+  if (c0 != cudaSuccess || c1 != cudaSuccess) return set_error(D3_ERR_CUDA, "d3_seg_crop: smem attribute");
+  const dim3 grid((out_h + EV_ROWS - 1) / EV_ROWS, n);
+  const float m[3] = {out_u8 ? 0.f : mean3[0], out_u8 ? 0.f : mean3[1], out_u8 ? 0.f : mean3[2]};
+  const float s[3] = {out_u8 ? 1.f : std3[0], out_u8 ? 1.f : std3[1], out_u8 ? 1.f : std3[2]};
+  if (out_u8)
+    seg_crop_kernel<true><<<grid, EV_THREADS, smem, STREAM(stream)>>>(
+        (const uint8_t*)src_u8, desc, (const uint8_t*)labels_u8, boxes, out_h, out_w, max_taps, m[0], m[1], m[2], s[0],
+        s[1], s[2], out, (uint8_t*)label_out);
+  else
+    seg_crop_kernel<false><<<grid, EV_THREADS, smem, STREAM(stream)>>>(
+        (const uint8_t*)src_u8, desc, (const uint8_t*)labels_u8, boxes, out_h, out_w, max_taps, m[0], m[1], m[2], s[0],
+        s[1], s[2], out, (uint8_t*)label_out);
+  D3_CHECK_LAUNCH();
+  return D3_OK;
 }
 
 int d3_knn_normalize(const float* x, int ldx, int R, int D, float* y_f32, void* y_bf16, int ldy, void* stream) {

@@ -95,6 +95,11 @@ SIGNATURES = {
     "d3_train_resized_crop": [P, P, P, I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, I, P],
     "d3_linear_inputs": [C.POINTER(C.c_void_p), I, I, I, P, I, P],
     "d3_linear_xent_fwd_bwd": [P, I, P, I, I, I, I, P, P, I, P],
+    "d3_seg_crop": [P, P, P, P, I, I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, I, P, P],
+    "d3_seg_bn_stats": [P, I, I, I, P, P, P, P, F, P],
+    "d3_seg_bn_apply": [P, I, LL, I, P, P, F, P, I, P],
+    "d3_seg_xent_fwd_bwd": [P, I, P, I, I, I, I, I, I, I, P, P, P, P, I, P],
+    "d3_seg_predict_confusion": [P, I, P, I, I, I, I, I, I, P, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

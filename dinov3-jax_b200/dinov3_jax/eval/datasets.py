@@ -1,5 +1,6 @@
-"""Labelled image datasets for evaluation.  Each item is (uint8 HWC RGB numpy array, int label); images keep their own
-sizes, the eval transform runs on the GPU (`ops.eval_resize_crop`).  Decoding is host plumbing in DataLoader workers."""
+"""Labelled image datasets for evaluation.  Each item is (uint8 HWC RGB numpy array, int label), or for segmentation
+(uint8 HWC RGB, uint8 HW label map); images keep their own sizes, the transforms run on the GPU (`ops.eval_resize_crop`,
+`ops.seg_crop`).  Decoding is host plumbing in DataLoader workers."""
 from __future__ import annotations
 
 import os
@@ -54,6 +55,70 @@ class NpzDataset:
 
     def __getitem__(self, i):
         return self.images[i], self.targets[i]
+
+
+IGNORE_LABEL = 255
+
+
+def reduce_zero_label(label: np.ndarray) -> np.ndarray:
+    """ADE20K's label convention: 0 (other) becomes 255 (ignored) and every other value v becomes v - 1 (255 stays)."""
+    label = np.asarray(label, dtype=np.uint8)
+    return np.where((label == 0) | (label == IGNORE_LABEL), IGNORE_LABEL, label.astype(np.int16) - 1).astype(np.uint8)
+
+
+class ADE20KSegmentation:
+    """ADE20K SceneParsing (150 classes) in the layout of the reference's data/datasets/ade20k.py: the file names of
+    `split` ("train" or "val") come from root/ADE20K_object150_<split>.txt, sorted; image `name` is root/images/<name>
+    and its label map root/annotations/<name without extension>.png.  Items are (uint8 HWC RGB, uint8 HW class ids,
+    255 = ignore) after `reduce_zero_label`."""
+
+    def __init__(self, root, split: str = "train"):
+        if split not in ("train", "val"):
+            raise ValueError(f"split must be 'train' or 'val', got {split!r}")
+        self.root, self.split = str(root), split
+        with open(os.path.join(self.root, f"ADE20K_object150_{split}.txt")) as f:
+            names = sorted(line.strip() for line in f.read().strip().split("\n") if line.strip())
+        self.images = [os.path.join(self.root, "images", n) for n in names]
+        self.labels = [os.path.join(self.root, "annotations", os.path.splitext(n)[0] + ".png") for n in names]
+
+    def __len__(self):
+        return len(self.images)
+
+    def __getitem__(self, i):
+        from PIL import Image
+        with Image.open(self.images[i]) as im:
+            img = np.asarray(im.convert("RGB"), dtype=np.uint8)
+        with Image.open(self.labels[i]) as lb:
+            label = reduce_zero_label(np.asarray(lb))
+        if label.shape != img.shape[:2]:
+            raise ValueError(f"{self.labels[i]}: label {label.shape} does not match image {img.shape[:2]}")
+        return img, label
+
+
+class SegNpzDataset:
+    """An .npz file with `images` (uint8 [N, H, W, 3]) and `labels` (uint8 [N, H, W], class ids, 255 = ignore)."""
+
+    def __init__(self, path):
+        with np.load(path, allow_pickle=False) as z:
+            self.images = np.asarray(z["images"])
+            self.labels = np.asarray(z["labels"])
+        if self.images.dtype != np.uint8 or self.images.ndim != 4 or self.images.shape[-1] != 3:
+            raise ValueError(f"{path}: images must be uint8 [N, H, W, 3], got {self.images.dtype} {self.images.shape}")
+        if self.labels.dtype != np.uint8 or self.labels.shape != self.images.shape[:3]:
+            raise ValueError(f"{path}: labels must be uint8 {list(self.images.shape[:3])}, got {self.labels.dtype} "
+                             f"{list(self.labels.shape)}")
+
+    def __len__(self):
+        return len(self.images)
+
+    def __getitem__(self, i):
+        return self.images[i], self.labels[i]
+
+
+def make_seg_dataset(path, split: str = "train"):
+    """An .npz file -> SegNpzDataset, a directory -> ADE20KSegmentation(path, split)."""
+    path = str(path)
+    return SegNpzDataset(path) if path.endswith(".npz") else ADE20KSegmentation(path, split)
 
 
 def make_eval_dataset(path):

@@ -593,3 +593,96 @@ def sgd_momentum(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, p_bf16: torc
     assert p_bf16 is None or (p_bf16.dtype == bf16 and p_bf16.is_contiguous() and p_bf16.shape == p.shape)
     N.check(N.init().d3_sgd_momentum(_p(p), _p(g), _p(m), _p(p_bf16), rows, cols, _p(lr), int(Cp), float(lr_scale),
                                      float(momentum), int(bool(first)), _s()), "d3_sgd_momentum")
+
+
+# ------------------------------------------------------------------------------------------ segmentation probe
+def seg_max_taps(sizes, resized) -> int:
+    """The filter taps of the widest window d3_seg_crop meets for images of (H, W) `sizes` resized to (rh, rw)
+    `resized`: torch's 2 * ceil(support) + 1 with support = 2 * max(input / resized, 1), over both axes."""
+    taps = 5
+    for (H, W), (rh, rw) in zip(sizes, resized):
+        for i, o in ((int(H), int(rh)), (int(W), int(rw))):
+            s = i / o
+            taps = max(taps, 2 * int(math.ceil(2.0 * s if s >= 1.0 else 2.0)) + 1)
+    return taps
+
+
+def seg_crop(src: torch.Tensor, desc: torch.Tensor, boxes: torch.Tensor, out: torch.Tensor, *, max_taps: int,
+             labels: torch.Tensor | None = None, label_out: torch.Tensor | None = None, mean=None, std=None):
+    """Resize + crop + flip of n packed uint8 HWC images and their label maps (d3_seg_crop).
+
+    src uint8 (flat), desc int64 [n, 3] = (byte offset, H, W), boxes int32 [n, 6] = (rh, rw, top, left, flip, 0) on the
+    device; out [n, out_h, out_w, 3]: bf16 normalised with mean / std, or uint8.  labels: uint8 (flat, image n's map at
+    offset desc[n, 0] / 3) and label_out uint8 [n, out_h, out_w], or both None."""
+    n, Ho, Wo = out.shape[0], out.shape[1], out.shape[2]
+    assert src.dtype == torch.uint8 and src.is_contiguous() and desc.dtype == torch.int64 and desc.is_contiguous()
+    assert boxes.dtype == torch.int32 and boxes.is_contiguous() and boxes.shape == (n, 6) and desc.shape == (n, 3)
+    assert out.shape == (n, Ho, Wo, 3) and out.is_contiguous() and out.dtype in (bf16, torch.uint8)
+    assert (labels is None) == (label_out is None)
+    if label_out is not None:
+        assert labels.dtype == torch.uint8 and labels.is_contiguous()
+        assert label_out.dtype == torch.uint8 and label_out.is_contiguous() and label_out.shape == (n, Ho, Wo)
+    u8 = out.dtype == torch.uint8
+    m = (C.c_float * 3)(*([0.0] * 3 if u8 else [float(v) for v in mean]))
+    s = (C.c_float * 3)(*([1.0] * 3 if u8 else [float(v) for v in std]))
+    N.check(N.init().d3_seg_crop(_p(src), _p(desc), _p(labels), _p(boxes), n, Ho, Wo, int(max_taps), m, s, _p(out),
+                                 int(u8), _p(label_out), _s()), "d3_seg_crop")
+    return out
+
+
+def seg_bn_stats(x: torch.Tensor, mean: torch.Tensor, var: torch.Tensor, running_mean: torch.Tensor | None = None,
+                 running_var: torch.Tensor | None = None, momentum: float = 0.1):
+    """Column mean and biased variance of bf16 x [M, N] into fp32 [N] mean / var; the running statistics (both or
+    neither) are updated as torch's BatchNorm in training mode does (d3_seg_bn_stats)."""
+    M, Nn = x.shape
+    assert x.dtype == bf16
+    for t in (mean, var, running_mean, running_var):
+        assert t is None or (t.dtype == f32 and t.is_contiguous() and t.numel() == Nn)
+    N.check(N.init().d3_seg_bn_stats(_p(x), _ld(x), M, Nn, _p(mean), _p(var), _p(running_mean), _p(running_var),
+                                     float(momentum), _s()), "d3_seg_bn_stats")
+
+
+def seg_bn_apply(x: torch.Tensor, mean: torch.Tensor, var: torch.Tensor, out: torch.Tensor, eps: float = 1e-5):
+    """out = bf16((x - mean) / sqrt(var + eps)) per column of bf16 x [M, N] (d3_seg_bn_apply)."""
+    M, Nn = x.shape
+    assert x.dtype == bf16 and out.dtype == bf16 and out.shape[0] >= M and out.shape[1] >= Nn
+    assert mean.dtype == f32 and var.dtype == f32 and mean.numel() == Nn and var.numel() == Nn
+    N.check(N.init().d3_seg_bn_apply(_p(x), _ld(x), M, Nn, _p(mean), _p(var), float(eps), _p(out), _ld(out), _s()),
+            "d3_seg_bn_apply")
+    return out
+
+
+def seg_xent_fwd_bwd(logits: torch.Tensor, labels: torch.Tensor, hw, num_classes: int, loss: torch.Tensor,
+                     count: torch.Tensor, dz_f32: torch.Tensor | None = None, dz_bf16: torch.Tensor | None = None,
+                     Cp: int | None = None):
+    """Mean cross-entropy over the valid pixels (label < num_classes; 255 is the ignore label) of the patch logits
+    upsampled bilinearly (align_corners=False) to the label size, and its gradient to the patch logits
+    (d3_seg_xent_fwd_bwd).  logits fp32 [B * h * w, >= num_classes] (ld any), labels uint8 [B, Hl, Wl], hw = (h, w);
+    loss fp32 [1], count int32 [1]; dz_f32 / dz_bf16 [>= B * h * w, >= Cp] (columns [num_classes, Cp) zeroed)."""
+    B, Hl, Wl = labels.shape
+    h, w = int(hw[0]), int(hw[1])
+    Cp = int(num_classes) if Cp is None else int(Cp)
+    assert logits.dtype == f32 and logits.shape[0] >= B * h * w and labels.dtype == torch.uint8 and labels.is_contiguous()
+    assert loss.dtype == f32 and count.dtype == torch.int32
+    ld = None
+    for t, dt in ((dz_f32, f32), (dz_bf16, bf16)):
+        if t is not None:
+            assert t.dtype == dt and t.shape[0] >= B * h * w and t.shape[1] >= Cp
+            assert ld is None or ld == _ld(t), "dz_f32 and dz_bf16 share one row stride"
+            ld = _ld(t)
+    N.check(N.init().d3_seg_xent_fwd_bwd(_p(logits), _ld(logits), _p(labels), B, h, w, Hl, Wl, int(num_classes), Cp,
+                                         _p(loss), _p(count), _p(dz_f32), _p(dz_bf16), ld or Cp, _s()),
+            "d3_seg_xent_fwd_bwd")
+
+
+def seg_predict_confusion(logits: torch.Tensor, labels: torch.Tensor, hw, num_classes: int, conf: torch.Tensor):
+    """conf int64 [C, C] += counts of (label, argmax of the upsampled logits) over the pixels with label < C
+    (d3_seg_predict_confusion); shapes as seg_xent_fwd_bwd."""
+    B, Hl, Wl = labels.shape
+    h, w = int(hw[0]), int(hw[1])
+    C_ = int(num_classes)
+    assert logits.dtype == f32 and logits.shape[0] >= B * h * w and labels.dtype == torch.uint8 and labels.is_contiguous()
+    assert conf.dtype == torch.int64 and conf.is_contiguous() and conf.shape == (C_, C_)
+    N.check(N.init().d3_seg_predict_confusion(_p(logits), _ld(logits), _p(labels), B, h, w, Hl, Wl, C_, _p(conf), _s()),
+            "d3_seg_predict_confusion")
+    return conf

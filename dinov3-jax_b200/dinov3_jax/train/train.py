@@ -238,6 +238,13 @@ def _linear_cfg(config) -> dict:
     return linear if linear.get("train_dataset_path") and linear.get("val_dataset_path") else {}
 
 
+def _seg_cfg(config) -> dict:
+    """The `evaluation.segmentation` block, or {} when it names no train / val dataset (then nothing is evaluated)."""
+    ev = config.get("evaluation", None) or {}
+    seg = dict(ev.get("segmentation", None) or {})
+    return seg if seg.get("train_dataset_path") and seg.get("val_dataset_path") else {}
+
+
 def eval_backbone(config, weights):
     """The frozen backbone k-NN evaluates, with the architecture of the run's `student.*` config (the depth is the
     number of blocks in the weights).  `weights`: a DinoVisionTransformer (returned as is); a `save_checkpoint`
@@ -332,6 +339,39 @@ def do_linear_eval(config, model, header):
     return results
 
 
+def do_seg_eval(config, model, header):
+    """Linear segmentation probe of the teacher backbone of `model` (see `eval_backbone`) on the
+    `evaluation.segmentation` datasets; rank 0 writes <output_dir>/eval/<header>/results_segmentation.json and returns
+    {"mIoU", "mAcc", "aAcc", "per_class_iou"} in percent ({} on other ranks).  Without configured datasets it logs one
+    line and returns {}."""
+    import json
+    from .. import distributed
+    seg = _seg_cfg(config)
+    if not seg:
+        if distributed.is_main_process():
+            print(f"do_seg_eval({header}): no evaluation.segmentation train / val dataset configured, nothing evaluated",
+                  flush=True)
+        return {}
+    backbone = eval_backbone(config, model)            # collective for a live engine under FSDP
+    if not distributed.is_main_process():
+        return {}
+    from ..eval import eval_segmentation, make_seg_dataset
+    c = config.crops
+    kw = {k: seg[k] for k in ("num_classes", "n_last_blocks", "batch_size", "crop_size", "iterations", "lr",
+                              "weight_decay", "warmup_iterations", "num_workers", "seed") if k in seg}
+    results = eval_segmentation(backbone, make_seg_dataset(seg["train_dataset_path"], "train"),
+                                make_seg_dataset(seg["val_dataset_path"], "val"),
+                                rgb_mean=c.get("rgb_mean", (0.485, 0.456, 0.406)),
+                                rgb_std=c.get("rgb_std", (0.229, 0.224, 0.225)), **kw)
+    out_dir = os.path.join(getattr(config.train, "output_dir", None) or ".", "eval", header)
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "results_segmentation.json"), "w") as f:
+        json.dump(results, f, indent=1)
+    print(f"do_seg_eval({header}): mIoU {results['mIoU']:.2f} mAcc {results['mAcc']:.2f} aAcc {results['aAcc']:.2f}",
+          flush=True)
+    return results
+
+
 def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None, max_iters: int = 0,
              print_freq: int = 10):
     """train/train.py:319-713.  `data_loader` (optional) yields the reference's collate dicts; by default it is built
@@ -374,8 +414,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
             next(it_loader)
     meters, nan_streak, t0 = {}, 0, time.time()
     ev = config.get("evaluation", None) or {}
-    knn_on, linear_on = bool(_knn_cfg(config)), bool(_linear_cfg(config))
-    eval_period = int(ev.get("eval_period_iterations", 0) or 0) if knn_on or linear_on else 0
+    knn_on, linear_on, seg_on = bool(_knn_cfg(config)), bool(_linear_cfg(config)), bool(_seg_cfg(config))
+    eval_period = int(ev.get("eval_period_iterations", 0) or 0) if knn_on or linear_on or seg_on else 0
     for it in range(start_iter, n_iters):
         try:
             data = next(it_loader)
@@ -396,6 +436,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
                 do_test(config, engine, f"training_{it}")
             if linear_on:
                 do_linear_eval(config, engine, f"training_{it}")
+            if seg_on:
+                do_seg_eval(config, engine, f"training_{it}")
         if it % print_freq == 0 or it == n_iters - 1:
             m = engine.read_metrics()                  # the only device->host sync of the loop
             if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
@@ -423,9 +465,9 @@ def main(argv=None):
     import random
     import numpy as np
     random.seed(args.seed); np.random.seed(args.seed); torch.manual_seed(args.seed)   # setup_job(seed=args.seed), :281
-    if args.eval not in ("", "knn", "linear"):
-        raise NotImplementedError(f"--eval {args.eval!r}: the evaluations are k-NN (--eval knn, or empty) and the linear "
-                                  "probe (--eval linear)")
+    if args.eval not in ("", "knn", "linear", "seg"):
+        raise NotImplementedError(f"--eval {args.eval!r}: the evaluations are k-NN (--eval knn, or empty), the linear "
+                                  "probe (--eval linear) and the linear segmentation probe (--eval seg)")
     if args.eval_only:                                 # train/train.py:304-311
         import json
         from ..checkpointer import find_latest_checkpoint
@@ -441,6 +483,8 @@ def main(argv=None):
             it = int(stored) + 1 if str(stored).lstrip("-").isdigit() else 0
         if args.eval == "linear":
             return do_linear_eval(config, str(weights), f"manual_{it}")
+        if args.eval == "seg":
+            return do_seg_eval(config, str(weights), f"manual_{it}")
         return do_test(config, str(weights), f"manual_{it}")
     model = SSLMetaArch(config)
     return do_train(config, model, resume=not args.no_resume, max_iters=args.max_iters, print_freq=args.print_freq)

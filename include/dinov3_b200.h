@@ -386,6 +386,37 @@ int d3_linear_xent_fwd_bwd(const float* logits, int ld, const int* labels, int B
 int d3_sgd_momentum(float* p, const float* g, float* m, void* p_bf16, long long rows, int cols, const float* lr, int Cp,
                     float lr_scale, float momentum, int first, void* stream);
 
+/* ---- linear segmentation probe (BatchNorm without affine + a 1x1 convolution on frozen patch features) ---------------
+ * Every entry point is deterministic (integer atomics only).  The head's logits are d3_gemm_bf16 (fp32 out, bias
+ * epilogue), its weight gradient d3_gemm_bf16 of dZ^T and the normalised rows, its bias gradient d3_colsum_bf16 of dZ,
+ * its update d3_adamw_ema.  Upsampling is torch's bilinear F.interpolate(align_corners=False) at any ratio.
+ * d3_seg_crop: n packed uint8 images (desc as d3_eval_resize_crop) with uint8 label maps of the same sizes (packed at
+ *   desc offset / 3 of labels_u8); boxes int32 [n, 6] (device) = (rh, rw, top, left, flip, unused): the image is resized
+ *   to rh x rw with d3_eval_resize_crop's arithmetic, and the out_h x out_w window at (top, left) is written (mirrored
+ *   within the part inside the resized image when flip != 0; outside it: 0 in the normalised image, 255 in the labels,
+ *   at the bottom / right).  out: bf16 NHWC (u8 / 255 - mean) / std, or (out_u8) uint8; label_out (optional) uint8
+ *   [n, out_h, out_w], torch 'nearest' from the label map.  max_taps as d3_eval_resize_crop for in / out = H / rh, W / rw.
+ * d3_seg_bn_stats: per column of bf16 x [M, N] (row stride ld): mean and biased var (fp32 [N]), as torch's BatchNorm in
+ *   training mode; run_mean / run_var (both or neither) <- (1 - momentum) run + momentum (mean, unbiased var).
+ * d3_seg_bn_apply: out[r, c] = bf16((x[r, c] - mean[c]) * rsqrt(var[c] + eps)).  N, ld, ld_out even.
+ * d3_seg_xent_fwd_bwd: logits fp32 [B * h * w, ld] (patch cells row-major, C <= ld classes), labels uint8 [B, Hl, Wl]
+ *   (>= C: ignored; 255 is the ignore label).  loss fp32 [1] = mean over the valid pixels of the cross-entropy of the
+ *   upsampled logits (0 when none is valid); count int32 [1] = the valid pixels; dz (fp32 and / or bf16 [B * h * w,
+ *   ld_dz], optional) = d loss / d logits in columns [0, C), 0 in [C, Cp).  2 <= C <= 256.  No full-resolution buffer.
+ * d3_seg_predict_confusion: conf int64 [C, C] += the (label, argmax of the upsampled logits) counts over the pixels with
+ *   label < C (argmax ties to the lower class).                                                                       */
+int d3_seg_crop(const void* src_u8, const long long* desc, const void* labels_u8, const int* boxes, int n, int out_h,
+                int out_w, int max_taps, const float* mean3 /*host*/, const float* std3 /*host*/, void* out, int out_u8,
+                void* label_out, void* stream);
+int d3_seg_bn_stats(const void* x_bf16, int ld, int M, int N, float* mean, float* var, float* run_mean, float* run_var,
+                    float momentum, void* stream);
+int d3_seg_bn_apply(const void* x_bf16, int ld, long long M, int N, const float* mean, const float* var, float eps,
+                    void* out_bf16, int ld_out, void* stream);
+int d3_seg_xent_fwd_bwd(const float* logits, int ld, const void* labels_u8, int B, int h, int w, int Hl, int Wl, int C,
+                        int Cp, float* loss, int* count, float* dz_f32, void* dz_bf16, int ld_dz, void* stream);
+int d3_seg_predict_confusion(const float* logits, int ld, const void* labels_u8, int B, int h, int w, int Hl, int Wl,
+                             int C, long long* conf, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
