@@ -16,6 +16,7 @@
 // confusion matrix are integer atomics, whose sums do not depend on order.
 #include "ptx.cuh"
 #include "d3_internal.h"
+#include "bilinear.cuh"
 
 #include <math.h>
 #include <stdio.h>
@@ -85,49 +86,9 @@ __global__ void seg_bn_apply_kernel(const __nv_bfloat16* __restrict__ x, int ld,
 }
 
 // --------------------------------------------------------------------------------------------- upsampling geometry
-struct SegGeom {
-  int B, h, w, Hl, Wl;
-  float sh, sw;       // h / Hl, w / Wl (torch's area_pixel_compute_scale in fp32)
-};
-
-__device__ __forceinline__ float seg_src(int d, float scale) { return fmaxf(__fmul_rn(d + 0.5f, scale) - 0.5f, 0.f); }
-
-// first output index in [0, n) whose source cell floor(seg_src) is >= t (n if none); seg_src is non-decreasing
-__device__ __forceinline__ int seg_first(int t, int n, float scale) {
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if ((int)seg_src(mid, scale) >= t) hi = mid; else lo = mid + 1;
-  }
-  return lo;
-}
-
 constexpr int SX_WARPS = 4;
 constexpr int SX_THREADS = SX_WARPS * 32;
 constexpr int SX_MAX_R = 8;                 // classes per lane: C <= 256
-
-// The tile's pixel rectangle [y_lo, y_hi) x [x_lo, x_hi), its four corner rows of the logits and the corner weights of
-// one of its pixels.
-struct SegTile {
-  int b, ty, tx, y1, x1, y_lo, y_hi, x_lo, x_hi;
-};
-
-__device__ __forceinline__ SegTile seg_tile(const SegGeom& g, int* range) {
-  SegTile t;
-  const int tile = blockIdx.x;
-  t.tx = tile % g.w;
-  t.ty = (tile / g.w) % g.h;
-  t.b = tile / (g.w * g.h);
-  t.y1 = min(t.ty + 1, g.h - 1);
-  t.x1 = min(t.tx + 1, g.w - 1);
-  if (threadIdx.x < 4) {
-    const int k = threadIdx.x;
-    range[k] = k < 2 ? seg_first(t.ty + k, g.Hl, g.sh) : seg_first(t.tx + k - 2, g.Wl, g.sw);
-  }
-  __syncthreads();
-  t.y_lo = range[0]; t.y_hi = range[1]; t.x_lo = range[2]; t.x_hi = range[3];
-  return t;
-}
 
 // the four corner logit rows (00, 01, 10, 11) of the lane's classes c = lane + 32 r
 template <int R>

@@ -100,6 +100,9 @@ SIGNATURES = {
     "d3_seg_bn_apply": [P, I, LL, I, P, P, F, P, I, P],
     "d3_seg_xent_fwd_bwd": [P, I, P, I, I, I, I, I, I, I, P, P, P, P, I, P],
     "d3_seg_predict_confusion": [P, I, P, I, I, I, I, I, I, P, P],
+    "d3_depth_crop": [P, P, P, P, I, I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, I, P, P],
+    "d3_depth_head_fwd_bwd": [P, I, P, I, I, I, I, I, I, I, F, F, P, P, P, P, I, P],
+    "d3_depth_predict_metrics": [P, I, P, I, I, I, I, I, I, F, F, I, I, I, I, P, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

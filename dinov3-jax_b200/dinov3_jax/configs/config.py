@@ -49,10 +49,10 @@ DEFAULTS = {
               "layerwise_decay": 0.9, "multi_tensor_optim": True, "adamw_beta1": 0.9, "adamw_beta2": 0.999},
     "checkpointing": {"period": 3750, "max_to_keep": 3},
     "distillation": {"enabled": False, "full_cfg_path": "", "checkpoint_path": ""},   # ssl_default_config.yaml:130-133
-    # k-NN (train.do_test), linear-probe (train.do_linear_eval) and linear segmentation (train.do_seg_eval) evaluations
-    # of the teacher backbone; empty dataset paths: nothing is evaluated.  `config_files` (the reference's list of
-    # evaluation configs) is accepted and not read.  The segmentation schedule is this project's default, not a
-    # published recipe's.
+    # k-NN (train.do_test), linear-probe (train.do_linear_eval), linear segmentation (train.do_seg_eval) and linear depth
+    # (train.do_depth_eval) evaluations of the teacher backbone; empty dataset paths: nothing is evaluated.
+    # `config_files` (the reference's list of evaluation configs) is accepted and not read.  The segmentation and depth
+    # schedules are this project's defaults, not a published recipe's.
     "evaluation": {"eval_period_iterations": 12500, "config_files": [],
                    "knn": {"train_dataset_path": "", "val_dataset_path": "", "nb_knn": [10, 20, 100, 200],
                            "temperature": 0.07, "batch_size": 256, "resize_size": 256, "crop_size": 224,
@@ -66,7 +66,12 @@ DEFAULTS = {
                    "segmentation": {"train_dataset_path": "", "val_dataset_path": "", "num_classes": 150,
                                     "n_last_blocks": 1, "batch_size": 16, "crop_size": 512, "iterations": 40000,
                                     "lr": 1e-3, "weight_decay": 1e-3, "warmup_iterations": 1500, "num_workers": 8,
-                                    "seed": 0}},
+                                    "seed": 0},
+                   "depth": {"train_dataset_path": "", "val_dataset_path": "", "n_last_blocks": 1, "use_cls_token": True,
+                             "n_bins": 256, "min_depth": 0.001, "max_depth": 10.0, "batch_size": 16,
+                             "crop_size": [416, 544], "iterations": 38400, "lr": 1e-3, "weight_decay": 1e-3,
+                             "warmup_iterations": 1500, "eval_crop": "eigen", "depth_scale": 1000, "num_workers": 8,
+                             "seed": 0}},
 }
 
 

@@ -1,12 +1,14 @@
 """Evaluation of a frozen backbone: k-NN classification on the normalised class token (`knn`), the linear probe on
-class tokens and the patch mean (`linear`), the linear segmentation probe on the patch tokens (`segmentation`), over
-image datasets read on the host (`datasets`)."""
-from .datasets import (ADE20KSegmentation, ImageFolder, NpzDataset, SegNpzDataset, make_eval_dataset,
-                       make_seg_dataset)
+class tokens and the patch mean (`linear`), the linear segmentation probe on the patch tokens (`segmentation`), the
+linear depth probe on the patch and class tokens (`depth`), over image datasets read on the host (`datasets`)."""
+from .datasets import (ADE20KSegmentation, DepthListDataset, DepthNpzDataset, ImageFolder, NpzDataset, SegNpzDataset,
+                       make_depth_dataset, make_eval_dataset, make_seg_dataset)
+from .depth import DepthLinearHead, depth_metrics, eval_depth, sample_depth_boxes
 from .knn import KnnClassifier, eval_knn, extract_features
 from .linear import LinearClassifiers, eval_linear
 from .segmentation import SegLinearHead, eval_segmentation
 
 __all__ = ["ImageFolder", "NpzDataset", "make_eval_dataset", "KnnClassifier", "eval_knn", "extract_features",
            "LinearClassifiers", "eval_linear", "ADE20KSegmentation", "SegNpzDataset", "make_seg_dataset",
-           "SegLinearHead", "eval_segmentation"]
+           "SegLinearHead", "eval_segmentation", "DepthNpzDataset", "DepthListDataset", "make_depth_dataset",
+           "DepthLinearHead", "sample_depth_boxes", "depth_metrics", "eval_depth"]

@@ -1,6 +1,7 @@
-"""Labelled image datasets for evaluation.  Each item is (uint8 HWC RGB numpy array, int label), or for segmentation
-(uint8 HWC RGB, uint8 HW label map); images keep their own sizes, the transforms run on the GPU (`ops.eval_resize_crop`,
-`ops.seg_crop`).  Decoding is host plumbing in DataLoader workers."""
+"""Labelled image datasets for evaluation.  Each item is (uint8 HWC RGB numpy array, int label), for segmentation
+(uint8 HWC RGB, uint8 HW label map), or for depth (uint8 HWC RGB, fp32 HW depth in metres); images keep their own
+sizes, the transforms run on the GPU (`ops.eval_resize_crop`, `ops.seg_crop`, `ops.depth_crop`).  Decoding is host
+plumbing in DataLoader workers."""
 from __future__ import annotations
 
 import os
@@ -119,6 +120,76 @@ def make_seg_dataset(path, split: str = "train"):
     """An .npz file -> SegNpzDataset, a directory -> ADE20KSegmentation(path, split)."""
     path = str(path)
     return SegNpzDataset(path) if path.endswith(".npz") else ADE20KSegmentation(path, split)
+
+
+class DepthNpzDataset:
+    """An .npz file with `images` (uint8 [N, H, W, 3]) and `depths` (float32 [N, H, W], metres; values outside
+    (min_depth, max_depth] are not scored)."""
+
+    def __init__(self, path):
+        with np.load(path, allow_pickle=False) as z:
+            self.images = np.asarray(z["images"])
+            self.depths = np.asarray(z["depths"])
+        if self.images.dtype != np.uint8 or self.images.ndim != 4 or self.images.shape[-1] != 3:
+            raise ValueError(f"{path}: images must be uint8 [N, H, W, 3], got {self.images.dtype} {self.images.shape}")
+        if self.depths.dtype != np.float32 or self.depths.shape != self.images.shape[:3]:
+            raise ValueError(f"{path}: depths must be float32 {list(self.images.shape[:3])}, got {self.depths.dtype} "
+                             f"{list(self.depths.shape)}")
+
+    def __len__(self):
+        return len(self.images)
+
+    def __getitem__(self, i):
+        return self.images[i], self.depths[i]
+
+
+class DepthListDataset:
+    """root/<split>.txt lists one `rgb_path depth_path` pair per line, relative to root (the NYU Depth v2 layout);
+    pairs are sorted by rgb path.  The depth is a 16-bit PNG holding metres * depth_scale (default 1000: millimetres);
+    0 means no measurement."""
+
+    def __init__(self, root, split: str = "train", depth_scale: float = 1000.0):
+        if split not in ("train", "val"):
+            raise ValueError(f"split must be 'train' or 'val', got {split!r}")
+        if not float(depth_scale) > 0:
+            raise ValueError(f"depth_scale must be positive, got {depth_scale}")
+        self.root, self.split, self.depth_scale = str(root), split, float(depth_scale)
+        pairs = []
+        with open(os.path.join(self.root, f"{split}.txt")) as f:
+            for n, line in enumerate(f, 1):
+                if not line.strip():
+                    continue
+                parts = line.split()
+                if len(parts) != 2:
+                    raise ValueError(f"{split}.txt line {n}: expected 'rgb_path depth_path', got {line.strip()!r}")
+                pairs.append(tuple(os.path.join(self.root, p) for p in parts))
+        pairs.sort()
+        for paths in pairs:
+            for q in paths:
+                if not os.path.isfile(q):
+                    raise FileNotFoundError(f"{split}.txt names {q}, which does not exist")
+        self.images, self.depth_files = [a for a, _ in pairs], [b for _, b in pairs]
+
+    def __len__(self):
+        return len(self.images)
+
+    def __getitem__(self, i):
+        from PIL import Image
+        with Image.open(self.images[i]) as im:
+            img = np.asarray(im.convert("RGB"), dtype=np.uint8)
+        with Image.open(self.depth_files[i]) as dp:
+            raw = np.asarray(dp)
+        if raw.dtype not in (np.uint16, np.int32) or raw.ndim != 2:
+            raise ValueError(f"{self.depth_files[i]}: expected a 16-bit single-channel PNG, got {raw.dtype} {raw.shape}")
+        if raw.shape != img.shape[:2]:
+            raise ValueError(f"{self.depth_files[i]}: depth {raw.shape} does not match image {img.shape[:2]}")
+        return img, (raw.astype(np.float64) / self.depth_scale).astype(np.float32)
+
+
+def make_depth_dataset(path, split: str = "train", depth_scale: float = 1000.0):
+    """An .npz file -> DepthNpzDataset, a directory -> DepthListDataset(path, split, depth_scale)."""
+    path = str(path)
+    return DepthNpzDataset(path) if path.endswith(".npz") else DepthListDataset(path, split, depth_scale)
 
 
 def make_eval_dataset(path):

@@ -686,3 +686,64 @@ def seg_predict_confusion(logits: torch.Tensor, labels: torch.Tensor, hw, num_cl
     N.check(N.init().d3_seg_predict_confusion(_p(logits), _ld(logits), _p(labels), B, h, w, Hl, Wl, C_, _p(conf), _s()),
             "d3_seg_predict_confusion")
     return conf
+
+
+# ------------------------------------------------------------------------------------------ depth probe
+def depth_crop(src: torch.Tensor, desc: torch.Tensor, boxes: torch.Tensor, out: torch.Tensor, *, max_taps: int,
+               depths: torch.Tensor | None = None, depth_out: torch.Tensor | None = None, mean=None, std=None):
+    """seg_crop's image (the same bits) and, optionally, the fp32 depth planes cropped from the same boxes by torch's
+    'nearest', 0 outside the resized image (d3_depth_crop).  depths: fp32 (flat, image n's plane at element
+    desc[n, 0] / 3) and depth_out fp32 [n, out_h, out_w], or both None; the rest as seg_crop."""
+    n, Ho, Wo = out.shape[0], out.shape[1], out.shape[2]
+    assert src.dtype == torch.uint8 and src.is_contiguous() and desc.dtype == torch.int64 and desc.is_contiguous()
+    assert boxes.dtype == torch.int32 and boxes.is_contiguous() and boxes.shape == (n, 6) and desc.shape == (n, 3)
+    assert out.shape == (n, Ho, Wo, 3) and out.is_contiguous() and out.dtype in (bf16, torch.uint8)
+    assert (depths is None) == (depth_out is None)
+    if depth_out is not None:
+        assert depths.dtype == f32 and depths.is_contiguous()
+        assert depth_out.dtype == f32 and depth_out.is_contiguous() and depth_out.shape == (n, Ho, Wo)
+    u8 = out.dtype == torch.uint8
+    m = (C.c_float * 3)(*([0.0] * 3 if u8 else [float(v) for v in mean]))
+    s = (C.c_float * 3)(*([1.0] * 3 if u8 else [float(v) for v in std]))
+    N.check(N.init().d3_depth_crop(_p(src), _p(desc), _p(depths), _p(boxes), n, Ho, Wo, int(max_taps), m, s, _p(out),
+                                   int(u8), _p(depth_out), _s()), "d3_depth_crop")
+    return out
+
+
+def depth_head_fwd_bwd(logits: torch.Tensor, gt: torch.Tensor, hw, n_bins: int, min_depth: float, max_depth: float,
+                       loss: torch.Tensor, count: torch.Tensor, dz_f32: torch.Tensor | None = None,
+                       dz_bf16: torch.Tensor | None = None, Cp: int | None = None):
+    """The scale-invariant log loss of the "linear" bin head's depth, upsampled bilinearly (align_corners=False) to the
+    ground truth, over its valid pixels (min_depth < gt <= max_depth), and its gradient to the bin logits
+    (d3_depth_head_fwd_bwd).  logits fp32 [B * h * w, >= n_bins] (ld any), gt fp32 [B, Hl, Wl], hw = (h, w); loss fp32
+    [1], count int32 [1]; dz_f32 / dz_bf16 [>= B * h * w, >= Cp] (columns [n_bins, Cp) zeroed)."""
+    B, Hl, Wl = gt.shape
+    h, w = int(hw[0]), int(hw[1])
+    Cp = int(n_bins) if Cp is None else int(Cp)
+    assert logits.dtype == f32 and logits.shape[0] >= B * h * w and gt.dtype == f32 and gt.is_contiguous()
+    assert loss.dtype == f32 and count.dtype == torch.int32
+    ld = None
+    for t, dt in ((dz_f32, f32), (dz_bf16, bf16)):
+        if t is not None:
+            assert t.dtype == dt and t.shape[0] >= B * h * w and t.shape[1] >= Cp
+            assert ld is None or ld == _ld(t), "dz_f32 and dz_bf16 share one row stride"
+            ld = _ld(t)
+    N.check(N.init().d3_depth_head_fwd_bwd(_p(logits), _ld(logits), _p(gt), B, h, w, Hl, Wl, int(n_bins), Cp,
+                                           float(min_depth), float(max_depth), _p(loss), _p(count), _p(dz_f32),
+                                           _p(dz_bf16), ld or Cp, _s()), "d3_depth_head_fwd_bwd")
+
+
+def depth_predict_metrics(logits: torch.Tensor, gt: torch.Tensor, hw, n_bins: int, min_depth: float, max_depth: float,
+                          sums: torch.Tensor, crop=None):
+    """sums fp64 [B, 9] = per image, over the valid pixels inside crop = (top, bottom, left, right) (None: all): the
+    count and the sums of abs_rel, sq_rel, squared error, squared log error, |log10 error| and the a1, a2, a3 hits of
+    the upsampled depth clamped to [min_depth, max_depth] (d3_depth_predict_metrics); shapes as depth_head_fwd_bwd."""
+    B, Hl, Wl = gt.shape
+    h, w = int(hw[0]), int(hw[1])
+    assert logits.dtype == f32 and logits.shape[0] >= B * h * w and gt.dtype == f32 and gt.is_contiguous()
+    assert sums.dtype == torch.float64 and sums.is_contiguous() and sums.shape == (B, 9)
+    top, bottom, left, right = (0, Hl, 0, Wl) if crop is None else (int(v) for v in crop)
+    N.check(N.init().d3_depth_predict_metrics(_p(logits), _ld(logits), _p(gt), B, h, w, Hl, Wl, int(n_bins),
+                                              float(min_depth), float(max_depth), top, bottom, left, right, _p(sums),
+                                              _s()), "d3_depth_predict_metrics")
+    return sums

@@ -245,6 +245,13 @@ def _seg_cfg(config) -> dict:
     return seg if seg.get("train_dataset_path") and seg.get("val_dataset_path") else {}
 
 
+def _depth_cfg(config) -> dict:
+    """The `evaluation.depth` block, or {} when it names no train / val dataset (then nothing is evaluated)."""
+    ev = config.get("evaluation", None) or {}
+    depth = dict(ev.get("depth", None) or {})
+    return depth if depth.get("train_dataset_path") and depth.get("val_dataset_path") else {}
+
+
 def eval_backbone(config, weights):
     """The frozen backbone k-NN evaluates, with the architecture of the run's `student.*` config (the depth is the
     number of blocks in the weights).  `weights`: a DinoVisionTransformer (returned as is); a `save_checkpoint`
@@ -372,6 +379,42 @@ def do_seg_eval(config, model, header):
     return results
 
 
+def do_depth_eval(config, model, header):
+    """Linear depth probe of the teacher backbone of `model` (see `eval_backbone`) on the `evaluation.depth` datasets;
+    rank 0 writes <output_dir>/eval/<header>/results_depth.json and returns {"abs_rel", "sq_rel", "rmse", "rmse_log",
+    "log10", "a1", "a2", "a3", "config"} ({} on other ranks), "config" echoing the evaluation.depth block.  Without
+    configured datasets it logs one line and returns {}."""
+    import json
+    from .. import distributed
+    depth = _depth_cfg(config)
+    if not depth:
+        if distributed.is_main_process():
+            print(f"do_depth_eval({header}): no evaluation.depth train / val dataset configured, nothing evaluated",
+                  flush=True)
+        return {}
+    backbone = eval_backbone(config, model)            # collective for a live engine under FSDP
+    if not distributed.is_main_process():
+        return {}
+    from ..eval import eval_depth, make_depth_dataset
+    c = config.crops
+    kw = {k: depth[k] for k in ("n_last_blocks", "use_cls_token", "n_bins", "min_depth", "max_depth", "batch_size",
+                                "crop_size", "iterations", "lr", "weight_decay", "warmup_iterations", "eval_crop",
+                                "num_workers", "seed") if k in depth}
+    scale = depth.get("depth_scale", 1000)
+    results = eval_depth(backbone, make_depth_dataset(depth["train_dataset_path"], "train", scale),
+                         make_depth_dataset(depth["val_dataset_path"], "val", scale),
+                         rgb_mean=c.get("rgb_mean", (0.485, 0.456, 0.406)),
+                         rgb_std=c.get("rgb_std", (0.229, 0.224, 0.225)), **kw)
+    results["config"] = {k: (list(v) if isinstance(v, (list, tuple)) else v) for k, v in depth.items()}
+    out_dir = os.path.join(getattr(config.train, "output_dir", None) or ".", "eval", header)
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "results_depth.json"), "w") as f:
+        json.dump(results, f, indent=1)
+    print(f"do_depth_eval({header}): abs_rel {results['abs_rel']:.4f} rmse {results['rmse']:.4f} "
+          f"a1 {results['a1']:.4f}", flush=True)
+    return results
+
+
 def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None, max_iters: int = 0,
              print_freq: int = 10):
     """train/train.py:319-713.  `data_loader` (optional) yields the reference's collate dicts; by default it is built
@@ -415,7 +458,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
     meters, nan_streak, t0 = {}, 0, time.time()
     ev = config.get("evaluation", None) or {}
     knn_on, linear_on, seg_on = bool(_knn_cfg(config)), bool(_linear_cfg(config)), bool(_seg_cfg(config))
-    eval_period = int(ev.get("eval_period_iterations", 0) or 0) if knn_on or linear_on or seg_on else 0
+    depth_on = bool(_depth_cfg(config))
+    eval_period = int(ev.get("eval_period_iterations", 0) or 0) if knn_on or linear_on or seg_on or depth_on else 0
     for it in range(start_iter, n_iters):
         try:
             data = next(it_loader)
@@ -438,6 +482,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
                 do_linear_eval(config, engine, f"training_{it}")
             if seg_on:
                 do_seg_eval(config, engine, f"training_{it}")
+            if depth_on:
+                do_depth_eval(config, engine, f"training_{it}")
         if it % print_freq == 0 or it == n_iters - 1:
             m = engine.read_metrics()                  # the only device->host sync of the loop
             if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
@@ -465,9 +511,10 @@ def main(argv=None):
     import random
     import numpy as np
     random.seed(args.seed); np.random.seed(args.seed); torch.manual_seed(args.seed)   # setup_job(seed=args.seed), :281
-    if args.eval not in ("", "knn", "linear", "seg"):
+    if args.eval not in ("", "knn", "linear", "seg", "depth"):
         raise NotImplementedError(f"--eval {args.eval!r}: the evaluations are k-NN (--eval knn, or empty), the linear "
-                                  "probe (--eval linear) and the linear segmentation probe (--eval seg)")
+                                  "probe (--eval linear), the linear segmentation probe (--eval seg) and the linear "
+                                  "depth probe (--eval depth)")
     if args.eval_only:                                 # train/train.py:304-311
         import json
         from ..checkpointer import find_latest_checkpoint
@@ -485,6 +532,8 @@ def main(argv=None):
             return do_linear_eval(config, str(weights), f"manual_{it}")
         if args.eval == "seg":
             return do_seg_eval(config, str(weights), f"manual_{it}")
+        if args.eval == "depth":
+            return do_depth_eval(config, str(weights), f"manual_{it}")
         return do_test(config, str(weights), f"manual_{it}")
     model = SSLMetaArch(config)
     return do_train(config, model, resume=not args.no_resume, max_iters=args.max_iters, print_freq=args.print_freq)

@@ -417,6 +417,32 @@ int d3_seg_xent_fwd_bwd(const float* logits, int ld, const void* labels_u8, int 
 int d3_seg_predict_confusion(const float* logits, int ld, const void* labels_u8, int B, int h, int w, int Hl, int Wl,
                              int C, long long* conf, void* stream);
 
+/* ---- linear depth probe (the segmentation probe's BatchNorm and 1x1 convolution to n_bins "linear" depth bins) -------
+ * Deterministic (no atomics).  Bin centres c_k = linspace(min_depth, max_depth, n_bins); per cell q_k = relu(z_k) + 0.1
+ * and depth d = sum_k q_k c_k / sum_k q_k; d is upsampled as d3_seg_xent_fwd_bwd's logits.  A ground-truth pixel is
+ * valid when min_depth < gt <= max_depth.
+ * d3_depth_crop: d3_seg_crop's image (the same bits) and, when depth_out != NULL, the fp32 depth planes of the same
+ *   sizes (packed at desc offset / 3 floats of depth_src) cropped from the same boxes by torch 'nearest' into
+ *   depth_out [n, out_h, out_w], 0 outside the resized image.
+ * d3_depth_head_fwd_bwd: logits fp32 [B * h * w, ld] (n_bins <= ld), gt fp32 [B, Hl, Wl].  loss fp32 [1] = the
+ *   scale-invariant log loss sqrt(var(g) + 0.15 mean(g)^2), g = log(d_hat + 1e-3) - log(gt + 1e-3) over the valid
+ *   pixels (unbiased var; 0 with fewer than 2); count int32 [1] = the valid pixels; dz (fp32 and / or bf16
+ *   [B * h * w, ld_dz], optional) = d loss / d logits in columns [0, n_bins), 0 in [n_bins, Cp).  No full-resolution
+ *   buffer.
+ * d3_depth_predict_metrics: sums fp64 [B, 9] = per image, over the valid pixels in rows [crop_top, crop_bottom) and
+ *   columns [crop_left, crop_right), with p = d_hat clamped to [min_depth, max_depth] and t = gt: the count, and the
+ *   sums of |p - t| / t, (p - t)^2 / t, (p - t)^2, (ln p - ln t)^2, |log10 p - log10 t|, and 1[max(p/t, t/p) < 1.25^k]
+ *   for k = 1, 2, 3 (fp32 within a tile, fp64 across tiles).                                                        */
+int d3_depth_crop(const void* src_u8, const long long* desc, const float* depth_src, const int* boxes, int n, int out_h,
+                  int out_w, int max_taps, const float* mean3 /*host*/, const float* std3 /*host*/, void* out,
+                  int out_u8, float* depth_out, void* stream);
+int d3_depth_head_fwd_bwd(const float* logits, int ld, const float* gt, int B, int h, int w, int Hl, int Wl,
+                          int n_bins, int Cp, float min_depth, float max_depth, float* loss, int* count, float* dz_f32,
+                          void* dz_bf16, int ld_dz, void* stream);
+int d3_depth_predict_metrics(const float* logits, int ld, const float* gt, int B, int h, int w, int Hl, int Wl,
+                             int n_bins, float min_depth, float max_depth, int crop_top, int crop_bottom,
+                             int crop_left, int crop_right, double* sums, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
