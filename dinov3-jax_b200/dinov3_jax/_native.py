@@ -103,6 +103,10 @@ SIGNATURES = {
     "d3_depth_crop": [P, P, P, P, I, I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, I, P, P],
     "d3_depth_head_fwd_bwd": [P, I, P, I, I, I, I, I, I, I, F, F, P, P, P, P, I, P],
     "d3_depth_predict_metrics": [P, I, P, I, I, I, I, I, I, F, F, I, I, I, I, P, P],
+    "d3_video_resize": [P, P, I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, P],
+    "d3_video_propagate": [P, I, P, I, P, P, I, I, I, I, I, I, F, P, P],
+    "d3_video_label_map": [P, I, I, I, I, I, I, P, P],
+    "d3_video_jf_counts": [P, P, I, I, I, I, I, P, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

@@ -49,8 +49,9 @@ DEFAULTS = {
               "layerwise_decay": 0.9, "multi_tensor_optim": True, "adamw_beta1": 0.9, "adamw_beta2": 0.999},
     "checkpointing": {"period": 3750, "max_to_keep": 3},
     "distillation": {"enabled": False, "full_cfg_path": "", "checkpoint_path": ""},   # ssl_default_config.yaml:130-133
-    # k-NN (train.do_test), linear-probe (train.do_linear_eval), linear segmentation (train.do_seg_eval) and linear depth
-    # (train.do_depth_eval) evaluations of the teacher backbone; empty dataset paths: nothing is evaluated.
+    # k-NN (train.do_test), linear-probe (train.do_linear_eval), linear segmentation (train.do_seg_eval), linear depth
+    # (train.do_depth_eval) and video segmentation (train.do_video_eval, DINO's label-propagation protocol) evaluations
+    # of the teacher backbone; empty dataset paths: nothing is evaluated.
     # `config_files` (the reference's list of evaluation configs) is accepted and not read.  The segmentation and depth
     # schedules are this project's defaults, not a published recipe's.
     "evaluation": {"eval_period_iterations": 12500, "config_files": [],
@@ -71,7 +72,10 @@ DEFAULTS = {
                              "n_bins": 256, "min_depth": 0.001, "max_depth": 10.0, "batch_size": 16,
                              "crop_size": [416, 544], "iterations": 38400, "lr": 1e-3, "weight_decay": 1e-3,
                              "warmup_iterations": 1500, "eval_crop": "eigen", "depth_scale": 1000, "num_workers": 8,
-                             "seed": 0}},
+                             "seed": 0},
+                   "video": {"dataset_path": "", "n_last_frames": 7, "size_mask_neighborhood": 12, "topk": 5,
+                             "temperature": 0.1, "short_side": 480, "batch_size": 16, "num_workers": 4,
+                             "save_masks": False}},
 }
 
 

@@ -1,14 +1,18 @@
 """Evaluation of a frozen backbone: k-NN classification on the normalised class token (`knn`), the linear probe on
 class tokens and the patch mean (`linear`), the linear segmentation probe on the patch tokens (`segmentation`), the
-linear depth probe on the patch and class tokens (`depth`), over image datasets read on the host (`datasets`)."""
-from .datasets import (ADE20KSegmentation, DepthListDataset, DepthNpzDataset, ImageFolder, NpzDataset, SegNpzDataset,
-                       make_depth_dataset, make_eval_dataset, make_seg_dataset)
+linear depth probe on the patch and class tokens (`depth`), video object segmentation by label propagation through the
+patch tokens (`video`), over image and video datasets read on the host (`datasets`)."""
+from .datasets import (ADE20KSegmentation, DavisDataset, DepthListDataset, DepthNpzDataset, ImageFolder, NpzDataset,
+                       SegNpzDataset, VideoNpzDataset, make_depth_dataset, make_eval_dataset, make_seg_dataset,
+                       make_video_dataset)
 from .depth import DepthLinearHead, depth_metrics, eval_depth, sample_depth_boxes
 from .knn import KnnClassifier, eval_knn, extract_features
 from .linear import LinearClassifiers, eval_linear
 from .segmentation import SegLinearHead, eval_segmentation
+from .video import eval_video_segmentation
 
 __all__ = ["ImageFolder", "NpzDataset", "make_eval_dataset", "KnnClassifier", "eval_knn", "extract_features",
            "LinearClassifiers", "eval_linear", "ADE20KSegmentation", "SegNpzDataset", "make_seg_dataset",
            "SegLinearHead", "eval_segmentation", "DepthNpzDataset", "DepthListDataset", "make_depth_dataset",
-           "DepthLinearHead", "sample_depth_boxes", "depth_metrics", "eval_depth"]
+           "DepthLinearHead", "sample_depth_boxes", "depth_metrics", "eval_depth", "DavisDataset", "VideoNpzDataset",
+           "make_video_dataset", "eval_video_segmentation"]

@@ -1,6 +1,7 @@
 """Labelled image datasets for evaluation.  Each item is (uint8 HWC RGB numpy array, int label), for segmentation
-(uint8 HWC RGB, uint8 HW label map), or for depth (uint8 HWC RGB, fp32 HW depth in metres); images keep their own
-sizes, the transforms run on the GPU (`ops.eval_resize_crop`, `ops.seg_crop`, `ops.depth_crop`).  Decoding is host
+(uint8 HWC RGB, uint8 HW label map), or for depth (uint8 HWC RGB, fp32 HW depth in metres); a video dataset yields
+whole sequences (`DavisDataset`).  Images keep their own sizes, the transforms run on the GPU (`ops.eval_resize_crop`,
+`ops.seg_crop`, `ops.depth_crop`, `ops.video_resize`).  Decoding is host
 plumbing in DataLoader workers."""
 from __future__ import annotations
 
@@ -190,6 +191,88 @@ def make_depth_dataset(path, split: str = "train", depth_scale: float = 1000.0):
     """An .npz file -> DepthNpzDataset, a directory -> DepthListDataset(path, split, depth_scale)."""
     path = str(path)
     return DepthNpzDataset(path) if path.endswith(".npz") else DepthListDataset(path, split, depth_scale)
+
+
+class DavisDataset:
+    """The DAVIS 2017 semi-supervised layout: root/ImageSets/2017/<split>.txt lists the sequences;
+    root/JPEGImages/480p/<seq>/*.jpg are the frames and root/Annotations/480p/<seq>/*.png the palette annotations, one
+    per frame, both sorted by name.  Item i is {"name", "frames" uint8 [N, H, W, 3], "masks" uint8 [N, H, W] (object ids,
+    255 void), "palette" (frame 0's, a list of 768 ints)}."""
+
+    def __init__(self, root, split: str = "val"):
+        self.root, self.split = str(root), split
+        lst = os.path.join(self.root, "ImageSets", "2017", f"{split}.txt")
+        if not os.path.isfile(lst):
+            raise FileNotFoundError(f"{lst} does not exist")
+        with open(lst) as f:
+            self.sequences = [line.strip() for line in f if line.strip()]
+        self.frames, self.annotations = [], []
+        for seq in self.sequences:
+            fd = os.path.join(self.root, "JPEGImages", "480p", seq)
+            ad = os.path.join(self.root, "Annotations", "480p", seq)
+            for d in (fd, ad):
+                if not os.path.isdir(d):
+                    raise FileNotFoundError(f"{split}.txt names sequence {seq}, but {d} does not exist")
+            frames = sorted(os.path.join(fd, e) for e in os.listdir(fd) if e.lower().endswith(".jpg"))
+            annots = sorted(os.path.join(ad, e) for e in os.listdir(ad) if e.lower().endswith(".png"))
+            if not frames or len(frames) != len(annots):
+                raise ValueError(f"{fd} holds {len(frames)} frames but {ad} holds {len(annots)} annotations")
+            self.frames.append(frames)
+            self.annotations.append(annots)
+
+    def __len__(self):
+        return len(self.sequences)
+
+    def __getitem__(self, i):
+        from PIL import Image
+        frames, masks, palette = [], [], None
+        for fp, ap in zip(self.frames[i], self.annotations[i]):
+            with Image.open(fp) as im:
+                frames.append(np.asarray(im.convert("RGB"), dtype=np.uint8))
+            with Image.open(ap) as an:
+                if an.mode != "P":
+                    raise ValueError(f"{ap}: expected a palette PNG, got mode {an.mode}")
+                if palette is None:
+                    palette = an.getpalette()
+                masks.append(np.asarray(an, dtype=np.uint8))
+            if masks[-1].shape != frames[-1].shape[:2] or frames[-1].shape != frames[0].shape:
+                raise ValueError(f"{ap}: annotation {masks[-1].shape} does not match frame {frames[-1].shape[:2]} "
+                                 f"(frame 0 {frames[0].shape[:2]})")
+        return {"name": self.sequences[i], "frames": np.stack(frames), "masks": np.stack(masks), "palette": palette}
+
+
+class VideoNpzDataset:
+    """An .npz file with `frames` (uint8 [N, H, W, 3]), `masks` (uint8 [N, H, W], object ids, 255 void) and
+    `sequence_starts` (int, the first frame of each sequence, ascending from 0).  Sequence i is named "%05d" % i and
+    has no palette."""
+
+    def __init__(self, path):
+        with np.load(path, allow_pickle=False) as z:
+            self.frames, self.masks = np.asarray(z["frames"]), np.asarray(z["masks"])
+            starts = np.asarray(z["sequence_starts"])
+        if self.frames.dtype != np.uint8 or self.frames.ndim != 4 or self.frames.shape[-1] != 3:
+            raise ValueError(f"{path}: frames must be uint8 [N, H, W, 3], got {self.frames.dtype} {self.frames.shape}")
+        if self.masks.dtype != np.uint8 or self.masks.shape != self.frames.shape[:3]:
+            raise ValueError(f"{path}: masks must be uint8 {list(self.frames.shape[:3])}, got {self.masks.dtype} "
+                             f"{list(self.masks.shape)}")
+        n = len(self.frames)
+        if (starts.ndim != 1 or not len(starts) or starts[0] != 0 or (np.diff(starts) <= 0).any()
+                or starts[-1] >= n):
+            raise ValueError(f"{path}: sequence_starts must ascend from 0 and stay below {n}, got {starts.tolist()}")
+        self.bounds = list(zip(starts.tolist(), starts[1:].tolist() + [n]))
+
+    def __len__(self):
+        return len(self.bounds)
+
+    def __getitem__(self, i):
+        a, b = self.bounds[i]
+        return {"name": f"{i:05d}", "frames": self.frames[a:b], "masks": self.masks[a:b], "palette": None}
+
+
+def make_video_dataset(path, split: str = "val"):
+    """An .npz file -> VideoNpzDataset, a directory -> DavisDataset(path, split)."""
+    path = str(path)
+    return VideoNpzDataset(path) if path.endswith(".npz") else DavisDataset(path, split)
 
 
 def make_eval_dataset(path):

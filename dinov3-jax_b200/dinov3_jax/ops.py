@@ -747,3 +747,64 @@ def depth_predict_metrics(logits: torch.Tensor, gt: torch.Tensor, hw, n_bins: in
                                               float(min_depth), float(max_depth), top, bottom, left, right, _p(sums),
                                               _s()), "d3_depth_predict_metrics")
     return sums
+
+
+# ------------------------------------------------------------------------------------------ video segmentation
+def video_resize(src: torch.Tensor, desc: torch.Tensor, out: torch.Tensor, *, mean, std) -> torch.Tensor:
+    """torch bilinear (align_corners=False, antialias=False) of n packed uint8 HWC frames / 255 to out bf16 [n, H, W, 3],
+    normalised with mean / std (d3_video_resize).  src uint8 (flat), desc int64 [n, 3] = (byte offset, H, W)."""
+    n, Ho, Wo = out.shape[0], out.shape[1], out.shape[2]
+    assert src.dtype == torch.uint8 and src.is_contiguous() and desc.dtype == torch.int64 and desc.is_contiguous()
+    assert desc.shape == (n, 3) and out.shape == (n, Ho, Wo, 3) and out.is_contiguous() and out.dtype == bf16
+    m = (C.c_float * 3)(*[float(v) for v in mean])
+    s = (C.c_float * 3)(*[float(v) for v in std])
+    N.check(N.init().d3_video_resize(_p(src), _p(desc), n, Ho, Wo, m, s, _p(out), _s()), "d3_video_resize")
+    return out
+
+
+def video_propagate(sim0: torch.Tensor, simr: torch.Tensor | None, lab0: torch.Tensor, labr: torch.Tensor | None,
+                    hw, radius: int, topk: int, temperature: float, out: torch.Tensor) -> torch.Tensor:
+    """out fp32 [h * w, C] = the soft labels of one target frame propagated from frame 0 (sim0 fp32 [h * w, >= h * w]
+    similarities, lab0 fp32 [h * w, C] labels) and the recent frames (simr fp32 [h * w, >= n * h * w], frame c at
+    columns [c h w, (c + 1) h w), labr fp32 [n * h * w, C]; both None when there are none) (d3_video_propagate)."""
+    h, w = int(hw[0]), int(hw[1])
+    P, Cc = h * w, lab0.shape[1]
+    assert sim0.dtype == f32 and sim0.shape[0] == P and sim0.shape[1] >= P
+    assert lab0.dtype == f32 and lab0.is_contiguous() and lab0.shape == (P, Cc)
+    assert out.dtype == f32 and out.is_contiguous() and out.shape == (P, Cc)
+    assert (simr is None) == (labr is None)
+    n = 0
+    if labr is not None:
+        assert labr.dtype == f32 and labr.is_contiguous() and labr.shape[1] == Cc and labr.shape[0] % P == 0
+        n = labr.shape[0] // P
+        assert simr.dtype == f32 and simr.shape[0] == P and simr.shape[1] >= n * P
+    N.check(N.init().d3_video_propagate(_p(sim0), _ld(sim0), _p(simr), _ld(simr) if simr is not None else 0, _p(lab0),
+                                        _p(labr), n, h, w, Cc, int(radius), int(topk), float(temperature), _p(out),
+                                        _s()), "d3_video_propagate")
+    return out
+
+
+def video_label_map(soft: torch.Tensor, hw, patch: int, out: torch.Tensor) -> torch.Tensor:
+    """out uint8 [H, W] = the argmax label map of the soft labels fp32 [h * w, C] upsampled by `patch` (bilinear),
+    min-max normalised per channel and sampled by nearest-exact at H x W (d3_video_label_map)."""
+    h, w = int(hw[0]), int(hw[1])
+    assert soft.dtype == f32 and soft.is_contiguous() and soft.dim() == 2 and soft.shape[0] == h * w
+    assert out.dtype == torch.uint8 and out.is_contiguous() and out.dim() == 2
+    N.check(N.init().d3_video_label_map(_p(soft), h, w, soft.shape[1], int(patch), out.shape[0], out.shape[1], _p(out),
+                                        _s()), "d3_video_label_map")
+    return out
+
+
+def video_jf_counts(pred: torch.Tensor, gt: torch.Tensor, num_objects: int, radius: int,
+                    counts: torch.Tensor) -> torch.Tensor:
+    """counts int64 [F, K, 6] = per frame and object 1..K: intersection, union (void = gt 255 excluded), pred and gt
+    boundary pixels, pred and gt boundary pixels matched within the disk of `radius` (d3_video_jf_counts).  pred, gt
+    uint8 [F, H, W]."""
+    F_, H, W = gt.shape
+    K = int(num_objects)
+    assert pred.dtype == torch.uint8 and gt.dtype == torch.uint8 and pred.shape == gt.shape
+    assert pred.is_contiguous() and gt.is_contiguous()
+    assert counts.dtype == torch.int64 and counts.is_contiguous() and counts.shape == (F_, K, 6)
+    N.check(N.init().d3_video_jf_counts(_p(pred), _p(gt), F_, H, W, K, int(radius), _p(counts), _s()),
+            "d3_video_jf_counts")
+    return counts

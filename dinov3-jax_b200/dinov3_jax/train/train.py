@@ -252,6 +252,13 @@ def _depth_cfg(config) -> dict:
     return depth if depth.get("train_dataset_path") and depth.get("val_dataset_path") else {}
 
 
+def _video_cfg(config) -> dict:
+    """The `evaluation.video` block, or {} when it names no dataset (then nothing is evaluated)."""
+    ev = config.get("evaluation", None) or {}
+    video = dict(ev.get("video", None) or {})
+    return video if video.get("dataset_path") else {}
+
+
 def eval_backbone(config, weights):
     """The frozen backbone k-NN evaluates, with the architecture of the run's `student.*` config (the depth is the
     number of blocks in the weights).  `weights`: a DinoVisionTransformer (returned as is); a `save_checkpoint`
@@ -415,6 +422,40 @@ def do_depth_eval(config, model, header):
     return results
 
 
+def do_video_eval(config, model, header):
+    """Video object segmentation by label propagation through the teacher backbone of `model` (see `eval_backbone`) on
+    the `evaluation.video` dataset; rank 0 writes <output_dir>/eval/<header>/results_video.json and returns {"J&F-Mean",
+    "J-Mean", "J-Recall", "J-Decay", "F-Mean", "F-Recall", "F-Decay", "sequences", "protocol", "config"} ({} on other
+    ranks), "config" echoing the evaluation.video block; with save_masks the predicted masks go to
+    <output_dir>/eval/<header>/Annotations/480p/<sequence>/.  Without a configured dataset it logs one line and
+    returns {}."""
+    import json
+    from .. import distributed
+    video = _video_cfg(config)
+    if not video:
+        if distributed.is_main_process():
+            print(f"do_video_eval({header}): no evaluation.video dataset configured, nothing evaluated", flush=True)
+        return {}
+    backbone = eval_backbone(config, model)            # collective for a live engine under FSDP
+    if not distributed.is_main_process():
+        return {}
+    from ..eval import eval_video_segmentation, make_video_dataset
+    c = config.crops
+    out_dir = os.path.join(getattr(config.train, "output_dir", None) or ".", "eval", header)
+    kw = {k: video[k] for k in ("n_last_frames", "size_mask_neighborhood", "topk", "temperature", "short_side",
+                                "batch_size", "num_workers", "save_masks") if k in video}
+    results = eval_video_segmentation(backbone, make_video_dataset(video["dataset_path"]), output_dir=out_dir,
+                                      rgb_mean=c.get("rgb_mean", (0.485, 0.456, 0.406)),
+                                      rgb_std=c.get("rgb_std", (0.229, 0.224, 0.225)), **kw)
+    results["config"] = {k: (list(v) if isinstance(v, (list, tuple)) else v) for k, v in video.items()}
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "results_video.json"), "w") as f:
+        json.dump(results, f, indent=1)
+    print(f"do_video_eval({header}): J&F-Mean {results['J&F-Mean']:.4f} J-Mean {results['J-Mean']:.4f} "
+          f"F-Mean {results['F-Mean']:.4f}", flush=True)
+    return results
+
+
 def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None, max_iters: int = 0,
              print_freq: int = 10):
     """train/train.py:319-713.  `data_loader` (optional) yields the reference's collate dicts; by default it is built
@@ -458,8 +499,9 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
     meters, nan_streak, t0 = {}, 0, time.time()
     ev = config.get("evaluation", None) or {}
     knn_on, linear_on, seg_on = bool(_knn_cfg(config)), bool(_linear_cfg(config)), bool(_seg_cfg(config))
-    depth_on = bool(_depth_cfg(config))
-    eval_period = int(ev.get("eval_period_iterations", 0) or 0) if knn_on or linear_on or seg_on or depth_on else 0
+    depth_on, video_on = bool(_depth_cfg(config)), bool(_video_cfg(config))
+    any_on = knn_on or linear_on or seg_on or depth_on or video_on
+    eval_period = int(ev.get("eval_period_iterations", 0) or 0) if any_on else 0
     for it in range(start_iter, n_iters):
         try:
             data = next(it_loader)
@@ -484,6 +526,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
                 do_seg_eval(config, engine, f"training_{it}")
             if depth_on:
                 do_depth_eval(config, engine, f"training_{it}")
+            if video_on:
+                do_video_eval(config, engine, f"training_{it}")
         if it % print_freq == 0 or it == n_iters - 1:
             m = engine.read_metrics()                  # the only device->host sync of the loop
             if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
@@ -511,10 +555,10 @@ def main(argv=None):
     import random
     import numpy as np
     random.seed(args.seed); np.random.seed(args.seed); torch.manual_seed(args.seed)   # setup_job(seed=args.seed), :281
-    if args.eval not in ("", "knn", "linear", "seg", "depth"):
+    if args.eval not in ("", "knn", "linear", "seg", "depth", "video"):
         raise NotImplementedError(f"--eval {args.eval!r}: the evaluations are k-NN (--eval knn, or empty), the linear "
-                                  "probe (--eval linear), the linear segmentation probe (--eval seg) and the linear "
-                                  "depth probe (--eval depth)")
+                                  "probe (--eval linear), the linear segmentation probe (--eval seg), the linear "
+                                  "depth probe (--eval depth) and video object segmentation (--eval video)")
     if args.eval_only:                                 # train/train.py:304-311
         import json
         from ..checkpointer import find_latest_checkpoint
@@ -534,6 +578,8 @@ def main(argv=None):
             return do_seg_eval(config, str(weights), f"manual_{it}")
         if args.eval == "depth":
             return do_depth_eval(config, str(weights), f"manual_{it}")
+        if args.eval == "video":
+            return do_video_eval(config, str(weights), f"manual_{it}")
         return do_test(config, str(weights), f"manual_{it}")
     model = SSLMetaArch(config)
     return do_train(config, model, resume=not args.no_resume, max_iters=args.max_iters, print_freq=args.print_freq)

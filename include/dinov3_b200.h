@@ -443,6 +443,31 @@ int d3_depth_predict_metrics(const float* logits, int ld, const float* gt, int B
                              int n_bins, float min_depth, float max_depth, int crop_top, int crop_bottom,
                              int crop_left, int crop_right, double* sums, void* stream);
 
+/* ---- video object segmentation by label propagation (DINO's eval_video_segmentation.py; see csrc/video.cu) -------
+ * d3_video_resize: n packed uint8 HWC frames (desc int64 [n, 3] = (byte offset, H, W)) -> bf16 NHWC [n, out_h, out_w, 3]:
+ *   torch bilinear (align_corners = False, antialias = False) of frame / 255 in fp32, then (v - mean) / std.
+ * d3_video_propagate: the soft labels out fp32 [h w, C] of one target frame.  sim0 fp32 [h w, ld0] = the target rows'
+ *   similarities to frame 0's rows; simr fp32 [h w, ldr] = those to the n_recent recent frames, frame c at columns
+ *   [c h w, (c + 1) h w); lab0 fp32 [h w, C] and labr fp32 [n_recent h w, C] their label rows.  Per target patch: the
+ *   candidates within radius rows and columns in every context frame (frame 0 first, then row, then column), the k-th
+ *   largest similarity as threshold (ties kept), weights exp((x - x_max) / temperature) normalised to sum 1, the
+ *   weighted sum of the kept label rows.  C <= 32, topk <= 32.  Deterministic (no atomics).
+ * d3_video_label_map: labels uint8 [out_h, out_w] = argmax over channels (lowest index on ties) of the soft map
+ *   fp32 [h, w, C] upsampled bilinearly by patch (align_corners = False), each channel with maximum > 0 min-max
+ *   normalised over the upsampled frame, sampled by torch nearest-exact at out_h x out_w.  No full-resolution buffer.
+ * d3_video_jf_counts: pred, gt uint8 [F, H, W] (gt 255 = void); counts int64 [F, K, 6] (zeroed here) per frame and
+ *   object k = 1..K: intersection and union outside void, the boundary pixels of pred and of gt (void cleared first),
+ *   and the boundary pixels of each with a boundary pixel of the other within the disk of radius `radius`.        */
+int d3_video_resize(const void* src_u8, const long long* desc, int n, int out_h, int out_w, const float* mean3 /*host*/,
+                    const float* std3 /*host*/, void* out, void* stream);
+int d3_video_propagate(const float* sim0, int ld0, const float* simr, int ldr, const float* lab0, const float* labr,
+                       int n_recent, int h, int w, int C, int radius, int topk, float temperature, float* out,
+                       void* stream);
+int d3_video_label_map(const float* soft, int h, int w, int C, int patch, int out_h, int out_w, void* labels_u8,
+                       void* stream);
+int d3_video_jf_counts(const void* pred_u8, const void* gt_u8, int F, int H, int W, int K, int radius,
+                       long long* counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
