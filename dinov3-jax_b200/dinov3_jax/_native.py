@@ -107,6 +107,9 @@ SIGNATURES = {
     "d3_video_propagate": [P, I, P, I, P, P, I, I, I, I, I, I, F, P, P],
     "d3_video_label_map": [P, I, I, I, I, I, I, P, P],
     "d3_video_jf_counts": [P, P, I, I, I, I, I, P, P],
+    "d3_corr_descriptors": [P, I, I, I, I, I, I, I, C.POINTER(C.c_int), I, P, I, P, P],
+    "d3_corr_gram": [P, I, I, I, I, I, P, P],
+    "d3_corr_argmax": [P, I, P, P, I, I, I, I, I, P, P, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

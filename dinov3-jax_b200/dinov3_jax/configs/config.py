@@ -50,8 +50,9 @@ DEFAULTS = {
     "checkpointing": {"period": 3750, "max_to_keep": 3},
     "distillation": {"enabled": False, "full_cfg_path": "", "checkpoint_path": ""},   # ssl_default_config.yaml:130-133
     # k-NN (train.do_test), linear-probe (train.do_linear_eval), linear segmentation (train.do_seg_eval), linear depth
-    # (train.do_depth_eval) and video segmentation (train.do_video_eval, DINO's label-propagation protocol) evaluations
-    # of the teacher backbone; empty dataset paths: nothing is evaluated.
+    # (train.do_depth_eval), video segmentation (train.do_video_eval, DINO's label-propagation protocol) and keypoint
+    # correspondence (train.do_correspondence_eval, SPair-71k PCK) evaluations of the teacher backbone; empty dataset
+    # paths: nothing is evaluated.
     # `config_files` (the reference's list of evaluation configs) is accepted and not read.  The segmentation and depth
     # schedules are this project's defaults, not a published recipe's.
     "evaluation": {"eval_period_iterations": 12500, "config_files": [],
@@ -75,7 +76,9 @@ DEFAULTS = {
                              "seed": 0},
                    "video": {"dataset_path": "", "n_last_frames": 7, "size_mask_neighborhood": 12, "topk": 5,
                              "temperature": 0.1, "short_side": 480, "batch_size": 16, "num_workers": 4,
-                             "save_masks": False}},
+                             "save_masks": False},
+                   "correspondence": {"dataset_path": "", "split": "test", "image_size": 512,
+                                      "alphas": [0.01, 0.05, 0.1], "batch_size": 16, "num_workers": 4}},
 }
 
 

@@ -1,9 +1,12 @@
 """Evaluation of a frozen backbone: k-NN classification on the normalised class token (`knn`), the linear probe on
 class tokens and the patch mean (`linear`), the linear segmentation probe on the patch tokens (`segmentation`), the
 linear depth probe on the patch and class tokens (`depth`), video object segmentation by label propagation through the
-patch tokens (`video`), over image and video datasets read on the host (`datasets`)."""
-from .datasets import (ADE20KSegmentation, DavisDataset, DepthListDataset, DepthNpzDataset, ImageFolder, NpzDataset,
-                       SegNpzDataset, VideoNpzDataset, make_depth_dataset, make_eval_dataset, make_seg_dataset,
+patch tokens (`video`), keypoint correspondence by nearest neighbour over the upsampled patch tokens
+(`correspondence`), over image, video and keypoint-pair datasets read on the host (`datasets`)."""
+from .correspondence import eval_correspondence
+from .datasets import (ADE20KSegmentation, CorrespondenceNpzDataset, DavisDataset, DepthListDataset, DepthNpzDataset,
+                       ImageFolder, NpzDataset, SegNpzDataset, SPairDataset, VideoNpzDataset,
+                       make_correspondence_dataset, make_depth_dataset, make_eval_dataset, make_seg_dataset,
                        make_video_dataset)
 from .depth import DepthLinearHead, depth_metrics, eval_depth, sample_depth_boxes
 from .knn import KnnClassifier, eval_knn, extract_features
@@ -15,4 +18,5 @@ __all__ = ["ImageFolder", "NpzDataset", "make_eval_dataset", "KnnClassifier", "e
            "LinearClassifiers", "eval_linear", "ADE20KSegmentation", "SegNpzDataset", "make_seg_dataset",
            "SegLinearHead", "eval_segmentation", "DepthNpzDataset", "DepthListDataset", "make_depth_dataset",
            "DepthLinearHead", "sample_depth_boxes", "depth_metrics", "eval_depth", "DavisDataset", "VideoNpzDataset",
-           "make_video_dataset", "eval_video_segmentation"]
+           "make_video_dataset", "eval_video_segmentation", "SPairDataset", "CorrespondenceNpzDataset",
+           "make_correspondence_dataset", "eval_correspondence"]

@@ -1,8 +1,8 @@
 """Labelled image datasets for evaluation.  Each item is (uint8 HWC RGB numpy array, int label), for segmentation
 (uint8 HWC RGB, uint8 HW label map), or for depth (uint8 HWC RGB, fp32 HW depth in metres); a video dataset yields
-whole sequences (`DavisDataset`).  Images keep their own sizes, the transforms run on the GPU (`ops.eval_resize_crop`,
-`ops.seg_crop`, `ops.depth_crop`, `ops.video_resize`).  Decoding is host
-plumbing in DataLoader workers."""
+whole sequences (`DavisDataset`), a correspondence dataset keypoint pairs over its images (`SPairDataset`).  Images
+keep their own sizes, the transforms run on the GPU (`ops.eval_resize_crop`, `ops.seg_crop`, `ops.depth_crop`,
+`ops.video_resize`).  Decoding is host plumbing in DataLoader workers."""
 from __future__ import annotations
 
 import os
@@ -273,6 +273,124 @@ def make_video_dataset(path, split: str = "val"):
     """An .npz file -> VideoNpzDataset, a directory -> DavisDataset(path, split)."""
     path = str(path)
     return VideoNpzDataset(path) if path.endswith(".npz") else DavisDataset(path, split)
+
+
+def _field(path, source, name):
+    if name not in source:
+        raise ValueError(f"{path}: field {name!r} is missing")
+    return source[name]
+
+
+class SPairDataset:
+    """The SPair-71k layout: every root/PairAnnotation/<split>/*.json, in sorted file-name order, is one pair, read for
+    src_imname, trg_imname, category, src_kps, trg_kps ([n, 2] x then y) and trg_bndbox (x1 y1 x2 y2); the images are
+    root/JPEGImages/<category>/<imname>.  `pairs[i]` is {"src", "trg" (image indices), "category", "src_kps",
+    "trg_kps" (float64 [n, 2]), "trg_bbox" (4 floats)}; `load_image(j)` decodes image j to uint8 HWC RGB.  Errors name
+    the file and the field."""
+
+    def __init__(self, root, split: str = "test"):
+        import json
+        self.root, self.split = str(root), split
+        d = os.path.join(self.root, "PairAnnotation", split)
+        if not os.path.isdir(d):
+            raise FileNotFoundError(f"{d} does not exist")
+        files = sorted(e for e in os.listdir(d) if e.endswith(".json"))
+        if not files:
+            raise FileNotFoundError(f"{d} holds no pair annotation (*.json)")
+        self.images, index, self.pairs = [], {}, []
+        for name in files:
+            path = os.path.join(d, name)
+            with open(path) as f:
+                a = json.load(f)
+            cat = str(_field(path, a, "category"))
+            ims = []
+            for key in ("src_imname", "trg_imname"):
+                im = os.path.join(self.root, "JPEGImages", cat, str(_field(path, a, key)))
+                if im not in index:
+                    if not os.path.isfile(im):
+                        raise FileNotFoundError(f"{path}: {key} names {im}, which does not exist")
+                    index[im] = len(self.images)
+                    self.images.append(im)
+                ims.append(index[im])
+            kps = []
+            for key in ("src_kps", "trg_kps"):
+                k = np.asarray(_field(path, a, key), dtype=np.float64)
+                if k.size == 0:
+                    k = k.reshape(0, 2)
+                if k.ndim != 2 or k.shape[1] != 2:
+                    raise ValueError(f"{path}: field {key!r} must be a list of [x, y], got shape {list(k.shape)}")
+                kps.append(k)
+            if len(kps[0]) != len(kps[1]):
+                raise ValueError(f"{path}: field 'trg_kps' has {len(kps[1])} points, 'src_kps' {len(kps[0])}")
+            box = np.asarray(_field(path, a, "trg_bndbox"), dtype=np.float64).reshape(-1)
+            if box.shape != (4,):
+                raise ValueError(f"{path}: field 'trg_bndbox' must be x1 y1 x2 y2, got {box.tolist()}")
+            self.pairs.append({"src": ims[0], "trg": ims[1], "category": cat, "src_kps": kps[0], "trg_kps": kps[1],
+                               "trg_bbox": box.tolist()})
+
+    def __len__(self):
+        return len(self.pairs)
+
+    def __getitem__(self, i):
+        return self.pairs[i]
+
+    def load_image(self, j):
+        from PIL import Image
+        with Image.open(self.images[j]) as im:
+            return np.asarray(im.convert("RGB"), dtype=np.uint8)
+
+
+class CorrespondenceNpzDataset:
+    """An .npz file with images (uint8 [N, H, W, 3]), pairs (int [M, 2]: source and target index), src_kps / trg_kps
+    (float [M, Kmax, 2], x then y, the first n_kps[m] rows of pair m used), n_kps (int [M]), trg_bbox (float [M, 4]:
+    x1 y1 x2 y2) and categories (str [M]); the same `pairs` and `load_image` as SPairDataset."""
+
+    def __init__(self, path):
+        path = str(path)
+        with np.load(path, allow_pickle=False) as z:
+            f = {k: np.asarray(_field(path, z, k)) for k in ("images", "pairs", "src_kps", "trg_kps", "n_kps",
+                                                              "trg_bbox", "categories")}
+        self.images = f["images"]
+        if self.images.dtype != np.uint8 or self.images.ndim != 4 or self.images.shape[-1] != 3:
+            raise ValueError(f"{path}: field 'images' must be uint8 [N, H, W, 3], got {self.images.dtype} "
+                             f"{list(self.images.shape)}")
+        pairs = f["pairs"]
+        M = len(pairs)
+        if pairs.ndim != 2 or pairs.shape[1] != 2 or pairs.dtype.kind not in "iu":
+            raise ValueError(f"{path}: field 'pairs' must be int [M, 2], got {pairs.dtype} {list(pairs.shape)}")
+        if M and (pairs.min() < 0 or pairs.max() >= len(self.images)):
+            raise ValueError(f"{path}: field 'pairs' indexes outside the {len(self.images)} images")
+        for k in ("src_kps", "trg_kps"):
+            if f[k].ndim != 3 or f[k].shape[0] != M or f[k].shape[2] != 2:
+                raise ValueError(f"{path}: field {k!r} must be float [{M}, Kmax, 2], got {list(f[k].shape)}")
+        n = f["n_kps"].reshape(-1)
+        if n.shape != (M,) or n.dtype.kind not in "iu" or (M and (n.min() < 0 or n.max() > f["src_kps"].shape[1]
+                                                               or n.max() > f["trg_kps"].shape[1])):
+            raise ValueError(f"{path}: field 'n_kps' must be int [{M}] within [0, Kmax], got {n.dtype} {n.tolist()}")
+        if f["trg_bbox"].shape != (M, 4):
+            raise ValueError(f"{path}: field 'trg_bbox' must be float [{M}, 4], got {list(f['trg_bbox'].shape)}")
+        if f["categories"].shape != (M,) or f["categories"].dtype.kind not in "US":
+            raise ValueError(f"{path}: field 'categories' must be str [{M}], got {f['categories'].dtype} "
+                             f"{list(f['categories'].shape)}")
+        self.pairs = [{"src": int(pairs[m, 0]), "trg": int(pairs[m, 1]), "category": str(f["categories"][m]),
+                       "src_kps": f["src_kps"][m, :n[m]].astype(np.float64),
+                       "trg_kps": f["trg_kps"][m, :n[m]].astype(np.float64),
+                       "trg_bbox": f["trg_bbox"][m].astype(np.float64).tolist()} for m in range(M)]
+
+    def __len__(self):
+        return len(self.pairs)
+
+    def __getitem__(self, i):
+        return self.pairs[i]
+
+    def load_image(self, j):
+        return self.images[j]
+
+
+def make_correspondence_dataset(path, split: str = "test"):
+    """An .npz file -> CorrespondenceNpzDataset, a directory -> SPairDataset(path, split)."""
+    path = str(path)
+    return CorrespondenceNpzDataset(path) if path.endswith(".npz") else SPairDataset(path, split)
 
 
 def make_eval_dataset(path):

@@ -808,3 +808,51 @@ def video_jf_counts(pred: torch.Tensor, gt: torch.Tensor, num_objects: int, radi
     N.check(N.init().d3_video_jf_counts(_p(pred), _p(gt), F_, H, W, K, int(radius), _p(counts), _s()),
             "d3_video_jf_counts")
     return counts
+
+
+# ------------------------------------------------------------------------------------------ keypoint correspondence
+def corr_descriptors(feats: torch.Tensor, n_maps: int, hw, out_hw, kp, out: torch.Tensor,
+                     qnorm: torch.Tensor) -> torch.Tensor:
+    """out bf16 [K, D] row k = the bilinear upsampling (align_corners=False) of patch map kp[k, 0] (feats bf16
+    [n_maps * h * w, D] rows) to out_hw sampled at pixel (x, y) = kp[k, 1:], L2-normalised; qnorm fp32 [K] the norms of
+    the rounded rows (d3_corr_descriptors).  kp: host integers [K, 3] = (map, x, y), checked before any launch."""
+    h, w = int(hw[0]), int(hw[1])
+    rows = [[int(v) for v in r] for r in kp]
+    assert all(len(r) == 3 for r in rows), "kp: (map, x, y) per keypoint"
+    K, D = len(rows), feats.shape[1]
+    kp_host = (C.c_int * (3 * K))(*[v for r in rows for v in r])
+    assert feats.dtype == bf16 and feats.shape[0] >= int(n_maps) * h * w
+    assert out.dtype == bf16 and out.shape[0] == K and out.shape[1] == D
+    assert qnorm.dtype == f32 and qnorm.is_contiguous() and qnorm.shape == (K,)
+    N.check(N.init().d3_corr_descriptors(_p(feats), _ld(feats), int(n_maps), h, w, D, int(out_hw[0]), int(out_hw[1]),
+                                         kp_host, K, _p(out), _ld(out), _p(qnorm), _s()), "d3_corr_descriptors")
+    return out
+
+
+def corr_gram(feats: torch.Tensor, n_maps: int, hw, gram: torch.Tensor) -> torch.Tensor:
+    """gram fp32 [n_maps * h * w, 5] = per patch its squared norm and its dot products with the right, lower,
+    lower-right and lower-left neighbours (0 where there is none) (d3_corr_gram)."""
+    h, w = int(hw[0]), int(hw[1])
+    assert feats.dtype == bf16 and feats.shape[0] >= int(n_maps) * h * w
+    assert gram.dtype == f32 and gram.is_contiguous() and gram.shape == (int(n_maps) * h * w, 5)
+    N.check(N.init().d3_corr_gram(_p(feats), _ld(feats), int(n_maps), h, w, feats.shape[1], _p(gram), _s()),
+            "d3_corr_gram")
+    return gram
+
+
+def corr_argmax(sim: torch.Tensor, gram: torch.Tensor, qnorm: torch.Tensor, hw, out_hw, xy: torch.Tensor,
+                cosine: torch.Tensor):
+    """For each of K keypoints, the pixel xy int32 [K, 2] = (x, y) of the out_hw bilinear upsampling of one target map
+    with the largest cosine to the descriptor, and that cosine fp32 [K] (d3_corr_argmax).  sim fp32 [K, >= h * w]: the
+    descriptors' dot products with the target's patches; gram fp32 [h * w, 5] the target's (corr_gram); qnorm fp32 [K]
+    the descriptors' norms (corr_descriptors).  Ties go to the lowest y * out_w + x."""
+    h, w = int(hw[0]), int(hw[1])
+    K = sim.shape[0]
+    assert sim.dtype == f32 and sim.shape[1] >= h * w
+    assert gram.dtype == f32 and gram.is_contiguous() and gram.shape == (h * w, 5)
+    assert qnorm.dtype == f32 and qnorm.is_contiguous() and qnorm.shape == (K,)
+    assert xy.dtype == torch.int32 and xy.is_contiguous() and xy.shape == (K, 2)
+    assert cosine.dtype == f32 and cosine.is_contiguous() and cosine.shape == (K,)
+    N.check(N.init().d3_corr_argmax(_p(sim), _ld(sim), _p(gram), _p(qnorm), K, h, w, int(out_hw[0]), int(out_hw[1]),
+                                    _p(xy), _p(cosine), _s()), "d3_corr_argmax")
+    return xy, cosine

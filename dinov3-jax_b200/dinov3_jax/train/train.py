@@ -259,6 +259,13 @@ def _video_cfg(config) -> dict:
     return video if video.get("dataset_path") else {}
 
 
+def _correspondence_cfg(config) -> dict:
+    """The `evaluation.correspondence` block, or {} when it names no dataset (then nothing is evaluated)."""
+    ev = config.get("evaluation", None) or {}
+    corr = dict(ev.get("correspondence", None) or {})
+    return corr if corr.get("dataset_path") else {}
+
+
 def eval_backbone(config, weights):
     """The frozen backbone k-NN evaluates, with the architecture of the run's `student.*` config (the depth is the
     number of blocks in the weights).  `weights`: a DinoVisionTransformer (returned as is); a `save_checkpoint`
@@ -456,6 +463,40 @@ def do_video_eval(config, model, header):
     return results
 
 
+def do_correspondence_eval(config, model, header):
+    """Keypoint correspondence (nearest neighbour over the upsampled patch features, PCK) through the teacher backbone of
+    `model` (see `eval_backbone`) on the `evaluation.correspondence` dataset; rank 0 writes
+    <output_dir>/eval/<header>/results_correspondence.json and returns {"PCK@a", "PCK-image@a" per alpha, "categories",
+    "n_pairs", "n_keypoints", "protocol", "config"} ({} on other ranks), "config" echoing the evaluation.correspondence
+    block.  Without a configured dataset it logs one line and returns {}."""
+    import json
+    from .. import distributed
+    corr = _correspondence_cfg(config)
+    if not corr:
+        if distributed.is_main_process():
+            print(f"do_correspondence_eval({header}): no evaluation.correspondence dataset configured, nothing "
+                  "evaluated", flush=True)
+        return {}
+    backbone = eval_backbone(config, model)            # collective for a live engine under FSDP
+    if not distributed.is_main_process():
+        return {}
+    from ..eval import eval_correspondence, make_correspondence_dataset
+    c = config.crops
+    out_dir = os.path.join(getattr(config.train, "output_dir", None) or ".", "eval", header)
+    kw = {k: corr[k] for k in ("image_size", "alphas", "batch_size", "num_workers") if k in corr}
+    results = eval_correspondence(backbone, make_correspondence_dataset(corr["dataset_path"], corr.get("split", "test")),
+                                  rgb_mean=c.get("rgb_mean", (0.485, 0.456, 0.406)),
+                                  rgb_std=c.get("rgb_std", (0.229, 0.224, 0.225)), **kw)
+    results["config"] = {k: (list(v) if isinstance(v, (list, tuple)) else v) for k, v in corr.items()}
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "results_correspondence.json"), "w") as f:
+        json.dump(results, f, indent=1)
+    a = results["protocol"]["alphas"][-1]
+    print(f"do_correspondence_eval({header}): PCK@{a:g} {results[f'PCK@{a:g}']:.4f} PCK-image@{a:g} "
+          f"{results[f'PCK-image@{a:g}']:.4f} over {results['n_pairs']} pairs", flush=True)
+    return results
+
+
 def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None, max_iters: int = 0,
              print_freq: int = 10):
     """train/train.py:319-713.  `data_loader` (optional) yields the reference's collate dicts; by default it is built
@@ -500,7 +541,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
     ev = config.get("evaluation", None) or {}
     knn_on, linear_on, seg_on = bool(_knn_cfg(config)), bool(_linear_cfg(config)), bool(_seg_cfg(config))
     depth_on, video_on = bool(_depth_cfg(config)), bool(_video_cfg(config))
-    any_on = knn_on or linear_on or seg_on or depth_on or video_on
+    corr_on = bool(_correspondence_cfg(config))
+    any_on = knn_on or linear_on or seg_on or depth_on or video_on or corr_on
     eval_period = int(ev.get("eval_period_iterations", 0) or 0) if any_on else 0
     for it in range(start_iter, n_iters):
         try:
@@ -528,6 +570,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
                 do_depth_eval(config, engine, f"training_{it}")
             if video_on:
                 do_video_eval(config, engine, f"training_{it}")
+            if corr_on:
+                do_correspondence_eval(config, engine, f"training_{it}")
         if it % print_freq == 0 or it == n_iters - 1:
             m = engine.read_metrics()                  # the only device->host sync of the loop
             if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
@@ -555,10 +599,11 @@ def main(argv=None):
     import random
     import numpy as np
     random.seed(args.seed); np.random.seed(args.seed); torch.manual_seed(args.seed)   # setup_job(seed=args.seed), :281
-    if args.eval not in ("", "knn", "linear", "seg", "depth", "video"):
+    if args.eval not in ("", "knn", "linear", "seg", "depth", "video", "correspondence"):
         raise NotImplementedError(f"--eval {args.eval!r}: the evaluations are k-NN (--eval knn, or empty), the linear "
                                   "probe (--eval linear), the linear segmentation probe (--eval seg), the linear "
-                                  "depth probe (--eval depth) and video object segmentation (--eval video)")
+                                  "depth probe (--eval depth), video object segmentation (--eval video) and keypoint "
+                                  "correspondence (--eval correspondence)")
     if args.eval_only:                                 # train/train.py:304-311
         import json
         from ..checkpointer import find_latest_checkpoint
@@ -580,6 +625,8 @@ def main(argv=None):
             return do_depth_eval(config, str(weights), f"manual_{it}")
         if args.eval == "video":
             return do_video_eval(config, str(weights), f"manual_{it}")
+        if args.eval == "correspondence":
+            return do_correspondence_eval(config, str(weights), f"manual_{it}")
         return do_test(config, str(weights), f"manual_{it}")
     model = SSLMetaArch(config)
     return do_train(config, model, resume=not args.no_resume, max_iters=args.max_iters, print_freq=args.print_freq)

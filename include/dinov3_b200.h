@@ -468,6 +468,24 @@ int d3_video_label_map(const float* soft, int h, int w, int C, int patch, int ou
 int d3_video_jf_counts(const void* pred_u8, const void* gt_u8, int F, int H, int W, int K, int radius,
                        long long* counts, void* stream);
 
+/* ---- keypoint correspondence over bilinearly upsampled patch features (see csrc/correspondence.cu) ---------------
+ * U(y, x) is torch's bilinear F.interpolate (align_corners = False) of an [h, w, D] bf16 patch map (rows of ld
+ * elements, map m at rows [m h w, (m + 1) h w)) to out_h x out_w.
+ * d3_corr_descriptors: out bf16 [K, ldo] row k = U_{map_k}(y_k, x_k) L2-normalised in fp32, rounded to bf16; qnorm
+ *   fp32 [K] the norm of each rounded row.  kp (host) int [K, 3] = (map, x, y), each checked against n_maps and
+ *   [0, out_w) x [0, out_h) before anything is launched.
+ * d3_corr_gram: gram fp32 [n_maps h w, 5] per patch (i, j): <f_ij, f_ij> and its dot products with the right, lower,
+ *   lower-right and lower-left neighbours (0 where the neighbour does not exist), fp32 in a fixed order.
+ * d3_corr_argmax: for each keypoint k, the pixel (x, y) of the target map that maximises the cosine of q_k with U(y, x),
+ *   from sim fp32 [K, lds] (row k = <q_k, f_p> over the target's h w patches, from d3_gemm_bf16), the target's gram
+ *   and qnorm; ties go to the lowest y out_w + x.  xy int [K, 2], cosine fp32 [K] the cosine there.  Nothing of
+ *   full resolution is written; deterministic (no atomics).                                                        */
+int d3_corr_descriptors(const void* feats, int ld, int n_maps, int h, int w, int D, int out_h, int out_w,
+                        const int* kp /*host*/, int K, void* out, int ldo, float* qnorm, void* stream);
+int d3_corr_gram(const void* feats, int ld, int n_maps, int h, int w, int D, float* gram, void* stream);
+int d3_corr_argmax(const float* sim, int lds, const float* gram, const float* qnorm, int K, int h, int w, int out_h,
+                   int out_w, int* xy, float* cosine, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
