@@ -110,6 +110,9 @@ SIGNATURES = {
     "d3_corr_descriptors": [P, I, I, I, I, I, I, I, C.POINTER(C.c_int), I, P, I, P, P],
     "d3_corr_gram": [P, I, I, I, I, I, P, P],
     "d3_corr_argmax": [P, I, P, P, I, I, I, I, I, P, P, P],
+    "d3_od_graph": [P, I, I, I, F, F, P, P, P],
+    "d3_od_fiedler": [P, P, I, I, F, I, P, P, P, P, P],
+    "d3_od_box": [P, I, I, I, I, C.POINTER(C.c_int), C.POINTER(C.c_int), P, I, P, P, P, P, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

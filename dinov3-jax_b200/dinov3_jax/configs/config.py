@@ -50,9 +50,10 @@ DEFAULTS = {
     "checkpointing": {"period": 3750, "max_to_keep": 3},
     "distillation": {"enabled": False, "full_cfg_path": "", "checkpoint_path": ""},   # ssl_default_config.yaml:130-133
     # k-NN (train.do_test), linear-probe (train.do_linear_eval), linear segmentation (train.do_seg_eval), linear depth
-    # (train.do_depth_eval), video segmentation (train.do_video_eval, DINO's label-propagation protocol) and keypoint
-    # correspondence (train.do_correspondence_eval, SPair-71k PCK) evaluations of the teacher backbone; empty dataset
-    # paths: nothing is evaluated.
+    # (train.do_depth_eval), video segmentation (train.do_video_eval, DINO's label-propagation protocol), keypoint
+    # correspondence (train.do_correspondence_eval, SPair-71k PCK) and unsupervised object discovery
+    # (train.do_discovery_eval, TokenCut CorLoc on VOC) evaluations of the teacher backbone; empty dataset paths:
+    # nothing is evaluated.
     # `config_files` (the reference's list of evaluation configs) is accepted and not read.  The segmentation and depth
     # schedules are this project's defaults, not a published recipe's.
     "evaluation": {"eval_period_iterations": 12500, "config_files": [],
@@ -78,7 +79,9 @@ DEFAULTS = {
                              "temperature": 0.1, "short_side": 480, "batch_size": 16, "num_workers": 4,
                              "save_masks": False},
                    "correspondence": {"dataset_path": "", "split": "test", "image_size": 512,
-                                      "alphas": [0.01, 0.05, 0.1], "batch_size": 16, "num_workers": 4}},
+                                      "alphas": [0.01, 0.05, 0.1], "batch_size": 16, "num_workers": 4},
+                   "discovery": {"dataset_path": "", "split": "trainval", "tau": 0.2, "eps": 1e-5,
+                                 "remove_difficult": False, "batch_size": 16, "num_workers": 4, "save_boxes": False}},
 }
 
 

@@ -1,6 +1,7 @@
 """Labelled image datasets for evaluation.  Each item is (uint8 HWC RGB numpy array, int label), for segmentation
 (uint8 HWC RGB, uint8 HW label map), or for depth (uint8 HWC RGB, fp32 HW depth in metres); a video dataset yields
-whole sequences (`DavisDataset`), a correspondence dataset keypoint pairs over its images (`SPairDataset`).  Images
+whole sequences (`DavisDataset`), a correspondence dataset keypoint pairs over its images (`SPairDataset`), a
+discovery dataset images with their object boxes (`VOCDiscoveryDataset`).  Images
 keep their own sizes, the transforms run on the GPU (`ops.eval_resize_crop`, `ops.seg_crop`, `ops.depth_crop`,
 `ops.video_resize`).  Decoding is host plumbing in DataLoader workers."""
 from __future__ import annotations
@@ -391,6 +392,105 @@ def make_correspondence_dataset(path, split: str = "test"):
     """An .npz file -> CorrespondenceNpzDataset, a directory -> SPairDataset(path, split)."""
     path = str(path)
     return CorrespondenceNpzDataset(path) if path.endswith(".npz") else SPairDataset(path, split)
+
+
+class VOCDiscoveryDataset:
+    """A PASCAL VOC root (VOC2007 or VOC2012): the ids of root/ImageSets/Main/<split>.txt, the images
+    root/JPEGImages/<id>.jpg and the annotations root/Annotations/<id>.xml (size/height, size/width and every
+    object/bndbox).  VOC's 1-based inclusive corners become [xmin - 1, ymin - 1, xmax, ymax]; remove_difficult drops
+    the objects whose `difficult` is 1.  `names`, `sizes` [(H, W)] and `boxes` [float64 [B, 4]] are read up front;
+    `load_image(i)` decodes image i to uint8 HWC RGB.  Errors name the file and the field."""
+
+    def __init__(self, root, split: str = "trainval", remove_difficult: bool = False):
+        import xml.etree.ElementTree as ET
+        self.root, self.split = str(root), split
+        lst = os.path.join(self.root, "ImageSets", "Main", f"{split}.txt")
+        if not os.path.isfile(lst):
+            raise FileNotFoundError(f"{lst} does not exist")
+        with open(lst) as f:
+            self.names = [line.split()[0] for line in f if line.strip()]
+        self.sizes, self.boxes = [], []
+        for name in self.names:
+            path = os.path.join(self.root, "Annotations", f"{name}.xml")
+            if not os.path.isfile(path):
+                raise FileNotFoundError(f"{split}.txt names {name}, but {path} does not exist")
+            try:
+                tree = ET.parse(path).getroot()
+            except ET.ParseError as e:
+                raise ValueError(f"{path}: not valid XML ({e})") from None
+            self.sizes.append((int(_xml_number(path, tree, "size/height")), int(_xml_number(path, tree, "size/width"))))
+            boxes = []
+            for obj in tree.findall("object"):
+                if remove_difficult and obj.find("difficult") is not None and _xml_number(path, obj, "difficult"):
+                    continue
+                if obj.find("bndbox") is None:
+                    raise ValueError(f"{path}: field 'object/bndbox' is missing")
+                x1, y1, x2, y2 = (_xml_number(path, obj, f"bndbox/{k}") for k in ("xmin", "ymin", "xmax", "ymax"))
+                boxes.append([x1 - 1.0, y1 - 1.0, x2, y2])
+            self.boxes.append(np.asarray(boxes, np.float64).reshape(-1, 4))
+        self.images = [os.path.join(self.root, "JPEGImages", f"{name}.jpg") for name in self.names]
+
+    def __len__(self):
+        return len(self.names)
+
+    def load_image(self, i):
+        from PIL import Image
+        with Image.open(self.images[i]) as im:
+            return np.asarray(im.convert("RGB"), dtype=np.uint8)
+
+
+def _xml_number(path, node, field) -> float:
+    e = node.find(field)
+    if e is None or e.text is None or not e.text.strip():
+        raise ValueError(f"{path}: field {field!r} is missing")
+    try:
+        return float(e.text)
+    except ValueError:
+        raise ValueError(f"{path}: field {field!r} is not a number: {e.text.strip()!r}") from None
+
+
+class DiscoveryNpzDataset:
+    """An .npz file with images (uint8 [N, Hmax, Wmax, 3]), sizes (int [N, 2]: H, W; image i is images[i, :H, :W]),
+    boxes (float [N, Bmax, 4]: x1 y1 x2 y2, 0-based continuous corners) and n_boxes (int [N], the first n_boxes[i] rows
+    used); the same `names`, `sizes`, `boxes` and `load_image` as VOCDiscoveryDataset, image i named "%05d" % i."""
+
+    def __init__(self, path):
+        path = str(path)
+        with np.load(path, allow_pickle=False) as z:
+            f = {k: np.asarray(_field(path, z, k)) for k in ("images", "sizes", "boxes", "n_boxes")}
+        im = f["images"]
+        if im.dtype != np.uint8 or im.ndim != 4 or im.shape[-1] != 3:
+            raise ValueError(f"{path}: field 'images' must be uint8 [N, H, W, 3], got {im.dtype} {list(im.shape)}")
+        n = len(im)
+        sz = f["sizes"]
+        if (sz.shape != (n, 2) or sz.dtype.kind not in "iu"
+                or (n and (sz.min() < 1 or sz[:, 0].max() > im.shape[1] or sz[:, 1].max() > im.shape[2]))):
+            raise ValueError(f"{path}: field 'sizes' must be int [{n}, 2] within [1, {im.shape[1]}] x "
+                             f"[1, {im.shape[2]}], got {sz.dtype} {list(sz.shape)}")
+        bx = f["boxes"]
+        if bx.ndim != 3 or bx.shape[0] != n or bx.shape[2] != 4 or bx.dtype.kind != "f":
+            raise ValueError(f"{path}: field 'boxes' must be float [{n}, Bmax, 4], got {bx.dtype} {list(bx.shape)}")
+        nb = f["n_boxes"].reshape(-1)
+        if nb.shape != (n,) or nb.dtype.kind not in "iu" or (n and (nb.min() < 0 or nb.max() > bx.shape[1])):
+            raise ValueError(f"{path}: field 'n_boxes' must be int [{n}] within [0, {bx.shape[1]}], got {nb.dtype} "
+                             f"{nb.tolist()}")
+        self.images = im
+        self.names = [f"{i:05d}" for i in range(n)]
+        self.sizes = [(int(h), int(w)) for h, w in sz]
+        self.boxes = [bx[i, :nb[i]].astype(np.float64) for i in range(n)]
+
+    def __len__(self):
+        return len(self.images)
+
+    def load_image(self, i):
+        H, W = self.sizes[i]
+        return self.images[i, :H, :W]
+
+
+def make_discovery_dataset(path, split: str = "trainval", remove_difficult: bool = False):
+    """An .npz file -> DiscoveryNpzDataset, a directory -> VOCDiscoveryDataset(path, split, remove_difficult)."""
+    path = str(path)
+    return DiscoveryNpzDataset(path) if path.endswith(".npz") else VOCDiscoveryDataset(path, split, remove_difficult)
 
 
 def make_eval_dataset(path):

@@ -856,3 +856,59 @@ def corr_argmax(sim: torch.Tensor, gram: torch.Tensor, qnorm: torch.Tensor, hw, 
     N.check(N.init().d3_corr_argmax(_p(sim), _ld(sim), _p(gram), _p(qnorm), K, h, w, int(out_hw[0]), int(out_hw[1]),
                                     _p(xy), _p(cosine), _s()), "d3_corr_argmax")
     return xy, cosine
+
+
+
+# ------------------------------------------------------------------------------------------ object discovery
+def od_graph(sim: torch.Tensor, tau: float, eps: float, bits: torch.Tensor, degree: torch.Tensor):
+    """The thresholded patch graph of n images of P patches (d3_od_graph): bits int32 [n, P, ceil(P / 32)] (bit j % 32
+    of word j / 32 of row i set when sim[m, i, j] > tau) and degree fp32 [n, P] = c_i + (P - c_i) eps.  sim fp32
+    [n, P, P], a view with unit inner stride of a buffer whose rows hold a multiple of 4 floats."""
+    n, P = sim.shape[0], sim.shape[1]
+    assert sim.dtype == f32 and sim.dim() == 3 and sim.shape[2] == P and sim.stride(2) == 1
+    assert sim.stride(0) == P * sim.stride(1), "the images' rows must follow one another"
+    assert bits.dtype == torch.int32 and bits.is_contiguous() and bits.shape == (n, P, -(-P // 32))
+    assert degree.dtype == f32 and degree.is_contiguous() and degree.shape == (n, P)
+    N.check(N.init().d3_od_graph(_p(sim), sim.stride(1), n, P, float(tau), float(eps), _p(bits), _p(degree), _s()),
+            "d3_od_graph")
+    return bits, degree
+
+
+def od_fiedler(bits: torch.Tensor, degree: torch.Tensor, eps: float, x: torch.Tensor, lambda2: torch.Tensor,
+               iters: torch.Tensor, converged: torch.Tensor, k_max: int = 256):
+    """The normalized-cut eigenvector of each image's graph (d3_od_fiedler): x fp32 [n, P] solves (D - A) x = lambda D x
+    at the second-smallest lambda (lambda2 fp32 [n]), x^T D x = 1; iters int32 [n] the Lanczos steps, converged int32
+    [n] 0 where k_max steps did not reach the residual bound.  bits, degree: od_graph's, with the same eps."""
+    n, P = degree.shape
+    assert bits.dtype == torch.int32 and bits.is_contiguous() and bits.shape == (n, P, -(-P // 32))
+    assert degree.dtype == f32 and degree.is_contiguous()
+    assert x.dtype == f32 and x.is_contiguous() and x.shape == (n, P)
+    for t, dt in ((lambda2, f32), (iters, torch.int32), (converged, torch.int32)):
+        assert t.dtype == dt and t.is_contiguous() and t.shape == (n,)
+    N.check(N.init().d3_od_fiedler(_p(bits), _p(degree), n, P, float(eps), int(k_max), _p(x), _p(lambda2),
+                                   _p(iters), _p(converged), _s()), "d3_od_fiedler")
+    return x, lambda2, iters, converged
+
+
+def od_box(x: torch.Tensor, grid, patch: int, sizes, n_gt, gt: torch.Tensor, fg: torch.Tensor, box: torch.Tensor,
+           best_iou: torch.Tensor, hit: torch.Tensor):
+    """TokenCut's box per image (d3_od_box): fg uint8 [n, h * w] the bipartition after the sign flip, box int32 [n, 4]
+    the pixel box (x0, y0, x1, y1) of the seed's 4-connected component, best_iou fp32 [n] against the image's
+    ground-truth boxes and hit int32 [n] = best_iou >= 0.5.  x fp32 [n, h * w] (od_fiedler); sizes host ints [n, 2] =
+    (H, W); n_gt host ints [n]; gt fp32 [n, b_max, 4] (x1 y1 x2 y2).  sizes and n_gt are checked before any launch."""
+    h, w = int(grid[0]), int(grid[1])
+    n = x.shape[0]
+    hw_ = [[int(v) for v in r] for r in sizes]
+    counts = [int(v) for v in n_gt]
+    assert len(hw_) == n and all(len(r) == 2 for r in hw_) and len(counts) == n
+    assert x.dtype == f32 and x.is_contiguous() and x.shape == (n, h * w)
+    assert gt.dtype == f32 and gt.is_contiguous() and gt.dim() == 3 and gt.shape[0] == n and gt.shape[2] == 4
+    assert fg.dtype == torch.uint8 and fg.is_contiguous() and fg.shape == (n, h * w)
+    assert box.dtype == torch.int32 and box.is_contiguous() and box.shape == (n, 4)
+    assert best_iou.dtype == f32 and best_iou.is_contiguous() and best_iou.shape == (n,)
+    assert hit.dtype == torch.int32 and hit.is_contiguous() and hit.shape == (n,)
+    sz = (C.c_int * max(2 * n, 1))(*[v for r in hw_ for v in r])
+    cnt = (C.c_int * max(n, 1))(*counts)
+    N.check(N.init().d3_od_box(_p(x), n, h, w, int(patch), sz, cnt, _p(gt), gt.shape[1], _p(fg), _p(box),
+                               _p(best_iou), _p(hit), _s()), "d3_od_box")
+    return box, best_iou, hit

@@ -486,6 +486,26 @@ int d3_corr_gram(const void* feats, int ld, int n_maps, int h, int w, int D, flo
 int d3_corr_argmax(const float* sim, int lds, const float* gram, const float* qnorm, int K, int h, int w, int out_h,
                    int out_w, int* xy, float* cosine, void* stream);
 
+/* ---- unsupervised object discovery: TokenCut's normalized cut (see csrc/discovery.cu) -----------------------------
+ * A launch covers n images with one grid of N = h w patches (2 <= N <= 4096); sim fp32 [n, N, lds] holds each image's
+ * patch similarities (d3_gemm_bf16).  Deterministic (no atomics).
+ * d3_od_graph: bits uint32 [n, N, ceil(N / 32)] with bit j % 32 of word j / 32 of row i set when sim_ij > tau; degree
+ *   fp32 [n, N] = c_i + (N - c_i) eps from the count c_i of set bits (A_ij = 1 above tau, else eps).
+ * d3_od_fiedler: per image the eigenvector x [n, N] of (D - A) x = lambda D x at the second-smallest lambda (lambda2
+ *   [n]), by deflated Lanczos on D^-1/2 A D^-1/2 with full reorthogonalisation, one CTA per image; x^T D x = 1.  It
+ *   stops when the residual bound falls to 1e-6 or after k_max <= 256 steps: iters [n] the steps taken, converged [n]
+ *   0 when k_max was reached first.
+ * d3_od_box: per image the bipartition fg_u8 [n, N] (x_i > mean(x), complemented when the seed argmax |x_i| is not in
+ *   it), the pixel box [n, 4] = (x0, y0, x1, y1) of the seed's 4-connected component clipped to the image, its best IoU
+ *   [n] with the image's ground-truth boxes gt fp32 [n, b_max, 4] (x1 y1 x2 y2) and hit [n] = best IoU >= 0.5.  sizes
+ *   (host) int [n, 2] = (H, W) must give the grid (ceil(H / patch) = h, ceil(W / patch) = w); n_gt (host) int [n] in
+ *   [0, b_max]; both checked before anything is launched.                                                        */
+int d3_od_graph(const float* sim, int lds, int n, int N, float tau, float eps, void* bits, float* degree, void* stream);
+int d3_od_fiedler(const void* bits, const float* degree, int n, int N, float eps, int k_max, float* x, float* lambda2,
+                  int* iters, int* converged, void* stream);
+int d3_od_box(const float* x, int n, int h, int w, int patch, const int* sizes /*host*/, const int* n_gt /*host*/,
+              const float* gt, int b_max, void* fg_u8, int* box, float* best_iou, int* hit, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
