@@ -113,6 +113,9 @@ SIGNATURES = {
     "d3_od_graph": [P, I, I, I, F, F, P, P, P],
     "d3_od_fiedler": [P, P, I, I, F, I, P, P, P, P, P],
     "d3_od_box": [P, I, I, I, I, C.POINTER(C.c_int), C.POINTER(C.c_int), P, I, P, P, P, P, P],
+    "d3_ret_resize": [P, LL, C.POINTER(C.c_longlong), I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, P],
+    "d3_ret_scale_sum": [P, I, LL, LL, P, P],
+    "d3_ret_rank_ap": [P, LL, I, I] + [C.POINTER(C.c_int)] * 6 + [P, P, P, P, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

@@ -51,9 +51,9 @@ DEFAULTS = {
     "distillation": {"enabled": False, "full_cfg_path": "", "checkpoint_path": ""},   # ssl_default_config.yaml:130-133
     # k-NN (train.do_test), linear-probe (train.do_linear_eval), linear segmentation (train.do_seg_eval), linear depth
     # (train.do_depth_eval), video segmentation (train.do_video_eval, DINO's label-propagation protocol), keypoint
-    # correspondence (train.do_correspondence_eval, SPair-71k PCK) and unsupervised object discovery
-    # (train.do_discovery_eval, TokenCut CorLoc on VOC) evaluations of the teacher backbone; empty dataset paths:
-    # nothing is evaluated.
+    # correspondence (train.do_correspondence_eval, SPair-71k PCK), unsupervised object discovery
+    # (train.do_discovery_eval, TokenCut CorLoc on VOC) and instance retrieval (train.do_retrieval_eval, revisited
+    # Oxford / Paris mAP) evaluations of the teacher backbone; empty dataset paths: nothing is evaluated.
     # `config_files` (the reference's list of evaluation configs) is accepted and not read.  The segmentation and depth
     # schedules are this project's defaults, not a published recipe's.
     "evaluation": {"eval_period_iterations": 12500, "config_files": [],
@@ -81,7 +81,10 @@ DEFAULTS = {
                    "correspondence": {"dataset_path": "", "split": "test", "image_size": 512,
                                       "alphas": [0.01, 0.05, 0.1], "batch_size": 16, "num_workers": 4},
                    "discovery": {"dataset_path": "", "split": "trainval", "tau": 0.2, "eps": 1e-5,
-                                 "remove_difficult": False, "batch_size": 16, "num_workers": 4, "save_boxes": False}},
+                                 "remove_difficult": False, "batch_size": 16, "num_workers": 4, "save_boxes": False},
+                   "retrieval": {"dataset_path": "", "dataset": "roxford5k", "image_size": 512,
+                                 "scales": [1.0, 0.7071067811865476, 0.5], "batch_size": 16, "num_workers": 4,
+                                 "save_ranks": False}},
 }
 
 

@@ -3,16 +3,19 @@ class tokens and the patch mean (`linear`), the linear segmentation probe on the
 linear depth probe on the patch and class tokens (`depth`), video object segmentation by label propagation through the
 patch tokens (`video`), keypoint correspondence by nearest neighbour over the upsampled patch tokens
 (`correspondence`), unsupervised object discovery by TokenCut's normalized cut on the patch tokens (`discovery`),
-over image, video, keypoint-pair and object-box datasets read on the host (`datasets`)."""
+instance retrieval by the multi-scale class token on revisited Oxford / Paris (`retrieval`), over image, video,
+keypoint-pair, object-box and retrieval datasets read on the host (`datasets`)."""
 from .correspondence import eval_correspondence
 from .datasets import (ADE20KSegmentation, CorrespondenceNpzDataset, DavisDataset, DepthListDataset, DepthNpzDataset,
-                       DiscoveryNpzDataset, ImageFolder, NpzDataset, SegNpzDataset, SPairDataset, VideoNpzDataset,
-                       VOCDiscoveryDataset, make_correspondence_dataset, make_depth_dataset, make_discovery_dataset,
-                       make_eval_dataset, make_seg_dataset, make_video_dataset)
+                       DiscoveryNpzDataset, ImageFolder, NpzDataset, RetrievalNpzDataset, RevisitedDataset,
+                       SegNpzDataset, SPairDataset, VideoNpzDataset, VOCDiscoveryDataset, make_correspondence_dataset,
+                       make_depth_dataset, make_discovery_dataset, make_eval_dataset, make_retrieval_dataset,
+                       make_seg_dataset, make_video_dataset)
 from .discovery import eval_object_discovery
 from .depth import DepthLinearHead, depth_metrics, eval_depth, sample_depth_boxes
 from .knn import KnnClassifier, eval_knn, extract_features
 from .linear import LinearClassifiers, eval_linear
+from .retrieval import eval_instance_retrieval
 from .segmentation import SegLinearHead, eval_segmentation
 from .video import eval_video_segmentation
 
@@ -22,4 +25,5 @@ __all__ = ["ImageFolder", "NpzDataset", "make_eval_dataset", "KnnClassifier", "e
            "DepthLinearHead", "sample_depth_boxes", "depth_metrics", "eval_depth", "DavisDataset", "VideoNpzDataset",
            "make_video_dataset", "eval_video_segmentation", "SPairDataset", "CorrespondenceNpzDataset",
            "make_correspondence_dataset", "eval_correspondence", "VOCDiscoveryDataset", "DiscoveryNpzDataset",
-           "make_discovery_dataset", "eval_object_discovery"]
+           "make_discovery_dataset", "eval_object_discovery", "RevisitedDataset", "RetrievalNpzDataset",
+           "make_retrieval_dataset", "eval_instance_retrieval"]

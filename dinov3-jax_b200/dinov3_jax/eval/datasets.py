@@ -1,12 +1,14 @@
 """Labelled image datasets for evaluation.  Each item is (uint8 HWC RGB numpy array, int label), for segmentation
 (uint8 HWC RGB, uint8 HW label map), or for depth (uint8 HWC RGB, fp32 HW depth in metres); a video dataset yields
 whole sequences (`DavisDataset`), a correspondence dataset keypoint pairs over its images (`SPairDataset`), a
-discovery dataset images with their object boxes (`VOCDiscoveryDataset`).  Images
+discovery dataset images with their object boxes (`VOCDiscoveryDataset`), a retrieval dataset database and query
+images with per-query ground-truth lists (`RevisitedDataset`).  Images
 keep their own sizes, the transforms run on the GPU (`ops.eval_resize_crop`, `ops.seg_crop`, `ops.depth_crop`,
 `ops.video_resize`).  Decoding is host plumbing in DataLoader workers."""
 from __future__ import annotations
 
 import os
+import pickle
 
 import numpy as np
 
@@ -497,3 +499,153 @@ def make_eval_dataset(path):
     """An .npz file -> NpzDataset, a directory -> ImageFolder."""
     path = str(path)
     return NpzDataset(path) if path.endswith(".npz") else ImageFolder(path)
+
+
+RETRIEVAL_DATASETS = ("roxford5k", "rparis6k")
+
+
+class _GndUnpickler(pickle.Unpickler):
+    """Builds builtin containers, numbers, strings and numpy arrays only: any other global is refused before it is
+    called, so a ground-truth pickle cannot run code."""
+
+    ALLOWED = {("builtins", n) for n in ("set", "frozenset", "list", "dict", "tuple", "int", "float", "complex", "bool",
+                                         "str", "bytes", "bytearray")} | {("_codecs", "encode")} | {
+        (m, n) for m in ("numpy.core.multiarray", "numpy._core.multiarray") for n in ("_reconstruct", "scalar")} | {
+        ("numpy", "ndarray"), ("numpy", "dtype")}
+
+    def __init__(self, f, path):
+        super().__init__(f)
+        self.path = path
+
+    def find_class(self, module, name):
+        if ("builtins" if module == "__builtin__" else module, name) not in self.ALLOWED:     # protocol 2 spelling
+            raise pickle.UnpicklingError(f"{self.path}: refuses the global {module}.{name} (only builtin containers, "
+                                         "numbers, strings and numpy arrays may be loaded)")
+        return super().find_class(module, name)
+
+
+def _gnd_indices(path, q, field, value, n) -> np.ndarray:
+    a = np.asarray(value)
+    if a.size and (a.dtype.kind not in "iu" or a.min() < 0 or a.max() >= n):
+        raise ValueError(f"{path}: field 'gnd[{q}].{field}' must hold database indices in [0, {n})")
+    return a.astype(np.int64).reshape(-1)
+
+
+class RevisitedDataset:
+    """A revisited Oxford / Paris root: root/gnd_<dataset>.pkl (imlist, qimlist, gnd: per query bbx, easy, hard, junk,
+    as lists or ndarrays) and the images root/jpg/<name>.jpg.  `db_names`, `q_names`, `db_sizes` and `q_sizes` [(H, W)]
+    (read from the JPEG headers), `q_bbx` float64 [Q, 4] (x1, y1, x2, y2), `easy`, `hard` and `junk` (int64 arrays per
+    query) are read up front; `load_db(i)` / `load_query(i)` decode an image to uint8 HWC RGB.  The pickle is loaded by
+    a restricted unpickler.  Errors name the file and the field."""
+
+    def __init__(self, root, dataset: str = "roxford5k"):
+        from PIL import Image
+        if dataset not in RETRIEVAL_DATASETS:
+            raise ValueError(f"dataset must be one of {RETRIEVAL_DATASETS}, got {dataset!r}")
+        self.root, self.name = str(root), dataset
+        path = os.path.join(self.root, f"gnd_{dataset}.pkl")
+        if not os.path.isfile(path):
+            raise FileNotFoundError(f"{path} does not exist")
+        with open(path, "rb") as f:
+            cfg = _GndUnpickler(f, path).load()
+        if not isinstance(cfg, dict):
+            raise ValueError(f"{path}: expected a dict with imlist, qimlist and gnd")
+        for k in ("imlist", "qimlist", "gnd"):
+            if k not in cfg:
+                raise ValueError(f"{path}: field {k!r} is missing")
+        self.db_names, self.q_names = [str(v) for v in cfg["imlist"]], [str(v) for v in cfg["qimlist"]]
+        gnd, n = list(cfg["gnd"]), len(self.db_names)
+        if len(gnd) != len(self.q_names):
+            raise ValueError(f"{path}: field 'gnd' has {len(gnd)} entries for {len(self.q_names)} queries")
+        self.q_bbx, self.easy, self.hard, self.junk = [], [], [], []
+        for q, g in enumerate(gnd):
+            for k in ("bbx", "easy", "hard", "junk"):
+                if not isinstance(g, dict) or k not in g:
+                    raise ValueError(f"{path}: field 'gnd[{q}].{k}' is missing")
+            bbx = np.asarray(g["bbx"], np.float64).reshape(-1)
+            if bbx.shape != (4,) or not np.isfinite(bbx).all():
+                raise ValueError(f"{path}: field 'gnd[{q}].bbx' must be 4 finite numbers (x1, y1, x2, y2)")
+            self.q_bbx.append(bbx)
+            for k, lst in (("easy", self.easy), ("hard", self.hard), ("junk", self.junk)):
+                lst.append(_gnd_indices(path, q, k, g[k], n))
+        self.q_bbx = np.asarray(self.q_bbx, np.float64).reshape(-1, 4)
+        self.db_images = [os.path.join(self.root, "jpg", f"{v}.jpg") for v in self.db_names]
+        self.q_images = [os.path.join(self.root, "jpg", f"{v}.jpg") for v in self.q_names]
+        self.db_sizes, self.q_sizes = [], []
+        for files, sizes in ((self.db_images, self.db_sizes), (self.q_images, self.q_sizes)):
+            for p in files:
+                if not os.path.isfile(p):
+                    raise FileNotFoundError(f"{path} names {os.path.basename(p)[:-4]}, but {p} does not exist")
+                with Image.open(p) as im:
+                    sizes.append((im.height, im.width))
+
+    @staticmethod
+    def _load(path):
+        from PIL import Image
+        with Image.open(path) as im:
+            return np.asarray(im.convert("RGB"), dtype=np.uint8)
+
+    def load_db(self, i):
+        return self._load(self.db_images[i])
+
+    def load_query(self, i):
+        return self._load(self.q_images[i])
+
+
+class RetrievalNpzDataset:
+    """An .npz file with db_images (uint8 [N, Hmax, Wmax, 3]) and db_sizes (int [N, 2]: H, W), q_images and q_sizes
+    likewise, q_bbx (float [Q, 4]: x1 y1 x2 y2) and the easy, hard and junk lists as CSR pairs (easy_ptr int [Q + 1]
+    from 0, easy_idx int database indices, and likewise hard_* and junk_*); the same fields and loaders as
+    RevisitedDataset, images named "%05d" % i.  Errors name the file and the field."""
+
+    def __init__(self, path, dataset: str = "roxford5k"):
+        path = str(path)
+        keys = ["db_images", "db_sizes", "q_images", "q_sizes", "q_bbx"] + [f"{k}_{s}" for k in ("easy", "hard", "junk")
+                                                                           for s in ("ptr", "idx")]
+        with np.load(path, allow_pickle=False) as z:
+            f = {k: np.asarray(_field(path, z, k)) for k in keys}
+        self.name = str(dataset)
+        for pre in ("db", "q"):
+            im, sz = f[f"{pre}_images"], f[f"{pre}_sizes"]
+            if im.dtype != np.uint8 or im.ndim != 4 or im.shape[-1] != 3:
+                raise ValueError(f"{path}: field '{pre}_images' must be uint8 [n, H, W, 3], got {im.dtype} "
+                                 f"{list(im.shape)}")
+            n = len(im)
+            if (sz.shape != (n, 2) or sz.dtype.kind not in "iu"
+                    or (n and (sz.min() < 1 or sz[:, 0].max() > im.shape[1] or sz[:, 1].max() > im.shape[2]))):
+                raise ValueError(f"{path}: field '{pre}_sizes' must be int [{n}, 2] within [1, {im.shape[1]}] x "
+                                 f"[1, {im.shape[2]}], got {sz.dtype} {list(sz.shape)}")
+        N, Q = len(f["db_images"]), len(f["q_images"])
+        bbx = f["q_bbx"]
+        if bbx.shape != (Q, 4) or bbx.dtype.kind not in "fiu" or not np.isfinite(bbx).all():
+            raise ValueError(f"{path}: field 'q_bbx' must be finite [{Q}, 4], got {bbx.dtype} {list(bbx.shape)}")
+        lists = {}
+        for k in ("easy", "hard", "junk"):
+            ptr, idx = f[f"{k}_ptr"].reshape(-1), f[f"{k}_idx"].reshape(-1)
+            if (ptr.shape != (Q + 1,) or ptr.dtype.kind not in "iu" or ptr[0] != 0 or (np.diff(ptr) < 0).any()
+                    or ptr[-1] != len(idx)):
+                raise ValueError(f"{path}: field '{k}_ptr' must be int [{Q + 1}], from 0, non-decreasing, up to "
+                                 f"len({k}_idx) = {len(idx)}")
+            if idx.size and (idx.dtype.kind not in "iu" or idx.min() < 0 or idx.max() >= N):
+                raise ValueError(f"{path}: field '{k}_idx' must hold database indices in [0, {N})")
+            lists[k] = [idx[ptr[q]:ptr[q + 1]].astype(np.int64) for q in range(Q)]
+        self.easy, self.hard, self.junk = lists["easy"], lists["hard"], lists["junk"]
+        self.db, self.q = f["db_images"], f["q_images"]
+        self.db_sizes = [(int(h), int(w)) for h, w in f["db_sizes"]]
+        self.q_sizes = [(int(h), int(w)) for h, w in f["q_sizes"]]
+        self.q_bbx = bbx.astype(np.float64)
+        self.db_names, self.q_names = [f"{i:05d}" for i in range(N)], [f"{i:05d}" for i in range(Q)]
+
+    def load_db(self, i):
+        H, W = self.db_sizes[i]
+        return self.db[i, :H, :W]
+
+    def load_query(self, i):
+        H, W = self.q_sizes[i]
+        return self.q[i, :H, :W]
+
+
+def make_retrieval_dataset(path, dataset: str = "roxford5k"):
+    """An .npz file -> RetrievalNpzDataset, a directory -> RevisitedDataset(path, dataset)."""
+    path = str(path)
+    return RetrievalNpzDataset(path, dataset) if path.endswith(".npz") else RevisitedDataset(path, dataset)

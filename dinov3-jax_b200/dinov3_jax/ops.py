@@ -8,6 +8,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 
+import numpy as np
 import torch
 
 from . import _native as N
@@ -912,3 +913,57 @@ def od_box(x: torch.Tensor, grid, patch: int, sizes, n_gt, gt: torch.Tensor, fg:
     N.check(N.init().d3_od_box(_p(x), n, h, w, int(patch), sz, cnt, _p(gt), gt.shape[1], _p(fg), _p(box),
                                _p(best_iou), _p(hit), _s()), "d3_od_box")
     return box, best_iou, hit
+
+
+# ------------------------------------------------------------------------------------------------ instance retrieval
+def ret_resize(src: torch.Tensor, desc, out: torch.Tensor, *, mean, std) -> torch.Tensor:
+    """torch's F.interpolate(bicubic, antialias=True, align_corners=False) of the crop box of each of n packed uint8
+    HWC images to out bf16 [n, h, w, 3], on float values, then (v / 255 - mean) / std (d3_ret_resize).  src uint8
+    (flat, on the device); desc host ints [n, 7] = (byte offset, H, W, x0, y0, x1, y1), the box [x0, x1) x [y0, y1);
+    checked before any launch."""
+    n, h, w = out.shape[0], out.shape[1], out.shape[2]
+    rows = [[int(v) for v in r] for r in desc]
+    assert src.dtype == torch.uint8 and src.is_contiguous()
+    assert out.dtype == bf16 and out.is_contiguous() and out.shape == (n, h, w, 3)
+    assert len(rows) == n and all(len(r) == 7 for r in rows)
+    d = (C.c_longlong * max(7 * n, 1))(*[v for r in rows for v in r])
+    m = (C.c_float * 3)(*[float(v) for v in mean])
+    s = (C.c_float * 3)(*[float(v) for v in std])
+    N.check(N.init().d3_ret_resize(_p(src), src.numel(), d, n, h, w, m, s, _p(out), _s()), "d3_ret_resize")
+    return out
+
+
+def ret_scale_sum(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """out fp32 [n, D] = x[0] + x[1] + ... + x[S - 1], added in that order, of x fp32 [S, n, D] (d3_ret_scale_sum)."""
+    S = x.shape[0]
+    assert x.dtype == f32 and x.is_contiguous() and x.dim() == 3
+    assert out.dtype == f32 and out.is_contiguous() and out.shape == x.shape[1:]
+    N.check(N.init().d3_ret_scale_sum(_p(x), S, out.numel(), out.numel(), _p(out), _s()), "d3_ret_scale_sum")
+    return out
+
+
+def _csr(ptr, idx):
+    """A host CSR pair as int32 arrays (kept alive by the caller while the C call reads them)."""
+    p, i = (np.ascontiguousarray(np.asarray(v).reshape(-1), dtype=np.int32) for v in (ptr, idx))
+    return p, i
+
+
+def ret_rank_ap(sim: torch.Tensor, n_cols: int, easy, hard, junk, ranks: torch.Tensor, ap: torch.Tensor,
+                pk: torch.Tensor, n_ok: torch.Tensor):
+    """The revisited ranking of the first n_cols columns of sim fp32 [Q, >= n_cols] (d3_ret_rank_ap): ranks int32
+    [n_easy + n_hard + n_junk] the exact 0-based rank of every list entry (easy, then hard, then junk entries), ap fp64
+    [Q, 3] and pk fp64 [Q, 3, 3] (P@1, P@5, P@10) for the Easy, Medium and Hard protocols, n_ok int32 [Q, 3].  easy,
+    hard, junk: host CSR pairs (ptr [Q + 1], idx), checked before any launch."""
+    Q = sim.shape[0]
+    assert sim.dtype == f32 and sim.dim() == 2 and sim.stride(1) == 1
+    lists = [_csr(*l) for l in (easy, hard, junk)]
+    assert all(l[0].size == Q + 1 for l in lists), "every list needs Q + 1 row pointers"
+    total = sum(l[1].size for l in lists)
+    assert ranks.dtype == torch.int32 and ranks.is_contiguous() and ranks.numel() == total
+    assert ap.dtype == torch.float64 and ap.is_contiguous() and ap.shape == (Q, 3)
+    assert pk.dtype == torch.float64 and pk.is_contiguous() and pk.shape == (Q, 3, 3)
+    assert n_ok.dtype == torch.int32 and n_ok.is_contiguous() and n_ok.shape == (Q, 3)
+    args = [a.ctypes.data_as(C.POINTER(C.c_int)) for l in lists for a in l]
+    N.check(N.init().d3_ret_rank_ap(_p(sim), sim.stride(0), Q, int(n_cols), *args, _p(ranks), _p(ap), _p(pk),
+                                    _p(n_ok), _s()), "d3_ret_rank_ap")
+    return ranks, ap, pk, n_ok

@@ -273,6 +273,13 @@ def _discovery_cfg(config) -> dict:
     return disc if disc.get("dataset_path") else {}
 
 
+def _retrieval_cfg(config) -> dict:
+    """The `evaluation.retrieval` block, or {} when it names no dataset (then nothing is evaluated)."""
+    ev = config.get("evaluation", None) or {}
+    ret = dict(ev.get("retrieval", None) or {})
+    return ret if ret.get("dataset_path") else {}
+
+
 def eval_backbone(config, weights):
     """The frozen backbone k-NN evaluates, with the architecture of the run's `student.*` config (the depth is the
     number of blocks in the weights).  `weights`: a DinoVisionTransformer (returned as is); a `save_checkpoint`
@@ -538,6 +545,40 @@ def do_discovery_eval(config, model, header):
     return results
 
 
+def do_retrieval_eval(config, model, header):
+    """Instance retrieval (revisited Oxford / Paris mAP of the multi-scale class token) through the teacher backbone of
+    `model` (see `eval_backbone`) on the `evaluation.retrieval` dataset; rank 0 writes
+    <output_dir>/eval/<header>/results_retrieval.json and returns {"mAP", "mP@k", "n_empty", "n_queries",
+    "n_database", "protocol", "config"} (and "ranks" with save_ranks; {} on other ranks), "config" echoing the
+    evaluation.retrieval block.  Without a configured dataset it logs one line and returns {}."""
+    import json
+    from .. import distributed
+    ret = _retrieval_cfg(config)
+    if not ret:
+        if distributed.is_main_process():
+            print(f"do_retrieval_eval({header}): no evaluation.retrieval dataset configured, nothing evaluated",
+                  flush=True)
+        return {}
+    backbone = eval_backbone(config, model)            # collective for a live engine under FSDP
+    if not distributed.is_main_process():
+        return {}
+    from ..eval import eval_instance_retrieval, make_retrieval_dataset
+    c = config.crops
+    out_dir = os.path.join(getattr(config.train, "output_dir", None) or ".", "eval", header)
+    kw = {k: ret[k] for k in ("image_size", "scales", "batch_size", "num_workers", "save_ranks") if k in ret}
+    dataset = make_retrieval_dataset(ret["dataset_path"], ret.get("dataset", "roxford5k"))
+    results = eval_instance_retrieval(backbone, dataset, rgb_mean=c.get("rgb_mean", (0.485, 0.456, 0.406)),
+                                      rgb_std=c.get("rgb_std", (0.229, 0.224, 0.225)), **kw)
+    results["config"] = {k: (list(v) if isinstance(v, (list, tuple)) else v) for k, v in ret.items()}
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "results_retrieval.json"), "w") as f:
+        json.dump(results, f, indent=1)
+    m = results["mAP"]
+    print(f"do_retrieval_eval({header}): mAP easy {m['easy']:.2f} medium {m['medium']:.2f} hard {m['hard']:.2f} over "
+          f"{results['n_queries']} queries and {results['n_database']} database images", flush=True)
+    return results
+
+
 def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None, max_iters: int = 0,
              print_freq: int = 10):
     """train/train.py:319-713.  `data_loader` (optional) yields the reference's collate dicts; by default it is built
@@ -583,7 +624,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
     knn_on, linear_on, seg_on = bool(_knn_cfg(config)), bool(_linear_cfg(config)), bool(_seg_cfg(config))
     depth_on, video_on = bool(_depth_cfg(config)), bool(_video_cfg(config))
     corr_on, disc_on = bool(_correspondence_cfg(config)), bool(_discovery_cfg(config))
-    any_on = knn_on or linear_on or seg_on or depth_on or video_on or corr_on or disc_on
+    ret_on = bool(_retrieval_cfg(config))
+    any_on = knn_on or linear_on or seg_on or depth_on or video_on or corr_on or disc_on or ret_on
     eval_period = int(ev.get("eval_period_iterations", 0) or 0) if any_on else 0
     for it in range(start_iter, n_iters):
         try:
@@ -615,6 +657,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
                 do_correspondence_eval(config, engine, f"training_{it}")
             if disc_on:
                 do_discovery_eval(config, engine, f"training_{it}")
+            if ret_on:
+                do_retrieval_eval(config, engine, f"training_{it}")
         if it % print_freq == 0 or it == n_iters - 1:
             m = engine.read_metrics()                  # the only device->host sync of the loop
             if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
@@ -642,12 +686,12 @@ def main(argv=None):
     import random
     import numpy as np
     random.seed(args.seed); np.random.seed(args.seed); torch.manual_seed(args.seed)   # setup_job(seed=args.seed), :281
-    if args.eval not in ("", "knn", "linear", "seg", "depth", "video", "correspondence", "discovery"):
+    if args.eval not in ("", "knn", "linear", "seg", "depth", "video", "correspondence", "discovery", "retrieval"):
         raise NotImplementedError(f"--eval {args.eval!r}: the evaluations are k-NN (--eval knn, or empty), the linear "
                                   "probe (--eval linear), the linear segmentation probe (--eval seg), the linear "
                                   "depth probe (--eval depth), video object segmentation (--eval video) and keypoint "
                                   "correspondence (--eval correspondence), and unsupervised object discovery "
-                                  "(--eval discovery)")
+                                  "(--eval discovery), and instance retrieval (--eval retrieval)")
     if args.eval_only:                                 # train/train.py:304-311
         import json
         from ..checkpointer import find_latest_checkpoint
@@ -673,6 +717,8 @@ def main(argv=None):
             return do_correspondence_eval(config, str(weights), f"manual_{it}")
         if args.eval == "discovery":
             return do_discovery_eval(config, str(weights), f"manual_{it}")
+        if args.eval == "retrieval":
+            return do_retrieval_eval(config, str(weights), f"manual_{it}")
         return do_test(config, str(weights), f"manual_{it}")
     model = SSLMetaArch(config)
     return do_train(config, model, resume=not args.no_resume, max_iters=args.max_iters, print_freq=args.print_freq)

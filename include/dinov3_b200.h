@@ -506,6 +506,27 @@ int d3_od_fiedler(const void* bits, const float* degree, int n, int N, float eps
 int d3_od_box(const float* x, int n, int h, int w, int patch, const int* sizes /*host*/, const int* n_gt /*host*/,
               const float* gt, int b_max, void* fg_u8, int* box, float* best_iou, int* hit, void* stream);
 
+/* ---- instance retrieval: revisited Oxford / Paris (see csrc/retrieval.cu) --------------------------------------------
+ * Deterministic (no float atomics).
+ * d3_ret_resize: n packed uint8 HWC images, desc (host) int64 [n, 7] = (byte offset, H, W, x0, y0, x1, y1) inside a
+ *   source buffer of src_bytes bytes; the crop box [x0, x1) x [y0, y1) of each image is resized to out_h x out_w with
+ *   torch's antialiased bicubic (align_corners = False) on float values and normalised, (v / 255 - mean) / std, into
+ *   bf16 NHWC [n, out_h, out_w, 3].  desc is checked before anything is launched.
+ * d3_ret_scale_sum: out[i] = x[i] + x[stride + i] + ... + x[(S - 1) stride + i] (scale order) for i < count, fp32.
+ * d3_ret_rank_ap: per query q of the fp32 similarities sim [Q, lds] (N columns), the exact 0-based rank of every
+ *   listed image j, #{i : s_qi > s_qj or (s_qi == s_qj and i < j)}, into ranks (device int [n_easy + n_hard +
+ *   n_junk], the easy entries, then the hard, then the junk, as in the index arrays), and for the Easy, Medium and
+ *   Hard protocols of the revisited benchmark ap [Q, 3] and pk [Q, 3, 3] (P@1, P@5, P@10) in fp64, n_ok [Q, 3] the ok
+ *   images (AP and P@k are NaN where it is 0).  The lists are host CSR pairs (ptr [Q + 1] from 0, idx in [0, N)),
+ *   at most 8192 entries per query over the three lists; all are checked before anything is launched.           */
+int d3_ret_resize(const void* src_u8, long long src_bytes, const long long* desc /*host*/, int n, int out_h, int out_w,
+                  const float* mean3 /*host*/, const float* std3 /*host*/, void* out, void* stream);
+int d3_ret_scale_sum(const float* x, int S, long long stride, long long count, float* out, void* stream);
+int d3_ret_rank_ap(const float* sim, long long lds, int Q, int N, const int* easy_ptr /*host*/,
+                   const int* easy_idx /*host*/, const int* hard_ptr /*host*/, const int* hard_idx /*host*/,
+                   const int* junk_ptr /*host*/, const int* junk_idx /*host*/, int* ranks, double* ap, double* pk,
+                   int* n_ok, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
