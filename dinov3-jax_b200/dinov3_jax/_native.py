@@ -80,6 +80,7 @@ SIGNATURES = {
     "d3_pool_tokens": [P, P, I, I, I, I, I, P],
     "d3_resize_tokens_bilinear_aa": [P, P, I, I, I, I, I, I, I, P],
     "d3_koleo_fwd_bwd_rows": [P, P, P, P, P, P, P, I, I, I, I, F, F, F, P],
+    "d3_koleo_topk_rows": [P, I, I, I, I, I, I, I, F, F, F, P, LL, P, P, P],
     "d3_aug_resized_crop": [P, I, I, I, P, I, P, I, P],
     "d3_aug_color": [P, P, I, I, P, P],
     "d3_aug_blur": [P, P, P, P, I, I, P],

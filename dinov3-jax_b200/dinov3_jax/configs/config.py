@@ -21,7 +21,9 @@ DEFAULTS = {
     "compute_precision": {"param_dtype": "bf16", "reduce_dtype": "fp32", "sharding_strategy": "SHARD_GRAD_OP"},
     "dino": {"loss_weight": 1.0, "global_ignore_diagonal": True, "head_n_prototypes": 65536, "head_bottleneck_dim": 256,
              "head_nlayers": 3, "head_hidden_dim": 2048, "koleo_loss_weight": 0.1, "koleo_loss_distributed": False,
-             "koleo_topk": 1, "reweight_dino_local_loss": False},
+             "koleo_topk": 1, "koleo_distributed_replicas": 0, "koleo_distributed_loss_group_size": None,
+             "koleo_distributed_loss_group_data": True, "reweight_dino_local_loss": False,
+             "local_loss_weight_schedule": {"start": 0.5, "peak": 0.5, "end": 0.5, "warmup_epochs": 0}},
     "ibot": {"loss_weight": 1.0, "mask_sample_probability": 0.5, "mask_ratio_min_max": [0.1, 0.5],
              "mask_random_circular_shift": False, "separate_head": True, "head_n_prototypes": 65536,
              "head_bottleneck_dim": 256, "head_nlayers": 3, "head_hidden_dim": 2048},

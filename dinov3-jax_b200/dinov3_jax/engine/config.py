@@ -47,6 +47,11 @@ class EngineConfig:
     student_temp: float = 0.1
     dino_loss_weight: float = 1.0
     koleo_loss_weight: float = 0.1
+    # dino.koleo_loss_distributed: top-k neighbours over the class tokens of a loss group of koleo_group_size images
+    # (None: every rank's), engine/koleo.py.  Off: the plain per-rank KoLeo (d3_koleo_fwd_bwd_rows)
+    koleo_distributed: bool = False
+    koleo_topk: int = 1
+    koleo_group_size: int | None = None
     ibot_loss_weight: float = 1.0
     clip_grad: float = 3.0
     ln_eps: float = 1e-6             # norm_layer layernorm: 1e-6, layernormbf16: 1e-5 (models/vision_transformer.py:38-42)
@@ -144,8 +149,7 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
     if cfg.student.ffn_layer not in ffn_table or cfg.student.norm_layer not in ("layernorm", "layernormbf16"):
         raise NotImplementedError("ffn_layer must be mlp | swiglu[32|64|128] and norm_layer layernorm | layernormbf16 "
                                   "(RMSNorm is not on the GPU path, SURVEY 8f)")
-    if cfg.dino.koleo_loss_distributed or cfg.dino.reweight_dino_local_loss:
-        raise NotImplementedError("distributed KoLeo inside the step / local-loss reweighting are not on the GPU path yet")
+    koleo_kw = koleo_config_from_reference_cfg(cfg)
     gram_kw = {}
     if cfg.gram.use_loss:
         gg = cfg.gram
@@ -171,8 +175,6 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
         if gsz is not None and int(gsz) != int(cfg.crops.global_crops_size) and \
                 str(gg.get("global_teacher_resize_method", "bicubic")) != "bicubic":
             raise NotImplementedError("gram.global_teacher_resize_method must be bicubic")
-        if gg.get("loss_weight_schedule", None):
-            raise NotImplementedError("gram.loss_weight_schedule: pass gram_loss_weight per step to Engine.train_step instead")
         if bool(gg.get("remove_neg", False)) and bool(gg.get("remove_only_teacher_neg", False)):
             raise ValueError("gram.remove_neg and gram.remove_only_teacher_neg are exclusive (loss/gram_loss.py:20)")
         if not gg.get("ema_teacher", False) and int(gg.get("it_load_ema_teacher", -1)) < 0:
@@ -229,7 +231,37 @@ def config_from_reference_cfg(cfg) -> EngineConfig:
         n_storage=int(cfg.student.n_storage_tokens), ln_eps=1e-5 if cfg.student.norm_layer == "layernormbf16" else 1e-6,
         ffn_layer=ffn_table[cfg.student.ffn_layer][0], swiglu_align=ffn_table[cfg.student.ffn_layer][1],
         mask_k_bias=bool(cfg.student.get("mask_k_bias", False)),
-        mlp_second_act=ffn_table[cfg.student.ffn_layer][0] == "mlp", **ibot_kw, **gram_kw)
+        mlp_second_act=ffn_table[cfg.student.ffn_layer][0] == "mlp", **ibot_kw, **gram_kw, **koleo_kw)
+
+
+def koleo_config_from_reference_cfg(cfg) -> dict:
+    """dino.koleo_loss_distributed / koleo_topk / koleo_distributed_loss_group_size / _group_data /
+    koleo_distributed_replicas (train/ssl_meta_arch.py:94-106) as EngineConfig fields.  A group size must be a
+    multiple of train.batch_size_per_gpu (that it divides the global batch is checked when the engine knows the
+    world size)."""
+    from .koleo import MAX_TOPK
+    d = cfg.dino
+    g = lambda key, default: d.get(key, default) if hasattr(d, "get") else getattr(d, key, default)
+    topk = int(g("koleo_topk", 1))
+    if not g("koleo_loss_distributed", False):
+        if topk != 1:
+            raise ValueError("dino.koleo_topk > 1 needs dino.koleo_loss_distributed: true (ssl_meta_arch.py:105)")
+        return {}
+    if int(g("koleo_distributed_replicas", 0) or 0) != 0:
+        raise ValueError("dino.koleo_distributed_replicas is no longer supported: it must be 0 (ssl_meta_arch.py:97)")
+    if not g("koleo_distributed_loss_group_data", True):
+        raise NotImplementedError("dino.koleo_distributed_loss_group_data: false: a loss group is always consecutive "
+                                  "ranks' images")
+    G = g("koleo_distributed_loss_group_size", None)
+    B = int(cfg.train.batch_size_per_gpu)
+    if G is not None:
+        G = int(G)
+        if G <= 0 or G % B:
+            raise ValueError(f"dino.koleo_distributed_loss_group_size {G} must be a multiple of "
+                             f"train.batch_size_per_gpu {B}")
+    if not 1 <= topk <= MAX_TOPK or (G is not None and topk > G - 1):
+        raise ValueError(f"dino.koleo_topk {topk} must be in [1, min({MAX_TOPK}, rows in the loss group - 1)]")
+    return dict(koleo_distributed=True, koleo_topk=topk, koleo_group_size=G)
 
 
 def distill_config_from_reference_cfg(cfg) -> EngineConfig | None:

@@ -135,6 +135,11 @@ class Engine:
         self.koleo_nrm = torch.empty(B, dtype=f32, device=dev)
         self.koleo_nn = torch.empty(B, dtype=i32, device=dev)
         self.koleo_coef = torch.empty(B, dtype=f32, device=dev)
+        if cfg.koleo_distributed:
+            from .koleo import DistributedKoLeo
+            self.koleo_dist = DistributedKoLeo(comm, B, D, cfg.n_global, cfg.koleo_topk, cfg.koleo_group_size, dev)
+        elif cfg.koleo_topk != 1:
+            raise ValueError("koleo_topk > 1 needs koleo_distributed (train/ssl_meta_arch.py:105)")
         self.metrics = torch.zeros(8, dtype=f32, device=dev)   # 0 dino_local 1 dino_global 2 koleo 3 ibot
         # backward scratch over the student stream
         T, Hd = self.student.T, cfg.ffn_width
@@ -168,6 +173,9 @@ class Engine:
         self.delta = [e(s.n, cfg.heads, s.N, dt=f32) for s in self.s_sets]
         self.dTok = [e(s.n * s.P, D) for s in self.s_sets]
         self._build_ce_tables()
+        # dino.reweight_dino_local_loss: the local rows' CE gradient weights are base * w (train_step sets w)
+        self.dino_local_loss_weight = 1.0
+        self._wg_local = self.ce_dino[3][ng:].clone()
         self._build_rows()
         self.step_count = 0
         self._gram = g = GramAnchor(cfg, self.s_sets[0], dev, self.fp8) if cfg.gram_use_loss else None
@@ -503,7 +511,10 @@ class Engine:
         self._head_bwd(self.h_s_ibot, "ibot_head", M)
         # KoLeo on the pre-head global cls tokens, per crop (train/ssl_meta_arch.py:513): loss weight
         # koleo_loss_weight * n_global * (1/n_global) per crop; metric = mean over crops
-        for c in range(cfg.n_global):
+        if cfg.koleo_distributed:
+            self.koleo_dist(self.cls_f32[:ng], self.metrics[2:3], self.h_s_dino.dA0, 1.0 / cfg.n_global,
+                            cfg.koleo_loss_weight)
+        for c in range(0 if cfg.koleo_distributed else cfg.n_global):
             ops.koleo_fwd_bwd(self.cls_f32[c * B:(c + 1) * B], self.koleo_xn, self.koleo_nrm, self.koleo_nn,
                               self.koleo_coef, self.metrics[2:3], self.h_s_dino.dA0[c * B:(c + 1) * B],
                               1.0 / cfg.n_global, cfg.koleo_loss_weight)
@@ -563,12 +574,23 @@ class Engine:
         for st in self.params.mods.values():
             ops.ema(st.t_master, st.master, st.t_bf16_shard, st.layout.n_mat_shard, float(momentum))
 
+    def set_dino_local_loss_weight(self, w: float):
+        """Multiply the local-crop DINO term (its loss in total_loss and its gradient) by w; the tables change only
+        when w does."""
+        w = float(w)
+        if w != self.dino_local_loss_weight:
+            torch.mul(self._wg_local, w, out=self.ce_dino[3][self.cfg.n_global * self.B:])
+            self.dino_local_loss_weight = w
+
     def train_step(self, batch: dict | None, *, teacher_temp: float, lr: float, wd: float, last_layer_lr: float,
-                   momentum: float, gram_loss_weight: float | None = None, iteration: int | None = None):
+                   momentum: float, gram_loss_weight: float | None = None, dino_local_loss_weight: float | None = None,
+                   iteration: int | None = None):
         if batch is not None:
             self.set_batch(batch)
         if gram_loss_weight is not None and self._gram is not None:   # gram.loss_weight_schedule[iteration] (:534-537)
             self._gram.weight = float(gram_loss_weight)
+        if dino_local_loss_weight is not None:            # dino.local_loss_weight_schedule[iteration] (:495-501)
+            self.set_dino_local_loss_weight(dino_local_loss_weight)
         self.gram_schedule(self.step_count if iteration is None else int(iteration))
         self.forward_backward(teacher_temp)
         self.optimizer_step(lr, wd, last_layer_lr, momentum)
@@ -586,9 +608,10 @@ class Engine:
         ng, nl = cfg.n_global, cfg.n_local
         g_terms, l_terms = ng * (ng - 1), ng * nl
         g_scale, l_scale = g_terms / (g_terms + l_terms), l_terms / (g_terms + l_terms)
-        loss = (cfg.dino_loss_weight * l_scale * m[0] + cfg.dino_loss_weight * g_scale * m[1]
+        w_local = self.dino_local_loss_weight
+        loss = (cfg.dino_loss_weight * l_scale * w_local * m[0] + cfg.dino_loss_weight * g_scale * m[1]
                 + cfg.koleo_loss_weight * ng * m[2] + cfg.ibot_loss_weight * m[3])
-        out = {"dino_local_crops_loss": m[0], "dino_local_loss_weight": 1.0, "dino_global_crops_loss": m[1],
+        out = {"dino_local_crops_loss": m[0], "dino_local_loss_weight": w_local, "dino_global_crops_loss": m[1],
                "koleo_loss": m[2], "ibot_loss": m[3], "local_batch_size": float(self.B)}
         if self.gram_active:
             loss += self._gram.read(m, out)

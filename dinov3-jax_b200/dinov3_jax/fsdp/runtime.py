@@ -40,6 +40,11 @@ class Comm:
         """out = concat over ranks of inp (tiled all-gather, fsdp/utils.py:66)."""
         return dist.all_gather_into_tensor(out, inp, group=self.group, async_op=async_op)
 
+    def all_to_all(self, out, inp):
+        """Slice q of inp (dim 0 cut into world equal slices) goes to rank q; out = the slices sent to this rank, in
+        rank order."""
+        dist.all_to_all_single(out, inp, group=self.group)
+
     def reduce_scatter_mean(self, out, inp, async_op=False):
         """out = this rank's slice of mean over ranks of inp (psum_scatter / axis_size, fsdp/utils.py:61-64)."""
         if self.backend == "nccl":

@@ -118,20 +118,37 @@ class KoLeoLoss:
 class KoLeoLossDistributed:
     """loss/koleo_loss.py:39-70: nearest neighbours are searched over the rows of ALL ranks (all-gather over "dp"),
     the loss is the mean over the local rows.  The gathered matrix is tiny ([world*B, D]); the neighbour search runs in
-    the same KoLeo kernels on the concatenated rows, and the rows of this rank are picked out of the per-row terms."""
+    the same KoLeo kernels on the concatenated rows, and the rows of this rank are picked out of the per-row terms.
+    With topk > 1 or a `loss_group_size` (images; a multiple of B dividing world*B) the search runs in
+    d3_koleo_topk_rows over this rank's group: the mean over the local rows and their topk neighbours (engine/koleo.py
+    states the semantics)."""
 
     def __init__(self, topk: int = 1, loss_group_size=None, comm=None):
-        if topk != 1:
-            raise NotImplementedError("KoLeoLossDistributed: topk > 1 is not on the GPU path")
-        self.comm, self.loss_group_size = comm, loss_group_size
+        from ..engine.koleo import MAX_TOPK
+        if not 1 <= int(topk) <= MAX_TOPK:
+            raise ValueError(f"KoLeoLossDistributed: topk {topk} must be in [1, {MAX_TOPK}]")
+        self.topk, self.comm, self.loss_group_size = int(topk), comm, loss_group_size
 
     def __call__(self, student_output, eps=1e-8):
         x = student_output.to(f32).contiguous()
         B, D = x.shape
         dev = x.device
-        if self.comm is None or self.comm.world == 1:
+        world, rank = (1, 0) if self.comm is None else (self.comm.world, self.comm.rank)
+        if self.topk > 1 or self.loss_group_size is not None:
+            from ..engine.koleo import ranks_per_group
+            R = ranks_per_group(world, B, self.loss_group_size, self.topk)
+            allx = x
+            if world > 1:
+                allx = torch.empty(world * B, D, device=dev)
+                self.comm.all_gather(allx, x)
+            n = world * B
+            met = torch.zeros(1, device=dev)
+            ops.koleo_topk(allx, ((rank // R) * R * B, R * B), rank * B, B, self.topk,
+                           ops.koleo_topk_scratch(n, D, B, self.topk, dev), met, torch.zeros(n, D, device=dev), 1.0,
+                           0.0, eps)
+            return met[0]
+        if world == 1:
             return KoLeoLoss()(x, eps)
-        world, rank = self.comm.world, self.comm.rank
         allx = torch.empty(world * B, D, device=dev)
         self.comm.all_gather(allx, x)
         n = world * B

@@ -428,6 +428,23 @@ def koleo_fwd_bwd(x, xn, nrm, nn, coef, metric, dx, w_metric, w_grad, eps=1e-8, 
                                            int(nrows), eps, w_metric, w_grad, _s()), "d3_koleo_fwd_bwd_rows")
 
 
+def koleo_topk_scratch(N, D, B, topk, device):
+    """fp32 scratch for koleo_topk: the normalised rows, their norms and the chosen pairs."""
+    return torch.empty(N * D + N + 2 * B * topk, dtype=f32, device=device)
+
+
+def koleo_topk(x, group, row0, B, topk, scratch, metric, dx, w_metric, w_grad, eps=1e-8):
+    """Top-k KoLeo of the gathered rows x [N, D]: local rows [row0, row0 + B) against the other rows of the loss group
+    `group` = (g0, gn).  metric += w_metric * loss; dx [N, D] += w_grad * this rank's gradient for every row."""
+    R, D = x.shape
+    assert x.dtype == f32 and dx.dtype == f32 and dx.shape == x.shape and x.is_contiguous() and dx.is_contiguous()
+    assert scratch.dtype == f32 and metric.dtype == f32
+    g0, gn = group
+    N.check(N.init().d3_koleo_topk_rows(_p(x), R, D, int(g0), int(gn), int(row0), int(B), int(topk), eps, w_metric,
+                                        w_grad, _p(scratch), scratch.numel(), _p(metric), _p(dx), _s()),
+            "d3_koleo_topk_rows")
+
+
 def swiglu_fwd(x12, h):
     """h[T,Hs] = silu(x12[:, :Hs]) * x12[:, Hs:] (bf16)."""
     T, Hs = h.shape

@@ -27,3 +27,29 @@ class CosineScheduler:
 
     def __getitem__(self, it):
         return self.final_value if it >= self.total_iters else self.schedule[it]
+
+
+class linear_warmup_cosine_decay:
+    """Upstream DINOv3's loss-weight (and v2) schedule (cosine_lr_scheduler.py:54-79; the reference passes
+    `endpoit=False` to np.linspace, so it does not run; parity unpinned):
+    [linspace(start, peak, warmup, endpoint=False) | end + (peak - end)(1 + cos(linspace(0, pi, cosine)))/2 | end ...],
+    cosine_iterations defaulting to total - warmup."""
+
+    def __init__(self, start, peak, end, warmup_iterations, total_iterations, cosine_iterations=None):
+        warmup_iterations, total_iterations = int(warmup_iterations), int(total_iterations)
+        if cosine_iterations is None:
+            cosine_iterations = total_iterations - warmup_iterations
+        cosine_iterations = int(cosine_iterations)
+        remaining = total_iterations - cosine_iterations - warmup_iterations
+        if warmup_iterations < 0 or cosine_iterations < 0 or remaining < 0:
+            raise ValueError(f"linear_warmup_cosine_decay: warmup {warmup_iterations} + cosine {cosine_iterations} "
+                             f"iterations exceed the total {total_iterations}")
+        linear = np.linspace(start, peak, warmup_iterations, endpoint=False)
+        cosine = (peak - end) * (np.cos(np.linspace(0, np.pi, cosine_iterations)) + 1) / 2 + end
+        self.schedule = np.concatenate([linear, cosine, np.full((remaining,), fill_value=end)]).astype(np.float64)
+
+    def gen(self):
+        return self.schedule
+
+    def __getitem__(self, idx):
+        return self.schedule[idx]

@@ -8,6 +8,7 @@ from __future__ import annotations
 
 from ..engine import Engine, config_from_reference_cfg, distill_config_from_reference_cfg
 from ..engine.params import lr_wd_multipliers
+from .cosine_lr_scheduler import linear_warmup_cosine_decay
 
 FP8_FILTERS = ("blocks",)
 
@@ -23,6 +24,19 @@ def fp8_from_config(config) -> bool:
         raise NotImplementedError(f"student.fp8_filter={flt!r}: FP8 runs only the block linears (fp8_filter: blocks = "
                                   "attn.qkv, attn.proj and mlp fc1 / fc2 or w1 / w2 / w3 of every block)")
     return True
+
+
+def loss_weight_schedule(config, sc) -> linear_warmup_cosine_decay:
+    """A {start, peak, end, warmup_epochs[, cosine_epochs]} block over OFFICIAL_EPOCH_LENGTH * optim.epochs
+    iterations (train/ssl_meta_arch.py:150-163,183-199)."""
+    if not sc:
+        raise ValueError("a loss-weight schedule needs {start, peak, end, warmup_epochs[, cosine_epochs]}")
+    per_epoch = int(config.train.OFFICIAL_EPOCH_LENGTH)
+    cosine = sc.get("cosine_epochs", None)
+    return linear_warmup_cosine_decay(start=sc.start, peak=sc.peak, end=sc.end,
+                                      warmup_iterations=per_epoch * int(sc.warmup_epochs),
+                                      total_iterations=per_epoch * int(config.optim.epochs),
+                                      cosine_iterations=None if cosine is None else per_epoch * int(cosine))
 
 
 class SSLMetaArch:
@@ -41,6 +55,12 @@ class SSLMetaArch:
         self.dino_loss_weight = config.dino.loss_weight
         self.dino_koleo_loss_weight = config.dino.koleo_loss_weight
         self.ibot_loss_weight = config.ibot.loss_weight
+        # dino.local_loss_weight_schedule (:150-163) and gram.loss_weight_schedule (:183-199): per-iteration weights
+        # that do_train passes to every step; None: the local weight is 1 and the gram weight gram.loss_weight
+        self.dino_local_loss_schedule = (loss_weight_schedule(config, config.dino.local_loss_weight_schedule)
+                                         if config.dino.get("reweight_dino_local_loss", False) else None)
+        gs = config.gram.get("loss_weight_schedule", None)
+        self.gram_loss_schedule = loss_weight_schedule(config, gs) if config.gram.use_loss and gs else None
         # gram anchoring (:165-254): same attribute names and the same configuration errors
         g = config.gram
         self.gram_use_loss = bool(g.use_loss)

@@ -594,6 +594,7 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
     init_reference_like(engine, seed=config.train.seed)
     schedules = build_schedulers(config)
     lr_s, wd_s, mom_s, temp_s, last_s = schedules
+    local_s, gram_s = (getattr(model, a, None) for a in ("dino_local_loss_schedule", "gram_loss_schedule"))
     total = len(lr_s.schedule)
     n_iters = min(total, max_iters) if max_iters else total
     # ---- resume / periodic checkpoints (train/train.py:447-469,695-706; <output_dir>/ckpt/<iteration>)
@@ -632,8 +633,10 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
             data = next(it_loader)
         except StopIteration:
             break
+        local_w, gram_w = (None if s is None else float(s[it]) for s in (local_s, gram_s))
         engine.train_step(data, teacher_temp=float(temp_s[it]), lr=float(lr_s[it]), wd=float(wd_s[it]),
-                          last_layer_lr=float(last_s[it]), momentum=float(mom_s[it]), iteration=it)
+                          last_layer_lr=float(last_s[it]), momentum=float(mom_s[it]), gram_loss_weight=gram_w,
+                          dino_local_loss_weight=local_w, iteration=it)
         if ck_cfg is not None and (it + 1) % int(ck_cfg.period) == 0:
             params_tree, opt_tree = engine_state(engine)                 # collective under FSDP (all-gathers the shards)
             if distributed.is_main_process():

@@ -288,6 +288,17 @@ int d3_resize_tokens_bilinear_aa(const float* src, float* dst, int n, int Hs, in
 int d3_koleo_fwd_bwd_rows(const float* x /*[B,D]*/, float* xn_scratch /*[B,D]*/, float* nrm_scratch /*[B]*/,
                           int* nn_scratch /*[B]*/, float* coef_scratch /*[B]*/, float* metric, float* dx /*[B,D] +=*/,
                           int B, int D, int row0, int nrows, float eps, float w_metric, float w_grad, void* stream);
+/* ---- Top-k KoLeo over gathered rows (dino.koleo_loss_distributed, loss/koleo_loss.py:39-70; parity unpinned) -------
+ * x holds the rows of every rank in rank order.  The loss group is rows [g0, g0+gn); this rank's rows [row0, row0+B)
+ * lie inside it.  Each row is normalised, xn = x/(||x||+eps); local row i takes the topk largest fp32 dots xn_i.xn_j
+ * over the group's other rows (ties to the lower j), and
+ *   metric += w_metric * L,  L = -1/(B topk) sum_{i,s} log(||xn_i - xn_nbr(i,s)|| + eps + eps)
+ *   dx[j]  += w_grad * dL/dx_j for every row j of the group (this rank's contribution; rows outside it untouched).
+ * 1 <= topk <= min(16, gn - 1); D % 4 == 0, D <= 6144; x, dx, scratch 16-byte aligned; scratch holds
+ * N*D + N + 2*B*topk floats.  No atomics: the same bits on every run.                                              */
+int d3_koleo_topk_rows(const float* x /*[N,D]*/, int N, int D, int g0, int gn, int row0, int B, int topk, float eps,
+                       float w_metric, float w_grad, float* scratch, long long scratch_floats, float* metric,
+                       float* dx /*[N,D] +=*/, void* stream);
 
 /* ---- optimiser (train/train.py:516-541 clip, :95-106,562-563 optax.adamw; train/ssl_meta_arch.py:650-652 EMA) -------
  * flat fp32 buffers; segs = array of {int64 start; float lr_mult, wd_mult; int is_last_layer, pad} sorted by start.  */
