@@ -117,6 +117,13 @@ SIGNATURES = {
     "d3_ret_resize": [P, LL, C.POINTER(C.c_longlong), I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, P],
     "d3_ret_scale_sum": [P, I, LL, LL, P, P],
     "d3_ret_rank_ap": [P, LL, I, I] + [C.POINTER(C.c_int)] * 6 + [P, P, P, P, P],
+    "d3_logreg_split_x": [P, I, I, I, I, P, P, P],
+    "d3_logreg_weights": [P, LL, P, I, I, I, P, P, P],
+    "d3_logreg_xent": [P, I, P, P, I, I, I, I, I, F, P, P, I, P],
+    "d3_logreg_finish": [P, P, P, P, P, P, P, I, I, I, P, P, P],
+    "d3_logreg_trial": [P, P, P, P, I, LL, P, P],
+    "d3_logreg_direction": [P, P, P, P, P, P, P, P, I, LL, I, P, P, P],
+    "d3_logreg_accept": [P, P, P, P, P, P, P, P, I, LL, I, P, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

@@ -54,8 +54,9 @@ DEFAULTS = {
     # k-NN (train.do_test), linear-probe (train.do_linear_eval), linear segmentation (train.do_seg_eval), linear depth
     # (train.do_depth_eval), video segmentation (train.do_video_eval, DINO's label-propagation protocol), keypoint
     # correspondence (train.do_correspondence_eval, SPair-71k PCK), unsupervised object discovery
-    # (train.do_discovery_eval, TokenCut CorLoc on VOC) and instance retrieval (train.do_retrieval_eval, revisited
-    # Oxford / Paris mAP) evaluations of the teacher backbone; empty dataset paths: nothing is evaluated.
+    # (train.do_discovery_eval, TokenCut CorLoc on VOC), instance retrieval (train.do_retrieval_eval, revisited
+    # Oxford / Paris mAP) and logistic regression (train.do_logreg_eval; C_values null: 10^linspace(-6, 5, 45))
+    # evaluations of the teacher backbone; empty dataset paths: nothing is evaluated.
     # `config_files` (the reference's list of evaluation configs) is accepted and not read.  The segmentation and depth
     # schedules are this project's defaults, not a published recipe's.
     "evaluation": {"eval_period_iterations": 12500, "config_files": [],
@@ -86,7 +87,11 @@ DEFAULTS = {
                                  "remove_difficult": False, "batch_size": 16, "num_workers": 4, "save_boxes": False},
                    "retrieval": {"dataset_path": "", "dataset": "roxford5k", "image_size": 512,
                                  "scales": [1.0, 0.7071067811865476, 0.5], "batch_size": 16, "num_workers": 4,
-                                 "save_ranks": False}},
+                                 "save_ranks": False},
+                   "logreg": {"train_dataset_path": "", "val_dataset_path": "", "C_values": None,
+                              "holdout_fraction": 0.1, "max_iter": 1000, "tol": 1e-6, "history": 10,
+                              "avgpool": False, "batch_size": 256, "resize_size": 256, "crop_size": 224,
+                              "num_workers": 8, "seed": 0}},
 }
 
 

@@ -3,7 +3,8 @@ class tokens and the patch mean (`linear`), the linear segmentation probe on the
 linear depth probe on the patch and class tokens (`depth`), video object segmentation by label propagation through the
 patch tokens (`video`), keypoint correspondence by nearest neighbour over the upsampled patch tokens
 (`correspondence`), unsupervised object discovery by TokenCut's normalized cut on the patch tokens (`discovery`),
-instance retrieval by the multi-scale class token on revisited Oxford / Paris (`retrieval`), over image, video,
+instance retrieval by the multi-scale class token on revisited Oxford / Paris (`retrieval`), multinomial logistic
+regression on the class token over a grid of regularisation strengths (`logreg`), over image, video,
 keypoint-pair, object-box and retrieval datasets read on the host (`datasets`)."""
 from .correspondence import eval_correspondence
 from .datasets import (ADE20KSegmentation, CorrespondenceNpzDataset, DavisDataset, DepthListDataset, DepthNpzDataset,
@@ -15,6 +16,7 @@ from .discovery import eval_object_discovery
 from .depth import DepthLinearHead, depth_metrics, eval_depth, sample_depth_boxes
 from .knn import KnnClassifier, eval_knn, extract_features
 from .linear import LinearClassifiers, eval_linear
+from .logreg import LogRegSweep, eval_log_regression
 from .retrieval import eval_instance_retrieval
 from .segmentation import SegLinearHead, eval_segmentation
 from .video import eval_video_segmentation
@@ -26,4 +28,4 @@ __all__ = ["ImageFolder", "NpzDataset", "make_eval_dataset", "KnnClassifier", "e
            "make_video_dataset", "eval_video_segmentation", "SPairDataset", "CorrespondenceNpzDataset",
            "make_correspondence_dataset", "eval_correspondence", "VOCDiscoveryDataset", "DiscoveryNpzDataset",
            "make_discovery_dataset", "eval_object_discovery", "RevisitedDataset", "RetrievalNpzDataset",
-           "make_retrieval_dataset", "eval_instance_retrieval"]
+           "make_retrieval_dataset", "eval_instance_retrieval", "LogRegSweep", "eval_log_regression"]

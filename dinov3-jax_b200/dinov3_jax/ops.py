@@ -613,6 +613,84 @@ def sgd_momentum(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, p_bf16: torc
                                      float(momentum), int(bool(first)), _s()), "d3_sgd_momentum")
 
 
+# --------------------------------------------------------------------------------------- logistic regression
+def _i32(t):
+    assert t.dtype == torch.int32 and t.is_contiguous()
+    return _p(t)
+
+
+def logreg_split_x(x: torch.Tensor, chunk: int, xa: torch.Tensor, xg: torch.Tensor | None = None):
+    """xa bf16 [rows, 3K] = [Xh | Xh | Xl] of the fp32 rows x [n, K] and, with xg bf16 [3 rows, K], chunk c of xg =
+    [Xh; Xl; Xh] of its rows (d3_logreg_split_x); rows = n rounded up to whole chunks, padding rows zero."""
+    n, K = x.shape
+    rows = -(-n // chunk) * chunk
+    assert x.dtype == f32 and xa.dtype == bf16 and xa.is_contiguous() and tuple(xa.shape) == (rows, 3 * K)
+    assert xg is None or (xg.dtype == bf16 and xg.is_contiguous() and tuple(xg.shape) == (3 * rows, K))
+    N.check(N.init().d3_logreg_split_x(_p(x), _ld(x), n, K, int(chunk), _p(xa), _p(xg), _s()), "d3_logreg_split_x")
+
+
+def logreg_weights(theta: torch.Tensor, act: torch.Tensor, Cp: int, K: int, wcat: torch.Tensor, bias: torch.Tensor):
+    """wcat bf16 [Ga Cp, 3K] = [Wh | Wl | Wh] and bias fp32 [Ga Cp] of the problems in act (d3_logreg_weights)."""
+    Ga = act.numel()
+    assert theta.dtype == f32 and theta.is_contiguous() and theta.shape[1] == Cp * K + Cp
+    assert wcat.dtype == bf16 and wcat.is_contiguous() and wcat.shape[0] >= Ga * Cp and wcat.shape[1] == 3 * K
+    assert bias.dtype == f32 and bias.is_contiguous() and bias.numel() >= Ga * Cp
+    N.check(N.init().d3_logreg_weights(_p(theta), theta.shape[1], _i32(act), Ga, Cp, K, _p(wcat), _p(bias), _s()),
+            "d3_logreg_weights")
+
+
+def logreg_xent(logits: torch.Tensor, bias: torch.Tensor, labels: torch.Tensor, n: int, Ga: int, C: int, Cp: int,
+                inv_n: float, loss: torch.Tensor, r: torch.Tensor):
+    """One row chunk of the cross-entropy (d3_logreg_xent): logits fp32 [rows, >= Ga Cp], labels int32 [>= n]; loss
+    float64 [Ga] += the chunk's loss / N, r bf16 [3 rows, >= Ga Cp] the split residual."""
+    rows = logits.shape[0]
+    assert logits.dtype == f32 and bias.dtype == f32 and labels.numel() >= n and loss.dtype == torch.float64
+    assert r.dtype == bf16 and r.shape[0] == 3 * rows and loss.is_contiguous() and loss.numel() >= Ga
+    N.check(N.init().d3_logreg_xent(_p(logits), _ld(logits), _p(bias), _i32(labels), int(n), rows, int(Ga), int(C),
+                                    int(Cp), float(inv_n), _p(loss), _p(r), _ld(r), _s()), "d3_logreg_xent")
+
+
+def logreg_finish(theta, gw, gb, loss, icn, d, act, Cp: int, K: int, grad, out):
+    """grad[g] = [gw_a + W_g icn_g | gb_a]; out float64 [Ga, 4] = (objective, grad . d, max |grad|, ||grad||^2)
+    (d3_logreg_finish)."""
+    Ga = act.numel()
+    for t in (theta, gw, gb, icn, grad) + (() if d is None else (d,)):
+        assert t.dtype == f32 and t.is_contiguous()
+    assert loss.dtype == torch.float64 and out.dtype == torch.float64 and out.numel() >= 4 * Ga
+    N.check(N.init().d3_logreg_finish(_p(theta), _p(gw), _p(gb), _p(loss), _p(icn), _p(d), _i32(act), Ga, int(Cp),
+                                      int(K), _p(grad), _p(out), _s()), "d3_logreg_finish")
+
+
+def logreg_trial(theta, d, alpha, act, theta_t):
+    """theta_t[g] = theta[g] + alpha[g] d[g] for the slots in act (d3_logreg_trial)."""
+    for t in (theta, d, alpha, theta_t):
+        assert t.dtype == f32 and t.is_contiguous()
+    N.check(N.init().d3_logreg_trial(_p(theta), _p(d), _p(alpha), _i32(act), act.numel(), theta.shape[1],
+                                     _p(theta_t), _s()), "d3_logreg_trial")
+
+
+def logreg_direction(grad, S, Y, rho, gamma, count, newest, act, d, gd):
+    """d[g] = -H_g grad[g], the L-BFGS two-loop recursion over each slot's history; gd float64 [Ga] = grad . d
+    (d3_logreg_direction)."""
+    G, m, P = S.shape
+    for t in (grad, S, Y, rho, gamma, d):
+        assert t.dtype == f32 and t.is_contiguous()
+    assert gd.dtype == torch.float64 and gd.numel() >= act.numel()
+    N.check(N.init().d3_logreg_direction(_p(grad), _p(S), _p(Y), _p(rho), _p(gamma), _i32(count), _i32(newest),
+                                         _i32(act), act.numel(), P, m, _p(d), _p(gd), _s()), "d3_logreg_direction")
+
+
+def logreg_accept(theta, grad, theta_t, grad_t, S, Y, slot, act, out):
+    """Pair (theta_t - theta, grad_t - grad) into slot[g] of S / Y, theta = theta_t, grad = grad_t; out float64
+    [Ga, 3] = (s.y, y.y, s.s) (d3_logreg_accept)."""
+    G, m, P = S.shape
+    for t in (theta, grad, theta_t, grad_t, S, Y):
+        assert t.dtype == f32 and t.is_contiguous()
+    assert out.dtype == torch.float64 and out.numel() >= 3 * act.numel()
+    N.check(N.init().d3_logreg_accept(_p(theta), _p(grad), _p(theta_t), _p(grad_t), _p(S), _p(Y), _i32(slot),
+                                      _i32(act), act.numel(), P, m, _p(out), _s()), "d3_logreg_accept")
+
+
 # ------------------------------------------------------------------------------------------ segmentation probe
 def seg_max_taps(sizes, resized) -> int:
     """The filter taps of the widest window d3_seg_crop meets for images of (H, W) `sizes` resized to (rh, rw)

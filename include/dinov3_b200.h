@@ -538,6 +538,36 @@ int d3_ret_rank_ap(const float* sim, long long lds, int Q, int N, const int* eas
                    const int* junk_ptr /*host*/, const int* junk_idx /*host*/, int* ranks, double* ap, double* pk,
                    int* n_ok, void* stream);
 
+/* ---- logistic-regression evaluation: L-BFGS over a grid of regularisation strengths (see csrc/logreg.cu) ---------
+ * Problem g's parameters are theta[g] = [W (Cp x K, row-major) | b (Cp)], P = Cp K + Cp floats, in [G, P] buffers
+ * indexed by slot; act (device int [Ga]) lists the slots a launch covers.  Deterministic (no float atomics).
+ * d3_logreg_split_x: x fp32 [n, ldx] -> xa bf16 [rows, 3K] = [Xh | Xh | Xl] and (when xg is given) xg bf16 [3 rows, K],
+ *   chunk c holding [Xh; Xl; Xh] of its rows; rows = n rounded up to whole chunks, padding rows zero.
+ * d3_logreg_weights: wcat bf16 [Ga Cp, 3K] = [Wh | Wl | Wh] per class row, bias fp32 [Ga Cp] (the logits GEMM operand).
+ * d3_logreg_xent: per (row, problem) of a chunk of `rows` rows (the first n real), z = logits + bias: loss[a] (double,
+ *   +=) gets sum_i (lse - z_y) inv_n; r bf16 [3 rows, ld_r] gets the residual (softmax - onehot) inv_n as hi, hi, lo.
+ * d3_logreg_finish: grad[g] = [gw_a + W icn_g | gb_a] (gw fp32 [Ga Cp, K], gb fp32 [Ga Cp]); out double [Ga, 4] = (loss
+ *   + icn ||W||^2 / 2, grad . d (0 without d), max |grad|, ||grad||^2).
+ * d3_logreg_trial: theta_t[g] = theta[g] + alpha[g] d[g] (alpha device fp32 [G]).
+ * d3_logreg_direction: d[g] = -H_g grad[g] by the L-BFGS two-loop recursion over count[g] pairs of S, Y [G, m, P]
+ *   (newest in slot newest[g]), rho [G, m] = 1 / s.y, gamma [G] = s.y / y.y of the newest pair; gd double [Ga] = grad.d.
+ * d3_logreg_accept: S, Y [g, slot[g]] = theta_t - theta, grad_t - grad; theta = theta_t, grad = grad_t; out double
+ *   [Ga, 3] = (s.y, y.y, s.s).  1 <= m <= 64.                                                                       */
+int d3_logreg_split_x(const float* x, int ldx, int n, int K, int chunk, void* xa, void* xg, void* stream);
+int d3_logreg_weights(const float* theta, long long P, const int* act, int Ga, int Cp, int K, void* wcat, float* bias,
+                      void* stream);
+int d3_logreg_xent(const float* logits, int ld, const float* bias, const int* labels, int n, int rows, int Ga, int C,
+                   int Cp, float inv_n, double* loss, void* r, int ld_r, void* stream);
+int d3_logreg_finish(const float* theta, const float* gw, const float* gb, const double* loss, const float* icn,
+                     const float* d, const int* act, int Ga, int Cp, int K, float* grad, double* out, void* stream);
+int d3_logreg_trial(const float* theta, const float* d, const float* alpha, const int* act, int Ga, long long P,
+                    float* theta_t, void* stream);
+int d3_logreg_direction(const float* grad, const float* S, const float* Y, const float* rho, const float* gamma,
+                        const int* count, const int* newest, const int* act, int Ga, long long P, int m, float* d,
+                        double* gd, void* stream);
+int d3_logreg_accept(float* theta, float* grad, const float* theta_t, const float* grad_t, float* S, float* Y,
+                     const int* slot, const int* act, int Ga, long long P, int m, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
