@@ -11,7 +11,7 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent
 CSRC = ROOT / "csrc"
 OUT = ROOT / "libdinov3_b200.so"
-SOURCES = ["api.cu", "gemm_tc.cu", "attention.cu", "elementwise.cu", "losses.cu", "optim.cu", "augment.cu", "convnext.cu", "fp8.cu", "knn.cu", "linear.cu", "seg.cu", "depth.cu", "video.cu", "correspondence.cu", "discovery.cu", "retrieval.cu", "koleo.cu", "logreg.cu"]
+SOURCES = ["api.cu", "gemm_tc.cu", "attention.cu", "elementwise.cu", "losses.cu", "optim.cu", "augment.cu", "convnext.cu", "fp8.cu", "knn.cu", "linear.cu", "seg.cu", "depth.cu", "video.cu", "correspondence.cu", "discovery.cu", "retrieval.cu", "koleo.cu", "logreg.cu", "attentive.cu"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 

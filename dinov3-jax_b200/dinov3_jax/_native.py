@@ -124,6 +124,11 @@ SIGNATURES = {
     "d3_logreg_trial": [P, P, P, P, I, LL, P, P],
     "d3_logreg_direction": [P, P, P, P, P, P, P, P, I, LL, I, P, P, P],
     "d3_logreg_accept": [P, P, P, P, P, P, P, P, I, LL, I, P, P],
+    "d3_atp_query_fwd": [P, P, P, P, I, I, P, P, P],
+    "d3_atp_query_bwd": [P, P, P, P, P, I, I, P, P, P, P, P],
+    "d3_atp_pool_fwd": [P, P, P, P, P, I, I, I, I, I, P, P, P],
+    "d3_atp_pool_bwd": [P, P, P, P, P, P, P, P, I, I, I, I, I, P, P, P, P, P],
+    "d3_atp_gelu_erf_bwd": [P, I, P, I, I, I, P, I, P],
     "d3_sumsq": [P, LL, P, P],
     "d3_ema": [P, P, P, LL, LL, F, P],
     "d3_adamw_ema": [P, P, P, P, P, P, P, LL, P, I, LL, P, F, F, F, F, F, F, F, I, F, P],

@@ -55,10 +55,11 @@ DEFAULTS = {
     # (train.do_depth_eval), video segmentation (train.do_video_eval, DINO's label-propagation protocol), keypoint
     # correspondence (train.do_correspondence_eval, SPair-71k PCK), unsupervised object discovery
     # (train.do_discovery_eval, TokenCut CorLoc on VOC), instance retrieval (train.do_retrieval_eval, revisited
-    # Oxford / Paris mAP) and logistic regression (train.do_logreg_eval; C_values null: 10^linspace(-6, 5, 45))
-    # evaluations of the teacher backbone; empty dataset paths: nothing is evaluated.
-    # `config_files` (the reference's list of evaluation configs) is accepted and not read.  The segmentation and depth
-    # schedules are this project's defaults, not a published recipe's.
+    # Oxford / Paris mAP), logistic regression (train.do_logreg_eval; C_values null: 10^linspace(-6, 5, 45)) and
+    # attentive-probe video classification (train.do_attentive_eval, a V-JEPA-style single-query probe; datasets are
+    # `path label` list files or .npz) evaluations of the teacher backbone; empty dataset paths: nothing is evaluated.
+    # `config_files` (the reference's list of evaluation configs) is accepted and not read.  The segmentation, depth
+    # and attentive-probe schedules are this project's defaults, not a published recipe's.
     "evaluation": {"eval_period_iterations": 12500, "config_files": [],
                    "knn": {"train_dataset_path": "", "val_dataset_path": "", "nb_knn": [10, 20, 100, 200],
                            "temperature": 0.07, "batch_size": 256, "resize_size": 256, "crop_size": 224,
@@ -91,7 +92,11 @@ DEFAULTS = {
                    "logreg": {"train_dataset_path": "", "val_dataset_path": "", "C_values": None,
                               "holdout_fraction": 0.1, "max_iter": 1000, "tol": 1e-6, "history": 10,
                               "avgpool": False, "batch_size": 256, "resize_size": 256, "crop_size": 224,
-                              "num_workers": 8, "seed": 0}},
+                              "num_workers": 8, "seed": 0},
+                   "attentive": {"train_dataset_path": "", "val_dataset_path": "",
+                                 "learning_rates": [1e-4, 3e-4, 1e-3], "epochs": 20, "warmup_epochs": 0,
+                                 "weight_decay": 0.01, "batch_size": 16, "num_frames": 16, "frame_step": 4,
+                                 "num_segments": 2, "num_views": 3, "crop_size": 224, "num_workers": 8, "seed": 0}},
 }
 
 

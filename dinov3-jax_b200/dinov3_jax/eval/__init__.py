@@ -4,14 +4,17 @@ linear depth probe on the patch and class tokens (`depth`), video object segment
 patch tokens (`video`), keypoint correspondence by nearest neighbour over the upsampled patch tokens
 (`correspondence`), unsupervised object discovery by TokenCut's normalized cut on the patch tokens (`discovery`),
 instance retrieval by the multi-scale class token on revisited Oxford / Paris (`retrieval`), multinomial logistic
-regression on the class token over a grid of regularisation strengths (`logreg`), over image, video,
-keypoint-pair, object-box and retrieval datasets read on the host (`datasets`)."""
+regression on the class token over a grid of regularisation strengths (`logreg`), video classification by an attentive
+probe over the frames' patch tokens (`attentive`), over image, video, keypoint-pair, object-box and retrieval datasets
+read on the host (`datasets`)."""
+from .attentive import AttentiveProbe, eval_attentive
 from .correspondence import eval_correspondence
 from .datasets import (ADE20KSegmentation, CorrespondenceNpzDataset, DavisDataset, DepthListDataset, DepthNpzDataset,
                        DiscoveryNpzDataset, ImageFolder, NpzDataset, RetrievalNpzDataset, RevisitedDataset,
-                       SegNpzDataset, SPairDataset, VideoNpzDataset, VOCDiscoveryDataset, make_correspondence_dataset,
-                       make_depth_dataset, make_discovery_dataset, make_eval_dataset, make_retrieval_dataset,
-                       make_seg_dataset, make_video_dataset)
+                       SegNpzDataset, SPairDataset, VideoClassListDataset, VideoClassNpzDataset, VideoNpzDataset,
+                       VOCDiscoveryDataset, make_correspondence_dataset, make_depth_dataset, make_discovery_dataset,
+                       make_eval_dataset, make_retrieval_dataset, make_seg_dataset, make_video_class_dataset,
+                       make_video_dataset)
 from .discovery import eval_object_discovery
 from .depth import DepthLinearHead, depth_metrics, eval_depth, sample_depth_boxes
 from .knn import KnnClassifier, eval_knn, extract_features
@@ -28,4 +31,6 @@ __all__ = ["ImageFolder", "NpzDataset", "make_eval_dataset", "KnnClassifier", "e
            "make_video_dataset", "eval_video_segmentation", "SPairDataset", "CorrespondenceNpzDataset",
            "make_correspondence_dataset", "eval_correspondence", "VOCDiscoveryDataset", "DiscoveryNpzDataset",
            "make_discovery_dataset", "eval_object_discovery", "RevisitedDataset", "RetrievalNpzDataset",
-           "make_retrieval_dataset", "eval_instance_retrieval", "LogRegSweep", "eval_log_regression"]
+           "make_retrieval_dataset", "eval_instance_retrieval", "LogRegSweep", "eval_log_regression",
+           "VideoClassListDataset", "VideoClassNpzDataset", "make_video_class_dataset", "AttentiveProbe",
+           "eval_attentive"]

@@ -2,7 +2,8 @@
 (uint8 HWC RGB, uint8 HW label map), or for depth (uint8 HWC RGB, fp32 HW depth in metres); a video dataset yields
 whole sequences (`DavisDataset`), a correspondence dataset keypoint pairs over its images (`SPairDataset`), a
 discovery dataset images with their object boxes (`VOCDiscoveryDataset`), a retrieval dataset database and query
-images with per-query ground-truth lists (`RevisitedDataset`).  Images
+images with per-query ground-truth lists (`RevisitedDataset`), a video classification dataset the frames of labelled
+videos (`VideoClassListDataset`).  Images
 keep their own sizes, the transforms run on the GPU (`ops.eval_resize_crop`, `ops.seg_crop`, `ops.depth_crop`,
 `ops.video_resize`).  Decoding is host plumbing in DataLoader workers."""
 from __future__ import annotations
@@ -649,3 +650,107 @@ def make_retrieval_dataset(path, dataset: str = "roxford5k"):
     """An .npz file -> RetrievalNpzDataset, a directory -> RevisitedDataset(path, dataset)."""
     path = str(path)
     return RetrievalNpzDataset(path, dataset) if path.endswith(".npz") else RevisitedDataset(path, dataset)
+
+
+class VideoClassListDataset:
+    """A list file of `path label` lines, one per video, paths relative to the list's directory.  A path is a video
+    file, decoded with OpenCV (cv2, imported when a video is read), or a directory of frame images sorted by name.
+    `frame_count(i)` is the container's frame count (a directory's image count); `load_frames(i, indices)` decodes only
+    up to the last index asked for and clamps the indices to the frames actually decoded.  A video that cannot be
+    opened or has no frame is an error naming its path."""
+
+    def __init__(self, path):
+        self.path = str(path)
+        root = os.path.dirname(os.path.abspath(self.path))
+        self.samples = []
+        with open(self.path) as f:
+            for k, line in enumerate(f, 1):
+                if not line.strip():
+                    continue
+                parts = line.rsplit(None, 1)
+                if len(parts) != 2 or not parts[1].lstrip("-").isdigit():
+                    raise ValueError(f"{self.path}:{k}: expected `path label`, got {line.strip()!r}")
+                self.samples.append((os.path.join(root, parts[0].strip()), int(parts[1])))
+        if not self.samples:
+            raise ValueError(f"{self.path}: no videos listed")
+        self.targets = [t for _, t in self.samples]
+
+    def __len__(self):
+        return len(self.samples)
+
+    def _frame_files(self, d):
+        files = sorted(f for f in os.listdir(d) if f.lower().endswith(IMG_EXTENSIONS))
+        if not files:
+            raise ValueError(f"{d}: no frame images")
+        return [os.path.join(d, f) for f in files]
+
+    def frame_count(self, i) -> int:
+        path = self.samples[i][0]
+        if os.path.isdir(path):
+            return len(self._frame_files(path))
+        import cv2
+        cap = cv2.VideoCapture(path)
+        try:
+            if not cap.isOpened():
+                raise ValueError(f"{path}: cannot open the video")
+            return max(int(cap.get(cv2.CAP_PROP_FRAME_COUNT)), 1)
+        finally:
+            cap.release()
+
+    def load_frames(self, i, indices) -> np.ndarray:
+        """uint8 [len(indices), H, W, 3] RGB frames."""
+        path = self.samples[i][0]
+        need = max(int(j) for j in indices)
+        if os.path.isdir(path):
+            from PIL import Image
+            files = self._frame_files(path)
+            frames = {}
+            for j in sorted(set(min(int(j), len(files) - 1) for j in indices)):
+                with Image.open(files[j]) as im:
+                    frames[j] = np.asarray(im.convert("RGB"), dtype=np.uint8)
+            return np.stack([frames[min(int(j), len(files) - 1)] for j in indices])
+        import cv2
+        cap = cv2.VideoCapture(path)
+        try:
+            if not cap.isOpened():
+                raise ValueError(f"{path}: cannot open the video")
+            decoded = []
+            while len(decoded) <= need:
+                ok, frame = cap.read()
+                if not ok:
+                    break
+                decoded.append(frame)
+        finally:
+            cap.release()
+        if not decoded:
+            raise ValueError(f"{path}: no frame could be decoded")
+        return np.stack([cv2.cvtColor(decoded[min(int(j), len(decoded) - 1)], cv2.COLOR_BGR2RGB) for j in indices])
+
+
+class VideoClassNpzDataset:
+    """An .npz file with `videos` (uint8 [N, F, H, W, 3]) and `labels` (integers [N])."""
+
+    def __init__(self, path):
+        with np.load(path, allow_pickle=False) as z:
+            self.videos = np.asarray(z["videos"])
+            self.targets = [int(v) for v in np.asarray(z["labels"]).reshape(-1)]
+        if self.videos.dtype != np.uint8 or self.videos.ndim != 5 or self.videos.shape[-1] != 3:
+            raise ValueError(f"{path}: videos must be uint8 [N, F, H, W, 3], got {self.videos.dtype} "
+                             f"{self.videos.shape}")
+        if len(self.targets) != len(self.videos):
+            raise ValueError(f"{path}: {len(self.videos)} videos but {len(self.targets)} labels")
+
+    def __len__(self):
+        return len(self.targets)
+
+    def frame_count(self, i) -> int:
+        return int(self.videos.shape[1])
+
+    def load_frames(self, i, indices) -> np.ndarray:
+        last = self.videos.shape[1] - 1
+        return self.videos[i][[min(int(j), last) for j in indices]]
+
+
+def make_video_class_dataset(path):
+    """A `.npz` path -> VideoClassNpzDataset; any other path -> VideoClassListDataset (a list file)."""
+    return VideoClassNpzDataset(path) if str(path).endswith(".npz") else VideoClassListDataset(path)

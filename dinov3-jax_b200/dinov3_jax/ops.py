@@ -691,6 +691,64 @@ def logreg_accept(theta, grad, theta_t, grad_t, S, Y, slot, act, out):
                                       _i32(act), act.numel(), P, m, _p(out), _s()), "d3_logreg_accept")
 
 
+# --------------------------------------------------------------------------------------------- attentive probe
+def _f32c(*ts):
+    for t in ts:
+        assert t.dtype == f32 and t.is_contiguous(), "expect contiguous fp32"
+
+
+def atp_query_fwd(q0, Wq, bq, Wk, H: int, q, kt):
+    """q = Wq q0 + bq (fp32 [D]) and the folded keys kt fp32 [H, D] = Wk_h^T q_h / sqrt(D / H) (d3_atp_query_fwd)."""
+    D = q0.numel()
+    _f32c(q0, Wq, bq, Wk, q, kt)
+    assert Wq.shape == (D, D) and Wk.shape == (D, D) and bq.numel() == D and q.numel() == D and kt.shape == (H, D)
+    N.check(N.init().d3_atp_query_fwd(_p(q0), _p(Wq), _p(bq), _p(Wk), D, int(H), _p(q), _p(kt), _s()),
+            "d3_atp_query_fwd")
+
+
+def atp_query_bwd(q0, Wq, Wk, q, dkt, dWq, dbq, dWk, dq0):
+    """From dkt [H, D]: dWk, dWq [D, D] and dbq [D] written, dq0 [D] += Wq^T dq (d3_atp_query_bwd)."""
+    H, D = dkt.shape
+    _f32c(q0, Wq, Wk, q, dkt, dWq, dbq, dWk, dq0)
+    assert dWq.shape == (D, D) and dWk.shape == (D, D) and dbq.numel() == D and dq0.numel() == D
+    N.check(N.init().d3_atp_query_bwd(_p(q0), _p(Wq), _p(Wk), _p(q), _p(dkt), D, H, _p(dWq), _p(dbq), _p(dWk), _p(dq0),
+                                      _s()), "d3_atp_query_bwd")
+
+
+def atp_pool_fwd(x: torch.Tensor, T: int, e, g1, b1, kt, ybar, lse):
+    """The folded pooling (d3_atp_pool_fwd): x bf16 [B, T * P, D] -> ybar fp32 [B, H, D] = sum_n p_{n,h} LN1(x_n + e_t),
+    lse fp32 [B, H]."""
+    B, NT, D = x.shape
+    H = kt.shape[0]
+    assert x.dtype == bf16 and x.is_contiguous() and NT % int(T) == 0
+    _f32c(e, g1, b1, kt, ybar, lse)
+    assert e.shape == (T, D) and g1.numel() == D and b1.numel() == D and ybar.shape == (B, H, D) and lse.shape == (B, H)
+    N.check(N.init().d3_atp_pool_fwd(_p(x), _p(e), _p(g1), _p(b1), _p(kt), B, int(T), NT // int(T), D, H, _p(ybar),
+                                     _p(lse), _s()), "d3_atp_pool_fwd")
+
+
+def atp_pool_bwd(x: torch.Tensor, T: int, e, g1, b1, kt, lse, ybar, dybar, dkt, dg1, db1, de):
+    """The pooling's backward (d3_atp_pool_bwd): from dybar fp32 [B, H, D], dkt [H, D], dg1, db1 [D] and de [T, D]
+    written (summed over the clips)."""
+    B, NT, D = x.shape
+    H = kt.shape[0]
+    assert x.dtype == bf16 and x.is_contiguous() and NT % int(T) == 0
+    _f32c(e, g1, b1, kt, lse, ybar, dybar, dkt, dg1, db1, de)
+    assert ybar.shape == (B, H, D) and dybar.shape == (B, H, D) and lse.shape == (B, H) and dkt.shape == (H, D)
+    assert e.shape == (T, D) and de.shape == (T, D) and dg1.numel() == D and db1.numel() == D
+    N.check(N.init().d3_atp_pool_bwd(_p(x), _p(e), _p(g1), _p(b1), _p(kt), _p(lse), _p(ybar), _p(dybar), B, int(T),
+                                     NT // int(T), D, H, _p(dkt), _p(dg1), _p(db1), _p(de), _s()), "d3_atp_pool_bwd")
+
+
+def atp_gelu_erf_bwd(dh: torch.Tensor, pre: torch.Tensor, out: torch.Tensor):
+    """out bf16 [rows, cols] = dh fp32 * GELU_erf'(pre bf16) (d3_atp_gelu_erf_bwd); row-major views."""
+    rows, cols = dh.shape
+    assert dh.dtype == f32 and pre.dtype == bf16 and out.dtype == bf16
+    assert pre.shape == (rows, cols) and out.shape == (rows, cols)
+    N.check(N.init().d3_atp_gelu_erf_bwd(_p(dh), _ld(dh), _p(pre), _ld(pre), rows, cols, _p(out), _ld(out), _s()),
+            "d3_atp_gelu_erf_bwd")
+
+
 # ------------------------------------------------------------------------------------------ segmentation probe
 def seg_max_taps(sizes, resized) -> int:
     """The filter taps of the widest window d3_seg_crop meets for images of (H, W) `sizes` resized to (rh, rw)

@@ -287,6 +287,13 @@ def _logreg_cfg(config) -> dict:
     return logreg if logreg.get("train_dataset_path") and logreg.get("val_dataset_path") else {}
 
 
+def _attentive_cfg(config) -> dict:
+    """The `evaluation.attentive` block, or {} when it names no train / val dataset (then nothing is evaluated)."""
+    ev = config.get("evaluation", None) or {}
+    att = dict(ev.get("attentive", None) or {})
+    return att if att.get("train_dataset_path") and att.get("val_dataset_path") else {}
+
+
 def eval_backbone(config, weights):
     """The frozen backbone k-NN evaluates, with the architecture of the run's `student.*` config (the depth is the
     number of blocks in the weights).  `weights`: a DinoVisionTransformer (returned as is); a `save_checkpoint`
@@ -624,6 +631,44 @@ def do_logreg_eval(config, model, header):
     return results
 
 
+def do_attentive_eval(config, model, header):
+    """Attentive-probe video classification of the teacher backbone of `model` (see `eval_backbone`) on the
+    `evaluation.attentive` datasets; rank 0 writes <output_dir>/eval/<header>/results_attentive.json and returns
+    {"probes" (per learning rate: val top-1, top-5, mean per-class accuracy), "best_probe", "top1", "top5",
+    "mean_per_class", the train / val video and clip counts, "protocol", "config"} ({} on other ranks).  Without
+    configured datasets it logs one line and returns {}."""
+    import json
+    from .. import distributed
+    att = _attentive_cfg(config)
+    if not att:
+        if distributed.is_main_process():
+            print(f"do_attentive_eval({header}): no evaluation.attentive train / val dataset configured, nothing "
+                  "evaluated", flush=True)
+        return {}
+    backbone = eval_backbone(config, model)            # collective for a live engine under FSDP
+    if not distributed.is_main_process():
+        return {}
+    from ..eval import eval_attentive, make_video_class_dataset
+    c = config.crops
+    kw = {k: att[k] for k in ("learning_rates", "epochs", "warmup_epochs", "weight_decay", "batch_size", "num_frames",
+                              "frame_step", "num_segments", "num_views", "crop_size", "num_workers", "seed") if k in att}
+    results = eval_attentive(backbone, make_video_class_dataset(att["train_dataset_path"]),
+                             make_video_class_dataset(att["val_dataset_path"]),
+                             rgb_mean=c.get("rgb_mean", (0.485, 0.456, 0.406)),
+                             rgb_std=c.get("rgb_std", (0.229, 0.224, 0.225)), **kw)
+    results["protocol"] = ("attentive probe (one query, the backbone's heads, temporal embedding, MLP block, linear "
+                           "classifier) on the last block's patch tokens of every frame; AdamW, cross-entropy, warm-up "
+                           "then cosine; val: mean softmax over segments x views, best learning rate by val top-1")
+    results["config"] = {k: (list(v) if isinstance(v, (list, tuple)) else v) for k, v in att.items()}
+    out_dir = os.path.join(getattr(config.train, "output_dir", None) or ".", "eval", header)
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "results_attentive.json"), "w") as f:
+        json.dump(results, f, indent=1)
+    print(f"do_attentive_eval({header}): {results['best_probe']['name']} top-1 {results['top1']:.2f} top-5 "
+          f"{results['top5']:.2f} mean per-class {results['mean_per_class']:.2f}", flush=True)
+    return results
+
+
 def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None, max_iters: int = 0,
              print_freq: int = 10):
     """train/train.py:319-713.  `data_loader` (optional) yields the reference's collate dicts; by default it is built
@@ -670,8 +715,9 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
     knn_on, linear_on, seg_on = bool(_knn_cfg(config)), bool(_linear_cfg(config)), bool(_seg_cfg(config))
     depth_on, video_on = bool(_depth_cfg(config)), bool(_video_cfg(config))
     corr_on, disc_on = bool(_correspondence_cfg(config)), bool(_discovery_cfg(config))
-    ret_on, logreg_on = bool(_retrieval_cfg(config)), bool(_logreg_cfg(config))
-    any_on = knn_on or linear_on or seg_on or depth_on or video_on or corr_on or disc_on or ret_on or logreg_on
+    ret_on, logreg_on, att_on = bool(_retrieval_cfg(config)), bool(_logreg_cfg(config)), bool(_attentive_cfg(config))
+    any_on = (knn_on or linear_on or seg_on or depth_on or video_on or corr_on or disc_on or ret_on or logreg_on
+              or att_on)
     eval_period = int(ev.get("eval_period_iterations", 0) or 0) if any_on else 0
     for it in range(start_iter, n_iters):
         try:
@@ -709,6 +755,8 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
                 do_retrieval_eval(config, engine, f"training_{it}")
             if logreg_on:
                 do_logreg_eval(config, engine, f"training_{it}")
+            if att_on:
+                do_attentive_eval(config, engine, f"training_{it}")
         if it % print_freq == 0 or it == n_iters - 1:
             m = engine.read_metrics()                  # the only device->host sync of the loop
             if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
@@ -736,10 +784,11 @@ def main(argv=None):
     import random
     import numpy as np
     random.seed(args.seed); np.random.seed(args.seed); torch.manual_seed(args.seed)   # setup_job(seed=args.seed), :281
-    if args.eval not in ("", "knn", "linear", "logreg", "seg", "depth", "video", "correspondence", "discovery",
-                         "retrieval"):
+    if args.eval not in ("", "knn", "linear", "logreg", "attentive", "seg", "depth", "video", "correspondence",
+                         "discovery", "retrieval"):
         raise NotImplementedError(f"--eval {args.eval!r}: the evaluations are k-NN (--eval knn, or empty), the linear "
-                                  "probe (--eval linear), logistic regression (--eval logreg), the linear "
+                                  "probe (--eval linear), logistic regression (--eval logreg), attentive-probe video "
+                                  "classification (--eval attentive), the linear "
                                   "segmentation probe (--eval seg), the linear "
                                   "depth probe (--eval depth), video object segmentation (--eval video) and keypoint "
                                   "correspondence (--eval correspondence), and unsupervised object discovery "
@@ -761,6 +810,8 @@ def main(argv=None):
             return do_linear_eval(config, str(weights), f"manual_{it}")
         if args.eval == "logreg":
             return do_logreg_eval(config, str(weights), f"manual_{it}")
+        if args.eval == "attentive":
+            return do_attentive_eval(config, str(weights), f"manual_{it}")
         if args.eval == "seg":
             return do_seg_eval(config, str(weights), f"manual_{it}")
         if args.eval == "depth":

@@ -568,6 +568,29 @@ int d3_logreg_direction(const float* grad, const float* S, const float* Y, const
 int d3_logreg_accept(float* theta, float* grad, const float* theta_t, const float* grad_t, float* S, float* Y,
                      const int* slot, const int* act, int Ga, long long P, int m, double* out, void* stream);
 
+/* ---- attentive-probe video classification: the probe's single-query pooling folded over the tokens (csrc/attentive.cu)
+ * One learnable query q0 [D] and H heads (dh = D / H): q = Wq q0 + bq, kt [H, D] = Wk_h^T q_h / sqrt(dh) per head (the
+ * keys folded into the query).  Clip tokens x bf16 [B, T * P, D] (T frames of P tokens, frame-major), temporal
+ * embedding e fp32 [T, D], LN1 scale g1 / bias b1 fp32 [D] (eps 1e-6).  Deterministic (no float atomics).
+ * d3_atp_query_fwd: q fp32 [D], kt fp32 [H, D] from fp32 q0, Wq [D, D], bq [D], Wk [D, D] (rows are outputs).
+ * d3_atp_query_bwd: from dkt [H, D]: dWk, dWq [D, D] and dbq [D] written; dq0 [D] += Wq^T dq.
+ * d3_atp_pool_fwd: ybar fp32 [B, H, D] = sum_n p_{n,h} LN1(x_n + e_t(n)), p = softmax_n((LN1(u_n) - b1) . kt_h);
+ *   lse fp32 [B, H] the softmax's log-sum-exp.  8 <= D <= 1536, D % 8 == 0, H | D, x 16-byte aligned.
+ * d3_atp_pool_bwd: from dybar fp32 [B, H, D] (and the forward's ybar, lse): dkt [H, D], dg1, db1 [D] and de [T, D]
+ *   written (summed over the clips).
+ * d3_atp_gelu_erf_bwd: out bf16 [rows, ld_out] = dh fp32 * GELU_erf'(pre bf16).                                     */
+int d3_atp_query_fwd(const float* q0, const float* Wq, const float* bq, const float* Wk, int D, int H, float* q,
+                     float* kt, void* stream);
+int d3_atp_query_bwd(const float* q0, const float* Wq, const float* Wk, const float* q, const float* dkt, int D, int H,
+                     float* dWq, float* dbq, float* dWk, float* dq0, void* stream);
+int d3_atp_pool_fwd(const void* x, const float* e, const float* g1, const float* b1, const float* kt, int B, int T,
+                    int P, int D, int H, float* ybar, float* lse, void* stream);
+int d3_atp_pool_bwd(const void* x, const float* e, const float* g1, const float* b1, const float* kt, const float* lse,
+                    const float* ybar, const float* dybar, int B, int T, int P, int D, int H, float* dkt, float* dg1,
+                    float* db1, float* de, void* stream);
+int d3_atp_gelu_erf_bwd(const float* dh, int ld_dh, const void* pre, int ld_pre, int rows, int cols, void* out,
+                        int ld_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
