@@ -13,6 +13,7 @@
 #include "d3_internal.h"
 #include "resample.cuh"
 
+#include <cstdio>
 #include <type_traits>
 
 namespace d3 {
@@ -29,6 +30,19 @@ struct AugCrop {
 };
 struct AugBlur { float sigma; };   // <= 0: no blur
 
+// one row per source image of a ragged batch (host-filled, 16 bytes): the images' HWC pixels are packed one after the
+// other in one buffer, image i starting at pixel `off`.  A dense [n, H, W, 3] batch has no table (nullptr) and the
+// geometry of image i is computed: a dense batch is a ragged batch of equal sizes.
+struct AugImage {
+  long long off;           // first pixel of the image in the packed buffer (element offset / 3)
+  int h, w;
+};
+static_assert(sizeof(AugImage) == 16, "AugImage is the 16-byte row of the host-filled image table");
+__device__ __forceinline__ AugImage image_of(const AugImage* __restrict__ imgs, int i, int H, int W) {
+  if (imgs) return imgs[i];
+  return AugImage{(long long)i * H * W, H, W};
+}
+
 // out[n, S, S, 3] (fp32, [0,1]) = antialiased bicubic resize of src[img, y0:y0+h, x0:x0+w] (+ horizontal flip).
 // Same definition as torch's _upsample_bicubic2d_aa (align_corners = False): per axis, scale = in/out,
 // support = 2 * max(scale, 1), taps j in [floor(center - support + 0.5), ...), weight cubic((j + 0.5 - center) / max(scale, 1)),
@@ -37,12 +51,13 @@ struct AugBlur { float sigma; };   // <= 0: no blur
 // share_color_jitter, or a base crop resized to the global / gram size).  CLAMP = false is the Resize of a normalised
 // tensor, which torchvision does not clamp.
 template <typename T, bool CLAMP>
-__global__ void aug_resized_crop_kernel(const T* __restrict__ src, int H, int W, const AugCrop* __restrict__ crops,
-                                        float* __restrict__ out, int S) {
+__global__ void aug_resized_crop_kernel(const T* __restrict__ src, const AugImage* __restrict__ imgs, int H, int W,
+                                        const AugCrop* __restrict__ crops, float* __restrict__ out, int S) {
   const int n = blockIdx.z;
   const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y * blockDim.y + threadIdx.y;
   if (ox >= S || oy >= S) return;
   const AugCrop c = crops[n];
+  const AugImage im = image_of(imgs, c.img, H, W);
   const int sx_out = c.flip ? (S - 1 - ox) : ox;        // flip after resize == sample the mirrored column
   const float scx = (float)c.w / S, scy = (float)c.h / S;
   const float isx = 1.f / fmaxf(scx, 1.f), isy = 1.f / fmaxf(scy, 1.f);
@@ -51,11 +66,11 @@ __global__ void aug_resized_crop_kernel(const T* __restrict__ src, int H, int W,
   int xmin, xmax, ymin, ymax;
   const float wxs = aa_window(cx, supx, isx, c.w, c.w, xmin, xmax);
   const float wys = aa_window(cy, supy, isy, c.h, c.h, ymin, ymax);
-  const T* base = src + ((size_t)c.img * H + c.y0) * W * 3 + (size_t)c.x0 * 3;
+  const T* base = src + ((size_t)im.off + (size_t)c.y0 * im.w) * 3 + (size_t)c.x0 * 3;
   float r = 0.f, g = 0.f, b = 0.f;
   for (int y = ymin; y < ymax; ++y) {
     const float wy = cubic_aa<float>((y - cy + 0.5f) * isy);
-    const T* row = base + (size_t)y * W * 3;
+    const T* row = base + (size_t)y * im.w * 3;
     float rr = 0.f, gg = 0.f, bb = 0.f;
     for (int x = xmin; x < xmax; ++x) {
       const float wx = cubic_aa<float>((x - cx + 0.5f) * isx);
@@ -118,16 +133,23 @@ __device__ __forceinline__ void jitter_op(int op, const AugCrop& c, float mean_g
 // Pass A: the jitter ops that come BEFORE contrast in this crop's order, plus the sum of the gray values of the result
 // (contrast blends with the mean gray of the image it is applied to).  Pass B: contrast and what follows, then
 // RandomGrayscale.  A crop without jitter / without a pending contrast simply passes through pass A untouched.
-// SQUARE: x holds S x S crops; otherwise S is the pixel count of each image (whole H x W sources).
-template <bool SQUARE>
-__global__ void aug_color_a_kernel(float* __restrict__ x, const AugCrop* __restrict__ crops, float* __restrict__ gray_sum,
-                                   int S) {
+// x holds n images of `npix` pixels each (S x S crops, or whole H x W sources), or with an image table the ragged
+// sources of a batch, each jittered with its own pixel count.
+__device__ __forceinline__ void color_geometry(const AugImage* __restrict__ imgs, int n, int npix, long long& off,
+                                               int& count) {
+  if (imgs) { const AugImage im = imgs[n]; off = im.off; count = im.h * im.w; }
+  else { off = (long long)n * npix; count = npix; }
+}
+__global__ void aug_color_a_kernel(float* __restrict__ x, const AugImage* __restrict__ imgs,
+                                   const AugCrop* __restrict__ crops, float* __restrict__ gray_sum, int npix_dense) {
   const int n = blockIdx.y;
   const AugCrop c = crops[n];
-  const int npix = SQUARE ? S * S : S;
+  long long off;
+  int npix;
+  color_geometry(imgs, n, npix_dense, off, npix);
   float local = 0.f;
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
-    float* px = x + ((size_t)n * npix + p) * 3;
+    float* px = x + ((size_t)off + p) * 3;
     float r = px[0], g = px[1], b = px[2];
     if (c.order[0] >= 0)
       for (int k = 0; k < 4 && c.order[k] != 1; ++k) jitter_op(c.order[k], c, 0.f, r, g, b);
@@ -138,15 +160,16 @@ __global__ void aug_color_a_kernel(float* __restrict__ x, const AugCrop* __restr
   for (int o = 16; o > 0; o >>= 1) local += __shfl_xor_sync(0xffffffffu, local, o);
   if ((threadIdx.x & 31) == 0) atomicAdd(&gray_sum[n], local);
 }
-template <bool SQUARE>
-__global__ void aug_color_b_kernel(float* __restrict__ x, const AugCrop* __restrict__ crops,
-                                   const float* __restrict__ gray_sum, int S) {
+__global__ void aug_color_b_kernel(float* __restrict__ x, const AugImage* __restrict__ imgs,
+                                   const AugCrop* __restrict__ crops, const float* __restrict__ gray_sum, int npix_dense) {
   const int n = blockIdx.y;
   const AugCrop c = crops[n];
-  const int npix = SQUARE ? S * S : S;
+  long long off;
+  int npix;
+  color_geometry(imgs, n, npix_dense, off, npix);
   const float mean_gray = gray_sum[n] / npix;
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
-    float* px = x + ((size_t)n * npix + p) * 3;
+    float* px = x + ((size_t)off + p) * 3;
     float r = px[0], g = px[1], b = px[2];
     if (c.order[0] >= 0) {
       int k = 0;
@@ -307,21 +330,60 @@ using namespace d3;
 
 extern "C" {
 
+// One launch of aug_resized_crop_kernel for every entry point: imgs = nullptr reads a dense [n_img, H, W, 3] batch.
+static int launch_resized_crop(const void* src, bool f32, int clamp, const AugImage* imgs, int H, int W,
+                               const void* crops, int n_crops, float* out, int S, void* stream) {
+  dim3 block(32, 8), grid((S + 31) / 32, (S + 7) / 8, n_crops);
+  const AugCrop* c = (const AugCrop*)crops;
+  if (!f32)
+    aug_resized_crop_kernel<uint8_t, true><<<grid, block, 0, STREAM(stream)>>>((const uint8_t*)src, imgs, H, W, c, out, S);
+  else if (clamp)
+    aug_resized_crop_kernel<float, true><<<grid, block, 0, STREAM(stream)>>>((const float*)src, imgs, H, W, c, out, S);
+  else
+    aug_resized_crop_kernel<float, false><<<grid, block, 0, STREAM(stream)>>>((const float*)src, imgs, H, W, c, out, S);
+  D3_CHECK_LAUNCH();
+  return D3_OK;
+}
+
+// Argument checks of the ragged entry points, before any CUDA call.  The crop records are read from their host copy:
+// every crop must name a row of the image table (its box is checked against that image's size by the caller, which
+// drew it).
+static int check_ragged(const char* what, const void* src, const void* imgs, int n_img, const void* crops,
+                        const void* crops_host, int n_crops, const void* out, int S) {
+  char buf[160];
+  if (!src || !imgs || !crops || !crops_host || !out) snprintf(buf, sizeof(buf), "%s: null pointer", what);
+  else if (n_img < 1) snprintf(buf, sizeof(buf), "%s: n_img < 1", what);
+  else if (S < 5) snprintf(buf, sizeof(buf), "%s: S < 5", what);
+  else {
+    const AugCrop* c = (const AugCrop*)crops_host;
+    int i = 0;
+    while (i < n_crops && c[i].img >= 0 && c[i].img < n_img) ++i;
+    if (i == n_crops) return D3_OK;
+    snprintf(buf, sizeof(buf), "%s: crop %d reads image %d of a %d-image table", what, i, c[i].img, n_img);
+  }
+  return set_error(D3_ERR_ARG, buf);
+}
+
 int d3_aug_resized_crop(const void* src_u8, int n_img, int H, int W, const void* crops, int n_crops, float* out, int S,
                         void* stream) {
   if (n_crops <= 0) return D3_OK;
   if (S < 5 || H <= 0 || W <= 0 || n_img <= 0) return set_error(D3_ERR_ARG, "d3_aug_resized_crop: bad geometry");
-  dim3 block(32, 8), grid((S + 31) / 32, (S + 7) / 8, n_crops);
-  aug_resized_crop_kernel<uint8_t, true><<<grid, block, 0, STREAM(stream)>>>((const uint8_t*)src_u8, H, W, (const AugCrop*)crops, out, S);
-  D3_CHECK_LAUNCH();
-  return D3_OK;
+  return launch_resized_crop(src_u8, false, 1, nullptr, H, W, crops, n_crops, out, S, stream);
+}
+
+int d3_aug_resized_crop_ragged(const void* src_u8, const void* imgs, int n_img, const void* crops, const void* crops_host,
+                               int n_crops, float* out, int S, void* stream) {
+  if (n_crops <= 0) return D3_OK;
+  if (int rc = check_ragged("d3_aug_resized_crop_ragged", src_u8, imgs, n_img, crops, crops_host, n_crops, out, S))
+    return rc;
+  return launch_resized_crop(src_u8, false, 1, (const AugImage*)imgs, 0, 0, crops, n_crops, out, S, stream);
 }
 
 int d3_aug_color(float* x, const void* crops, int n_crops, int S, float* gray_sum /* [n_crops] zeroed */, void* stream) {
   if (n_crops <= 0) return D3_OK;
   dim3 grid(min((S * S + 255) / 256, 64), n_crops);
-  aug_color_a_kernel<true><<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)crops, gray_sum, S);
-  aug_color_b_kernel<true><<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)crops, gray_sum, S);
+  aug_color_a_kernel<<<grid, 256, 0, STREAM(stream)>>>(x, nullptr, (const AugCrop*)crops, gray_sum, S * S);
+  aug_color_b_kernel<<<grid, 256, 0, STREAM(stream)>>>(x, nullptr, (const AugCrop*)crops, gray_sum, S * S);
   D3_CHECK_LAUNCH();
   count_launch(1);
   return D3_OK;
@@ -352,12 +414,27 @@ int d3_aug_resized_crop_f32(const float* src, int n_img, int H, int W, const voi
                             int clamp, void* stream) {
   if (n_crops <= 0) return D3_OK;
   if (S < 5 || H <= 0 || W <= 0 || n_img <= 0) return set_error(D3_ERR_ARG, "d3_aug_resized_crop_f32: bad geometry");
-  dim3 block(32, 8), grid((S + 31) / 32, (S + 7) / 8, n_crops);
-  if (clamp)
-    aug_resized_crop_kernel<float, true><<<grid, block, 0, STREAM(stream)>>>(src, H, W, (const AugCrop*)crops, out, S);
-  else
-    aug_resized_crop_kernel<float, false><<<grid, block, 0, STREAM(stream)>>>(src, H, W, (const AugCrop*)crops, out, S);
+  return launch_resized_crop(src, true, clamp, nullptr, H, W, crops, n_crops, out, S, stream);
+}
+
+int d3_aug_resized_crop_ragged_f32(const float* src, const void* imgs, int n_img, const void* crops,
+                                   const void* crops_host, int n_crops, float* out, int S, int clamp, void* stream) {
+  if (n_crops <= 0) return D3_OK;
+  if (int rc = check_ragged("d3_aug_resized_crop_ragged_f32", src, imgs, n_img, crops, crops_host, n_crops, out, S))
+    return rc;
+  return launch_resized_crop(src, true, clamp, (const AugImage*)imgs, 0, 0, crops, n_crops, out, S, stream);
+}
+
+// share_color_jitter: fp32 copy of the n_pix packed source pixels, then the jitter of each whole image with its record
+static int color_images(const uint8_t* src, long long n_pix, const AugImage* imgs, int n_img, int npix_dense,
+                        const void* recs, float* x, float* gray_sum, int blocks_per_image, void* stream) {
+  const long long n = n_pix * 3;
+  aug_u8_to_f32_kernel<<<(int)std::min<long long>((n + 255) / 256, 4096), 256, 0, STREAM(stream)>>>(src, x, n);
+  dim3 grid(blocks_per_image, n_img);
+  aug_color_a_kernel<<<grid, 256, 0, STREAM(stream)>>>(x, imgs, (const AugCrop*)recs, gray_sum, npix_dense);
+  aug_color_b_kernel<<<grid, 256, 0, STREAM(stream)>>>(x, imgs, (const AugCrop*)recs, gray_sum, npix_dense);
   D3_CHECK_LAUNCH();
+  count_launch(2);
   return D3_OK;
 }
 
@@ -365,15 +442,15 @@ int d3_aug_color_images(const void* src_u8, int n_img, int H, int W, const void*
                         void* stream) {
   if (n_img <= 0) return D3_OK;
   if (H <= 0 || W <= 0) return set_error(D3_ERR_ARG, "d3_aug_color_images: bad geometry");
-  const long long n = (long long)n_img * H * W * 3;
-  aug_u8_to_f32_kernel<<<(int)std::min<long long>((n + 255) / 256, 4096), 256, 0, STREAM(stream)>>>(
-      (const uint8_t*)src_u8, x, n);
-  dim3 grid(min((H * W + 255) / 256, 64), n_img);
-  aug_color_a_kernel<false><<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)recs, gray_sum, H * W);
-  aug_color_b_kernel<false><<<grid, 256, 0, STREAM(stream)>>>(x, (const AugCrop*)recs, gray_sum, H * W);
-  D3_CHECK_LAUNCH();
-  count_launch(2);
-  return D3_OK;
+  return color_images((const uint8_t*)src_u8, (long long)n_img * H * W, nullptr, n_img, H * W, recs, x, gray_sum,
+                      min((H * W + 255) / 256, 64), stream);
+}
+
+int d3_aug_color_images_ragged(const void* src_u8, long long n_pix, const void* imgs, int n_img, const void* recs,
+                               const void* recs_host, float* x, float* gray_sum, void* stream) {
+  if (int rc = check_ragged("d3_aug_color_images_ragged", src_u8, imgs, n_img, recs, recs_host, n_img, x, 5)) return rc;
+  if (!gray_sum || n_pix < 1) return set_error(D3_ERR_ARG, "d3_aug_color_images_ragged: null gray_sum or n_pix < 1");
+  return color_images((const uint8_t*)src_u8, n_pix, (const AugImage*)imgs, n_img, 0, recs, x, gray_sum, 64, stream);
 }
 
 int d3_aug_solarize(float* x, const void* crops, int n_crops, int S, void* stream) {

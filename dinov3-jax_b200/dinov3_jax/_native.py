@@ -89,6 +89,9 @@ SIGNATURES = {
     "d3_aug_color_images": [P, I, I, I, P, P, P, P],
     "d3_aug_solarize": [P, P, I, I, P],
     "d3_aug_local_windows": [P, I, I, P, P, I, I, P, P, P, P, P],
+    "d3_aug_resized_crop_ragged": [P, P, I, P, P, I, P, I, P],
+    "d3_aug_resized_crop_ragged_f32": [P, P, I, P, P, I, P, I, I, P],
+    "d3_aug_color_images_ragged": [P, LL, P, I, P, P, P, P, P],
     "d3_eval_resize_crop": [P, P, I, I, I, I, C.POINTER(C.c_float), C.POINTER(C.c_float), P, I, P],
     "d3_knn_normalize": [P, I, I, I, P, P, I, P],
     "d3_topk_merge": [P, LL, I, I, I, P, P, I, I, I, P],

@@ -29,6 +29,11 @@ The other options of the reference constructor follow data/augmentations.py:70-2
   share_color_jitter             one ColorJitter + RandomGrayscale per source image, before any crop; no per-crop jitter
   teacher_no_color_jitter        only fills `global_crops_teacher`, which the collate never reads: no effect on the batch
 
+A batch is either a dense [B, H, W, 3] uint8 tensor or a `RaggedImages`: B images of their own sizes packed into one
+buffer, as a real dataset decodes them.  Each image's crop boxes are drawn from its own size, and the first crop reads
+it in place (csrc/augment.cu: a dense batch is a ragged batch of equal sizes); everything after that first crop works
+on dense crops.
+
 The kernels (csrc/augment.cu) are deterministic functions of those parameters and are tested against torchvision's
 float implementations.  `GpuBatchPipeline` adds the iBOT block masks (host `MaskingGenerator`, as in the reference's
 collate) and yields the batch dict `Engine.set_batch` consumes.
@@ -49,6 +54,8 @@ CROP_DTYPE = np.dtype([("img", "<i4"), ("x0", "<i4"), ("y0", "<i4"), ("w", "<i4"
                        ("order", "<i4", (4,)), ("fb", "<f4"), ("fc", "<f4"), ("fs", "<f4"), ("fh", "<f4"),
                        ("gray", "<i4"), ("solarize", "<i4")])
 assert CROP_DTYPE.itemsize == 64
+IMAGE_DTYPE = np.dtype([("off", "<i8"), ("h", "<i4"), ("w", "<i4")])      # one row of a ragged batch's image table
+assert IMAGE_DTYPE.itemsize == 16
 
 IMAGENET_DEFAULT_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_DEFAULT_STD = (0.229, 0.224, 0.225)
@@ -73,6 +80,53 @@ def _resized_crop_params(rng, H, W, scale, ratio=(3.0 / 4.0, 4.0 / 3.0)):
     else:
         w, h = W, H
     return (H - h) // 2, (W - w) // 2, h, w
+
+
+class RaggedImages:
+    """B images of their own sizes: `data` is one 1-D buffer holding each image's HWC pixels in turn (uint8, or fp32 in
+    [0, 1]), `sizes` their (H, W).  `table` is the image table the kernels read, with each image's first pixel."""
+
+    def __init__(self, data: torch.Tensor, sizes):
+        self.data = data
+        self.sizes = np.asarray(sizes, dtype=np.int64).reshape(-1, 2)
+        assert (self.sizes > 0).all(), "every image needs at least one pixel"
+        pix = self.sizes[:, 0] * self.sizes[:, 1]
+        self.table = np.zeros(len(self.sizes), dtype=IMAGE_DTYPE)
+        self.table["off"][1:] = np.cumsum(pix)[:-1]
+        self.table["h"], self.table["w"] = self.sizes[:, 0], self.sizes[:, 1]
+        self.n_pix = int(pix.sum())
+        assert data.dim() == 1 and data.numel() == 3 * self.n_pix, (tuple(data.shape), self.n_pix)
+        self._d_table = None
+
+    @classmethod
+    def from_images(cls, images, device=None) -> "RaggedImages":
+        """Pack a list of [H, W, 3] tensors or arrays (one dtype) into one buffer on `device`."""
+        ts = [torch.as_tensor(im) for im in images]
+        data = torch.cat([t.reshape(-1) for t in ts])
+        return cls(data if device is None else data.to(device), [t.shape[:2] for t in ts])
+
+    def __len__(self):
+        return len(self.sizes)
+
+    def with_data(self, data: torch.Tensor) -> "RaggedImages":
+        """The same images' layout over another buffer (the fp32 jittered copy of share_color_jitter)."""
+        out = RaggedImages(data, self.sizes)
+        out._d_table = self._d_table if data.device == self.device else None
+        return out
+
+    @property
+    def device(self):
+        return self.data.device
+
+    def image(self, i: int) -> torch.Tensor:
+        """Image i as an [H, W, 3] view of the buffer."""
+        o, (h, w) = int(self.table["off"][i]), self.sizes[i]
+        return self.data[3 * o:3 * (o + h * w)].view(int(h), int(w), 3)
+
+    def d_table(self) -> torch.Tensor:
+        if self._d_table is None:
+            self._d_table = torch.from_numpy(self.table.view(np.uint8).reshape(-1).copy()).to(self.device, non_blocking=True)
+        return self._d_table
 
 
 class GpuDataAugmentationDINO:
@@ -117,19 +171,21 @@ class GpuDataAugmentationDINO:
             rec["order"][i] = -1
         rec["gray"][i] = int(rng.random() < 0.2)
 
-    def sample(self, B: int, H: int, W: int):
+    def sample(self, B: int, H, W):
         """Crop records (crop-major: crop index outer, image inner, like the collate's stacking) and blur sigmas for the
         2 global and n_local local crop sets.  The global records' boxes are the base crops at `base_size`.  With
         local_crops_subset_of_global_crops a local record is a window: img = its base crop's row in the global records,
-        (y0, x0) = (rx, ry), w = h = local size, no flip of its own."""
+        (y0, x0) = (rx, ry), w = h = local size, no flip of its own.  H and W are the images' sizes: one int for the
+        whole batch, or one per image; each image's boxes are drawn from its own size, with the same draws either way."""
         rng = self.rng
+        Hs, Ws = (np.broadcast_to(np.asarray(v, dtype=np.int64), (B,)) for v in (H, W))
         g = np.zeros(2 * B, dtype=CROP_DTYPE)
         l = np.zeros(self.n_local * B, dtype=CROP_DTYPE)
         gb = np.zeros(2 * B, dtype=np.float32)
         lb = np.zeros(self.n_local * B, dtype=np.float32)
 
         def fill(rec, i, img, scale, blur_apply_p, solarize_p, sig):
-            y0, x0, h, w = _resized_crop_params(rng, H, W, scale)
+            y0, x0, h, w = _resized_crop_params(rng, int(Hs[img]), int(Ws[img]), scale)
             rec["img"][i], rec["x0"][i], rec["y0"][i], rec["w"][i], rec["h"][i] = img, x0, y0, w, h
             rec["flip"][i] = int(rng.random() < self.flip_p)
             if self.share_color_jitter:
@@ -179,11 +235,28 @@ class GpuDataAugmentationDINO:
     def _dev(records: np.ndarray, dev):
         return torch.from_numpy(records.view(np.uint8).reshape(-1).copy()).to(dev, non_blocking=True)
 
-    def _crop(self, src: torch.Tensor, d_crops, n: int, S: int, key, clamp: bool = True) -> torch.Tensor:
-        """[n, S, S, 3] fp32 resized crops of src (uint8 images, or fp32 [0,1] images)."""
+    def _crop(self, src, crops: np.ndarray, d_crops, S: int, key, clamp: bool = True) -> torch.Tensor:
+        """[n, S, S, 3] fp32 resized crops of src (uint8 images, or fp32 [0,1] images; dense or RaggedImages) by the
+        host records `crops`, whose device copy is d_crops."""
         lib = N.init()
-        B, H, W, _ = src.shape
+        n = crops.shape[0]
         x = self._buf((key, S), (n, S, S, 3), torch.float32, src.device)
+        if isinstance(src, RaggedImages):
+            hw = src.sizes[crops["img"]]
+            assert ((crops["img"] >= 0) & (crops["img"] < len(src))).all()
+            assert ((crops["x0"] >= 0) & (crops["y0"] >= 0) & (crops["w"] > 0) & (crops["h"] > 0)
+                    & (crops["x0"] + crops["w"] <= hw[:, 1]) & (crops["y0"] + crops["h"] <= hw[:, 0])).all(), \
+                "a crop box reaches outside its image"
+            h_crops = crops.ctypes.data_as(C.c_void_p)
+            if src.data.dtype == torch.uint8:
+                N.check(lib.d3_aug_resized_crop_ragged(N.ptr(src.data), N.ptr(src.d_table()), len(src), N.ptr(d_crops),
+                                                       h_crops, n, N.ptr(x), S, N.stream_ptr()), "d3_aug_resized_crop_ragged")
+            else:
+                N.check(lib.d3_aug_resized_crop_ragged_f32(N.ptr(src.data), N.ptr(src.d_table()), len(src), N.ptr(d_crops),
+                                                           h_crops, n, N.ptr(x), S, int(clamp), N.stream_ptr()),
+                        "d3_aug_resized_crop_ragged_f32")
+            return x
+        B, H, W, _ = src.shape
         if src.dtype == torch.uint8:
             N.check(lib.d3_aug_resized_crop(N.ptr(src), B, H, W, N.ptr(d_crops), n, N.ptr(x), S, N.stream_ptr()),
                     "d3_aug_resized_crop")
@@ -197,7 +270,8 @@ class GpuDataAugmentationDINO:
         n, M = x.shape[0], x.shape[1]
         if M == S:
             return x
-        return self._crop(x, self._dev(self._whole(n, M), x.device), n, S, key, clamp)
+        whole = self._whole(n, M)
+        return self._crop(x, whole, self._dev(whole, x.device), S, key, clamp)
 
     @staticmethod
     def _whole(n: int, M: int) -> np.ndarray:
@@ -228,21 +302,34 @@ class GpuDataAugmentationDINO:
         N.check(lib.d3_aug_blur(N.ptr(x), N.ptr(t1), N.ptr(t2), N.ptr(d_sig), n, S, s), "d3_aug_blur")
         return self._finish(t2, d_crops) if finish else t2
 
-    def apply(self, images_u8: torch.Tensor, crops: np.ndarray, sigmas: np.ndarray, S: int) -> torch.Tensor:
-        """images_u8 [B,H,W,3] uint8 on the GPU (or the fp32 jittered sources of share_color_jitter); returns
-        [n_crops, S, S, 3] bf16 (normalised)."""
-        assert images_u8.dtype in (torch.uint8, torch.float32) and images_u8.is_cuda and images_u8.is_contiguous() \
-            and images_u8.shape[-1] == 3
-        d_crops = self._dev(crops, images_u8.device)
-        return self._distort(self._crop(images_u8, d_crops, crops.shape[0], S, "x"), d_crops, sigmas)
+    def apply(self, images_u8, crops: np.ndarray, sigmas: np.ndarray, S: int) -> torch.Tensor:
+        """images_u8 [B,H,W,3] uint8 on the GPU, or a RaggedImages (or the fp32 jittered sources of
+        share_color_jitter); returns [n_crops, S, S, 3] bf16 (normalised)."""
+        data = images_u8.data if isinstance(images_u8, RaggedImages) else images_u8
+        assert data.dtype in (torch.uint8, torch.float32) and data.is_cuda and data.is_contiguous()
+        assert isinstance(images_u8, RaggedImages) or images_u8.shape[-1] == 3
+        d_crops = self._dev(crops, data.device)
+        return self._distort(self._crop(images_u8, crops, d_crops, S, "x"), d_crops, sigmas)
 
-    def jitter_sources(self, images_u8: torch.Tensor, recs: np.ndarray) -> torch.Tensor:
-        """share_color_jitter: fp32 [B,H,W,3] copy of the sources, each jittered with its record."""
-        B, H, W, _ = images_u8.shape
+    def jitter_sources(self, images_u8, recs: np.ndarray):
+        """share_color_jitter: fp32 copy of the sources, each jittered with its record: [B,H,W,3] for a dense batch, a
+        RaggedImages with the same layout for a ragged one (contrast takes each image's own mean gray)."""
         dev = images_u8.device
+        d_recs = self._dev(recs, dev)
+        if isinstance(images_u8, RaggedImages):
+            B = len(images_u8)
+            n = 3 * images_u8.n_pix                             # one buffer that grows to the largest batch seen
+            if self._scratch.get("src_ragged") is None or self._scratch["src_ragged"].numel() < n:
+                self._scratch["src_ragged"] = torch.empty(n, dtype=torch.float32, device=dev)
+            x = self._scratch["src_ragged"][:n]
+            gsum = torch.zeros(B, dtype=torch.float32, device=dev)
+            N.check(N.init().d3_aug_color_images_ragged(N.ptr(images_u8.data), images_u8.n_pix, N.ptr(images_u8.d_table()),
+                                                        B, N.ptr(d_recs), recs.ctypes.data_as(C.c_void_p), N.ptr(x),
+                                                        N.ptr(gsum), N.stream_ptr()), "d3_aug_color_images_ragged")
+            return images_u8.with_data(x)
+        B, H, W, _ = images_u8.shape
         x = self._buf(("src", H, W), (B, H, W, 3), torch.float32, dev)
         gsum = torch.zeros(B, dtype=torch.float32, device=dev)
-        d_recs = self._dev(recs, dev)
         N.check(N.init().d3_aug_color_images(N.ptr(images_u8), B, H, W, N.ptr(d_recs), N.ptr(x), N.ptr(gsum),
                                              N.stream_ptr()), "d3_aug_color_images")
         return x
@@ -264,8 +351,12 @@ class GpuDataAugmentationDINO:
                                               N.ptr(tmp), N.ptr(y), N.ptr(gsum), N.stream_ptr()), "d3_aug_local_windows")
         return self._finish(y, d_crops)
 
-    def __call__(self, images_u8: torch.Tensor) -> dict:
-        B, H, W, _ = images_u8.shape
+    def __call__(self, images_u8) -> dict:
+        """images_u8: a dense [B, H, W, 3] uint8 tensor on the GPU, or a RaggedImages of uint8 images there."""
+        if isinstance(images_u8, RaggedImages):
+            B, H, W = len(images_u8), images_u8.sizes[:, 0], images_u8.sizes[:, 1]
+        else:
+            B, H, W, _ = images_u8.shape
         src = images_u8
         if self.share_color_jitter:
             src = self.jitter_sources(images_u8, self.sample_source_jitter(B))
@@ -276,7 +367,7 @@ class GpuDataAugmentationDINO:
         # base crops at max(global, gram); what reads the undistorted base runs before the jitter works in place on it
         dev = images_u8.device
         d_g = self._dev(g, dev)
-        base = self._crop(src, d_g, 2 * B, self.base_size, "base")
+        base = self._crop(src, g, d_g, self.base_size, "base")
         out = {"collated_local_crops": self.local_windows(base, l, lb) if self.subset else self.apply(src, l, lb, self.ls)}
         if self.gram is None:
             out["collated_global_crops"] = self._distort(base, d_g, gb)
@@ -294,7 +385,7 @@ class GpuDataAugmentationDINO:
 
 
 class GpuBatchPipeline:
-    """uint8 image batch on the GPU -> the batch dict of data/collate.py:72-93 (crops from the kernels above, iBOT block
+    """uint8 image batch on the GPU (dense or ragged) -> the batch dict of data/collate.py:72-93 (crops from the kernels above, iBOT block
     masks from the reference's host generator as in its collate).  `config` is the reference-shaped config."""
 
     def __init__(self, config, seed: int = 0):
@@ -317,10 +408,11 @@ class GpuBatchPipeline:
         self.mask_probability = config.ibot.mask_sample_probability
         self.circular = bool(config.ibot.get("mask_random_circular_shift", False))
 
-    def __call__(self, images_u8: torch.Tensor) -> dict:
+    def __call__(self, images_u8) -> dict:
+        """images_u8: a dense [B, H, W, 3] uint8 tensor on the GPU, or a RaggedImages of uint8 images there."""
         out = self.aug(images_u8)
         n_global = out["collated_global_crops"].shape[0]
         out.update(collate_masks(n_global, self.n_tokens, self.mask_ratio, self.mask_probability, self.mask_generator,
                                  self.circular))
-        out["global_batch_size"] = images_u8.shape[0]
+        out["global_batch_size"] = len(images_u8)
         return out

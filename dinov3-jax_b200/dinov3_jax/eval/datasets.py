@@ -13,7 +13,7 @@ import pickle
 
 import numpy as np
 
-IMG_EXTENSIONS = (".jpg", ".jpeg", ".png", ".ppm", ".bmp", ".pgm", ".tif", ".tiff", ".webp")
+from ..data.image_loader import IMG_EXTENSIONS, decode_rgb, list_images
 
 
 class ImageFolder:
@@ -28,19 +28,15 @@ class ImageFolder:
         self.class_to_idx = {c: i for i, c in enumerate(self.classes)}
         self.samples = []
         for c in self.classes:
-            for d, _, files in sorted(os.walk(os.path.join(self.root, c), followlinks=True)):
-                self.samples += [(os.path.join(d, f), self.class_to_idx[c]) for f in sorted(files)
-                                 if f.lower().endswith(IMG_EXTENSIONS)]
+            self.samples += [(p, self.class_to_idx[c]) for p in list_images(os.path.join(self.root, c))]
         self.targets = [t for _, t in self.samples]
 
     def __len__(self):
         return len(self.samples)
 
     def __getitem__(self, i):
-        from PIL import Image
         path, target = self.samples[i]
-        with Image.open(path) as im:
-            return np.asarray(im.convert("RGB"), dtype=np.uint8), target
+        return decode_rgb(path), target
 
 
 class NpzDataset:

@@ -170,6 +170,10 @@ def build_data_loader_from_cfg(config, model, start_iter: int = 0):
                            and `collate_data_and_cast` (the full host pipeline, no files needed);
       synthetic:gpu        the same image distribution generated in HBM (uint8 [B,224,224,3]) through the ON-GPU
                            augmentation + mask pipeline (data/gpu_augment.py, SURVEY §8f.3): no host pixel work at all;
+      gpu:ImageNet:split=TRAIN:root=R, gpu:ImageFolder:root=R
+                           image files decoded by PIL in DataLoader workers, cropped and augmented on the GPU at each
+                           image's own size (data/image_loader.py); resumable: the indices and crops of an iteration
+                           depend on (train.seed, rank, world, iteration) only;
       anything else        the reference's `make_dataset` / `make_data_loader` (data/loaders.py), which stay in the
                            reference checkout and resolve through the package overlay (needs that checkout + its deps).
     """
@@ -201,6 +205,9 @@ def build_data_loader_from_cfg(config, model, start_iter: int = 0):
                 lo, hi = noise.amin((1, 2, 3), keepdim=True), noise.amax((1, 2, 3), keepdim=True)
                 yield pipe(((noise - lo) / (hi - lo) * 255).to(torch.uint8))
         return gpu_batches()
+    if path.startswith("gpu:"):
+        from ..data.image_loader import GpuImageLoader
+        return GpuImageLoader(config, start_iter=start_iter, rank=rank, world=world)
     img_size, patch = config.crops.global_crops_size, config.student.patch_size
     grid = img_size // patch
     mask_generator = MaskingGenerator(input_size=(grid, grid), max_num_patches=0.5 * img_size // patch * img_size // patch)
@@ -719,58 +726,65 @@ def do_train(config, model: SSLMetaArch, resume: bool = False, data_loader=None,
     any_on = (knn_on or linear_on or seg_on or depth_on or video_on or corr_on or disc_on or ret_on or logreg_on
               or att_on)
     eval_period = int(ev.get("eval_period_iterations", 0) or 0) if any_on else 0
-    for it in range(start_iter, n_iters):
-        try:
-            data = next(it_loader)
-        except StopIteration:
-            break
-        local_w, gram_w = (None if s is None else float(s[it]) for s in (local_s, gram_s))
-        engine.train_step(data, teacher_temp=float(temp_s[it]), lr=float(lr_s[it]), wd=float(wd_s[it]),
-                          last_layer_lr=float(last_s[it]), momentum=float(mom_s[it]), gram_loss_weight=gram_w,
-                          dino_local_loss_weight=local_w, iteration=it)
-        if ck_cfg is not None and (it + 1) % int(ck_cfg.period) == 0:
-            params_tree, opt_tree = engine_state(engine)                 # collective under FSDP (all-gathers the shards)
-            if distributed.is_main_process():
-                save_checkpoint(os.path.join(ckpt_dir, str(it)), iteration=it, params=params_tree,
-                                optimizer_state=opt_tree, overwrite=True)
-                keep_last_n_checkpoints(ckpt_dir, ck_cfg.max_to_keep)
-                if "keep_every" in ck_cfg and (it + 1) % int(ck_cfg.keep_every) == 0:
-                    keep_checkpoint_copy(os.path.join(ckpt_dir, str(it)))
-        if eval_period > 0 and (it + 1) % eval_period == 0:          # train/train.py:689-692
-            if knn_on:
-                do_test(config, engine, f"training_{it}")
-            if linear_on:
-                do_linear_eval(config, engine, f"training_{it}")
-            if seg_on:
-                do_seg_eval(config, engine, f"training_{it}")
-            if depth_on:
-                do_depth_eval(config, engine, f"training_{it}")
-            if video_on:
-                do_video_eval(config, engine, f"training_{it}")
-            if corr_on:
-                do_correspondence_eval(config, engine, f"training_{it}")
-            if disc_on:
-                do_discovery_eval(config, engine, f"training_{it}")
-            if ret_on:
-                do_retrieval_eval(config, engine, f"training_{it}")
-            if logreg_on:
-                do_logreg_eval(config, engine, f"training_{it}")
-            if att_on:
-                do_attentive_eval(config, engine, f"training_{it}")
-        if it % print_freq == 0 or it == n_iters - 1:
-            m = engine.read_metrics()                  # the only device->host sync of the loop
-            if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
-                nan_streak += 1
-                if nan_streak > 2:
-                    raise RuntimeError("loss is NaN for more than 2 consecutive reads")
-            else:
-                nan_streak = 0
-            meters = m
-            if distributed.is_main_process():
-                dt = (time.time() - t0) / (it - start_iter + 1)
-                print(f"it {it}: loss {m['total_loss']:.4f} dino_l {m['dino_local_crops_loss']:.4f} dino_g "
-                      f"{m['dino_global_crops_loss']:.4f} koleo {m['koleo_loss']:.4f} ibot {m['ibot_loss']:.4f} "
-                      f"({dt * 1e3:.1f} ms/it)", flush=True)
+    try:
+        for it in range(start_iter, n_iters):
+            try:
+                data = next(it_loader)
+            except StopIteration:
+                break
+            local_w, gram_w = (None if s is None else float(s[it]) for s in (local_s, gram_s))
+            engine.train_step(data, teacher_temp=float(temp_s[it]), lr=float(lr_s[it]), wd=float(wd_s[it]),
+                              last_layer_lr=float(last_s[it]), momentum=float(mom_s[it]), gram_loss_weight=gram_w,
+                              dino_local_loss_weight=local_w, iteration=it)
+            if ck_cfg is not None and (it + 1) % int(ck_cfg.period) == 0:
+                params_tree, opt_tree = engine_state(engine)             # collective under FSDP (all-gathers the shards)
+                if distributed.is_main_process():
+                    save_checkpoint(os.path.join(ckpt_dir, str(it)), iteration=it, params=params_tree,
+                                    optimizer_state=opt_tree, overwrite=True)
+                    keep_last_n_checkpoints(ckpt_dir, ck_cfg.max_to_keep)
+                    if "keep_every" in ck_cfg and (it + 1) % int(ck_cfg.keep_every) == 0:
+                        keep_checkpoint_copy(os.path.join(ckpt_dir, str(it)))
+            if eval_period > 0 and (it + 1) % eval_period == 0:      # train/train.py:689-692
+                if knn_on:
+                    do_test(config, engine, f"training_{it}")
+                if linear_on:
+                    do_linear_eval(config, engine, f"training_{it}")
+                if seg_on:
+                    do_seg_eval(config, engine, f"training_{it}")
+                if depth_on:
+                    do_depth_eval(config, engine, f"training_{it}")
+                if video_on:
+                    do_video_eval(config, engine, f"training_{it}")
+                if corr_on:
+                    do_correspondence_eval(config, engine, f"training_{it}")
+                if disc_on:
+                    do_discovery_eval(config, engine, f"training_{it}")
+                if ret_on:
+                    do_retrieval_eval(config, engine, f"training_{it}")
+                if logreg_on:
+                    do_logreg_eval(config, engine, f"training_{it}")
+                if att_on:
+                    do_attentive_eval(config, engine, f"training_{it}")
+            if it % print_freq == 0 or it == n_iters - 1:
+                m = engine.read_metrics()                  # the only device->host sync of the loop
+                if math.isnan(m["total_loss"]):            # NaN guard of train/train.py:656-667, evaluated on read
+                    nan_streak += 1
+                    if nan_streak > 2:
+                        raise RuntimeError("loss is NaN for more than 2 consecutive reads")
+                else:
+                    nan_streak = 0
+                meters = m
+                if distributed.is_main_process():
+                    dt = (time.time() - t0) / (it - start_iter + 1)
+                    print(f"it {it}: loss {m['total_loss']:.4f} dino_l {m['dino_local_crops_loss']:.4f} dino_g "
+                          f"{m['dino_global_crops_loss']:.4f} koleo {m['koleo_loss']:.4f} ibot {m['ibot_loss']:.4f} "
+                          f"({dt * 1e3:.1f} ms/it)", flush=True)
+    finally:
+        if not user_loader:                  # the loader's workers end with the run, whether it returns or raises
+            for obj in (it_loader, data_loader):
+                close = getattr(obj, "close", None)
+                if callable(close):
+                    close()
     return meters
 
 

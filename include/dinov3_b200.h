@@ -346,6 +346,26 @@ int d3_aug_solarize(float* x /*[n_crops,S,S,3] in place*/, const void* crops, in
 int d3_aug_local_windows(const float* base /*[n_base,M,M,3]*/, int n_base, int M, const void* crops, const void* blur,
                          int n_crops, int L, float* win, float* tmp, float* y /*[n_crops,L,L,3]*/,
                          float* gray_sum /*[n_crops] zeroed*/, void* stream);
+/* Ragged sources: B decoded images of their own sizes, their HWC pixels packed one after the other in one buffer,
+ * with a device table of one 16-byte row per image,
+ *   struct { long long off; int h, w; }   (off = the image's first pixel in the buffer, in pixels),
+ * and crops drawn from each image's own size.  The crops are the same kernel as the dense entries above (a dense batch
+ * is a ragged batch of equal sizes); everything after the first crop works on dense base crops.  `crops_host` /
+ * `recs_host` are the host copies of the device records: a record whose img is outside the table is refused with
+ * D3_ERR_ARG before any CUDA call, as are null pointers and n_img < 1.  That each box lies inside its own image is
+ * the caller's to check (it drew the boxes from the sizes).
+ *  - d3_aug_resized_crop_ragged / _f32: RandomResizedCrop of uint8, or of fp32 [0,1] (clamp as above), sources.
+ *  - d3_aug_color_images_ragged: share_color_jitter on ragged sources; x is the fp32 copy of the n_pix packed pixels
+ *    with the same offsets, and contrast blends with the mean gray of each image's own h * w pixels.               */
+int d3_aug_resized_crop_ragged(const void* src_u8 /*packed HWC*/, const void* imgs /*device [n_img]*/, int n_img,
+                               const void* crops /*device*/, const void* crops_host, int n_crops,
+                               float* out /*[n_crops,S,S,3]*/, int S, void* stream);
+int d3_aug_resized_crop_ragged_f32(const float* src /*packed HWC in [0,1]*/, const void* imgs, int n_img,
+                                   const void* crops, const void* crops_host, int n_crops, float* out, int S, int clamp,
+                                   void* stream);
+int d3_aug_color_images_ragged(const void* src_u8 /*packed HWC*/, long long n_pix, const void* imgs, int n_img,
+                               const void* recs /*device [n_img]*/, const void* recs_host, float* x /*packed HWC*/,
+                               float* gray_sum /*[n_img] zeroed*/, void* stream);
 
 /* ---- k-NN evaluation (the DINO / DINOv2 / DINOv3 k-NN protocol on the teacher's normalised class token) ---------
  * The similarities of a query tile with a bank chunk are d3_gemm_bf16 (fp32 out) of L2-normalised bf16 rows; these
